@@ -1,7 +1,7 @@
 #!/usr/bin/env python
-"""bench.py — audio-frames/sec (fwd+bwd[+all-reduce]+Adam) of SpeechTransformer-base on N B200s.
+"""bench.py — audio-frames/sec (fwd+bwd[+all-reduce]+Adam) of SpeechTransformer-base on N H100s.
 
-  python bench.py [--gpus N] [--steps K] [--warmup W]            # this repo's CUDA path (libb200st)
+  python bench.py [--gpus N] [--steps K] [--warmup W] [--dump-outputs DIR]   # this repo's CUDA path (libb200st)
   python bench.py --impl reference [--steps K] [--warmup W]      # the reference algorithm's CPU path (oracle port)
   torchrun --nnodes=1 --nproc-per-node N ... bench.py --gpus N   # one rank per GPU, NCCL
 
@@ -47,12 +47,24 @@ def flops_per_step(B, T, L, V=8192, d=256, H=4, ffn=2048, C=256, F=80, enc=12, d
 
 
 def load_peaks():
-    p = os.path.join(ROOT, "MEASURED_PEAKS.json")
-    if os.path.exists(p):
-        j = json.load(open(p))
-        return dict(tflops_sustained=j.get("bf16_tflops_sustained"), tflops_burst=j.get("bf16_tflops"), hbm_gbs=j.get("hbm_gbs"),
-                    source="measured (MEASURED_PEAKS.json)")
-    return dict(tflops_sustained=1400.0, tflops_burst=1590.0, hbm_gbs=6650.0, source="fallback (B200_PROFILING.md)")
+    """Data-sheet peaks of the H100 SXM (dense 16-bit tensor rate, HBM3 bandwidth, 700 W card): the denominators of the
+    `frac` fields, not rates this program has reached."""
+    return dict(tflops_sustained=989.0, hbm_gbs=3350.0, source="NVIDIA H100 SXM data sheet")
+
+
+def dump_outputs(out_dir, trainer, losses):
+    """What a caller of the timed path holds after its last step, as float32 .npy files: the loss of every timed step and the
+    parameters the last step left behind (a fixed, seeded sample of at most 4 Mi elements: the arena is larger than 64 MB)."""
+    import numpy as np
+    import torch
+    os.makedirs(out_dir, exist_ok=True)
+    np.save(os.path.join(out_dir, "loss.npy"), np.asarray([float(x) for x in losses], dtype=np.float32))
+    params = trainer.rt.params.detach().reshape(-1).float()
+    n = params.numel()
+    if n > (1 << 22):
+        idx = torch.from_numpy(np.sort(np.random.RandomState(1234).choice(n, 1 << 22, replace=False))).to(params.device)
+        params = params[idx]
+    np.save(os.path.join(out_dir, "params_sample.npy"), params.cpu().numpy())
 
 
 class ClockSampler(threading.Thread):
@@ -108,7 +120,7 @@ class ClockSampler(threading.Thread):
 
 # ------------------------------------------------------------------------------------------------------
 # CPU arm: the reference algorithm on host cores (oracle port — the reference's TF2 path cannot run: no TF wheel,
-# and /root/reference does not exist on the GPU box; its PyTorch mirror has no working backward, SURVEY §8c)
+# and the reference tree is not present where the benchmark runs; its PyTorch mirror has no working backward, SURVEY §8c)
 # ------------------------------------------------------------------------------------------------------
 def cpu_reference_step_time(B, T, L, steps, warmup, threads):
     import torch
@@ -302,8 +314,7 @@ def encoder_block_roofline(WL, dtype, peaks, iters=20):
     tf = gf / us_layer * 1e3           # GFLOP / us = PFLOP/s
     return {"what": "TransformerEncoder forward (dropout on) replayed as one CUDA graph, time / 12 layers (includes 1/12 of the "
                     "input cast and final LayerNorm)", "fwd_us_per_layer": us_layer, "gflop_per_layer": gf, "achieved": tf,
-            "unit": "TFLOP/s", "frac": tf / peaks["tflops_sustained"], "frac_of_burst_peak": tf / peaks["tflops_burst"],
-            "target": ">= 0.70 (<= %.1f us)" % (gf / (0.7 * peaks["tflops_sustained"]) * 1e3)}
+            "unit": "TFLOP/s", "frac": tf / peaks["tflops_sustained"]}
 
 
 def run_decode(args):
@@ -344,7 +355,7 @@ def run_decode(args):
         e[2].record()
         torch.cuda.synchronize()
         enc_ms, dec_ms = e[0].elapsed_time(e[1]), e[1].elapsed_time(e[2])
-        # the same search as a per-token CUDA graph (round-2 first version), for the comparison
+        # the same search as a per-token CUDA graph (the earlier version), for the comparison
         cache2 = D.create_decoding_cache(rt, enc, bias, steps, shadow)
         D.greedy_search(rt, inputs, tm["bos_id"], tm["eos_id"], tm["unk_id"], cache=cache2, persistent=False, **kw)    # warm-up
         cache2 = D.create_decoding_cache(rt, enc, bias, steps, shadow)
@@ -405,7 +416,7 @@ def run_gpu(args):
                                                   use_cuda_graph=not args.no_graph)
     dev = torch.device("cuda", local_rank)
 
-    # resident-input arm: a few distinct batches already in HBM (activations per step ~4 GB >> 126 MB L2)
+    # resident-input arm: a few distinct batches already in HBM (activations per step ~4 GB >> 50 MB L2)
     n_batches = 4
     if WL.get("ragged"):
         # cfg-4: frame budget 24000 / GPU over the reference's length buckets (neurst/tasks/speech2text.py:38-56,296-310):
@@ -467,6 +478,8 @@ def run_gpu(args):
     sampler.mark(t_w0, time.time())
     launches = lib.launch_count() - launches0
     loss_val = float(losses[-1])
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, trainer, losses[-args.steps:])
     for i in range(2):
         e2e_step(i)
     t_w0 = time.time()
@@ -474,7 +487,7 @@ def run_gpu(args):
     sampler.mark(t_w0, time.time())
     sampler.stop()
 
-    # roofline pass (not timed): per-launch CUDA events around the tcgen05 GEMM launches of ONE step
+    # roofline pass (not timed): per-launch CUDA events around the wgmma GEMM launches of ONE step
     # (every rank runs the same steps — train_step contains the gradient all-reduce — only rank 0 reports)
     torch.cuda.synchronize()
     lib.profile_begin()
@@ -512,7 +525,7 @@ def run_gpu(args):
     def leave(code=0):
         # Multi-rank exit: every rank has passed the final barrier; the NCCL communicators (torch's and the library's) are
         # left to the process teardown — ncclCommDestroy is an intra-node collective and a destructor-time call on one rank
-        # while another is already gone blocks forever (seen in round 2) — so the ranks exit without running destructors.
+        # while another is already gone blocks forever — so the ranks exit without running destructors.
         sys.stdout.flush(); sys.stderr.flush()
         if world > 1:
             os._exit(code)
@@ -542,7 +555,7 @@ def run_gpu(args):
                                                                    "[%d,%d,80] L=%d" % (B, T, L) if not WL.get("ragged") else
                                                                    "length buckets %s (T,B,L), src_length~U(0.6T,T)" % (shapes,)),
                    "global_batch_frames": frames, "real_frames_per_sec": real_frames / (ms_step * 1e-3), "parallelism": "dp%d" % world, "cuda_graph": not args.no_graph, "kernels_per_step": int(launches_per_step),
-                   "l2_policy": "inputs+activations per step (~4 GB) exceed the 126 MB L2; 4 rotating input batches",
+                   "l2_policy": "inputs+activations per step (~4 GB) exceed the 50 MB L2; 4 rotating input batches",
                    "loss_last_step": loss_val,
                    "loss_scale_state": (dict(zip(("scale", "finite_steps_in_a_row", "last_step_skipped", "skipped_steps", "applied_steps",
                                                   "global_grad_norm"), [float(x) for x in trainer.rt.loss_scale_state[:6].tolist()]))
@@ -552,34 +565,22 @@ def run_gpu(args):
                 "d2h_bytes_per_step": 4, "ms_per_step": ms_e2e / args.steps},
         "gpu_launches": int(launches_per_step * args.steps),
     }
-    # roofline of the dominant kernel family (tc_gemm_kernel / tc_wgrad_group_kernel: ~160 launches, ~42 % of the step): algorithmic FLOPs of those
-    # launches / their durations: the GEMMs of one eagerly launched step are recorded and each is replayed back to back
-    # inside the library with CUDA events around the repetitions (a graph replay cannot be bracketed per kernel).  `traffic` = DRAM bytes per launch from the committed ncu pass
-    # (profiles/r02_gemm_traffic.json, same command), averaged like `achieved`.
-    step_rf = {"achieved": ach, "frac": ach / peaks["tflops_sustained"], "frac_of_burst_peak": ach / peaks["tflops_burst"],
+    # roofline of the GEMM kernel family (tc_gemm_kernel / tc_wgrad_group_kernel): algorithmic FLOPs of those launches / their
+    # durations: the GEMMs of one eagerly launched step are recorded and each is replayed back to back inside the library
+    # with CUDA events around the repetitions (a graph replay cannot be bracketed per kernel).  DRAM traffic is not measured.
+    step_rf = {"achieved": ach, "frac": ach / peaks["tflops_sustained"],
                "algorithmic_flops_per_step": fl, "mflop_per_frame": fl / (frames / world) / 1e6,
                "note": "all kernels of the step / step time"}
-    traffic, ncu_share = None, None
-    for name in ("r02_gemm_traffic.json", "r01_gemm_traffic.json"):      # committed ncu pass of this command (latest round first)
-        try:
-            with open(os.path.join(ROOT, "profiles", name)) as f:
-                tj = json.load(f)
-            traffic = tj["dram_bytes_total"] / max(1, tj["launches"])
-            ncu_share = tj.get("share_of_step")
-            break
-        except Exception:
-            continue
     if gemm and gemm["ms"] > 0:
         g_tf = gemm["flops"] / (gemm["ms"] * 1e-3) / 1e12
-        line["roofline"] = {"bound": "tensor", "kernel": "tc_gemm_kernel (all instantiations) + tc_wgrad_group_kernel (tcgen05 GEMMs outside the fused FFN / attention kernels)", "achieved": g_tf,
+        line["roofline"] = {"bound": "tensor", "kernel": "tc_gemm_kernel (all instantiations) + tc_wgrad_group_kernel (wgmma GEMMs outside the fused FFN / attention kernels)", "achieved": g_tf,
                             "peak": peaks["tflops_sustained"], "unit": "TFLOP/s", "frac": g_tf / peaks["tflops_sustained"],
-                            "peak_burst": peaks["tflops_burst"], "frac_of_burst_peak": g_tf / peaks["tflops_burst"],
-                            "traffic": traffic, "peak_source": peaks["source"], "launches_per_step": gemm["launches"],
+                            "traffic": None, "peak_source": peaks["source"], "launches_per_step": gemm["launches"],
                             "avg_launch_us": gemm["ms"] * 1e3 / max(1, gemm["launches"]),
                             "algorithmic_flops_per_launch": gemm["flops"] / max(1, gemm["launches"]),
-                            "share_of_step": gemm["ms"] / ms_step, "share_of_step_ncu": ncu_share,
+                            "share_of_step": gemm["ms"] / ms_step,
                             "share_note": "sum of the per-launch GEMM durations (each GEMM of one step replayed back to back, "
-                                          "CUDA events, no host gaps) / timed step; ncu share from the committed launch list",
+                                          "CUDA events, no host gaps) / timed step",
                             "step": step_rf}
     else:
         line["roofline"] = {"bound": "tensor", "kernel": "whole step", "achieved": ach, "peak": peaks["tflops_sustained"],
@@ -596,8 +597,12 @@ def run_gpu(args):
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--gpus", type=int, default=1)
-    ap.add_argument("--steps", type=int, default=10)
+    ap.add_argument("--steps", type=int, default=10, help="timed training steps (the decode workload always decodes its 200 tokens)")
     ap.add_argument("--warmup", type=int, default=3)
+    ap.add_argument("--dump-outputs", default="", metavar="DIR",
+                    help="training workloads only: after the timed steps write their losses and a seeded sample of the updated "
+                         "parameters to DIR/*.npy; split-K and FFN-slice reductions use fp32 atomics, so two runs agree to rounding, "
+                         "not bit for bit")
     ap.add_argument("--impl", default="b200", choices=["b200", "reference"])
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--cpu-worker", default="", help=argparse.SUPPRESS)
@@ -609,6 +614,8 @@ def main():
                     help="cfg2 = BASELINE headline [32,1000,80]; cfg3 / cfg3w = [8|64,1500,80]; cfg4 = speech_transformer_m ragged buckets; "
                          "decode = cfg-5 greedy decode")
     args = ap.parse_args()
+    if args.dump_outputs and (args.impl == "reference" or args.workload == "decode"):
+        ap.error("--dump-outputs is implemented for the training workloads of the CUDA path only")
     if args.cpu_ref_worker:
         cpu_ref_worker(args.cpu_ref_worker)
         return
@@ -627,6 +634,8 @@ def main():
         cmd += ["--dtype", args.dtype, "--workload", args.workload]
         if args.no_cpu_baseline:
             cmd.append("--no-cpu-baseline")
+        if args.dump_outputs:
+            cmd += ["--dump-outputs", args.dump_outputs]
         sys.exit(subprocess.call(cmd))
     if args.workload == "decode":
         run_decode(args)

@@ -1,4 +1,4 @@
-/* libb200st — C ABI of the B200-native SpeechTransformer hot path.
+/* libb200st — C ABI of the H100-native SpeechTransformer hot path.
  *
  * Drop-in boundary for bytedance/neurst (reference @ /root/reference).  The reference is pure Python; its
  * "FFI" for this path is the class registry (neurst/utils/registry.py:24-137) through which Trainer and the
@@ -30,7 +30,7 @@ int64_t b200st_launch_count(void);
 /* ---- generic contraction (tf.einsum / Dense / tf.matmul sites; neurst/layers/common_layers.py:270,276-288,
  *      multi_head_attention.py:145,215; text_modalities.py:104-108) ---------------------------------------
  * C[b2][b1][m][n] = epi(alpha * sum_k A(m,k) B(n,k)); operands K-major (mn_major=0) or MN-major (1).
- * bf16 operands -> tcgen05/TMEM/TMA kernel; fp32 operands -> fp32 FMA kernel (parity mode). */
+ * bf16 operands -> wgmma/TMA kernel; fp32 operands -> fp32 FMA kernel (parity mode). */
 typedef struct {
   const void* ptr; int32_t dtype; int32_t mn_major; int64_t ld, sb1, sb2;
 } b200st_operand;
@@ -56,7 +56,7 @@ int b200st_gemm(const b200st_gemm_args* args, void* stream);
  * (neurst/models/transformer.py), 2 = TransformerEncoder stack only (layers/encoders/transformer_encoder.py:23-136),
  * 3 = TransformerDecoder stack only (layers/decoders/transformer_decoder.py:23-228), 4 = MultiHeadAttention /
  * MultiHeadSelfAttention (layers/attentions/multi_head_attention.py:21-290).
- * precision: B200ST_F32 = fp32 FMA kernels (parity mode, any shape); B200ST_F16 / B200ST_BF16 = tcgen05 kernels with every
+ * precision: B200ST_F32 = fp32 FMA kernels (parity mode, any shape); B200ST_F16 / B200ST_BF16 = wgmma kernels with every
  * 16-bit tensor (weights shadow, activations, activation gradients) in that type, fp32 accumulation, fp32 master weights,
  * fp32 parameter gradients.  B200ST_F16 is the reference's own mixed precision (mixed_float16 + dynamic loss scaling,
  * neurst/training/training_utils.py:73-81,413-416): 11-bit significands, needs loss scaling (b200st_batch.loss_scale_dev +
@@ -191,7 +191,7 @@ int b200st_greedy_search(b200st_handle h, const b200st_buffers* buf, const b200s
 /* mode the last b200st_greedy_search actually ran in: 2 persistent kernel, 1 captured graph, 0 eager launches */
 int32_t b200st_greedy_used_graph(void);
 
-/* 16-bit shadow of the parameter arena (tcgen05 operands); shadow_dtype = B200ST_BF16 or B200ST_F16 */
+/* 16-bit shadow of the parameter arena (wgmma operands); shadow_dtype = B200ST_BF16 or B200ST_F16 */
 int b200st_refresh_shadow(const float* params, void* shadow, int32_t shadow_dtype, int64_t numel, void* stream);
 
 /* Optimizer step of GradAccumKerasModel.train_step (neurst/training/gradaccum_keras_model.py:222-240): unscale ->
@@ -255,14 +255,13 @@ int b200st_dropout_mask(uint64_t seed, uint64_t stream_id, int64_t n, float p, u
 /* tests/bench only: time `iters` back-to-back launches of one GEMM with CUDA events on `stream` (no host overhead) */
 int b200st_gemm_bench(const b200st_gemm_args* args, int32_t iters, float* ms_per_iter, void* stream);
 
-/* bench only: per-launch CUDA-event timing of the tcgen05 GEMM launches issued between begin and end
+/* bench only: per-launch CUDA-event timing of the wgmma GEMM launches issued between begin and end
  * (sum of kernel durations in ms, sum of their algorithmic FLOPs, number of launches) */
 int b200st_profile_begin(void);
 int b200st_profile_end(double* gemm_ms, double* gemm_flops, int64_t* gemm_launches);
 
-/* tests only: override tcgen05 shared-memory descriptor fields / tile config (0 = default) */
-int b200st_debug_tc(uint32_t mn_lbo, uint32_t mn_sbo, uint32_t k_lbo, uint32_t k_sbo, int32_t force_bn,
-                    int32_t force_stages, int32_t max_ctas);
+/* tests / tools only: override the GEMM tile configuration (0 = default): N tile, ring depth (>= 2), CTA count */
+int b200st_debug_tc(int32_t force_bn, int32_t force_stages, int32_t max_ctas);
 
 #ifdef __cplusplus
 }

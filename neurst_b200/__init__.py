@@ -1,6 +1,6 @@
-"""neurst_b200 — B200-native SpeechTransformer hot path (libb200st) behind the bytedance/neurst class registry.
+"""neurst_b200 — H100-native SpeechTransformer hot path (libb200st) behind the bytedance/neurst class registry.
 
-Importing the package registers the B200 classes into the reference's registries when the reference is importable
+Importing the package registers the H100 classes into the reference's registries when the reference is importable
 (`--include neurst_b200` in the reference CLI does exactly this import, neurst/utils/flags_core.py:207-247); without the
 reference on sys.path the package is a stand-alone library (models / layers / trainer / decode on top of the C ABI).
 """

@@ -1,4 +1,4 @@
-"""Builds libb200st.so in-tree with nvcc for sm_100a (no torch headers, plain C ABI).
+"""Builds libb200st.so in-tree with nvcc for sm_90a (no torch headers, plain C ABI).
 
 Usage: python neurst_b200/csrc/build.py [--force]
 """
@@ -12,7 +12,7 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 OUT = os.path.join(os.path.dirname(HERE), "libb200st.so")
 OBJ = os.path.join(HERE, "build")
 NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
-FLAGS = ["-gencode", "arch=compute_100a,code=sm_100a", "-lineinfo", "-O3", "-std=c++17",
+FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17",
          "-Xcompiler", "-fPIC", "--expt-relaxed-constexpr"]
 
 

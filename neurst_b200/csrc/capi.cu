@@ -87,10 +87,8 @@ int b200st_profile_end(double* gemm_ms, double* gemm_flops, int64_t* gemm_launch
   return tc_profile_end(gemm_ms, gemm_flops, gemm_launches);
 }
 
-int b200st_debug_tc(uint32_t mn_lbo, uint32_t mn_sbo, uint32_t k_lbo, uint32_t k_sbo, int32_t force_bn,
-                    int32_t force_stages, int32_t max_ctas) {
+int b200st_debug_tc(int32_t force_bn, int32_t force_stages, int32_t max_ctas) {
   TcDebug& d = tc_debug();
-  d.mn_lbo_bytes = mn_lbo; d.mn_sbo_bytes = mn_sbo; d.k_lbo_bytes = k_lbo; d.k_sbo_bytes = k_sbo;
   d.force_bn = force_bn; d.force_stages = force_stages; d.max_ctas = max_ctas;
   return 0;
 }
@@ -364,7 +362,7 @@ extern "C" int b200st_dropout_mask(uint64_t seed, uint64_t stream_id, int64_t n,
   if (!out || n < 0) B200ST_FAIL("bad arguments");
   if (n == 0) return 0;
   int64_t g = (n + 255) / 256;
-  if (g > 148 * 16) g = 148 * 16;
+  if (g > 132 * 16) g = 132 * 16;
   launch_pdl(b200st::dropout_mask_kernel, (int)g, 256, 0, reinterpret_cast<cudaStream_t>(stream), seed, stream_id, n, p, out);
   B200ST_LAUNCH_CHECK();
   return 0;

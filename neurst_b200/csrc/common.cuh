@@ -1,4 +1,4 @@
-// Shared device/host helpers for libb200st (sm_100a only).
+// Shared device/host helpers for libb200st (sm_90a only).
 #pragma once
 #include <cstdlib>
 #include <cuda_runtime.h>
@@ -98,7 +98,7 @@ __device__ __forceinline__ float warp_max(float v) {
 
 // ---- counter-based RNG for dropout: Philox4x32-7 ---------------------------------------
 // (7 rounds: the smallest round count of Philox4x32 that Salmon et al. report as passing BigCrush; the generator of all
-// keep-bits of a step is integer-ALU bound — 0.26 ms of the cfg-2 step with 10 rounds, measured by tools/ablate_step.py)
+// keep-bits of a step is integer-ALU bound, so fewer rounds are directly fewer instructions; tools/ablate_step.py isolates its cost)
 // One call yields 4 x 32 random bits for counter (idx4, stream) under key (seed).  Dropout at element
 // index e uses call (e >> 2) and lane (e & 3), so forward and backward regenerate identical masks.
 struct Philox4 { uint32_t x, y, z, w; };

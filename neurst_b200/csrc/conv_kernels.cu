@@ -6,7 +6,7 @@
 // NORMALISED activation xhat + 1/sigma ("normalised-save"): gamma/beta/ReLU are applied by the im2col in flight and the
 // backward reads xhat back, so it needs neither the convolution recompute nor the statistics.  Other shapes use the
 // generic kernels (filter in shared memory, post-ReLU activation stored, z1 recomputed in the backward).
-// conv2 is lowered to tcgen05 GEMMs through im2col (forward / wgrad) and a dcol GEMM (dgrad); the dgrad's col2im
+// conv2 is lowered to wgmma GEMMs through im2col (forward / wgrad) and a dcol GEMM (dgrad); the dgrad's col2im
 // gather is fused with the ReLU mask, the LayerNorm backward of conv1 and the parameter-gradient partial sums.
 // conv1's filter gradient is one more split-K GEMM over the tiny im2col of the fbank (written by the same kernel).
 #include "kernels.cuh"
@@ -246,17 +246,7 @@ __global__ void __launch_bounds__(256, (CPL <= 8 ? 3 : 1)) conv1_fwd_kernel(cons
 // ahead and broadcast with shuffles, each warp walks a contiguous range of positions.
 // SAVE: store xhat + 1/sigma (normalised-save mode); else y = relu(LN(z) * gamma + beta).
 // ---------------------------------------------------------------------------------------------
-// d{0,1} += a * b{0,1} as one packed fp32x2 instruction (FFMA2, sm_100): half the issue slots of two FFMAs
-__device__ __forceinline__ void ffma2_bcast(float& d0, float& d1, float a, float b0, float b1) {
-  uint64_t av, bv, cv;
-  asm("mov.b64 %0, {%1, %1};" : "=l"(av) : "f"(a));
-  asm("mov.b64 %0, {%1, %2};" : "=l"(bv) : "f"(b0), "f"(b1));
-  asm("mov.b64 %0, {%1, %2};" : "=l"(cv) : "f"(d0), "f"(d1));
-  asm("fma.rn.f32x2 %0, %1, %2, %0;" : "+l"(cv) : "l"(av), "l"(bv));
-  asm("mov.b64 {%0, %1}, %2;" : "=f"(d0), "=f"(d1) : "l"(cv));
-}
-
-template <typename T, bool SAVE, bool F2 = false>
+template <typename T, bool SAVE>
 __global__ void __launch_bounds__(256, 2) conv1_fwd_c256_kernel(const float* __restrict__ src, const float* __restrict__ w,
                                                                 const float* __restrict__ bias, const float* __restrict__ gamma,
                                                                 const float* __restrict__ beta, float eps, T* __restrict__ y,
@@ -272,8 +262,8 @@ __global__ void __launch_bounds__(256, 2) conv1_fwd_c256_kernel(const float* __r
   if (!SAVE) { ld8<float>(gamma + 8 * lane, greg); ld8<float>(beta + 8 * lane, bereg); }
   const int64_t npos = (int64_t)B * T1 * F1;
   const int64_t nwarps = (int64_t)gridDim.x * (blockDim.x >> 5);
-  // each warp walks a contiguous range of positions: neighbouring positions share fbank taps (L1 hits); the warp-interleaved
-  // order was measured slower here (233 vs 203 us) although it helps the backward kernel slightly
+  // each warp walks a contiguous range of positions: neighbouring positions share fbank taps (L1 hits)
+  // (the backward kernel interleaves positions across warps instead)
   const int64_t per = (npos + nwarps - 1) / nwarps;
   const int64_t wid = (int64_t)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
   int64_t pos = wid * per;
@@ -291,8 +281,8 @@ __global__ void __launch_bounds__(256, 2) conv1_fwd_c256_kernel(const float* __r
     }
     return v;
   };
-  // the taps of the next RING-1 positions are in flight during the math of the current one (one position ahead left the
-  // warps waiting on L2: 203 us for 0.28 GB of traffic, ncu round 2)
+  // the taps of the next RING-1 positions are in flight during the math of the current one (with only one position
+  // ahead the warps wait on L2)
   constexpr int RING = 4;
   int64_t ipos = pos;
   int ib = b, it1 = t1, if1 = f1;
@@ -312,13 +302,8 @@ __global__ void __launch_bounds__(256, 2) conv1_fwd_c256_kernel(const float* __r
 #pragma unroll
     for (int tp = 0; tp < 9; ++tp) {
       const float x = __shfl_sync(0xffffffffu, xv, tp);
-      if constexpr (F2) {
 #pragma unroll
-        for (int i = 0; i < 8; i += 2) ffma2_bcast(z[i], z[i + 1], x, wreg[tp][i], wreg[tp][i + 1]);
-      } else {
-#pragma unroll
-        for (int i = 0; i < 8; ++i) z[i] = fmaf(x, wreg[tp][i], z[i]);
-      }
+      for (int i = 0; i < 8; ++i) z[i] = fmaf(x, wreg[tp][i], z[i]);
     }
     float s1 = 0.f;
 #pragma unroll
@@ -486,7 +471,7 @@ __global__ void __launch_bounds__(256, 2) conv1_bwd_xhat_c256_kernel(
   const int64_t npos = (int64_t)B * T1 * F1;
   const int64_t nwarps = (int64_t)gridDim.x * (blockDim.x >> 5);
   const int64_t wid = (int64_t)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
-  int64_t pos = wid;                       // warp-interleaved positions: the grid sweeps one contiguous window of xhat / dz1 (-10 us vs a range per warp)
+  int64_t pos = wid;                       // warp-interleaved positions: the grid sweeps one contiguous window of xhat / dz1
   const int64_t pos_end = npos;
   const int step_f = (int)(nwarps % F1), step_t = (int)((nwarps / F1) % T1), step_b = (int)(nwarps / ((int64_t)F1 * T1));
   if (pos < pos_end) {
@@ -495,7 +480,7 @@ __global__ void __launch_bounds__(256, 2) conv1_bwd_xhat_c256_kernel(
     int b = (int)(pos / ((int64_t)F1 * T1));
     const int tap_dt = lane / 3 - 1, tap_df = lane % 3 - 1;      // lanes 0..8 own one fbank tap each
     // every global load of a position (fbank tap, xhat row, 1/sigma, dcol rows) is issued RING-1 positions ahead: the kernel is
-    // bound by bytes in flight, not by bandwidth (ncu, round 2: 2.8 TB/s with one position ahead) — the implicit variant loads
+    // bound by bytes in flight, not by bandwidth — the implicit variant loads
     // one gradient row instead of four and spends the freed registers on a deeper ring
     constexpr int NDC = IMPLICIT ? 1 : 4;
     constexpr int RING = IMPLICIT ? 4 : 2;
@@ -762,14 +747,12 @@ static int conv1_fwd_launch(const float* src, const float* w, const float* b, co
   const int T1 = (T + 1) / 2, F1 = (F + 1) / 2;
   const int64_t npos = (int64_t)B * T1 * F1;
   if (npos == 0) return 0;
-  const int grid = pick_grid(npos, 8 * 4, 148 * 12);
+  const int grid = pick_grid(npos, 8 * 4, 132 * 12);
   const bool vec = (C % 8 == 0) && ((reinterpret_cast<uintptr_t>(y1) & 15) == 0);
   if (vec && C == 256 && Cin == 1 && (use_ln || rstd_out) && ((reinterpret_cast<uintptr_t>(w) & 15) == 0) &&
       ((reinterpret_cast<uintptr_t>(b) & 15) == 0) && (rstd_out || (((reinterpret_cast<uintptr_t>(gamma) | reinterpret_cast<uintptr_t>(beta)) & 15) == 0))) {
-    const int grid1 = pick_grid(npos, 8 * 16, 148 * 2);
-    static const bool f2 = getenv("B200ST_NO_CONV1_FFMA2") == nullptr;   // packed fp32x2 FMAs (same rounding: fma.rn per element; 6.155 vs 6.173 ms step)
-    if (rstd_out && f2) DISPATCH_DTYPE(y_dtype, TT, (launch_pdl(conv1_fwd_c256_kernel<TT, true, true>, grid1, 256, 0, s, src, w, b, gamma, beta, eps, (TT*)y1, rstd_out, B, T, F, T1, F1)));
-    else if (rstd_out) DISPATCH_DTYPE(y_dtype, TT, (launch_pdl(conv1_fwd_c256_kernel<TT, true>, grid1, 256, 0, s, src, w, b, gamma, beta, eps, (TT*)y1, rstd_out, B, T, F, T1, F1)));
+    const int grid1 = pick_grid(npos, 8 * 16, 132 * 2);
+    if (rstd_out) DISPATCH_DTYPE(y_dtype, TT, (launch_pdl(conv1_fwd_c256_kernel<TT, true>, grid1, 256, 0, s, src, w, b, gamma, beta, eps, (TT*)y1, rstd_out, B, T, F, T1, F1)));
     else DISPATCH_DTYPE(y_dtype, TT, (launch_pdl(conv1_fwd_c256_kernel<TT, false>, grid1, 256, 0, s, src, w, b, gamma, beta, eps, (TT*)y1, rstd_out, B, T, F, T1, F1)));
     ++g_kernel_launches;
     B200ST_LAUNCH_CHECK();
@@ -798,7 +781,7 @@ int conv1_bwd_fused(const float* src, const float* w, const float* b, const floa
   const int T1 = (T + 1) / 2, F1 = (F + 1) / 2, T2 = (T1 + 1) / 2, F2 = (F1 + 1) / 2;
   const int64_t npos = (int64_t)B * T1 * F1;
   if (npos == 0) return 0;
-  const int grid = pick_grid(npos, 8 * 4, 148 * 8);
+  const int grid = pick_grid(npos, 8 * 4, 132 * 8);
   const size_t smem = (size_t)(9 * Cin + 1 + 3) * ((C + 255) & ~255) * sizeof(float);
   B200ST_CHECK(smem <= 48 * 1024, "conv1 filter does not fit the default shared memory");
   const bool vec = (C % 8 == 0) && ((reinterpret_cast<uintptr_t>(y1) & 15) == 0) && ((reinterpret_cast<uintptr_t>(dcol) & 15) == 0) &&
@@ -828,7 +811,7 @@ int conv1_bwd_from_xhat(const float* src, const void* gamma, const void* beta, c
   const int T1 = (T + 1) / 2, F1 = (F + 1) / 2, T2 = (T1 + 1) / 2, F2 = (F1 + 1) / 2;
   const int64_t npos = (int64_t)B * T1 * F1;
   if (npos == 0) return 0;
-  const int grid = pick_grid(npos, 8 * 16, 148 * 2);
+  const int grid = pick_grid(npos, 8 * 16, 132 * 2);
   const int tu = F2 > 0 && F2 <= 128 ? 128 / F2 : 1, ub = (T2 + tu - 1) / tu;
   if (implicit_tiles) {
     B200ST_CHECK(F2 <= 128, "implicit conv2 dgrad layout needs F2 <= 128");
@@ -853,13 +836,13 @@ int im2col_3x3s2_affine(const void* y1, void* col, int dtype, int B, int T1, int
   const int T2 = (T1 + 1) / 2, F2 = (F1 + 1) / 2;
   const int64_t nchunks = (int64_t)B * T2 * F2 * 9;
   if (nchunks == 0 || (ablate_mask() & ABL_CONV)) return 0;
-  const int grid = pick_grid(nchunks, 8 * 8, 148 * 16);
+  const int grid = pick_grid(nchunks, 8 * 8, 132 * 16);
   const int esz = dtype_size(dtype);
   const bool vec = ((C * esz) % 16 == 0) && ((reinterpret_cast<uintptr_t>(y1) & 15) == 0) && ((reinterpret_cast<uintptr_t>(col) & 15) == 0) &&
                    ((reinterpret_cast<uintptr_t>(gamma) & 15) == 0) && ((reinterpret_cast<uintptr_t>(beta) & 15) == 0);
   const bool one = vec && C * esz == 32 * 16;
   if (one) {
-    const int grid_r = pick_grid(nchunks / 9, 8 * 4, 148 * 8);
+    const int grid_r = pick_grid(nchunks / 9, 8 * 4, 132 * 8);
     DISPATCH_DTYPE(dtype, TT, (launch_pdl(im2col_row_kernel<TT>, grid_r, 256, 0, s, (const TT*)y1, (TT*)col, B, T1, F1, T2, F2, (const TT*)gamma, (const TT*)beta)));
   }
   else if (vec) DISPATCH_DTYPE(dtype, TT, (launch_pdl(im2col_kernel<TT, true, false>, grid, 256, 0, s, (const TT*)y1, (TT*)col, B, T1, F1, C, T2, F2, (const TT*)gamma, (const TT*)beta)));

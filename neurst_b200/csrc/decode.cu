@@ -334,8 +334,8 @@ __global__ void greedy_init_kernel(GreedyState g, const int64_t* __restrict__ bo
 // =============================================================================================================
 // Persistent greedy search: ONE cooperative launch decodes the whole hypothesis.  Every block is resident (grid = #SMs),
 // the phases of a token (embed | per layer: LN+QKV, self-attention+out-proj, LN+Q, cross-attention+out-proj, LN+FFN1,
-// ReLU+FFN2 | LN+logits | pick) are separated by a grid-wide barrier (one atomic + spin on a monotonic counter, ~1 us)
-// instead of a kernel boundary (~7 us of launch latency each), work items of a phase are distributed round-robin over
+// ReLU+FFN2 | LN+logits | pick) are separated by a grid-wide barrier (one atomic + spin on a monotonic counter)
+// instead of a kernel boundary (a launch latency each), work items of a phase are distributed round-robin over
 // the blocks.  Data produced by other blocks in an earlier phase is read with ld.global.cg (L1 is not coherent);
 // weights and the cross-attention memory never change and go through the read-only path.
 // =============================================================================================================
@@ -711,7 +711,7 @@ int step_launch(const StepCtx& c, const TW* wbase, const int64_t* ids, const int
                (const float*)nullptr, c.P(p + ".ffn.b1"), 0.f, W(p + ".ffn.w2"), c.P(p + ".ffn.b2"), x, B, f, d);
     g_kernel_launches += cf.with_cross_attention && st.Tm > 0 ? 6 : 4;
   }
-  launch_pdl(logits_step_kernel<TW>, 148 * 2, 256, sizeof(float) * (size_t)B * d, c.s, (const float*)x, c.P("dec.out_ln.gamma"),
+  launch_pdl(logits_step_kernel<TW>, 132 * 2, 256, sizeof(float) * (size_t)B * d, c.s, (const float*)x, c.P("dec.out_ln.gamma"),
              c.P("dec.out_ln.beta"), cf.ln_eps, W("trg.emb"), c.P("trg.bias"), logits_out, B, d, V);
   g_kernel_launches += 2;
   B200ST_LAUNCH_CHECK();

@@ -20,7 +20,7 @@ namespace b200st {
     DISPATCH_DTYPE(d0, T, __VA_ARGS__);                                                       \
   } while (0)
 
-static inline int grid_for(int64_t work, int per_block, int cap = 148 * 16) {
+static inline int grid_for(int64_t work, int per_block, int cap = 132 * 16) {
   int64_t g = (work + per_block - 1) / per_block;
   if (g < 1) g = 1;
   return (int)(g > cap ? cap : g);
@@ -377,7 +377,7 @@ int layernorm_bwd_next(const void* dy, int dy_dtype, const void* x, int x_dtype,
                        cudaStream_t s) {
   if (rows == 0 || (ablate_mask() & ABL_LN_BWD)) return 0;
   B200ST_CHECK(cols <= 1024, "layernorm_bwd supports cols <= 1024");
-  const int grid = grid_for(rows, 8 * 2, 148 * 8);      // 2 rows in flight per warp; long inputs loop
+  const int grid = grid_for(rows, 8 * 2, 132 * 8);      // 2 rows in flight per warp; long inputs loop
   const size_t smem = 2 * (size_t)cols * sizeof(float);
 #define LN_BWD_LAUNCH(CPL)                                                                                              \
   DISPATCH_UNIFORM3(dy_dtype, x_dtype, dx_dtype, TT,                                                                    \
@@ -683,7 +683,7 @@ int colsum_accum(const void* dY, int dtype, int64_t M, int N, int64_t ld, float*
   if (vec) {
     const int gx = ceil_div(N, 256);
     int gy = (int)((M + 63) / 64);
-    const int cap = (148 * 4 + gx - 1) / gx;
+    const int cap = (132 * 4 + gx - 1) / gx;
     if (gy > cap) gy = cap;
     if (gy < 1) gy = 1;
     DISPATCH_DTYPE(dtype, T, (launch_pdl(colsum_vec_kernel<T>, dim3(gx, gy), 256, 0, s, (const T*)dY, M, N, ld, db)));
@@ -1052,7 +1052,7 @@ __global__ void __launch_bounds__(256) dropout_bits_multi_kernel(const DropBitsT
 }
 int dropout_bits_multi(const DropBitsTable& t, uint64_t seed, const uint64_t* seed_ptr, uint8_t* base, cudaStream_t s) {
   if (t.n == 0 || t.goff[t.n] == 0 || (ablate_mask() & ABL_DROPBITS)) return 0;
-  launch_pdl(dropout_bits_multi_kernel, grid_for((t.goff[t.n] + 3) / 4, 256, 148 * 8), 256, 0, s, t, seed, seed_ptr, base);
+  launch_pdl(dropout_bits_multi_kernel, grid_for((t.goff[t.n] + 3) / 4, 256, 132 * 8), 256, 0, s, t, seed, seed_ptr, base);
   ++g_kernel_launches;
   B200ST_LAUNCH_CHECK();
   return 0;

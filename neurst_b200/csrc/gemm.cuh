@@ -1,8 +1,8 @@
-// GEMM problem description shared by the tcgen05 (bf16) and the SIMT (fp32) kernels.
+// GEMM problem description shared by the wgmma (bf16) and the SIMT (fp32) kernels.
 //
 //   C[b2][b1][m][n] (op)= epilogue( alpha * sum_k A[b2][b1](m,k) * B[b2][b1](n,k) )
 //
-// A is logically [M,K], B is logically [N,K] ("NT" form, the tcgen05 native form).  Each operand is
+// A is logically [M,K], B is logically [N,K] ("NT" form, the wgmma native form).  Each operand is
 // either K-major (k contiguous, ld = stride between rows m / n) or MN-major (m / n contiguous,
 // ld = stride between successive k).  Every contraction of the model (dense fwd / dgrad / wgrad,
 // QK^T, PV and their backward products, conv2 as im2col GEMM) is one GemmArgs.
@@ -13,7 +13,7 @@ namespace b200st {
 
 struct GemmOperand {
   const void* ptr;
-  int dtype;        // F32 (SIMT path) or BF16 (tcgen05 path)
+  int dtype;        // F32 (SIMT path) or BF16 (wgmma path)
   int mn_major;     // 0: K contiguous, 1: M/N contiguous
   int64_t ld;       // elements
   int64_t sb1, sb2; // batch strides (elements)
@@ -72,7 +72,7 @@ int gemm_simt_f32(const GemmArgs& g, cudaStream_t stream);
 int gemm_tc_bf16(const GemmArgs& g, cudaStream_t stream);
 // weight gradients of one backward block in one launch; returns 2 when the group does not qualify (nothing launched), 1 on error
 int gemm_wgrad_group(const GemmArgs* gs, int n, cudaStream_t stream);
-// Dispatch on operand dtype: F32 operands -> SIMT fp32 FMA kernel, BF16 operands -> tcgen05 kernel.
+// Dispatch on operand dtype: F32 operands -> SIMT fp32 FMA kernel, BF16 operands -> wgmma kernel.
 int gemm(const GemmArgs& g, cudaStream_t stream);
 
 // Fused FFN forward (tc_gemm.cu: fused_mlp_fwd_kernel): x_out(fp32, pre-initialised with the residual) += post-dropout of
@@ -85,13 +85,11 @@ int fused_mlp_fwd(const void* X, int dtype, int M, int d, int ffn, const void* W
 int fused_mlp_bwd(const void* dY, int dtype, int M, int d, int ffn, const void* W1, const void* W2, const void* F1, float scale,
                   void* dF1, float* dH, cudaStream_t stream, int* tickets = nullptr);
 
-// Debug knobs for the descriptor probe (tests only). 0 restores defaults.
+// Tile-configuration overrides (tests / tools only). 0 restores defaults.
 struct TcDebug {
-  uint32_t mn_lbo_bytes, mn_sbo_bytes, k_lbo_bytes, k_sbo_bytes;
   int force_bn;     // 0 = auto
-  int force_stages; // 0 = auto
+  int force_stages; // 0 = auto; at least 2 (one slot stays in flight while the next is issued)
   int max_ctas;     // 0 = #SMs
-  int one_cta_per_sm; // 1 = disable the 2-CTAs-per-SM mode of the BN <= 128 variants
   int reserve_sms;    // SMs left to concurrent communication kernels (set by the model while gradient all-reduces overlap)
 };
 TcDebug& tc_debug();

@@ -1,6 +1,6 @@
 // Host launchers of the non-GEMM kernels (LayerNorm, softmax, dropout casts, reductions, positions,
 // embedding, label-smoothed CE, Adam, conv front-end).  All activations are `dtype`-tagged raw pointers
-// (F32 in the fp32 parity mode, BF16 in the tcgen05 mode); statistics, residual stream, gradients of
+// (F32 in the fp32 parity mode, BF16 in the wgmma mode); statistics, residual stream, gradients of
 // parameters and the loss are always fp32.
 #pragma once
 #include "common.cuh"
@@ -102,7 +102,7 @@ struct DropBitsTable {
 int dropout_bits_multi(const DropBitsTable& t, uint64_t seed, const uint64_t* seed_ptr, uint8_t* base, cudaStream_t s);
 int fill_f32(float* x, float v, int64_t n, cudaStream_t s);
 
-// ---- fused attention (16-bit operand type `dt` = BF16 or F16, head dim 64): tcgen05 QK^T / PV with on-chip online softmax (attention.cu) ----
+// ---- fused attention (16-bit operand type `dt` = BF16 or F16, head dim 64): wgmma QK^T / PV with on-chip online softmax (attention.cu) ----
 // q/k/v/ctx/dctx/dq/dk/dv: bf16 views [B*T, ld], head h at columns [h*64, h*64+64); bias fp32 [B,Tk] or null;
 // lse fp32 [B,H,Tq] (written by forward, read by backward); dq_scratch fp32 [B*Tq, H*64] followed by [B*H*Tq] floats (rowsum(dO*O)).
 // kv_len (optional, int32 [B]): keys >= kv_len[b] all carry the -1e9 padding bias — their probabilities are exactly 0 in

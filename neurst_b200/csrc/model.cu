@@ -954,7 +954,7 @@ static int speech_front_bwd(Ctx& c, const float* src, const float* dx0, const Fr
                         cf.in_channels, C, cf.conv_layer_norm, c.st));
   }
   {
-    // dW1[9*Cin, C] += col1^T dz1   (split-K tcgen05 GEMM over all B*T1*F1 positions)
+    // dW1[9*Cin, C] += col1^T dz1   (split-K wgmma GEMM over all B*T1*F1 positions)
     GemmArgs g = gemm_defaults();
     g.M = 9 * cf.in_channels; g.N = C; g.K = (int)R1;
     g.A = GemmOperand{col1, c.adt, 1, K1p, 0, 0};

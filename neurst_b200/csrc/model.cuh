@@ -17,7 +17,7 @@ struct Config {
   int model_type;
   int d, heads, ffn, enc_layers, dec_layers, vocab, src_vocab;
   int feat, in_channels, channels, conv_layer_norm;
-  int precision;              // F32: fp32 FMA kernels (parity mode); BF16 / F16: tcgen05 kernels with that 16-bit type
+  int precision;              // F32: fp32 FMA kernels (parity mode); BF16 / F16: wgmma kernels with that 16-bit type
   float ln_eps, attention_dropout, ffn_dropout, postprocess_dropout, label_smoothing;
   int share_src_trg_embedding;
   // MODEL_MHA only

@@ -153,7 +153,7 @@ __global__ void cast16_kernel(const float* __restrict__ x, T* __restrict__ y, in
     y[i] = from_f32<T>(x[i]);
 }
 
-int grid_for(int64_t work, int per_block, int cap = 148 * 16) {
+int grid_for(int64_t work, int per_block, int cap = 132 * 16) {
   int64_t g = (work + per_block - 1) / per_block;
   if (g < 1) g = 1;
   return (int)(g > cap ? cap : g);
@@ -183,7 +183,7 @@ int optimizer_step(const OptimArgs& a, const TensorTable& tt, cudaStream_t s) {
     B200ST_CHECK(tt.n > 0 && tt.n <= 512, "clip_norm / dynamic loss scale support up to 512 parameter tensors");
     B200ST_CHECK(a.n % 8 == 0, "clip_norm / dynamic loss scale need an arena padded to a multiple of 8 elements");
     B200ST_CUDA(cudaMemsetAsync(a.tensor_sumsq, 0, sizeof(float) * (size_t)(tt.n + 1), s));
-    launch_pdl(grad_stats_kernel, grid_for(a.n, 8192, 148 * 8), 256, 0, s, (const float*)a.g, a.n, tt, a.tensor_sumsq);
+    launch_pdl(grad_stats_kernel, grid_for(a.n, 8192, 132 * 8), 256, 0, s, (const float*)a.g, a.n, tt, a.tensor_sumsq);
     ++g_kernel_launches;
     if (a.ctl) { launch_pdl(latch_unscale_kernel, 1, 32, 0, s, a.ctl); ++g_kernel_launches; }
     launch_pdl(step_control_kernel, 1, 32, 0, s, a.tensor_sumsq, tt.n, a.ctl, a.grad_scale, a.growth_steps > 0.f ? a.growth_steps : 2000.f,

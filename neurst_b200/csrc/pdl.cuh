@@ -1,6 +1,6 @@
 // Programmatic dependent launch (PDL): every kernel of the library is launched with
 // cudaLaunchAttributeProgrammaticStreamSerialization and starts with griddepcontrol.wait, so the launch latency and
-// the prologue (barrier init, TMEM allocation, tensor-map prefetch, smem tables) of kernel N+1 overlap the tail of
+// the prologue (barrier init, tensor-map prefetch, smem tables) of kernel N+1 overlap the tail of
 // kernel N — the step is ~600 short dependent kernels, i.e. launch-latency sensitive.  Correctness rule: no global memory
 // access before pdl_wait().  In a stream capture these launches become programmatic graph edges.
 #pragma once

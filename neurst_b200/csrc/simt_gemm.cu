@@ -1,8 +1,8 @@
-// fp32 CUDA-core GEMM with the same GemmArgs contract as the tcgen05 kernel.
+// fp32 CUDA-core GEMM with the same GemmArgs contract as the wgmma kernel.
 //
 // Used (a) for the fp32 parity mode — every contraction in full fp32 FMA so the CUDA path can be held to
 // the reference's own KAT tolerances (tests/neurst/**: sum(d^2) < 1e-9) at the toy shapes of those tests
-// (d = 4..16, which no tensor-core tile fits) — and (b) as the on-device cross-check of the tcgen05 kernel.
+// (d = 4..16, which no tensor-core tile fits) — and (b) as the on-device cross-check of the wgmma kernel.
 // Operands may be fp32 or bf16 in memory; accumulation is always fp32.
 #include "gemm.cuh"
 #include "pdl.cuh"

@@ -1,13 +1,13 @@
-// tcgen05 / TMEM / TMA bf16 GEMM for sm_100a.
+// wgmma / TMA 16-bit GEMM for sm_90a.
 //
-// Persistent, warp-specialised kernel (one CTA per SM, 320 threads):
-//   warp 0      : TMA producer  (cp.async.bulk.tensor -> 128B-swizzled smem ring, mbarrier complete_tx)
-//   warp 1      : TMEM allocator + single-thread tcgen05.mma issuer (fp32 accumulators in TMEM, 2 stages)
-//   warps 2..9  : epilogue (tcgen05.ld 32x32b -> registers -> fused epilogue -> 128B-swizzled smem staging box -> TMA
-//                 store, or TMA reduce-add for split-K / accumulate), 2 warps per TMEM lane quadrant
+// Persistent, warp-specialised kernel (one CTA per SM, 384 threads = 3 warpgroups):
+//   warpgroup 0    : TMA producer (one thread: cp.async.bulk.tensor -> 128B-swizzled smem ring, mbarrier complete_tx);
+//                    gives its registers to the consumers (setmaxnreg)
+//   warpgroups 1, 2: consumers, 64 rows of the 128-row tile each: wgmma.mma_async from the smem ring into fp32 register
+//                    accumulators (one k-block in flight behind the one being issued), then the fused epilogue straight
+//                    from the accumulator fragments to global memory (plain stores, or fp32 atomics for split-K / accumulate)
 // Tile: 128 x BN x 64 (BN in {64,128,256}); operands may be K-major or MN-major (wgrad / PV products),
 // batched through 4-D tensor maps; optional split-K.  Every launch is a programmatic dependent launch (pdl.cuh).
-// Measurements behind the design choices: profiles/r01_gemm_notes.md.
 //
 // Replaces the cuBLAS calls behind tf.einsum / Dense / Conv2D at the reference sites listed in
 // SURVEY.md §2.3 (K3,K4,K8,K9,K10,K11,K13,K15), e.g. neurst/layers/common_layers.py:270,276-288.
@@ -27,10 +27,11 @@ namespace {
 
 constexpr int BM = 128;
 constexpr int BK = 64;                  // 64 bf16 = 128 B = one swizzle row
-constexpr int kThreads = 320;              // TMA warp + MMA warp + 8 epilogue warps
+constexpr int kThreads = 384;           // producer warpgroup + 2 consumer warpgroups
+constexpr int kConsumerWarps = 8;
 constexpr int kSmemLimit = 232448;      // 227 KB
 constexpr uint32_t kABytes = BM * BK * 2;
-constexpr uint32_t kStagingBytes = 8 * 2 * 4096;   // per epilogue warp: two 32-row x 128-byte boxes (ping-pong)
+constexpr int kProducerRegs = 40, kConsumerRegs = 232;   // 128 * 40 + 256 * 232 = 384 * 168 registers
 
 struct TcParams {
   int M, N, K;
@@ -38,16 +39,12 @@ struct TcParams {
   int m_tiles, n_tiles, splitk, kb_total, kb_per_split;
   int64_t num_tiles;
   int stages;
-  uint32_t a_lbo, a_sbo, b_lbo, b_sbo;   // descriptor byte offsets
-  uint32_t a_kstep, b_kstep;             // smem byte advance per UMMA_K=16
-  uint32_t idesc;
   void* C;
   int c_dtype;
   int64_t ldc, c_sb1, c_sb2;
   GemmEpilogue epi;
-  int atomic;
-  int use_tma_store;    // epilogue writes C through per-warp smem boxes + TMA store (aligned, non-ragged tiles)
-  int c_reduce;         // C += (atomic / accumulate): cp.reduce.async.bulk.tensor .add
+  int atomic;           // C += through fp32 atomics (split-K or accumulate)
+  int vec2;             // C may be written two columns at a time (even N, ld and batch strides; 8-byte aligned base)
   // implicit transposed-convolution A operand (conv2 data gradient, see gemm_conv2_dgrad): A tile = a [conv_tu x conv_v]
   // patch of positions x 64 channels of dY[B, T2, F2, C], shifted by the tap; k-block kb = (tap, 64-channel chunk)
   int conv;             // 0 = off
@@ -56,8 +53,6 @@ struct TcParams {
   int conv_kpc;         // k-blocks per tap (C / 64)
   int conv_dt[4], conv_df[4], conv_wrow[4];   // per tap: time / frequency shift into dY, first row of the tap in the weight matrix
   uint32_t conv_a_bytes;                      // bytes one A box delivers (64 ch x conv_v x conv_tu x 2)
-  long long* dbg_trace; // perf experiments only: [cta][tile][8] clock64 stamps
-  int dbg_epi;          // perf experiments only (B200ST_EPI_MODE): 1 = no TMA store, 2 = no smem staging either, 3 = no TMEM read
 };
 
 struct TileCoord { int b2, b1, m_blk, n_blk, split; };
@@ -72,147 +67,84 @@ __device__ __forceinline__ TileCoord decode_tile(const TcParams& p, int64_t tile
   return t;
 }
 
-enum OutMode : int { OUT_BF16 = 0, OUT_F32 = 1, OUT_ATOMIC = 2, OUT_F16 = 3 };
-__host__ __device__ constexpr bool out_is16(int o) { return o == OUT_BF16 || o == OUT_F16; }
-
-// Cold path (ragged N, unaligned rows, on-the-fly Philox): compact, not unrolled, out of line — keeps the kernel's hot
-// code small enough for the instruction cache (the first version inlined every variant: 17 k SASS instructions).
-__device__ __noinline__ void epilogue_chunk_general(const TcParams& p, const float* acc, int m, int n0, int64_t bidx,
-                                                    int64_t boff_c, int64_t boff_mask, int64_t boff_res) {
-  const GemmEpilogue& ep = p.epi;
-#pragma unroll 1
-  for (int j = 0; j < 32; ++j) {
-    const int n = n0 + j;
-    if (n >= p.N) break;
-    const uint64_t e_idx = (uint64_t)((bidx * p.M + m) * (int64_t)p.N + n);
-    const float v = gemm_epilogue_value(ep, acc[j], m, n, boff_mask, boff_res, e_idx);
-    const int64_t idx = boff_c + (int64_t)m * p.ldc + n;
-    if (p.atomic) atomicAdd(reinterpret_cast<float*>(p.C) + idx, v);
-    else if (p.c_dtype == F32) reinterpret_cast<float*>(p.C)[idx] = ep.accumulate ? reinterpret_cast<float*>(p.C)[idx] + v : v;
-    else store_from_f32(p.C, p.c_dtype, idx, v);
+// The smem operand ring shared by the producer thread and the consumer warps: `full` barriers count the producer's
+// expect_tx arrival, `empty` barriers one arrival per consumer warp.
+struct Ring {
+  uint32_t smem, bars, stage_bytes;
+  int stages, stage;
+  uint32_t phase;
+  __device__ __forceinline__ uint32_t full() const { return bars + 8u * stage; }
+  __device__ __forceinline__ uint32_t empty(int s) const { return bars + 8u * (stages + s); }
+  __device__ __forceinline__ uint32_t slot() const { return smem + (uint32_t)stage * stage_bytes; }
+  __device__ __forceinline__ void advance() { if (++stage == stages) { stage = 0; phase ^= 1u; } }
+  __device__ __forceinline__ void init() const {
+    for (int s = 0; s < stages; ++s) { ptx::mbar_init(bars + 8u * s, 1); ptx::mbar_init(empty(s), kConsumerWarps); }
   }
-}
-
-// Per-row epilogue context: everything that does not change between the 32-column chunks of one tile row.
-struct EpiRow {
-  const float* bias;    // at n_base or null
-  const char* mask;     // at n_base or null
-  const float* res;     // at n_base or null
-  const uint8_t* bits;  // dropout keep-bits at element (row, n_base) or null
-  bool row_ok;          // m < M (rows beyond M are clipped by the TMA store; their loads are skipped)
 };
 
-// alpha / bias / relu / relu-mask / dropout bits / residual on one 32-column chunk (thread = one output row)
-template <int OUT>
-__device__ __forceinline__ void epilogue_math(const TcParams& p, const uint32_t (&r)[32], const EpiRow& e, int co, float relu_floor,
-                                              float (&v)[32]) {
-  const GemmEpilogue& ep = p.epi;
-  if (e.bias) {
-    const float4* b4 = reinterpret_cast<const float4*>(e.bias + co);
+// Consumer warpgroup `wg`: acc[64 x BN] = sum over the next nkb ring slots of A_slot[64 wg .. 64 wg + 64, :] B_slot^T.
+// The wgmma group of slot i stays in flight while slot i + 1 is issued; a slot is released once its group has retired.
+template <int BN, bool A_MN, bool B_MN, bool BF>
+__device__ __forceinline__ void consume_kblocks(float (&acc)[BN / 2], Ring& r, int nkb, int wg, int lane) {
+  int prev = -1;
+  for (int i = 0; i < nkb; ++i) {
+    ptx::mbar_wait(r.full(), r.phase);
+    const uint32_t sa = r.slot() + (uint32_t)wg * 8192u, sb = r.slot() + kABytes;
+    ptx::fence_acc(acc);
+    ptx::wgmma_fence();
 #pragma unroll
-    for (int j = 0; j < 8; ++j) {
-      const float4 bb = __ldg(b4 + j);
-      v[4 * j + 0] = fmaxf(fmaf(__uint_as_float(r[4 * j + 0]), ep.alpha, bb.x), relu_floor);
-      v[4 * j + 1] = fmaxf(fmaf(__uint_as_float(r[4 * j + 1]), ep.alpha, bb.y), relu_floor);
-      v[4 * j + 2] = fmaxf(fmaf(__uint_as_float(r[4 * j + 2]), ep.alpha, bb.z), relu_floor);
-      v[4 * j + 3] = fmaxf(fmaf(__uint_as_float(r[4 * j + 3]), ep.alpha, bb.w), relu_floor);
+    for (int k = 0; k < BK / 16; ++k)
+      ptx::WgmmaSS<BN, BF, A_MN, B_MN>::mma(acc, A_MN ? ptx::desc_mnmajor(sa, k) : ptx::desc_kmajor(sa, k),
+                                             B_MN ? ptx::desc_mnmajor(sb, k) : ptx::desc_kmajor(sb, k), (i > 0 || k > 0) ? 1 : 0);
+    ptx::wgmma_commit();
+    if (prev >= 0) {
+      ptx::wgmma_wait<1>();
+      if (lane == 0) ptx::mbar_arrive(r.empty(prev));
     }
-  } else if (ep.relu || ep.alpha != 1.f) {
-#pragma unroll
-    for (int j = 0; j < 32; ++j) v[j] = fmaxf(__uint_as_float(r[j]) * ep.alpha, relu_floor);
+    prev = r.stage;
+    r.advance();
+  }
+  ptx::wgmma_wait<0>();
+  ptx::fence_acc(acc);
+  if (prev >= 0 && lane == 0) ptx::mbar_arrive(r.empty(prev));
+}
+
+// Fused epilogue of one accumulator pair (row m, columns n and n + 1): alpha / bias / relu / mask / dropout / residual as
+// gemm_epilogue_value defines them, then a store or an fp32 atomic add.
+__device__ __forceinline__ void epilogue_pair(const TcParams& p, float a0, float a1, int m, int n, int64_t bidx, int64_t boff_c,
+                                              int64_t boff_mask, int64_t boff_res) {
+  const uint64_t e_idx = (uint64_t)((bidx * p.M + m) * (int64_t)p.N + n);
+  const bool two = n + 1 < p.N;
+  const float v0 = gemm_epilogue_value(p.epi, a0, m, n, boff_mask, boff_res, e_idx);
+  const float v1 = two ? gemm_epilogue_value(p.epi, a1, m, n + 1, boff_mask, boff_res, e_idx + 1) : 0.f;
+  const int64_t idx = boff_c + (int64_t)m * p.ldc + n;
+  if (p.atomic) {
+    float* c = reinterpret_cast<float*>(p.C) + idx;
+    if (p.vec2 && two) atomicAdd(reinterpret_cast<float2*>(c), make_float2(v0, v1));
+    else { atomicAdd(c, v0); if (two) atomicAdd(c + 1, v1); }
+  } else if (p.c_dtype == F32) {
+    float* c = reinterpret_cast<float*>(p.C) + idx;
+    if (p.vec2 && two) *reinterpret_cast<float2*>(c) = make_float2(v0, v1);
+    else { c[0] = v0; if (two) c[1] = v1; }
   } else {
-#pragma unroll
-    for (int j = 0; j < 32; ++j) v[j] = __uint_as_float(r[j]);
-  }
-  if (OUT == OUT_ATOMIC || !e.row_ok) return;
-  if (e.mask) {
-    if (ep.mask_dtype != F32) {
-      // 16-bit mask source (bf16 or fp16): "> 0" <=> sign bit clear and magnitude bits non-zero, format-independent
-      const uint4* mp = reinterpret_cast<const uint4*>(e.mask + co * 2);
-#pragma unroll
-      for (int j = 0; j < 4; ++j) {
-        const uint4 pk = __ldg(mp + j);
-        const uint32_t w[4] = {pk.x, pk.y, pk.z, pk.w};
-#pragma unroll
-        for (int i = 0; i < 4; ++i) {
-          const uint32_t lo = w[i] & 0xffffu, hi = w[i] >> 16;
-          if (!(lo != 0u && lo < 0x8000u)) v[8 * j + 2 * i] = 0.f;
-          if (!(hi != 0u && hi < 0x8000u)) v[8 * j + 2 * i + 1] = 0.f;
-        }
-      }
-    } else {
-      const float4* mp = reinterpret_cast<const float4*>(e.mask + co * 4);
-#pragma unroll
-      for (int j = 0; j < 8; ++j) {
-        const float4 f = __ldg(mp + j);
-        if (!(f.x > 0.f)) v[4 * j] = 0.f;
-        if (!(f.y > 0.f)) v[4 * j + 1] = 0.f;
-        if (!(f.z > 0.f)) v[4 * j + 2] = 0.f;
-        if (!(f.w > 0.f)) v[4 * j + 3] = 0.f;
-      }
-    }
-  }
-  if (e.bits) {
-    const uint32_t keep32 = __ldg(reinterpret_cast<const uint32_t*>(e.bits + (co >> 3)));
-#pragma unroll
-    for (int j = 0; j < 32; ++j) v[j] = ((keep32 >> j) & 1u) ? v[j] * ep.drop.scale : 0.f;
-  }
-  if (e.res) {
-    const float4* rp = reinterpret_cast<const float4*>(e.res + co);
-#pragma unroll
-    for (int j = 0; j < 8; ++j) {
-      const float4 rr = __ldg(rp + j);
-      v[4 * j + 0] += rr.x; v[4 * j + 1] += rr.y; v[4 * j + 2] += rr.z; v[4 * j + 3] += rr.w;
-    }
+    if (p.vec2 && two) reinterpret_cast<uint32_t*>(p.C)[idx >> 1] = pack2_16(v0, v1, p.c_dtype);
+    else { store_from_f32(p.C, p.c_dtype, idx, v0); if (two) store_from_f32(p.C, p.c_dtype, idx + 1, v1); }
   }
 }
 
-// Writes this lane's row of a 32-column chunk into the warp's staging box ([32 rows x 128 B], 128B-swizzled, i.e. the
-// layout the C tensor map expects): bf16 = half a row (64 B) at chunk-in-box `cb`, fp32 = the whole 128-byte row.
-template <int OUT>
-__device__ __forceinline__ void stage_chunk(uint32_t buf, int lane, int cb, const float (&v)[32]) {
-  const uint32_t row = buf + (uint32_t)lane * 128u;
-  const uint32_t sw = (uint32_t)(lane & 7);
-  if (out_is16(OUT)) {
-    constexpr int dt = OUT == OUT_F16 ? F16 : BF16;
-#pragma unroll
-    for (int j = 0; j < 4; ++j) {
-      const uint32_t h0 = pack2_16(v[8 * j], v[8 * j + 1], dt), h1 = pack2_16(v[8 * j + 2], v[8 * j + 3], dt);
-      const uint32_t h2 = pack2_16(v[8 * j + 4], v[8 * j + 5], dt), h3 = pack2_16(v[8 * j + 6], v[8 * j + 7], dt);
-      const uint32_t addr = row + ((((uint32_t)(cb * 4 + j)) ^ sw) << 4);
-      asm volatile("st.shared.v4.b32 [%0], {%1, %2, %3, %4};" ::"r"(addr), "r"(h0), "r"(h1), "r"(h2), "r"(h3) : "memory");
-    }
-  } else {
-#pragma unroll
-    for (int j = 0; j < 8; ++j) {
-      const uint32_t addr = row + ((((uint32_t)j) ^ sw) << 4);
-      asm volatile("st.shared.v4.b32 [%0], {%1, %2, %3, %4};" ::"r"(addr), "r"(__float_as_uint(v[4 * j])), "r"(__float_as_uint(v[4 * j + 1])),
-                   "r"(__float_as_uint(v[4 * j + 2])), "r"(__float_as_uint(v[4 * j + 3]))
-                   : "memory");
-    }
-  }
-}
-
-template <int BN, bool A_MN, bool B_MN, int OUT>
+template <int BN, bool A_MN, bool B_MN, bool BF>
 __global__ void __launch_bounds__(kThreads, 1)
-tc_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
-               const __grid_constant__ CUtensorMap tmC, const TcParams p) {
+tc_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, const TcParams p) {
   extern __shared__ uint8_t smem_raw[];
   constexpr uint32_t kBBytes = BN * BK * 2;
   constexpr uint32_t kStageBytes = kABytes + kBBytes;
-  constexpr uint32_t kTmemCols = (2 * BN <= 32) ? 32 : (2 * BN <= 64) ? 64 : (2 * BN <= 128) ? 128 : (2 * BN <= 256) ? 256 : 512;
 
-  const uint32_t smem_base = (ptx::smem_u32(smem_raw) + 1023u) & ~1023u;
-  const int stages = p.stages;
-  const uint32_t stage_out = smem_base + stages * kStageBytes;   // 8 warps x 2 x 4 KB epilogue staging boxes
-  const uint32_t bar_base = stage_out + kStagingBytes;           // 8-byte barriers
-  auto full_bar = [&](int s) { return bar_base + 8u * s; };
-  auto empty_bar = [&](int s) { return bar_base + 8u * (stages + s); };
-  auto tfull_bar = [&](int s) { return bar_base + 8u * (2 * stages + s); };
-  auto tempty_bar = [&](int s) { return bar_base + 8u * (2 * stages + 2 + s); };
-  const uint32_t tmem_slot = bar_base + 8u * (2 * stages + 4);
-  volatile uint32_t* tmem_slot_ptr =
-      reinterpret_cast<volatile uint32_t*>(smem_raw + (tmem_slot - ptx::smem_u32(smem_raw)));
+  Ring ring;
+  ring.smem = (ptx::smem_u32(smem_raw) + 1023u) & ~1023u;
+  ring.stages = p.stages;
+  ring.stage_bytes = kStageBytes;
+  ring.bars = ring.smem + (uint32_t)p.stages * kStageBytes;
+  ring.stage = 0; ring.phase = 0;
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
@@ -220,214 +152,83 @@ tc_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
   if (warp == 0 && lane == 0) {
     ptx::prefetch_tensormap(&tmA);
     ptx::prefetch_tensormap(&tmB);
-    if (p.use_tma_store) ptx::prefetch_tensormap(&tmC);
-    for (int s = 0; s < stages; ++s) { ptx::mbar_init(full_bar(s), 1); ptx::mbar_init(empty_bar(s), 1); }
-    for (int s = 0; s < 2; ++s) { ptx::mbar_init(tfull_bar(s), 1); ptx::mbar_init(tempty_bar(s), 8); }
+    ring.init();
     ptx::fence_mbar_init();
   }
-  if (warp == 1) {
-    ptx::tmem_alloc(tmem_slot, kTmemCols);
-    ptx::tmem_relinquish();
-  }
-  ptx::tc_fence_before();
   __syncthreads();
-  ptx::tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot_ptr;
-  pdl_wait();      // everything above (barriers, TMEM, descriptor prefetch) overlaps the previous kernel's tail
+  pdl_wait();      // everything above (barriers, descriptor prefetch) overlaps the previous kernel's tail
   pdl_trigger();
 
-  if (warp == 0) {
+  if (warp < 4) {
     // ===================== TMA producer =====================
-    if (lane == 0) {
-      int stage = 0; uint32_t phase = 0;
+    ptx::reg_dealloc<kProducerRegs>();
+    if (warp == 0 && lane == 0) {
       for (int64_t tile = blockIdx.x; tile < p.num_tiles; tile += gridDim.x) {
         const TileCoord t = decode_tile(p, tile);
         const int kb0 = t.split * p.kb_per_split;
         const int kb1 = min(p.kb_total, kb0 + p.kb_per_split);
-        int tix = (int)((tile - blockIdx.x) / gridDim.x);
         for (int kb = kb0; kb < kb1; ++kb) {
-          ptx::mbar_wait(empty_bar(stage), phase ^ 1u);
-          if (p.dbg_trace && kb == kb0 && tix < 8) p.dbg_trace[((int64_t)blockIdx.x * 8 + tix) * 8 + 0] = clock64();
-          const uint32_t sa = smem_base + stage * kStageBytes;
+          ptx::mbar_wait(ring.empty(ring.stage), ring.phase ^ 1u);
+          const uint32_t sa = ring.slot();
           const uint32_t sb = sa + kABytes;
           if constexpr (!A_MN && !B_MN) {
             if (p.conv) {
               const int tap = kb / p.conv_kpc, c0 = (kb - tap * p.conv_kpc) * BK;
-              ptx::mbar_arrive_expect_tx(full_bar(stage), p.conv_a_bytes + kBBytes);
-              ptx::tma_load_4d(sa, &tmA, full_bar(stage), c0, p.conv_df[tap], (t.m_blk % p.conv_ub) * p.conv_tu + p.conv_dt[tap],
+              ptx::mbar_arrive_expect_tx(ring.full(), p.conv_a_bytes + kBBytes);
+              ptx::tma_load_4d(sa, &tmA, ring.full(), c0, p.conv_df[tap], (t.m_blk % p.conv_ub) * p.conv_tu + p.conv_dt[tap],
                                t.m_blk / p.conv_ub);
-              ptx::tma_load_4d(sb, &tmB, full_bar(stage), c0, p.conv_wrow[tap] + t.n_blk * BN, 0, 0);
-              if (++stage == stages) { stage = 0; phase ^= 1u; }
+              ptx::tma_load_4d(sb, &tmB, ring.full(), c0, p.conv_wrow[tap] + t.n_blk * BN, 0, 0);
+              ring.advance();
               continue;
             }
           }
-          ptx::mbar_arrive_expect_tx(full_bar(stage), kStageBytes);
+          ptx::mbar_arrive_expect_tx(ring.full(), kStageBytes);
           if (A_MN) {
 #pragma unroll
             for (int c = 0; c < BM / 64; ++c)
-              ptx::tma_load_4d(sa + c * (64 * BK * 2), &tmA, full_bar(stage), t.m_blk * BM + c * 64, kb * BK, t.b1, t.b2);
+              ptx::tma_load_4d(sa + c * (64 * BK * 2), &tmA, ring.full(), t.m_blk * BM + c * 64, kb * BK, t.b1, t.b2);
           } else {
-            ptx::tma_load_4d(sa, &tmA, full_bar(stage), kb * BK, t.m_blk * BM, t.b1, t.b2);
+            ptx::tma_load_4d(sa, &tmA, ring.full(), kb * BK, t.m_blk * BM, t.b1, t.b2);
           }
           if (B_MN) {
 #pragma unroll
             for (int c = 0; c < BN / 64; ++c)
-              ptx::tma_load_4d(sb + c * (64 * BK * 2), &tmB, full_bar(stage), t.n_blk * BN + c * 64, kb * BK, t.b1, t.b2);
+              ptx::tma_load_4d(sb + c * (64 * BK * 2), &tmB, ring.full(), t.n_blk * BN + c * 64, kb * BK, t.b1, t.b2);
           } else {
-            ptx::tma_load_4d(sb, &tmB, full_bar(stage), kb * BK, t.n_blk * BN, t.b1, t.b2);
+            ptx::tma_load_4d(sb, &tmB, ring.full(), kb * BK, t.n_blk * BN, t.b1, t.b2);
           }
-          if (++stage == stages) { stage = 0; phase ^= 1u; }
+          ring.advance();
         }
-      }
-    }
-  } else if (warp == 1) {
-    // ===================== MMA issuer =====================
-    if (lane == 0) {
-      int stage = 0; uint32_t phase = 0;
-      int acc = 0; uint32_t acc_phase = 0;
-      for (int64_t tile = blockIdx.x; tile < p.num_tiles; tile += gridDim.x) {
-        const TileCoord t = decode_tile(p, tile);
-        const int kb0 = t.split * p.kb_per_split;
-        const int kb1 = min(p.kb_total, kb0 + p.kb_per_split);
-        int tix = (int)((tile - blockIdx.x) / gridDim.x);
-        if (p.dbg_trace && tix < 8) p.dbg_trace[((int64_t)blockIdx.x * 8 + tix) * 8 + 1] = clock64();
-        ptx::mbar_wait(tempty_bar(acc), acc_phase ^ 1u);
-        ptx::tc_fence_after();
-        if (p.dbg_trace && tix < 8) p.dbg_trace[((int64_t)blockIdx.x * 8 + tix) * 8 + 2] = clock64();
-        const uint32_t tmem_d = tmem_base + (uint32_t)(acc * BN);
-        for (int kb = kb0; kb < kb1; ++kb) {
-          ptx::mbar_wait(full_bar(stage), phase);
-          ptx::tc_fence_after();
-          if (p.dbg_trace && tix < 8 && kb == kb0) p.dbg_trace[((int64_t)blockIdx.x * 8 + tix) * 8 + 3] = clock64();
-          const uint32_t sa = smem_base + stage * kStageBytes;
-          const uint32_t sb = sa + kABytes;
-#pragma unroll
-          for (int k = 0; k < BK / 16; ++k) {
-            const uint64_t da = ptx::make_smem_desc_sw128(sa + k * p.a_kstep, p.a_lbo, p.a_sbo);
-            const uint64_t db = ptx::make_smem_desc_sw128(sb + k * p.b_kstep, p.b_lbo, p.b_sbo);
-            ptx::mma_f16_ss(tmem_d, da, db, p.idesc, (kb > kb0 || k > 0) ? 1u : 0u);
-          }
-          ptx::mma_commit(empty_bar(stage));     // frees the smem slot when these MMAs retire
-          if (++stage == stages) { stage = 0; phase ^= 1u; }
-        }
-        ptx::mma_commit(tfull_bar(acc));         // accumulator ready for the epilogue warps
-        if (p.dbg_trace && tix < 8) p.dbg_trace[((int64_t)blockIdx.x * 8 + tix) * 8 + 4] = clock64();
-        if (++acc == 2) { acc = 0; acc_phase ^= 1u; }
       }
     }
   } else {
-    // ===================== epilogue warps (2..9) =====================
-    // warp w may only touch TMEM lanes [32*(w%4), +32); the two warps sharing a quadrant split the columns.
-    const int quad = warp & 3;
-    const int half = (warp - 2) >> 2;              // 0 or 1
-    const int row_in_tile = quad * 32 + lane;
-    int acc = 0; uint32_t acc_phase = 0;
+    // ===================== consumer warpgroups =====================
+    ptx::reg_alloc<kConsumerRegs>();
+    const int wg = (warp >> 2) - 1, g = lane >> 2, q = lane & 3;
     const GemmEpilogue& ep = p.epi;
-    const float relu_floor = ep.relu ? 0.f : -INFINITY;
+    float acc[BN / 2];
+#pragma unroll
+    for (int i = 0; i < BN / 2; ++i) acc[i] = 0.f;
     for (int64_t tile = blockIdx.x; tile < p.num_tiles; tile += gridDim.x) {
       const TileCoord t = decode_tile(p, tile);
-      const int tix = (int)((tile - blockIdx.x) / gridDim.x);
-      if (p.dbg_trace && tix < 8 && warp == 2 && lane == 0) p.dbg_trace[((int64_t)blockIdx.x * 8 + tix) * 8 + 5] = clock64();
-      ptx::mbar_wait(tfull_bar(acc), acc_phase);
-      ptx::tc_fence_after();
-      if (p.dbg_trace && tix < 8 && warp == 2 && lane == 0) p.dbg_trace[((int64_t)blockIdx.x * 8 + tix) * 8 + 6] = clock64();
-      const int m = t.m_blk * BM + row_in_tile;
+      const int kb0 = t.split * p.kb_per_split;
+      const int kb1 = min(p.kb_total, kb0 + p.kb_per_split);
+      consume_kblocks<BN, A_MN, B_MN, BF>(acc, ring, kb1 - kb0, wg, lane);
+      const int m0 = t.m_blk * BM + wg * 64 + (warp & 3) * 16 + g;
+      const int n0 = t.n_blk * BN + 2 * q;
       const int64_t bidx = (int64_t)t.b2 * p.nb1 + t.b1;
       const int64_t boff_c = (int64_t)t.b2 * p.c_sb2 + (int64_t)t.b1 * p.c_sb1;
       const int64_t boff_mask = (int64_t)t.b2 * ep.mask_sb2 + (int64_t)t.b1 * ep.mask_sb1;
       const int64_t boff_res = (int64_t)t.b2 * ep.res_sb2 + (int64_t)t.b1 * ep.res_sb1;
-      const uint32_t taddr_row = tmem_base + ((uint32_t)(quad * 32) << 16) + (uint32_t)(acc * BN);
-      const int n_base = t.n_blk * BN;
-      const int c_begin = half * (BN / 2);
-      const bool tile_tma = p.use_tma_store && (n_base + BN <= p.N);     // warp-uniform
-      if (tile_tma) {
-        // ---- TMA-store path: TMEM -> registers -> fused math -> swizzled smem box -> cp.async.bulk.tensor store ----
-        EpiRow er;
-        er.row_ok = m < p.M;
-        er.bias = ep.bias ? ep.bias + n_base : nullptr;
-        er.mask = (ep.mask_src && er.row_ok) ? reinterpret_cast<const char*>(ep.mask_src) +
-                                                   (size_t)(boff_mask + (int64_t)m * ep.mask_ld + n_base) * (ep.mask_dtype == F32 ? 4 : 2)
-                                             : nullptr;
-        er.res = (ep.residual && er.row_ok) ? ep.residual + boff_res + (int64_t)m * ep.res_ld + n_base : nullptr;
-        er.bits = (ep.drop.p > 0.f && er.row_ok) ? ep.drop.bits + ((uint64_t)((bidx * p.M + m) * (int64_t)p.N + n_base) >> 3) : nullptr;
-        constexpr int kColsPerBox = out_is16(OUT) ? 64 : 32;
-        // BN = 64 with bf16 output: one 64-column box per quadrant, written by the half-0 warp alone
-        constexpr bool kSingle = (BN / 2 < kColsPerBox);
-        constexpr int kBoxes = kSingle ? 1 : BN / 2 / kColsPerBox;
-        const int c_begin_box = kSingle ? 0 : c_begin;
-        const int n_boxes = (kSingle && half == 1) ? 0 : kBoxes;
-        const uint32_t my_stage = stage_out + (uint32_t)(warp - 2) * 8192u;
-#pragma unroll 1
-        for (int bx = 0; bx < n_boxes; ++bx) {
-          const uint32_t buf = my_stage + (uint32_t)(bx & 1) * 4096u;
-          if (lane == 0) asm volatile("cp.async.bulk.wait_group.read 1;" ::: "memory");   // the box written 2 iterations ago is drained
-          __syncwarp();
 #pragma unroll
-          for (int cb = 0; cb < kColsPerBox / 32; ++cb) {
-            const int co = c_begin_box + bx * kColsPerBox + cb * 32;
-            uint32_t r[32];
-            if (p.dbg_epi >= 3) {
-#pragma unroll
-              for (int j = 0; j < 32; ++j) r[j] = (uint32_t)(co + j);
-            } else {
-              ptx::tmem_ld_32x32b_x32(taddr_row + (uint32_t)co, r);
-              ptx::tmem_ld_wait();
-            }
-            float v[32];
-            epilogue_math<OUT>(p, r, er, co, relu_floor, v);
-            if (p.dbg_epi >= 2) {
-              float sacc = 0.f;
-#pragma unroll
-              for (int j = 0; j < 32; ++j) sacc += v[j];
-              if (sacc == 1.2345e-30f) stage_chunk<OUT>(buf, lane, cb, v);     // keeps the math alive, never taken
-            } else {
-              stage_chunk<OUT>(buf, lane, cb, v);
-            }
-          }
-          ptx::fence_proxy_async_smem();
-          __syncwarp();
-          if (lane == 0 && p.dbg_epi == 0) {
-            const int cn = n_base + c_begin_box + bx * kColsPerBox, cm = t.m_blk * BM + quad * 32;
-            if (p.c_reduce)
-              asm volatile("cp.reduce.async.bulk.tensor.4d.global.shared::cta.add.tile.bulk_group [%0, {%2, %3, %4, %5}], [%1];"
-                           ::"l"(&tmC), "r"(buf), "r"(cn), "r"(cm), "r"(t.b1), "r"(t.b2) : "memory");
-            else
-              asm volatile("cp.async.bulk.tensor.4d.global.shared::cta.tile.bulk_group [%0, {%2, %3, %4, %5}], [%1];"
-                           ::"l"(&tmC), "r"(buf), "r"(cn), "r"(cm), "r"(t.b1), "r"(t.b2) : "memory");
-            asm volatile("cp.async.bulk.commit_group;" ::: "memory");
-          }
-        }
-      } else {
-        // ---- general path (ragged N, unaligned operands, on-the-fly Philox): per-element, compact ----
-#pragma unroll 1
-        for (int co = c_begin; co < c_begin + BN / 2; co += 32) {
-          if (n_base + co >= p.N) break;
-          uint32_t r[32];
-          __syncwarp();
-          ptx::tmem_ld_32x32b_x32(taddr_row + (uint32_t)co, r);
-          ptx::tmem_ld_wait();
-          if (m < p.M) {
-            float acc_v[32];
-#pragma unroll
-            for (int j = 0; j < 32; ++j) acc_v[j] = __uint_as_float(r[j]);
-            epilogue_chunk_general(p, acc_v, m, n_base + co, bidx, boff_c, boff_mask, boff_res);
-          }
+      for (int j = 0; j < BN / 8; ++j) {
+        const int n = n0 + 8 * j;
+        if (n < p.N) {
+          if (m0 < p.M) epilogue_pair(p, acc[4 * j], acc[4 * j + 1], m0, n, bidx, boff_c, boff_mask, boff_res);
+          if (m0 + 8 < p.M) epilogue_pair(p, acc[4 * j + 2], acc[4 * j + 3], m0 + 8, n, bidx, boff_c, boff_mask, boff_res);
         }
       }
-      ptx::tc_fence_before();
-      __syncwarp();
-      if (p.dbg_trace && tix < 8 && warp == 2 && lane == 0) p.dbg_trace[((int64_t)blockIdx.x * 8 + tix) * 8 + 7] = clock64();
-      if (lane == 0) ptx::mbar_arrive(tempty_bar(acc));
-      if (++acc == 2) { acc = 0; acc_phase ^= 1u; }
     }
-    if (lane == 0) asm volatile("cp.async.bulk.wait_group 0;" ::: "memory");   // all of this warp's TMA stores are complete
-  }
-
-  ptx::tc_fence_before();
-  __syncthreads();
-  if (warp == 1) {
-    ptx::tc_fence_after();
-    ptx::tmem_dealloc(tmem_base, kTmemCols);
   }
 }
 
@@ -436,14 +237,15 @@ tc_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
 // Grouped weight-gradient GEMM: up to kMaxGroup products  dW_g[K_in, N_out] += X_g^T dY_g  of one backward block in ONE
 // persistent launch (TF autodiff of the Dense / einsum sites of a sublayer: neurst/layers/common_layers.py:270-288,
 // multi_head_attention.py:145-215).  Each product alone has 2..16 output tiles and needs split-K over the B*T rows to fill
-// 148 SMs, i.e. every CTA reduce-adds a full 128 x 256 fp32 tile for a handful of k-blocks of MMA work and every launch pays
-// the fixed ~6 us; together the products of a block give one wave of work units with k-ranges 3-4x longer (tools/ablate_step.py:
-// the weight-gradient launches cost 0.84 ms of the 6.46 ms cfg-2 step although they run on the side stream).
-// Same pipeline as tc_gemm_kernel<256, true, true, OUT_ATOMIC>; a work unit = (product, m tile, n tile, k split).
+// the SMs, i.e. every CTA reduce-adds a full 128 x 256 fp32 tile for a handful of k-blocks of MMA work and every launch pays
+// its fixed cost; together the products of a block give one wave of work units with k-ranges several times longer.
+// Same pipeline as tc_gemm_kernel<256, true, true>; a work unit = (product, m tile, n tile, k split).
 // =============================================================================================================
 constexpr int kMaxGroup = 4;
 struct TcGroupProb {
-  CUtensorMap ta, tb, tc;
+  CUtensorMap ta, tb;
+  float* C;
+  int64_t ldc;
   int m_tiles, n_tiles, splitk, kb_total, kb_per_split, tile_begin;
   float alpha;
   int pad_;
@@ -451,7 +253,6 @@ struct TcGroupProb {
 struct TcGroup {
   TcGroupProb prob[kMaxGroup];
   int n, num_tiles, stages;
-  uint32_t idesc;
 };
 struct GroupTile { int gi, m_blk, n_blk, kb0, kb1; };
 __device__ __forceinline__ GroupTile group_tile(const TcGroup& g, int tile) {
@@ -470,23 +271,19 @@ __device__ __forceinline__ GroupTile group_tile(const TcGroup& g, int tile) {
   return t;
 }
 
+template <bool BF>
 __global__ void __launch_bounds__(kThreads, 1) tc_wgrad_group_kernel(const __grid_constant__ TcGroup grp) {
   extern __shared__ uint8_t smem_raw[];
   constexpr int BN = 256;
   constexpr uint32_t kBBytes = BN * BK * 2;
   constexpr uint32_t kStageBytes = kABytes + kBBytes;
-  constexpr uint32_t kMnLbo = 64u * BK * 2, kMnSbo = 1024u, kMnKstep = 16u * 128u;
 
-  const uint32_t smem_base = (ptx::smem_u32(smem_raw) + 1023u) & ~1023u;
-  const int stages = grp.stages;
-  const uint32_t stage_out = smem_base + stages * kStageBytes;
-  const uint32_t bar_base = stage_out + kStagingBytes;
-  auto full_bar = [&](int s) { return bar_base + 8u * s; };
-  auto empty_bar = [&](int s) { return bar_base + 8u * (stages + s); };
-  auto tfull_bar = [&](int s) { return bar_base + 8u * (2 * stages + s); };
-  auto tempty_bar = [&](int s) { return bar_base + 8u * (2 * stages + 2 + s); };
-  const uint32_t tmem_slot = bar_base + 8u * (2 * stages + 4);
-  volatile uint32_t* tmem_slot_ptr = reinterpret_cast<volatile uint32_t*>(smem_raw + (tmem_slot - ptx::smem_u32(smem_raw)));
+  Ring ring;
+  ring.smem = (ptx::smem_u32(smem_raw) + 1023u) & ~1023u;
+  ring.stages = grp.stages;
+  ring.stage_bytes = kStageBytes;
+  ring.bars = ring.smem + (uint32_t)grp.stages * kStageBytes;
+  ring.stage = 0; ring.phase = 0;
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
@@ -494,120 +291,55 @@ __global__ void __launch_bounds__(kThreads, 1) tc_wgrad_group_kernel(const __gri
     for (int i = 0; i < grp.n; ++i) {
       ptx::prefetch_tensormap(&grp.prob[i].ta);
       ptx::prefetch_tensormap(&grp.prob[i].tb);
-      ptx::prefetch_tensormap(&grp.prob[i].tc);
     }
-    for (int s = 0; s < stages; ++s) { ptx::mbar_init(full_bar(s), 1); ptx::mbar_init(empty_bar(s), 1); }
-    for (int s = 0; s < 2; ++s) { ptx::mbar_init(tfull_bar(s), 1); ptx::mbar_init(tempty_bar(s), 8); }
+    ring.init();
     ptx::fence_mbar_init();
   }
-  if (warp == 1) {
-    ptx::tmem_alloc(tmem_slot, 512);
-    ptx::tmem_relinquish();
-  }
-  ptx::tc_fence_before();
   __syncthreads();
-  ptx::tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot_ptr;
   pdl_wait();
   pdl_trigger();
 
-  if (warp == 0) {
-    if (lane == 0) {
-      int stage = 0; uint32_t phase = 0;
+  if (warp < 4) {
+    ptx::reg_dealloc<kProducerRegs>();
+    if (warp == 0 && lane == 0) {
       for (int tile = blockIdx.x; tile < grp.num_tiles; tile += gridDim.x) {
         const GroupTile t = group_tile(grp, tile);
         const CUtensorMap* ma = &grp.prob[t.gi].ta;
         const CUtensorMap* mb = &grp.prob[t.gi].tb;
         for (int kb = t.kb0; kb < t.kb1; ++kb) {
-          ptx::mbar_wait(empty_bar(stage), phase ^ 1u);
-          const uint32_t sa = smem_base + stage * kStageBytes;
+          ptx::mbar_wait(ring.empty(ring.stage), ring.phase ^ 1u);
+          const uint32_t sa = ring.slot();
           const uint32_t sb = sa + kABytes;
-          ptx::mbar_arrive_expect_tx(full_bar(stage), kStageBytes);
+          ptx::mbar_arrive_expect_tx(ring.full(), kStageBytes);
 #pragma unroll
           for (int c = 0; c < BM / 64; ++c)
-            ptx::tma_load_4d(sa + c * (64 * BK * 2), ma, full_bar(stage), t.m_blk * BM + c * 64, kb * BK, 0, 0);
+            ptx::tma_load_4d(sa + c * (64 * BK * 2), ma, ring.full(), t.m_blk * BM + c * 64, kb * BK, 0, 0);
 #pragma unroll
           for (int c = 0; c < BN / 64; ++c)
-            ptx::tma_load_4d(sb + c * (64 * BK * 2), mb, full_bar(stage), t.n_blk * BN + c * 64, kb * BK, 0, 0);
-          if (++stage == stages) { stage = 0; phase ^= 1u; }
+            ptx::tma_load_4d(sb + c * (64 * BK * 2), mb, ring.full(), t.n_blk * BN + c * 64, kb * BK, 0, 0);
+          ring.advance();
         }
-      }
-    }
-  } else if (warp == 1) {
-    if (lane == 0) {
-      int stage = 0; uint32_t phase = 0;
-      int acc = 0; uint32_t acc_phase = 0;
-      for (int tile = blockIdx.x; tile < grp.num_tiles; tile += gridDim.x) {
-        const GroupTile t = group_tile(grp, tile);
-        ptx::mbar_wait(tempty_bar(acc), acc_phase ^ 1u);
-        ptx::tc_fence_after();
-        const uint32_t tmem_d = tmem_base + (uint32_t)(acc * BN);
-        for (int kb = t.kb0; kb < t.kb1; ++kb) {
-          ptx::mbar_wait(full_bar(stage), phase);
-          ptx::tc_fence_after();
-          const uint32_t sa = smem_base + stage * kStageBytes;
-          const uint32_t sb = sa + kABytes;
-#pragma unroll
-          for (int k = 0; k < BK / 16; ++k) {
-            const uint64_t da = ptx::make_smem_desc_sw128(sa + k * kMnKstep, kMnLbo, kMnSbo);
-            const uint64_t db = ptx::make_smem_desc_sw128(sb + k * kMnKstep, kMnLbo, kMnSbo);
-            ptx::mma_f16_ss(tmem_d, da, db, grp.idesc, (kb > t.kb0 || k > 0) ? 1u : 0u);
-          }
-          ptx::mma_commit(empty_bar(stage));
-          if (++stage == stages) { stage = 0; phase ^= 1u; }
-        }
-        ptx::mma_commit(tfull_bar(acc));
-        if (++acc == 2) { acc = 0; acc_phase ^= 1u; }
       }
     }
   } else {
-    const int quad = warp & 3;
-    const int half = (warp - 2) >> 2;
-    int acc = 0; uint32_t acc_phase = 0;
-    const uint32_t my_stage = stage_out + (uint32_t)(warp - 2) * 8192u;
+    ptx::reg_alloc<kConsumerRegs>();
+    const int wg = (warp >> 2) - 1, g = lane >> 2, q = lane & 3;
+    float acc[BN / 2];
+#pragma unroll
+    for (int i = 0; i < BN / 2; ++i) acc[i] = 0.f;
     for (int tile = blockIdx.x; tile < grp.num_tiles; tile += gridDim.x) {
       const GroupTile t = group_tile(grp, tile);
-      const CUtensorMap* mc = &grp.prob[t.gi].tc;
       const float alpha = grp.prob[t.gi].alpha;
-      ptx::mbar_wait(tfull_bar(acc), acc_phase);
-      ptx::tc_fence_after();
-      const uint32_t taddr_row = tmem_base + ((uint32_t)(quad * 32) << 16) + (uint32_t)(acc * BN);
-      const int c_begin = half * (BN / 2);
-#pragma unroll 1
-      for (int bx = 0; bx < BN / 2 / 32; ++bx) {
-        const uint32_t buf = my_stage + (uint32_t)(bx & 1) * 4096u;
-        if (lane == 0) asm volatile("cp.async.bulk.wait_group.read 1;" ::: "memory");
-        __syncwarp();
-        const int co = c_begin + bx * 32;
-        uint32_t r[32];
-        ptx::tmem_ld_32x32b_x32(taddr_row + (uint32_t)co, r);
-        ptx::tmem_ld_wait();
-        float v[32];
+      consume_kblocks<BN, true, true, BF>(acc, ring, t.kb1 - t.kb0, wg, lane);
+      // M % 128 == 0 and N % 256 == 0 (gemm_wgrad_group): no edge tiles
+      float* c = grp.prob[t.gi].C + (int64_t)(t.m_blk * BM + wg * 64 + (warp & 3) * 16 + g) * grp.prob[t.gi].ldc + t.n_blk * BN + 2 * q;
+      const int64_t row8 = 8 * grp.prob[t.gi].ldc;
 #pragma unroll
-        for (int j = 0; j < 32; ++j) v[j] = __uint_as_float(r[j]) * alpha;
-        stage_chunk<OUT_ATOMIC>(buf, lane, 0, v);
-        ptx::fence_proxy_async_smem();
-        __syncwarp();
-        if (lane == 0) {
-          const int cn = t.n_blk * BN + co, cm = t.m_blk * BM + quad * 32;
-          asm volatile("cp.reduce.async.bulk.tensor.4d.global.shared::cta.add.tile.bulk_group [%0, {%2, %3, %4, %5}], [%1];"
-                       ::"l"(mc), "r"(buf), "r"(cn), "r"(cm), "r"(0), "r"(0) : "memory");
-          asm volatile("cp.async.bulk.commit_group;" ::: "memory");
-        }
+      for (int j = 0; j < BN / 8; ++j) {
+        atomicAdd(reinterpret_cast<float2*>(c + 8 * j), make_float2(acc[4 * j] * alpha, acc[4 * j + 1] * alpha));
+        atomicAdd(reinterpret_cast<float2*>(c + row8 + 8 * j), make_float2(acc[4 * j + 2] * alpha, acc[4 * j + 3] * alpha));
       }
-      ptx::tc_fence_before();
-      __syncwarp();
-      if (lane == 0) ptx::mbar_arrive(tempty_bar(acc));
-      if (++acc == 2) { acc = 0; acc_phase ^= 1u; }
     }
-    if (lane == 0) asm volatile("cp.async.bulk.wait_group 0;" ::: "memory");
-  }
-
-  ptx::tc_fence_before();
-  __syncthreads();
-  if (warp == 1) {
-    ptx::tc_fence_after();
-    ptx::tmem_dealloc(tmem_base, 512);
   }
 }
 
@@ -616,16 +348,14 @@ __global__ void __launch_bounds__(kThreads, 1) tc_wgrad_group_kernel(const __gri
 // Fused Transformer FFN forward (SURVEY K11):  x_out += dropout_post( dropout_ffn(relu(X W1 + b1)) W2 + b2 )
 //   neurst/layers/common_layers.py:145-160 (TransformerFFN) inside the pre-norm wrapper (:73-85); X = LN(x_in) (16-bit),
 //   x_out is pre-initialised with the residual x_in by the LayerNorm kernel.
-// One CTA = (128-row tile, slice of the hidden dimension).  The X tile (128 x d, d <= 256) stays in shared memory; the hidden
-// activations of a 128-column chunk are produced in TMEM (GEMM1), turned into the 16-bit A operand of GEMM2 in shared
-// memory by the epilogue warps (bias, ReLU, dropout) — and TMA-stored to HBM only because the backward pass needs them —
-// while GEMM2 accumulates the [128 x d] output tile in TMEM across all chunks.  Only the weights stream (L2 -> smem):
-// 2 x 64 KB per chunk for 2 x 1024 MMA cycles, vs 4 x that for the two unfused GEMMs, and the [M, ffn] hidden tensor is
-// never read back.  Slices of the hidden dimension reduce into x_out with fp32 TMA reduce-add (dropout is a mask: linear).
-//   warp 0: TMA producer (X once, then weight stages in consumption order)     warp 1: MMA issuer
-//   warps 2-9: epilogue (hidden chunk: TMEM -> regs -> smem operand + TMA store; final: TMEM -> regs -> smem -> reduce-add)
-//   TMEM: [0,256) output accumulator, [256,384) / [384,512) hidden accumulators (double buffered)
-//   smem: X 64 KB | H 2 x 32 KB | weight ring 3 x 32 KB (reused as the output staging boxes at the end)
+// One CTA = (128-row tile, slice of the hidden dimension); each consumer warpgroup owns 64 of the rows.  The X tile
+// (128 x D, D in {128, 256}) stays in shared memory; the hidden activations of a 128-column chunk are accumulated in
+// registers (GEMM1), get bias, ReLU and dropout there, are written to HBM only because the backward pass needs them, and
+// go, packed to 16 bits, straight back into the tensor cores as the register A operand of GEMM2, which accumulates the
+// [64 x D] output rows in registers across all chunks.  Only the weights stream (L2 -> smem), and the [M, ffn] hidden
+// tensor is never read back.  Slices of the hidden dimension reduce into x_out with fp32 atomics (dropout is a mask: linear).
+//   warpgroup 0: TMA producer (X once, then per chunk the W1 stages and the W2 stages, in consumption order)
+//   smem: X 64 KB | weight ring 3 x 32 KB
 // =============================================================================================================
 struct MlpParams {
   int M, d, ffn;
@@ -633,72 +363,54 @@ struct MlpParams {
   int splits;                  // hidden slices (gridDim.x = m_tiles * splits)
   const float* b1; const float* b2;
   DropoutSpec drop_ffn, drop_post;
-  uint32_t idesc_g1, idesc_g2;
   // backward (dgrad chain) variant: hidden epilogue = alpha * acc masked by (mask_src > 0), no bias / ReLU / dropout bits
   int relu;
   float alpha;
   const void* mask_src; int64_t mask_ld;
+  uint16_t* F1;                // [M, ffn] hidden activations (forward) / hidden gradient (backward), 16-bit
+  float* out;                  // [M, d] fp32, added into
   int* tickets;                // deterministic mode: [m_tiles] zero-initialised; slice s adds after slices < s (self-resetting)
 };
 constexpr int kMlpStages = 3;
 constexpr uint32_t kMlpStageBytes = 32768;
-constexpr uint32_t kMlpXBytes = 65536, kMlpHBytes = 32768;
-constexpr size_t kMlpSmem = 1024 + kMlpXBytes + 2 * kMlpHBytes + kMlpStages * kMlpStageBytes + 256 + 1024;
+constexpr uint32_t kMlpXBytes = 65536;
+constexpr size_t kMlpSmem = 1024 + kMlpXBytes + kMlpStages * kMlpStageBytes + 256;
 
 // B_MN: weights as MN-major B operands (forward: W1 [d, ffn], W2 [ffn, d] in the TF [in, out] layout) or K-major (backward:
 // the same arrays read transposed: G1 uses W2 rows = hidden units, G2 uses W1 rows = model dims)
-template <int DT, bool B_MN>
+template <int DT, bool B_MN, int D>
 __global__ void __launch_bounds__(kThreads, 1)
 fused_mlp_fwd_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_constant__ CUtensorMap tmW1,
-                     const __grid_constant__ CUtensorMap tmW2, const __grid_constant__ CUtensorMap tmF1,
-                     const __grid_constant__ CUtensorMap tmOut, const MlpParams p) {
+                     const __grid_constant__ CUtensorMap tmW2, const MlpParams p) {
   extern __shared__ uint8_t smem_raw[];
+  constexpr bool BF = DT == BF16;
+  constexpr int kbx = D / BK;                  // k-blocks of GEMM1
   const uint32_t base = (ptx::smem_u32(smem_raw) + 1023u) & ~1023u;
   const uint32_t sX = base;
-  const uint32_t sH = sX + kMlpXBytes;
-  const uint32_t sW = sH + 2 * kMlpHBytes;
+  const uint32_t sW = sX + kMlpXBytes;
   const uint32_t bars = sW + kMlpStages * kMlpStageBytes;
   const uint32_t x_full = bars;
   auto w_full = [&](int s2) { return bars + 8u * (1 + s2); };
   auto w_empty = [&](int s2) { return bars + 8u * (1 + kMlpStages + s2); };
-  auto ht_full = [&](int b) { return bars + 8u * (1 + 2 * kMlpStages + b); };        // hidden accumulator ready (MMA -> epilogue)
-  auto ht_empty = [&](int b) { return bars + 8u * (3 + 2 * kMlpStages + b); };       // hidden accumulator drained (epilogue -> MMA)
-  auto hs_full = [&](int b) { return bars + 8u * (5 + 2 * kMlpStages + b); };        // hidden operand in smem (epilogue -> MMA)
-  auto hs_empty = [&](int b) { return bars + 8u * (7 + 2 * kMlpStages + b); };       // GEMM2 finished reading it (MMA -> epilogue)
-  const uint32_t out_full = bars + 8u * (9 + 2 * kMlpStages);
-  const uint32_t tmem_slot = bars + 8u * (10 + 2 * kMlpStages);
-  const uint32_t bias_off = bars + 256u;           // 1 KB: [2][128] bias floats of the current / next hidden chunk
-  volatile uint32_t* tmem_slot_ptr = reinterpret_cast<volatile uint32_t*>(smem_raw + (tmem_slot - ptx::smem_u32(smem_raw)));
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int m_blk = blockIdx.x / p.splits, split = blockIdx.x % p.splits;
   const int C = p.chunks_per_cta;
   const int chunk0 = split * C;
-  const int kbx = p.d / BK;                    // k-blocks of GEMM1 (<= 4)
 
   if (warp == 0 && lane == 0) {
     ptx::prefetch_tensormap(&tmX); ptx::prefetch_tensormap(&tmW1); ptx::prefetch_tensormap(&tmW2);
-    ptx::prefetch_tensormap(&tmF1); ptx::prefetch_tensormap(&tmOut);
     ptx::mbar_init(x_full, 1);
-    for (int s2 = 0; s2 < kMlpStages; ++s2) { ptx::mbar_init(w_full(s2), 1); ptx::mbar_init(w_empty(s2), 1); }
-    for (int b = 0; b < 2; ++b) {
-      ptx::mbar_init(ht_full(b), 1); ptx::mbar_init(ht_empty(b), 8);
-      ptx::mbar_init(hs_full(b), 8); ptx::mbar_init(hs_empty(b), 1);
-    }
-    ptx::mbar_init(out_full, 1);
+    for (int s2 = 0; s2 < kMlpStages; ++s2) { ptx::mbar_init(w_full(s2), 1); ptx::mbar_init(w_empty(s2), kConsumerWarps); }
     ptx::fence_mbar_init();
   }
-  if (warp == 1) { ptx::tmem_alloc_n<512>(tmem_slot); ptx::tmem_relinquish(); }
-  ptx::tc_fence_before();
   __syncthreads();
-  ptx::tc_fence_after();
-  const uint32_t tmem = *tmem_slot_ptr;
   pdl_wait();
   pdl_trigger();
-  const uint32_t tOut = tmem, tH0 = tmem + 256;
 
-  if (warp == 0) {
-    if (lane == 0) {
+  if (warp < 4) {
+    ptx::reg_dealloc<kProducerRegs>();
+    if (warp == 0 && lane == 0) {
       ptx::mbar_arrive_expect_tx(x_full, (uint32_t)kbx * kABytes);
       for (int kb = 0; kb < kbx; ++kb) ptx::tma_load_4d(sX + kb * kABytes, &tmX, x_full, kb * BK, m_blk * BM, 0, 0);
       int it = 0;
@@ -708,14 +420,14 @@ fused_mlp_fwd_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_const
         dst = sW + st * kMlpStageBytes;
         ++it;
       };
-      auto load_w1 = [&](int c) {          // GEMM1 B operand of chunk c: [K = d rows, N = 128 cols] as 2 k-blocks per stage
+      for (int c = 0; c < C; ++c) {
+        // GEMM1 B operand of chunk c: [K = d rows, N = 128 cols] as 2 k-blocks per stage
         const int n0 = (chunk0 + c) * 128;
         for (int s2 = 0; s2 < kbx; s2 += 2) {
           int st; uint32_t dst;
           stage_wait(st, dst);
-          const int nkb = min(2, kbx - s2);
-          ptx::mbar_arrive_expect_tx(w_full(st), (uint32_t)nkb * 16384u);
-          for (int j = 0; j < nkb; ++j) {
+          ptx::mbar_arrive_expect_tx(w_full(st), 2u * 16384u);
+          for (int j = 0; j < 2; ++j) {
             if (B_MN) {
               for (int i = 0; i < 2; ++i)
                 ptx::tma_load_4d(dst + j * 16384 + i * 8192, &tmW1, w_full(st), n0 + i * 64, (s2 + j) * BK, 0, 0);
@@ -724,216 +436,123 @@ fused_mlp_fwd_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_const
             }
           }
         }
-      };
-      auto load_w2 = [&](int c) {          // GEMM2 B operand of chunk c: [K = 128 hidden rows, N = d cols], one k-block per stage
-        const int k0 = (chunk0 + c) * 128;
+        // GEMM2 B operand of chunk c: [K = 128 hidden rows, N = d cols], one k-block per stage
         for (int kb = 0; kb < 2; ++kb) {
           int st; uint32_t dst;
           stage_wait(st, dst);
-          ptx::mbar_arrive_expect_tx(w_full(st), (uint32_t)(p.d / 64) * 8192u);
+          ptx::mbar_arrive_expect_tx(w_full(st), (uint32_t)(D / 64) * 8192u);
           if (B_MN) {
-            for (int i = 0; i < p.d / 64; ++i)
-              ptx::tma_load_4d(dst + i * 8192, &tmW2, w_full(st), i * 64, k0 + kb * BK, 0, 0);
+            for (int i = 0; i < D / 64; ++i)
+              ptx::tma_load_4d(dst + i * 8192, &tmW2, w_full(st), i * 64, n0 + kb * BK, 0, 0);
           } else {
-            ptx::tma_load_4d(dst, &tmW2, w_full(st), k0 + kb * BK, 0, 0, 0);                        // [d rows x 64 k]
+            ptx::tma_load_4d(dst, &tmW2, w_full(st), n0 + kb * BK, 0, 0, 0);                        // [d rows x 64 k]
           }
         }
-      };
-      // consumption order of the MMA warp: GEMM1 runs two chunks ahead of GEMM2 (see there)
-      load_w1(0);
-      if (C > 1) load_w1(1);
-      for (int c = 0; c < C; ++c) { if (c + 2 < C) load_w1(c + 2); load_w2(c); }
-    }
-  } else if (warp == 1) {
-    if (lane == 0) {
-      int it = 0;
-      auto stage_get = [&](uint32_t& src) {
-        const int st = it % kMlpStages;
-        ptx::mbar_wait(w_full(st), ((uint32_t)(it / kMlpStages)) & 1u);
-        ptx::tc_fence_after();
-        src = sW + st * kMlpStageBytes;
-        ++it;
-        return st;
-      };
-      auto gemm1 = [&](int c) {
-        const int b = c & 1;
-        ptx::mbar_wait(ht_empty(b), (((uint32_t)c >> 1) & 1u) ^ 1u);
-        ptx::tc_fence_after();
-        const uint32_t tH = tH0 + (uint32_t)b * 128u;
-        for (int s2 = 0; s2 < kbx; s2 += 2) {
-          uint32_t src;
-          const int st = stage_get(src);
-          const int nkb = min(2, kbx - s2);
-          for (int j = 0; j < nkb; ++j) {
-            const uint32_t sa = sX + (uint32_t)(s2 + j) * kABytes, sb = src + (uint32_t)j * 16384u;
-#pragma unroll
-            for (int k = 0; k < BK / 16; ++k)
-              ptx::mma_f16_ss(tH, ptx::make_smem_desc_sw128(sa + k * 32, 16, 1024),
-                              B_MN ? ptx::make_smem_desc_sw128(sb + k * 2048, 8192, 1024) : ptx::make_smem_desc_sw128(sb + k * 32, 16, 1024),
-                              p.idesc_g1, (s2 + j > 0 || k > 0) ? 1u : 0u);
-          }
-          ptx::mma_commit(w_empty(st));
-        }
-        ptx::mma_commit(ht_full(b));
-      };
-      auto gemm2 = [&](int c) {
-        const int b = c & 1;
-        ptx::mbar_wait(hs_full(b), ((uint32_t)c >> 1) & 1u);
-        ptx::tc_fence_after();
-        for (int kb = 0; kb < 2; ++kb) {
-          uint32_t src;
-          const int st = stage_get(src);
-          const uint32_t sa = sH + (uint32_t)b * kMlpHBytes + (uint32_t)kb * kABytes;
-#pragma unroll
-          for (int k = 0; k < BK / 16; ++k)
-            ptx::mma_f16_ss(tOut, ptx::make_smem_desc_sw128(sa + k * 32, 16, 1024),
-                            B_MN ? ptx::make_smem_desc_sw128(src + k * 2048, 8192, 1024) : ptx::make_smem_desc_sw128(src + k * 32, 16, 1024),
-                            p.idesc_g2, (c > 0 || kb > 0 || k > 0) ? 1u : 0u);
-          ptx::mma_commit(w_empty(st));
-        }
-        ptx::mma_commit(hs_empty(b));
-      };
-      ptx::mbar_wait(x_full, 0);
-      ptx::tc_fence_after();
-      // GEMM1 of chunk c + 2 is issued BEFORE GEMM2 of chunk c: GEMM2(c) has to wait for the epilogue warps to turn the hidden
-      // accumulator of chunk c into its smem operand, and the tensor pipe spends that time on the next-but-one GEMM1 (its TMEM
-      // buffer (c & 1) is free as soon as the epilogue of chunk c has loaded its registers)
-      gemm1(0);
-      if (C > 1) gemm1(1);
-      for (int c = 0; c < C; ++c) { if (c + 2 < C) gemm1(c + 2); gemm2(c); }
-      ptx::mma_commit(out_full);
+      }
     }
   } else {
-    const int quad = warp & 3, half = (warp - 2) >> 2;
-    const int m = m_blk * BM + quad * 32 + lane;
-    const bool row_ok = m < p.M;
-    const uint32_t lane_addr = (uint32_t)(quad * 32) << 16;
-    // ---- hidden chunks: TMEM -> bias, ReLU, dropout (forward) / relu'-dropout' mask (backward) -> 16-bit A operand of GEMM2
-    // (+ TMA store: the backward pass / the W1 weight gradient need it).  With 230 KB of shared memory there is no L1 left, so
-    // every global operand of the epilogue is fetched one chunk AHEAD: the 64 bias values of each column half go through a
-    // 1 KB double buffer in shared memory (loaded by the quad-0 warps), the dropout keep-words / the 16-bit mask row of the
-    // thread sit in registers across the wait for the accumulator.
-    float* bias_s = reinterpret_cast<float*>(smem_raw + (bias_off - ptx::smem_u32(smem_raw)));      // [2][128]
+    ptx::reg_alloc<kConsumerRegs>();
+    const int wg = (warp >> 2) - 1, g = lane >> 2, q = lane & 3;
+    const int m0 = m_blk * BM + wg * 64 + (warp & 3) * 16 + g;       // this thread's rows: m0 and m0 + 8
     const bool use_bits = p.drop_ffn.p > 0.f;
     const float dscale = use_bits ? p.drop_ffn.scale : 1.f;
     const float hidden_floor = p.relu ? 0.f : -INFINITY;
-    auto epi_bar = [] { asm volatile("bar.sync 1, 256;" ::: "memory"); };
-    uint32_t keep_n[2] = {0xffffffffu, 0xffffffffu};
-    uint4 mask_n[B_MN ? 1 : 8];
-    auto prefetch = [&](int c) {          // global operands of chunk c
-      const int n0 = (chunk0 + c) * 128 + half * 64;
-      if (quad == 0 && p.b1) {
-        bias_s[(c & 1) * 128 + half * 64 + lane] = __ldg(p.b1 + n0 + lane);
-        bias_s[(c & 1) * 128 + half * 64 + 32 + lane] = __ldg(p.b1 + n0 + 32 + lane);
-      }
-      if (use_bits && row_ok) {
-        const uint2 w = __ldg(reinterpret_cast<const uint2*>(p.drop_ffn.bits + ((uint64_t)((int64_t)m * p.ffn + n0) >> 3)));
-        keep_n[0] = w.x; keep_n[1] = w.y;
-      }
-      if (!B_MN) {
-        if (p.mask_src && row_ok) {
-          const uint4* mp = reinterpret_cast<const uint4*>(reinterpret_cast<const char*>(p.mask_src) + ((int64_t)m * p.mask_ld + n0) * 2);
-#pragma unroll
-          for (int j = 0; j < 8; ++j) mask_n[j] = __ldg(mp + j);
-        } else {
-#pragma unroll
-          for (int j = 0; j < 8; ++j) mask_n[j] = make_uint4(0, 0, 0, 0);
-        }
-      }
+    int it = 0;
+    auto stage_get = [&](uint32_t& src) {
+      const int st = it % kMlpStages;
+      ptx::mbar_wait(w_full(st), ((uint32_t)(it / kMlpStages)) & 1u);
+      src = sW + st * kMlpStageBytes;
+      ++it;
+      return st;
     };
-    prefetch(0);
-    epi_bar();
+    float out[D / 2];
+#pragma unroll
+    for (int i = 0; i < D / 2; ++i) out[i] = 0.f;
+    ptx::mbar_wait(x_full, 0);
     for (int c = 0; c < C; ++c) {
-      const int b = c & 1;
-      const int n0 = (chunk0 + c) * 128 + half * 64;          // this warp's 64 hidden columns
-      const uint32_t keep[2] = {keep_n[0], keep_n[1]};
-      uint4 mask_c[B_MN ? 1 : 8];
-      if (!B_MN) {
+      // The 128 hidden columns of chunk c go through the registers as two halves of 64 (GEMM1 half, epilogue, GEMM2 k-block),
+      // so that the [64 x D] output accumulator and the hidden fragments fit the register file; the W1 stages are read by
+      // both halves and released after the second.
+      uint32_t w1src[kbx / 2];
+      int w1st[kbx / 2];
 #pragma unroll
-        for (int j = 0; j < 8; ++j) mask_c[j] = mask_n[j];
-      }
-      if (c + 1 < C) prefetch(c + 1);                          // in flight across the wait for the accumulator
-      ptx::mbar_wait(ht_full(b), ((uint32_t)c >> 1) & 1u);
-      ptx::tc_fence_after();
-      float v[2][32];
-      {
-        uint32_t r0[32], r1[32];
-        __syncwarp();
-        ptx::tmem_ld_32x32b_x32(tH0 + (uint32_t)b * 128u + lane_addr + (uint32_t)(half * 64), r0);
-        ptx::tmem_ld_32x32b_x32(tH0 + (uint32_t)b * 128u + lane_addr + (uint32_t)(half * 64 + 32), r1);
-        ptx::tmem_ld_wait();
-        ptx::tc_fence_before();
-        __syncwarp();
-        if (lane == 0) ptx::mbar_arrive(ht_empty(b));           // the accumulator can be overwritten by GEMM1 of chunk c + 2
-        const float* bs = bias_s + b * 128 + half * 64;
+      for (int h = 0; h < 2; ++h) {
+        // ---- GEMM1: hidden accumulator [64 x 64] ----
+        float hid[32];
 #pragma unroll
-        for (int hh = 0; hh < 2; ++hh) {
-          const uint32_t (&r)[32] = hh ? r1 : r0;
+        for (int i = 0; i < 32; ++i) hid[i] = 0.f;
+        if (h == 0) {
 #pragma unroll
-          for (int j4 = 0; j4 < 8; ++j4) {
-            float4 bb = make_float4(0.f, 0.f, 0.f, 0.f);
-            if (p.b1) bb = *reinterpret_cast<const float4*>(bs + hh * 32 + 4 * j4);          // broadcast LDS.128
-            v[hh][4 * j4 + 0] = fmaxf(fmaf(__uint_as_float(r[4 * j4 + 0]), p.alpha, bb.x), hidden_floor);
-            v[hh][4 * j4 + 1] = fmaxf(fmaf(__uint_as_float(r[4 * j4 + 1]), p.alpha, bb.y), hidden_floor);
-            v[hh][4 * j4 + 2] = fmaxf(fmaf(__uint_as_float(r[4 * j4 + 2]), p.alpha, bb.z), hidden_floor);
-            v[hh][4 * j4 + 3] = fmaxf(fmaf(__uint_as_float(r[4 * j4 + 3]), p.alpha, bb.w), hidden_floor);
-          }
-          if (use_bits) {
-            const uint32_t k32 = keep[hh];
+          for (int s2 = 0; s2 < kbx / 2; ++s2) w1st[s2] = stage_get(w1src[s2]);
+        }
+        ptx::fence_acc(hid);
+        ptx::wgmma_fence();
 #pragma unroll
-            for (int j = 0; j < 32; ++j) v[hh][j] = ((k32 >> j) & 1u) ? v[hh][j] * dscale : 0.f;
-          }
-          if (!B_MN) {
-            // 16-bit mask source (bf16 / fp16): "> 0" <=> sign clear and magnitude bits non-zero
+        for (int kb = 0; kb < kbx; ++kb) {
+          const uint32_t sa = sX + (uint32_t)kb * kABytes + (uint32_t)wg * 8192u;
+          const uint32_t sb = w1src[kb >> 1] + (uint32_t)(kb & 1) * 16384u + (uint32_t)h * 8192u;
 #pragma unroll
-            for (int j = 0; j < 4; ++j) {
-              const uint4 pk = mask_c[hh * 4 + j];
-              const uint32_t w[4] = {pk.x, pk.y, pk.z, pk.w};
+          for (int k = 0; k < BK / 16; ++k)
+            ptx::WgmmaSS<64, BF, 0, B_MN>::mma(hid, ptx::desc_kmajor(sa, k), B_MN ? ptx::desc_mnmajor(sb, k) : ptx::desc_kmajor(sb, k),
+                                               (kb > 0 || k > 0) ? 1 : 0);
+        }
+        ptx::wgmma_commit();
+        ptx::wgmma_wait<0>();
+        ptx::fence_acc(hid);
+        if (h == 1 && lane == 0) {
 #pragma unroll
-              for (int i = 0; i < 4; ++i) {
-                const uint32_t lo = w[i] & 0xffffu, hi = w[i] >> 16;
-                if (!(lo != 0u && lo < 0x8000u)) v[hh][8 * j + 2 * i] = 0.f;
-                if (!(hi != 0u && hi < 0x8000u)) v[hh][8 * j + 2 * i + 1] = 0.f;
-              }
+          for (int s2 = 0; s2 < kbx / 2; ++s2) ptx::mbar_arrive(w_empty(w1st[s2]));
+        }
+        // ---- hidden epilogue on the fragments: bias, ReLU, dropout (forward) / relu'-dropout' mask (backward); store; pack ----
+        const int n0 = (chunk0 + c) * 128 + h * 64 + 2 * q;
+        uint32_t a16[4][4];
+#pragma unroll
+        for (int j = 0; j < 8; ++j) {
+          const int n = n0 + 8 * j;
+          float2 bb = make_float2(0.f, 0.f);
+          if (p.b1) bb = __ldg(reinterpret_cast<const float2*>(p.b1 + n));
+#pragma unroll
+          for (int hr = 0; hr < 2; ++hr) {
+            const int m = m0 + 8 * hr;
+            const bool row_ok = m < p.M;
+            float v0 = fmaxf(fmaf(hid[4 * j + 2 * hr], p.alpha, bb.x), hidden_floor);
+            float v1 = fmaxf(fmaf(hid[4 * j + 2 * hr + 1], p.alpha, bb.y), hidden_floor);
+            if (use_bits && row_ok) {
+              const uint32_t kb = (uint32_t)__ldg(p.drop_ffn.bits + ((uint64_t)((int64_t)m * p.ffn + n) >> 3)) >> (2 * q);
+              v0 = (kb & 1u) ? v0 * dscale : 0.f;
+              v1 = (kb & 2u) ? v1 * dscale : 0.f;
             }
+            if (!B_MN && p.mask_src && row_ok) {
+              // 16-bit mask source (bf16 / fp16): "> 0" <=> sign clear and magnitude bits non-zero
+              const uint32_t w = __ldg(reinterpret_cast<const uint32_t*>(reinterpret_cast<const uint16_t*>(p.mask_src) + (int64_t)m * p.mask_ld + n));
+              const uint32_t lo = w & 0xffffu, hi = w >> 16;
+              if (!(lo != 0u && lo < 0x8000u)) v0 = 0.f;
+              if (!(hi != 0u && hi < 0x8000u)) v1 = 0.f;
+            }
+            const uint32_t pk = pack2_16(v0, v1, DT);
+            if (row_ok) *reinterpret_cast<uint32_t*>(p.F1 + (int64_t)m * p.ffn + n) = pk;
+            a16[j >> 1][(j & 1) * 2 + hr] = pk;
           }
         }
-      }
-      // operand buffer b: GEMM2 of chunk c - 2 has finished reading it, and this warp's own TMA store of chunk c - 2 too
-      ptx::mbar_wait(hs_empty(b), (((uint32_t)c >> 1) & 1u) ^ 1u);
-      if (lane == 0) asm volatile("cp.async.bulk.wait_group.read 1;" ::: "memory");
-      __syncwarp();
-      const uint32_t tile = sH + (uint32_t)b * kMlpHBytes + (uint32_t)half * kABytes + (uint32_t)(quad * 32) * 128u;
-      stage_chunk<DT == F16 ? OUT_F16 : OUT_BF16>(tile, lane, 0, v[0]);
-      stage_chunk<DT == F16 ? OUT_F16 : OUT_BF16>(tile, lane, 1, v[1]);
-      ptx::fence_proxy_async_smem();
-      __syncwarp();
-      if (lane == 0) {
-        ptx::mbar_arrive(hs_full(b));
-        asm volatile("cp.async.bulk.tensor.4d.global.shared::cta.tile.bulk_group [%0, {%2, %3, %4, %5}], [%1];"
-                     ::"l"(&tmF1), "r"(tile), "r"(n0), "r"(m_blk * BM + quad * 32), "r"(0), "r"(0) : "memory");
-        asm volatile("cp.async.bulk.commit_group;" ::: "memory");
-      }
-      epi_bar();                 // bias of chunk c + 1 is in shared memory; buffer (c & 1) may be refilled next iteration
-    }
-    // output bias (slice 0 only) through the same 1 KB of shared memory, keep-words of the output tile in registers
-    const int ncol = p.d / 2;                                    // columns per half
-    const bool add_b2 = split == 0 && p.b2 != nullptr;
-    if (add_b2 && (int)threadIdx.x - 64 < p.d) bias_s[threadIdx.x - 64] = __ldg(p.b2 + (threadIdx.x - 64));
-    uint32_t keep_o[4] = {0xffffffffu, 0xffffffffu, 0xffffffffu, 0xffffffffu};
-    if (p.drop_post.p > 0.f && row_ok) {
-      const uint32_t* kp = reinterpret_cast<const uint32_t*>(p.drop_post.bits + ((uint64_t)((int64_t)m * p.d + half * ncol) >> 3));
+        // ---- GEMM2: out[64 x D] += hidden half (registers) x the matching 64 rows of the W2 chunk ----
+        uint32_t src;
+        const int st = stage_get(src);
+        ptx::fence_acc(out);
+        ptx::wgmma_fence();
 #pragma unroll
-      for (int j = 0; j < 4; ++j) if (j < ncol / 32) keep_o[j] = __ldg(kp + j);
+        for (int k = 0; k < BK / 16; ++k)
+          ptx::WgmmaRS<D, BF, B_MN>::mma(out, a16[k], B_MN ? ptx::desc_mnmajor(src, k) : ptx::desc_kmajor(src, k),
+                                         (c > 0 || h > 0 || k > 0) ? 1 : 0);
+        ptx::wgmma_commit();
+        ptx::wgmma_wait<0>();
+        ptx::fence_acc(out);
+        if (lane == 0) ptx::mbar_arrive(w_empty(st));
+      }
     }
-    epi_bar();
-    // ---- output tile: TMEM -> (+ b2 on slice 0) -> post dropout -> fp32 reduce-add into x_out ----
-    ptx::mbar_wait(out_full, 0);
-    ptx::tc_fence_after();
-    if (lane == 0) asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory");
-    __syncwarp();
-    const float pscale = p.drop_post.p > 0.f ? p.drop_post.scale : 1.f;
-    const uint32_t my_stage = sW + (uint32_t)(warp - 2) * 8192u;  // weight ring is free now: 8 warps x 2 x 4 KB boxes
+    // ---- output rows: (+ b2 on slice 0) -> post dropout -> fp32 add into x_out ----
+    const bool add_b2 = split == 0 && p.b2 != nullptr;
+    const bool post = p.drop_post.p > 0.f;
+    const float pscale = post ? p.drop_post.scale : 1.f;
     if (p.tickets && p.splits > 1) {
       // deterministic reduction order: slice s adds only after slices 0 .. s-1 of this row tile have completed theirs
       if (lane == 0) {
@@ -943,47 +562,31 @@ fused_mlp_fwd_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_const
       }
       __syncwarp();
     }
-#pragma unroll 1
-    for (int bx = 0; bx < ncol / 32; ++bx) {
-      const int co = half * ncol + bx * 32;
-      const uint32_t buf = my_stage + (uint32_t)(bx & 1) * 4096u;
-      if (lane == 0) asm volatile("cp.async.bulk.wait_group.read 1;" ::: "memory");
-      __syncwarp();
-      uint32_t r[32];
-      ptx::tmem_ld_32x32b_x32(tOut + lane_addr + (uint32_t)co, r);
-      ptx::tmem_ld_wait();
-      float v[32];
-      const uint32_t k32 = keep_o[bx & 3];
 #pragma unroll
-      for (int j4 = 0; j4 < 8; ++j4) {
-        float4 bb = make_float4(0.f, 0.f, 0.f, 0.f);
-        if (add_b2) bb = *reinterpret_cast<const float4*>(bias_s + co + 4 * j4);
-        v[4 * j4 + 0] = __uint_as_float(r[4 * j4 + 0]) + bb.x; v[4 * j4 + 1] = __uint_as_float(r[4 * j4 + 1]) + bb.y;
-        v[4 * j4 + 2] = __uint_as_float(r[4 * j4 + 2]) + bb.z; v[4 * j4 + 3] = __uint_as_float(r[4 * j4 + 3]) + bb.w;
-      }
+    for (int j = 0; j < D / 8; ++j) {
+      const int n = 8 * j + 2 * q;
+      float2 bb = make_float2(0.f, 0.f);
+      if (add_b2) bb = __ldg(reinterpret_cast<const float2*>(p.b2 + n));
 #pragma unroll
-      for (int j = 0; j < 32; ++j) v[j] = ((k32 >> j) & 1u) ? v[j] * pscale : 0.f;
-      stage_chunk<OUT_F32>(buf, lane, 0, v);
-      ptx::fence_proxy_async_smem();
-      __syncwarp();
-      if (lane == 0) {
-        asm volatile("cp.reduce.async.bulk.tensor.4d.global.shared::cta.add.tile.bulk_group [%0, {%2, %3, %4, %5}], [%1];"
-                     ::"l"(&tmOut), "r"(buf), "r"(co), "r"(m_blk * BM + quad * 32), "r"(0), "r"(0) : "memory");
-        asm volatile("cp.async.bulk.commit_group;" ::: "memory");
+      for (int hr = 0; hr < 2; ++hr) {
+        const int m = m0 + 8 * hr;
+        if (m < p.M) {
+          float v0 = out[4 * j + 2 * hr] + bb.x, v1 = out[4 * j + 2 * hr + 1] + bb.y;
+          if (post) {
+            const uint32_t kb = (uint32_t)__ldg(p.drop_post.bits + ((uint64_t)((int64_t)m * p.d + n) >> 3)) >> (2 * q);
+            v0 = (kb & 1u) ? v0 * pscale : 0.f;
+            v1 = (kb & 2u) ? v1 * pscale : 0.f;
+          }
+          atomicAdd(reinterpret_cast<float2*>(p.out + (int64_t)m * p.d + n), make_float2(v0, v1));
+        }
       }
     }
-    if (lane == 0) asm volatile("cp.async.bulk.wait_group 0;" ::: "memory");
     if (p.tickets && p.splits > 1) {
       __threadfence();
-      epi_bar();                                   // all 8 warps' reductions have been performed
-      if (threadIdx.x == 64) atomicExch(p.tickets + m_blk, split + 1 == p.splits ? 0 : split + 1);
+      asm volatile("bar.sync 1, 256;" ::: "memory");      // all 8 warps' additions have been performed
+      if (threadIdx.x == 128) atomicExch(p.tickets + m_blk, split + 1 == p.splits ? 0 : split + 1);
     }
-    ptx::tc_fence_before();
   }
-
-  ptx::tc_fence_before();
-  __syncthreads();
-  if (warp == 1) { ptx::tc_fence_after(); ptx::tmem_dealloc(tmem, 512); }
 }
 
 // -------------------------------------------------------------------------------------------
@@ -1056,37 +659,6 @@ int make_operand_map(const GemmOperand& op, int rows, int K, int nb1, int nb2, i
   return 0;
 }
 
-// Output tensor map: dims (N, M, nb1, nb2); box = {128 bytes of columns, 32 rows} (one epilogue warp), 128B swizzle.
-int make_out_map(const void* C, int c_dtype, int N, int M, int nb1, int nb2, int64_t ldc, int64_t sb1, int64_t sb2, CUtensorMap* out) {
-  EncodeTiledFn fn = get_encode_fn();
-  B200ST_CHECK(fn != nullptr, "cuTensorMapEncodeTiled unavailable (no CUDA driver?)");
-  const uint64_t es = c_dtype == F32 ? 4 : 2;
-  uint64_t s1 = nb1 > 1 ? (uint64_t)sb1 : (uint64_t)ldc * M;
-  uint64_t s2 = nb2 > 1 ? (uint64_t)sb2 : s1 * (uint64_t)nb1;
-  if (s1 == 0) s1 = (uint64_t)ldc * M;
-  if (s2 == 0) s2 = s1 * (uint64_t)nb1;
-  cuuint64_t dims[4] = {(cuuint64_t)N, (cuuint64_t)M, (cuuint64_t)nb1, (cuuint64_t)nb2};
-  cuuint64_t strides[3] = {(cuuint64_t)ldc * es, s1 * es, s2 * es};
-  cuuint32_t box[4] = {(cuuint32_t)(128 / es), 32u, 1u, 1u};
-  cuuint32_t estr[4] = {1u, 1u, 1u, 1u};
-  if (strides[1] % 16 != 0) strides[1] = (strides[1] + 15) / 16 * 16;   // size-1 batch dims: any legal stride
-  if (strides[2] % 16 != 0) strides[2] = (strides[2] + 15) / 16 * 16;
-  MapKey key{{(uint64_t)(uintptr_t)C, (uint64_t)N, (uint64_t)M, (uint64_t)nb1, (uint64_t)nb2, strides[0], strides[1], strides[2],
-              0x1000u + es, 7u | ((uint64_t)c_dtype << 8)}};
-  {
-    std::lock_guard<std::mutex> lk(g_map_mu);
-    auto it = g_map_cache.find(key);
-    if (it != g_map_cache.end()) { *out = it->second; return 0; }
-  }
-  CUresult r = fn(out, c_dtype == F32 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT32 : c_dtype == F16 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT16 : CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 4, const_cast<void*>(C), dims,
-                  strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_NONE,
-                  CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-  if (r != CUDA_SUCCESS) B200ST_FAIL("cuTensorMapEncodeTiled (output) failed with CUresult " + std::to_string((int)r));
-  std::lock_guard<std::mutex> lk(g_map_mu);
-  g_map_cache.emplace(key, *out);
-  return 0;
-}
-
 int g_num_sms = 0;
 int64_t g_launches = 0;
 }  // namespace
@@ -1101,7 +673,7 @@ void tc_count_launch() { ++g_launches; }
 
 namespace {
 
-// optional GEMM profile (bench.py roofline pass; off in the timed region): every tcgen05 GEMM issued between begin and
+// optional GEMM profile (bench.py roofline pass; off in the timed region): every tensor-core GEMM issued between begin and
 // end is RECORDED (arguments only); tc_profile_end() then replays each recorded GEMM back to back (1 warm-up + kReps timed
 // launches bracketed by one event pair, no host gap between them) and reports the per-launch average.  The buffers of the
 // step are still alive (same workspace), accumulate / reduce epilogues only add into gradients nobody reads afterwards.
@@ -1115,36 +687,32 @@ struct ProfRec { GemmArgs g; cudaStream_t stream; int bn, splitk; int group_n = 
 bool g_prof = false;
 std::vector<ProfRec> g_prof_recs;
 
-template <int BN, bool A_MN, bool B_MN, int OUT>
-int launch_out(const CUtensorMap& ta, const CUtensorMap& tb, const CUtensorMap& tc, const TcParams& p, int grid, size_t smem,
-               cudaStream_t stream) {
-  auto kern = tc_gemm_kernel<BN, A_MN, B_MN, OUT>;
+template <int BN, bool A_MN, bool B_MN, bool BF>
+int launch_kernel(const CUtensorMap& ta, const CUtensorMap& tb, const TcParams& p, int grid, size_t smem, cudaStream_t stream) {
+  auto kern = tc_gemm_kernel<BN, A_MN, B_MN, BF>;
   static bool attr_set = false;
   if (!attr_set) {
     B200ST_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemLimit));
     attr_set = true;
   }
-  launch_pdl(kern, grid, kThreads, smem, stream, ta, tb, tc, p);
+  launch_pdl(kern, grid, kThreads, smem, stream, ta, tb, p);
   B200ST_LAUNCH_CHECK();
   return 0;
 }
 
 template <int BN, bool A_MN, bool B_MN>
-int launch_variant(const CUtensorMap& ta, const CUtensorMap& tb, const CUtensorMap& tc, const TcParams& p, int grid, size_t smem,
-                   cudaStream_t stream) {
-  if (p.atomic) return launch_out<BN, A_MN, B_MN, OUT_ATOMIC>(ta, tb, tc, p, grid, smem, stream);
-  if (p.c_dtype == F32) return launch_out<BN, A_MN, B_MN, OUT_F32>(ta, tb, tc, p, grid, smem, stream);
-  if (p.c_dtype == F16) return launch_out<BN, A_MN, B_MN, OUT_F16>(ta, tb, tc, p, grid, smem, stream);
-  return launch_out<BN, A_MN, B_MN, OUT_BF16>(ta, tb, tc, p, grid, smem, stream);
+int launch_variant(bool bf, const CUtensorMap& ta, const CUtensorMap& tb, const TcParams& p, int grid, size_t smem, cudaStream_t stream) {
+  if (bf) return launch_kernel<BN, A_MN, B_MN, true>(ta, tb, p, grid, smem, stream);
+  return launch_kernel<BN, A_MN, B_MN, false>(ta, tb, p, grid, smem, stream);
 }
 
 template <int BN>
-int launch_bn(bool a_mn, bool b_mn, const CUtensorMap& ta, const CUtensorMap& tb, const CUtensorMap& tc, const TcParams& p, int grid,
-              size_t smem, cudaStream_t stream) {
-  if (!a_mn && !b_mn) return launch_variant<BN, false, false>(ta, tb, tc, p, grid, smem, stream);
-  if (!a_mn && b_mn) return launch_variant<BN, false, true>(ta, tb, tc, p, grid, smem, stream);
-  if (a_mn && !b_mn) return launch_variant<BN, true, false>(ta, tb, tc, p, grid, smem, stream);
-  return launch_variant<BN, true, true>(ta, tb, tc, p, grid, smem, stream);
+int launch_bn(bool a_mn, bool b_mn, bool bf, const CUtensorMap& ta, const CUtensorMap& tb, const TcParams& p, int grid, size_t smem,
+              cudaStream_t stream) {
+  if (!a_mn && !b_mn) return launch_variant<BN, false, false>(bf, ta, tb, p, grid, smem, stream);
+  if (!a_mn && b_mn) return launch_variant<BN, false, true>(bf, ta, tb, p, grid, smem, stream);
+  if (a_mn && !b_mn) return launch_variant<BN, true, false>(bf, ta, tb, p, grid, smem, stream);
+  return launch_variant<BN, true, true>(bf, ta, tb, p, grid, smem, stream);
 }
 
 }  // namespace
@@ -1162,10 +730,9 @@ int gemm_tc_bf16(const GemmArgs& g, cudaStream_t stream) { return gemm_tc_impl(g
 
 namespace {
 int gemm_tc_impl(const GemmArgs& g, cudaStream_t stream, const ConvA* conv) {
-  B200ST_CHECK(is16(g.A.dtype) && is16(g.B.dtype), "tcgen05 GEMM needs 16-bit (bf16 / fp16) operands");
-  // measured on B200 (round 2): a kind::f16 MMA whose A and B formats differ raises an illegal-instruction fault, although
-  // the instruction descriptor encodes them separately — so the library refuses mixed products up front
-  B200ST_CHECK(g.A.dtype == g.B.dtype, "tcgen05 kind::f16 needs A and B in the same 16-bit format (both bf16 or both fp16)");
+  B200ST_CHECK(is16(g.A.dtype) && is16(g.B.dtype), "tensor-core GEMM needs 16-bit (bf16 / fp16) operands");
+  // wgmma has no mixed bf16 x fp16 form: the library refuses mixed products up front
+  B200ST_CHECK(g.A.dtype == g.B.dtype, "wgmma needs A and B in the same 16-bit format (both bf16 or both fp16)");
   B200ST_CHECK(g.M > 0 && g.N > 0 && g.K > 0 && g.nb1 > 0 && g.nb2 > 0, "empty GEMM");
   if (const int abl = ablate_mask()) {
     const bool wgrad = g.A.mn_major && g.B.mn_major;
@@ -1186,10 +753,10 @@ int gemm_tc_impl(const GemmArgs& g, cudaStream_t stream, const ConvA* conv) {
   const int64_t batch = (int64_t)g.nb1 * g.nb2;
 
   // ---- joint choice of the N tile and the split-K factor ----
-  // Per k-block a CTA needs max(tensor time, L2->smem fill time): 4 MMAs of 128 x c x 16 take 2c cycles; the operand
-  // bytes (16 KB + 128c B) arrive at ~44 B/cycle/SM (measured, profiles/r01_gemm_notes.md).  The epilogue overlaps the
-  // next tile's main loop.  Split-K (fp32 TMA reduce-add epilogue) is allowed for linear accumulate epilogues only and is
-  // chosen so that the tile count fills the 148 SMs once.
+  // Cost model per k-block of a CTA: max(tensor time, L2->smem fill time): the wgmmas of a 128 x c x 64 block take about
+  // 4c cycles, the operand bytes (16 KB + 128c B) are assumed to arrive at ~44 B/cycle/SM (an estimate, not measured on
+  // H100).  The epilogue runs after the main loop of its tile.  Split-K (fp32 atomic epilogue) is allowed for linear
+  // accumulate epilogues only and is chosen so that the tile count fills the SMs once.
   const bool linear_epi = !g.epi.relu && !g.epi.mask_src && g.epi.drop.p == 0.f && !g.epi.residual && !g.epi.bias;
   const bool split_ok = linear_epi && g.c_dtype == F32 && g.epi.accumulate;
   if (g.splitk > 1) B200ST_CHECK(split_ok, "split-K needs a linear fp32 accumulate epilogue");
@@ -1215,10 +782,10 @@ int gemm_tc_impl(const GemmArgs& g, cudaStream_t stream, const ConvA* conv) {
         const int kb_per = ceil_div(p.kb_total, sk);
         const int64_t tiles = tiles0 * ceil_div(p.kb_total, kb_per);
         const int64_t waves = (tiles + num_sms - 1) / num_sms;
-        const double fill = (16384.0 + 128.0 * c) / 44.0, mma = 2.0 * c;
+        const double fill = (16384.0 + 128.0 * c) / 44.0, mma = 4.0 * c;
         const double mainloop = kb_per * (fill > mma ? fill : mma);
         const double epi = (sk > 1 ? 14.0 : 10.0) * c + 600.0;
-        const double cost = (double)waves * ((mainloop > epi ? mainloop : epi) + 800.0) + (sk > 1 ? 500.0 : 0.0);
+        const double cost = (double)waves * (mainloop + epi + 800.0) + (sk > 1 ? 500.0 : 0.0);
         if (cost < best) { best = cost; best_bn = c; best_sk = sk; }
         if (sk <= sk_lo) break;
       }
@@ -1230,56 +797,25 @@ int gemm_tc_impl(const GemmArgs& g, cudaStream_t stream, const ConvA* conv) {
   p.kb_per_split = ceil_div(p.kb_total, splitk);
   splitk = ceil_div(p.kb_total, p.kb_per_split);   // no empty trailing split
   p.splitk = splitk;
-  p.atomic = (splitk > 1) ? 1 : 0;
-  p.dbg_epi = getenv("B200ST_EPI_MODE") ? atoi(getenv("B200ST_EPI_MODE")) : 0;
-  p.dbg_trace = getenv("B200ST_DEBUG_TRACE_PTR") ? reinterpret_cast<long long*>(strtoull(getenv("B200ST_DEBUG_TRACE_PTR"), nullptr, 0)) : nullptr;
   p.n_tiles = ceil_div(g.N, bn);
   p.num_tiles = batch * p.m_tiles * p.n_tiles * splitk;
 
   const uint32_t stage_bytes = kABytes + (uint32_t)bn * BK * 2;
-  const int ctas_per_sm = 1;   // (two co-resident CTAs per SM were measured: no gain, see profiles/r01_gemm_notes.md)
-  const int smem_budget = (ctas_per_sm == 2 ? (kSmemLimit / 2 - 1024) : kSmemLimit) - (int)kStagingBytes;
-  int stages = dbg.force_stages > 0 ? dbg.force_stages : (int)((smem_budget - 2048) / stage_bytes);
+  int stages = dbg.force_stages > 0 ? dbg.force_stages : (int)((kSmemLimit - 2048) / stage_bytes);
   if (stages > 8) stages = 8;
+  if (stages < 2) stages = 2;      // consume_kblocks keeps one slot in flight before it releases the previous one
   p.stages = stages;
-  const size_t smem = 1024 + (size_t)stages * stage_bytes + kStagingBytes + 8 * (2 * stages + 5) + 16;
+  const size_t smem = 1024 + (size_t)stages * stage_bytes + 16 * stages + 16;
   B200ST_CHECK(smem <= (size_t)kSmemLimit, "smem budget exceeded");
-
-  // descriptors
-  const uint32_t mn_lbo = dbg.mn_lbo_bytes ? dbg.mn_lbo_bytes : 64u * BK * 2;   // next 64-wide MN chunk (TMA box)
-  const uint32_t mn_sbo = dbg.mn_sbo_bytes ? dbg.mn_sbo_bytes : 1024u;          // next group of 8 k-rows
-  const uint32_t k_lbo = dbg.k_lbo_bytes ? dbg.k_lbo_bytes : 16u;               // ignored for swizzled K-major
-  const uint32_t k_sbo = dbg.k_sbo_bytes ? dbg.k_sbo_bytes : 1024u;             // next group of 8 rows
-  p.a_lbo = g.A.mn_major ? mn_lbo : k_lbo;  p.a_sbo = g.A.mn_major ? mn_sbo : k_sbo;
-  p.b_lbo = g.B.mn_major ? mn_lbo : k_lbo;  p.b_sbo = g.B.mn_major ? mn_sbo : k_sbo;
-  p.a_kstep = g.A.mn_major ? 16u * 128u : 32u;
-  p.b_kstep = g.B.mn_major ? 16u * 128u : 32u;
-  p.idesc = ptx::make_idesc_16(bn, g.A.mn_major, g.B.mn_major, g.A.dtype == BF16, g.B.dtype == BF16);
 
   p.C = g.C; p.c_dtype = g.c_dtype; p.ldc = g.ldc; p.c_sb1 = g.c_sb1; p.c_sb2 = g.c_sb2;
   p.epi = g.epi;
   if (g.epi.accumulate) B200ST_CHECK(g.c_dtype == F32, "accumulate needs fp32 C");
-
-  // ---- output path: TMA store through per-warp staging boxes when everything is 16-byte aligned ----
-  const uint64_t esz_c = g.c_dtype == F32 ? 4 : 2;
-  auto al16 = [](const void* ptr) { return (reinterpret_cast<uintptr_t>(ptr) & 15) == 0; };
-  bool tma_ok = al16(g.C) && (g.ldc * esz_c) % 16 == 0 && (g.nb1 == 1 || (g.c_sb1 * esz_c) % 16 == 0) &&
-                (g.nb2 == 1 || (g.c_sb2 * esz_c) % 16 == 0) && g.N >= bn;
-  if (g.epi.bias) tma_ok = tma_ok && al16(g.epi.bias);
-  if (g.epi.mask_src) {
-    const uint64_t em = g.epi.mask_dtype == F32 ? 4 : 2;   // bf16 and fp16 masks are both read as sign/magnitude words
-    tma_ok = tma_ok && al16(g.epi.mask_src) && (g.epi.mask_ld * em) % 16 == 0 && (g.epi.mask_sb1 * em) % 16 == 0 &&
-             (g.epi.mask_sb2 * em) % 16 == 0;
-  }
-  if (g.epi.residual)
-    tma_ok = tma_ok && al16(g.epi.residual) && (g.epi.res_ld * 4) % 16 == 0 && (g.epi.res_sb1 * 4) % 16 == 0 && (g.epi.res_sb2 * 4) % 16 == 0;
-  if (g.epi.drop.p > 0.f) tma_ok = tma_ok && g.epi.drop.bits != nullptr && (g.N % 32 == 0);
-  if (getenv("B200ST_NO_TMA_STORE")) tma_ok = false;
-  p.use_tma_store = tma_ok ? 1 : 0;
-  p.c_reduce = (p.atomic || g.epi.accumulate) ? 1 : 0;
-  CUtensorMap tc;
-  std::memset(&tc, 0, sizeof(tc));
-  if (tma_ok) B200ST_TRY(make_out_map(g.C, g.c_dtype, g.N, g.M, g.nb1, g.nb2, g.ldc, g.c_sb1, g.c_sb2, &tc));
+  p.atomic = (splitk > 1 || g.epi.accumulate) ? 1 : 0;
+  // paired stores / atomics need every (row, even column) element of C 8-byte (fp32) or 4-byte (16-bit) aligned
+  const uintptr_t pair_bytes = g.c_dtype == F32 ? 8 : 4;
+  p.vec2 = ((reinterpret_cast<uintptr_t>(g.C) % pair_bytes) == 0 && g.ldc % 2 == 0 && (g.nb1 == 1 || g.c_sb1 % 2 == 0) &&
+            (g.nb2 == 1 || g.c_sb2 % 2 == 0)) ? 1 : 0;
 
   CUtensorMap ta, tb;
   if (conv) {
@@ -1308,7 +844,7 @@ int gemm_tc_impl(const GemmArgs& g, cudaStream_t stream, const ConvA* conv) {
     B200ST_TRY(make_operand_map(g.B, g.N, g.K, g.nb1, g.nb2, bn, &tb));
   }
 
-  const int max_grid = num_sms * ctas_per_sm;
+  const int max_grid = num_sms;
   const int grid = (int)(p.num_tiles < max_grid ? p.num_tiles : max_grid);
   ++g_launches;
   if (g_prof) {
@@ -1317,10 +853,11 @@ int gemm_tc_impl(const GemmArgs& g, cudaStream_t stream, const ConvA* conv) {
     g_prof_recs.push_back(r);
   }
   int rc = 0;
+  const bool bf = g.A.dtype == BF16;
   switch (bn) {
-    case 64: rc = launch_bn<64>(g.A.mn_major, g.B.mn_major, ta, tb, tc, p, grid, smem, stream); break;
-    case 128: rc = launch_bn<128>(g.A.mn_major, g.B.mn_major, ta, tb, tc, p, grid, smem, stream); break;
-    case 256: rc = launch_bn<256>(g.A.mn_major, g.B.mn_major, ta, tb, tc, p, grid, smem, stream); break;
+    case 64: rc = launch_bn<64>(g.A.mn_major, g.B.mn_major, bf, ta, tb, p, grid, smem, stream); break;
+    case 128: rc = launch_bn<128>(g.A.mn_major, g.B.mn_major, bf, ta, tb, p, grid, smem, stream); break;
+    case 256: rc = launch_bn<256>(g.A.mn_major, g.B.mn_major, bf, ta, tb, p, grid, smem, stream); break;
     default: B200ST_FAIL("unsupported BN");
   }
   return rc;
@@ -1379,7 +916,7 @@ int gemm_wgrad_group(const GemmArgs* gs, int n, cudaStream_t stream) {
     const bool plain = !g.epi.relu && !g.epi.mask_src && g.epi.drop.p == 0.f && !g.epi.residual && !g.epi.bias && g.epi.accumulate;
     if (!(is16(g.A.dtype) && g.A.dtype == g.B.dtype && g.A.dtype == gs[0].A.dtype && g.A.mn_major && g.B.mn_major && plain &&
           g.c_dtype == F32 && g.nb1 == 1 && g.nb2 == 1 && g.M % BM == 0 && g.N % 256 == 0 && g.K > 0 && g.splitk <= 1 &&
-          (reinterpret_cast<uintptr_t>(g.C) & 15) == 0 && (g.ldc * 4) % 16 == 0))
+          (reinterpret_cast<uintptr_t>(g.C) & 7) == 0 && g.ldc % 2 == 0))
       return 2;
   }
   if (ablate_mask() & ABL_WGRAD) return 0;
@@ -1420,20 +957,20 @@ int gemm_wgrad_group(const GemmArgs* gs, int n, cudaStream_t stream) {
     tile += q.m_tiles * q.n_tiles * q.splitk;
     B200ST_TRY(make_operand_map(g.A, g.M, g.K, 1, 1, BM, &q.ta));
     B200ST_TRY(make_operand_map(g.B, g.N, g.K, 1, 1, 256, &q.tb));
-    B200ST_TRY(make_out_map(g.C, F32, g.N, g.M, 1, 1, g.ldc, 0, 0, &q.tc));
+    q.C = reinterpret_cast<float*>(g.C); q.ldc = g.ldc;
   }
   grp.num_tiles = tile;
   const uint32_t stage_bytes = kABytes + 256u * BK * 2;
-  int stages = (int)((kSmemLimit - (int)kStagingBytes - 2048) / stage_bytes);
+  int stages = (int)((kSmemLimit - 2048) / stage_bytes);
   if (stages > 8) stages = 8;
   grp.stages = stages;
-  grp.idesc = ptx::make_idesc_16(256, 1, 1, gs[0].A.dtype == BF16, gs[0].B.dtype == BF16);
-  const size_t smem = 1024 + (size_t)stages * stage_bytes + kStagingBytes + 8 * (2 * stages + 5) + 16;
+  const size_t smem = 1024 + (size_t)stages * stage_bytes + 16 * stages + 16;
   B200ST_CHECK(smem <= (size_t)kSmemLimit, "smem budget exceeded");
-  static bool attr_set = false;
-  if (!attr_set) {
-    B200ST_CUDA(cudaFuncSetAttribute(tc_wgrad_group_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemLimit));
-    attr_set = true;
+  auto kern = gs[0].A.dtype == BF16 ? tc_wgrad_group_kernel<true> : tc_wgrad_group_kernel<false>;
+  static bool attr_set[2] = {false, false};
+  if (!attr_set[gs[0].A.dtype == BF16]) {
+    B200ST_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemLimit));
+    attr_set[gs[0].A.dtype == BF16] = true;
   }
   const int grid = grp.num_tiles < num_sms ? grp.num_tiles : num_sms;
   ++g_launches;
@@ -1443,7 +980,7 @@ int gemm_wgrad_group(const GemmArgs* gs, int n, cudaStream_t stream) {
     for (int i = 1; i < n; ++i) r.rest[i - 1] = gs[i];
     g_prof_recs.push_back(r);
   }
-  launch_pdl(tc_wgrad_group_kernel, grid, kThreads, smem, stream, grp);
+  launch_pdl(kern, grid, kThreads, smem, stream, grp);
   B200ST_LAUNCH_CHECK();
   return 0;
 }
@@ -1475,21 +1012,21 @@ int fused_mlp_fwd(const void* X, int dtype, int M, int d, int ffn, const void* W
   p.M = M; p.d = d; p.ffn = ffn; p.splits = splits; p.chunks_per_cta = chunks / splits;
   p.b1 = b1; p.b2 = b2; p.drop_ffn = drop_ffn; p.drop_post = drop_post;
   p.relu = 1; p.alpha = 1.f; p.mask_src = nullptr; p.mask_ld = 0; p.tickets = tickets;
-  p.idesc_g1 = ptx::make_idesc_16(128, 0, 1, dtype == BF16, dtype == BF16);
-  p.idesc_g2 = ptx::make_idesc_16(d, 0, 1, dtype == BF16, dtype == BF16);
-  CUtensorMap tx, tw1, tw2, tf1, tout;
+  p.F1 = reinterpret_cast<uint16_t*>(F1); p.out = x_out;
+  B200ST_CHECK((reinterpret_cast<uintptr_t>(F1) & 3) == 0 && (reinterpret_cast<uintptr_t>(x_out) & 7) == 0, "fused MLP: unaligned output");
+  CUtensorMap tx, tw1, tw2;
   B200ST_TRY(make_operand_map(GemmOperand{X, dtype, 0, d, 0, 0}, M, d, 1, 1, BM, &tx));
   B200ST_TRY(make_operand_map(GemmOperand{W1, dtype, 1, ffn, 0, 0}, ffn, d, 1, 1, 64, &tw1));
   B200ST_TRY(make_operand_map(GemmOperand{W2, dtype, 1, d, 0, 0}, d, ffn, 1, 1, 64, &tw2));
-  B200ST_TRY(make_out_map(F1, dtype, ffn, M, 1, 1, ffn, 0, 0, &tf1));
-  B200ST_TRY(make_out_map(x_out, F32, d, M, 1, 1, d, 0, 0, &tout));
-  auto kern = dtype == F16 ? fused_mlp_fwd_kernel<F16, true> : fused_mlp_fwd_kernel<BF16, true>;
-  static bool attr[2] = {false, false};
-  if (!attr[dtype == F16]) {
+  auto kern = d == 256 ? (dtype == F16 ? fused_mlp_fwd_kernel<F16, true, 256> : fused_mlp_fwd_kernel<BF16, true, 256>)
+                       : (dtype == F16 ? fused_mlp_fwd_kernel<F16, true, 128> : fused_mlp_fwd_kernel<BF16, true, 128>);
+  static bool attr[4] = {false, false, false, false};
+  const int ai = (dtype == F16 ? 1 : 0) + (d == 256 ? 2 : 0);
+  if (!attr[ai]) {
     B200ST_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kMlpSmem));
-    attr[dtype == F16] = true;
+    attr[ai] = true;
   }
-  launch_pdl(kern, m_tiles * splits, kThreads, kMlpSmem, stream, tx, tw1, tw2, tf1, tout, p);
+  launch_pdl(kern, m_tiles * splits, kThreads, kMlpSmem, stream, tx, tw1, tw2, p);
   ++g_launches;
   B200ST_LAUNCH_CHECK();
   return 0;
@@ -1515,21 +1052,22 @@ int fused_mlp_bwd(const void* dY, int dtype, int M, int d, int ffn, const void* 
   p.M = M; p.d = d; p.ffn = ffn; p.splits = splits; p.chunks_per_cta = chunks / splits;
   p.b1 = nullptr; p.b2 = nullptr; p.drop_ffn = no_dropout(); p.drop_post = no_dropout();
   p.relu = 0; p.alpha = scale; p.mask_src = F1; p.mask_ld = ffn; p.tickets = tickets;
-  p.idesc_g1 = ptx::make_idesc_16(128, 0, 0, dtype == BF16, dtype == BF16);
-  p.idesc_g2 = ptx::make_idesc_16(d, 0, 0, dtype == BF16, dtype == BF16);
-  CUtensorMap tx, tw1, tw2, tf1, tout;
+  p.F1 = reinterpret_cast<uint16_t*>(dF1); p.out = dH;
+  B200ST_CHECK((reinterpret_cast<uintptr_t>(dF1) & 3) == 0 && (reinterpret_cast<uintptr_t>(dH) & 7) == 0 &&
+               (reinterpret_cast<uintptr_t>(F1) & 3) == 0, "fused MLP: unaligned buffer");
+  CUtensorMap tx, tw1, tw2;
   B200ST_TRY(make_operand_map(GemmOperand{dY, dtype, 0, d, 0, 0}, M, d, 1, 1, BM, &tx));
   B200ST_TRY(make_operand_map(GemmOperand{W2, dtype, 0, d, 0, 0}, ffn, d, 1, 1, 128, &tw1));     // G1: rows = hidden units, k = d
   B200ST_TRY(make_operand_map(GemmOperand{W1, dtype, 0, ffn, 0, 0}, d, ffn, 1, 1, d, &tw2));      // G2: rows = model dims, k = hidden
-  B200ST_TRY(make_out_map(dF1, dtype, ffn, M, 1, 1, ffn, 0, 0, &tf1));
-  B200ST_TRY(make_out_map(dH, F32, d, M, 1, 1, d, 0, 0, &tout));
-  auto kern = dtype == F16 ? fused_mlp_fwd_kernel<F16, false> : fused_mlp_fwd_kernel<BF16, false>;
-  static bool attr[2] = {false, false};
-  if (!attr[dtype == F16]) {
+  auto kern = d == 256 ? (dtype == F16 ? fused_mlp_fwd_kernel<F16, false, 256> : fused_mlp_fwd_kernel<BF16, false, 256>)
+                       : (dtype == F16 ? fused_mlp_fwd_kernel<F16, false, 128> : fused_mlp_fwd_kernel<BF16, false, 128>);
+  static bool attr[4] = {false, false, false, false};
+  const int ai = (dtype == F16 ? 1 : 0) + (d == 256 ? 2 : 0);
+  if (!attr[ai]) {
     B200ST_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kMlpSmem));
-    attr[dtype == F16] = true;
+    attr[ai] = true;
   }
-  launch_pdl(kern, m_tiles * splits, kThreads, kMlpSmem, stream, tx, tw1, tw2, tf1, tout, p);
+  launch_pdl(kern, m_tiles * splits, kThreads, kMlpSmem, stream, tx, tw1, tw2, p);
   ++g_launches;
   B200ST_LAUNCH_CHECK();
   return 0;

@@ -298,7 +298,7 @@ def profile_begin():
 
 
 def profile_end():
-    """-> (sum of tcgen05 GEMM kernel ms, sum of their algorithmic FLOPs, launches) since profile_begin()."""
+    """-> (sum of wgmma GEMM kernel ms, sum of their algorithmic FLOPs, launches) since profile_begin()."""
     ms, fl, n = C.c_double(0), C.c_double(0), C.c_int64(0)
     check(load().b200st_profile_end(C.byref(ms), C.byref(fl), C.byref(n)))
     return ms.value, fl.value, n.value

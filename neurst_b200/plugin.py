@@ -10,7 +10,7 @@ ones when TensorFlow — hence the reference's TF packages — imports):
 
 Registering a *different* class under an existing name raises in the reference (registry.py:120-122), so the drop-in uses
 new names; `override=True` additionally points the stock names ("SpeechTransformer", "TransformerEncoder", ...) at the
-B200 classes by assigning REGISTRIES[backend][registry][name] directly, which is what a deployment that wants existing
+H100 classes by assigning REGISTRIES[backend][registry][name] directly, which is what a deployment that wants existing
 yaml files to run unchanged does.
 
 Each registered class subclasses the registry's base class (`issubclass` is enforced, registry.py:111-112), exposes the
@@ -116,7 +116,7 @@ def _make_layer_class(base, cls_name, impl_cls):
 
 
 def register(override=False):
-    """Writes the B200 classes into the reference registries.  Returns {backend: {registry: [names]}}.
+    """Writes the H100 classes into the reference registries.  Returns {backend: {registry: [names]}}.
     Needs `neurst.utils.registry` + `neurst_pt` importable (the reference on sys.path); raises ImportError otherwise."""
     if _REGISTERED and not override:
         return _REGISTERED

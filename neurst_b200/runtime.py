@@ -333,7 +333,11 @@ class GraphedTrainStep:
         torch.cuda.current_stream().wait_stream(side)
         torch.cuda.synchronize()
         g = torch.cuda.CUDAGraph()
-        with torch.cuda.graph(g):
+        # thread-local capture mode.  Observed in global mode: the Prefetcher thread of the training entry pins its next batch
+        # (Tensor.pin_memory -> cudaHostAlloc) while this thread captures, which invalidates the capture
+        # (cudaErrorStreamCaptureInvalidated at capture_end, and torch's graph state stays broken for later captures).
+        # The captured region itself issues kernel launches only, so nothing this thread does needs the global check.
+        with torch.cuda.graph(g, capture_error_mode="thread_local"):
             self._launch()
         rt.grads.copy_(saved)                  # discard the warm-up / capture-time accumulation
         self.graph = g

@@ -1,4 +1,4 @@
-"""ORACLE (test infrastructure only): recipe that stages the UNMODIFIED reference PyTorch mirror for the GPU box.
+"""ORACLE (test infrastructure only): recipe that stages the UNMODIFIED reference PyTorch mirror for a machine without the reference.
 
     python oracle/build_ref.py          # run in the build container (needs /root/reference); also run by __graft_entry__.build()
 
@@ -6,8 +6,8 @@ The reference's only implementation of this path that can run without TensorFlow
 autograd fails, SURVEY.md 8c).  It is Python, so "building" it means staging: this script copies
     /root/reference/neurst_pt/**.py           (the models / layers themselves)
     /root/reference/neurst/utils/*.py         (registry, flags, configurable ... imported by neurst_pt)
-byte for byte into oracle/_ref/ (git-ignored: reference sources never enter the history; NOT gpurun-ignored: the copy
-travels to the GPU box like a built .so) and writes oracle/_ref/MANIFEST.json with the SHA-256 of every file.  Users:
+byte for byte into oracle/_ref/ (git-ignored: reference sources never enter the history; the copy can be carried to a
+machine without the reference like a built .so) and writes oracle/_ref/MANIFEST.json with the SHA-256 of every file.  Users:
 `bench.py`'s CPU legs (`cpu_baseline.reference_forward`, kind "reference": the unmodified reference forward timed on the
 host cores) and tests/test_oracle.py (the staged copy reproduces the committed refpt fixtures).  Loaded through
 oracle/ref_shim.py with NEURST_REFERENCE pointing at oracle/_ref.

@@ -1,5 +1,5 @@
 """ORACLE (test infrastructure only): generates tests/golden/*.npz.  Run in the build container only
-(`python oracle/make_golden.py`); it reads /root/reference, which does not exist on the GPU box.
+(`python oracle/make_golden.py`); it reads the reference tree ($NEURST_REFERENCE), which the test machines need not have.
 
 Two kinds of fixtures:
   kat_*.npz   — the TF-generated known-answer vectors hard-coded in the reference's own tests
@@ -242,6 +242,10 @@ def make_refpt():
             emb = sm(src.clone())
             conv = sm._embedding_layer(src.clone())
         P = pt_speech_transformer_params(model)
+        big = {"P:" + k: v.astype(np.float32) for k, v in P.items() if v.size >= 32768}      # second file: no file above 1 MB
+        if sum(v.nbytes for v in big.values()) > 400000:
+            np.savez(os.path.join(OUT, name + "_part2.npz"), **big)
+            P = {k: v for k, v in P.items() if "P:" + k not in big}
         np.savez(os.path.join(OUT, name + ".npz"), src=src.numpy(), src_length=lengths.numpy(),
                  trg_input=trg_input.numpy(), logits=logits.numpy(), emb=emb.numpy(), conv=conv.numpy(),
                  cfg=np.array([mk["d"], mk["heads"], mk["enc_layers"], mk["dec_layers"], mk["ffn_size"], mk["channels"],
@@ -250,7 +254,40 @@ def make_refpt():
         print(name, "logits", tuple(logits.shape))
 
 
+def make_interchange():
+    """interchange_reference.json: what tests/test_interchange_cpu.py compares with when the reference tree is absent —
+    the unmodified reference forward on the oracle's seeded weights (through the checkpoint weight map) and the reference's
+    create_audio_bucket_boundaries for the tested (maxlen, minlen) pairs."""
+    import ast
+    import json
+    import torch
+    from oracle import build_ref, restatement as R
+    from neurst_b200 import checkpoints as CK
+    cfg = dict(model="speech", d=16, heads=2, enc_layers=2, dec_layers=2, ffn=24, channels=8, feat=80, in_channels=1, vocab=20)
+    os.environ["NEURST_REFERENCE_SRC"] = REF
+    model = build_ref.reference_speech_transformer(cfg, 20)
+    P = R.init_params(cfg, seed=5, random_bias=True)
+    CK.to_reference_pt(P, model)
+    g = torch.Generator().manual_seed(0)
+    src = torch.randn(2, 41, 80, 1, generator=g)
+    lens = torch.tensor([41, 30]); ti = torch.randint(0, 17, (2, 5), generator=g)
+    with torch.no_grad():
+        ref = model({"src": src, "src_length": lens, "trg_input": ti}, is_training=False)
+    tree = ast.parse(open(os.path.join(REF, "neurst/tasks/speech2text.py")).read())
+    fn = next(n for n in tree.body if isinstance(n, ast.FunctionDef) and n.name == "create_audio_bucket_boundaries")
+    ns = {"math": __import__("math")}
+    exec(compile(ast.Module([fn], []), "ref", "exec"), ns)
+    pairs = [(3000, 128), (2000, 100), (800, None), (3000, 300)]
+    out = {"source": "unmodified reference neurst_pt SpeechTransformer forward / neurst.tasks.speech2text.create_audio_bucket_boundaries",
+           "logits_shape": list(ref.shape), "logits": [float(x) for x in ref.reshape(-1).tolist()],
+           "bucket_boundaries": [{"maxlen": a, "minlen": b, "boundaries": list(ns["create_audio_bucket_boundaries"](a, b))} for a, b in pairs]}
+    with open(os.path.join(OUT, "interchange_reference.json"), "w") as f:
+        json.dump(out, f)
+    print("interchange_reference.json", tuple(ref.shape))
+
+
 if __name__ == "__main__":
     os.makedirs(OUT, exist_ok=True)
     make_kats()
     make_refpt()
+    make_interchange()

@@ -4,7 +4,7 @@
 It installs a fake `tensorflow` module exposing the few symbols neurst_pt / neurst.utils touch
 (tf.nest, tf.io.gfile, tf.errors.OpError), pre-seeds `neurst` / `neurst.utils` as namespace packages so that
 neurst/__init__.py (which imports every TF sub-package) is never executed, and stubs `neurst.utils.compat`.
-/root/reference does not exist on the GPU box: only oracle/make_golden.py (run here) uses this shim.
+Machines that run the tests need not have the reference tree: only oracle/make_golden.py uses this shim.
 """
 import importlib
 import os

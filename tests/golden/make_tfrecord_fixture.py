@@ -1,6 +1,6 @@
 """Generates tests/golden/tfrecord_fixture.json from the reference's own TFRecord fixtures
 (/root/reference/tests/examples/train.tfrecords-0000?-of-00004, written by TensorFlow from train.example.*.bpe.txt with
-tests/examples/example_create_seq2seq_tfrecrods.yml).  Run in the build container (the GPU box has no /root/reference):
+tests/examples/example_create_seq2seq_tfrecrods.yml).  Run where the reference tree is present:
 
     python tests/golden/make_tfrecord_fixture.py
 

@@ -61,7 +61,9 @@ def kat_params(kat, cfg, default_stack, dtype=torch.float32):
 
 
 def refpt_case(name, dtype=torch.float32):
-    z = load(name)
+    z = dict(load(name))
+    if os.path.exists(os.path.join(GOLDEN, name + "_part2.npz")):      # the larger weights live in a second file (1 MB per file)
+        z.update(load(name + "_part2"))
     P = {k[2:]: t(v, dtype) for k, v in z.items() if k.startswith("P:")}
     d, heads, enc_layers, dec_layers, ffn, channels, vocab = [int(x) for x in z["cfg"]]
     cfg = dict(model="speech", d=d, heads=heads, enc_layers=enc_layers, dec_layers=dec_layers, ffn=ffn,

@@ -4,7 +4,7 @@ T=3000 buckets (cfg-4); ragged lengths, dropout off/on.  CUDA path through the C
 EVERY gradient tensor.  Tolerances (max-abs logits on O(1) logits / relative L2 per gradient tensor):
   fp32     1e-4 / 1e-3   (reference's own TF<->PT tolerance class, SURVEY Appx A.11)
   mixed16  5e-3 / 4e-2   (= fp16: the reference's mixed_float16 — fp16 operands and activations, fp32 accumulation, dynamic
-           loss scale; measured 2.7e-3..3.2e-3 / 2.1e-2..3.0e-2 on B200, DESIGN.md section 2)
+           loss scale)
   bf16     6e-2 / 1.5e-1 (8-bit significand operands everywhere; kept as the comparison point)
 """
 import time

@@ -1,4 +1,4 @@
-"""tcgen05 GEMM through the C ABI (b200st_gemm) vs a torch fp32 contraction of the same 16-bit-rounded operands:
+"""wgmma GEMM through the C ABI (b200st_gemm) vs a torch fp32 contraction of the same 16-bit-rounded operands:
 K-major / MN-major operands, bf16 and fp16 operand formats, every output type, split-K accumulate, fused epilogues.
 Mixed A/B formats are refused by the library (they fault on the hardware)."""
 import pytest

@@ -1,5 +1,5 @@
 """CUDA path (through the C ABI) vs the oracle and the committed golden fixtures — SpeechTransformer
-forward, loss and every gradient.  fp32 precision is held to the reference's own tolerances; bf16 (tcgen05)
+forward, loss and every gradient.  fp32 precision is held to the reference's own tolerances; bf16 (wgmma)
 to the stated looser bounds."""
 import numpy as np
 import pytest
@@ -128,7 +128,7 @@ FUSED_CFG = dict(model="speech", d=128, heads=2, enc_layers=2, dec_layers=2, ffn
 
 @pytest.mark.parametrize("T,dropout", [(600, 0.0), (600, 0.1), (1100, 0.1)])
 def test_fused_attention_path_vs_oracle(T, dropout):
-    """head dim 64 => the fused tcgen05 flash-attention kernels (forward + backward): multiple q tiles / kv blocks,
+    """head dim 64 => the fused wgmma flash-attention kernels (forward + backward): multiple q tiles / kv blocks,
     ragged key lengths (additive -1e9 key bias), causal decoder self-attention, cross-attention, Philox dropout."""
     cfg = FUSED_CFG
     P = R.init_params(cfg, seed=11, random_bias=True)

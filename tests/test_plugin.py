@@ -1,17 +1,27 @@
-"""The registry drop-in: with the reference on sys.path (build container only — skipped on the GPU box, where
-/root/reference does not exist) `neurst_b200.plugin.register()` makes the reference's OWN `build_model` return the
+"""The registry drop-in: with the reference on sys.path (the installed tree, else the copy build() stages under oracle/_ref,
+which holds neurst/utils and neurst_pt) `neurst_b200.plugin.register()` makes the reference's OWN `build_model` return the
 libb200st-backed class, through the `class_or_method_args` branch of registry.build_x (neurst/utils/registry.py:90-102)."""
 import os
 
 import pytest
 import torch
 
-REF = os.environ.get("NEURST_REFERENCE", "/root/reference")
-needs_ref = pytest.mark.skipif(not os.path.isdir(REF), reason="reference tree not present (GPU box)")
+def _reference_root():
+    ref = os.environ.get("NEURST_REFERENCE", "/root/reference")
+    if os.path.isdir(os.path.join(ref, "neurst_pt")):
+        return ref
+    from oracle import build_ref
+    return build_ref.staged()
+
+
+needs_ref = pytest.mark.skipif(_reference_root() is None, reason="neither the reference tree nor its staged copy (build()) is present")
 
 
 def _register():
+    import importlib
+    os.environ["NEURST_REFERENCE"] = _reference_root()
     from oracle import ref_shim
+    importlib.reload(ref_shim)
     ref_shim.install()
     from neurst_b200 import plugin
     return plugin, plugin.register()

@@ -20,7 +20,7 @@ from neurst_b200 import tfrecord as R
 
 HERE = os.path.dirname(os.path.abspath(__file__))
 GOLD = json.load(open(os.path.join(HERE, "golden", "tfrecord_fixture.json")))
-REF_EX = "/root/reference/tests/examples"
+REF_EX = os.path.join(os.environ.get("NEURST_REFERENCE", "/root/reference"), "tests", "examples")
 
 
 def _example_class():
@@ -71,7 +71,24 @@ def test_records_written_by_tensorflow(tmp_path):
     assert list(R.read_records(str(p))) == []
 
 
-@pytest.mark.skipif(not os.path.isdir(REF_EX), reason="reference tree not present")
+def test_sample_of_the_reference_fixture():
+    """tests/golden/tfrecord_sample.tfrecords: the first 300 records of the reference's TensorFlow-written shard 0, byte for
+    byte — framing, both CRCs, payload digest and the decoded ids against the values recorded from the whole fixture."""
+    g = GOLD["sample"]
+    h, hl, n = hashlib.sha256(), hashlib.sha256(), 0
+    for rec in R.read_records(os.path.join(HERE, "golden", g["name"]), verify=2):
+        h.update(rec.tobytes()); n += 1
+        ex = R.parse_example(rec)
+        assert set(ex) == {"feature", "label"} and ex["label"][0] == "int64"
+        assert [int(ex["label"][1][-1])] == g["eos_id"]             # EOS-terminated targets
+        hl.update(np.asarray(ex["label"][1], dtype="<i8").tobytes()); hl.update(np.asarray(ex["feature"][1], dtype="<i8").tobytes())
+    assert (n, h.hexdigest(), hl.hexdigest()) == (g["records"], g["payload_sha256"], g["ids_sha256"])
+    els = list(R.load_tfrecords(os.path.join(HERE, "golden", g["name"]), {"feature": R.VarLenInt64, "label": R.VarLenInt64}))
+    assert len(els) == n and all(int(e["label"][-1]) == g["eos_id"][0] for e in els)
+
+
+@pytest.mark.skipif(not os.path.isdir(REF_EX), reason="the whole 600 KB fixture is only read where the reference tree is installed; "
+                    "test_sample_of_the_reference_fixture covers a stored sample of it")
 def test_whole_reference_fixture():
     files = sorted(glob.glob(os.path.join(REF_EX, "train.tfrecords-*")))
     assert [os.path.basename(f) for f in files] == [g["name"] for g in GOLD["files"]]

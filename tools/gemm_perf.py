@@ -1,4 +1,4 @@
-"""C-level timing (no Python overhead) of the tcgen05 GEMM at the model's shapes. Results -> gpurun_out/gemm_perf.json"""
+"""C-level timing (no Python overhead) of the wgmma GEMM at the model's shapes. Results -> bench_out/gemm_perf.json"""
 import json
 import os
 import sys
@@ -18,7 +18,7 @@ def rnd(*s):
 
 
 def run(tag, M, N, K, out_dtype=torch.bfloat16, bn=0, stages=0, a_mn=False, b_mn=False, **kw):
-    L.b200st_debug_tc(0, 0, 0, 0, bn, stages, 0)
+    L.b200st_debug_tc(bn, stages, 0)
     A = rnd(K, M) if a_mn else rnd(M, K)
     B = rnd(K, N) if b_mn else rnd(N, K)
     Cc = torch.zeros(M, N, device=dev, dtype=out_dtype)
@@ -47,5 +47,5 @@ run("big_4096", 4096, 4096, 4096)
 # wgrad forms (split-K, fp32 accumulate)
 run("wgrad_ffn_K8000", 256, 2048, 8000, out_dtype=torch.float32, a_mn=True, b_mn=True, accumulate=True, splitk=0)
 run("wgrad_conv2_K160000", 2304, 256, 160000, out_dtype=torch.float32, a_mn=True, b_mn=True, accumulate=True, splitk=0)
-os.makedirs(os.path.join(ROOT, "gpurun_out"), exist_ok=True)
-json.dump(res, open(os.path.join(ROOT, "gpurun_out", "gemm_perf.json"), "w"), indent=1)
+os.makedirs(os.path.join(ROOT, "bench_out"), exist_ok=True)
+json.dump(res, open(os.path.join(ROOT, "bench_out", "gemm_perf.json"), "w"), indent=1)

@@ -1,9 +1,9 @@
-"""Per-launch tcgen05 GEMM timing of one training step (cfg-2) -> gpurun_out/gemm_step.csv + aggregated summary."""
+"""Per-launch wgmma GEMM timing of one training step (cfg-2) -> bench_out/gemm_step.csv + aggregated summary."""
 import collections, csv, os, sys
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
-os.makedirs(os.path.join(ROOT, "gpurun_out"), exist_ok=True)
-os.environ["B200ST_PROFILE_CSV"] = os.path.join(ROOT, "gpurun_out", "gemm_step.csv")
+os.makedirs(os.path.join(ROOT, "bench_out"), exist_ok=True)
+os.environ["B200ST_PROFILE_CSV"] = os.path.join(ROOT, "bench_out", "gemm_step.csv")
 import torch
 from neurst_b200 import lib
 from neurst_b200.trainer import build_speech_transformer_trainer, synthetic_batch
