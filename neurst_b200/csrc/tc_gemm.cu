@@ -354,8 +354,12 @@ __global__ void __launch_bounds__(kThreads, 1) tc_wgrad_group_kernel(const __gri
 // go, packed to 16 bits, straight back into the tensor cores as the register A operand of GEMM2, which accumulates the
 // [64 x D] output rows in registers across all chunks.  Only the weights stream (L2 -> smem), and the [M, ffn] hidden
 // tensor is never read back.  Slices of the hidden dimension reduce into x_out with fp32 atomics (dropout is a mask: linear).
-//   warpgroup 0: TMA producer (X once, then per chunk the W1 stages and the W2 stages, in consumption order)
-//   smem: X 64 KB | weight ring 3 x 32 KB
+//   256 threads = the two consumer warpgroups and nothing else: a CTA of at most two warpgroups is compiled to a 255-register
+//   budget, which the [64 x 256] output accumulator plus the hidden fragments need for the wgmmas to stay asynchronous (with a
+//   third, producer warpgroup the budget is 168 and the d = 256 accumulators spill).  Thread 0 issues the TMA loads: X once,
+//   then the static weight schedule (per chunk the W1 stages, then the W2 stages); it refills a ring stage as soon as all
+//   eight warps have released it.
+//   smem: X 64 KB | weight ring 4 x 32 KB (one whole chunk at d = 256)
 // =============================================================================================================
 struct MlpParams {
   int M, d, ffn;
@@ -371,7 +375,8 @@ struct MlpParams {
   float* out;                  // [M, d] fp32, added into
   int* tickets;                // deterministic mode: [m_tiles] zero-initialised; slice s adds after slices < s (self-resetting)
 };
-constexpr int kMlpStages = 3;
+constexpr int kMlpThreads = 256;
+constexpr int kMlpStages = 4;
 constexpr uint32_t kMlpStageBytes = 32768;
 constexpr uint32_t kMlpXBytes = 65536;
 constexpr size_t kMlpSmem = 1024 + kMlpXBytes + kMlpStages * kMlpStageBytes + 256;
@@ -379,12 +384,15 @@ constexpr size_t kMlpSmem = 1024 + kMlpXBytes + kMlpStages * kMlpStageBytes + 25
 // B_MN: weights as MN-major B operands (forward: W1 [d, ffn], W2 [ffn, d] in the TF [in, out] layout) or K-major (backward:
 // the same arrays read transposed: G1 uses W2 rows = hidden units, G2 uses W1 rows = model dims)
 template <int DT, bool B_MN, int D>
-__global__ void __launch_bounds__(kThreads, 1)
+__global__ void __launch_bounds__(kMlpThreads, 1)
 fused_mlp_fwd_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_constant__ CUtensorMap tmW1,
                      const __grid_constant__ CUtensorMap tmW2, const MlpParams p) {
   extern __shared__ uint8_t smem_raw[];
   constexpr bool BF = DT == BF16;
   constexpr int kbx = D / BK;                  // k-blocks of GEMM1
+  constexpr int kW1Items = kbx / 2;            // W1 ring items per chunk (2 k-blocks each)
+  constexpr int kItems = kW1Items + 2;         // ring items per chunk: the W1 items, then the 2 W2 k-blocks
+  static_assert(kMlpStages >= 3, "a warp releases item i only after it has waited for items up to i + 2");
   const uint32_t base = (ptx::smem_u32(smem_raw) + 1023u) & ~1023u;
   const uint32_t sX = base;
   const uint32_t sW = sX + kMlpXBytes;
@@ -397,8 +405,9 @@ fused_mlp_fwd_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_const
   const int m_blk = blockIdx.x / p.splits, split = blockIdx.x % p.splits;
   const int C = p.chunks_per_cta;
   const int chunk0 = split * C;
+  const bool producer = threadIdx.x == 0;
 
-  if (warp == 0 && lane == 0) {
+  if (producer) {
     ptx::prefetch_tensormap(&tmX); ptx::prefetch_tensormap(&tmW1); ptx::prefetch_tensormap(&tmW2);
     ptx::mbar_init(x_full, 1);
     for (int s2 = 0; s2 < kMlpStages; ++s2) { ptx::mbar_init(w_full(s2), 1); ptx::mbar_init(w_empty(s2), kConsumerWarps); }
@@ -408,184 +417,209 @@ fused_mlp_fwd_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_const
   pdl_wait();
   pdl_trigger();
 
-  if (warp < 4) {
-    ptx::reg_dealloc<kProducerRegs>();
-    if (warp == 0 && lane == 0) {
-      ptx::mbar_arrive_expect_tx(x_full, (uint32_t)kbx * kABytes);
-      for (int kb = 0; kb < kbx; ++kb) ptx::tma_load_4d(sX + kb * kABytes, &tmX, x_full, kb * BK, m_blk * BM, 0, 0);
-      int it = 0;
-      auto stage_wait = [&](int& st, uint32_t& dst) {
-        st = it % kMlpStages;
-        ptx::mbar_wait(w_empty(st), (((uint32_t)(it / kMlpStages)) & 1u) ^ 1u);
-        dst = sW + st * kMlpStageBytes;
-        ++it;
-      };
-      for (int c = 0; c < C; ++c) {
-        // GEMM1 B operand of chunk c: [K = d rows, N = 128 cols] as 2 k-blocks per stage
-        const int n0 = (chunk0 + c) * 128;
-        for (int s2 = 0; s2 < kbx; s2 += 2) {
-          int st; uint32_t dst;
-          stage_wait(st, dst);
-          ptx::mbar_arrive_expect_tx(w_full(st), 2u * 16384u);
-          for (int j = 0; j < 2; ++j) {
-            if (B_MN) {
-              for (int i = 0; i < 2; ++i)
-                ptx::tma_load_4d(dst + j * 16384 + i * 8192, &tmW1, w_full(st), n0 + i * 64, (s2 + j) * BK, 0, 0);
-            } else {
-              ptx::tma_load_4d(dst + j * 16384, &tmW1, w_full(st), (s2 + j) * BK, n0, 0, 0);      // [128 rows x 64 k]
-            }
-          }
-        }
-        // GEMM2 B operand of chunk c: [K = 128 hidden rows, N = d cols], one k-block per stage
-        for (int kb = 0; kb < 2; ++kb) {
-          int st; uint32_t dst;
-          stage_wait(st, dst);
-          ptx::mbar_arrive_expect_tx(w_full(st), (uint32_t)(D / 64) * 8192u);
-          if (B_MN) {
-            for (int i = 0; i < D / 64; ++i)
-              ptx::tma_load_4d(dst + i * 8192, &tmW2, w_full(st), i * 64, n0 + kb * BK, 0, 0);
-          } else {
-            ptx::tma_load_4d(dst, &tmW2, w_full(st), n0 + kb * BK, 0, 0, 0);                        // [d rows x 64 k]
-          }
+  // Producer side (thread 0 only): ring item `it` goes to stage it % kMlpStages once all 8 warps have released the item
+  // kMlpStages before it.  Every warp waits only for items up to i + 2 before it releases item i, so this wait cannot
+  // depend on a load that has not been issued yet.
+  auto issue = [&](int it) {
+    if (it >= C * kItems) return;
+    const int st = it % kMlpStages, r = it % kItems;
+    const int n0 = (chunk0 + it / kItems) * 128;
+    const uint32_t dst = sW + st * kMlpStageBytes;
+    ptx::mbar_wait(w_empty(st), (((uint32_t)(it / kMlpStages)) & 1u) ^ 1u);
+    if (r < kW1Items) {
+      // GEMM1 B operand of the chunk: [K = d rows, N = 128 cols], k-blocks 2r and 2r + 1
+      ptx::mbar_arrive_expect_tx(w_full(st), 2u * 16384u);
+      for (int j = 0; j < 2; ++j) {
+        if (B_MN) {
+          for (int i = 0; i < 2; ++i)
+            ptx::tma_load_4d(dst + j * 16384 + i * 8192, &tmW1, w_full(st), n0 + i * 64, (2 * r + j) * BK, 0, 0);
+        } else {
+          ptx::tma_load_4d(dst + j * 16384, &tmW1, w_full(st), (2 * r + j) * BK, n0, 0, 0);      // [128 rows x 64 k]
         }
       }
-    }
-  } else {
-    ptx::reg_alloc<kConsumerRegs>();
-    const int wg = (warp >> 2) - 1, g = lane >> 2, q = lane & 3;
-    const int m0 = m_blk * BM + wg * 64 + (warp & 3) * 16 + g;       // this thread's rows: m0 and m0 + 8
-    const bool use_bits = p.drop_ffn.p > 0.f;
-    const float dscale = use_bits ? p.drop_ffn.scale : 1.f;
-    const float hidden_floor = p.relu ? 0.f : -INFINITY;
-    int it = 0;
-    auto stage_get = [&](uint32_t& src) {
-      const int st = it % kMlpStages;
-      ptx::mbar_wait(w_full(st), ((uint32_t)(it / kMlpStages)) & 1u);
-      src = sW + st * kMlpStageBytes;
-      ++it;
-      return st;
-    };
-    float out[D / 2];
-#pragma unroll
-    for (int i = 0; i < D / 2; ++i) out[i] = 0.f;
-    ptx::mbar_wait(x_full, 0);
-    for (int c = 0; c < C; ++c) {
-      // The 128 hidden columns of chunk c go through the registers as two halves of 64 (GEMM1 half, epilogue, GEMM2 k-block),
-      // so that the [64 x D] output accumulator and the hidden fragments fit the register file; the W1 stages are read by
-      // both halves and released after the second.
-      uint32_t w1src[kbx / 2];
-      int w1st[kbx / 2];
-#pragma unroll
-      for (int h = 0; h < 2; ++h) {
-        // ---- GEMM1: hidden accumulator [64 x 64] ----
-        float hid[32];
-#pragma unroll
-        for (int i = 0; i < 32; ++i) hid[i] = 0.f;
-        if (h == 0) {
-#pragma unroll
-          for (int s2 = 0; s2 < kbx / 2; ++s2) w1st[s2] = stage_get(w1src[s2]);
-        }
-        ptx::fence_acc(hid);
-        ptx::wgmma_fence();
-#pragma unroll
-        for (int kb = 0; kb < kbx; ++kb) {
-          const uint32_t sa = sX + (uint32_t)kb * kABytes + (uint32_t)wg * 8192u;
-          const uint32_t sb = w1src[kb >> 1] + (uint32_t)(kb & 1) * 16384u + (uint32_t)h * 8192u;
-#pragma unroll
-          for (int k = 0; k < BK / 16; ++k)
-            ptx::WgmmaSS<64, BF, 0, B_MN>::mma(hid, ptx::desc_kmajor(sa, k), B_MN ? ptx::desc_mnmajor(sb, k) : ptx::desc_kmajor(sb, k),
-                                               (kb > 0 || k > 0) ? 1 : 0);
-        }
-        ptx::wgmma_commit();
-        ptx::wgmma_wait<0>();
-        ptx::fence_acc(hid);
-        if (h == 1 && lane == 0) {
-#pragma unroll
-          for (int s2 = 0; s2 < kbx / 2; ++s2) ptx::mbar_arrive(w_empty(w1st[s2]));
-        }
-        // ---- hidden epilogue on the fragments: bias, ReLU, dropout (forward) / relu'-dropout' mask (backward); store; pack ----
-        const int n0 = (chunk0 + c) * 128 + h * 64 + 2 * q;
-        uint32_t a16[4][4];
-#pragma unroll
-        for (int j = 0; j < 8; ++j) {
-          const int n = n0 + 8 * j;
-          float2 bb = make_float2(0.f, 0.f);
-          if (p.b1) bb = __ldg(reinterpret_cast<const float2*>(p.b1 + n));
-#pragma unroll
-          for (int hr = 0; hr < 2; ++hr) {
-            const int m = m0 + 8 * hr;
-            const bool row_ok = m < p.M;
-            float v0 = fmaxf(fmaf(hid[4 * j + 2 * hr], p.alpha, bb.x), hidden_floor);
-            float v1 = fmaxf(fmaf(hid[4 * j + 2 * hr + 1], p.alpha, bb.y), hidden_floor);
-            if (use_bits && row_ok) {
-              const uint32_t kb = (uint32_t)__ldg(p.drop_ffn.bits + ((uint64_t)((int64_t)m * p.ffn + n) >> 3)) >> (2 * q);
-              v0 = (kb & 1u) ? v0 * dscale : 0.f;
-              v1 = (kb & 2u) ? v1 * dscale : 0.f;
-            }
-            if (!B_MN && p.mask_src && row_ok) {
-              // 16-bit mask source (bf16 / fp16): "> 0" <=> sign clear and magnitude bits non-zero
-              const uint32_t w = __ldg(reinterpret_cast<const uint32_t*>(reinterpret_cast<const uint16_t*>(p.mask_src) + (int64_t)m * p.mask_ld + n));
-              const uint32_t lo = w & 0xffffu, hi = w >> 16;
-              if (!(lo != 0u && lo < 0x8000u)) v0 = 0.f;
-              if (!(hi != 0u && hi < 0x8000u)) v1 = 0.f;
-            }
-            const uint32_t pk = pack2_16(v0, v1, DT);
-            if (row_ok) *reinterpret_cast<uint32_t*>(p.F1 + (int64_t)m * p.ffn + n) = pk;
-            a16[j >> 1][(j & 1) * 2 + hr] = pk;
-          }
-        }
-        // ---- GEMM2: out[64 x D] += hidden half (registers) x the matching 64 rows of the W2 chunk ----
-        uint32_t src;
-        const int st = stage_get(src);
-        ptx::fence_acc(out);
-        ptx::wgmma_fence();
-#pragma unroll
-        for (int k = 0; k < BK / 16; ++k)
-          ptx::WgmmaRS<D, BF, B_MN>::mma(out, a16[k], B_MN ? ptx::desc_mnmajor(src, k) : ptx::desc_kmajor(src, k),
-                                         (c > 0 || h > 0 || k > 0) ? 1 : 0);
-        ptx::wgmma_commit();
-        ptx::wgmma_wait<0>();
-        ptx::fence_acc(out);
-        if (lane == 0) ptx::mbar_arrive(w_empty(st));
+    } else {
+      // GEMM2 B operand of the chunk: [K = 128 hidden rows, N = d cols], k-block kb
+      const int kb = r - kW1Items;
+      ptx::mbar_arrive_expect_tx(w_full(st), (uint32_t)(D / 64) * 8192u);
+      if (B_MN) {
+        for (int i = 0; i < D / 64; ++i)
+          ptx::tma_load_4d(dst + i * 8192, &tmW2, w_full(st), i * 64, n0 + kb * BK, 0, 0);
+      } else {
+        ptx::tma_load_4d(dst, &tmW2, w_full(st), n0 + kb * BK, 0, 0, 0);                        // [d rows x 64 k]
       }
     }
-    // ---- output rows: (+ b2 on slice 0) -> post dropout -> fp32 add into x_out ----
-    const bool add_b2 = split == 0 && p.b2 != nullptr;
-    const bool post = p.drop_post.p > 0.f;
-    const float pscale = post ? p.drop_post.scale : 1.f;
-    if (p.tickets && p.splits > 1) {
-      // deterministic reduction order: slice s adds only after slices 0 .. s-1 of this row tile have completed theirs
-      if (lane == 0) {
-        const volatile int* tk = p.tickets + m_blk;
-        while (*tk != split) { }
-        __threadfence();
-      }
-      __syncwarp();
-    }
+  };
+  if (producer) {
+    ptx::mbar_arrive_expect_tx(x_full, (uint32_t)kbx * kABytes);
+    for (int kb = 0; kb < kbx; ++kb) ptx::tma_load_4d(sX + kb * kABytes, &tmX, x_full, kb * BK, m_blk * BM, 0, 0);
+    for (int it = 0; it < kMlpStages; ++it) issue(it);
+  }
+  __syncwarp();
+
+  const int wg = warp >> 2, g = lane >> 2, q = lane & 3;
+  const int m0 = m_blk * BM + wg * 64 + (warp & 3) * 16 + g;       // this thread's rows: m0 and m0 + 8
+  const bool use_bits = p.drop_ffn.p > 0.f;
+  const float dscale = use_bits ? p.drop_ffn.scale : 1.f;
+  const float hidden_floor = p.relu ? 0.f : -INFINITY;
+  auto stage_get = [&](int it) {
+    const int st = it % kMlpStages;
+    ptx::mbar_wait(w_full(st), ((uint32_t)(it / kMlpStages)) & 1u);
+    return sW + st * kMlpStageBytes;
+  };
+  auto release = [&](int it) {
+    if (lane == 0) ptx::mbar_arrive(w_empty(it % kMlpStages));
+    if (producer) issue(it + kMlpStages);
+    __syncwarp();
+  };
+  float out[D / 2];
 #pragma unroll
-    for (int j = 0; j < D / 8; ++j) {
-      const int n = 8 * j + 2 * q;
-      float2 bb = make_float2(0.f, 0.f);
-      if (add_b2) bb = __ldg(reinterpret_cast<const float2*>(p.b2 + n));
+  for (int i = 0; i < D / 2; ++i) out[i] = 0.f;
+  ptx::mbar_wait(x_full, 0);
+  for (int c = 0; c < C; ++c) {
+    // The 128 hidden columns of chunk c go through the registers as two halves of 64 (GEMM1 half, epilogue, GEMM2 k-block),
+    // so that the [64 x D] output accumulator and the hidden fragments fit the register file; the W1 items are read by
+    // both halves and released after the second.
+    const int item0 = c * kItems;
+    uint32_t w1src[kW1Items];
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      const int n0 = (chunk0 + c) * 128 + h * 64 + 2 * q;
+      // the epilogue's dropout-bit bytes (forward) / F1 mask words (backward) do not depend on the accumulator: they are
+      // loaded before GEMM1 is issued and folded into keep bits while it runs
+      uint32_t ew[2][8];
 #pragma unroll
       for (int hr = 0; hr < 2; ++hr) {
         const int m = m0 + 8 * hr;
-        if (m < p.M) {
-          float v0 = out[4 * j + 2 * hr] + bb.x, v1 = out[4 * j + 2 * hr + 1] + bb.y;
-          if (post) {
-            const uint32_t kb = (uint32_t)__ldg(p.drop_post.bits + ((uint64_t)((int64_t)m * p.d + n) >> 3)) >> (2 * q);
-            v0 = (kb & 1u) ? v0 * pscale : 0.f;
-            v1 = (kb & 2u) ? v1 * pscale : 0.f;
-          }
-          atomicAdd(reinterpret_cast<float2*>(p.out + (int64_t)m * p.d + n), make_float2(v0, v1));
+#pragma unroll
+        for (int j = 0; j < 8; ++j) {
+          const int n = n0 + 8 * j;
+          ew[hr][j] = 0u;
+          if (use_bits && m < p.M) ew[hr][j] = (uint32_t)__ldg(p.drop_ffn.bits + ((uint64_t)((int64_t)m * p.ffn + n) >> 3)) >> (2 * q);
+          if (!B_MN && p.mask_src && m < p.M)
+            ew[hr][j] = __ldg(reinterpret_cast<const uint32_t*>(reinterpret_cast<const uint16_t*>(p.mask_src) + (int64_t)m * p.mask_ld + n));
         }
       }
+      // ---- GEMM1: hidden accumulator [64 x 64] ----
+      float hid[32];
+#pragma unroll
+      for (int i = 0; i < 32; ++i) hid[i] = 0.f;
+      if (h == 0) {
+#pragma unroll
+        for (int s2 = 0; s2 < kW1Items; ++s2) w1src[s2] = stage_get(item0 + s2);
+      }
+      ptx::fence_acc(hid);
+      ptx::wgmma_fence();
+#pragma unroll
+      for (int kb = 0; kb < kbx; ++kb) {
+        const uint32_t sa = sX + (uint32_t)kb * kABytes + (uint32_t)wg * 8192u;
+        const uint32_t sb = w1src[kb >> 1] + (uint32_t)(kb & 1) * 16384u + (uint32_t)h * 8192u;
+#pragma unroll
+        for (int k = 0; k < BK / 16; ++k)
+          ptx::WgmmaSS<64, BF, 0, B_MN>::mma(hid, ptx::desc_kmajor(sa, k), B_MN ? ptx::desc_mnmajor(sb, k) : ptx::desc_kmajor(sb, k),
+                                             (kb > 0 || k > 0) ? 1 : 0);
+      }
+      ptx::wgmma_commit();
+      // keep bits of element pair (row m0 + 8 hr, columns n0 + 8 j + {0, 1}): bits 16 hr + 2 j + {0, 1}
+      uint32_t keep = 0u;
+#pragma unroll
+      for (int hr = 0; hr < 2; ++hr) {
+#pragma unroll
+        for (int j = 0; j < 8; ++j) {
+          const uint32_t w = ew[hr][j];
+          uint32_t k2 = w & 3u;
+          if (!B_MN && p.mask_src) {
+            // 16-bit mask source (bf16 / fp16): "> 0" <=> sign clear and magnitude bits non-zero
+            const uint32_t lo = w & 0xffffu, hi = w >> 16;
+            k2 = ((lo != 0u && lo < 0x8000u) ? 1u : 0u) | ((hi != 0u && hi < 0x8000u) ? 2u : 0u);
+          }
+          keep |= k2 << (16 * hr + 2 * j);
+        }
+      }
+      asm volatile("" : "+r"(keep));            // computed before the wait, not after it
+      ptx::wgmma_wait<0>();
+      ptx::fence_acc(hid);
+      if (h == 1) {
+#pragma unroll
+        for (int s2 = 0; s2 < kW1Items; ++s2) release(item0 + s2);
+      }
+      // ---- hidden epilogue on the fragments: bias, ReLU, dropout (forward) / relu'-dropout' mask (backward); store; pack ----
+      uint32_t a16[4][4];
+#pragma unroll
+      for (int j = 0; j < 8; ++j) {
+        const int n = n0 + 8 * j;
+        float2 bb = make_float2(0.f, 0.f);
+        if (p.b1) bb = __ldg(reinterpret_cast<const float2*>(p.b1 + n));
+#pragma unroll
+        for (int hr = 0; hr < 2; ++hr) {
+          const int m = m0 + 8 * hr;
+          const bool row_ok = m < p.M;
+          float v0 = fmaxf(fmaf(hid[4 * j + 2 * hr], p.alpha, bb.x), hidden_floor);
+          float v1 = fmaxf(fmaf(hid[4 * j + 2 * hr + 1], p.alpha, bb.y), hidden_floor);
+          const uint32_t k2 = keep >> (16 * hr + 2 * j);
+          if (use_bits && row_ok) {
+            v0 = (k2 & 1u) ? v0 * dscale : 0.f;
+            v1 = (k2 & 2u) ? v1 * dscale : 0.f;
+          }
+          if (!B_MN && p.mask_src && row_ok) {
+            if (!(k2 & 1u)) v0 = 0.f;
+            if (!(k2 & 2u)) v1 = 0.f;
+          }
+          const uint32_t pk = pack2_16(v0, v1, DT);
+          if (row_ok) *reinterpret_cast<uint32_t*>(p.F1 + (int64_t)m * p.ffn + n) = pk;
+          a16[j >> 1][(j & 1) * 2 + hr] = pk;
+        }
+      }
+      // ---- GEMM2: out[64 x D] += hidden half (registers) x the matching 64 rows of the W2 chunk ----
+      const int w2_item = item0 + kW1Items + h;
+      const uint32_t src = stage_get(w2_item);
+      ptx::fence_acc(out);
+      ptx::wgmma_fence();
+#pragma unroll
+      for (int k = 0; k < BK / 16; ++k)
+        ptx::WgmmaRS<D, BF, B_MN>::mma(out, a16[k], B_MN ? ptx::desc_mnmajor(src, k) : ptx::desc_kmajor(src, k),
+                                       (c > 0 || h > 0 || k > 0) ? 1 : 0);
+      ptx::wgmma_commit();
+      ptx::wgmma_wait<0>();
+      ptx::fence_acc(out);
+      release(w2_item);
     }
-    if (p.tickets && p.splits > 1) {
+  }
+  // ---- output rows: (+ b2 on slice 0) -> post dropout -> fp32 add into x_out ----
+  const bool add_b2 = split == 0 && p.b2 != nullptr;
+  const bool post = p.drop_post.p > 0.f;
+  const float pscale = post ? p.drop_post.scale : 1.f;
+  if (p.tickets && p.splits > 1) {
+    // deterministic reduction order: slice s adds only after slices 0 .. s-1 of this row tile have completed theirs
+    if (lane == 0) {
+      const volatile int* tk = p.tickets + m_blk;
+      while (*tk != split) { }
       __threadfence();
-      asm volatile("bar.sync 1, 256;" ::: "memory");      // all 8 warps' additions have been performed
-      if (threadIdx.x == 128) atomicExch(p.tickets + m_blk, split + 1 == p.splits ? 0 : split + 1);
     }
+    __syncwarp();
+  }
+#pragma unroll
+  for (int j = 0; j < D / 8; ++j) {
+    const int n = 8 * j + 2 * q;
+    float2 bb = make_float2(0.f, 0.f);
+    if (add_b2) bb = __ldg(reinterpret_cast<const float2*>(p.b2 + n));
+#pragma unroll
+    for (int hr = 0; hr < 2; ++hr) {
+      const int m = m0 + 8 * hr;
+      if (m < p.M) {
+        float v0 = out[4 * j + 2 * hr] + bb.x, v1 = out[4 * j + 2 * hr + 1] + bb.y;
+        if (post) {
+          const uint32_t kb = (uint32_t)__ldg(p.drop_post.bits + ((uint64_t)((int64_t)m * p.d + n) >> 3)) >> (2 * q);
+          v0 = (kb & 1u) ? v0 * pscale : 0.f;
+          v1 = (kb & 2u) ? v1 * pscale : 0.f;
+        }
+        atomicAdd(reinterpret_cast<float2*>(p.out + (int64_t)m * p.d + n), make_float2(v0, v1));
+      }
+    }
+  }
+  if (p.tickets && p.splits > 1) {
+    __threadfence();
+    __syncthreads();                           // all 8 warps' additions have been performed
+    if (threadIdx.x == 0) atomicExch(p.tickets + m_blk, split + 1 == p.splits ? 0 : split + 1);
   }
 }
 
@@ -1026,7 +1060,7 @@ int fused_mlp_fwd(const void* X, int dtype, int M, int d, int ffn, const void* W
     B200ST_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kMlpSmem));
     attr[ai] = true;
   }
-  launch_pdl(kern, m_tiles * splits, kThreads, kMlpSmem, stream, tx, tw1, tw2, p);
+  launch_pdl(kern, m_tiles * splits, kMlpThreads, kMlpSmem, stream, tx, tw1, tw2, p);
   ++g_launches;
   B200ST_LAUNCH_CHECK();
   return 0;
@@ -1067,7 +1101,7 @@ int fused_mlp_bwd(const void* dY, int dtype, int M, int d, int ffn, const void* 
     B200ST_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kMlpSmem));
     attr[ai] = true;
   }
-  launch_pdl(kern, m_tiles * splits, kThreads, kMlpSmem, stream, tx, tw1, tw2, p);
+  launch_pdl(kern, m_tiles * splits, kMlpThreads, kMlpSmem, stream, tx, tw1, tw2, p);
   ++g_launches;
   B200ST_LAUNCH_CHECK();
   return 0;
