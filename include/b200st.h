@@ -190,6 +190,31 @@ int b200st_greedy_search(b200st_handle h, const b200st_buffers* buf, const b200s
                          void* stream);
 /* mode the last b200st_greedy_search actually ran in: 2 persistent kernel, 1 captured graph, 0 eager launches */
 int32_t b200st_greedy_used_graph(void);
+/* sequence_beam_search (neurst/layers/search/beam_search.py:254-439): per step, log_softmax with the greedy search's masks,
+ * accumulated log-probability times the length penalty (1/len for length_penalty < 0, else ((5+len)/6)^-length_penalty),
+ * top-beam_size over the beam_size*V candidates of each utterance (only the first beam's at step 0; lower flat index on
+ * ties), then the top_k beams of each utterance by logprob * penalty(length), best first.
+ *   st->B counts UTTERANCES: cross_kv and memory_bias are b200st_decode_init's for the B utterances (the memory is not
+ *   tiled per beam), while self_kv [dec_layers][2][B*beam_size][max_len][d] and scratch
+ *   (b200st_decode_scratch_floats(h, B*beam_size) floats) are sized for B*beam_size rows.  B*beam_size <= 8.
+ *   out_ids [B*top_k][max_steps] padded with EOS, out_scores / out_logprob / out_len [B*top_k], utterance-major.
+ *   state_words: b200st_beam_state_bytes(h, B, beam_size, st->max_len) bytes of device memory.
+ *   use_graph: 1 = the step captured once into a CUDA graph and replayed, 0 = eager launches.  beam_size == 1 is the greedy
+ *   search (b200st_greedy_search, where use_graph 2 selects its persistent kernel) with the score computed from its result.
+ * Invalid arguments (B*beam_size > 8, top_k outside 1..beam_size, max_steps > max_len, null buffers) fail before anything is
+ * launched. */
+typedef struct {
+  const int64_t* bos_ids;       /* [B] */
+  int32_t eos_id, unk_id, min_len, max_steps;
+  int32_t beam_size, top_k;
+  float length_penalty;
+  int64_t* out_ids; float* out_scores; float* out_logprob; int32_t* out_len;
+  void* state_words;
+  int32_t use_graph;
+} b200st_beam_args;
+int64_t b200st_beam_state_bytes(b200st_handle h, int32_t B, int32_t beam_size, int32_t max_len);
+int b200st_beam_search(b200st_handle h, const b200st_buffers* buf, const b200st_decode_state* st, const b200st_beam_args* a,
+                       void* stream);
 
 /* 16-bit shadow of the parameter arena (wgmma operands); shadow_dtype = B200ST_BF16 or B200ST_F16 */
 int b200st_refresh_shadow(const float* params, void* shadow, int32_t shadow_dtype, int64_t numel, void* stream);

@@ -15,7 +15,9 @@ Host mirror of
 Keys understood (the ones of examples/speech_transformer/*/st_training_args.yml): entry.class / entry.params {train_steps,
 summary_steps, save_checkpoint_steps, update_cycle, clip_value, clip_norm, criterion.params.label_smoothing, optimizer.params,
 lr_schedule.params, pretrain_model}, dataset.class AudioTFRecordDataset / dataset.params, task.class SpeechToText /
-task.params, model.class / model.params / hparams_set, model_dir, dtype.  Transcripts must already be token ids (the
+task.params, model.class / model.params / hparams_set, model_dir, dtype, and for `predict` the keys of the prediction
+recipes: `entry: predict` (the alias of entry.class) and search_method beam_search / search_method.params {beam_size,
+length_penalty, top_k, maximum_decode_length, extra_decode_length, minimum_decode_length, enable_unk}.  Transcripts must already be token ids (the
 reference's `create_tfrecords` with a projected transcript): its tokenizers / BPE are outside this path and raw text is
 refused with that message.  Checkpoints are NumPy archives keyed by the reference's variable names (checkpoints.py).
 """
@@ -31,7 +33,8 @@ import torch
 
 LOG = logging.getLogger("neurst_b200")
 
-SECTIONS = ("entry.params", "task.params", "dataset.params", "model.params")
+SECTIONS = ("entry.params", "task.params", "dataset.params", "model.params", "search_method.params")
+TOP_LEVEL = ("model_dir", "hparams_set", "dtype", "output_file", "entry", "search_method")
 
 
 # ------------------------------------------------------------------------------------------------ configuration
@@ -96,7 +99,7 @@ def load_config(paths, overrides=()):
         with open(p) as f:
             cfg = deep_merge(cfg, yaml.safe_load(f) or {})
     for key, val in overrides:
-        if "." in key or key in ("model_dir", "hparams_set", "dtype", "output_file"):
+        if "." in key or key in TOP_LEVEL:
             _set_dotted(cfg, key, val)
             continue
         hits = [s for s in SECTIONS if isinstance(cfg.get(s), dict) and key in cfg[s]]
@@ -125,6 +128,39 @@ def target_meta(task_params):
     n = int(n)
     return {"vocab_size": n, "unk_id": n - 3, "bos_id": n - 2, "eos_id": n - 1, "pad_id": n - 1, "padding_mode": "eos_as_padding",
             "tokens": tokens}
+
+
+def _module_name(cfg, name):
+    """`name.class` or its alias `name` (flags_core.py:293-299: the `.class` key wins when both are given)."""
+    v = cfg.get(name + ".class", cfg.get(name))
+    if isinstance(v, dict):
+        v = v.get("class")
+    return v
+
+
+def resolve_search(cfg, ep, tp):
+    """Search settings of `predict`.  Without search_method: greedy with the lengths of entry.params (as before).  With
+    search_method BeamSearch: its parameters (search_method.params, then entry.params) with BeamSearch's defaults
+    (beam_search.py:465-490)."""
+    length_default = int(ep.get("maximum_decode_length", tp.get("max_trg_len") or 256))
+    method = _module_name(cfg, "search_method")
+    if method is None:
+        return None, {"maximum_decode_length": length_default, "extra_decode_length": int(ep.get("extra_decode_length", 50)),
+                      "minimum_decode_length": int(ep.get("minimum_decode_length", 0))}
+    if str(method).lower().replace("_", "") != "beamsearch":
+        raise SystemExit("search_method %r is outside this path (beam_search only)" % method)
+    sp = dict(cfg.get("search_method.params") or {})
+
+    def get(key, default):
+        v = sp.get(key, ep.get(key))
+        return default if v is None else v
+
+    lp = sp.get("length_penalty", ep.get("length_penalty", 0.6))
+    return "beam_search", {"maximum_decode_length": int(get("maximum_decode_length", length_default)),
+                           "extra_decode_length": int(get("extra_decode_length", 50)),
+                           "minimum_decode_length": int(get("minimum_decode_length", 0)),
+                           "beam_size": int(get("beam_size", 4)), "length_penalty": -1.0 if lp is None else float(lp),
+                           "top_k": int(get("top_k", 1)), "enable_unk": bool(get("enable_unk", False))}
 
 
 def resolve(cfg, world=1):
@@ -165,8 +201,9 @@ def resolve(cfg, world=1):
     dsp = dict(cfg.get("dataset.params") or {})
     dataset = {"data_path": dsp.get("data_path"), "feature_key": dsp.get("feature_key", "audio"),
                "transcript_key": dsp.get("transcript_key", "transcript")}
-    return {
-        "entry": str(cfg.get("entry.class", "trainer")).lower(),
+    search_method, search = resolve_search(cfg, ep, tp)
+    plan = {
+        "entry": str(_module_name(cfg, "entry") or "trainer").lower(),
         "model_dir": cfg.get("model_dir") or ep.get("model_dir") or "./b200st_model",
         "precision": {"float16": "fp16", "fp16": "fp16", "bfloat16": "bf16", "bf16": "bf16", "float32": "fp32", "fp32": "fp32"}[
             str(cfg.get("dtype", "float16")).lower()],
@@ -177,11 +214,12 @@ def resolve(cfg, world=1):
         "clip_value": ep.get("clip_value"), "clip_norm": ep.get("clip_norm"), "pretrain_model": ep.get("pretrain_model"),
         "seed": int(ep.get("random_seed", 1234) or 1234), "max_to_keep": int(ep.get("checkpoints_max_to_keep", 8)),
         "task": task, "dataset": dataset, "trg_meta": target_meta(tp),
-        "search": {"maximum_decode_length": int(ep.get("maximum_decode_length", tp.get("max_trg_len") or 256)),
-                   "extra_decode_length": int(ep.get("extra_decode_length", 50)),
-                   "minimum_decode_length": int(ep.get("minimum_decode_length", 0))},
+        "search": search,
         "output_file": cfg.get("output_file") or ep.get("output_file"),
     }
+    if search_method:
+        plan["search_method"] = search_method
+    return plan
 
 
 # ------------------------------------------------------------------------------------------------ checkpoints
@@ -335,6 +373,10 @@ def predict(plan):
     dim = plan["task"]["audio_feature_dim"] * plan["task"]["audio_feature_channels"]
     hyps = []
     group = []
+    beam = plan.get("search_method") == "beam_search"
+    per_call = MAX_ROWS // plan["search"]["beam_size"] if beam else MAX_ROWS
+    if per_call < 1:
+        raise SystemExit("beam_size %d exceeds the %d rows a decoding step holds" % (plan["search"]["beam_size"], MAX_ROWS))
 
     def flush():
         if not group:
@@ -344,14 +386,16 @@ def predict(plan):
         for j, e in enumerate(group):
             src[j, :int(e["audio_length"])] = e["audio"]
         batch = task.example_to_input({"audio": src, "audio_length": torch.tensor([int(e["audio_length"]) for e in group])}, infer=True)
-        ids, logprob = model.greedy_search({"src": batch["src"], "src_length": batch["src_length"]}, **plan["search"])
-        for row, lp in zip(ids.cpu().tolist(), logprob.cpu().tolist()):
+        search = model.beam_search if beam else model.greedy_search
+        # beam search: top_k rows per utterance, consecutive (the reference's [B*top_k] order)
+        ids, score = search({"src": batch["src"], "src_length": batch["src_length"]}, **plan["search"])
+        for row, lp in zip(ids.cpu().tolist(), score.cpu().tolist()):
             hyps.append((ids_to_text(row, tm["eos_id"], tm.get("tokens")), lp))
         group.clear()
 
     for ex in examples:
         group.append(ex)
-        if len(group) == MAX_ROWS:
+        if len(group) == per_call:
             flush()
     flush()
     out = plan["output_file"]

@@ -22,7 +22,7 @@ using namespace b200st;
 extern "C" {
 
 const char* b200st_last_error(void) { return g_last_error.c_str(); }
-int b200st_version(void) { return 201; }
+int b200st_version(void) { return 202; }
 int64_t b200st_launch_count(void) { return g_kernel_launches + tc_launch_count(); }
 
 static GemmOperand to_operand(const b200st_operand& o) {
@@ -249,6 +249,20 @@ int b200st_greedy_search(b200st_handle h, const b200st_buffers* buf, const b200s
   return greedy_search(h->m, to_buffers(buf), to_state(st), g, reinterpret_cast<cudaStream_t>(stream));
 }
 int32_t b200st_greedy_used_graph(void) { return last_greedy_used_graph(); }
+int64_t b200st_beam_state_bytes(b200st_handle h, int32_t B, int32_t beam_size, int32_t max_len) {
+  if (!h) return -1;
+  return beam_state_bytes(B, beam_size, max_len);
+}
+int b200st_beam_search(b200st_handle h, const b200st_buffers* buf, const b200st_decode_state* st, const b200st_beam_args* a,
+                       void* stream) {
+  if (!h || !buf || !st || !a) B200ST_FAIL("null argument");
+  BeamArgs b{};
+  b.bos_ids = a->bos_ids; b.eos_id = a->eos_id; b.unk_id = a->unk_id; b.min_len = a->min_len; b.max_steps = a->max_steps;
+  b.beam_size = a->beam_size; b.top_k = a->top_k; b.length_penalty = a->length_penalty;
+  b.out_ids = a->out_ids; b.out_scores = a->out_scores; b.out_logprob = a->out_logprob; b.out_len = a->out_len;
+  b.state_words = a->state_words; b.use_graph = a->use_graph;
+  return beam_search(h->m, to_buffers(buf), to_state(st), b, reinterpret_cast<cudaStream_t>(stream));
+}
 int b200st_refresh_shadow(const float* params, void* shadow, int32_t shadow_dtype, int64_t numel, void* stream) {
   if (!params || !shadow) B200ST_FAIL("null argument");
   return cast_f32_to_16(params, shadow, shadow_dtype, numel, reinterpret_cast<cudaStream_t>(stream));

@@ -1,6 +1,6 @@
-// Incremental (cached) decoding and greedy search on the device — SURVEY.md §8 f1, BASELINE cfg-5.
+// Incremental (cached) decoding, greedy and beam search on the device — SURVEY.md §8 f1, BASELINE cfg-5.
 //
-// Replaces, for beam_size = 1, the loop  sequence_beam_search -> symbols_to_logits_fn -> TransformerDecoder.call(cache)
+// Replaces the loop  sequence_beam_search -> symbols_to_logits_fn -> TransformerDecoder.call(cache)
 //   neurst/layers/search/beam_search.py:254-439 (search loop, finished / EOS / UNK / min-length masking :70-138,373-395)
 //   neurst/models/encoder_decoder_model.py:211-261 (symbols_to_logits_fn: embed(time) -> decoder(cache) -> logits)
 //   neurst/layers/decoders/transformer_decoder.py:105-147,171-228 (cache creation, cached step)
@@ -137,25 +137,36 @@ __global__ void __launch_bounds__(128) gemv_kernel(const float* __restrict__ in,
 // (accumulated straight into the residual stream x).  SELF: q/k/v come from the qkv accumulator, k/v are appended to the
 // cache at position `time` (multi_head_attention.py:271-276); else q from `qsrc`, keys = pre-projected memory with the
 // additive memory bias.  q is scaled by dh^-0.5 after the projection bias (multi_head_attention.py:203).
-template <typename TW, bool SELF>
+// BEAM (beam search, rows = utterances x beam): the self-attention key/value of position j < time of row b live in the
+// slot of row anc[b][j] (the ancestry table kept by beam_select_kernel, so beams are reordered without copying the
+// cache); position `time` is always the row's own slot.  Cross-attention reads the memory of utterance b / beam, which
+// is projected once per utterance.
+template <typename TW, bool SELF, bool BEAM = false>
 __global__ void __launch_bounds__(256) attn_step_kernel(const float* __restrict__ qsrc, int q_ld, float* __restrict__ kcache,
                                                         float* __restrict__ vcache, int kv_ld, int cache_rows,
                                                         const float* __restrict__ mem_bias, const TW* __restrict__ Wo,
                                                         const float* __restrict__ bo, float* __restrict__ x, int d, int dh, int Tm,
-                                                        const int* __restrict__ time_dev) {
+                                                        const int* __restrict__ time_dev, const int* __restrict__ anc = nullptr,
+                                                        int beam = 1) {
   pdl_wait();
   pdl_trigger();
-  extern __shared__ float sm[];          // q[dh] | ctx[dh] | scores[nk] | red[8]
+  extern __shared__ float sm[];          // q[dh] | ctx[dh] | scores[nk] | red[8] (| BEAM && SELF: slot of each key [nk])
   const int h = blockIdx.x, b = blockIdx.y;
   const int t = *time_dev;
   const int nk = SELF ? t + 1 : Tm;
+  const int mb = (BEAM && !SELF) ? b / beam : b;      // memory row
   float* q = sm;
   float* ctx = sm + dh;
   float* sc = sm + 2 * dh;
   float* red = sc + nk;
+  int* slot = reinterpret_cast<int*>(red + 8);
   const float* qrow = qsrc + (int64_t)b * q_ld + h * dh;
-  float* kbase = kcache + (int64_t)b * cache_rows * kv_ld + h * dh;
-  float* vbase = vcache + (int64_t)b * cache_rows * kv_ld + h * dh;
+  float* kbase = kcache + (int64_t)mb * cache_rows * kv_ld + h * dh;
+  float* vbase = vcache + (int64_t)mb * cache_rows * kv_ld + h * dh;
+  // key j is read at kb + koff(j): the own row's cache, or (BEAM && SELF) cache slot (anc[b][j], j) of the whole cache
+  const float* kb = (BEAM && SELF) ? kcache + h * dh : kbase;
+  const float* vb = (BEAM && SELF) ? vcache + h * dh : vbase;
+  auto koff = [&](int j) -> int64_t { return (BEAM && SELF) ? (int64_t)slot[j] * kv_ld : (int64_t)j * kv_ld; };
   const float alpha = rsqrtf((float)dh);
   for (int c = threadIdx.x; c < dh; c += blockDim.x) {
     q[c] = qrow[c] * alpha;
@@ -164,11 +175,13 @@ __global__ void __launch_bounds__(256) attn_step_kernel(const float* __restrict_
       vbase[(int64_t)t * kv_ld + c] = qrow[2 * d + c];
     }
   }
+  if (BEAM && SELF)
+    for (int j = threadIdx.x; j < nk; j += blockDim.x) slot[j] = (j < t ? anc[(int64_t)b * cache_rows + j] : b) * cache_rows + j;
   __syncthreads();
   // scores: one thread per key — its dh-float key row is read with independent 16-byte loads (no cross-lane reduction,
   // every load of the row in flight at once: the loop is latency-bound otherwise)
   for (int j = threadIdx.x; j < nk; j += blockDim.x) {
-    const float* kr = kbase + (int64_t)j * kv_ld;
+    const float* kr = kb + koff(j);
     float s = 0.f;
     if ((dh & 3) == 0) {
 #pragma unroll 4
@@ -179,7 +192,7 @@ __global__ void __launch_bounds__(256) attn_step_kernel(const float* __restrict_
     } else {
       for (int c = 0; c < dh; ++c) s = fmaf(q[c], kr[c], s);
     }
-    sc[j] = s + ((!SELF && mem_bias) ? mem_bias[(int64_t)b * Tm + j] : 0.f);
+    sc[j] = s + ((!SELF && mem_bias) ? mem_bias[(int64_t)mb * Tm + j] : 0.f);
   }
   __syncthreads();
   float mx = -INFINITY;
@@ -198,12 +211,12 @@ __global__ void __launch_bounds__(256) attn_step_kernel(const float* __restrict_
       float a0 = 0.f, a1 = 0.f, a2 = 0.f, a3 = 0.f;
       int j = part;
       for (; j + 3 * nparts < nk; j += 4 * nparts) {
-        a0 = fmaf(sc[j], vbase[(int64_t)j * kv_ld + c], a0);
-        a1 = fmaf(sc[j + nparts], vbase[(int64_t)(j + nparts) * kv_ld + c], a1);
-        a2 = fmaf(sc[j + 2 * nparts], vbase[(int64_t)(j + 2 * nparts) * kv_ld + c], a2);
-        a3 = fmaf(sc[j + 3 * nparts], vbase[(int64_t)(j + 3 * nparts) * kv_ld + c], a3);
+        a0 = fmaf(sc[j], vb[koff(j) + c], a0);
+        a1 = fmaf(sc[j + nparts], vb[koff(j + nparts) + c], a1);
+        a2 = fmaf(sc[j + 2 * nparts], vb[koff(j + 2 * nparts) + c], a2);
+        a3 = fmaf(sc[j + 3 * nparts], vb[koff(j + 3 * nparts) + c], a3);
       }
-      for (; j < nk; j += nparts) a0 = fmaf(sc[j], vbase[(int64_t)j * kv_ld + c], a0);
+      for (; j < nk; j += nparts) a0 = fmaf(sc[j], vb[koff(j) + c], a0);
       atomicAdd(&ctx[c], (a0 + a1 + a2 + a3) * inv);
     }
   }
@@ -328,6 +341,205 @@ __global__ void greedy_init_kernel(GreedyState g, const int64_t* __restrict__ bo
   if (i < B) { g.ids[i] = bos[i]; g.finished[i] = 0; g.length[i] = 0; g.logprob[i] = 0.f; }
   if (i == 0) { *g.time = 0; *g.all_finished = 0; }
   for (int j = i; j < B * max_steps; j += gridDim.x * blockDim.x) g.out[j] = eos;   // padded with EOS (beam_search.py:428-436)
+}
+
+// ---- beam search (beam_search.py:71-251,380-437): rows = utterances x beam, row u*beam + k holds beam k of utterance u ----
+constexpr int KMAX = MAXB;     // largest beam: every beam of an utterance is a row of the same step
+struct BeamState {
+  int64_t* ids;          // [rows] current input ids
+  float* logprob;        // [rows] accumulated log probability
+  int32_t* finished;     // [rows]
+  int32_t* length;       // [rows] decoding length
+  int32_t* anc;          // [rows][max_len] cache row whose slot holds position j of the hypothesis now in row r
+  int32_t* hist;         // [rows][max_len] word chosen at step j for row r
+  int32_t* time;         // [1]
+  int32_t* all_finished; // [1]
+  uint32_t* ticket;      // [1] blocks done with the current step (the last one publishes time / all_finished)
+};
+
+// _calculate_length_penalty (beam_search.py:24-40): 1/len for alpha < 0, else ((5 + len) / 6)^-alpha
+__device__ __forceinline__ float length_penalty(int len, float alpha) {
+  return alpha < 0.f ? 1.f / (float)len : powf((5.f + (float)len) / 6.f, -alpha);
+}
+// tf.nn.top_k order: higher score first, the lower flat index on ties
+__device__ __forceinline__ bool cand_better(float s, int i, float s2, int i2) { return s > s2 || (s == s2 && i < i2); }
+
+// One search step of one utterance (block = utterance, so every row it reads or reorders is its own): log_softmax of each
+// beam row with the finished / UNK / min-length masks (:71-142,380-388), accumulated log-probabilities times the length
+// penalty of next_length = length + 1 - finished (:145-179), top-`beam` over the beam*V candidates (only the first beam's
+// V at time 0; :181-190), then the reorder of the row state and of the ancestry table (:395-404).  The top-k is a
+// per-thread register top-KMAX over the thread's candidates followed by `beam` rounds of a block-wide arg-max.
+__global__ void __launch_bounds__(1024) beam_select_kernel(const float* __restrict__ logits, BeamState s, int beam, int V, int eos,
+                                                           int unk, int min_len, float alpha, int max_len) {
+  pdl_wait();
+  pdl_trigger();
+  __shared__ float red[32];
+  __shared__ float sval[32];
+  __shared__ int sidx[32];
+  __shared__ float lse[KMAX], pen[KMAX], lprev[KMAX];
+  __shared__ int fin[KMAX], nlen[KMAX], win[KMAX];
+  const int r0 = blockIdx.x * beam;
+  const int t = *s.time;
+  const int lane = threadIdx.x & 31, w = threadIdx.x >> 5, nw = blockDim.x >> 5;
+  for (int b = 0; b < beam; ++b) {
+    const float* z = logits + (int64_t)(r0 + b) * V;
+    float mx = -INFINITY;
+    for (int v = threadIdx.x; v < V; v += blockDim.x) mx = fmaxf(mx, z[v]);
+    mx = block_max(mx, red);
+    float se = 0.f;
+    for (int v = threadIdx.x; v < V; v += blockDim.x) se += expf(z[v] - mx);
+    se = block_sum(se, red);
+    if (threadIdx.x == 0) {
+      lse[b] = mx + logf(se);
+      fin[b] = s.finished[r0 + b] != 0;
+      lprev[b] = s.logprob[r0 + b];
+      nlen[b] = s.length[r0 + b] + 1 - fin[b];
+      pen[b] = length_penalty(nlen[b], alpha);
+    }
+  }
+  __syncthreads();
+  // accumulated log-probability of candidate (beam b, word v), un-penalised
+  auto acc_of = [&](int b, int v) -> float {
+    float lp = logits[(int64_t)(r0 + b) * V + v] - lse[b];
+    if (fin[b]) lp = (v == eos) ? 0.f : kFloatMin;
+    if (v == unk) lp += kFloatMin;
+    if (v == eos && t < min_len - 1) lp += kFloatMin;
+    return lp + lprev[b];
+  };
+  float vs[KMAX];
+  int is[KMAX];
+#pragma unroll
+  for (int q = 0; q < KMAX; ++q) { vs[q] = -INFINITY; is[q] = 0x7fffffff; }
+  const int nb = t == 0 ? 1 : beam;
+  for (int b = 0; b < nb; ++b) {
+    for (int v = threadIdx.x; v < V; v += blockDim.x) {
+      const float sc = acc_of(b, v) * pen[b];
+      const int i = b * V + v;
+      if (cand_better(sc, i, vs[KMAX - 1], is[KMAX - 1])) {
+        vs[KMAX - 1] = sc; is[KMAX - 1] = i;
+#pragma unroll
+        for (int q = KMAX - 1; q > 0; --q) {
+          if (cand_better(vs[q], is[q], vs[q - 1], is[q - 1])) {
+            const float tv = vs[q]; vs[q] = vs[q - 1]; vs[q - 1] = tv;
+            const int ti = is[q]; is[q] = is[q - 1]; is[q - 1] = ti;
+          }
+        }
+      }
+    }
+  }
+  for (int k = 0; k < beam; ++k) {
+    float bv = vs[0];
+    int bi = is[0];
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) {
+      const float ov = __shfl_xor_sync(0xffffffffu, bv, o);
+      const int oi = __shfl_xor_sync(0xffffffffu, bi, o);
+      if (cand_better(ov, oi, bv, bi)) { bv = ov; bi = oi; }
+    }
+    __syncthreads();
+    if (lane == 0) { sval[w] = bv; sidx[w] = bi; }
+    __syncthreads();
+    if (threadIdx.x == 0) {
+      for (int i = 1; i < nw; ++i)
+        if (cand_better(sval[i], sidx[i], bv, bi)) { bv = sval[i]; bi = sidx[i]; }
+      win[k] = bi < nb * V ? bi : 0;
+    }
+    __syncthreads();
+    if (is[0] == win[k]) {                        // flat indices are unique: exactly one thread pops its head
+#pragma unroll
+      for (int q = 0; q < KMAX - 1; ++q) { vs[q] = vs[q + 1]; is[q] = is[q + 1]; }
+      vs[KMAX - 1] = -INFINITY; is[KMAX - 1] = 0x7fffffff;
+    }
+  }
+  // new row r0 + j continues beam p = win[j] / V with word win[j] % V (every old value was read into shared memory above)
+  if ((int)threadIdx.x < beam) {
+    const int j = threadIdx.x, p = win[j] / V, word = win[j] % V;
+    const int r = r0 + j;
+    s.ids[r] = word;
+    s.logprob[r] = acc_of(p, word);
+    s.length[r] = nlen[p];
+    s.finished[r] = word == eos ? 1 : 0;
+    s.hist[(int64_t)r * max_len + t] = word;
+  }
+  // ancestry: anc'[r0 + j][col] = anc[r0 + p][col] for col < t, and r0 + p at col = t (the parent's own slot).  A thread
+  // owns whole columns, so reading every parent's entry before writing needs no barrier.
+  for (int col = threadIdx.x; col <= t; col += blockDim.x) {
+    int nv[KMAX];
+#pragma unroll
+    for (int j = 0; j < KMAX; ++j) {
+      if (j < beam) {
+        const int p = r0 + win[j] / V;
+        nv[j] = col == t ? p : s.anc[(int64_t)p * max_len + col];
+      }
+    }
+#pragma unroll
+    for (int j = 0; j < KMAX; ++j)
+      if (j < beam) s.anc[(int64_t)(r0 + j) * max_len + col] = nv[j];
+  }
+  // the last block of the step publishes all_finished (every row of every utterance) and advances time: every block has
+  // read `time` before it takes its ticket
+  __threadfence();
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    __threadfence();
+    if (atomicAdd(s.ticket, 1u) == gridDim.x - 1) {
+      __threadfence();
+      int all = 1;
+      for (int r = 0; r < (int)gridDim.x * beam; ++r) all &= __ldcg(s.finished + r) != 0 ? 1 : 0;
+      *s.all_finished = all;
+      *s.ticket = 0;
+      *s.time = t + 1;
+    }
+  }
+}
+
+__global__ void beam_init_kernel(BeamState s, const int64_t* __restrict__ bos, int rows, int beam) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i < rows) { s.ids[i] = bos[i / beam]; s.logprob[i] = 0.f; s.finished[i] = 0; s.length[i] = 0; }   // stack_beam_size
+  if (i == 0) { *s.time = 0; *s.all_finished = 0; *s.ticket = 0; }
+}
+
+// _extract_beam_results (beam_search.py:217-251,428-437), block = utterance: the top_k beams by logprob * penalty(length),
+// best first (lower beam on ties); hypothesis j-th token = hist[anc[r][j + 1]][j] (the row that consumed it as its next
+// input), the last step's from hist[r]; EOS after the steps taken.
+__global__ void beam_extract_kernel(BeamState s, int beam, int top_k, float alpha, int eos, int max_len, int max_steps,
+                                    int64_t* __restrict__ out_ids, float* __restrict__ out_scores, float* __restrict__ out_logprob,
+                                    int32_t* __restrict__ out_len) {
+  __shared__ float sc[KMAX];
+  __shared__ int order[KMAX];
+  const int u = blockIdx.x, r0 = u * beam;
+  const int T = *s.time;
+  if (threadIdx.x == 0) {
+    int used = 0;
+    for (int b = 0; b < beam; ++b) sc[b] = s.logprob[r0 + b] * length_penalty(s.length[r0 + b], alpha);
+    for (int k = 0; k < top_k; ++k) {
+      int best = -1;
+      for (int b = 0; b < beam; ++b)
+        if (!((used >> b) & 1) && (best < 0 || sc[b] > sc[best])) best = b;
+      used |= 1 << best;
+      order[k] = best;
+    }
+  }
+  __syncthreads();
+  if ((int)threadIdx.x < top_k) {
+    const int k = threadIdx.x, r = r0 + order[k], o = u * top_k + k;
+    out_scores[o] = sc[order[k]];
+    out_logprob[o] = s.logprob[r];
+    out_len[o] = s.length[r];
+  }
+  for (int i = threadIdx.x; i < top_k * max_steps; i += blockDim.x) {
+    const int k = i / max_steps, j = i % max_steps, r = r0 + order[k];
+    int tok = eos;
+    if (j < T) tok = s.hist[(int64_t)(j + 1 < T ? s.anc[(int64_t)r * max_len + j + 1] : r) * max_len + j];
+    out_ids[(int64_t)(u * top_k + k) * max_steps + j] = tok;
+  }
+}
+
+// beam_size = 1 runs the greedy search; its score is the accumulated log-probability times the length penalty
+__global__ void beam1_score_kernel(const float* __restrict__ logprob, const int32_t* __restrict__ length, float* __restrict__ scores,
+                                   int B, float alpha) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i < B) scores[i] = logprob[i] * length_penalty(length[i], alpha);
 }
 
 
@@ -670,8 +882,17 @@ struct StepCtx {
   int64_t off(const std::string& n) const { const int i = m.find(n); return i < 0 ? -1 : m.params[i].offset; }
 };
 
+// Shared-memory bytes of the self-attention step: q | ctx | scores | red, plus the slot of each key in beam search.
+size_t self_attn_smem(const Config& cf, int max_len, bool beam) {
+  const int dh = cf.d / cf.heads;
+  return sizeof(float) * (size_t)(2 * dh + max_len + 8) + (beam ? sizeof(int) * (size_t)max_len : 0);
+}
+
+// One decoder step over st.B rows.  anc != null: beam search with `beam` rows per utterance (st.B = utterances x beam):
+// self-attention follows the ancestry table, cross-attention reads the memory of row / beam.
 template <typename TW>
-int step_launch(const StepCtx& c, const TW* wbase, const int64_t* ids, const int32_t* time_dev, float* logits_out) {
+int step_launch(const StepCtx& c, const TW* wbase, const int64_t* ids, const int32_t* time_dev, float* logits_out,
+                const int* anc, int beam) {
   const Config& cf = c.m.cfg;
   const DecodeState& st = c.st;
   const int B = st.B, d = cf.d, H = cf.heads, dh = d / H, f = cf.ffn, V = cf.vocab;
@@ -681,7 +902,7 @@ int step_launch(const StepCtx& c, const TW* wbase, const int64_t* ids, const int
   B200ST_CUDA(cudaMemsetAsync(st.scratch + lo.qkv, 0, sizeof(float) * (size_t)(lo.logits - lo.qkv), c.s));
   auto W = [&](const std::string& n) { return wbase + c.off(n); };
   launch_pdl(embed_step_kernel<TW>, (B * d + 255) / 256, 256, 0, c.s, ids, W("trg.emb"), x, B, d, V, time_dev);
-  const int64_t self_layer = 2 * (int64_t)B * st.max_len * d, cross_layer = (int64_t)B * st.Tm * 2 * d;
+  const int64_t self_layer = 2 * (int64_t)B * st.max_len * d, cross_layer = (int64_t)(B / beam) * st.Tm * 2 * d;
   for (int i = 0; i < cf.dec_layers; ++i) {
     const std::string p = "dec." + std::to_string(i);
     float* qkv = st.scratch + lo.qkv + (int64_t)i * B * 3 * d;
@@ -692,17 +913,19 @@ int step_launch(const StepCtx& c, const TW* wbase, const int64_t* ids, const int
                c.P(p + ".self.ln.beta"), (const float*)nullptr, cf.ln_eps, W(p + ".self.qkv.kernel"), c.P(p + ".self.qkv.bias"), qkv, B, d, 3 * d);
     float* sk = st.self_kv + (int64_t)i * self_layer;
     float* sv = sk + (int64_t)B * st.max_len * d;
-    const size_t smem_self = sizeof(float) * (size_t)(2 * dh + st.max_len + 8);
-    launch_pdl(attn_step_kernel<TW, true>, dim3(H, B), 256, smem_self, c.s, (const float*)qkv, 3 * d, sk, sv, d, st.max_len,
-               (const float*)nullptr, W(p + ".self.out.kernel"), c.P(p + ".self.out.bias"), x, d, dh, 0, time_dev);
+    const size_t smem_self = self_attn_smem(cf, st.max_len, anc != nullptr);
+    launch_pdl(anc ? attn_step_kernel<TW, true, true> : attn_step_kernel<TW, true>, dim3(H, B), 256, smem_self, c.s,
+               (const float*)qkv, 3 * d, sk, sv, d, st.max_len, (const float*)nullptr, W(p + ".self.out.kernel"),
+               c.P(p + ".self.out.bias"), x, d, dh, 0, time_dev, anc, beam);
     // encoder-decoder attention block over the pre-projected memory
     if (cf.with_cross_attention && st.Tm > 0) {
       launch_pdl(gemv_kernel<TW, 0>, dim3((d + 127) / 128, (d + 31) / 32), 128, 0, c.s, (const float*)x, c.P(p + ".cross.ln.gamma"),
                  c.P(p + ".cross.ln.beta"), (const float*)nullptr, cf.ln_eps, W(p + ".cross.q.kernel"), c.P(p + ".cross.q.bias"), qc, B, d, d);
       float* ck = st.cross_kv + (int64_t)i * cross_layer;
       const size_t smem_cross = sizeof(float) * (size_t)(2 * dh + st.Tm + 8);
-      launch_pdl(attn_step_kernel<TW, false>, dim3(H, B), 256, smem_cross, c.s, (const float*)qc, d, ck, ck + d, 2 * d, st.Tm,
-                 st.memory_bias, W(p + ".cross.out.kernel"), c.P(p + ".cross.out.bias"), x, d, dh, st.Tm, time_dev);
+      launch_pdl(anc ? attn_step_kernel<TW, false, true> : attn_step_kernel<TW, false>, dim3(H, B), 256, smem_cross, c.s,
+                 (const float*)qc, d, ck, ck + d, 2 * d, st.Tm, st.memory_bias, W(p + ".cross.out.kernel"),
+                 c.P(p + ".cross.out.bias"), x, d, dh, st.Tm, time_dev, anc, beam);
     }
     // feed-forward block
     launch_pdl(gemv_kernel<TW, 0>, dim3((f + 127) / 128, (d + 31) / 32), 128, 0, c.s, (const float*)x, c.P(p + ".ffn.ln.gamma"),
@@ -718,13 +941,53 @@ int step_launch(const StepCtx& c, const TW* wbase, const int64_t* ids, const int
   return 0;
 }
 
-int step_dispatch(const StepCtx& c, const int64_t* ids, const int32_t* time_dev, float* logits_out) {
+int step_dispatch(const StepCtx& c, const int64_t* ids, const int32_t* time_dev, float* logits_out, const int* anc = nullptr,
+                  int beam = 1) {
   if (c.st.use_shadow) {
     B200ST_CHECK(is16(c.m.adt) && c.buf.shadow, "use_shadow needs a 16-bit precision handle and its shadow arena");
-    if (c.m.adt == F16) return step_launch(c, reinterpret_cast<const __half*>(c.buf.shadow), ids, time_dev, logits_out);
-    return step_launch(c, reinterpret_cast<const __nv_bfloat16*>(c.buf.shadow), ids, time_dev, logits_out);
+    if (c.m.adt == F16) return step_launch(c, reinterpret_cast<const __half*>(c.buf.shadow), ids, time_dev, logits_out, anc, beam);
+    return step_launch(c, reinterpret_cast<const __nv_bfloat16*>(c.buf.shadow), ids, time_dev, logits_out, anc, beam);
   }
-  return step_launch(c, c.buf.params, ids, time_dev, logits_out);
+  return step_launch(c, c.buf.params, ids, time_dev, logits_out, anc, beam);
+}
+
+// Per-token loop of both searches: step 0 eagerly (also warms function attributes outside the capture), then one step —
+// decoder kernels + the search's pick — captured ONCE into a CUDA graph and replayed (use_graph), or launched eagerly;
+// stops when every row has finished (checked every 8 tokens through a pinned flag) or after `max_steps`.  *graphed tells
+// whether the graph was used.  The caller's stream must not be capturing.
+template <typename StepFn>
+int run_token_loop(cudaStream_t s, int max_steps, bool use_graph, const int32_t* all_finished, StepFn&& one_step, bool* graphed_out) {
+  cudaGraph_t graph = nullptr;
+  cudaGraphExec_t exec = nullptr;
+  bool graphed = false;
+  if (use_graph) {
+    B200ST_TRY(one_step());
+    if (cudaStreamBeginCapture(s, cudaStreamCaptureModeThreadLocal) == cudaSuccess) {
+      const int rc = one_step();
+      cudaError_t e = cudaStreamEndCapture(s, &graph);
+      if (rc == 0 && e == cudaSuccess && graph && cudaGraphInstantiate(&exec, graph, 0) == cudaSuccess) graphed = true;
+      else { cudaGetLastError(); pdl_launch_error() = cudaSuccess; }
+    } else {
+      cudaGetLastError();
+    }
+  }
+  *graphed_out = graphed;
+  static thread_local int32_t* flag_host = nullptr;     // pinned word for the "all rows finished" poll
+  if (!flag_host) B200ST_CUDA(cudaMallocHost(&flag_host, sizeof(int32_t)));
+  *flag_host = 0;
+  int rc = 0;
+  for (int t = use_graph ? 1 : 0; t < max_steps && rc == 0; ++t) {
+    if (graphed) { if (cudaGraphLaunch(exec, s) != cudaSuccess) { set_last_error("decode graph launch failed"); rc = 1; } }
+    else rc = one_step();
+    if (rc == 0 && (t % 8 == 7 || t + 1 == max_steps)) {
+      cudaMemcpyAsync(flag_host, all_finished, sizeof(int32_t), cudaMemcpyDeviceToHost, s);
+      if (cudaStreamSynchronize(s) != cudaSuccess) { set_last_error("decode step failed"); rc = 1; }
+      if (*flag_host) break;
+    }
+  }
+  if (exec) cudaGraphExecDestroy(exec);
+  if (graph) cudaGraphDestroy(graph);
+  return rc;
 }
 
 
@@ -887,37 +1150,89 @@ int greedy_search(const Model& m, const Buffers& buf, const DecodeState& st, con
     B200ST_LAUNCH_CHECK();
     return 0;
   };
-  cudaGraph_t graph = nullptr;
-  cudaGraphExec_t exec = nullptr;
   bool graphed = false;
-  if (ga.use_graph) {
-    B200ST_TRY(one_step());                     // step 0 eagerly (also warms function attributes outside the capture)
-    if (cudaStreamBeginCapture(s, cudaStreamCaptureModeThreadLocal) == cudaSuccess) {
-      const int rc = one_step();
-      cudaError_t e = cudaStreamEndCapture(s, &graph);
-      if (rc == 0 && e == cudaSuccess && graph && cudaGraphInstantiate(&exec, graph, 0) == cudaSuccess) graphed = true;
-      else { cudaGetLastError(); pdl_launch_error() = cudaSuccess; }
-    } else {
-      cudaGetLastError();
-    }
-  }
+  const int rc = run_token_loop(s, ga.max_steps, ga.use_graph != 0, g.all_finished, one_step, &graphed);
   g_last_greedy_graph = graphed ? 1 : 0;
-  static thread_local int32_t* flag_host = nullptr;     // pinned word for the "all rows finished" poll
-  if (!flag_host) B200ST_CUDA(cudaMallocHost(&flag_host, sizeof(int32_t)));
-  *flag_host = 0;
-  int rc = 0;
-  for (int t = ga.use_graph ? 1 : 0; t < ga.max_steps && rc == 0; ++t) {
-    if (graphed) { if (cudaGraphLaunch(exec, s) != cudaSuccess) { set_last_error("decode graph launch failed"); rc = 1; } }
-    else rc = one_step();
-    if (rc == 0 && (t % 8 == 7 || t + 1 == ga.max_steps)) {
-      cudaMemcpyAsync(flag_host, g.all_finished, sizeof(int32_t), cudaMemcpyDeviceToHost, s);
-      if (cudaStreamSynchronize(s) != cudaSuccess) { set_last_error("decode step failed"); rc = 1; }
-      if (*flag_host) break;
-    }
-  }
-  if (exec) cudaGraphExecDestroy(exec);
-  if (graph) cudaGraphDestroy(graph);
   return rc;
+}
+
+int64_t beam_state_bytes(int B, int beam, int max_len) {
+  if (B < 1 || beam < 1 || max_len < 1) return -1;
+  const int64_t rows = (int64_t)B * beam;
+  const int64_t words = rows * (8 + 4 + 4 + 4) + 16 + 2 * rows * max_len * 4;   // ids | logprob | finished | length | 4 words | anc | hist
+  const int64_t bytes = (words + 255) / 256 * 256;
+  return bytes < 512 ? 512 : bytes;                 // beam_size 1 runs the greedy search in the same words (>= 256 bytes)
+}
+
+// sequence_beam_search (beam_search.py:254-439) with the per-token step of the greedy search on B x beam rows.
+int beam_search(const Model& m, const Buffers& buf, const DecodeState& st, const BeamArgs& a, cudaStream_t s) {
+  B200ST_TRY(check_state(m, st));
+  const Config& cf = m.cfg;
+  const int beam = a.beam_size;
+  B200ST_CHECK(beam >= 1, "beam_size must be >= 1");
+  B200ST_CHECK(a.top_k >= 1 && a.top_k <= beam, "top_k must be in 1..beam_size");
+  B200ST_CHECK((int64_t)st.B * beam <= MAXB, "beam search decodes at most " + std::to_string(MAXB) + " rows (utterances x beam_size) per call, got " +
+                                              std::to_string(st.B) + " x " + std::to_string(beam));
+  B200ST_CHECK(beam <= cf.vocab, "beam_size exceeds the vocabulary");
+  B200ST_CHECK(a.max_steps >= 1 && a.max_steps <= st.max_len, "max_steps must be within the cache length");
+  B200ST_CHECK(a.bos_ids && a.out_ids && a.out_scores && a.out_len && a.out_logprob && a.state_words, "beam_search: null argument");
+  if (beam == 1) {           // the reference's beam 1 is the greedy search
+    GreedyArgs ga{};
+    ga.bos_ids = a.bos_ids; ga.eos_id = a.eos_id; ga.unk_id = a.unk_id; ga.min_len = a.min_len; ga.max_steps = a.max_steps;
+    ga.out_ids = a.out_ids; ga.out_len = a.out_len; ga.out_logprob = a.out_logprob; ga.state_words = a.state_words;
+    ga.use_graph = a.use_graph;
+    B200ST_TRY(greedy_search(m, buf, st, ga, s));
+    beam1_score_kernel<<<1, 32, 0, s>>>(a.out_logprob, a.out_len, a.out_scores, st.B, a.length_penalty);
+    B200ST_CUDA(cudaGetLastError());
+    return 0;
+  }
+  const int rows = st.B * beam;
+  DecodeState rs = st;                    // the step runs on every beam row; cross_kv / memory_bias stay per utterance
+  rs.B = rows;
+  B200ST_TRY(check_state(m, rs));
+  const size_t smem_self = self_attn_smem(cf, st.max_len, true);
+  B200ST_CHECK(smem_self <= 200 * 1024, "decode: too many keys for the shared-memory score buffer");
+  B200ST_TRY(raise_all_smem(cf, st));
+  B200ST_TRY(raise_smem(attn_step_kernel<float, true, true>, smem_self));
+  B200ST_TRY(raise_smem(attn_step_kernel<__half, true, true>, smem_self));
+  B200ST_TRY(raise_smem(attn_step_kernel<__nv_bfloat16, true, true>, smem_self));
+  const size_t smem_cross = sizeof(float) * (size_t)(2 * (cf.d / cf.heads) + st.Tm + 8);
+  B200ST_TRY(raise_smem(attn_step_kernel<float, false, true>, smem_cross));
+  B200ST_TRY(raise_smem(attn_step_kernel<__half, false, true>, smem_cross));
+  B200ST_TRY(raise_smem(attn_step_kernel<__nv_bfloat16, false, true>, smem_cross));
+  // device words: [ids rows x int64][logprob rows][finished rows][length rows][time][all_finished][ticket][pad][anc][hist]
+  char* w = reinterpret_cast<char*>(a.state_words);
+  BeamState bs{};
+  bs.ids = reinterpret_cast<int64_t*>(w); w += sizeof(int64_t) * rows;
+  bs.logprob = reinterpret_cast<float*>(w); w += sizeof(float) * rows;
+  bs.finished = reinterpret_cast<int32_t*>(w); w += sizeof(int32_t) * rows;
+  bs.length = reinterpret_cast<int32_t*>(w); w += sizeof(int32_t) * rows;
+  bs.time = reinterpret_cast<int32_t*>(w); w += sizeof(int32_t);
+  bs.all_finished = reinterpret_cast<int32_t*>(w); w += sizeof(int32_t);
+  bs.ticket = reinterpret_cast<uint32_t*>(w); w += 2 * sizeof(int32_t);
+  bs.anc = reinterpret_cast<int32_t*>(w); w += sizeof(int32_t) * (size_t)rows * st.max_len;
+  bs.hist = reinterpret_cast<int32_t*>(w);
+  const DecodeLayout lo = layout_of(cf, rows);
+  float* logits = rs.scratch + lo.logits;
+  beam_init_kernel<<<1, 32, 0, s>>>(bs, a.bos_ids, rows, beam);
+  B200ST_CUDA(cudaGetLastError());
+  StepCtx c{m, buf, rs, s};
+  auto one_step = [&]() -> int {
+    B200ST_TRY(step_dispatch(c, bs.ids, bs.time, logits, bs.anc, beam));
+    launch_pdl(beam_select_kernel, st.B, 1024, 0, s, (const float*)logits, bs, beam, cf.vocab, a.eos_id, a.unk_id, a.min_len,
+               a.length_penalty, st.max_len);
+    ++g_kernel_launches;
+    B200ST_LAUNCH_CHECK();
+    return 0;
+  };
+  bool graphed = false;
+  B200ST_TRY(run_token_loop(s, a.max_steps, a.use_graph != 0, bs.all_finished, one_step, &graphed));
+  B200ST_CHECK(graphed || !a.use_graph, "beam search could not capture its step into a CUDA graph");
+  beam_extract_kernel<<<st.B, 256, 0, s>>>(bs, beam, a.top_k, a.length_penalty, a.eos_id, st.max_len, a.max_steps, a.out_ids,
+                                           a.out_scores, a.out_logprob, a.out_len);
+  ++g_kernel_launches;
+  B200ST_CUDA(cudaGetLastError());
+  return 0;
 }
 
 }  // namespace b200st

@@ -138,5 +138,21 @@ int decode_step(const Model& m, const Buffers& buf, const DecodeState& st, const
                 float* logits, cudaStream_t s);
 int last_greedy_used_graph();      // 1 / 0 for the last greedy_search of this process (-1: none yet)
 int greedy_search(const Model& m, const Buffers& buf, const DecodeState& st, const GreedyArgs& ga, cudaStream_t s);
+struct BeamArgs {
+  const int64_t* bos_ids;        // [B] device, one per utterance
+  int eos_id, unk_id;            // unk_id < 0: UNK allowed
+  int min_len, max_steps;
+  int beam_size, top_k;
+  float length_penalty;          // alpha; < 0: 1 / length
+  int64_t* out_ids;              // [B * top_k, max_steps] device, padded with EOS
+  float* out_scores;             // [B * top_k] logprob * length penalty, best first per utterance
+  float* out_logprob;            // [B * top_k]
+  int32_t* out_len;              // [B * top_k]
+  void* state_words;             // >= beam_state_bytes(B, beam_size, max_len)
+  int use_graph;
+};
+int64_t beam_state_bytes(int B, int beam, int max_len);
+// st.B counts utterances; self_kv and scratch are sized for B * beam_size rows, cross_kv / memory_bias for B
+int beam_search(const Model& m, const Buffers& buf, const DecodeState& st, const BeamArgs& a, cudaStream_t s);
 
 }  // namespace b200st

@@ -3,10 +3,11 @@
 Host mirror of
   EncoderDecoderModel.get_symbols_to_logits_fn      neurst/models/encoder_decoder_model.py:211-261
   TransformerDecoder.create_decoding_internal_cache neurst/layers/decoders/transformer_decoder.py:105-147
-  sequence_beam_search (beam_size = 1)              neurst/layers/search/beam_search.py:254-439
+  sequence_beam_search                              neurst/layers/search/beam_search.py:254-439
   SequenceGenerator                                 neurst/exps/sequence_generator.py:62-86
 
-Everything numeric is a library call (b200st_encode / b200st_decode_init / b200st_decode_step / b200st_greedy_search):
+Everything numeric is a library call (b200st_encode / b200st_decode_init / b200st_decode_step / b200st_greedy_search /
+b200st_beam_search):
 the key/value caches are preallocated device buffers owned by `DecodingCache`, the token ids and the position live on the
 device, and the greedy loop replays one captured CUDA graph per token inside the library.
 """
@@ -20,18 +21,22 @@ MAX_ROWS = 8      # rows (batch x beam) per decoding step supported by the decod
 
 
 class DecodingCache:
-    """`cache` argument of symbols_to_logits_fn: encoder memory (pre-projected per layer) + self-attention K/V."""
+    """`cache` argument of symbols_to_logits_fn: encoder memory (pre-projected per layer) + self-attention K/V.
 
-    def __init__(self, rt, B, Tm, max_len, memory_bias, use_shadow=False):
+    beam > 1 (beam search): the memory stays one copy per utterance, the self-attention cache and the step scratch hold
+    B * beam rows."""
+
+    def __init__(self, rt, B, Tm, max_len, memory_bias, use_shadow=False, beam=1):
         cfg = rt.config
-        if not 1 <= B <= MAX_ROWS:
-            raise L.B200STError("decoding supports 1..%d rows per step, got %d" % (MAX_ROWS, B))
+        if beam < 1 or not 1 <= B * beam <= MAX_ROWS:
+            raise L.B200STError("decoding supports 1..%d rows (utterances x beam) per step, got %d x %d" % (MAX_ROWS, B, beam))
         dev = rt.device
-        self.rt, self.B, self.Tm, self.max_len = rt, B, Tm, max_len
+        self.rt, self.B, self.Tm, self.max_len, self.beam = rt, B, Tm, max_len, beam
+        rows = B * beam
         self.cross_kv = torch.zeros(cfg.dec_layers, B, max(Tm, 1), 2 * cfg.d, dtype=torch.float32, device=dev)
-        self.self_kv = torch.zeros(cfg.dec_layers, 2, B, max_len, cfg.d, dtype=torch.float32, device=dev)
+        self.self_kv = torch.zeros(cfg.dec_layers, 2, rows, max_len, cfg.d, dtype=torch.float32, device=dev)
         self.memory_bias = memory_bias
-        n = int(rt.lib.b200st_decode_scratch_floats(rt.handle, B))
+        n = int(rt.lib.b200st_decode_scratch_floats(rt.handle, rows))
         self.scratch = torch.zeros(n, dtype=torch.float32, device=dev)
         self.time = torch.zeros(1, dtype=torch.int32, device=dev)
         st = L.DecodeState()
@@ -47,9 +52,10 @@ class DecodingCache:
         d, H = self.rt.config.d, self.rt.config.heads
         out = {}
         for i in range(self.rt.config.dec_layers):
+            rows = self.self_kv.shape[2]
             out["layer_%d" % i] = {
-                "self_attention": {"keys": self.self_kv[i, 0, :, :upto].reshape(self.B, upto, H, d // H),
-                                   "values": self.self_kv[i, 1, :, :upto].reshape(self.B, upto, H, d // H)},
+                "self_attention": {"keys": self.self_kv[i, 0, :, :upto].reshape(rows, upto, H, d // H),
+                                   "values": self.self_kv[i, 1, :, :upto].reshape(rows, upto, H, d // H)},
                 "memory": {"keys": self.cross_kv[i, :, :, :d], "values": self.cross_kv[i, :, :, d:]}}
         return out
 
@@ -92,10 +98,10 @@ def encode(rt, inputs):
     return enc, bias
 
 
-def create_decoding_cache(rt, encoder_outputs, memory_bias, max_len, use_shadow=False):
+def create_decoding_cache(rt, encoder_outputs, memory_bias, max_len, use_shadow=False, beam=1):
     """create_decoding_internal_cache(is_inference=True) + memorize_memory for every layer."""
     B, Tm, _ = encoder_outputs.shape
-    cache = DecodingCache(rt, B, Tm, max_len, memory_bias.contiguous() if memory_bias is not None else None, use_shadow)
+    cache = DecodingCache(rt, B, Tm, max_len, memory_bias.contiguous() if memory_bias is not None else None, use_shadow, beam)
     bufs = _bufs(rt)
     enc = encoder_outputs.to(torch.float32).contiguous()
     L.check(rt.lib.b200st_decode_init(rt.handle, C.byref(bufs), enc.data_ptr(), C.byref(cache.state), L._stream()))
@@ -159,3 +165,72 @@ def greedy_search(rt, inputs, bos_id, eos_id, unk_id=None, maximum_decode_length
     if steps < maximum_decode_length:      # padded to the fixed output length with EOS (beam_search.py:428-436)
         out = torch.cat([out, torch.full((B, maximum_decode_length - steps), int(eos_id), dtype=torch.int64, device=dev)], 1)
     return out, logprob, length
+
+
+def _search_steps(Tm, maximum_decode_length, extra_decode_length, minimum_decode_length):
+    """maximum_search_steps = max(min(T' + extra, maximum), minimum) (beam_search.py:366-372)."""
+    return max(min(Tm + extra_decode_length, maximum_decode_length), minimum_decode_length)
+
+
+def beam_search(rt, inputs, bos_id, eos_id, unk_id=None, beam_size=4, length_penalty=0.6, top_k=1, maximum_decode_length=256,
+                extra_decode_length=50, minimum_decode_length=0, enable_unk=False, use_shadow=False, use_graph=True, cache=None):
+    """sequence_beam_search (beam_search.py:254-439) on the device: returns (hypotheses int64 [B*top_k, maximum_decode_length]
+    padded with EOS, scores fp32 [B*top_k] = logprob * length penalty, best first per utterance, accumulated log-probabilities
+    [B*top_k], decoding lengths [B*top_k]).  length_penalty < 0 (or None) scores by 1/length.  At most MAX_ROWS // beam_size
+    utterances per call.  beam_size 1 is the greedy search (with its persistent kernel when use_graph)."""
+    beam_size, top_k = int(beam_size), int(top_k)
+    if beam_size < 1:
+        raise L.B200STError("beam_size must be >= 1, got %d" % beam_size)
+    if not 1 <= top_k <= beam_size:
+        raise L.B200STError("top_k must be in 1..beam_size (%d), got %d" % (beam_size, top_k))
+    if minimum_decode_length >= maximum_decode_length:          # BeamSearch.call (beam_search.py:531-532)
+        raise L.B200STError("minimum_decode_length must be less than maximum_decode_length")
+    alpha = -1.0 if length_penalty is None else float(length_penalty)
+    if cache is None:
+        B = int(inputs["src"].shape[0])
+        if B * beam_size > MAX_ROWS:
+            raise L.B200STError("beam search decodes at most %d rows (utterances x beam_size) per call, got %d x %d"
+                                % (MAX_ROWS, B, beam_size))
+        enc, bias = encode(rt, inputs)
+        cache = create_decoding_cache(rt, enc, bias, maximum_decode_length, use_shadow, beam=beam_size)
+    elif cache.self_kv.shape[2] < cache.B * beam_size:
+        raise L.B200STError("the decoding cache holds %d rows, beam search needs %d" % (cache.self_kv.shape[2], cache.B * beam_size))
+    B, Tm = cache.B, cache.Tm
+    steps = _search_steps(Tm, maximum_decode_length, extra_decode_length, minimum_decode_length)
+    dev = rt.device
+    bos = torch.as_tensor(bos_id).to(device=dev, dtype=torch.int64).reshape(-1)
+    if bos.numel() == 1:
+        bos = bos.repeat(B)
+    bos = bos.contiguous()
+    n = B * top_k
+    out = torch.empty(n, max(steps, 1), dtype=torch.int64, device=dev)
+    scores = torch.zeros(n, dtype=torch.float32, device=dev)
+    logprob = torch.zeros(n, dtype=torch.float32, device=dev)
+    length = torch.zeros(n, dtype=torch.int32, device=dev)
+    nbytes = int(rt.lib.b200st_beam_state_bytes(rt.handle, B, beam_size, cache.max_len))
+    if nbytes <= 0:
+        raise L.B200STError("beam search state sizing failed: " + rt.lib.b200st_last_error().decode())
+    words = torch.zeros((nbytes + 7) // 8, dtype=torch.int64, device=dev)
+    a = L.BeamArgs()
+    a.bos_ids, a.eos_id = bos.data_ptr(), int(eos_id)
+    a.unk_id = -1 if (enable_unk or unk_id is None) else int(unk_id)
+    a.min_len, a.max_steps = int(minimum_decode_length), int(steps)     # the library refuses steps beyond the cache
+    a.beam_size, a.top_k, a.length_penalty = beam_size, top_k, alpha
+    a.out_ids, a.out_scores, a.out_logprob, a.out_len = out.data_ptr(), scores.data_ptr(), logprob.data_ptr(), length.data_ptr()
+    a.state_words = words.data_ptr()
+    a.use_graph = (2 if beam_size == 1 else 1) if use_graph else 0
+    bufs = _bufs(rt)
+    cur = torch.cuda.current_stream(dev)
+    side = getattr(rt, "_decode_stream", None)
+    if side is None:
+        side = rt._decode_stream = torch.cuda.Stream(device=dev)
+    side.wait_stream(cur)
+    with torch.cuda.stream(side):
+        L.check(rt.lib.b200st_beam_search(rt.handle, C.byref(bufs), C.byref(cache.state), C.byref(a), L._stream()))
+    cur.wait_stream(side)
+    if beam_size == 1 and use_graph and int(rt.lib.b200st_greedy_used_graph()) < 1:
+        raise L.B200STError("greedy search could neither run its persistent kernel nor capture its step graph")
+    out = out[:, :steps]
+    if steps < maximum_decode_length:      # padded to the fixed output length with EOS (beam_search.py:428-436)
+        out = torch.cat([out, torch.full((n, maximum_decode_length - steps), int(eos_id), dtype=torch.int64, device=dev)], 1)
+    return out, scores, logprob, length

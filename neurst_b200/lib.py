@@ -10,7 +10,7 @@ _LIB_PATH = os.path.join(_HERE, "libb200st.so")
 _lib = None
 
 F32, BF16, F16 = 0, 1, 2
-ABI_VERSION = 201    # must equal b200st_version(): bumped whenever a struct in include/b200st.h changes layout
+ABI_VERSION = 202    # must equal b200st_version(): bumped whenever a struct in include/b200st.h changes layout
 
 
 class B200STError(RuntimeError):
@@ -204,6 +204,13 @@ class GreedyArgs(C.Structure):
                 ("state_words", C.c_void_p), ("use_graph", C.c_int32)]
 
 
+class BeamArgs(C.Structure):
+    _fields_ = [("bos_ids", C.c_void_p), ("eos_id", C.c_int32), ("unk_id", C.c_int32), ("min_len", C.c_int32),
+                ("max_steps", C.c_int32), ("beam_size", C.c_int32), ("top_k", C.c_int32), ("length_penalty", C.c_float),
+                ("out_ids", C.c_void_p), ("out_scores", C.c_void_p), ("out_logprob", C.c_void_p), ("out_len", C.c_void_p),
+                ("state_words", C.c_void_p), ("use_graph", C.c_int32)]
+
+
 # every symbol include/b200st.h declares (tests/test_abi.py checks the .so exports all of them)
 EXPORTS = [
     "b200st_last_error", "b200st_version", "b200st_launch_count", "b200st_gemm", "b200st_gemm_bench", "b200st_debug_tc", "b200st_profile_begin", "b200st_profile_end",
@@ -211,7 +218,7 @@ EXPORTS = [
     "b200st_workspace_bytes", "b200st_forward", "b200st_forward_backward", "b200st_refresh_shadow", "b200st_adam_step", "b200st_optimizer_step",
     "b200st_comm_unique_id", "b200st_comm_init", "b200st_comm_broadcast", "b200st_comm_destroy", "b200st_comm_stats", "b200st_train_step",
     "b200st_encode", "b200st_encode_workspace_bytes", "b200st_decode_scratch_floats", "b200st_decode_init", "b200st_decode_step",
-    "b200st_greedy_search", "b200st_greedy_used_graph",
+    "b200st_greedy_search", "b200st_greedy_used_graph", "b200st_beam_state_bytes", "b200st_beam_search",
     "b200st_encoder_forward", "b200st_decoder_forward", "b200st_mha_forward", "b200st_lsce", "b200st_layernorm_fwd",
     "b200st_layernorm_bwd", "b200st_softmax_fwd", "b200st_conv1_ln_relu_fwd", "b200st_dropout_stream_id", "b200st_dropout_mask",
 ]
@@ -249,6 +256,9 @@ def _declare(lib):
                                        C.c_void_p, C.c_void_p]
     lib.b200st_greedy_search.argtypes = [C.c_void_p, C.POINTER(Buffers), C.POINTER(DecodeState), C.POINTER(GreedyArgs),
                                          C.c_void_p]
+    lib.b200st_beam_state_bytes.restype = C.c_int64
+    lib.b200st_beam_state_bytes.argtypes = [C.c_void_p, C.c_int32, C.c_int32, C.c_int32]
+    lib.b200st_beam_search.argtypes = [C.c_void_p, C.POINTER(Buffers), C.POINTER(DecodeState), C.POINTER(BeamArgs), C.c_void_p]
     lib.b200st_adam_step.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64, C.c_float,
                                      C.c_float, C.c_float, C.c_float, C.c_int64, C.c_float, C.c_int32, C.c_void_p]
     lib.b200st_encoder_forward.argtypes = [C.c_void_p, C.POINTER(Buffers), C.c_void_p, C.c_void_p, C.c_int32, C.c_int32,

@@ -211,6 +211,21 @@ class _EncoderDecoder:
                                           extra_decode_length, minimum_decode_length, enable_unk, use_shadow)
         return ids, logprob
 
+    def beam_search(self, inputs, beam_size=4, length_penalty=0.6, top_k=1, maximum_decode_length=256, extra_decode_length=50,
+                    minimum_decode_length=0, enable_unk=False, use_shadow=False):
+        """SequenceGenerator with search_method BeamSearch (neurst/layers/search/beam_search.py:439-530) on the device:
+        -> (hypotheses [B*top_k, maximum_decode_length], scores [B*top_k]), BeamSearch.call's return.  At most
+        decode.MAX_ROWS // beam_size utterances per call."""
+        from neurst_b200 import decode as D
+        tm = self._trg_meta
+        B = inputs["src"].shape[0]
+        bos = inputs.get("trg_input")
+        if bos is None:
+            bos = torch.full((B,), int(tm["bos_id"]), dtype=torch.long)
+        ids, scores, _, _ = D.beam_search(self._rt, inputs, bos, tm["eos_id"], tm.get("unk_id"), beam_size, length_penalty, top_k,
+                                          maximum_decode_length, extra_decode_length, minimum_decode_length, enable_unk, use_shadow)
+        return ids, scores
+
     def evaluate(self, inputs, is_training=False):
         """logits + criterion outputs (nll_sum [B], n_tokens [B], loss) in one call."""
         return self._rt.run(self._batch(inputs, is_training, want_logits=True), backward=False)
