@@ -285,9 +285,6 @@ int b200st_gemm_bench(const b200st_gemm_args* args, int32_t iters, float* ms_per
 int b200st_profile_begin(void);
 int b200st_profile_end(double* gemm_ms, double* gemm_flops, int64_t* gemm_launches);
 
-/* tests / tools only: override the GEMM tile configuration (0 = default): N tile, ring depth (>= 2), CTA count */
-int b200st_debug_tc(int32_t force_bn, int32_t force_stages, int32_t max_ctas);
-
 #ifdef __cplusplus
 }
 #endif

@@ -536,7 +536,6 @@ constexpr size_t kFwdSmemFixed = 1024 + (size_t)(1 + 2 + 1) * kTile16K + 8 * 7 +
 int attention_fwd_fused(int dt, const void* q, int64_t q_ld, const void* k, int64_t k_ld, const void* v, int64_t v_ld, int B, int H,
                         int Tq, int Tk, const float* bias, int causal, DropoutSpec drop, void* ctx, int64_t ctx_ld, float* lse,
                         cudaStream_t s, const int32_t* kv_len) {
-  if (ablate_mask() & ABL_ATTN_FWD) return 0;
   B200ST_CHECK(Tq > 0 && Tk > 0 && B > 0 && H > 0, "empty attention");
   B200ST_CHECK(B <= 65535 && H <= 65535, "attention grid too large");
   B200ST_CHECK(is16(dt), "fused attention needs a 16-bit operand type");
@@ -573,7 +572,6 @@ int attention_bwd_fused(int dt, const void* q, int64_t q_ld, const void* k, int6
                         int64_t ctx_ld, const void* dctx, int64_t dctx_ld, const float* lse, int B, int H, int Tq, int Tk,
                         const float* bias, int causal, DropoutSpec drop, float* dq_scratch, void* dq, int64_t dq_ld, void* dk,
                         int64_t dk_ld, void* dv, int64_t dv_ld, cudaStream_t s, const int32_t* kv_len) {
-  if (ablate_mask() & ABL_ATTN_BWD) return 0;
   B200ST_CHECK(Tq > 0 && Tk > 0 && B > 0 && H > 0 && B <= 65535 && H <= 65535, "bad attention shape");
   B200ST_CHECK(is16(dt), "fused attention needs a 16-bit operand type");
   CUtensorMap tq, tk, tv, tdo;

@@ -14,6 +14,8 @@ static thread_local std::string g_last_error;
 void set_last_error(const std::string& s) { g_last_error = s; }
 int64_t g_kernel_launches = 0;
 cudaError_t& pdl_launch_error() { static thread_local cudaError_t e = cudaSuccess; return e; }
+// B200ST_NO_PDL only drops the launch attribute (every kernel computes the same thing), so that torch.profiler kernel
+// times do not include the griddepcontrol.wait of a kernel launched early under its predecessor
 bool pdl_enabled() { static const bool on = getenv("B200ST_NO_PDL") == nullptr; return on; }
 }  // namespace b200st
 
@@ -85,12 +87,6 @@ static int convert_gemm(const b200st_gemm_args* a, GemmArgs& g) {
 int b200st_profile_begin(void) { tc_profile_begin(); return 0; }
 int b200st_profile_end(double* gemm_ms, double* gemm_flops, int64_t* gemm_launches) {
   return tc_profile_end(gemm_ms, gemm_flops, gemm_launches);
-}
-
-int b200st_debug_tc(int32_t force_bn, int32_t force_stages, int32_t max_ctas) {
-  TcDebug& d = tc_debug();
-  d.force_bn = force_bn; d.force_stages = force_stages; d.max_ctas = max_ctas;
-  return 0;
 }
 
 

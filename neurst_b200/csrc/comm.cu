@@ -69,6 +69,10 @@ struct NcclConfig227 {
   int collnetEnable, CTAPolicy, shrinkShare, nvlsCTAs;
 };
 
+// The all-reduces run UNDER the backward kernels: cap the SMs NCCL may take (its kernels hold an SM for the whole
+// transfer, and the persistent GEMM grids are sized to the SMs that are left, see comm_reserved_sms)
+constexpr int kNcclMaxCtas = 8;
+
 struct GradSync {
   ncclComm_t comm = nullptr;
   int nranks = 1, rank = 0;
@@ -94,22 +98,16 @@ int comm_init(GradSync** out, const char* id128, int nranks, int rank) {
   g->nranks = nranks; g->rank = rank;
   ncclUniqueId id;
   std::memcpy(id.internal, id128, 128);
-  // The all-reduces run UNDER the backward kernels: cap the SMs NCCL may take (its kernels hold an SM for the whole
-  // transfer, and the persistent GEMM grids are sized to the SMs that are left, see comm_reserved_sms)
-  const char* env = getenv("B200ST_NCCL_MAX_CTAS");
-  g->max_ctas = env ? atoi(env) : 8;
   ncclResult_t r = 1;
-  if (g->max_ctas > 0 && nccl().CommInitRankConfig) {
+  if (nccl().CommInitRankConfig) {
     NcclConfig227 cfg;
     const int undef = (int)0x80000000;
     cfg.size = sizeof(NcclConfig227); cfg.magic = 0xcafebeefu; cfg.version = 22703u;
-    cfg.blocking = undef; cfg.cgaClusterSize = undef; cfg.minCTAs = undef; cfg.maxCTAs = g->max_ctas;
+    cfg.blocking = undef; cfg.cgaClusterSize = undef; cfg.minCTAs = undef; cfg.maxCTAs = kNcclMaxCtas;
     cfg.netName = nullptr; cfg.splitShare = undef; cfg.trafficClass = undef; cfg.commName = nullptr;
     cfg.collnetEnable = undef; cfg.CTAPolicy = undef; cfg.shrinkShare = undef; cfg.nvlsCTAs = undef;
     r = nccl().CommInitRankConfig(&g->comm, nranks, id, rank, &cfg);
-    if (r != 0) g->max_ctas = 0;
-  } else {
-    g->max_ctas = 0;
+    if (r == 0) g->max_ctas = kNcclMaxCtas;
   }
   if (r != 0) r = nccl().CommInitRank(&g->comm, nranks, id, rank);
   if (r != 0) { delete g; B200ST_FAIL(std::string("ncclCommInitRank: ") + nccl().GetErrorString(r)); }

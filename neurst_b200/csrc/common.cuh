@@ -98,7 +98,7 @@ __device__ __forceinline__ float warp_max(float v) {
 
 // ---- counter-based RNG for dropout: Philox4x32-7 ---------------------------------------
 // (7 rounds: the smallest round count of Philox4x32 that Salmon et al. report as passing BigCrush; the generator of all
-// keep-bits of a step is integer-ALU bound, so fewer rounds are directly fewer instructions; tools/ablate_step.py isolates its cost)
+// keep-bits of a step is integer-ALU bound, so fewer rounds are directly fewer instructions)
 // One call yields 4 x 32 random bits for counter (idx4, stream) under key (seed).  Dropout at element
 // index e uses call (e >> 2) and lane (e & 3), so forward and backward regenerate identical masks.
 struct Philox4 { uint32_t x, y, z, w; };
@@ -161,14 +161,5 @@ __device__ __forceinline__ bool drop_keep1(const DropoutSpec& d, uint64_t e) {
 }
 
 static inline int ceil_div(int64_t a, int64_t b) { return (int)((a + b - 1) / b); }
-
-// Measurement aid (tools/ablate_step.py): B200ST_ABLATE is a bit mask of kernel classes whose launches are SKIPPED, to
-// read each class's contribution to the step off the critical path (results are garbage while it is set).
-enum : int { ABL_COLSUM = 1, ABL_WGRAD = 2, ABL_LN_FWD = 4, ABL_LN_BWD = 8, ABL_ATTN_FWD = 16, ABL_ATTN_BWD = 32, ABL_MLP_FWD = 64,
-              ABL_MLP_BWD = 128, ABL_GEMM = 256, ABL_OPTIM = 512, ABL_DROPBITS = 1024, ABL_CONV = 2048 };
-inline int ablate_mask() {
-  const char* e = getenv("B200ST_ABLATE");
-  return e ? atoi(e) : 0;
-}
 
 }  // namespace b200st

@@ -736,7 +736,6 @@ int conv1_ln_relu_fwd(const float* src, const float* w, const float* b, const fl
 // normalised-save forward: xhat = LN-normalised conv1 output (no gamma/beta/ReLU) + 1/sigma per position
 int conv1_norm_fwd(const float* src, const float* w, const float* b, float eps, void* xhat, int dtype, float* rstd, int B, int T,
                    int F, int Cin, int C, cudaStream_t s) {
-  if (ablate_mask() & ABL_CONV) return 0;
   B200ST_CHECK(rstd != nullptr, "conv1_norm_fwd needs the rstd buffer");
   return conv1_fwd_launch(src, w, b, nullptr, nullptr, eps, xhat, dtype, B, T, F, Cin, C, 0, rstd, s);
 }
@@ -804,7 +803,6 @@ int conv1_bwd_fused(const float* src, const float* w, const float* b, const floa
 int conv1_bwd_from_xhat(const float* src, const void* gamma, const void* beta, const void* xhat, const float* rstd,
                         const void* dcol, int dtype, void* dz1, void* col1, int K1p, float* db, float* dgamma, float* dbeta, int B,
                         int T, int F, int C, cudaStream_t s, int implicit_tiles) {
-  if (ablate_mask() & ABL_CONV) return 0;
   B200ST_CHECK(C == 256 && K1p >= 9 && K1p <= 32, "conv1_bwd_from_xhat supports C == 256, Cin == 1");
   B200ST_CHECK(((reinterpret_cast<uintptr_t>(xhat) | reinterpret_cast<uintptr_t>(dcol) | reinterpret_cast<uintptr_t>(dz1) |
                  reinterpret_cast<uintptr_t>(gamma) | reinterpret_cast<uintptr_t>(beta)) & 15) == 0, "conv1 backward buffers must be 16-byte aligned");
@@ -835,7 +833,7 @@ int im2col_3x3s2_affine(const void* y1, void* col, int dtype, int B, int T1, int
                         cudaStream_t s) {
   const int T2 = (T1 + 1) / 2, F2 = (F1 + 1) / 2;
   const int64_t nchunks = (int64_t)B * T2 * F2 * 9;
-  if (nchunks == 0 || (ablate_mask() & ABL_CONV)) return 0;
+  if (nchunks == 0) return 0;
   const int grid = pick_grid(nchunks, 8 * 8, 132 * 16);
   const int esz = dtype_size(dtype);
   const bool vec = ((C * esz) % 16 == 0) && ((reinterpret_cast<uintptr_t>(y1) & 15) == 0) && ((reinterpret_cast<uintptr_t>(col) & 15) == 0) &&

@@ -153,7 +153,7 @@ int layernorm_fwd(const void* x, int x_dtype, const float* gamma, const float* b
 // + xcopy (optional): fp32 copy of the input rows, written in the same pass
 int layernorm_fwd_copy(const void* x, int x_dtype, const float* gamma, const float* beta, float eps, void* y, int y_dtype,
                        float* y32, float* mean, float* rstd, int64_t rows, int cols, int relu, float* xcopy, cudaStream_t s) {
-  if (rows == 0 || (ablate_mask() & ABL_LN_FWD)) return 0;
+  if (rows == 0) return 0;
   const int grid = grid_for(rows, 8 * 2);
   const bool vec = (cols % 4 == 0) && cols <= 1024 && ((reinterpret_cast<uintptr_t>(x) & 15) == 0) &&
                    ((reinterpret_cast<uintptr_t>(y) & 15) == 0) && ((reinterpret_cast<uintptr_t>(gamma) & 15) == 0) &&
@@ -375,7 +375,7 @@ int layernorm_bwd_next(const void* dy, int dy_dtype, const void* x, int x_dtype,
                        const float* gamma, const float* beta, const float* dres, void* dx, int dx_dtype, float* dgamma,
                        float* dbeta, int64_t rows, int cols, int relu, void* dnext, int dnext_dtype, DropoutSpec ndrop,
                        cudaStream_t s) {
-  if (rows == 0 || (ablate_mask() & ABL_LN_BWD)) return 0;
+  if (rows == 0) return 0;
   B200ST_CHECK(cols <= 1024, "layernorm_bwd supports cols <= 1024");
   const int grid = grid_for(rows, 8 * 2, 132 * 8);      // 2 rows in flight per warp; long inputs loop
   const size_t smem = 2 * (size_t)cols * sizeof(float);
@@ -677,7 +677,7 @@ __global__ void colsum_kernel(const T* __restrict__ dY, int64_t M, int N, int64_
   }
 }
 int colsum_accum(const void* dY, int dtype, int64_t M, int N, int64_t ld, float* db, cudaStream_t s) {
-  if (M == 0 || N == 0 || (ablate_mask() & ABL_COLSUM)) return 0;
+  if (M == 0 || N == 0) return 0;
   const int esz = dtype_size(dtype);
   const bool vec = (N % 8 == 0) && ((ld * esz) % (8 * esz) == 0) && ((reinterpret_cast<uintptr_t>(dY) & (8 * esz - 1)) == 0);
   if (vec) {
@@ -1051,7 +1051,7 @@ __global__ void __launch_bounds__(256) dropout_bits_multi_kernel(const DropBitsT
   }
 }
 int dropout_bits_multi(const DropBitsTable& t, uint64_t seed, const uint64_t* seed_ptr, uint8_t* base, cudaStream_t s) {
-  if (t.n == 0 || t.goff[t.n] == 0 || (ablate_mask() & ABL_DROPBITS)) return 0;
+  if (t.n == 0 || t.goff[t.n] == 0) return 0;
   launch_pdl(dropout_bits_multi_kernel, grid_for((t.goff[t.n] + 3) / 4, 256, 132 * 8), 256, 0, s, t, seed, seed_ptr, base);
   ++g_kernel_launches;
   B200ST_LAUNCH_CHECK();

@@ -85,14 +85,9 @@ int fused_mlp_fwd(const void* X, int dtype, int M, int d, int ffn, const void* W
 int fused_mlp_bwd(const void* dY, int dtype, int M, int d, int ffn, const void* W1, const void* W2, const void* F1, float scale,
                   void* dF1, float* dH, cudaStream_t stream, int* tickets = nullptr);
 
-// Tile-configuration overrides (tests / tools only). 0 restores defaults.
-struct TcDebug {
-  int force_bn;     // 0 = auto
-  int force_stages; // 0 = auto; at least 2 (one slot stays in flight while the next is issued)
-  int max_ctas;     // 0 = #SMs
-  int reserve_sms;    // SMs left to concurrent communication kernels (set by the model while gradient all-reduces overlap)
-};
-TcDebug& tc_debug();
+// SMs left to concurrent communication kernels: the persistent GEMM and fused-FFN grids are sized to the rest of the
+// device.  The model sets it while gradient all-reduces overlap the backward pass; 0 = none.
+void set_reserved_sms(int n);
 int64_t tc_launch_count();
 void tc_count_launch();
 void tc_profile_begin();

@@ -172,7 +172,7 @@ int cast_f32_to_16(const float* x, void* y, int y_dtype, int64_t n, cudaStream_t
 }
 
 int optimizer_step(const OptimArgs& a, const TensorTable& tt, cudaStream_t s) {
-  if (a.n == 0 || (ablate_mask() & ABL_OPTIM)) return 0;
+  if (a.n == 0) return 0;
   B200ST_CHECK(((reinterpret_cast<uintptr_t>(a.p) | reinterpret_cast<uintptr_t>(a.g) | reinterpret_cast<uintptr_t>(a.m) |
                  reinterpret_cast<uintptr_t>(a.v)) & 15) == 0 && (reinterpret_cast<uintptr_t>(a.shadow) & 7) == 0,
                "optimizer: arenas must be 16-byte aligned");

@@ -694,7 +694,19 @@ int make_operand_map(const GemmOperand& op, int rows, int K, int nb1, int nb2, i
 }
 
 int g_num_sms = 0;
+int g_reserved_sms = 0;
 int64_t g_launches = 0;
+
+// SMs a persistent grid may fill: the device's, less those reserved for communication kernels (set_reserved_sms)
+int usable_sms(int* out) {
+  if (g_num_sms == 0) {
+    int dev = 0;
+    B200ST_CUDA(cudaGetDevice(&dev));
+    B200ST_CUDA(cudaDeviceGetAttribute(&g_num_sms, cudaDevAttrMultiProcessorCount, dev));
+  }
+  *out = g_reserved_sms > 0 && g_reserved_sms < g_num_sms ? g_num_sms - g_reserved_sms : g_num_sms;
+  return 0;
+}
 }  // namespace
 
 // 16-bit 4-D tensor map (inner, rows, nb1, nb2) with a {box_inner<=64, box_rows} box, 128B swizzle.
@@ -751,10 +763,7 @@ int launch_bn(bool a_mn, bool b_mn, bool bf, const CUtensorMap& ta, const CUtens
 
 }  // namespace
 
-TcDebug& tc_debug() {
-  static TcDebug d{};
-  return d;
-}
+void set_reserved_sms(int n) { g_reserved_sms = n; }
 int64_t tc_launch_count() { return g_launches; }
 
 namespace {
@@ -768,17 +777,8 @@ int gemm_tc_impl(const GemmArgs& g, cudaStream_t stream, const ConvA* conv) {
   // wgmma has no mixed bf16 x fp16 form: the library refuses mixed products up front
   B200ST_CHECK(g.A.dtype == g.B.dtype, "wgmma needs A and B in the same 16-bit format (both bf16 or both fp16)");
   B200ST_CHECK(g.M > 0 && g.N > 0 && g.K > 0 && g.nb1 > 0 && g.nb2 > 0, "empty GEMM");
-  if (const int abl = ablate_mask()) {
-    const bool wgrad = g.A.mn_major && g.B.mn_major;
-    if ((wgrad && (abl & ABL_WGRAD)) || (!wgrad && (abl & ABL_GEMM))) return 0;
-  }
-  if (g_num_sms == 0) {
-    int dev = 0;
-    B200ST_CUDA(cudaGetDevice(&dev));
-    B200ST_CUDA(cudaDeviceGetAttribute(&g_num_sms, cudaDevAttrMultiProcessorCount, dev));
-  }
-  const TcDebug& dbg = tc_debug();
-  const int num_sms = dbg.max_ctas > 0 ? dbg.max_ctas : (dbg.reserve_sms > 0 && dbg.reserve_sms < g_num_sms ? g_num_sms - dbg.reserve_sms : g_num_sms);
+  int num_sms = 0;
+  B200ST_TRY(usable_sms(&num_sms));
 
   TcParams p{};
   p.M = g.M; p.N = g.N; p.K = g.K; p.nb1 = g.nb1; p.nb2 = g.nb2;
@@ -794,15 +794,14 @@ int gemm_tc_impl(const GemmArgs& g, cudaStream_t stream, const ConvA* conv) {
   const bool linear_epi = !g.epi.relu && !g.epi.mask_src && g.epi.drop.p == 0.f && !g.epi.residual && !g.epi.bias;
   const bool split_ok = linear_epi && g.c_dtype == F32 && g.epi.accumulate;
   if (g.splitk > 1) B200ST_CHECK(split_ok, "split-K needs a linear fp32 accumulate epilogue");
-  int bn = dbg.force_bn, splitk = g.splitk >= 1 ? g.splitk : 1;
+  int bn = 0, splitk = g.splitk >= 1 ? g.splitk : 1;
   {
     double best = 1e30;
     int best_bn = 0, best_sk = 1;
     const int cands[3] = {256, 128, 64};
     for (int c : cands) {
-      if (dbg.force_bn && c != dbg.force_bn) continue;
       if (conv && c != 256) continue;
-      if (!dbg.force_bn && c > 64 && c >= 2 * ((g.N + 63) / 64 * 64)) continue;   // do not pad N by 2x or more
+      if (c > 64 && c >= 2 * ((g.N + 63) / 64 * 64)) continue;   // do not pad N by 2x or more
       const int64_t tiles0 = batch * p.m_tiles * ceil_div(g.N, c);
       int sk_lo = splitk, sk_hi = splitk;
       if (g.splitk == 0 && split_ok) {
@@ -835,7 +834,7 @@ int gemm_tc_impl(const GemmArgs& g, cudaStream_t stream, const ConvA* conv) {
   p.num_tiles = batch * p.m_tiles * p.n_tiles * splitk;
 
   const uint32_t stage_bytes = kABytes + (uint32_t)bn * BK * 2;
-  int stages = dbg.force_stages > 0 ? dbg.force_stages : (int)((kSmemLimit - 2048) / stage_bytes);
+  int stages = (int)((kSmemLimit - 2048) / stage_bytes);
   if (stages > 8) stages = 8;
   if (stages < 2) stages = 2;      // consume_kblocks keeps one slot in flight before it releases the previous one
   p.stages = stages;
@@ -944,7 +943,7 @@ int64_t conv2_dgrad_implicit_elems(int B, int T2, int F2, int C) {
 // fp32-accumulate MN-major x MN-major 16-bit GEMM with M % 128 == 0 and N % 256 == 0; returns 2 (nothing launched) when the
 // group does not qualify, so that the caller issues the products one by one.
 int gemm_wgrad_group(const GemmArgs* gs, int n, cudaStream_t stream) {
-  if (n < 2 || n > kMaxGroup || getenv("B200ST_NO_GROUPED_WGRAD")) return 2;
+  if (n < 2 || n > kMaxGroup) return 2;
   for (int i = 0; i < n; ++i) {
     const GemmArgs& g = gs[i];
     const bool plain = !g.epi.relu && !g.epi.mask_src && g.epi.drop.p == 0.f && !g.epi.residual && !g.epi.bias && g.epi.accumulate;
@@ -953,14 +952,8 @@ int gemm_wgrad_group(const GemmArgs* gs, int n, cudaStream_t stream) {
           (reinterpret_cast<uintptr_t>(g.C) & 7) == 0 && g.ldc % 2 == 0))
       return 2;
   }
-  if (ablate_mask() & ABL_WGRAD) return 0;
-  if (g_num_sms == 0) {
-    int dev = 0;
-    B200ST_CUDA(cudaGetDevice(&dev));
-    B200ST_CUDA(cudaDeviceGetAttribute(&g_num_sms, cudaDevAttrMultiProcessorCount, dev));
-  }
-  const TcDebug& dbg = tc_debug();
-  const int num_sms = dbg.max_ctas > 0 ? dbg.max_ctas : (dbg.reserve_sms > 0 && dbg.reserve_sms < g_num_sms ? g_num_sms - dbg.reserve_sms : g_num_sms);
+  int num_sms = 0;
+  B200ST_TRY(usable_sms(&num_sms));
   TcGroup grp;
   std::memset(&grp, 0, sizeof(grp));
   grp.n = n;
@@ -1023,25 +1016,25 @@ int gemm_wgrad_group(const GemmArgs* gs, int n, cudaStream_t stream) {
 // Fused FFN forward (see fused_mlp_fwd_kernel).  X: 16-bit [M, d] (LayerNorm output); W1 [d, ffn], W2 [ffn, d] in the same
 // 16-bit type (TF layouts); F1 out [M, ffn] (saved for the backward pass); x_out fp32 [M, d] must already hold the residual.
 bool fused_mlp_supported(int M, int d, int ffn, int dtype) {
-  return is16(dtype) && (d == 128 || d == 256) && ffn % 128 == 0 && M > 0 && !getenv("B200ST_NO_FUSED_MLP");
+  return is16(dtype) && (d == 128 || d == 256) && ffn % 128 == 0 && M > 0;
+}
+// slices of the hidden dimension: the most CTAs that still fit one wave, with an equal number of chunks per slice
+static int mlp_splits(int m_tiles, int chunks, int* splits) {
+  int num_sms = 0;
+  B200ST_TRY(usable_sms(&num_sms));
+  *splits = 1;
+  for (int s = 1; s <= chunks; ++s)
+    if (chunks % s == 0 && (int64_t)m_tiles * s <= num_sms) *splits = s;
+  return 0;
 }
 int fused_mlp_fwd(const void* X, int dtype, int M, int d, int ffn, const void* W1, const float* b1, const void* W2, const float* b2,
                   DropoutSpec drop_ffn, DropoutSpec drop_post, void* F1, float* x_out, cudaStream_t stream, int* tickets) {
-  if (ablate_mask() & ABL_MLP_FWD) return 0;
   B200ST_CHECK(fused_mlp_supported(M, d, ffn, dtype), "fused MLP: unsupported shape / dtype");
-  if (g_num_sms == 0) {
-    int dev = 0;
-    B200ST_CUDA(cudaGetDevice(&dev));
-    B200ST_CUDA(cudaDeviceGetAttribute(&g_num_sms, cudaDevAttrMultiProcessorCount, dev));
-  }
   if (drop_ffn.p > 0.f) B200ST_CHECK(drop_ffn.bits != nullptr, "fused MLP needs precomputed dropout bits");
   if (drop_post.p > 0.f) B200ST_CHECK(drop_post.bits != nullptr, "fused MLP needs precomputed dropout bits");
   const int m_tiles = ceil_div(M, BM), chunks = ffn / 128;
-  // slices of the hidden dimension: the most CTAs that still fit one wave, with an equal number of chunks per slice
   int splits = 1;
-  for (int s2 = 1; s2 <= chunks; ++s2)
-    if (chunks % s2 == 0 && (int64_t)m_tiles * s2 <= g_num_sms - tc_debug().reserve_sms) splits = s2;
-  if (getenv("B200ST_MLP_SPLITS")) { const int f = atoi(getenv("B200ST_MLP_SPLITS")); if (f >= 1 && chunks % f == 0) splits = f; }
+  B200ST_TRY(mlp_splits(m_tiles, chunks, &splits));
   MlpParams p{};
   p.M = M; p.d = d; p.ffn = ffn; p.splits = splits; p.chunks_per_cta = chunks / splits;
   p.b1 = b1; p.b2 = b2; p.drop_ffn = drop_ffn; p.drop_post = drop_post;
@@ -1070,18 +1063,10 @@ int fused_mlp_fwd(const void* X, int dtype, int M, int d, int ffn, const void* W
 // dH += dF1 W1^T (fp32, dH must be zero-initialised).  Same kernel, weights read as K-major B operands.
 int fused_mlp_bwd(const void* dY, int dtype, int M, int d, int ffn, const void* W1, const void* W2, const void* F1, float scale,
                   void* dF1, float* dH, cudaStream_t stream, int* tickets) {
-  if (ablate_mask() & ABL_MLP_BWD) return 0;
   B200ST_CHECK(fused_mlp_supported(M, d, ffn, dtype), "fused MLP: unsupported shape / dtype");
-  if (g_num_sms == 0) {
-    int dev = 0;
-    B200ST_CUDA(cudaGetDevice(&dev));
-    B200ST_CUDA(cudaDeviceGetAttribute(&g_num_sms, cudaDevAttrMultiProcessorCount, dev));
-  }
   const int m_tiles = ceil_div(M, BM), chunks = ffn / 128;
   int splits = 1;
-  for (int s2 = 1; s2 <= chunks; ++s2)
-    if (chunks % s2 == 0 && (int64_t)m_tiles * s2 <= g_num_sms - tc_debug().reserve_sms) splits = s2;
-  if (getenv("B200ST_MLP_SPLITS")) { const int f = atoi(getenv("B200ST_MLP_SPLITS")); if (f >= 1 && chunks % f == 0) splits = f; }
+  B200ST_TRY(mlp_splits(m_tiles, chunks, &splits));
   MlpParams p{};
   p.M = M; p.d = d; p.ffn = ffn; p.splits = splits; p.chunks_per_cta = chunks / splits;
   p.b1 = nullptr; p.b2 = nullptr; p.drop_ffn = no_dropout(); p.drop_post = no_dropout();
@@ -1116,6 +1101,7 @@ int tc_profile_end(double* ms, double* flops, int64_t* launches) {
   g_prof = false;
   constexpr int kReps = 4;
   double tms = 0, tf = 0;
+  // B200ST_PROFILE_CSV only names a file for the per-GEMM rows (tools/step_profile.py reads it); nothing computed changes
   FILE* dump = getenv("B200ST_PROFILE_CSV") ? fopen(getenv("B200ST_PROFILE_CSV"), "w") : nullptr;
   if (dump) fprintf(dump, "M,N,K,batch,bn,splitk,a_mn,b_mn,epi,us,tflops\n");
   cudaEvent_t e0, e1;

@@ -22,6 +22,16 @@ def test_library_exports_every_declared_symbol():
     assert lib.b200st_version() == L.ABI_VERSION
 
 
+def test_library_reads_only_measurement_environment_variables():
+    """Every kernel path is chosen from dtype, shapes and config; the only environment variables the library reads
+    concern measurement: launching without PDL for profiler kernel times, and the GEMM profile's CSV file."""
+    csrc = os.path.join(ROOT, "neurst_b200", "csrc")
+    src = "".join(open(os.path.join(csrc, f)).read() for f in sorted(os.listdir(csrc)) if f.endswith((".cu", ".cuh")))
+    names = re.findall(r'\bgetenv\s*\(\s*"([^"]*)"', src)
+    assert len(names) == len(re.findall(r"\bgetenv\s*\(", src)), "getenv with a name that is not a string literal"
+    assert set(names) == {"B200ST_NO_PDL", "B200ST_PROFILE_CSV"}, sorted(set(names))
+
+
 def test_io_library_exports_every_declared_symbol():
     import ctypes
     from neurst_b200.csrc import build as B

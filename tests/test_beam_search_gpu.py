@@ -88,7 +88,9 @@ def test_all_beams_sorted_and_teacher_forced_logprob():
     hyp2, scores2 = model.beam_search(inputs, beam_size=beam, top_k=beam, length_penalty=0.6, maximum_decode_length=24,
                                       extra_decode_length=8)
     torch.cuda.synchronize()
-    assert torch.equal(hyp2, ids) and torch.equal(scores2, scores)
+    # two separate searches: the decoder step reduces with fp32 atomics, so the scores of two runs agree to rounding, not
+    # bit for bit (the same tolerance as beam 1 against greedy below)
+    assert torch.equal(hyp2, ids) and torch.allclose(scores2, scores, rtol=1e-5, atol=0.0), (scores2.tolist(), scores.tolist())
     s = scores.cpu().view(2, beam)
     assert bool((s[:, :-1] >= s[:, 1:]).all()), s
     n = ids.shape[0]

@@ -1,4 +1,5 @@
-"""C-level timing (no Python overhead) of the wgmma GEMM at the model's shapes. Results -> bench_out/gemm_perf.json"""
+"""C-level timing (no Python overhead) of the wgmma GEMM at the model's shapes and epilogues, with the tile configuration
+the library picks. Results -> bench_out/gemm_perf.json"""
 import json
 import os
 import sys
@@ -8,7 +9,6 @@ sys.path.insert(0, ROOT)
 import torch  # noqa
 from neurst_b200 import lib  # noqa
 
-L = lib.load()
 dev = "cuda"
 res = {}
 
@@ -17,35 +17,51 @@ def rnd(*s):
     return torch.randn(*s, device=dev).to(torch.bfloat16)
 
 
-def run(tag, M, N, K, out_dtype=torch.bfloat16, bn=0, stages=0, a_mn=False, b_mn=False, **kw):
-    L.b200st_debug_tc(bn, stages, 0)
+def run(tag, M, N, K, out_dtype=torch.bfloat16, a_mn=False, b_mn=False, **kw):
     A = rnd(K, M) if a_mn else rnd(M, K)
     B = rnd(K, N) if b_mn else rnd(N, K)
     Cc = torch.zeros(M, N, device=dev, dtype=out_dtype)
-    ms = lib.gemm_bench(A, B, Cc, iters=30, a_mn=a_mn, b_mn=b_mn, **kw)
+    ms = lib.gemm_bench(A, B, Cc, iters=50, a_mn=a_mn, b_mn=b_mn, **kw)
     r = dict(ms=ms, tflops=2.0 * M * N * K / ms / 1e9)
     res[tag] = r
-    print(tag, r, flush=True)
+    print("%-40s %8.1f us %8.1f TF" % (tag, ms * 1e3, r["tflops"]), flush=True)
 
 
-for bn in (0, 64, 128, 256):
-    run("ffn1_M8192_N2048_K256_bn%d" % bn, 8192, 2048, 256, bn=bn)
-run("ffn1_f32out", 8192, 2048, 256, out_dtype=torch.float32)
-for st in (2, 4):
-    run("ffn1_bn128_stages%d" % st, 8192, 2048, 256, bn=128, stages=st)
-for bn in (0, 128, 256):
-    run("ffn2_M8192_N256_K2048_bn%d" % bn, 8192, 256, 2048, bn=bn)
-run("qkv_M8192_N768_K256", 8192, 768, 256)
-run("qkv_bmn", 8192, 768, 256, b_mn=True)
-run("out_M8192_N256_K256", 8192, 256, 256)
-for bn in (0, 128, 256):
-    run("conv2_M160000_N256_K2304_bn%d" % bn, 160000, 256, 2304, bn=bn)
-run("dense_M8000_N256_K5120", 8000, 256, 5120)
-run("logits_M2816_N8192_K256", 2816, 8192, 256, out_dtype=torch.float32)
-run("big_8192", 8192, 8192, 8192)
-run("big_4096", 4096, 4096, 4096)
-# wgrad forms (split-K, fp32 accumulate)
-run("wgrad_ffn_K8000", 256, 2048, 8000, out_dtype=torch.float32, a_mn=True, b_mn=True, accumulate=True, splitk=0)
-run("wgrad_conv2_K160000", 2304, 256, 160000, out_dtype=torch.float32, a_mn=True, b_mn=True, accumulate=True, splitk=0)
+# FFN1 [M, 256] x [256, 2048] and its epilogues
+for M in (8000, 8192):
+    run("ffn1 M=%d" % M, M, 2048, 256)
+    run("ffn1 b_mn M=%d" % M, M, 2048, 256, b_mn=True)
+bias = torch.randn(2048, device=dev)
+run("ffn1 bias", 8000, 2048, 256, b_mn=True, bias=bias)
+run("ffn1 bias relu", 8000, 2048, 256, b_mn=True, bias=bias, relu=True)
+run("ffn1 bias relu drop(philox)", 8000, 2048, 256, b_mn=True, bias=bias, relu=True, dropout=(0.1, 1, 2))
+run("ffn1 mask", 8000, 2048, 256, mask_src=rnd(8000, 2048))
+run("ffn1 f32 out", 8000, 2048, 256, out_dtype=torch.float32)
+run("ffn1 f32 out + residual", 8000, 2048, 256, out_dtype=torch.float32, residual=torch.randn(8000, 2048, device=dev))
+# FFN2, attention projections
+bias2, res2 = torch.randn(256, device=dev), torch.randn(8000, 256, device=dev)
+run("ffn2 M=8192", 8192, 256, 2048)
+run("ffn2 M=8000", 8000, 256, 2048)
+run("ffn2 f32 bias res", 8000, 256, 2048, out_dtype=torch.float32, bias=bias2, residual=res2, b_mn=True)
+run("qkv", 8192, 768, 256)
+run("qkv b_mn", 8192, 768, 256, b_mn=True)
+run("qkv bias", 8000, 768, 256, b_mn=True, bias=torch.randn(768, device=dev))
+run("out-proj M=8192", 8192, 256, 256)
+run("out-proj M=8000", 8000, 256, 256)
+run("out-proj f32 bias res", 8000, 256, 256, out_dtype=torch.float32, bias=bias2, residual=res2, b_mn=True)
+# front-end, output layer, large squares
+run("conv2 M=160000", 160000, 256, 2304)
+run("dense M=8000 K=5120", 8000, 256, 5120)
+run("logits f32 out", 2816, 8192, 256, out_dtype=torch.float32)
+run("big 8192", 8192, 8192, 8192)
+run("big 4096", 4096, 4096, 4096)
+# weight gradients (MN-major operands, fp32 accumulate): split-K picked by the library, then fixed factors
+wg = dict(out_dtype=torch.float32, a_mn=True, b_mn=True, accumulate=True)
+run("wgrad ffn 256x2048xK8000 auto", 256, 2048, 8000, splitk=0, **wg)
+for sk in (1, 2, 4, 8, 16):
+    run("wgrad ffn 256x2048xK8000 splitk=%d" % sk, 256, 2048, 8000, splitk=sk, **wg)
+for sk in (1, 4, 8, 13, 26):
+    run("wgrad qkv 256x768xK8000 splitk=%d" % sk, 256, 768, 8000, splitk=sk, **wg)
+run("wgrad conv2 2304x256xK160000 auto", 2304, 256, 160000, splitk=0, **wg)
 os.makedirs(os.path.join(ROOT, "bench_out"), exist_ok=True)
 json.dump(res, open(os.path.join(ROOT, "bench_out", "gemm_perf.json"), "w"), indent=1)

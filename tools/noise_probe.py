@@ -1,6 +1,6 @@
-"""Dev tool: run-to-run noise of the gradient arena (same batch, same dropout seed, repeated eager backward passes),
-with kernel families switched off one at a time to localise its source."""
-import os, sys
+"""Dev tool: run-to-run noise of the gradient arena (same batch, same dropout seed, repeated eager backward passes) in the
+default mode, the deterministic mode, on the unfused reference path and at a larger batch."""
+import sys
 sys.path.insert(0, ".")
 import torch
 from neurst_b200 import lib as L
@@ -29,16 +29,5 @@ def probe(tag, prec="fp16", dropout=0.1, disable_fused=False, B=4, T=160, Lq=12,
 
 probe("fp16 default")
 probe("fp16 deterministic slices", deterministic=True)
-os.environ["B200ST_MLP_SPLITS"] = "1"
-probe("fp16 fused MLP, 1 hidden slice")
-del os.environ["B200ST_MLP_SPLITS"]
-os.environ["B200ST_NO_FUSED_MLP_BWD"] = "1"
-probe("fp16 fused MLP fwd only")
-del os.environ["B200ST_NO_FUSED_MLP_BWD"]
-os.environ["B200ST_NO_FUSED_MLP"] = "1"
-probe("fp16 no fused MLP")
 probe("fp16 no fused MLP, no fused attn", disable_fused=True)
-del os.environ["B200ST_NO_FUSED_MLP"]
-os.environ["B200ST_NO_SIDE_STREAM"] = "1"
-probe("fp16 no side stream (new process only)")
 probe("fp16 big batch", B=8, T=400, Lq=40)
