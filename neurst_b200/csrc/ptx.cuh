@@ -72,6 +72,15 @@ __device__ __forceinline__ void tma_load_4d(uint32_t dst_smem, const void* tmap,
 }
 __device__ __forceinline__ void fence_proxy_async_smem() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
 
+// ---- named barriers (ids 1..15; 0 is __syncthreads) -------------------------------------------
+// `threads` counts every thread of both sides (a multiple of 32): sync blocks until it is reached, arrive does not block.
+__device__ __forceinline__ void named_bar_sync(int id, int threads) {
+  asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(threads) : "memory");
+}
+__device__ __forceinline__ void named_bar_arrive(int id, int threads) {
+  asm volatile("bar.arrive %0, %1;" ::"r"(id), "r"(threads) : "memory");
+}
+
 // ---- wgmma ---------------------------------------------------------------------------------
 // One warpgroup (4 consecutive warps, the first a multiple of 4) computes D[64 x N] (+)= A[64 x 16] * B[N x 16]^T per
 // instruction, fp32 accumulators in registers.  Accumulator fragment of thread t (warp w = t / 32 of the warpgroup, g = lane / 4,

@@ -1,13 +1,19 @@
 // wgmma / TMA 16-bit GEMM for sm_90a.
 //
 // Persistent, warp-specialised kernel (one CTA per SM, 384 threads = 3 warpgroups):
-//   warpgroup 0    : TMA producer (one thread: cp.async.bulk.tensor -> 128B-swizzled smem ring, mbarrier complete_tx);
-//                    gives its registers to the consumers (setmaxnreg)
-//   warpgroups 1, 2: consumers, 64 rows of the 128-row tile each: wgmma.mma_async from the smem ring into fp32 register
-//                    accumulators (one k-block in flight behind the one being issued), then the fused epilogue straight
-//                    from the accumulator fragments to global memory (plain stores, or fp32 atomics for split-K / accumulate)
-// Tile: 128 x BN x 64 (BN in {64,128,256}); operands may be K-major or MN-major (wgrad / PV products),
-// batched through 4-D tensor maps; optional split-K.  Every launch is a programmatic dependent launch (pdl.cuh).
+//   warpgroup 0    : TMA producer (one thread: cp.async.bulk.tensor -> 128B-swizzled smem ring, mbarrier complete_tx), filling
+//                    the ring with the k-blocks of the CTA's tiles in tile order; gives its registers to the consumers (setmaxnreg)
+//   warpgroups 1, 2: ping-pong consumers.  Each owns whole 128 x BN output tiles, alternating over the CTA's tiles, and
+//                    accumulates one with two m64 wgmma.mma_async per k16 step into fp32 registers (one k-block in flight
+//                    behind the one being issued).  Their main loops take turns through an ordered hand-off on two named
+//                    barriers, so one warpgroup's fused epilogue runs while the other's wgmmas keep the tensor cores busy.
+//                    Epilogue: per 64-row half, the fragments go to the warpgroup's own fp32 staging buffer in shared memory;
+//                    the warpgroup then reads it back row by row (a warp covers 64 consecutive columns) and applies the fused
+//                    epilogue with coalesced plain stores, or fp32 atomics for split-K / accumulate.  The generic epilogue
+//                    code exists once in a rolled loop instead of once per fragment register.
+// Tile: 128 x BN x 64 (BN in {64,128}: the 128 x 128 accumulator is 128 registers per thread of the 168-register budget of a
+// 384-thread CTA); operands may be K-major or MN-major (wgrad / PV products), batched through 4-D tensor maps; optional
+// split-K.  Every launch is a programmatic dependent launch (pdl.cuh).
 //
 // Replaces the cuBLAS calls behind tf.einsum / Dense / Conv2D at the reference sites listed in
 // SURVEY.md §2.3 (K3,K4,K8,K9,K10,K11,K13,K15), e.g. neurst/layers/common_layers.py:270,276-288.
@@ -29,6 +35,11 @@ constexpr int BM = 128;
 constexpr int BK = 64;                  // 64 bf16 = 128 B = one swizzle row
 constexpr int kThreads = 384;           // producer warpgroup + 2 consumer warpgroups
 constexpr int kConsumerWarps = 8;
+constexpr int kOrderBar = 1;            // named barriers kOrderBar + wg: "consumer warpgroup wg may start its main loop"
+constexpr int kEpiBar = 3;              // named barriers kEpiBar + wg: the 4 warps of warpgroup wg around its staging buffer
+// Epilogue staging buffer of one consumer warpgroup: 64 rows x BN fp32 accumulators.  Rows are BN + 8 floats apart, so the
+// 8-byte fragment stores of a half-warp (rows g..g+3, columns 2q) hit 32 distinct banks.
+__host__ __device__ constexpr uint32_t staging_bytes(int bn) { return 64u * (uint32_t)(bn + 8) * 4u; }
 constexpr int kSmemLimit = 232448;      // 227 KB
 constexpr uint32_t kABytes = BM * BK * 2;
 constexpr int kProducerRegs = 40, kConsumerRegs = 232;   // 128 * 40 + 256 * 232 = 384 * 168 registers
@@ -68,7 +79,7 @@ __device__ __forceinline__ TileCoord decode_tile(const TcParams& p, int64_t tile
 }
 
 // The smem operand ring shared by the producer thread and the consumer warps: `full` barriers count the producer's
-// expect_tx arrival, `empty` barriers one arrival per consumer warp.
+// expect_tx arrival, `empty` barriers one arrival per warp that reads the slot (init(releasers)).
 struct Ring {
   uint32_t smem, bars, stage_bytes;
   int stages, stage;
@@ -77,8 +88,15 @@ struct Ring {
   __device__ __forceinline__ uint32_t empty(int s) const { return bars + 8u * (stages + s); }
   __device__ __forceinline__ uint32_t slot() const { return smem + (uint32_t)stage * stage_bytes; }
   __device__ __forceinline__ void advance() { if (++stage == stages) { stage = 0; phase ^= 1u; } }
-  __device__ __forceinline__ void init() const {
-    for (int s = 0; s < stages; ++s) { ptx::mbar_init(bars + 8u * s, 1); ptx::mbar_init(empty(s), kConsumerWarps); }
+  // step over n slots that another warpgroup consumes
+  __device__ __forceinline__ void skip(int n) {
+    stage += n;
+    const int wraps = stage / stages;
+    stage -= wraps * stages;
+    phase ^= (uint32_t)wraps & 1u;
+  }
+  __device__ __forceinline__ void init(int releasers) const {
+    for (int s = 0; s < stages; ++s) { ptx::mbar_init(bars + 8u * s, 1); ptx::mbar_init(empty(s), releasers); }
   }
 };
 
@@ -132,9 +150,46 @@ __device__ __forceinline__ void epilogue_pair(const TcParams& p, float a0, float
   }
 }
 
+// Consumer warpgroup main loop of one whole 128 x BN tile: acc[h] (rows 64 h .. 64 h + 63) = sum over the next nkb ring slots
+// of A_slot[64 h .. 64 h + 63, :] B_slot^T.  Same pipelining as consume_kblocks; the slots are released by this warpgroup's 4
+// warps alone.  `handoff` (bar.arrive on the other warpgroup's order barrier) runs once the last k-block's wgmmas are issued,
+// so the other warpgroup's main loop queues behind them while this one drains its last group and runs its epilogue.
+template <int BN, bool A_MN, bool B_MN, bool BF>
+__device__ __forceinline__ void consume_tile(float (&acc)[2][BN / 2], Ring& r, int nkb, int lane, int handoff) {
+  int prev = -1;
+  for (int i = 0; i < nkb; ++i) {
+    ptx::mbar_wait(r.full(), r.phase);
+    const uint32_t sa = r.slot(), sb = r.slot() + kABytes;
+    ptx::fence_acc(acc[0]);
+    ptx::fence_acc(acc[1]);
+    ptx::wgmma_fence();
+#pragma unroll
+    for (int k = 0; k < BK / 16; ++k) {
+      const uint64_t db = B_MN ? ptx::desc_mnmajor(sb, k) : ptx::desc_kmajor(sb, k);
+#pragma unroll
+      for (int h = 0; h < 2; ++h)
+        ptx::WgmmaSS<BN, BF, A_MN, B_MN>::mma(acc[h], A_MN ? ptx::desc_mnmajor(sa + h * 8192u, k) : ptx::desc_kmajor(sa + h * 8192u, k),
+                                               db, (i > 0 || k > 0) ? 1 : 0);
+    }
+    ptx::wgmma_commit();
+    if (prev >= 0) {
+      ptx::wgmma_wait<1>();
+      if (lane == 0) ptx::mbar_arrive(r.empty(prev));
+    }
+    prev = r.stage;
+    r.advance();
+  }
+  if (handoff >= 0) ptx::named_bar_arrive(handoff, 256);
+  ptx::wgmma_wait<0>();
+  ptx::fence_acc(acc[0]);
+  ptx::fence_acc(acc[1]);
+  if (prev >= 0 && lane == 0) ptx::mbar_arrive(r.empty(prev));
+}
+
 template <int BN, bool A_MN, bool B_MN, bool BF>
 __global__ void __launch_bounds__(kThreads, 1)
 tc_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, const TcParams p) {
+  static_assert(BN <= 128, "a consumer warpgroup holds the whole 128 x BN accumulator");
   extern __shared__ uint8_t smem_raw[];
   constexpr uint32_t kBBytes = BN * BK * 2;
   constexpr uint32_t kStageBytes = kABytes + kBBytes;
@@ -143,7 +198,8 @@ tc_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
   ring.smem = (ptx::smem_u32(smem_raw) + 1023u) & ~1023u;
   ring.stages = p.stages;
   ring.stage_bytes = kStageBytes;
-  ring.bars = ring.smem + (uint32_t)p.stages * kStageBytes;
+  const uint32_t staging = ring.smem + (uint32_t)p.stages * kStageBytes;      // 2 x staging_bytes(BN)
+  ring.bars = staging + 2u * staging_bytes(BN);
   ring.stage = 0; ring.phase = 0;
 
   const int warp = threadIdx.x >> 5;
@@ -152,7 +208,7 @@ tc_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
   if (warp == 0 && lane == 0) {
     ptx::prefetch_tensormap(&tmA);
     ptx::prefetch_tensormap(&tmB);
-    ring.init();
+    ring.init(4);         // a slot is read by the 4 warps of the warpgroup that owns its tile
     ptx::fence_mbar_init();
   }
   __syncthreads();
@@ -202,30 +258,55 @@ tc_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
       }
     }
   } else {
-    // ===================== consumer warpgroups =====================
+    // ===================== consumer warpgroups (ping-pong) =====================
+    // Warpgroup wg takes the CTA's tiles j = wg, wg + 2, ...  The main loop of tile j starts after that of tile j - 1 has
+    // been issued: the warpgroup waits on its own order barrier (except for tile 0) and, when tile j + 1 exists, arrives on
+    // the other's.  Every arrive is matched by exactly one wait of the other warpgroup.
     ptx::reg_alloc<kConsumerRegs>();
     const int wg = (warp >> 2) - 1, g = lane >> 2, q = lane & 3;
     const GemmEpilogue& ep = p.epi;
-    float acc[BN / 2];
+    const int tid = threadIdx.x & 127;
+    float* stg = reinterpret_cast<float*>(smem_raw + (staging - ptx::smem_u32(smem_raw)) + (uint32_t)wg * staging_bytes(BN));
+    float acc[2][BN / 2];
 #pragma unroll
-    for (int i = 0; i < BN / 2; ++i) acc[i] = 0.f;
-    for (int64_t tile = blockIdx.x; tile < p.num_tiles; tile += gridDim.x) {
+    for (int i = 0; i < BN / 2; ++i) acc[0][i] = acc[1][i] = 0.f;
+    int j = 0;
+    for (int64_t tile = blockIdx.x; tile < p.num_tiles; tile += gridDim.x, ++j) {
       const TileCoord t = decode_tile(p, tile);
       const int kb0 = t.split * p.kb_per_split;
       const int kb1 = min(p.kb_total, kb0 + p.kb_per_split);
-      consume_kblocks<BN, A_MN, B_MN, BF>(acc, ring, kb1 - kb0, wg, lane);
-      const int m0 = t.m_blk * BM + wg * 64 + (warp & 3) * 16 + g;
-      const int n0 = t.n_blk * BN + 2 * q;
+      if ((j & 1) != wg) {
+        ring.skip(kb1 - kb0);
+        continue;
+      }
+      if (j > 0) ptx::named_bar_sync(kOrderBar + wg, 256);
+      const int handoff = tile + gridDim.x < p.num_tiles ? kOrderBar + (wg ^ 1) : -1;
+      consume_tile<BN, A_MN, B_MN, BF>(acc, ring, kb1 - kb0, lane, handoff);
       const int64_t bidx = (int64_t)t.b2 * p.nb1 + t.b1;
       const int64_t boff_c = (int64_t)t.b2 * p.c_sb2 + (int64_t)t.b1 * p.c_sb1;
       const int64_t boff_mask = (int64_t)t.b2 * ep.mask_sb2 + (int64_t)t.b1 * ep.mask_sb1;
       const int64_t boff_res = (int64_t)t.b2 * ep.res_sb2 + (int64_t)t.b1 * ep.res_sb1;
+      constexpr int kLd = BN + 8, kPairs = BN / 2, kRowStep = 128 / kPairs;
+      const int cp = tid % kPairs, n = t.n_blk * BN + 2 * cp;
 #pragma unroll
-      for (int j = 0; j < BN / 8; ++j) {
-        const int n = n0 + 8 * j;
+      for (int h = 0; h < 2; ++h) {
+        ptx::named_bar_sync(kEpiBar + wg, 128);          // the previous half's reads are done
+#pragma unroll
+        for (int jj = 0; jj < BN / 8; ++jj) {
+          const int r = (warp & 3) * 16 + g, c = 8 * jj + 2 * q;
+          *reinterpret_cast<float2*>(stg + r * kLd + c) = make_float2(acc[h][4 * jj], acc[h][4 * jj + 1]);
+          *reinterpret_cast<float2*>(stg + (r + 8) * kLd + c) = make_float2(acc[h][4 * jj + 2], acc[h][4 * jj + 3]);
+        }
+        ptx::named_bar_sync(kEpiBar + wg, 128);
         if (n < p.N) {
-          if (m0 < p.M) epilogue_pair(p, acc[4 * j], acc[4 * j + 1], m0, n, bidx, boff_c, boff_mask, boff_res);
-          if (m0 + 8 < p.M) epilogue_pair(p, acc[4 * j + 2], acc[4 * j + 3], m0 + 8, n, bidx, boff_c, boff_mask, boff_res);
+#pragma unroll 4
+          for (int r = tid / kPairs; r < 64; r += kRowStep) {
+            const int m = t.m_blk * BM + h * 64 + r;
+            if (m < p.M) {
+              const float2 v = *reinterpret_cast<const float2*>(stg + r * kLd + 2 * cp);
+              epilogue_pair(p, v.x, v.y, m, n, bidx, boff_c, boff_mask, boff_res);
+            }
+          }
         }
       }
     }
@@ -292,7 +373,7 @@ __global__ void __launch_bounds__(kThreads, 1) tc_wgrad_group_kernel(const __gri
       ptx::prefetch_tensormap(&grp.prob[i].ta);
       ptx::prefetch_tensormap(&grp.prob[i].tb);
     }
-    ring.init();
+    ring.init(kConsumerWarps);
     ptx::fence_mbar_init();
   }
   __syncthreads();
@@ -787,10 +868,12 @@ int gemm_tc_impl(const GemmArgs& g, cudaStream_t stream, const ConvA* conv) {
   const int64_t batch = (int64_t)g.nb1 * g.nb2;
 
   // ---- joint choice of the N tile and the split-K factor ----
-  // Cost model per k-block of a CTA: max(tensor time, L2->smem fill time): the wgmmas of a 128 x c x 64 block take about
-  // 4c cycles, the operand bytes (16 KB + 128c B) are assumed to arrive at ~44 B/cycle/SM (an estimate, not measured on
-  // H100).  The epilogue runs after the main loop of its tile.  Split-K (fp32 atomic epilogue) is allowed for linear
-  // accumulate epilogues only and is chosen so that the tile count fills the SMs once.
+  // Cost model of a CTA's share of the tiles.  Main loop of one tile, per k-block: max(tensor time, L2->smem fill time): the
+  // wgmmas of a 128 x c x 64 block take about 4c cycles, the operand bytes (16 KB + 128c B) are assumed to arrive at
+  // ~44 B/cycle/SM (an estimate, not measured on H100).  The two consumer warpgroups take turns on the tensor cores, so a
+  // tile's epilogue (one warpgroup, 128 rows) hides under the other warpgroup's main loop as far as that is long enough.
+  // Split-K (fp32 atomic epilogue) is allowed for linear accumulate epilogues only and is chosen so that the tile count fills
+  // the SMs once.
   const bool linear_epi = !g.epi.relu && !g.epi.mask_src && g.epi.drop.p == 0.f && !g.epi.residual && !g.epi.bias;
   const bool split_ok = linear_epi && g.c_dtype == F32 && g.epi.accumulate;
   if (g.splitk > 1) B200ST_CHECK(split_ok, "split-K needs a linear fp32 accumulate epilogue");
@@ -798,9 +881,9 @@ int gemm_tc_impl(const GemmArgs& g, cudaStream_t stream, const ConvA* conv) {
   {
     double best = 1e30;
     int best_bn = 0, best_sk = 1;
-    const int cands[3] = {256, 128, 64};
+    const int cands[2] = {128, 64};
     for (int c : cands) {
-      if (conv && c != 256) continue;
+      if (conv && c != 128) continue;
       if (c > 64 && c >= 2 * ((g.N + 63) / 64 * 64)) continue;   // do not pad N by 2x or more
       const int64_t tiles0 = batch * p.m_tiles * ceil_div(g.N, c);
       int sk_lo = splitk, sk_hi = splitk;
@@ -814,11 +897,12 @@ int gemm_tc_impl(const GemmArgs& g, cudaStream_t stream, const ConvA* conv) {
       for (int sk = sk_hi; sk >= sk_lo; sk = (sk > sk_lo && sk > 1) ? (sk == sk_hi && sk_hi > 2 ? sk / 2 : sk - 1) : sk_lo - 1) {
         const int kb_per = ceil_div(p.kb_total, sk);
         const int64_t tiles = tiles0 * ceil_div(p.kb_total, kb_per);
-        const int64_t waves = (tiles + num_sms - 1) / num_sms;
+        const int64_t per_cta = (tiles + num_sms - 1) / num_sms;
         const double fill = (16384.0 + 128.0 * c) / 44.0, mma = 4.0 * c;
         const double mainloop = kb_per * (fill > mma ? fill : mma);
-        const double epi = (sk > 1 ? 14.0 : 10.0) * c + 600.0;
-        const double cost = (double)waves * (mainloop + epi + 800.0) + (sk > 1 ? 500.0 : 0.0);
+        const double epi = (sk > 1 ? 28.0 : 20.0) * c + 600.0;
+        const double per_tile = mainloop > 0.5 * (mainloop + epi) ? mainloop : 0.5 * (mainloop + epi);
+        const double cost = (double)per_cta * per_tile + 0.5 * epi + 800.0 + (sk > 1 ? 500.0 : 0.0);
         if (cost < best) { best = cost; best_bn = c; best_sk = sk; }
         if (sk <= sk_lo) break;
       }
@@ -834,11 +918,11 @@ int gemm_tc_impl(const GemmArgs& g, cudaStream_t stream, const ConvA* conv) {
   p.num_tiles = batch * p.m_tiles * p.n_tiles * splitk;
 
   const uint32_t stage_bytes = kABytes + (uint32_t)bn * BK * 2;
-  int stages = (int)((kSmemLimit - 2048) / stage_bytes);
+  int stages = (int)((kSmemLimit - 2048 - 2 * staging_bytes(bn)) / stage_bytes);
   if (stages > 8) stages = 8;
-  if (stages < 2) stages = 2;      // consume_kblocks keeps one slot in flight before it releases the previous one
+  if (stages < 2) stages = 2;      // consume_tile keeps one slot in flight before it releases the previous one
   p.stages = stages;
-  const size_t smem = 1024 + (size_t)stages * stage_bytes + 16 * stages + 16;
+  const size_t smem = 1024 + (size_t)stages * stage_bytes + 2 * staging_bytes(bn) + 16 * stages + 16;
   B200ST_CHECK(smem <= (size_t)kSmemLimit, "smem budget exceeded");
 
   p.C = g.C; p.c_dtype = g.c_dtype; p.ldc = g.ldc; p.c_sb1 = g.c_sb1; p.c_sb2 = g.c_sb2;
@@ -852,7 +936,7 @@ int gemm_tc_impl(const GemmArgs& g, cudaStream_t stream, const ConvA* conv) {
 
   CUtensorMap ta, tb;
   if (conv) {
-    B200ST_CHECK(bn == 256 && splitk == 1 && !g.A.mn_major && !g.B.mn_major && g.nb1 == 1 && g.nb2 == 1 && conv->C % BK == 0 &&
+    B200ST_CHECK(bn == 128 && splitk == 1 && !g.A.mn_major && !g.B.mn_major && g.nb1 == 1 && g.nb2 == 1 && conv->C % BK == 0 &&
                      g.K == conv->ntaps * conv->C && g.M == conv->B * conv->ub * BM && conv->F2 * conv->tu <= BM && conv->ntaps <= 4,
                  "implicit conv dgrad: unsupported shape");
     p.conv = 1; p.conv_ub = conv->ub; p.conv_tu = conv->tu; p.conv_kpc = conv->C / BK;
@@ -890,7 +974,6 @@ int gemm_tc_impl(const GemmArgs& g, cudaStream_t stream, const ConvA* conv) {
   switch (bn) {
     case 64: rc = launch_bn<64>(g.A.mn_major, g.B.mn_major, bf, ta, tb, p, grid, smem, stream); break;
     case 128: rc = launch_bn<128>(g.A.mn_major, g.B.mn_major, bf, ta, tb, p, grid, smem, stream); break;
-    case 256: rc = launch_bn<256>(g.A.mn_major, g.B.mn_major, bf, ta, tb, p, grid, smem, stream); break;
     default: B200ST_FAIL("unsupported BN");
   }
   return rc;

@@ -1,12 +1,17 @@
-"""Kernel-time breakdown of one eager training step (cfg-2) with torch.profiler (CUPTI), aggregated by kernel."""
-import collections, os, re, sys
+"""Kernel-time breakdown of one eager training step (cfg-2) with torch.profiler (CUPTI), aggregated by kernel.
+
+Usage: python tools/torch_prof.py [--dtype fp16|bf16|fp32]   (default fp16, the precision bench.py times)"""
+import argparse, collections, os, re, sys
 os.environ.setdefault("B200ST_NO_PDL", "1")   # with PDL a dependent kernel's duration includes its wait on the predecessor
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 import torch
 from torch.profiler import profile, ProfilerActivity
 from neurst_b200.trainer import build_speech_transformer_trainer, synthetic_batch
-tr, _ = build_speech_transformer_trainer("speech_transformer_s", 8192, precision="bf16", label_smoothing=0.1)
+ap = argparse.ArgumentParser()
+ap.add_argument("--dtype", default="fp16", choices=["fp16", "bf16", "fp32"])
+args = ap.parse_args()
+tr, _ = build_speech_transformer_trainer("speech_transformer_s", 8192, precision=args.dtype, label_smoothing=0.1)
 b = synthetic_batch(32, 1000, 88, 8192, device="cuda")
 for i in range(3):
     tr.train_step(b, seed=i + 1)
