@@ -7,11 +7,14 @@
 //
 // forward : grid (q tiles of 128, H, B), 384 threads: warpgroup 0 = TMA producer, warpgroups 1-2 = 64 query rows each; the
 //           probabilities go back into the tensor cores as the register A operand of the PV product.
-// backward: attn_bwd_prep_kernel (zero dQ, D = rowsum(dO * O)), then grid (kv blocks of 128, H, B), 384 threads: K_j / V_j
-//           resident, each consumer warpgroup owns 64 keys and computes the transposed tiles S^T = K Q^T and dP^T = V dO^T, so
+// backward: attn_bwd_prep_kernel (zero dQ, D = rowsum(dO * O)), then grid (kv blocks of 128, H, B), 256 threads = two
+//           compute warpgroups (255-register budget; thread 0 also issues the TMA loads of a two-stage Q / dO ring): K_j / V_j
+//           resident, each warpgroup owns 64 keys and computes the transposed tiles S^T = K Q^T and dP^T = V dO^T, so
 //           that P^T and dS^T are register A operands of the dV / dK products (accumulated in registers over the q tiles);
-//           dS^T also goes through shared memory as the MN-major A operand of dQ = dS K, reduced across kv blocks with fp32
-//           vector RED into a scratch buffer (cast_rows_kernel -> bf16).
+//           dS^T also goes through shared memory as the MN-major A operand of dQ = dS K.  The next 64-query half's S^T / dP^T
+//           and its keep-bit loads are issued before the wait on the current dV / dK / dQ group; the two warpgroups' dQ
+//           partials are summed through shared memory and reduced across kv blocks with one fp32 RED per element into a
+//           scratch buffer (cast_rows_kernel -> bf16).
 #include "gemm.cuh"
 #include "kernels.cuh"
 #include "pdl.cuh"
@@ -29,7 +32,8 @@ constexpr float kLog2e = 1.4426950408889634f;
 constexpr float kLn2 = 0.6931471805599453f;
 constexpr float kMaskMin = -1.0e9f;   // neurst/utils/compat.py:24
 constexpr uint32_t kTile16K = 128 * 64 * 2;      // [128 rows x 64 bf16] swizzled tile
-constexpr int kAttnThreads = 384;                // TMA warpgroup + 2 compute warpgroups
+constexpr int kAttnThreads = 384;                // forward: TMA warpgroup + 2 compute warpgroups
+constexpr int kBwdThreads = 256;                 // 2 compute warpgroups; thread 0 also issues the TMA loads
 constexpr int kAttnConsumerWarps = 8;
 
 struct AttnParams {
@@ -79,18 +83,28 @@ __device__ __forceinline__ void load_keep64(const DropoutSpec& d, bool row_ok, i
     keep[1] = byte[4] | (byte[5] << 8) | (byte[6] << 16) | (byte[7] << 24);
     return;
   }
+  // no bitmap: regenerate with Philox (stand-alone attention API); rolled, and each word indexed by a constant so that
+  // keep[] stays in registers
+#pragma unroll
+  for (int w = 0; w < 2; ++w) {
 #pragma unroll 1
-  for (int g = 0; g < 8; ++g) {           // no bitmap: regenerate with Philox (stand-alone attention API)
-    if (k0 + 8 * g < Tkp) {
-      const uint32_t byte = dropout_keep8(dropout_seed(d), d.stream, (uint64_t)(row_bit0 + k0 + 8 * g) >> 3, thresh);
-      keep[g >> 2] = (keep[g >> 2] & ~(0xffu << (8 * (g & 3)))) | (byte << (8 * (g & 3)));
+    for (int g = 0; g < 4; ++g) {
+      const int k8 = k0 + 32 * w + 8 * g;
+      if (k8 < Tkp) {
+        const uint32_t byte = dropout_keep8(dropout_seed(d), d.stream, (uint64_t)(row_bit0 + k8) >> 3, thresh);
+        keep[w] = (keep[w] & ~(0xffu << (8 * g))) | (byte << (8 * g));
+      }
     }
   }
 }
-// the keep-byte of keys [k8, k8 + 8) of one query row (k8 % 8 == 0; Tkp % 8 == 0 keeps rows byte-aligned)
-__device__ __forceinline__ uint32_t load_keep8(const DropoutSpec& d, bool ok, int64_t row_bit0, int k8, int Tkp, uint32_t thresh) {
-  if (!(d.p > 0.f) || !ok || k8 >= Tkp) return 0xffu;
-  return drop_keep8(d, (uint64_t)(row_bit0 + k8) >> 3, thresh);
+// the keep-bits of keys [k16, k16 + 16) of one query row (k16 % 16 == 0; Tkp % 8 == 0 keeps rows byte-aligned); bits of keys
+// >= Tkp read as 1.  When the row's byte offset is even (always when Tkp % 16 == 0) the two bytes are one 16-bit load.
+__device__ __forceinline__ uint32_t load_keep16(const DropoutSpec& d, bool ok, int64_t row_bit0, int k16, int Tkp, uint32_t thresh) {
+  if (!ok || k16 >= Tkp) return 0xffffu;
+  const uint64_t byte = (uint64_t)(row_bit0 + k16) >> 3;
+  const bool hi = k16 + 8 < Tkp;
+  if (d.bits && hi && (byte & 1u) == 0) return __ldg(reinterpret_cast<const uint16_t*>(d.bits + byte));
+  return drop_keep8(d, byte, thresh) | ((hi ? drop_keep8(d, byte + 1, thresh) : 0xffu) << 8);
 }
 
 // ==============================================================================================================
@@ -163,13 +177,13 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__
         btab[k] = (k < p.Tk) ? (bias_row ? __ldg(bias_row + k) * kLog2e : 0.f) : -INFINITY;
       asm volatile("bar.sync 1, 256;" ::: "memory");
     }
-    int qrow[2]; int64_t bit0[2]; bool qok[2];
+    int qrow[2]; bool qok[2];
 #pragma unroll
     for (int r = 0; r < 2; ++r) {
       qrow[r] = qt * BQ + row0 + 8 * r;
       qok[r] = qrow[r] < p.Tq;
-      bit0[r] = (((int64_t)b * p.H + h) * p.Tq + qrow[r]) * p.Tkp;
     }
+    const int64_t bit0 = (((int64_t)b * p.H + h) * p.Tq + qrow[0]) * p.Tkp;   // keep-bit of row qrow[0], key 0 (row + 8: + 8 Tkp)
     float m[2] = {-INFINITY, -INFINITY}, l[2] = {0.f, 0.f};   // running row max (log2 domain), this thread's partial row sums
     float o[32];
 #pragma unroll
@@ -191,9 +205,9 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__
 #pragma unroll
       for (int r = 0; r < 2; ++r) {
         uint32_t k2[2];
-        load_keep64(p.drop, qok[r] && use_drop, bit0[r], j * BKV, p.Tkp, thresh, k2);
+        load_keep64(p.drop, qok[r] && use_drop, bit0 + 8 * r * p.Tkp, j * BKV, p.Tkp, thresh, k2);
         keep[r][0] = k2[0]; keep[r][1] = k2[1];
-        load_keep64(p.drop, qok[r] && use_drop, bit0[r], j * BKV + 64, p.Tkp, thresh, k2);
+        load_keep64(p.drop, qok[r] && use_drop, bit0 + 8 * r * p.Tkp, j * BKV + 64, p.Tkp, thresh, k2);
         keep[r][2] = k2[0]; keep[r][3] = k2[1];
       }
       ptx::wgmma_wait<0>();
@@ -282,7 +296,7 @@ __device__ __forceinline__ void red_add_v2(float* addr, float a, float b) {
 }
 
 template <bool CAUSAL, int DT>
-__global__ void __launch_bounds__(kAttnThreads, 1)
+__global__ void __launch_bounds__(kBwdThreads, 1)
 attn_bwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmK,
                 const __grid_constant__ CUtensorMap tmV, const __grid_constant__ CUtensorMap tmdO, const AttnParams p) {
   extern __shared__ uint8_t smem_raw[];
@@ -290,15 +304,17 @@ attn_bwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__
   const uint32_t base = (ptx::smem_u32(smem_raw) + 1023u) & ~1023u;
   const uint32_t sK = base;                          // 16 KB
   const uint32_t sV = sK + kTile16K;                 // 16 KB
-  const uint32_t sQ = sV + kTile16K;                 // 2 x 16 KB
-  const uint32_t sdO = sQ + 2 * kTile16K;            // 2 x 16 KB
-  const uint32_t sdS = sdO + 2 * kTile16K;           // 2 warpgroups x 2 buffers x 8 KB: dS^T [64 keys x 64 queries]
-  const uint32_t bars = sdS + 2 * kTile16K;
+  const uint32_t sQ = sV + kTile16K;                 // 2 stages x 16 KB
+  const uint32_t sdO = sQ + 2 * kTile16K;            // 2 stages x 16 KB
+  const uint32_t sdS = sdO + 2 * kTile16K;           // 2 warpgroups x 2 halves x 8 KB: dS^T [64 keys x 64 queries]
+  const uint32_t sX = sdS + 2 * kTile16K;            // 2 warpgroups x 2 halves x 8 KB: dQ partials handed to the other warpgroup
+  const uint32_t sLD = sX + 2 * kTile16K;            // 2 stages x (LSE[128] * log2(e), D[128]) fp32
+  const uint32_t sB = sLD + 2048;                    // key bias * log2(e) of this kv block, 128 floats
+  const uint32_t bars = sB + 512;
   const uint32_t kv_full = bars;
   auto qdo_full = [&](int s) { return bars + 8u * (1 + s); };
   auto qdo_empty = [&](int s) { return bars + 8u * (3 + s); };
-  const uint32_t sB = bars + 128;                    // key bias * log2(e) of this kv block, 128 floats
-  float* btab = reinterpret_cast<float*>(smem_raw + (sB - ptx::smem_u32(smem_raw)));
+  auto smem_f = [&](uint32_t a) { return reinterpret_cast<float*>(smem_raw + (a - ptx::smem_u32(smem_raw))); };
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int jb = blockIdx.x, h = blockIdx.y, b = blockIdx.z;
@@ -317,7 +333,9 @@ attn_bwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__
     return;
   }
 
-  if (warp == 0 && lane == 0) {
+  const bool producer = threadIdx.x == 0;
+  const int row_lse = (b * p.H + h) * p.Tq;         // first LSE / D element of this (b, h)
+  if (producer) {
     ptx::prefetch_tensormap(&tmQ); ptx::prefetch_tensormap(&tmK); ptx::prefetch_tensormap(&tmV); ptx::prefetch_tensormap(&tmdO);
     ptx::mbar_init(kv_full, 1);
     for (int s = 0; s < 2; ++s) { ptx::mbar_init(qdo_full(s), 1); ptx::mbar_init(qdo_empty(s), kAttnConsumerWarps); }
@@ -327,156 +345,205 @@ attn_bwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__
   pdl_wait();      // everything above (barriers, descriptor prefetch) overlaps the previous kernel's tail
   pdl_trigger();
 
-  if (warp < 4) {
-    ptx::reg_dealloc<40>();
-    if (warp == 0 && lane == 0) {
-      ptx::mbar_arrive_expect_tx(kv_full, 2 * kTile16K);
-      ptx::tma_load_4d(sK, &tmK, kv_full, 0, jb * BKV, h, b);
-      ptx::tma_load_4d(sV, &tmV, kv_full, 0, jb * BKV, h, b);
-      for (int i = 0; i < nq; ++i) {
-        const int st = i & 1;
-        ptx::mbar_wait(qdo_empty(st), (((uint32_t)i >> 1) & 1u) ^ 1u);
-        ptx::mbar_arrive_expect_tx(qdo_full(st), 2 * kTile16K);
-        ptx::tma_load_4d(sQ + st * kTile16K, &tmQ, qdo_full(st), 0, i * BQ, h, b);
-        ptx::tma_load_4d(sdO + st * kTile16K, &tmdO, qdo_full(st), 0, i * BQ, h, b);
+  // Producer side (thread 0 only): query tile i (Q and dO) goes to stage i % 2 once all 8 warps have released tile i - 2.
+  auto load_tile = [&](int i) {
+    const int st = i & 1;
+    ptx::mbar_arrive_expect_tx(qdo_full(st), 2 * kTile16K);
+    ptx::tma_load_4d(sQ + st * kTile16K, &tmQ, qdo_full(st), 0, i * BQ, h, b);
+    ptx::tma_load_4d(sdO + st * kTile16K, &tmdO, qdo_full(st), 0, i * BQ, h, b);
+  };
+  // The tile's 128 LSE (times log2 e; +inf past Tq, so that P = 0 there) and 128 D values go to the LSE / D stage i % 2, one
+  // value per thread.  The loads are issued under the MMAs of the tile before; a 256-thread barrier precedes every first read,
+  // and a stage is rewritten only after the barrier that follows the last read of the tile it held.
+  auto load_lse_d = [&](int i) {
+    const int t = threadIdx.x & 127, q = i * BQ + t;
+    float v;
+    if (threadIdx.x < 128) v = q < p.Tq ? __ldg(p.lse + row_lse + q) * kLog2e : INFINITY;
+    else v = q < p.Tq ? __ldg(p.dvec + row_lse + q) : 0.f;
+    smem_f(sLD + (i & 1) * 1024)[threadIdx.x] = v;
+  };
+  if (producer) {
+    ptx::mbar_arrive_expect_tx(kv_full, 2 * kTile16K);
+    ptx::tma_load_4d(sK, &tmK, kv_full, 0, jb * BKV, h, b);
+    ptx::tma_load_4d(sV, &tmV, kv_full, 0, jb * BKV, h, b);
+    for (int i = 0; i < nq && i < 2; ++i) load_tile(i);
+  }
+  load_lse_d(0);
+  {
+    float* btab = smem_f(sB);
+    const float* bias_row = p.bias ? p.bias + (int64_t)b * p.Tk : nullptr;
+    const int t = threadIdx.x, k = jb * BKV + t;
+    if (t < BKV) btab[t] = (k < p.Tk) ? (bias_row ? __ldg(bias_row + k) * kLog2e : 0.f) : -INFINITY;
+    __syncthreads();
+  }
+
+  // Warpgroup wg owns keys [64 wg, 64 wg + 64) of the block; thread = 2 keys (g, g + 8 of the warp's 16) x the query columns
+  // 8 c + 2 qd + {0, 1} of the transposed tiles.  Branch-free element math as in the forward kernel; the dropout scale is
+  // folded into dS (FFMA) and into the dV epilogue.
+  const int wg = warp >> 2, g = lane >> 2, qd = lane & 3;
+  const int krow0 = wg * 64 + (warp & 3) * 16 + g;          // key row inside the block (+ 8 for the second)
+  const uint32_t thresh = dropout_thresh16(p.drop.p);
+  const float a2 = p.alpha * kLog2e;
+  const float cmask = kMaskMin * kLog2e;
+  const bool use_drop = p.drop.p > 0.f;
+  const float dscale = use_drop ? p.drop.scale : 1.0f;
+  const float kbias[2] = {smem_f(sB)[krow0], smem_f(sB)[krow0 + 8]};
+  const int key[2] = {jb * BKV + krow0, jb * BKV + krow0 + 8};
+  const int key16 = key[0] & ~15;                           // key[0] & 7 == g, key[1] = key[0] + 8
+  const uint32_t sK_wg = sK + (uint32_t)wg * 8192u, sV_wg = sV + (uint32_t)wg * 8192u;
+  const int nu = 2 * nq;                                    // units of work: the two 64-query halves of every query tile
+
+  float dv[32], dk[32], st_[32], dpt[32];
+  uint32_t kb[16];                                          // keep bits of (query column 2 c8 + e) x keys key16 .. key16 + 15
+#pragma unroll
+  for (int t = 0; t < 32; ++t) { dv[t] = 0.f; dk[t] = 0.f; }
+  // S^T = K Q^T ; dP^T = V dO^T ([64 keys x 64 queries] each) of unit u, and its keep bits (loaded while the MMAs run)
+  auto issue_sdp = [&](int u) {
+    const uint32_t q_h = sQ + ((u >> 1) & 1) * kTile16K + (uint32_t)(u & 1) * 8192u;
+    const uint32_t do_h = sdO + ((u >> 1) & 1) * kTile16K + (uint32_t)(u & 1) * 8192u;
+#pragma unroll
+    for (int t = 0; t < 32; ++t) { st_[t] = 0.f; dpt[t] = 0.f; }
+    ptx::fence_acc(st_); ptx::fence_acc(dpt);
+    ptx::wgmma_fence();
+#pragma unroll
+    for (int k = 0; k < DH / 16; ++k)
+      ptx::WgmmaSS<64, BF, 0, 0>::mma(st_, ptx::desc_kmajor(sK_wg, k), ptx::desc_kmajor(q_h, k), k > 0 ? 1 : 0);
+#pragma unroll
+    for (int k = 0; k < DH / 16; ++k)
+      ptx::WgmmaSS<64, BF, 0, 0>::mma(dpt, ptx::desc_kmajor(sV_wg, k), ptx::desc_kmajor(do_h, k), k > 0 ? 1 : 0);
+    ptx::wgmma_commit();
+#pragma unroll
+    for (int t = 0; t < 16; ++t) {
+      const int q = (u >> 1) * BQ + (u & 1) * 64 + 8 * (t >> 1) + 2 * qd + (t & 1);
+      kb[t] = load_keep16(p.drop, use_drop && q < p.Tq, ((int64_t)row_lse + q) * p.Tkp, key16, p.Tkp, thresh);
+    }
+  };
+
+  ptx::mbar_wait(kv_full, 0);
+  ptx::mbar_wait(qdo_full(0), 0);
+  issue_sdp(0);
+  for (int u = 0; u < nu; ++u) {
+    const int i = u >> 1, hq = u & 1, st = i & 1;
+    const uint32_t q_h = sQ + st * kTile16K + (uint32_t)hq * 8192u, do_h = sdO + st * kTile16K + (uint32_t)hq * 8192u;
+    const float* lse_s = smem_f(sLD + st * 1024) + hq * 64;
+    const float* d_s = lse_s + 128;
+    ptx::wgmma_wait<0>();
+    ptx::fence_acc(st_); ptx::fence_acc(dpt);
+    uint32_t p16[4][4], ds16[4][4];
+    const uint32_t ds_buf = sdS + (uint32_t)(2 * wg + hq) * 8192u;
+#pragma unroll
+    for (int c8 = 0; c8 < 8; ++c8) {
+      const int ql = 8 * c8 + 2 * qd;                   // query column inside the half
+      const int q0 = i * BQ + hq * 64 + ql;
+      const float2 lse2 = *reinterpret_cast<const float2*>(lse_s + ql), Dq = *reinterpret_cast<const float2*>(d_s + ql);
+#pragma unroll
+      for (int r = 0; r < 2; ++r) {
+        float pd[2], ds[2];
+#pragma unroll
+        for (int e = 0; e < 2; ++e) {
+          float x = fmaf(st_[4 * c8 + 2 * r + e], a2, kbias[r]);
+          if (CAUSAL) x = (key[r] > q0 + e + (p.Tk - p.Tq)) ? x + cmask : x;
+          const float pr = ex2_approx(x - (e ? lse2.y : lse2.x));
+          const bool kp = (kb[2 * c8 + e] >> (8 * r + g)) & 1u;
+          const float dpv = kp ? dpt[4 * c8 + 2 * r + e] : 0.f;
+          pd[e] = kp ? pr : 0.f;
+          ds[e] = pr * fmaf(dpv, dscale, -(e ? Dq.y : Dq.x));
+        }
+        const uint32_t pp = pack_bf16(pd[0], pd[1]), dd = pack_bf16(ds[0], ds[1]);
+        p16[c8 >> 1][(c8 & 1) * 2 + r] = pp;
+        ds16[c8 >> 1][(c8 & 1) * 2 + r] = dd;
+        // dS^T -> shared memory, MN-major A operand of dQ = dS K: row = key (128 B = 64 queries), 128B swizzle
+        const int kr = krow0 - wg * 64 + 8 * r;
+        const uint32_t addr = ds_buf + (uint32_t)kr * 128u + ((uint32_t)(c8 ^ (kr & 7)) << 4) + (uint32_t)qd * 4u;
+        asm volatile("st.shared.b32 [%0], %1;" ::"r"(addr), "r"(dd) : "memory");
       }
     }
-  } else {
-    // compute warpgroup wg owns keys [64 wg, 64 wg + 64) of the block; thread = 2 keys (g, g + 8 of the warp's 16) x the
-    // query columns 8 c + 2 qd + {0, 1} of the transposed tiles.  Branch-free element math as in the forward kernel; the
-    // dropout scale is folded into dS (FFMA) and into the dV epilogue.
-    ptx::reg_alloc<232>();
-    const int wg = (warp >> 2) - 1, g = lane >> 2, qd = lane & 3;
-    const int krow0 = wg * 64 + (warp & 3) * 16 + g;          // key row inside the block (+ 8 for the second)
-    const uint32_t thresh = dropout_thresh16(p.drop.p);
-    const float a2 = p.alpha * kLog2e;
-    const float cmask = kMaskMin * kLog2e;
-    const bool use_drop = p.drop.p > 0.f;
-    const float dscale = use_drop ? p.drop.scale : 1.0f;
+    ptx::fence_proxy_async_smem();       // dS^T (generic-proxy writes) -> visible to the tensor-core (async) proxy
+    ptx::named_bar_sync(1 + wg, 128);
+    // dV += P^T dO ; dK += dS^T Q (contraction over the 64 queries) ; dQ[64 queries x 64] = dS K (over this warpgroup's 64 keys)
+    float dq[32];
+#pragma unroll
+    for (int t = 0; t < 32; ++t) dq[t] = 0.f;
+    ptx::fence_acc(dv); ptx::fence_acc(dk); ptx::fence_acc(dq);
+    ptx::wgmma_fence();
+#pragma unroll
+    for (int k = 0; k < 4; ++k) {
+      ptx::WgmmaRS<DH, BF, 1>::mma(dv, p16[k], ptx::desc_mnmajor(do_h, k), 1);
+      ptx::WgmmaRS<DH, BF, 1>::mma(dk, ds16[k], ptx::desc_mnmajor(q_h, k), 1);
+      ptx::WgmmaSS<DH, BF, 1, 1>::mma(dq, ptx::desc_mnmajor(ds_buf, k), ptx::desc_mnmajor(sK_wg, k), k > 0 ? 1 : 0);
+    }
+    ptx::wgmma_commit();
+    // the next unit's S^T / dP^T run under this unit's dQ reduction
+    if (u + 1 < nu) {
+      if (hq == 1) ptx::mbar_wait(qdo_full((i + 1) & 1), ((uint32_t)(i + 1) >> 1) & 1u);
+      issue_sdp(u + 1);
+      if (hq == 1) load_lse_d(i + 1);
+      ptx::wgmma_wait<1>();
+    } else {
+      ptx::wgmma_wait<0>();
+    }
+    ptx::fence_acc(dv); ptx::fence_acc(dk); ptx::fence_acc(dq);
+    // dQ: both warpgroups hold partials of the same 64 x 64 block (over different keys).  Warpgroup 0 sums and reduces
+    // columns [0, 32), warpgroup 1 columns [32, 64): each hands the other half of its fragment over through shared memory,
+    // laid out [float4 j][thread] so that the stores and loads are free of bank conflicts.  The buffers alternate with
+    // hq, so one barrier per unit also orders a buffer's reads before its next writes.
     {
-      const float* bias_row = p.bias ? p.bias + (int64_t)b * p.Tk : nullptr;
-      const int t = threadIdx.x - 128;
-      if (t < BKV) {
-        const int k = jb * BKV + t;
-        btab[t] = (k < p.Tk) ? (bias_row ? __ldg(bias_row + k) * kLog2e : 0.f) : -INFINITY;
+      const int tw = threadIdx.x & 127;
+      float4* xo = reinterpret_cast<float4*>(smem_f(sX + (uint32_t)(2 * wg + hq) * 8192u));
+      const float4* xi = reinterpret_cast<const float4*>(smem_f(sX + (uint32_t)(2 * (1 - wg) + hq) * 8192u));
+#pragma unroll
+      for (int j = 0; j < 4; ++j) {                   // fragment indices stay compile-time: select, do not index by wg
+        const int a = 4 * j, c = 16 + 4 * j;
+        xo[j * 128 + tw] = wg ? make_float4(dq[a], dq[a + 1], dq[a + 2], dq[a + 3]) : make_float4(dq[c], dq[c + 1], dq[c + 2], dq[c + 3]);
       }
-      asm volatile("bar.sync 1, 256;" ::: "memory");
+      ptx::named_bar_sync(3, 256);
+      float sum[16];
+#pragma unroll
+      for (int j = 0; j < 4; ++j) {
+        const float4 o = xi[j * 128 + tw];
+        const int a = 4 * j, c = 16 + 4 * j;
+        sum[4 * j] = o.x + (wg ? dq[c] : dq[a]);
+        sum[4 * j + 1] = o.y + (wg ? dq[c + 1] : dq[a + 1]);
+        sum[4 * j + 2] = o.z + (wg ? dq[c + 2] : dq[a + 2]);
+        sum[4 * j + 3] = o.w + (wg ? dq[c + 3] : dq[a + 3]);
+      }
+#pragma unroll
+      for (int r = 0; r < 2; ++r) {
+        const int q = i * BQ + hq * 64 + (warp & 3) * 16 + g + 8 * r;
+        if (q < p.Tq) {
+          float* dq_row = p.dq_acc + ((int64_t)b * p.Tq + q) * p.dq_ld + h * DH + wg * 32 + 2 * qd;
+#pragma unroll
+          for (int c8 = 0; c8 < 4; ++c8) red_add_v2(dq_row + 8 * c8, sum[4 * c8 + 2 * r] * p.alpha, sum[4 * c8 + 2 * r + 1] * p.alpha);
+        }
+      }
     }
-    const float kbias[2] = {btab[krow0], btab[krow0 + 8]};
-    const int key[2] = {jb * BKV + krow0, jb * BKV + krow0 + 8};
-    const uint32_t sK_wg = sK + (uint32_t)wg * 8192u, sV_wg = sV + (uint32_t)wg * 8192u;
-    const uint32_t sdS_wg = sdS + (uint32_t)wg * 16384u;
-    float dv[32], dk[32];
-#pragma unroll
-    for (int i = 0; i < 32; ++i) { dv[i] = 0.f; dk[i] = 0.f; }
-    ptx::mbar_wait(kv_full, 0);
-    for (int i = 0; i < nq; ++i) {
-      const int st = i & 1;
-      const uint32_t q_s = sQ + st * kTile16K, do_s = sdO + st * kTile16K;
-      ptx::mbar_wait(qdo_full(st), ((uint32_t)i >> 1) & 1u);
-#pragma unroll
-      for (int hq = 0; hq < 2; ++hq) {                // the 128 queries of the tile in two halves of 64
-        const uint32_t q_h = q_s + (uint32_t)hq * 8192u, do_h = do_s + (uint32_t)hq * 8192u;
-        // S^T = K Q^T ; dP^T = V dO^T   ([64 keys x 64 queries] each)
-        float st_[32], dpt[32];
-#pragma unroll
-        for (int t = 0; t < 32; ++t) { st_[t] = 0.f; dpt[t] = 0.f; }
-        ptx::fence_acc(st_); ptx::fence_acc(dpt);
-        ptx::wgmma_fence();
-#pragma unroll
-        for (int k = 0; k < DH / 16; ++k)
-          ptx::WgmmaSS<64, BF, 0, 0>::mma(st_, ptx::desc_kmajor(sK_wg, k), ptx::desc_kmajor(q_h, k), k > 0 ? 1 : 0);
-#pragma unroll
-        for (int k = 0; k < DH / 16; ++k)
-          ptx::WgmmaSS<64, BF, 0, 0>::mma(dpt, ptx::desc_kmajor(sV_wg, k), ptx::desc_kmajor(do_h, k), k > 0 ? 1 : 0);
-        ptx::wgmma_commit();
-        ptx::wgmma_wait<0>();
-        ptx::fence_acc(st_); ptx::fence_acc(dpt);
-        uint32_t p16[4][4], ds16[4][4];
-        const uint32_t ds_buf = sdS_wg + (uint32_t)hq * 8192u;
-#pragma unroll
-        for (int c8 = 0; c8 < 8; ++c8) {
-          const int q0 = i * BQ + hq * 64 + 8 * c8 + 2 * qd;
-          float lse2[2], Dq[2]; int64_t bit0[2]; bool qv[2];
-#pragma unroll
-          for (int e = 0; e < 2; ++e) {
-            const int q = q0 + e;
-            qv[e] = q < p.Tq;
-            const int64_t row_g = ((int64_t)b * p.H + h) * p.Tq + q;
-            Dq[e] = qv[e] ? __ldg(p.dvec + row_g) : 0.f;
-            lse2[e] = qv[e] ? __ldg(p.lse + row_g) * kLog2e : INFINITY;      // +inf on padding rows => P = 0
-            bit0[e] = row_g * p.Tkp;
-          }
-#pragma unroll
-          for (int r = 0; r < 2; ++r) {
-            float pd[2], ds[2];
-#pragma unroll
-            for (int e = 0; e < 2; ++e) {
-              float x = fmaf(st_[4 * c8 + 2 * r + e], a2, kbias[r]);
-              if (CAUSAL) x = (key[r] > q0 + e + (p.Tk - p.Tq)) ? x + cmask : x;
-              const float pr = ex2_approx(x - lse2[e]);
-              bool kp = true;
-              if (use_drop) kp = (load_keep8(p.drop, qv[e], bit0[e], key[r] & ~7, p.Tkp, thresh) >> (key[r] & 7)) & 1u;
-              const float dpv = kp ? dpt[4 * c8 + 2 * r + e] : 0.f;
-              pd[e] = kp ? pr : 0.f;
-              ds[e] = pr * fmaf(dpv, dscale, -Dq[e]);
-            }
-            const uint32_t pp = pack_bf16(pd[0], pd[1]), dd = pack_bf16(ds[0], ds[1]);
-            p16[c8 >> 1][(c8 & 1) * 2 + r] = pp;
-            ds16[c8 >> 1][(c8 & 1) * 2 + r] = dd;
-            // dS^T -> shared memory, MN-major A operand of dQ = dS K: row = key (128 B = 64 queries), 128B swizzle
-            const int kr = krow0 - wg * 64 + 8 * r;
-            const uint32_t addr = ds_buf + (uint32_t)kr * 128u + ((uint32_t)(c8 ^ (kr & 7)) << 4) + (uint32_t)qd * 4u;
-            asm volatile("st.shared.b32 [%0], %1;" ::"r"(addr), "r"(dd) : "memory");
-          }
-        }
-        ptx::fence_proxy_async_smem();       // dS^T (generic-proxy writes) -> visible to the tensor-core (async) proxy
-        asm volatile("bar.sync %0, 128;" ::"r"(2 + wg) : "memory");
-        // dV += P^T dO ; dK += dS^T Q (contraction over the 64 queries) ; dQ[64 queries x 64] = dS K (over this warpgroup's 64 keys)
-        float dq[32];
-#pragma unroll
-        for (int t = 0; t < 32; ++t) dq[t] = 0.f;
-        ptx::fence_acc(dv); ptx::fence_acc(dk); ptx::fence_acc(dq);
-        ptx::wgmma_fence();
-#pragma unroll
-        for (int k = 0; k < 4; ++k) {
-          ptx::WgmmaRS<DH, BF, 1>::mma(dv, p16[k], ptx::desc_mnmajor(do_h, k), 1);
-          ptx::WgmmaRS<DH, BF, 1>::mma(dk, ds16[k], ptx::desc_mnmajor(q_h, k), 1);
-          ptx::WgmmaSS<DH, BF, 1, 1>::mma(dq, ptx::desc_mnmajor(ds_buf, k), ptx::desc_mnmajor(sK_wg, k), k > 0 ? 1 : 0);
-        }
-        ptx::wgmma_commit();
-        ptx::wgmma_wait<0>();
-        ptx::fence_acc(dv); ptx::fence_acc(dk); ptx::fence_acc(dq);
-        // dQ rows of this half: fp32 reduction across kv blocks and warpgroups
-#pragma unroll
-        for (int r = 0; r < 2; ++r) {
-          const int q = i * BQ + hq * 64 + (warp & 3) * 16 + g + 8 * r;
-          if (q < p.Tq) {
-            float* dq_row = p.dq_acc + ((int64_t)b * p.Tq + q) * p.dq_ld + h * DH + 2 * qd;
-#pragma unroll
-            for (int c8 = 0; c8 < 8; ++c8) red_add_v2(dq_row + 8 * c8, dq[4 * c8 + 2 * r] * p.alpha, dq[4 * c8 + 2 * r + 1] * p.alpha);
-          }
-        }
-      }
+    if (hq == 1) {
       if (lane == 0) ptx::mbar_arrive(qdo_empty(st));
+      if (producer && i + 2 < nq) {
+        ptx::mbar_wait(qdo_empty(st), ((uint32_t)i >> 1) & 1u);
+        load_tile(i + 2);
+      }
+      __syncwarp();
     }
-    // ---- dV, dK of this warpgroup's keys ----
+  }
+  ptx::wgmma_wait<0>();      // nothing is pending after the last unit; ptxas cannot tell, and would insert this wait itself
+  ptx::fence_acc(dv); ptx::fence_acc(dk);
+  // ---- dV, dK of this warpgroup's keys ----
 #pragma unroll
-    for (int r = 0; r < 2; ++r) {
-      if (key[r] < p.Tk) {
-        uint16_t* dv_row = p.dv + ((int64_t)b * p.Tk + key[r]) * p.dv_ld + h * DH + 2 * qd;
-        uint16_t* dk_row = p.dk + ((int64_t)b * p.Tk + key[r]) * p.dk_ld + h * DH + 2 * qd;
+  for (int r = 0; r < 2; ++r) {
+    if (key[r] < p.Tk) {
+      uint16_t* dv_row = p.dv + ((int64_t)b * p.Tk + key[r]) * p.dv_ld + h * DH + 2 * qd;
+      uint16_t* dk_row = p.dk + ((int64_t)b * p.Tk + key[r]) * p.dk_ld + h * DH + 2 * qd;
 #pragma unroll
-        for (int c8 = 0; c8 < 8; ++c8) {
-          *reinterpret_cast<uint32_t*>(dv_row + 8 * c8) = pack_bf16(dv[4 * c8 + 2 * r] * dscale, dv[4 * c8 + 2 * r + 1] * dscale);
-          *reinterpret_cast<uint32_t*>(dk_row + 8 * c8) = pack_bf16(dk[4 * c8 + 2 * r] * p.alpha, dk[4 * c8 + 2 * r + 1] * p.alpha);
-        }
+      for (int c8 = 0; c8 < 8; ++c8) {
+        *reinterpret_cast<uint32_t*>(dv_row + 8 * c8) = pack_bf16(dv[4 * c8 + 2 * r] * dscale, dv[4 * c8 + 2 * r + 1] * dscale);
+        *reinterpret_cast<uint32_t*>(dk_row + 8 * c8) = pack_bf16(dk[4 * c8 + 2 * r] * p.alpha, dk[4 * c8 + 2 * r + 1] * p.alpha);
       }
     }
   }
 }
 
-constexpr size_t kBwdSmem = 1024 + (size_t)(2 + 2 + 2 + 2) * kTile16K + 128 + 512 + 64;
+constexpr size_t kBwdSmem = 1024 + (size_t)(2 + 2 + 2 + 2 + 2 + 2) * kTile16K + 2048 + 512 + 64;
 
 // One warp per (b, q) row: zero the fp32 dQ accumulator row and compute D[b,h,q] = sum_c dO[b,q,h,c] * O[b,q,h,c].
 template <int DT>
@@ -615,7 +682,7 @@ int attention_bwd_fused(int dt, const void* q, int64_t q_ld, const void* k, int6
   dim3 grid((Tk + BKV - 1) / BKV, H, B);
   auto kern = causal ? (dt == F16 ? attn_bwd_kernel<true, F16> : attn_bwd_kernel<true, BF16>)
                      : (dt == F16 ? attn_bwd_kernel<false, F16> : attn_bwd_kernel<false, BF16>);
-  launch_pdl(kern, grid, kAttnThreads, kBwdSmem, s, tq, tk, tv, tdo, p);
+  launch_pdl(kern, grid, kBwdThreads, kBwdSmem, s, tq, tk, tv, tdo, p);
   B200ST_LAUNCH_CHECK();
   const int64_t n8 = rows * (H * DH / 8);
   int64_t g = (n8 + 255) / 256;
