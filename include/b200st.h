@@ -158,7 +158,10 @@ int64_t b200st_encode_workspace_bytes(b200st_handle h, int32_t B, int32_t T);
  *   cross_kv  fp32 [dec_layers][B][Tm][2d]: memory keys | values, projected once (transformer_layers.py:156-170)
  *   self_kv   fp32 [dec_layers][2][B][max_len][d]: self-attention key / value cache (multi_head_attention.py:271-289)
  *   scratch   b200st_decode_scratch_floats(h, B) floats
- * use_shadow 0: weights read from the fp32 master arena (token ids identical to an fp32 reference); 1: 16-bit shadow. */
+ * use_shadow 0: weights read from the fp32 master arena (token ids identical to an fp32 reference); 1: the handle's
+ *   16-bit shadow (half the bytes) for trg.emb (embedding and tied logits) and, per decoder layer, self.qkv.kernel,
+ *   self.out.kernel, cross.q.kernel, cross.out.kernel, ffn.w1 and ffn.w2.  Biases, LayerNorm parameters and the
+ *   cross-attention K/V projection (b200st_decode_init) always use the fp32 master arena; all arithmetic is fp32. */
 typedef struct {
   int32_t B, Tm, max_len;
   float* cross_kv; float* self_kv;

@@ -177,13 +177,6 @@ def test_cfg5_beam_token_ids_exact():
           (ref["steps"], int(ref["length"][0]), n_distinct, ref["gap"], float(ref["scores"][0]), float(scores[0])))
     _check(ref, ids, scores, length, min_gap=5e-6, rtol=2e-3)
     assert n_distinct >= 8, "degenerate hypothesis: the test would not exercise the context dependence"
-    rt16 = U.speech_runtime(cfg, "fp16")
-    rt16.load_parameters(P)
-    ids16, _, _, _ = D.beam_search(rt16, dict(src=src, src_length=lens), bos, eos, unk, beam_size=4, length_penalty=-1.0,
-                                   maximum_decode_length=200, extra_decode_length=50, use_shadow=True)
-    agree = int((ids16.cpu()[0] == ref["hypotheses"][0]).long().cumprod(0).sum())
-    print("[cfg-5 beam 4] fp16 weights: first %d of %d tokens identical to the fp32 oracle" % (agree, ref["hypotheses"].shape[1]))
-    assert agree >= 1
 
 
 def test_predict_with_beam_search_through_the_entry(tmp_path):
