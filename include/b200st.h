@@ -161,7 +161,14 @@ int64_t b200st_encode_workspace_bytes(b200st_handle h, int32_t B, int32_t T);
  * use_shadow 0: weights read from the fp32 master arena (token ids identical to an fp32 reference); 1: the handle's
  *   16-bit shadow (half the bytes) for trg.emb (embedding and tied logits) and, per decoder layer, self.qkv.kernel,
  *   self.out.kernel, cross.q.kernel, cross.out.kernel, ffn.w1 and ffn.w2.  Biases, LayerNorm parameters and the
- *   cross-attention K/V projection (b200st_decode_init) always use the fp32 master arena; all arithmetic is fp32. */
+ *   cross-attention K/V projection (b200st_decode_init) always use the fp32 master arena; all arithmetic is fp32.
+ * Rows per step (B, or B*beam_size in beam search): 1..8 with use_shadow 0; 1..B200ST_DECODE_MAX_ROWS with use_shadow 1.
+ *   Above 8 rows the step runs its projections on the tensor cores: each fp32 activation is split into a sum of 16-bit
+ *   terms (2 for fp16, 3 for bf16) multiplied by the same 16-bit weights with fp32 accumulation, so the step keeps the
+ *   contract above (and needs d, ffn multiples of 64 and vocab a multiple of 8).  With fp16 weights every activation
+ *   entering a projection must lie within the fp16 range, as in the reference's mixed_float16.  That step uses no
+ *   floating-point atomics: it is bit-reproducible, and a row's result does not depend on the other rows of the step. */
+#define B200ST_DECODE_MAX_ROWS 256
 typedef struct {
   int32_t B, Tm, max_len;
   float* cross_kv; float* self_kv;
@@ -184,10 +191,11 @@ typedef struct {
   const int64_t* bos_ids;
   int32_t eos_id, unk_id, min_len, max_steps;
   int64_t* out_ids; int32_t* out_len; float* out_logprob;
-  void* state_words;            /* >= 256 bytes of device memory */
+  void* state_words;            /* >= 256 bytes of device memory for B <= 8; above 8 rows
+                                 * b200st_beam_state_bytes(h, B, 1, st->max_len) bytes */
   int32_t use_graph;            /* 2: ONE persistent cooperative kernel for the whole search (grid-wide barriers between the
-                                 * phases of a token; falls back to 1 when the grid cannot be co-scheduled); 1: one captured
-                                 * CUDA graph of ~40 kernels replayed per token; 0: eager launches */
+                                 * phases of a token; falls back to 1 when the grid cannot be co-scheduled, and always above
+                                 * 8 rows); 1: one captured CUDA graph of ~40 kernels replayed per token; 0: eager launches */
 } b200st_greedy_args;
 int b200st_greedy_search(b200st_handle h, const b200st_buffers* buf, const b200st_decode_state* st, const b200st_greedy_args* a,
                          void* stream);
@@ -199,13 +207,14 @@ int32_t b200st_greedy_used_graph(void);
  * ties), then the top_k beams of each utterance by logprob * penalty(length), best first.
  *   st->B counts UTTERANCES: cross_kv and memory_bias are b200st_decode_init's for the B utterances (the memory is not
  *   tiled per beam), while self_kv [dec_layers][2][B*beam_size][max_len][d] and scratch
- *   (b200st_decode_scratch_floats(h, B*beam_size) floats) are sized for B*beam_size rows.  B*beam_size <= 8.
+ *   (b200st_decode_scratch_floats(h, B*beam_size) floats) are sized for B*beam_size rows.  B*beam_size <= 8 with
+ *   st->use_shadow 0, <= B200ST_DECODE_MAX_ROWS with use_shadow 1; beam_size <= 8.
  *   out_ids [B*top_k][max_steps] padded with EOS, out_scores / out_logprob / out_len [B*top_k], utterance-major.
  *   state_words: b200st_beam_state_bytes(h, B, beam_size, st->max_len) bytes of device memory.
  *   use_graph: 1 = the step captured once into a CUDA graph and replayed, 0 = eager launches.  beam_size == 1 is the greedy
  *   search (b200st_greedy_search, where use_graph 2 selects its persistent kernel) with the score computed from its result.
- * Invalid arguments (B*beam_size > 8, top_k outside 1..beam_size, max_steps > max_len, null buffers) fail before anything is
- * launched. */
+ * Invalid arguments (too many rows, beam_size > 8, top_k outside 1..beam_size, max_steps > max_len, null buffers) fail
+ * before anything is launched. */
 typedef struct {
   const int64_t* bos_ids;       /* [B] */
   int32_t eos_id, unk_id, min_len, max_steps;

@@ -17,7 +17,8 @@ summary_steps, save_checkpoint_steps, update_cycle, clip_value, clip_norm, crite
 lr_schedule.params, pretrain_model}, dataset.class AudioTFRecordDataset / dataset.params, task.class SpeechToText /
 task.params, model.class / model.params / hparams_set, model_dir, dtype, and for `predict` the keys of the prediction
 recipes: `entry: predict` (the alias of entry.class) and search_method beam_search / search_method.params {beam_size,
-length_penalty, top_k, maximum_decode_length, extra_decode_length, minimum_decode_length, enable_unk}.  Transcripts must already be token ids (the
+length_penalty, top_k, maximum_decode_length, extra_decode_length, minimum_decode_length, enable_unk}, and the top-level
+batch_size (utterances per call; with a 16-bit dtype decoded from the 16-bit weights).  Transcripts must already be token ids (the
 reference's `create_tfrecords` with a projected transcript): its tokenizers / BPE are outside this path and raw text is
 refused with that message.  Checkpoints are NumPy archives keyed by the reference's variable names (checkpoints.py).
 """
@@ -217,6 +218,8 @@ def resolve(cfg, world=1):
         "search": search,
         "output_file": cfg.get("output_file") or ep.get("output_file"),
     }
+    if cfg.get("batch_size") is not None:     # prediction recipes: utterances per batch (SequenceGenerator)
+        plan["batch_size"] = int(cfg["batch_size"])
     if search_method:
         plan["search_method"] = search_method
     return plan
@@ -361,7 +364,7 @@ def ids_to_text(ids, eos_id, tokens):
 
 def predict(plan):
     from neurst_b200 import checkpoints as CK
-    from neurst_b200.decode import MAX_ROWS
+    from neurst_b200.decode import MAX_ROWS, MAX_ROWS_SHADOW
     world, rank, _ = _dist_setup()
     model = _build_model(plan)
     path, step = latest_checkpoint(plan["model_dir"])
@@ -374,9 +377,24 @@ def predict(plan):
     hyps = []
     group = []
     beam = plan.get("search_method") == "beam_search"
-    per_call = MAX_ROWS // plan["search"]["beam_size"] if beam else MAX_ROWS
+    width = plan["search"]["beam_size"] if beam else 1
+    per_call = MAX_ROWS // width
     if per_call < 1:
         raise SystemExit("beam_size %d exceeds the %d rows a decoding step holds" % (plan["search"]["beam_size"], MAX_ROWS))
+    # the recipes' batch_size (utterances per batch): with 16-bit weights the batch is decoded in one call from the 16-bit
+    # shadow, up to MAX_ROWS_SHADOW rows (utterances x beam) per step; the fp32 weights hold MAX_ROWS rows per step
+    search_kw = dict(plan["search"])
+    if plan.get("batch_size") is not None:
+        if plan["precision"] == "fp32":
+            LOG.info("predict: dtype float32 decodes %d utterance(s) per call (at most %d rows per step), not batch_size %d",
+                     min(per_call, plan["batch_size"]), MAX_ROWS, plan["batch_size"])
+            per_call = min(per_call, plan["batch_size"])
+        else:
+            if not 1 <= plan["batch_size"] * width <= MAX_ROWS_SHADOW:
+                raise SystemExit("batch_size %d x beam_size %d exceeds the %d rows a decoding step holds"
+                                 % (plan["batch_size"], width, MAX_ROWS_SHADOW))
+            per_call = plan["batch_size"]
+            search_kw["use_shadow"] = True
 
     def flush():
         if not group:
@@ -388,7 +406,7 @@ def predict(plan):
         batch = task.example_to_input({"audio": src, "audio_length": torch.tensor([int(e["audio_length"]) for e in group])}, infer=True)
         search = model.beam_search if beam else model.greedy_search
         # beam search: top_k rows per utterance, consecutive (the reference's [B*top_k] order)
-        ids, score = search({"src": batch["src"], "src_length": batch["src_length"]}, **plan["search"])
+        ids, score = search({"src": batch["src"], "src_length": batch["src_length"]}, **search_kw)
         for row, lp in zip(ids.cpu().tolist(), score.cpu().tolist()):
             hyps.append((ids_to_text(row, tm["eos_id"], tm.get("tokens")), lp))
         group.clear()

@@ -95,6 +95,29 @@ __device__ __forceinline__ float warp_max(float v) {
   for (int o = 16; o > 0; o >>= 1) v = fmaxf(v, __shfl_xor_sync(0xffffffffu, v, o));
   return v;
 }
+// block-wide sum / max (every thread gets the result); sm: >= 32 floats of shared memory.  Fixed reduction order.
+__device__ __forceinline__ float block_sum(float v, float* sm) {
+  v = warp_sum(v);
+  const int lane = threadIdx.x & 31, w = threadIdx.x >> 5, nw = (blockDim.x + 31) >> 5;
+  __syncthreads();
+  if (lane == 0) sm[w] = v;
+  __syncthreads();
+  float t = (threadIdx.x < nw) ? sm[threadIdx.x] : 0.f;
+  if (w == 0) { t = warp_sum(t); if (lane == 0) sm[0] = t; }
+  __syncthreads();
+  return sm[0];
+}
+__device__ __forceinline__ float block_max(float v, float* sm) {
+  v = warp_max(v);
+  const int lane = threadIdx.x & 31, w = threadIdx.x >> 5, nw = (blockDim.x + 31) >> 5;
+  __syncthreads();
+  if (lane == 0) sm[w] = v;
+  __syncthreads();
+  float t = (threadIdx.x < nw) ? sm[threadIdx.x] : -INFINITY;
+  if (w == 0) { t = warp_max(t); if (lane == 0) sm[0] = t; }
+  __syncthreads();
+  return sm[0];
+}
 
 // ---- counter-based RNG for dropout: Philox4x32-7 ---------------------------------------
 // (7 rounds: the smallest round count of Philox4x32 that Salmon et al. report as passing BigCrush; the generator of all

@@ -18,6 +18,10 @@
 //
 // Weights are read either from the fp32 master arena (token ids identical to an fp32 reference) or from the 16-bit
 // shadow (half the bytes).  All arithmetic and both caches are fp32.
+//
+// Steps of more than 8 rows (shadow only, up to 256) take the wide step of decode_rows.cu instead of these GEMV kernels;
+// the embedding, the searches' selection / bookkeeping kernels and the token loop are shared.
+#include "decode_rows.cuh"
 #include "model.cuh"
 #include "pdl.cuh"
 
@@ -32,29 +36,6 @@ constexpr int MAXB = 8;        // rows per step (batch x beam = batch for greedy
 constexpr float kFloatMin = -1.0e9f;
 
 template <typename TW> __device__ __forceinline__ float wf(const TW* p, int64_t i) { return to_f32(p[i]); }
-
-__device__ __forceinline__ float block_sum(float v, float* sm) {
-  v = warp_sum(v);
-  const int lane = threadIdx.x & 31, w = threadIdx.x >> 5, nw = (blockDim.x + 31) >> 5;
-  __syncthreads();
-  if (lane == 0) sm[w] = v;
-  __syncthreads();
-  float t = (threadIdx.x < nw) ? sm[threadIdx.x] : 0.f;
-  if (w == 0) { t = warp_sum(t); if (lane == 0) sm[0] = t; }
-  __syncthreads();
-  return sm[0];
-}
-__device__ __forceinline__ float block_max(float v, float* sm) {
-  v = warp_max(v);
-  const int lane = threadIdx.x & 31, w = threadIdx.x >> 5, nw = (blockDim.x + 31) >> 5;
-  __syncthreads();
-  if (lane == 0) sm[w] = v;
-  __syncthreads();
-  float t = (threadIdx.x < nw) ? sm[threadIdx.x] : -INFINITY;
-  if (w == 0) { t = warp_max(t); if (lane == 0) sm[0] = t; }
-  __syncthreads();
-  return sm[0];
-}
 
 __device__ __forceinline__ float sinusoid_at(int t, int c, int d) {   // common_layers.py:400-408 (concat(sin, cos))
   const int half = d / 2;
@@ -941,8 +922,24 @@ int step_launch(const StepCtx& c, const TW* wbase, const int64_t* ids, const int
   return 0;
 }
 
+// More than 8 rows: the embedding of the current symbols into x (scratch offset 0), then the wide step (decode_rows.cu).
+// rows_check has run before.
+int step_rows(const StepCtx& c, const int64_t* ids, const int32_t* time_dev, float* logits_out, const int* anc, int beam) {
+  const Config& cf = c.m.cfg;
+  const int n = c.st.B * cf.d;
+  if (c.m.adt == F16)
+    launch_pdl(embed_step_kernel<__half>, (n + 255) / 256, 256, 0, c.s, ids, reinterpret_cast<const __half*>(c.buf.shadow) + c.off("trg.emb"),
+               c.st.scratch, c.st.B, cf.d, cf.vocab, time_dev);
+  else
+    launch_pdl(embed_step_kernel<__nv_bfloat16>, (n + 255) / 256, 256, 0, c.s, ids,
+               reinterpret_cast<const __nv_bfloat16*>(c.buf.shadow) + c.off("trg.emb"), c.st.scratch, c.st.B, cf.d, cf.vocab, time_dev);
+  ++g_kernel_launches;
+  return rows_step(c.m, c.buf, c.st, time_dev, logits_out, anc, beam, c.s);
+}
+
 int step_dispatch(const StepCtx& c, const int64_t* ids, const int32_t* time_dev, float* logits_out, const int* anc = nullptr,
                   int beam = 1) {
+  if (c.st.B > MAXB) return step_rows(c, ids, time_dev, logits_out, anc, beam);
   if (c.st.use_shadow) {
     B200ST_CHECK(is16(c.m.adt) && c.buf.shadow, "use_shadow needs a 16-bit precision handle and its shadow arena");
     if (c.m.adt == F16) return step_launch(c, reinterpret_cast<const __half*>(c.buf.shadow), ids, time_dev, logits_out, anc, beam);
@@ -1046,7 +1043,8 @@ int launch_persistent(const Model& m, const Buffers& buf, const DecodeState& st,
 int check_state(const Model& m, const DecodeState& st) {
   const Config& cf = m.cfg;
   B200ST_CHECK(cf.model_type == MODEL_SPEECH || cf.model_type == MODEL_TEXT, "decoding needs an encoder-decoder handle");
-  B200ST_CHECK(st.B >= 1 && st.B <= MAXB, "decode batch must be 1.." + std::to_string(MAXB));
+  const int max_rows = st.use_shadow ? kDecodeMaxRows : MAXB;      // more than 8 rows: the wide step, 16-bit shadow only
+  B200ST_CHECK(st.B >= 1 && st.B <= max_rows, "decode batch must be 1.." + std::to_string(max_rows));
   B200ST_CHECK(st.max_len >= 1 && st.Tm >= 0, "bad decode lengths");
   B200ST_CHECK(st.self_kv && st.scratch && (st.Tm == 0 || st.cross_kv), "decode state buffers missing");
   const int dh = cf.d / cf.heads;
@@ -1075,7 +1073,7 @@ int raise_all_smem(const Config& cf, const DecodeState& st) {
 static int g_last_greedy_graph = -1;
 int last_greedy_used_graph() { return g_last_greedy_graph; }
 
-int64_t decode_scratch_floats(const Model& m, int B) { return layout_of(m.cfg, B).total + 64; }
+int64_t decode_scratch_floats(const Model& m, int B) { return B > MAXB ? rows_scratch_floats(m.cfg, B) : layout_of(m.cfg, B).total + 64; }
 
 // memorize_memory (transformer_layers.py:156-160): K/V projections of the encoder output, once per utterance, fp32
 int decode_init(const Model& m, const Buffers& buf, const float* enc_out, const DecodeState& st, cudaStream_t s) {
@@ -1104,6 +1102,7 @@ int decode_step(const Model& m, const Buffers& buf, const DecodeState& st, const
                 float* logits, cudaStream_t s) {
   B200ST_TRY(check_state(m, st));
   B200ST_CHECK(symbols && time_dev && logits, "decode_step: null argument");
+  if (st.B > MAXB) B200ST_TRY(rows_check(m, buf, st, 1));
   B200ST_TRY(raise_all_smem(m.cfg, st));
   StepCtx c{m, buf, st, s};
   return step_dispatch(c, symbols, time_dev, logits);
@@ -1116,22 +1115,26 @@ int greedy_search(const Model& m, const Buffers& buf, const DecodeState& st, con
   const Config& cf = m.cfg;
   B200ST_CHECK(ga.max_steps >= 1 && ga.max_steps <= st.max_len, "max_steps must be within the cache length");
   B200ST_CHECK(ga.bos_ids && ga.out_ids && ga.out_len && ga.out_logprob && ga.state_words, "greedy_search: null argument");
+  const bool wide = st.B > MAXB;
+  if (wide) B200ST_TRY(rows_check(m, buf, st, 1));
   B200ST_TRY(raise_all_smem(cf, st));
-  // device words: [ids B x int64][finished B][length B][time][all_finished]
+  // device words: [ids x int64][finished][time][all_finished] with 8 row slots, or B row slots and a [ticket] above 8 rows
   char* w = reinterpret_cast<char*>(ga.state_words);
+  const int nw = wide ? st.B : MAXB;
   GreedyState g{};
-  g.ids = reinterpret_cast<int64_t*>(w); w += sizeof(int64_t) * MAXB;
-  g.finished = reinterpret_cast<int32_t*>(w); w += sizeof(int32_t) * MAXB;
+  g.ids = reinterpret_cast<int64_t*>(w); w += sizeof(int64_t) * nw;
+  g.finished = reinterpret_cast<int32_t*>(w); w += sizeof(int32_t) * nw;
   g.length = ga.out_len;
   g.logprob = ga.out_logprob;
   g.out = ga.out_ids;
   g.time = reinterpret_cast<int32_t*>(w); w += sizeof(int32_t);
-  g.all_finished = reinterpret_cast<int32_t*>(w);
-  const DecodeLayout lo = layout_of(cf, st.B);
-  float* logits = st.scratch + lo.logits;
+  g.all_finished = reinterpret_cast<int32_t*>(w); w += sizeof(int32_t);
+  uint32_t* ticket = reinterpret_cast<uint32_t*>(w);
+  float* logits = st.scratch + (wide ? rows_logits_offset(cf, st.B) : layout_of(cf, st.B).logits);
   greedy_init_kernel<<<8, 256, 0, s>>>(g, ga.bos_ids, st.B, ga.max_steps, ga.eos_id);
   B200ST_CUDA(cudaGetLastError());
-  if (ga.use_graph == 2) {       // persistent mode: one cooperative launch for the whole search
+  if (wide) B200ST_CUDA(cudaMemsetAsync(ticket, 0, sizeof(uint32_t), s));
+  if (ga.use_graph == 2 && !wide) {       // persistent mode: one cooperative launch for the whole search
     bool done = false;
     if (st.use_shadow) {
       B200ST_CHECK(is16(m.adt) && buf.shadow, "use_shadow needs a 16-bit precision handle and its shadow arena");
@@ -1145,8 +1148,13 @@ int greedy_search(const Model& m, const Buffers& buf, const DecodeState& st, con
   StepCtx c{m, buf, st, s};
   auto one_step = [&]() -> int {
     B200ST_TRY(step_dispatch(c, g.ids, g.time, logits));
-    launch_pdl(greedy_pick_kernel, 1, 1024, 0, s, (const float*)logits, g, st.B, cf.vocab, ga.eos_id, ga.unk_id, ga.min_len, ga.max_steps);
-    ++g_kernel_launches;
+    if (wide) {
+      rows_greedy_pick(logits, g.ids, g.finished, g.length, g.logprob, g.out, g.time, g.all_finished, ticket, st.B, cf.vocab, ga.eos_id,
+                       ga.unk_id, ga.min_len, ga.max_steps, s);
+    } else {
+      launch_pdl(greedy_pick_kernel, 1, 1024, 0, s, (const float*)logits, g, st.B, cf.vocab, ga.eos_id, ga.unk_id, ga.min_len, ga.max_steps);
+      ++g_kernel_launches;
+    }
     B200ST_LAUNCH_CHECK();
     return 0;
   };
@@ -1171,8 +1179,11 @@ int beam_search(const Model& m, const Buffers& buf, const DecodeState& st, const
   const int beam = a.beam_size;
   B200ST_CHECK(beam >= 1, "beam_size must be >= 1");
   B200ST_CHECK(a.top_k >= 1 && a.top_k <= beam, "top_k must be in 1..beam_size");
-  B200ST_CHECK((int64_t)st.B * beam <= MAXB, "beam search decodes at most " + std::to_string(MAXB) + " rows (utterances x beam_size) per call, got " +
-                                              std::to_string(st.B) + " x " + std::to_string(beam));
+  const int max_rows = st.use_shadow ? kDecodeMaxRows : MAXB;      // more than 8 rows: the wide step, 16-bit shadow only
+  B200ST_CHECK((int64_t)st.B * beam <= max_rows, "beam search decodes at most " + std::to_string(max_rows) +
+                                                 " rows (utterances x beam_size) per call, got " + std::to_string(st.B) + " x " +
+                                                 std::to_string(beam));
+  B200ST_CHECK(beam <= KMAX, "beam_size must be at most " + std::to_string(KMAX));
   B200ST_CHECK(beam <= cf.vocab, "beam_size exceeds the vocabulary");
   B200ST_CHECK(a.max_steps >= 1 && a.max_steps <= st.max_len, "max_steps must be within the cache length");
   B200ST_CHECK(a.bos_ids && a.out_ids && a.out_scores && a.out_len && a.out_logprob && a.state_words, "beam_search: null argument");
@@ -1182,7 +1193,7 @@ int beam_search(const Model& m, const Buffers& buf, const DecodeState& st, const
     ga.out_ids = a.out_ids; ga.out_len = a.out_len; ga.out_logprob = a.out_logprob; ga.state_words = a.state_words;
     ga.use_graph = a.use_graph;
     B200ST_TRY(greedy_search(m, buf, st, ga, s));
-    beam1_score_kernel<<<1, 32, 0, s>>>(a.out_logprob, a.out_len, a.out_scores, st.B, a.length_penalty);
+    beam1_score_kernel<<<(st.B + 255) / 256, 256, 0, s>>>(a.out_logprob, a.out_len, a.out_scores, st.B, a.length_penalty);
     B200ST_CUDA(cudaGetLastError());
     return 0;
   }
@@ -1190,6 +1201,7 @@ int beam_search(const Model& m, const Buffers& buf, const DecodeState& st, const
   DecodeState rs = st;                    // the step runs on every beam row; cross_kv / memory_bias stay per utterance
   rs.B = rows;
   B200ST_TRY(check_state(m, rs));
+  if (rows > MAXB) B200ST_TRY(rows_check(m, buf, rs, beam));
   const size_t smem_self = self_attn_smem(cf, st.max_len, true);
   B200ST_CHECK(smem_self <= 200 * 1024, "decode: too many keys for the shared-memory score buffer");
   B200ST_TRY(raise_all_smem(cf, st));
@@ -1212,9 +1224,8 @@ int beam_search(const Model& m, const Buffers& buf, const DecodeState& st, const
   bs.ticket = reinterpret_cast<uint32_t*>(w); w += 2 * sizeof(int32_t);
   bs.anc = reinterpret_cast<int32_t*>(w); w += sizeof(int32_t) * (size_t)rows * st.max_len;
   bs.hist = reinterpret_cast<int32_t*>(w);
-  const DecodeLayout lo = layout_of(cf, rows);
-  float* logits = rs.scratch + lo.logits;
-  beam_init_kernel<<<1, 32, 0, s>>>(bs, a.bos_ids, rows, beam);
+  float* logits = rs.scratch + (rows > MAXB ? rows_logits_offset(cf, rows) : layout_of(cf, rows).logits);
+  beam_init_kernel<<<(rows + 255) / 256, 256, 0, s>>>(bs, a.bos_ids, rows, beam);
   B200ST_CUDA(cudaGetLastError());
   StepCtx c{m, buf, rs, s};
   auto one_step = [&]() -> int {

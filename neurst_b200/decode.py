@@ -17,19 +17,26 @@ import torch
 
 from neurst_b200 import lib as L
 
-MAX_ROWS = 8      # rows (batch x beam) per decoding step supported by the decode kernels
+MAX_ROWS = 8      # rows (batch x beam) per decoding step with the fp32 master weights
+MAX_ROWS_SHADOW = 256   # with the 16-bit shadow (use_shadow=True): above 8 rows the step runs on the tensor cores
+
+
+def max_rows(use_shadow):
+    """Rows (utterances x beam) one decoding step holds."""
+    return MAX_ROWS_SHADOW if use_shadow else MAX_ROWS
 
 
 class DecodingCache:
     """`cache` argument of symbols_to_logits_fn: encoder memory (pre-projected per layer) + self-attention K/V.
 
     beam > 1 (beam search): the memory stays one copy per utterance, the self-attention cache and the step scratch hold
-    B * beam rows."""
+    B * beam rows: at most MAX_ROWS with the fp32 weights, MAX_ROWS_SHADOW with use_shadow."""
 
     def __init__(self, rt, B, Tm, max_len, memory_bias, use_shadow=False, beam=1):
         cfg = rt.config
-        if beam < 1 or not 1 <= B * beam <= MAX_ROWS:
-            raise L.B200STError("decoding supports 1..%d rows (utterances x beam) per step, got %d x %d" % (MAX_ROWS, B, beam))
+        limit = max_rows(use_shadow)
+        if beam < 1 or not 1 <= B * beam <= limit:
+            raise L.B200STError("decoding supports 1..%d rows (utterances x beam) per step, got %d x %d" % (limit, B, beam))
         dev = rt.device
         self.rt, self.B, self.Tm, self.max_len, self.beam = rt, B, Tm, max_len, beam
         rows = B * beam
@@ -141,14 +148,18 @@ def greedy_search(rt, inputs, bos_id, eos_id, unk_id=None, maximum_decode_length
     out = torch.empty(B, steps, dtype=torch.int64, device=dev)
     length = torch.zeros(B, dtype=torch.int32, device=dev)
     logprob = torch.zeros(B, dtype=torch.float32, device=dev)
-    words = torch.zeros(64, dtype=torch.int64, device=dev)
+    nbytes = int(rt.lib.b200st_beam_state_bytes(rt.handle, B, 1, cache.max_len))    # >= 512; holds B rows' words
+    if nbytes <= 0:
+        raise L.B200STError("greedy search state sizing failed: " + rt.lib.b200st_last_error().decode())
+    words = torch.zeros((nbytes + 7) // 8, dtype=torch.int64, device=dev)
     a = L.GreedyArgs()
     a.bos_ids, a.eos_id = bos.data_ptr(), int(eos_id)
     a.unk_id = -1 if (enable_unk or unk_id is None) else int(unk_id)
     a.min_len, a.max_steps = int(minimum_decode_length), int(steps)
     a.out_ids, a.out_len, a.out_logprob = out.data_ptr(), length.data_ptr(), logprob.data_ptr()
     # persistent: the whole search is ONE cooperative kernel (grid barriers between the phases of a token); otherwise one
-    # captured CUDA graph of ~40 kernels is replayed per token (use_graph) or every kernel is launched eagerly
+    # captured CUDA graph of ~40 kernels is replayed per token (use_graph) or every kernel is launched eagerly.  Above 8
+    # rows there is no persistent kernel: the library replays the captured graph instead
     a.state_words, a.use_graph = words.data_ptr(), (2 if (persistent and use_graph) else int(bool(use_graph)))
     bufs = _bufs(rt)
     # the library captures the step into a CUDA graph: that needs a real (non-legacy-default) stream
@@ -176,8 +187,8 @@ def beam_search(rt, inputs, bos_id, eos_id, unk_id=None, beam_size=4, length_pen
                 extra_decode_length=50, minimum_decode_length=0, enable_unk=False, use_shadow=False, use_graph=True, cache=None):
     """sequence_beam_search (beam_search.py:254-439) on the device: returns (hypotheses int64 [B*top_k, maximum_decode_length]
     padded with EOS, scores fp32 [B*top_k] = logprob * length penalty, best first per utterance, accumulated log-probabilities
-    [B*top_k], decoding lengths [B*top_k]).  length_penalty < 0 (or None) scores by 1/length.  At most MAX_ROWS // beam_size
-    utterances per call.  beam_size 1 is the greedy search (with its persistent kernel when use_graph)."""
+    [B*top_k], decoding lengths [B*top_k]).  length_penalty < 0 (or None) scores by 1/length.  At most
+    max_rows(use_shadow) // beam_size utterances per call, and beam_size <= 8.  beam_size 1 is the greedy search (with its persistent kernel when use_graph)."""
     beam_size, top_k = int(beam_size), int(top_k)
     if beam_size < 1:
         raise L.B200STError("beam_size must be >= 1, got %d" % beam_size)
@@ -188,9 +199,9 @@ def beam_search(rt, inputs, bos_id, eos_id, unk_id=None, beam_size=4, length_pen
     alpha = -1.0 if length_penalty is None else float(length_penalty)
     if cache is None:
         B = int(inputs["src"].shape[0])
-        if B * beam_size > MAX_ROWS:
+        if B * beam_size > max_rows(use_shadow):
             raise L.B200STError("beam search decodes at most %d rows (utterances x beam_size) per call, got %d x %d"
-                                % (MAX_ROWS, B, beam_size))
+                                % (max_rows(use_shadow), B, beam_size))
         enc, bias = encode(rt, inputs)
         cache = create_decoding_cache(rt, enc, bias, maximum_decode_length, use_shadow, beam=beam_size)
     elif cache.self_kv.shape[2] < cache.B * beam_size:

@@ -200,7 +200,8 @@ class _EncoderDecoder:
     def greedy_search(self, inputs, maximum_decode_length=256, extra_decode_length=50, minimum_decode_length=0, enable_unk=False,
                       use_shadow=False):
         """SequenceGenerator with search_method BeamSearch(beam_size=1) (neurst/exps/sequence_generator.py:62-86,
-        neurst/layers/search/beam_search.py:254-439) on the device: -> (token ids [B, maximum_decode_length], log-probs [B])."""
+        neurst/layers/search/beam_search.py:254-439) on the device: -> (token ids [B, maximum_decode_length], log-probs [B]).
+        At most decode.MAX_ROWS (8) utterances per call with the fp32 weights, decode.MAX_ROWS_SHADOW (256) with use_shadow."""
         from neurst_b200 import decode as D
         tm = self._trg_meta
         B = inputs["src"].shape[0]
@@ -215,7 +216,8 @@ class _EncoderDecoder:
                     minimum_decode_length=0, enable_unk=False, use_shadow=False):
         """SequenceGenerator with search_method BeamSearch (neurst/layers/search/beam_search.py:439-530) on the device:
         -> (hypotheses [B*top_k, maximum_decode_length], scores [B*top_k]), BeamSearch.call's return.  At most
-        decode.MAX_ROWS // beam_size utterances per call."""
+        decode.MAX_ROWS // beam_size utterances per call with the fp32 weights, decode.MAX_ROWS_SHADOW // beam_size with
+        use_shadow (the 16-bit weights; beam_size <= 8)."""
         from neurst_b200 import decode as D
         tm = self._trg_meta
         B = inputs["src"].shape[0]
