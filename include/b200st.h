@@ -227,6 +227,28 @@ typedef struct {
 int64_t b200st_beam_state_bytes(b200st_handle h, int32_t B, int32_t beam_size, int32_t max_len);
 int b200st_beam_search(b200st_handle h, const b200st_buffers* buf, const b200st_decode_state* st, const b200st_beam_args* a,
                        void* stream);
+/* Ensemble decoding: sequence_beam_search over EncoderDecoderEnsembleModel (neurst/models/encoder_decoder_ensemble_model.py;
+ * neurst/layers/search/beam_search.py:97-115,486-515).  Per step every member runs its decoder step on the same rows, and the
+ * search continues from log(sum_m w_m softmax(logits_m)) (evaluated as a log-sum-exp over the members) with the masks,
+ * scores and outputs of b200st_beam_search.
+ *   members[m]: a handle, its buffers and its decode state, each as for b200st_beam_search (st->B counts utterances; cross_kv
+ *   and memory_bias are that member's b200st_decode_init for the B utterances; self_kv and scratch are sized for
+ *   B*beam_size rows of that member's handle).  Every member keeps its own caches and scratch; they share the beam state.
+ *   Must agree across members: vocab, st->B, st->Tm and st->max_len.  d, heads and the layer counts may differ, and the
+ *   members' precisions and use_shadow too, as long as every member can decode B*beam_size rows: above 8 rows every member
+ *   needs use_shadow 1 and a 16-bit handle.
+ *   weight: finite and >= 0 with a positive sum; the library normalises the weights to sum 1 (BeamSearch's
+ *   ensemble_weights: "average" is 1/n each).  A zero weight leaves that member out of the mixture.
+ *   a: as for b200st_beam_search; state_words holds b200st_beam_state_bytes(members[0].h, B, beam_size, st->max_len) bytes.
+ *   beam_size 1 runs the beam path with one beam (the reference's greedy search is sequence_beam_search(beam_size=1)).
+ * n_members is 1..B200ST_ENSEMBLE_MAX_MODELS; one member is exactly b200st_beam_search.  Invalid arguments fail before anything
+ * is launched. */
+#define B200ST_ENSEMBLE_MAX_MODELS 8
+typedef struct {
+  b200st_handle h; const b200st_buffers* buf; const b200st_decode_state* st;
+  float weight;                 /* >= 0; normalised by the library */
+} b200st_ensemble_member;
+int b200st_ensemble_beam_search(const b200st_ensemble_member* members, int32_t n_members, const b200st_beam_args* a, void* stream);
 
 /* 16-bit shadow of the parameter arena (wgmma operands); shadow_dtype = B200ST_BF16 or B200ST_F16 */
 int b200st_refresh_shadow(const float* params, void* shadow, int32_t shadow_dtype, int64_t numel, void* stream);

@@ -18,7 +18,10 @@ lr_schedule.params, pretrain_model}, dataset.class AudioTFRecordDataset / datase
 task.params, model.class / model.params / hparams_set, model_dir, dtype, and for `predict` the keys of the prediction
 recipes: `entry: predict` (the alias of entry.class) and search_method beam_search / search_method.params {beam_size,
 length_penalty, top_k, maximum_decode_length, extra_decode_length, minimum_decode_length, enable_unk}, and the top-level
-batch_size (utterances per call; with a 16-bit dtype decoded from the 16-bit weights).  Transcripts must already be token ids (the
+batch_size (utterances per call; with a 16-bit dtype decoded from the 16-bit weights).  Several model_dirs (a yaml list or a
+comma-separated string) make `predict` decode with their ensemble, weighted by search_method.params / entry.params
+ensemble_weights ("average" or comma-separated numbers); each member is rebuilt from its model_configs.yml, which `train`
+writes.  Transcripts must already be token ids (the
 reference's `create_tfrecords` with a projected transcript): its tokenizers / BPE are outside this path and raw text is
 refused with that message.  Checkpoints are NumPy archives keyed by the reference's variable names (checkpoints.py).
 """
@@ -203,9 +206,16 @@ def resolve(cfg, world=1):
     dataset = {"data_path": dsp.get("data_path"), "feature_key": dsp.get("feature_key", "audio"),
                "transcript_key": dsp.get("transcript_key", "transcript")}
     search_method, search = resolve_search(cfg, ep, tp)
+    entry = str(_module_name(cfg, "entry") or "trainer").lower()
+    model_dirs = flatten_string_list(cfg.get("model_dir") or ep.get("model_dir") or "./b200st_model")
+    if not model_dirs:
+        raise SystemExit("model_dir names no directory")
+    if len(model_dirs) > 1 and entry in ("trainer", "train"):
+        raise SystemExit("training writes one model_dir, got %d: %s" % (len(model_dirs), ", ".join(model_dirs)))
     plan = {
-        "entry": str(_module_name(cfg, "entry") or "trainer").lower(),
-        "model_dir": cfg.get("model_dir") or ep.get("model_dir") or "./b200st_model",
+        "entry": entry,
+        # several directories: `predict` decodes with the ensemble of their models (SequenceGenerator._build_and_restore_model)
+        "model_dir": model_dirs[0] if len(model_dirs) == 1 else model_dirs,
         "precision": {"float16": "fp16", "fp16": "fp16", "bfloat16": "bf16", "bf16": "bf16", "float32": "fp32", "fp32": "fp32"}[
             str(cfg.get("dtype", "float16")).lower()],
         "model_params": model_params, "optimizer": opt, "lr_schedule": lr,
@@ -222,7 +232,25 @@ def resolve(cfg, world=1):
         plan["batch_size"] = int(cfg["batch_size"])
     if search_method:
         plan["search_method"] = search_method
+    if len(model_dirs) > 1:
+        # BeamSearch's ensemble_weights: search_method.params, then entry.params (where the flat --ensemble_weights lands)
+        sp = cfg.get("search_method.params") or {}
+        spec = sp.get("ensemble_weights", ep.get("ensemble_weights"))
+        from neurst_b200.decode import ensemble_weights
+        try:
+            plan["ensemble_weights"] = ensemble_weights("average" if spec is None else spec, len(model_dirs))
+        except ValueError as e:
+            raise SystemExit("ensemble_weights %r for %d models: %s" % (spec, len(model_dirs), e))
     return plan
+
+
+def flatten_string_list(arg):
+    """A string or a list of strings, each of which may hold comma-separated items -> the list of items (the reference's
+    neurst/utils/misc.py:64-74)."""
+    if arg is None:
+        return None
+    items = arg if isinstance(arg, (list, tuple)) else [arg]
+    return [c.strip() for cs in items for c in str(cs).split(",") if c.strip()]
 
 
 # ------------------------------------------------------------------------------------------------ checkpoints
@@ -249,6 +277,35 @@ def save_checkpoint(rt, model_dir, step, max_to_keep=8):
     with open(os.path.join(model_dir, "checkpoint"), "w") as f:          # the index file the reference's managers keep
         json.dump({"model_checkpoint_path": os.path.basename(path), "all_model_checkpoint_paths": [os.path.basename(p) for _, p in kept[-max_to_keep:]]}, f)
     return path
+
+
+MODEL_CONFIGS = "model_configs.yml"
+
+
+def write_model_configs(plan):
+    """<model_dir>/model_configs.yml with the model's class and parameters (ModelConfigs.dump, written when training begins as
+    the reference's checkpoint callback does, neurst/training/callbacks.py:81): what an ensemble member is rebuilt from."""
+    import yaml
+    os.makedirs(plan["model_dir"], exist_ok=True)
+    path = os.path.join(plan["model_dir"], MODEL_CONFIGS)
+    with open(path + ".tmp", "w") as f:
+        yaml.safe_dump({"model.class": "SpeechTransformer", "model.params": dict(plan["model_params"])}, f, default_flow_style=False)
+    os.replace(path + ".tmp", path)
+
+
+def member_model_params(plan, model_dir):
+    """Architecture of one ensemble member: <model_dir>/model_configs.yml when it exists (ModelConfigs.load), else the run's
+    model.params / hparams_set."""
+    import yaml
+    path = os.path.join(model_dir, MODEL_CONFIGS)
+    if not os.path.exists(path):
+        return plan["model_params"]
+    with open(path) as f:
+        cfg = yaml.safe_load(f) or {}
+    cls = str(cfg.get("model.class", "SpeechTransformer")).lower().replace("_", "")
+    if cls not in ("speechtransformer", "b200speechtransformer", "b200st"):
+        raise SystemExit("%s: model.class %r is outside this path (SpeechTransformer only)" % (path, cfg.get("model.class")))
+    return dict(cfg.get("model.params") or {})
 
 
 # ------------------------------------------------------------------------------------------------ entries
@@ -318,6 +375,8 @@ def train(plan):
                                   summary_steps=plan["summary_steps"] if rank == 0 else 0, logger=LOG.info)
     trainer.global_step = start_step
     trainer.broadcast_parameters()
+    if rank == 0:
+        write_model_configs(plan)
     task, examples = _examples(plan, rank, world, training=True)
     gen = torch.Generator().manual_seed(plan["seed"] + rank)
     from neurst_b200.data import Prefetcher
@@ -362,15 +421,30 @@ def ids_to_text(ids, eos_id, tokens):
     return " ".join(words).replace("@@ ", "")                            # BPE continuation marks (subword-nmt convention)
 
 
-def predict(plan):
+def _restore(plan, model_dir):
     from neurst_b200 import checkpoints as CK
-    from neurst_b200.decode import MAX_ROWS, MAX_ROWS_SHADOW
-    world, rank, _ = _dist_setup()
     model = _build_model(plan)
-    path, step = latest_checkpoint(plan["model_dir"])
+    path, step = latest_checkpoint(model_dir)
     if not path:
-        raise SystemExit("no ckpt-*.npz under %s" % plan["model_dir"])
+        raise SystemExit("no ckpt-*.npz under %s" % model_dir)
     CK.load_npz(model.runtime, path)
+    return model, step
+
+
+def predict(plan):
+    from neurst_b200.decode import MAX_ROWS, MAX_ROWS_SHADOW
+    from neurst_b200.models import EncoderDecoderEnsembleModel
+    world, rank, _ = _dist_setup()
+    ensemble = isinstance(plan["model_dir"], list)
+    if ensemble:
+        # SequenceGenerator._build_and_restore_model: each member from its own directory, all at the run's dtype
+        members = [_restore(dict(plan, model_params=member_model_params(plan, d)), d) for d in plan["model_dir"]]
+        model = EncoderDecoderEnsembleModel.new([m for m, _ in members])
+        step = [s for _, s in members]
+        LOG.info("predict: ensemble of %d models (%s), weights %s", model.model_num, ", ".join(plan["model_dir"]),
+                 plan["ensemble_weights"])
+    else:
+        model, step = _restore(plan, plan["model_dir"])
     task, examples = _examples(plan, rank, world, training=False)
     tm = plan["trg_meta"]
     dim = plan["task"]["audio_feature_dim"] * plan["task"]["audio_feature_channels"]
@@ -384,6 +458,8 @@ def predict(plan):
     # the recipes' batch_size (utterances per batch): with 16-bit weights the batch is decoded in one call from the 16-bit
     # shadow, up to MAX_ROWS_SHADOW rows (utterances x beam) per step; the fp32 weights hold MAX_ROWS rows per step
     search_kw = dict(plan["search"])
+    if ensemble:
+        search_kw["ensemble_weights"] = plan["ensemble_weights"]
     if plan.get("batch_size") is not None:
         if plan["precision"] == "fp32":
             LOG.info("predict: dtype float32 decodes %d utterance(s) per call (at most %d rows per step), not batch_size %d",

@@ -249,15 +249,31 @@ int64_t b200st_beam_state_bytes(b200st_handle h, int32_t B, int32_t beam_size, i
   if (!h) return -1;
   return beam_state_bytes(B, beam_size, max_len);
 }
-int b200st_beam_search(b200st_handle h, const b200st_buffers* buf, const b200st_decode_state* st, const b200st_beam_args* a,
-                       void* stream) {
-  if (!h || !buf || !st || !a) B200ST_FAIL("null argument");
+static BeamArgs to_beam_args(const b200st_beam_args* a) {
   BeamArgs b{};
   b.bos_ids = a->bos_ids; b.eos_id = a->eos_id; b.unk_id = a->unk_id; b.min_len = a->min_len; b.max_steps = a->max_steps;
   b.beam_size = a->beam_size; b.top_k = a->top_k; b.length_penalty = a->length_penalty;
   b.out_ids = a->out_ids; b.out_scores = a->out_scores; b.out_logprob = a->out_logprob; b.out_len = a->out_len;
   b.state_words = a->state_words; b.use_graph = a->use_graph;
-  return beam_search(h->m, to_buffers(buf), to_state(st), b, reinterpret_cast<cudaStream_t>(stream));
+  return b;
+}
+int b200st_beam_search(b200st_handle h, const b200st_buffers* buf, const b200st_decode_state* st, const b200st_beam_args* a,
+                       void* stream) {
+  if (!h || !buf || !st || !a) B200ST_FAIL("null argument");
+  return beam_search(h->m, to_buffers(buf), to_state(st), to_beam_args(a), reinterpret_cast<cudaStream_t>(stream));
+}
+static_assert(B200ST_ENSEMBLE_MAX_MODELS == kEnsembleMaxModels, "include/b200st.h and model.cuh disagree on the ensemble size");
+int b200st_ensemble_beam_search(const b200st_ensemble_member* members, int32_t n_members, const b200st_beam_args* a, void* stream) {
+  if (n_members < 1 || n_members > B200ST_ENSEMBLE_MAX_MODELS)
+    B200ST_FAIL("an ensemble has 1.." + std::to_string(B200ST_ENSEMBLE_MAX_MODELS) + " members, got " + std::to_string(n_members));
+  if (!members || !a) B200ST_FAIL("null argument");
+  EnsembleMember em[B200ST_ENSEMBLE_MAX_MODELS];
+  for (int i = 0; i < n_members; ++i) {
+    const b200st_ensemble_member& x = members[i];
+    if (!x.h || !x.buf || !x.st) B200ST_FAIL("ensemble member " + std::to_string(i) + ": null argument");
+    em[i] = EnsembleMember{&x.h->m, to_buffers(x.buf), to_state(x.st), x.weight};
+  }
+  return ensemble_beam_search(em, n_members, to_beam_args(a), reinterpret_cast<cudaStream_t>(stream));
 }
 int b200st_refresh_shadow(const float* params, void* shadow, int32_t shadow_dtype, int64_t numel, void* stream) {
   if (!params || !shadow) B200ST_FAIL("null argument");

@@ -21,10 +21,12 @@
 //
 // Steps of more than 8 rows (shadow only, up to 256) take the wide step of decode_rows.cu instead of these GEMV kernels;
 // the embedding, the searches' selection / bookkeeping kernels and the token loop are shared.
+#include "beam.cuh"
 #include "decode_rows.cuh"
 #include "model.cuh"
 #include "pdl.cuh"
 
+#include <algorithm>
 #include <cmath>
 #include <vector>
 
@@ -33,7 +35,6 @@ namespace b200st {
 namespace {
 
 constexpr int MAXB = 8;        // rows per step (batch x beam = batch for greedy)
-constexpr float kFloatMin = -1.0e9f;
 
 template <typename TW> __device__ __forceinline__ float wf(const TW* p, int64_t i) { return to_f32(p[i]); }
 
@@ -324,155 +325,8 @@ __global__ void greedy_init_kernel(GreedyState g, const int64_t* __restrict__ bo
   for (int j = i; j < B * max_steps; j += gridDim.x * blockDim.x) g.out[j] = eos;   // padded with EOS (beam_search.py:428-436)
 }
 
-// ---- beam search (beam_search.py:71-251,380-437): rows = utterances x beam, row u*beam + k holds beam k of utterance u ----
-constexpr int KMAX = MAXB;     // largest beam: every beam of an utterance is a row of the same step
-struct BeamState {
-  int64_t* ids;          // [rows] current input ids
-  float* logprob;        // [rows] accumulated log probability
-  int32_t* finished;     // [rows]
-  int32_t* length;       // [rows] decoding length
-  int32_t* anc;          // [rows][max_len] cache row whose slot holds position j of the hypothesis now in row r
-  int32_t* hist;         // [rows][max_len] word chosen at step j for row r
-  int32_t* time;         // [1]
-  int32_t* all_finished; // [1]
-  uint32_t* ticket;      // [1] blocks done with the current step (the last one publishes time / all_finished)
-};
-
-// _calculate_length_penalty (beam_search.py:24-40): 1/len for alpha < 0, else ((5 + len) / 6)^-alpha
-__device__ __forceinline__ float length_penalty(int len, float alpha) {
-  return alpha < 0.f ? 1.f / (float)len : powf((5.f + (float)len) / 6.f, -alpha);
-}
-// tf.nn.top_k order: higher score first, the lower flat index on ties
-__device__ __forceinline__ bool cand_better(float s, int i, float s2, int i2) { return s > s2 || (s == s2 && i < i2); }
-
-// One search step of one utterance (block = utterance, so every row it reads or reorders is its own): log_softmax of each
-// beam row with the finished / UNK / min-length masks (:71-142,380-388), accumulated log-probabilities times the length
-// penalty of next_length = length + 1 - finished (:145-179), top-`beam` over the beam*V candidates (only the first beam's
-// V at time 0; :181-190), then the reorder of the row state and of the ancestry table (:395-404).  The top-k is a
-// per-thread register top-KMAX over the thread's candidates followed by `beam` rounds of a block-wide arg-max.
-__global__ void __launch_bounds__(1024) beam_select_kernel(const float* __restrict__ logits, BeamState s, int beam, int V, int eos,
-                                                           int unk, int min_len, float alpha, int max_len) {
-  pdl_wait();
-  pdl_trigger();
-  __shared__ float red[32];
-  __shared__ float sval[32];
-  __shared__ int sidx[32];
-  __shared__ float lse[KMAX], pen[KMAX], lprev[KMAX];
-  __shared__ int fin[KMAX], nlen[KMAX], win[KMAX];
-  const int r0 = blockIdx.x * beam;
-  const int t = *s.time;
-  const int lane = threadIdx.x & 31, w = threadIdx.x >> 5, nw = blockDim.x >> 5;
-  for (int b = 0; b < beam; ++b) {
-    const float* z = logits + (int64_t)(r0 + b) * V;
-    float mx = -INFINITY;
-    for (int v = threadIdx.x; v < V; v += blockDim.x) mx = fmaxf(mx, z[v]);
-    mx = block_max(mx, red);
-    float se = 0.f;
-    for (int v = threadIdx.x; v < V; v += blockDim.x) se += expf(z[v] - mx);
-    se = block_sum(se, red);
-    if (threadIdx.x == 0) {
-      lse[b] = mx + logf(se);
-      fin[b] = s.finished[r0 + b] != 0;
-      lprev[b] = s.logprob[r0 + b];
-      nlen[b] = s.length[r0 + b] + 1 - fin[b];
-      pen[b] = length_penalty(nlen[b], alpha);
-    }
-  }
-  __syncthreads();
-  // accumulated log-probability of candidate (beam b, word v), un-penalised
-  auto acc_of = [&](int b, int v) -> float {
-    float lp = logits[(int64_t)(r0 + b) * V + v] - lse[b];
-    if (fin[b]) lp = (v == eos) ? 0.f : kFloatMin;
-    if (v == unk) lp += kFloatMin;
-    if (v == eos && t < min_len - 1) lp += kFloatMin;
-    return lp + lprev[b];
-  };
-  float vs[KMAX];
-  int is[KMAX];
-#pragma unroll
-  for (int q = 0; q < KMAX; ++q) { vs[q] = -INFINITY; is[q] = 0x7fffffff; }
-  const int nb = t == 0 ? 1 : beam;
-  for (int b = 0; b < nb; ++b) {
-    for (int v = threadIdx.x; v < V; v += blockDim.x) {
-      const float sc = acc_of(b, v) * pen[b];
-      const int i = b * V + v;
-      if (cand_better(sc, i, vs[KMAX - 1], is[KMAX - 1])) {
-        vs[KMAX - 1] = sc; is[KMAX - 1] = i;
-#pragma unroll
-        for (int q = KMAX - 1; q > 0; --q) {
-          if (cand_better(vs[q], is[q], vs[q - 1], is[q - 1])) {
-            const float tv = vs[q]; vs[q] = vs[q - 1]; vs[q - 1] = tv;
-            const int ti = is[q]; is[q] = is[q - 1]; is[q - 1] = ti;
-          }
-        }
-      }
-    }
-  }
-  for (int k = 0; k < beam; ++k) {
-    float bv = vs[0];
-    int bi = is[0];
-#pragma unroll
-    for (int o = 16; o > 0; o >>= 1) {
-      const float ov = __shfl_xor_sync(0xffffffffu, bv, o);
-      const int oi = __shfl_xor_sync(0xffffffffu, bi, o);
-      if (cand_better(ov, oi, bv, bi)) { bv = ov; bi = oi; }
-    }
-    __syncthreads();
-    if (lane == 0) { sval[w] = bv; sidx[w] = bi; }
-    __syncthreads();
-    if (threadIdx.x == 0) {
-      for (int i = 1; i < nw; ++i)
-        if (cand_better(sval[i], sidx[i], bv, bi)) { bv = sval[i]; bi = sidx[i]; }
-      win[k] = bi < nb * V ? bi : 0;
-    }
-    __syncthreads();
-    if (is[0] == win[k]) {                        // flat indices are unique: exactly one thread pops its head
-#pragma unroll
-      for (int q = 0; q < KMAX - 1; ++q) { vs[q] = vs[q + 1]; is[q] = is[q + 1]; }
-      vs[KMAX - 1] = -INFINITY; is[KMAX - 1] = 0x7fffffff;
-    }
-  }
-  // new row r0 + j continues beam p = win[j] / V with word win[j] % V (every old value was read into shared memory above)
-  if ((int)threadIdx.x < beam) {
-    const int j = threadIdx.x, p = win[j] / V, word = win[j] % V;
-    const int r = r0 + j;
-    s.ids[r] = word;
-    s.logprob[r] = acc_of(p, word);
-    s.length[r] = nlen[p];
-    s.finished[r] = word == eos ? 1 : 0;
-    s.hist[(int64_t)r * max_len + t] = word;
-  }
-  // ancestry: anc'[r0 + j][col] = anc[r0 + p][col] for col < t, and r0 + p at col = t (the parent's own slot).  A thread
-  // owns whole columns, so reading every parent's entry before writing needs no barrier.
-  for (int col = threadIdx.x; col <= t; col += blockDim.x) {
-    int nv[KMAX];
-#pragma unroll
-    for (int j = 0; j < KMAX; ++j) {
-      if (j < beam) {
-        const int p = r0 + win[j] / V;
-        nv[j] = col == t ? p : s.anc[(int64_t)p * max_len + col];
-      }
-    }
-#pragma unroll
-    for (int j = 0; j < KMAX; ++j)
-      if (j < beam) s.anc[(int64_t)(r0 + j) * max_len + col] = nv[j];
-  }
-  // the last block of the step publishes all_finished (every row of every utterance) and advances time: every block has
-  // read `time` before it takes its ticket
-  __threadfence();
-  __syncthreads();
-  if (threadIdx.x == 0) {
-    __threadfence();
-    if (atomicAdd(s.ticket, 1u) == gridDim.x - 1) {
-      __threadfence();
-      int all = 1;
-      for (int r = 0; r < (int)gridDim.x * beam; ++r) all &= __ldcg(s.finished + r) != 0 ? 1 : 0;
-      *s.all_finished = all;
-      *s.ticket = 0;
-      *s.time = t + 1;
-    }
-  }
-}
+// ---- beam search: BeamState and beam_select_kernel live in beam.cuh ----
+static_assert(KMAX == MAXB, "every beam of an utterance is a row of the same step");
 
 __global__ void beam_init_kernel(BeamState s, const int64_t* __restrict__ bos, int rows, int beam) {
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
@@ -1068,6 +922,37 @@ int raise_all_smem(const Config& cf, const DecodeState& st) {
   return 0;
 }
 
+// Shared-memory bytes of the cross-attention step: q | ctx | scores | red.
+size_t cross_attn_smem(const Config& cf, int Tm) { return sizeof(float) * (size_t)(2 * (cf.d / cf.heads) + Tm + 8); }
+
+// The beam variants of the attention step (self: smem_self, cross: smem_cross bytes)
+int raise_beam_smem(size_t smem_self, size_t smem_cross) {
+  B200ST_TRY(raise_smem(attn_step_kernel<float, true, true>, smem_self));
+  B200ST_TRY(raise_smem(attn_step_kernel<__half, true, true>, smem_self));
+  B200ST_TRY(raise_smem(attn_step_kernel<__nv_bfloat16, true, true>, smem_self));
+  B200ST_TRY(raise_smem(attn_step_kernel<float, false, true>, smem_cross));
+  B200ST_TRY(raise_smem(attn_step_kernel<__half, false, true>, smem_cross));
+  B200ST_TRY(raise_smem(attn_step_kernel<__nv_bfloat16, false, true>, smem_cross));
+  return 0;
+}
+
+// The beam state in beam_state_bytes(B, beam, max_len) device words:
+//   [ids rows x int64][logprob rows][finished rows][length rows][time][all_finished][ticket][pad][anc][hist]
+BeamState beam_state_at(void* words, int rows, int max_len) {
+  char* w = reinterpret_cast<char*>(words);
+  BeamState bs{};
+  bs.ids = reinterpret_cast<int64_t*>(w); w += sizeof(int64_t) * rows;
+  bs.logprob = reinterpret_cast<float*>(w); w += sizeof(float) * rows;
+  bs.finished = reinterpret_cast<int32_t*>(w); w += sizeof(int32_t) * rows;
+  bs.length = reinterpret_cast<int32_t*>(w); w += sizeof(int32_t) * rows;
+  bs.time = reinterpret_cast<int32_t*>(w); w += sizeof(int32_t);
+  bs.all_finished = reinterpret_cast<int32_t*>(w); w += sizeof(int32_t);
+  bs.ticket = reinterpret_cast<uint32_t*>(w); w += 2 * sizeof(int32_t);
+  bs.anc = reinterpret_cast<int32_t*>(w); w += sizeof(int32_t) * (size_t)rows * max_len;
+  bs.hist = reinterpret_cast<int32_t*>(w);
+  return bs;
+}
+
 }  // namespace
 
 static int g_last_greedy_graph = -1;
@@ -1205,32 +1090,15 @@ int beam_search(const Model& m, const Buffers& buf, const DecodeState& st, const
   const size_t smem_self = self_attn_smem(cf, st.max_len, true);
   B200ST_CHECK(smem_self <= 200 * 1024, "decode: too many keys for the shared-memory score buffer");
   B200ST_TRY(raise_all_smem(cf, st));
-  B200ST_TRY(raise_smem(attn_step_kernel<float, true, true>, smem_self));
-  B200ST_TRY(raise_smem(attn_step_kernel<__half, true, true>, smem_self));
-  B200ST_TRY(raise_smem(attn_step_kernel<__nv_bfloat16, true, true>, smem_self));
-  const size_t smem_cross = sizeof(float) * (size_t)(2 * (cf.d / cf.heads) + st.Tm + 8);
-  B200ST_TRY(raise_smem(attn_step_kernel<float, false, true>, smem_cross));
-  B200ST_TRY(raise_smem(attn_step_kernel<__half, false, true>, smem_cross));
-  B200ST_TRY(raise_smem(attn_step_kernel<__nv_bfloat16, false, true>, smem_cross));
-  // device words: [ids rows x int64][logprob rows][finished rows][length rows][time][all_finished][ticket][pad][anc][hist]
-  char* w = reinterpret_cast<char*>(a.state_words);
-  BeamState bs{};
-  bs.ids = reinterpret_cast<int64_t*>(w); w += sizeof(int64_t) * rows;
-  bs.logprob = reinterpret_cast<float*>(w); w += sizeof(float) * rows;
-  bs.finished = reinterpret_cast<int32_t*>(w); w += sizeof(int32_t) * rows;
-  bs.length = reinterpret_cast<int32_t*>(w); w += sizeof(int32_t) * rows;
-  bs.time = reinterpret_cast<int32_t*>(w); w += sizeof(int32_t);
-  bs.all_finished = reinterpret_cast<int32_t*>(w); w += sizeof(int32_t);
-  bs.ticket = reinterpret_cast<uint32_t*>(w); w += 2 * sizeof(int32_t);
-  bs.anc = reinterpret_cast<int32_t*>(w); w += sizeof(int32_t) * (size_t)rows * st.max_len;
-  bs.hist = reinterpret_cast<int32_t*>(w);
+  B200ST_TRY(raise_beam_smem(smem_self, cross_attn_smem(cf, st.Tm)));
+  const BeamState bs = beam_state_at(a.state_words, rows, st.max_len);
   float* logits = rs.scratch + (rows > MAXB ? rows_logits_offset(cf, rows) : layout_of(cf, rows).logits);
   beam_init_kernel<<<(rows + 255) / 256, 256, 0, s>>>(bs, a.bos_ids, rows, beam);
   B200ST_CUDA(cudaGetLastError());
   StepCtx c{m, buf, rs, s};
   auto one_step = [&]() -> int {
     B200ST_TRY(step_dispatch(c, bs.ids, bs.time, logits, bs.anc, beam));
-    launch_pdl(beam_select_kernel, st.B, 1024, 0, s, (const float*)logits, bs, beam, cf.vocab, a.eos_id, a.unk_id, a.min_len,
+    launch_pdl(beam_select_kernel<false>, st.B, 1024, 0, s, (const float*)logits, bs, beam, cf.vocab, a.eos_id, a.unk_id, a.min_len,
                a.length_penalty, st.max_len);
     ++g_kernel_launches;
     B200ST_LAUNCH_CHECK();
@@ -1241,6 +1109,100 @@ int beam_search(const Model& m, const Buffers& buf, const DecodeState& st, const
   B200ST_CHECK(graphed || !a.use_graph, "beam search could not capture its step into a CUDA graph");
   beam_extract_kernel<<<st.B, 256, 0, s>>>(bs, beam, a.top_k, a.length_penalty, a.eos_id, st.max_len, a.max_steps, a.out_ids,
                                            a.out_scores, a.out_logprob, a.out_len);
+  ++g_kernel_launches;
+  B200ST_CUDA(cudaGetLastError());
+  return 0;
+}
+
+// sequence_beam_search over EncoderDecoderEnsembleModel (encoder_decoder_ensemble_model.py, beam_search.py:97-115): per
+// token every member steps on the same B x beam rows (its own self-attention cache, cross K/V and scratch; the shared ids
+// and ancestry table of the one beam state), ensemble_logprob mixes their distributions over member 0's logits, and
+// beam_select_kernel<true> selects on the mixture.  beam_size 1 runs this same beam path, as the reference's greedy search
+// is sequence_beam_search(beam_size=1).  One member is the plain beam_search: the reference takes a plain log_softmax then.
+int ensemble_beam_search(const EnsembleMember* mem, int n, const BeamArgs& a, cudaStream_t s) {
+  B200ST_CHECK(mem != nullptr && n >= 1 && n <= kEnsembleMaxModels,
+               "an ensemble has 1.." + std::to_string(kEnsembleMaxModels) + " members, got " + std::to_string(n));
+  double wsum = 0.0;
+  for (int i = 0; i < n; ++i) {
+    const float w = mem[i].weight;
+    B200ST_CHECK(mem[i].m != nullptr, "ensemble member " + std::to_string(i) + ": null handle");
+    B200ST_CHECK(std::isfinite(w) && w >= 0.f,
+                 "ensemble weights must be finite and >= 0, member " + std::to_string(i) + " has " + std::to_string(w));
+    wsum += w;
+  }
+  B200ST_CHECK(wsum > 0.0, "ensemble weights must have a positive sum");
+  if (n == 1) return beam_search(*mem[0].m, mem[0].buf, mem[0].st, a, s);
+  const DecodeState& st0 = mem[0].st;
+  const int beam = a.beam_size, V = mem[0].m->cfg.vocab;
+  B200ST_CHECK(beam >= 1, "beam_size must be >= 1");
+  B200ST_CHECK(a.top_k >= 1 && a.top_k <= beam, "top_k must be in 1..beam_size");
+  B200ST_CHECK(beam <= KMAX, "beam_size must be at most " + std::to_string(KMAX));
+  B200ST_CHECK(beam <= V, "beam_size exceeds the vocabulary");
+  B200ST_CHECK(a.max_steps >= 1 && a.max_steps <= st0.max_len, "max_steps must be within the cache length");
+  B200ST_CHECK(a.bos_ids && a.out_ids && a.out_scores && a.out_len && a.out_logprob && a.state_words,
+               "ensemble_beam_search: null argument");
+  const int rows = st0.B * beam;
+  std::vector<StepCtx> ctx;
+  std::vector<float*> logits;
+  size_t smem_self = 0, smem_cross = 0, rows_self = 0, rows_cross = 0;
+  for (int i = 0; i < n; ++i) {
+    const Model& m = *mem[i].m;
+    const Config& cf = m.cfg;
+    const DecodeState& st = mem[i].st;
+    const std::string who = "ensemble member " + std::to_string(i) + ": ";
+    B200ST_CHECK(cf.model_type == MODEL_SPEECH || cf.model_type == MODEL_TEXT, who + "decoding needs an encoder-decoder handle");
+    B200ST_CHECK(cf.vocab == V, who + "vocabulary of " + std::to_string(cf.vocab) + " differs from member 0's " + std::to_string(V));
+    B200ST_CHECK(st.B == st0.B && st.Tm == st0.Tm && st.max_len == st0.max_len,
+                 who + "decode state (B, Tm, max_len) = (" + std::to_string(st.B) + ", " + std::to_string(st.Tm) + ", " +
+                 std::to_string(st.max_len) + ") differs from member 0's (" + std::to_string(st0.B) + ", " + std::to_string(st0.Tm) +
+                 ", " + std::to_string(st0.max_len) + ")");
+    const int max_rows = st.use_shadow ? kDecodeMaxRows : MAXB;      // more than 8 rows: the wide step, 16-bit shadow only
+    B200ST_CHECK(rows <= max_rows, who + "beam search decodes at most " + std::to_string(max_rows) + " rows (utterances x beam_size) per " +
+                                   "call" + (st.use_shadow ? "" : " without use_shadow") + ", got " + std::to_string(st.B) + " x " +
+                                   std::to_string(beam));
+    B200ST_TRY(check_state(m, st));
+    if (st.use_shadow) B200ST_CHECK(is16(m.adt) && mem[i].buf.shadow, who + "use_shadow needs a 16-bit precision handle and its shadow arena");
+    DecodeState rs = st;                  // the step runs on every beam row; cross_kv / memory_bias stay per utterance
+    rs.B = rows;
+    B200ST_TRY(check_state(m, rs));
+    if (rows > MAXB) {
+      B200ST_TRY(rows_check(m, mem[i].buf, rs, beam));
+      rows_self = std::max(rows_self, rows_self_smem(cf, st.max_len));
+      rows_cross = std::max(rows_cross, rows_cross_smem(cf, st.Tm, beam));
+    }
+    const size_t ss = self_attn_smem(cf, st.max_len, true);
+    B200ST_CHECK(ss <= 200 * 1024, "decode: too many keys for the shared-memory score buffer");
+    smem_self = std::max(smem_self, ss);
+    smem_cross = std::max(smem_cross, cross_attn_smem(cf, st.Tm));
+    ctx.push_back(StepCtx{m, mem[i].buf, rs, s});
+    logits.push_back(rs.scratch + (rows > MAXB ? rows_logits_offset(cf, rows) : layout_of(cf, rows).logits));
+  }
+  // The dynamic shared-memory limit is an attribute of the kernel, not of the launch: set member after member, a member with
+  // a smaller head or model width would lower it below what an earlier member's attention launch needs.  So each attention
+  // kernel is raised once, to the largest need over the members, before the first step (and the capture).
+  B200ST_TRY(raise_beam_smem(smem_self, smem_cross));
+  if (rows > MAXB) B200ST_TRY(rows_raise_smem(rows_self, rows_cross));
+  EnsembleMix mix{};
+  mix.n = n;
+  for (int i = 0; i < n; ++i) {
+    mix.z[i] = logits[i];
+    mix.logw[i] = (float)std::log((double)mem[i].weight / wsum);       // a zero weight: -inf, which contributes nothing
+  }
+  const BeamState bs = beam_state_at(a.state_words, rows, st0.max_len);
+  beam_init_kernel<<<(rows + 255) / 256, 256, 0, s>>>(bs, a.bos_ids, rows, beam);
+  B200ST_CUDA(cudaGetLastError());
+  auto one_step = [&]() -> int {
+    for (int i = 0; i < n; ++i) B200ST_TRY(step_dispatch(ctx[i], bs.ids, bs.time, logits[i], bs.anc, beam));
+    ensemble_logprob(mix, rows, V, s);
+    beam_select_logprobs(logits[0], bs, st0.B, beam, V, a.eos_id, a.unk_id, a.min_len, a.length_penalty, st0.max_len, s);
+    B200ST_LAUNCH_CHECK();
+    return 0;
+  };
+  bool graphed = false;
+  B200ST_TRY(run_token_loop(s, a.max_steps, a.use_graph != 0, bs.all_finished, one_step, &graphed));
+  B200ST_CHECK(graphed || !a.use_graph, "ensemble beam search could not capture its step into a CUDA graph");
+  beam_extract_kernel<<<st0.B, 256, 0, s>>>(bs, beam, a.top_k, a.length_penalty, a.eos_id, st0.max_len, a.max_steps, a.out_ids,
+                                            a.out_scores, a.out_logprob, a.out_len);
   ++g_kernel_launches;
   B200ST_CUDA(cudaGetLastError());
   return 0;

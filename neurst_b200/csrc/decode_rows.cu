@@ -605,6 +605,13 @@ int rows_check(const Model& m, const Buffers& buf, const DecodeState& st, int be
   }
   const size_t ss = self_smem(cf, st.max_len), cs = cross_smem(cf, st.Tm, beam);
   B200ST_CHECK(ss <= 200 * 1024 && cs <= 200 * 1024, "decode: too many keys for the shared-memory score buffer");
+  return rows_raise_smem(ss, cs);
+}
+
+size_t rows_self_smem(const Config& c, int max_len) { return self_smem(c, max_len); }
+size_t rows_cross_smem(const Config& c, int Tm, int beam) { return cross_smem(c, Tm, beam); }
+
+int rows_raise_smem(size_t ss, size_t cs) {
   if (ss > 48 * 1024) B200ST_CUDA(cudaFuncSetAttribute(rows_self_attn_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)ss));
   if (cs > 48 * 1024) B200ST_CUDA(cudaFuncSetAttribute(rows_cross_attn_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)cs));
   return 0;

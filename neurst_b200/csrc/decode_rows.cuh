@@ -11,6 +11,11 @@ int64_t rows_scratch_floats(const Config& c, int B);
 int64_t rows_logits_offset(const Config& c, int B);
 // Checks what the wide step needs beyond check_state (shadow, dims, shared memory); nothing is launched.
 int rows_check(const Model& m, const Buffers& buf, const DecodeState& st, int beam);
+// Dynamic shared memory of the wide step's self- and cross-attention kernels, and the call that sets both kernels' limits
+// (rows_check sets them for its own model; an ensemble sets them once to the largest need of its members)
+size_t rows_self_smem(const Config& c, int max_len);
+size_t rows_cross_smem(const Config& c, int Tm, int beam);
+int rows_raise_smem(size_t self_bytes, size_t cross_bytes);
 // Every decoder layer and the tied logits of one step on st.B rows; anc / beam as step_launch in decode.cu.
 int rows_step(const Model& m, const Buffers& buf, const DecodeState& st, const int32_t* time_dev, float* logits, const int* anc,
               int beam, cudaStream_t s);

@@ -154,5 +154,14 @@ struct BeamArgs {
 int64_t beam_state_bytes(int B, int beam, int max_len);
 // st.B counts utterances; self_kv and scratch are sized for B * beam_size rows, cross_kv / memory_bias for B
 int beam_search(const Model& m, const Buffers& buf, const DecodeState& st, const BeamArgs& a, cudaStream_t s);
+constexpr int kEnsembleMaxModels = 8;      // B200ST_ENSEMBLE_MAX_MODELS
+struct EnsembleMember {
+  const Model* m;
+  Buffers buf;
+  DecodeState st;                // as beam_search's: B utterances, self_kv / scratch for B * beam_size rows
+  float weight;                  // >= 0, normalised over the members
+};
+// beam_search over the weighted mixture of n members' next-token distributions, one beam state for all members
+int ensemble_beam_search(const EnsembleMember* members, int n, const BeamArgs& a, cudaStream_t s);
 
 }  // namespace b200st

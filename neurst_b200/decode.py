@@ -7,7 +7,7 @@ Host mirror of
   SequenceGenerator                                 neurst/exps/sequence_generator.py:62-86
 
 Everything numeric is a library call (b200st_encode / b200st_decode_init / b200st_decode_step / b200st_greedy_search /
-b200st_beam_search):
+b200st_beam_search / b200st_ensemble_beam_search):
 the key/value caches are preallocated device buffers owned by `DecodingCache`, the token ids and the position live on the
 device, and the greedy loop replays one captured CUDA graph per token inside the library.
 """
@@ -244,4 +244,103 @@ def beam_search(rt, inputs, bos_id, eos_id, unk_id=None, beam_size=4, length_pen
     out = out[:, :steps]
     if steps < maximum_decode_length:      # padded to the fixed output length with EOS (beam_search.py:428-436)
         out = torch.cat([out, torch.full((n, maximum_decode_length - steps), int(eos_id), dtype=torch.int64, device=dev)], 1)
+    return out, scores, logprob, length
+
+
+def ensemble_weights(spec, n):
+    """BeamSearch._get_ensemble_weights (beam_search.py:486-515): "average" gives 1/n each; comma-separated numbers (or a
+    list of them) must count exactly n and are normalised to sum 1.  Whether the values are usable (finite, >= 0, a positive
+    sum) is checked by the library, which normalises them again."""
+    if spec is None or (isinstance(spec, str) and spec.strip() == "average"):
+        return [1.0 / n] * n
+    if isinstance(spec, (int, float)):          # one number, as a yaml or command-line value parses
+        spec = [spec]
+    eles = [float(x) for x in (spec.strip().split(",") if isinstance(spec, str) else spec)]
+    if len(eles) != n:
+        raise ValueError("The number of manual weights must have equal to the models.")
+    total = sum(eles)
+    return [x / total for x in eles] if total > 0 else eles
+
+
+def ensemble_beam_search(rts, inputs, bos_id, eos_id, unk_id=None, weights="average", beam_size=4, length_penalty=0.6, top_k=1,
+                         maximum_decode_length=256, extra_decode_length=50, minimum_decode_length=0, enable_unk=False,
+                         use_shadow=False, use_graph=True, caches=None):
+    """sequence_beam_search over an ensemble (EncoderDecoderEnsembleModel, beam_search.py:97-115) on the device: every step
+    mixes the members' next-token distributions, log(sum_m w_m softmax(logits_m)), and searches on the mixture.  `rts` are
+    the members' runtimes (same vocabulary); each runs its own encoder and keeps its own DecodingCache(beam=beam_size)
+    (`caches`: one per member, built by create_decoding_cache).  `weights`: "average", comma-separated numbers or a list
+    (ensemble_weights).  Returns what beam_search returns.  beam_size 1 is the ensemble's greedy search; one member is
+    exactly beam_search."""
+    rts = list(rts)
+    n = len(rts)
+    if not 1 <= n <= L.ENSEMBLE_MAX_MODELS:
+        raise L.B200STError("an ensemble has 1..%d members, got %d" % (L.ENSEMBLE_MAX_MODELS, n))
+    w = ensemble_weights(weights, n)
+    beam_size, top_k = int(beam_size), int(top_k)
+    if beam_size < 1:
+        raise L.B200STError("beam_size must be >= 1, got %d" % beam_size)
+    if not 1 <= top_k <= beam_size:
+        raise L.B200STError("top_k must be in 1..beam_size (%d), got %d" % (beam_size, top_k))
+    if minimum_decode_length >= maximum_decode_length:          # BeamSearch.call (beam_search.py:531-532)
+        raise L.B200STError("minimum_decode_length must be less than maximum_decode_length")
+    alpha = -1.0 if length_penalty is None else float(length_penalty)
+    if caches is None:
+        B = int(inputs["src"].shape[0])
+        if B * beam_size > max_rows(use_shadow):
+            raise L.B200STError("beam search decodes at most %d rows (utterances x beam_size) per call, got %d x %d"
+                                % (max_rows(use_shadow), B, beam_size))
+        caches = []
+        for rt in rts:
+            enc, bias = encode(rt, inputs)
+            caches.append(create_decoding_cache(rt, enc, bias, maximum_decode_length, use_shadow, beam=beam_size))
+    caches = list(caches)
+    if len(caches) != n:
+        raise L.B200STError("%d decoding caches for %d ensemble members" % (len(caches), n))
+    for c in caches:
+        if c.self_kv.shape[2] < c.B * beam_size:
+            raise L.B200STError("the decoding cache holds %d rows, beam search needs %d" % (c.self_kv.shape[2], c.B * beam_size))
+    rt0, c0 = rts[0], caches[0]
+    B, Tm = c0.B, c0.Tm
+    steps = _search_steps(Tm, maximum_decode_length, extra_decode_length, minimum_decode_length)
+    dev = rt0.device
+    bos = torch.as_tensor(bos_id).to(device=dev, dtype=torch.int64).reshape(-1)
+    if bos.numel() == 1:
+        bos = bos.repeat(B)
+    bos = bos.contiguous()
+    k = B * top_k
+    out = torch.empty(k, max(steps, 1), dtype=torch.int64, device=dev)
+    scores = torch.zeros(k, dtype=torch.float32, device=dev)
+    logprob = torch.zeros(k, dtype=torch.float32, device=dev)
+    length = torch.zeros(k, dtype=torch.int32, device=dev)
+    nbytes = int(rt0.lib.b200st_beam_state_bytes(rt0.handle, B, beam_size, c0.max_len))
+    if nbytes <= 0:
+        raise L.B200STError("beam search state sizing failed: " + rt0.lib.b200st_last_error().decode())
+    words = torch.zeros((nbytes + 7) // 8, dtype=torch.int64, device=dev)
+    a = L.BeamArgs()
+    a.bos_ids, a.eos_id = bos.data_ptr(), int(eos_id)
+    a.unk_id = -1 if (enable_unk or unk_id is None) else int(unk_id)
+    a.min_len, a.max_steps = int(minimum_decode_length), int(steps)
+    a.beam_size, a.top_k, a.length_penalty = beam_size, top_k, alpha
+    a.out_ids, a.out_scores, a.out_logprob, a.out_len = out.data_ptr(), scores.data_ptr(), logprob.data_ptr(), length.data_ptr()
+    a.state_words = words.data_ptr()
+    # one member is beam_search itself, whose beam 1 is the greedy search with its persistent kernel
+    a.use_graph = (2 if beam_size == 1 else 1) if use_graph else 0
+    bufs = [_bufs(rt) for rt in rts]
+    members = (L.EnsembleMember * n)()
+    for i, (rt, c) in enumerate(zip(rts, caches)):
+        members[i].h, members[i].buf, members[i].st = rt.handle, C.pointer(bufs[i]), C.pointer(c.state)
+        members[i].weight = w[i]
+    cur = torch.cuda.current_stream(dev)
+    side = getattr(rt0, "_decode_stream", None)
+    if side is None:
+        side = rt0._decode_stream = torch.cuda.Stream(device=dev)
+    side.wait_stream(cur)
+    with torch.cuda.stream(side):
+        L.check(rt0.lib.b200st_ensemble_beam_search(members, n, C.byref(a), L._stream()))
+    cur.wait_stream(side)
+    if n == 1 and beam_size == 1 and use_graph and int(rt0.lib.b200st_greedy_used_graph()) < 1:
+        raise L.B200STError("greedy search could neither run its persistent kernel nor capture its step graph")
+    out = out[:, :steps]
+    if steps < maximum_decode_length:      # padded to the fixed output length with EOS (beam_search.py:428-436)
+        out = torch.cat([out, torch.full((k, maximum_decode_length - steps), int(eos_id), dtype=torch.int64, device=dev)], 1)
     return out, scores, logprob, length

@@ -211,6 +211,13 @@ class BeamArgs(C.Structure):
                 ("state_words", C.c_void_p), ("use_graph", C.c_int32)]
 
 
+ENSEMBLE_MAX_MODELS = 8    # B200ST_ENSEMBLE_MAX_MODELS
+
+
+class EnsembleMember(C.Structure):
+    _fields_ = [("h", C.c_void_p), ("buf", C.POINTER(Buffers)), ("st", C.POINTER(DecodeState)), ("weight", C.c_float)]
+
+
 # every symbol include/b200st.h declares (tests/test_abi.py checks the .so exports all of them)
 EXPORTS = [
     "b200st_last_error", "b200st_version", "b200st_launch_count", "b200st_gemm", "b200st_gemm_bench", "b200st_profile_begin", "b200st_profile_end",
@@ -219,6 +226,7 @@ EXPORTS = [
     "b200st_comm_unique_id", "b200st_comm_init", "b200st_comm_broadcast", "b200st_comm_destroy", "b200st_comm_stats", "b200st_train_step",
     "b200st_encode", "b200st_encode_workspace_bytes", "b200st_decode_scratch_floats", "b200st_decode_init", "b200st_decode_step",
     "b200st_greedy_search", "b200st_greedy_used_graph", "b200st_beam_state_bytes", "b200st_beam_search",
+    "b200st_ensemble_beam_search",
     "b200st_encoder_forward", "b200st_decoder_forward", "b200st_mha_forward", "b200st_lsce", "b200st_layernorm_fwd",
     "b200st_layernorm_bwd", "b200st_softmax_fwd", "b200st_conv1_ln_relu_fwd", "b200st_dropout_stream_id", "b200st_dropout_mask",
 ]
@@ -259,6 +267,7 @@ def _declare(lib):
     lib.b200st_beam_state_bytes.restype = C.c_int64
     lib.b200st_beam_state_bytes.argtypes = [C.c_void_p, C.c_int32, C.c_int32, C.c_int32]
     lib.b200st_beam_search.argtypes = [C.c_void_p, C.POINTER(Buffers), C.POINTER(DecodeState), C.POINTER(BeamArgs), C.c_void_p]
+    lib.b200st_ensemble_beam_search.argtypes = [C.POINTER(EnsembleMember), C.c_int32, C.POINTER(BeamArgs), C.c_void_p]
     lib.b200st_adam_step.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64, C.c_float,
                                      C.c_float, C.c_float, C.c_float, C.c_int64, C.c_float, C.c_int32, C.c_void_p]
     lib.b200st_encoder_forward.argtypes = [C.c_void_p, C.POINTER(Buffers), C.c_void_p, C.c_void_p, C.c_int32, C.c_int32,

@@ -2,6 +2,7 @@
 
   SpeechTransformer          neurst/models/speech_transformer.py:27-280  (PT twin neurst_pt/models/speech_transformer.py)
   Transformer                neurst/models/transformer.py:27-260         (cfg-1 plumbing model)
+  EncoderDecoderEnsembleModel  neurst/models/encoder_decoder_ensemble_model.py  (generation only)
   LabelSmoothedCrossEntropy  neurst/criterions/label_smoothed_cross_entropy.py:26-157
 
 `Model.new(args, src_meta, trg_meta)` takes the reference's flat `model.params` dict (the yaml / hparams_set keys);
@@ -287,6 +288,75 @@ class Transformer(_EncoderDecoder):
             postprocess_dropout=args.get("encoder.layer_postprocess_dropout_rate", 0.), label_smoothing=label_smoothing,
             share_src_trg_embedding=share)
         return cls(args, src_meta, trg_meta, Runtime(cfg, device))
+
+
+class EncoderDecoderEnsembleModel:
+    """ neurst/models/encoder_decoder_ensemble_model.py: several encoder-decoder models decoding as one, for generation only.
+    Its searches mix the members' next-token distributions on the device at every step (decode.ensemble_beam_search). """
+
+    def __init__(self, encoder_decoder_models):
+        self._encoder_decoder_models = list(encoder_decoder_models)
+
+    @classmethod
+    def new(cls, encoder_decoder_models):
+        return cls(encoder_decoder_models)
+
+    @property
+    def model_num(self):
+        return len(self._encoder_decoder_models)
+
+    @property
+    def models(self):
+        return list(self._encoder_decoder_models)
+
+    def get_symbols_to_logits_fn(self, inputs, is_training=False, is_inference=True, decode_padded_length=None):
+        """-> (symbols_to_logits_fn(symbols, cache_per_model, time=None) returning the list of the members' logits [B, V],
+        generation_initializer whose decoder_internal_cache is the list of the members' caches), as the reference's."""
+        fns, init = [], None
+        for model in self._encoder_decoder_models:
+            fn, model_init = model.get_symbols_to_logits_fn(inputs, False, True, decode_padded_length=decode_padded_length)
+            fns.append(fn)
+            if init is None:
+                init = dict(model_init, decoder_internal_cache=[model_init["decoder_internal_cache"]])
+            else:
+                init["decoder_internal_cache"].append(model_init["decoder_internal_cache"])
+
+        def symbols_to_logits_fn(symbols, cache_per_model, time=None):
+            return [fn(symbols, cache, time=time) for fn, cache in zip(fns, cache_per_model)]
+
+        return symbols_to_logits_fn, init
+
+    def _bos(self, inputs):
+        bos = inputs.get("trg_input")
+        if bos is None:
+            bos = torch.full((inputs["src"].shape[0],), int(self._encoder_decoder_models[0]._trg_meta["bos_id"]), dtype=torch.long)
+        return bos
+
+    def beam_search(self, inputs, beam_size=4, length_penalty=0.6, top_k=1, maximum_decode_length=256, extra_decode_length=50,
+                    minimum_decode_length=0, enable_unk=False, ensemble_weights="average", use_shadow=False):
+        """BeamSearch with `ensemble_weights` over the members -> (hypotheses [B*top_k, maximum_decode_length],
+        scores [B*top_k]), with the row limits of the single model's beam_search."""
+        from neurst_b200 import decode as D
+        tm = self._encoder_decoder_models[0]._trg_meta
+        ids, scores, _, _ = D.ensemble_beam_search([m.runtime for m in self._encoder_decoder_models], inputs, self._bos(inputs),
+                                                   tm["eos_id"], tm.get("unk_id"), ensemble_weights, beam_size, length_penalty, top_k,
+                                                   maximum_decode_length, extra_decode_length, minimum_decode_length, enable_unk,
+                                                   use_shadow)
+        return ids, scores
+
+    def greedy_search(self, inputs, maximum_decode_length=256, extra_decode_length=50, minimum_decode_length=0, enable_unk=False,
+                      ensemble_weights="average", use_shadow=False):
+        """The ensemble's beam_search with beam_size 1 (the reference's greedy search) -> (token ids [B, maximum_decode_length],
+        log-probs [B])."""
+        from neurst_b200 import decode as D
+        tm = self._encoder_decoder_models[0]._trg_meta
+        ids, _, logprob, _ = D.ensemble_beam_search([m.runtime for m in self._encoder_decoder_models], inputs, self._bos(inputs),
+                                                    tm["eos_id"], tm.get("unk_id"), ensemble_weights, 1, 0.6, 1, maximum_decode_length,
+                                                    extra_decode_length, minimum_decode_length, enable_unk, use_shadow)
+        return ids, logprob
+
+    def call(self, inputs, is_training=True):
+        raise NotImplementedError("No need to implement call function for EncoderDecoderEnsembleModel.")
 
 
 class LabelSmoothedCrossEntropy:
