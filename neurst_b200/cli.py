@@ -21,7 +21,8 @@ length_penalty, top_k, maximum_decode_length, extra_decode_length, minimum_decod
 batch_size (utterances per call; with a 16-bit dtype decoded from the 16-bit weights).  Several model_dirs (a yaml list or a
 comma-separated string) make `predict` decode with their ensemble, weighted by search_method.params / entry.params
 ensemble_weights ("average" or comma-separated numbers); each member is rebuilt from its model_configs.yml, which `train`
-writes.  Transcripts must already be token ids (the
+writes.  validator.class / validator.params (CriterionValidator, SeqGenerationValidator) validate during `train`
+(neurst_b200/validation.py).  Transcripts must already be token ids (the
 reference's `create_tfrecords` with a projected transcript): its tokenizers / BPE are outside this path and raw text is
 refused with that message.  Checkpoints are NumPy archives keyed by the reference's variable names (checkpoints.py).
 """
@@ -37,8 +38,14 @@ import torch
 
 LOG = logging.getLogger("neurst_b200")
 
-SECTIONS = ("entry.params", "task.params", "dataset.params", "model.params", "search_method.params")
-TOP_LEVEL = ("model_dir", "hparams_set", "dtype", "output_file", "entry", "search_method")
+SECTIONS = ("entry.params", "task.params", "dataset.params", "model.params", "search_method.params", "validator.params")
+TOP_LEVEL = ("model_dir", "hparams_set", "dtype", "output_file", "entry", "search_method", "validator")
+# the validators' flags (neurst/training/validator.py, criterion_validator.py, seq_generation_validator.py): a flat
+# `--eval_steps 500` lands in validator.params, as the reference's registered flags do
+VALIDATOR_FLAGS = ("eval_steps", "eval_start_at", "eval_on_begin", "eval_dataset", "eval_dataset.params", "eval_batch_size",
+                   "eval_task_args", "eval_criterion", "eval_criterion.params", "eval_search_method", "eval_search_method.params",
+                   "eval_metric", "eval_metric.params", "eval_estop_patience", "eval_best_checkpoint_path",
+                   "eval_auto_average_checkpoints", "eval_best_avg_checkpoint_path", "eval_top_checkpoints_to_keep")
 
 
 # ------------------------------------------------------------------------------------------------ configuration
@@ -109,6 +116,8 @@ def load_config(paths, overrides=()):
         hits = [s for s in SECTIONS if isinstance(cfg.get(s), dict) and key in cfg[s]]
         if len(hits) > 1:
             raise SystemExit("flag --%s is ambiguous (%s): use the dotted form" % (key, ", ".join(hits)))
+        if not hits and key in VALIDATOR_FLAGS:
+            hits = ["validator.params"]
         cfg.setdefault(hits[0] if hits else "entry.params", {})[key] = val
     return cfg
 
@@ -165,6 +174,83 @@ def resolve_search(cfg, ep, tp):
                            "minimum_decode_length": int(get("minimum_decode_length", 0)),
                            "beam_size": int(get("beam_size", 4)), "length_penalty": -1.0 if lp is None else float(lp),
                            "top_k": int(get("top_k", 1)), "enable_unk": bool(get("enable_unk", False))}
+
+
+def _as_dict(v, what):
+    if v is None:
+        return {}
+    if not isinstance(v, dict):
+        raise SystemExit("%s must be a mapping, got %r" % (what, v))
+    return dict(v)
+
+
+def resolve_validator(cfg, tp):
+    """validator.class (or its alias `validator`) with validator.params, the flags and defaults of Validator,
+    CriterionValidator and SeqGenerationValidator; None without a validator."""
+    cls = _module_name(cfg, "validator")
+    if cls is None:
+        return None
+    name = {"criterionvalidator": "CriterionValidator", "seqgenerationvalidator": "SeqGenerationValidator"}.get(
+        str(cls).lower().replace("_", ""))
+    if name is None:
+        raise SystemExit("validator.class %r is outside this path (CriterionValidator, SeqGenerationValidator)" % cls)
+    vp = _as_dict(cfg.get("validator.params"), "validator.params")
+    for k in VALIDATOR_FLAGS:               # dotted command-line keys such as --eval_dataset.params.data_path
+        if k in cfg:
+            vp = deep_merge(vp, {k: cfg[k]})
+
+    def module(key):
+        return vp.get(key + ".class", vp.get(key)), _as_dict(vp.get(key + ".params"), "validator.params." + key + ".params")
+
+    ds_cls, dsp = module("eval_dataset")
+    if ds_cls is None or not dsp.get("data_path"):
+        raise SystemExit("validator %s needs eval_dataset with eval_dataset.params.data_path" % name)
+    if str(ds_cls).lower().replace("_", "") not in ("audiotfrecorddataset", "audiotfrecord"):
+        raise SystemExit("eval_dataset %r is outside this path (AudioTFRecordDataset only)" % ds_cls)
+    task_args = _as_dict(vp.get("eval_task_args"), "eval_task_args")
+    unknown = sorted(set(task_args) - {"batch_size", "truncate_src", "max_src_len"})
+    if unknown:
+        raise SystemExit("eval_task_args %s are outside this path (batch_size, truncate_src, max_src_len)" % ", ".join(unknown))
+    crit_cls, critp = module("eval_criterion")
+    if crit_cls is not None and str(crit_cls).lower().replace("_", "") != "labelsmoothedcrossentropy":
+        raise SystemExit("eval_criterion %r is outside this path (label_smoothed_cross_entropy only)" % crit_cls)
+    plan = {"class": name, "eval_steps": int(vp.get("eval_steps", 1000)), "eval_start_at": int(vp.get("eval_start_at", 0)),
+            "eval_on_begin": bool(vp.get("eval_on_begin", False)),
+            "dataset": {"data_path": dsp["data_path"], "feature_key": dsp.get("feature_key", "audio"),
+                        "transcript_key": dsp.get("transcript_key", "transcript")},
+            "batch_size": int(vp.get("eval_batch_size", 32)),
+            "task_args": {k: v for k, v in task_args.items() if k != "batch_size"},
+            # the reference builds the eval criterion from its own params: label_smoothing defaults to 0
+            "criterion": crit_cls is not None, "label_smoothing": float(critp.get("label_smoothing", 0.0)),
+            "search_method": None, "search": None, "metric": None}
+    if plan["eval_steps"] <= 0 or plan["batch_size"] <= 0:
+        raise SystemExit("eval_steps and eval_batch_size must be positive")
+    if name == "SeqGenerationValidator":
+        method, sp = module("eval_search_method")
+        metric, metric_params = module("eval_metric")
+        if metric_params:
+            # the restated metrics take no parameters; their language is the target data pipeline's
+            raise SystemExit("eval_metric.params %s are outside this path (the metrics take no parameters; the language "
+                             "is task.params' *_data_pipeline.params.language)" % ", ".join(sorted(metric_params)))
+        if method is not None:
+            plan["search_method"], plan["search"] = resolve_search({"search_method": method, "search_method.params": sp}, {}, tp)
+        language = "en"                     # the metric's language: the target data pipeline's (get_eval_metric)
+        for k in ("transcript_data_pipeline.params", "trg_data_pipeline.params", "translation_data_pipeline.params"):
+            if isinstance(tp.get(k), dict) and tp[k].get("language"):
+                language = tp[k]["language"]
+        if metric is not None:
+            from neurst_b200.metrics import build_metric
+            try:
+                build_metric(metric, language)
+            except ValueError as e:
+                raise SystemExit(str(e))
+            plan["metric"] = str(metric)
+        plan.update(language=language, estop_patience=int(vp.get("eval_estop_patience", 0) or 0),
+                    best_checkpoint_path=vp.get("eval_best_checkpoint_path"),
+                    auto_average_checkpoints=bool(vp.get("eval_auto_average_checkpoints", True)),
+                    best_avg_checkpoint_path=vp.get("eval_best_avg_checkpoint_path"),
+                    top_checkpoints_to_keep=int(vp.get("eval_top_checkpoints_to_keep", 10)))
+    return plan
 
 
 def resolve(cfg, world=1):
@@ -232,6 +318,13 @@ def resolve(cfg, world=1):
         plan["batch_size"] = int(cfg["batch_size"])
     if search_method:
         plan["search_method"] = search_method
+    validator = resolve_validator(cfg, tp)
+    if validator is not None:
+        plan["validator"] = validator
+        if validator["search_method"]:
+            # eval_batch_size x beam_size must fit a decoding step: refused now, not at the first validation
+            from neurst_b200.validation import generation_plan
+            decode_settings(generation_plan(plan))
     if len(model_dirs) > 1:
         # BeamSearch's ensemble_weights: search_method.params, then entry.params (where the flat --ensemble_weights lands)
         sp = cfg.get("search_method.params") or {}
@@ -262,6 +355,23 @@ def latest_checkpoint(model_dir):
         if m and int(m.group(1)) >= best[1]:
             best = (p, int(m.group(1)))
     return best
+
+
+def restore_checkpoint(model_dir):
+    """(path, step) of the archive to restore from a directory: the one the `checkpoint` index names as
+    model_checkpoint_path when it exists (the kept-best `ckpt-<step>-<metric>.npz` of best/ and best_avg/), else the
+    newest `ckpt-<step>.npz`.  In a directory `train` wrote the index names the newest archive, so both agree."""
+    try:
+        with open(os.path.join(model_dir, "checkpoint")) as f:
+            name = json.load(f)["model_checkpoint_path"]
+    except (OSError, ValueError, KeyError, TypeError):
+        name = None
+    if name:
+        path = os.path.join(model_dir, os.path.basename(name))
+        m = re.match(r"ckpt-(\d+)(-[^/]*)?\.npz$", os.path.basename(path))
+        if m and os.path.isfile(path):
+            return path, int(m.group(1))
+    return latest_checkpoint(model_dir)
 
 
 def save_checkpoint(rt, model_dir, step, max_to_keep=8):
@@ -331,15 +441,16 @@ def _build_model(plan):
     return SpeechTransformer.new(plan["model_params"], src_meta, tm, precision=plan["precision"], label_smoothing=plan["label_smoothing"])
 
 
-def _examples(plan, rank, world, training):
-    """Endless (training) or single-pass stream of preprocessed samples of this rank's file shard."""
+def _examples(plan, rank, world, training, with_label=None):
+    """Endless (training) or single-pass stream of preprocessed samples of this rank's file shard (with the transcripts
+    when training or `with_label`)."""
     from neurst_b200.data import SpeechToText
     from neurst_b200.tfrecord import AudioTFRecordDataset
     ds = AudioTFRecordDataset(plan["dataset"])
     tk = dict(plan["task"])
     task = SpeechToText({k: v for k, v in plan["trg_meta"].items() if k != "tokens"}, world=1,
                         padding_mode=plan["trg_meta"]["padding_mode"], **tk)
-    proc = task.preprocess_fn(ds.status, training=training, with_label=training)
+    proc = task.preprocess_fn(ds.status, training=training, with_label=training if with_label is None else with_label)
     from neurst_b200.tfrecord import glob_tfrecords
     shards = world if len(glob_tfrecords(plan["dataset"]["data_path"])) >= world else 1     # fewer files than ranks: every rank reads all
 
@@ -365,7 +476,7 @@ def train(plan):
         LOG.info("restored %s", start_path)
     elif plan["pretrain_model"]:
         src = plan["pretrain_model"][0] if isinstance(plan["pretrain_model"], (list, tuple)) else plan["pretrain_model"]
-        src = latest_checkpoint(src)[0] if os.path.isdir(src) else src
+        src = restore_checkpoint(src)[0] if os.path.isdir(src) else src
         CK.load_npz(model.runtime, src, strict=False)
         LOG.info("initialised from %s", src)
     else:
@@ -377,19 +488,27 @@ def train(plan):
     trainer.broadcast_parameters()
     if rank == 0:
         write_model_configs(plan)
+    validator = None
+    if plan.get("validator"):
+        from neurst_b200.validation import Validator
+        validator = Validator(plan, model, rank, world)
+        if plan["validator"]["eval_on_begin"]:
+            validator.validate(start_step)
     task, examples = _examples(plan, rank, world, training=True)
     gen = torch.Generator().manual_seed(plan["seed"] + rank)
     from neurst_b200.data import Prefetcher
     import itertools
     last = None
+    early_stopped = False
     micro_target = (plan["train_steps"] - start_step) * plan["update_cycle"]
     if micro_target > 0:
         # reading, parsing, padding and pinning of the next batches run in a background thread (tf.data prefetch's role)
         batches = Prefetcher(itertools.islice((per_rank[0] for per_rank in task.train_batches(examples, generator=gen, pin=True)),
                                               micro_target), depth=4, init=lambda: torch.cuda.set_device(local))
         try:
-            losses = HostPipeline(trainer).run(batches, seed0=start_step * plan["update_cycle"] + 1)
-            saved_at = start_step
+            pipeline = HostPipeline(trainer)
+            losses = pipeline.run(batches, seed0=start_step * plan["update_cycle"] + 1)
+            saved_at = validated_at = start_step
             for loss in losses:
                 if loss is not None:
                     last = loss
@@ -398,6 +517,14 @@ def train(plan):
                     torch.cuda.synchronize()
                     save_checkpoint(model.runtime, plan["model_dir"], step, plan["max_to_keep"])
                     saved_at = step
+                # the step's kernels (and its optimizer update) are done once validate() synchronises; the next step is
+                # launched only when this generator resumes, so every rank validates the same weights
+                if validator is not None and step > validated_at and validator.due(step):
+                    validated_at = step
+                    if validator.validate(step)[1]:
+                        early_stopped = True
+                        last = pipeline.latest_loss()      # the losses arrive one step late: read the stopping step's
+                        break
         finally:
             batches.close()
     torch.cuda.synchronize()
@@ -406,7 +533,10 @@ def train(plan):
     if world > 1:
         trainer.close()
         torch.distributed.barrier()
-    return {"global_step": trainer.global_step, "loss": last}
+    res = {"global_step": trainer.global_step, "loss": last}
+    if validator is not None:
+        res.update(early_stopped=early_stopped, validations=validator.history)
+    return res
 
 
 def ids_to_text(ids, eos_id, tokens):
@@ -424,15 +554,54 @@ def ids_to_text(ids, eos_id, tokens):
 def _restore(plan, model_dir):
     from neurst_b200 import checkpoints as CK
     model = _build_model(plan)
-    path, step = latest_checkpoint(model_dir)
+    path, step = restore_checkpoint(model_dir)
     if not path:
         raise SystemExit("no ckpt-*.npz under %s" % model_dir)
     CK.load_npz(model.runtime, path)
     return model, step
 
 
-def predict(plan):
+def decode_settings(plan):
+    """(utterances per search call, search keyword arguments) of `predict` and the validators' generation.  The recipes'
+    batch_size (utterances per batch): with 16-bit weights the batch is decoded in one call from the 16-bit shadow, up
+    to MAX_ROWS_SHADOW rows (utterances x beam) per step; the fp32 weights hold MAX_ROWS rows per step."""
     from neurst_b200.decode import MAX_ROWS, MAX_ROWS_SHADOW
+    beam = plan.get("search_method") == "beam_search"
+    width = plan["search"]["beam_size"] if beam else 1
+    per_call = MAX_ROWS // width
+    if per_call < 1:
+        raise SystemExit("beam_size %d exceeds the %d rows a decoding step holds" % (plan["search"]["beam_size"], MAX_ROWS))
+    search_kw = dict(plan["search"])
+    if plan.get("batch_size") is not None:
+        if plan["precision"] == "fp32":
+            LOG.info("dtype float32 decodes %d utterance(s) per call (at most %d rows per step), not batch_size %d",
+                     min(per_call, plan["batch_size"]), MAX_ROWS, plan["batch_size"])
+            per_call = min(per_call, plan["batch_size"])
+        else:
+            if not 1 <= plan["batch_size"] * width <= MAX_ROWS_SHADOW:
+                raise SystemExit("batch_size %d x beam_size %d exceeds the %d rows a decoding step holds"
+                                 % (plan["batch_size"], width, MAX_ROWS_SHADOW))
+            per_call = plan["batch_size"]
+            search_kw["use_shadow"] = True
+    return per_call, search_kw
+
+
+def decode_group(model, task, plan, group, search_kw):
+    """One search call over preprocessed samples -> [(ids_to_text hypothesis, score)], top_k rows per utterance,
+    consecutive (the reference's [B*top_k] order)."""
+    tm = plan["trg_meta"]
+    dim = plan["task"]["audio_feature_dim"] * plan["task"]["audio_feature_channels"]
+    T = max(int(e["audio_length"]) for e in group)
+    src = torch.zeros(len(group), T, dim)
+    for j, e in enumerate(group):
+        src[j, :int(e["audio_length"])] = e["audio"]
+    batch = task.example_to_input({"audio": src, "audio_length": torch.tensor([int(e["audio_length"]) for e in group])}, infer=True)
+    search = model.beam_search if plan.get("search_method") == "beam_search" else model.greedy_search
+    ids, score = search({"src": batch["src"], "src_length": batch["src_length"]}, **search_kw)
+    return [(ids_to_text(row, tm["eos_id"], tm.get("tokens")), lp) for row, lp in zip(ids.cpu().tolist(), score.cpu().tolist())]
+
+
+def predict(plan):
     from neurst_b200.models import EncoderDecoderEnsembleModel
     world, rank, _ = _dist_setup()
     ensemble = isinstance(plan["model_dir"], list)
@@ -446,52 +615,18 @@ def predict(plan):
     else:
         model, step = _restore(plan, plan["model_dir"])
     task, examples = _examples(plan, rank, world, training=False)
-    tm = plan["trg_meta"]
-    dim = plan["task"]["audio_feature_dim"] * plan["task"]["audio_feature_channels"]
-    hyps = []
-    group = []
-    beam = plan.get("search_method") == "beam_search"
-    width = plan["search"]["beam_size"] if beam else 1
-    per_call = MAX_ROWS // width
-    if per_call < 1:
-        raise SystemExit("beam_size %d exceeds the %d rows a decoding step holds" % (plan["search"]["beam_size"], MAX_ROWS))
-    # the recipes' batch_size (utterances per batch): with 16-bit weights the batch is decoded in one call from the 16-bit
-    # shadow, up to MAX_ROWS_SHADOW rows (utterances x beam) per step; the fp32 weights hold MAX_ROWS rows per step
-    search_kw = dict(plan["search"])
+    per_call, search_kw = decode_settings(plan)
     if ensemble:
         search_kw["ensemble_weights"] = plan["ensemble_weights"]
-    if plan.get("batch_size") is not None:
-        if plan["precision"] == "fp32":
-            LOG.info("predict: dtype float32 decodes %d utterance(s) per call (at most %d rows per step), not batch_size %d",
-                     min(per_call, plan["batch_size"]), MAX_ROWS, plan["batch_size"])
-            per_call = min(per_call, plan["batch_size"])
-        else:
-            if not 1 <= plan["batch_size"] * width <= MAX_ROWS_SHADOW:
-                raise SystemExit("batch_size %d x beam_size %d exceeds the %d rows a decoding step holds"
-                                 % (plan["batch_size"], width, MAX_ROWS_SHADOW))
-            per_call = plan["batch_size"]
-            search_kw["use_shadow"] = True
-
-    def flush():
-        if not group:
-            return
-        T = max(int(e["audio_length"]) for e in group)
-        src = torch.zeros(len(group), T, dim)
-        for j, e in enumerate(group):
-            src[j, :int(e["audio_length"])] = e["audio"]
-        batch = task.example_to_input({"audio": src, "audio_length": torch.tensor([int(e["audio_length"]) for e in group])}, infer=True)
-        search = model.beam_search if beam else model.greedy_search
-        # beam search: top_k rows per utterance, consecutive (the reference's [B*top_k] order)
-        ids, score = search({"src": batch["src"], "src_length": batch["src_length"]}, **search_kw)
-        for row, lp in zip(ids.cpu().tolist(), score.cpu().tolist()):
-            hyps.append((ids_to_text(row, tm["eos_id"], tm.get("tokens")), lp))
-        group.clear()
-
+    hyps = []
+    group = []
     for ex in examples:
         group.append(ex)
         if len(group) == per_call:
-            flush()
-    flush()
+            hyps.extend(decode_group(model, task, plan, group, search_kw))
+            group = []
+    if group:
+        hyps.extend(decode_group(model, task, plan, group, search_kw))
     out = plan["output_file"]
     if out and rank == 0:
         with open(out, "w", encoding="utf-8") as f:
@@ -507,6 +642,8 @@ def main(argv=None):
     plan = resolve(cfg, world=int(os.environ.get("WORLD_SIZE", "1")))
     if plan["entry"] in ("trainer", "train"):
         res = train(plan)
+        if "validations" in res:
+            res["validations"] = [{k: v for k, v in r.items() if k != "hypotheses"} for r in res["validations"]]
     elif plan["entry"] in ("predict", "sequencegenerator", "sequence_generator"):
         res = predict(plan)
         res = {"checkpoint_step": res["checkpoint_step"], "n_hypotheses": len(res["hypotheses"])}

@@ -230,14 +230,20 @@ class HostPipeline:
             self.consumed[slot].record(cur)
             self.loss_host[slot:slot + 1].copy_(loss.reshape(1), non_blocking=True)   # D2H of this step's loss
             self.loss_ready[slot].record(cur)
+            self._latest = slot
             prev = None
             if i > 0:
                 self.loss_ready[slot ^ 1].synchronize()
                 prev = float(self.loss_host[slot ^ 1])
             yield prev
             i += 1
-        self.loss_ready[(i - 1) & 1].synchronize()
-        yield float(self.loss_host[(i - 1) & 1])
+        yield self.latest_loss()
+
+    def latest_loss(self):
+        """The loss of the newest step `run` launched, which its generator yields only on the next resume: for a caller
+        that stops iterating early."""
+        self.loss_ready[self._latest].synchronize()
+        return float(self.loss_host[self._latest])
 
 
 def build_speech_transformer_trainer(hparams_set="speech_transformer_s", vocab_size=8192, feature_dim=80, precision="bf16",
