@@ -22,6 +22,7 @@
 #include "ptx.cuh"
 
 #include <mutex>
+#include <type_traits>
 #include <unordered_map>
 #include <vector>
 #include <cstring>
@@ -430,17 +431,25 @@ __global__ void __launch_bounds__(kThreads, 1) tc_wgrad_group_kernel(const __gri
 //   neurst/layers/common_layers.py:145-160 (TransformerFFN) inside the pre-norm wrapper (:73-85); X = LN(x_in) (16-bit),
 //   x_out is pre-initialised with the residual x_in by the LayerNorm kernel.
 // One CTA = (128-row tile, slice of the hidden dimension); each consumer warpgroup owns 64 of the rows.  The X tile
-// (128 x D, D in {128, 256}) stays in shared memory; the hidden activations of a 128-column chunk are accumulated in
+// (128 x D, D in {128, 256}) stays in shared memory; the hidden activations of a 64-column half are accumulated in
 // registers (GEMM1), get bias, ReLU and dropout there, are written to HBM only because the backward pass needs them, and
 // go, packed to 16 bits, straight back into the tensor cores as the register A operand of GEMM2, which accumulates the
-// [64 x D] output rows in registers across all chunks.  Only the weights stream (L2 -> smem), and the [M, ffn] hidden
+// [64 x D] output rows in registers across all halves.  Only the weights stream (L2 -> smem), and the [M, ffn] hidden
 // tensor is never read back.  Slices of the hidden dimension reduce into x_out with fp32 atomics (dropout is a mask: linear).
 //   256 threads = the two consumer warpgroups and nothing else: a CTA of at most two warpgroups is compiled to a 255-register
 //   budget, which the [64 x 256] output accumulator plus the hidden fragments need for the wgmmas to stay asynchronous (with a
-//   third, producer warpgroup the budget is 168 and the d = 256 accumulators spill).  Thread 0 issues the TMA loads: X once,
-//   then the static weight schedule (per chunk the W1 stages, then the W2 stages); it refills a ring stage as soon as all
-//   eight warps have released it.
-//   smem: X 64 KB | weight ring 4 x 32 KB (one whole chunk at d = 256)
+//   third, producer warpgroup the budget is 168 and the d = 256 accumulators spill).
+//   Step s of a warpgroup issues GEMM2 of half s - 1 and GEMM1 of half s back to back and waits for both; the hidden
+//   epilogue of half s follows on CUDA cores.  The two warpgroups take turns through two named barriers, as in
+//   tc_gemm_kernel: warpgroup 0 issues step s once warpgroup 1 has issued step s - 1, and warpgroup 1 issues step s once
+//   warpgroup 0 has, so one warpgroup's wait and epilogue run while the other's wgmmas keep the tensor cores busy.  The
+//   epilogue's reads that do not depend on the accumulator (dropout-bit bytes / F1 mask words) are issued a step ahead.
+//   Weight ring: item 2s = the W1 columns of half s, item 2s + 1 = the W2 rows of half s (D x 64 16-bit weights each); step
+//   s reads items 2s - 1 and 2s and releases both after its wait.  Warpgroup 1 releases every item after warpgroup 0, so
+//   its first thread issues the TMA loads (X once, then the refill of a stage once all eight warps have released it) and
+//   warpgroup 0 never waits for a refill it did not need.  With 5 stages, the items of step s are requested when step
+//   s - 3 (item 2s - 1) and step s - 2 (item 2s) release theirs.
+//   smem: X 64 KB | weight ring 5 x 32 KB
 // =============================================================================================================
 struct MlpParams {
   int M, d, ffn;
@@ -457,10 +466,11 @@ struct MlpParams {
   int* tickets;                // deterministic mode: [m_tiles] zero-initialised; slice s adds after slices < s (self-resetting)
 };
 constexpr int kMlpThreads = 256;
-constexpr int kMlpStages = 4;
-constexpr uint32_t kMlpStageBytes = 32768;
+constexpr int kMlpStages = 5;
+constexpr uint32_t kMlpStageBytes = 32768;     // one ring item at d = 256
 constexpr uint32_t kMlpXBytes = 65536;
 constexpr size_t kMlpSmem = 1024 + kMlpXBytes + kMlpStages * kMlpStageBytes + 256;
+static_assert(kMlpSmem <= (size_t)kSmemLimit, "fused MLP smem");
 
 // B_MN: weights as MN-major B operands (forward: W1 [d, ffn], W2 [ffn, d] in the TF [in, out] layout) or K-major (backward:
 // the same arrays read transposed: G1 uses W2 rows = hidden units, G2 uses W1 rows = model dims)
@@ -471,9 +481,9 @@ fused_mlp_fwd_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_const
   extern __shared__ uint8_t smem_raw[];
   constexpr bool BF = DT == BF16;
   constexpr int kbx = D / BK;                  // k-blocks of GEMM1
-  constexpr int kW1Items = kbx / 2;            // W1 ring items per chunk (2 k-blocks each)
-  constexpr int kItems = kW1Items + 2;         // ring items per chunk: the W1 items, then the 2 W2 k-blocks
-  static_assert(kMlpStages >= 3, "a warp releases item i only after it has waited for items up to i + 2");
+  constexpr uint32_t kItemBytes = D * 128u;    // D x 64 16-bit weights
+  static_assert(kItemBytes <= kMlpStageBytes, "a ring item fits one stage");
+  static_assert(kMlpStages >= 4, "the refills a step waits for are issued by earlier steps' releases");
   const uint32_t base = (ptx::smem_u32(smem_raw) + 1023u) & ~1023u;
   const uint32_t sX = base;
   const uint32_t sW = sX + kMlpXBytes;
@@ -484,9 +494,9 @@ fused_mlp_fwd_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_const
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int m_blk = blockIdx.x / p.splits, split = blockIdx.x % p.splits;
-  const int C = p.chunks_per_cta;
-  const int chunk0 = split * C;
-  const bool producer = threadIdx.x == 0;
+  const int H = 2 * p.chunks_per_cta;                  // 64-column hidden halves of this CTA's slice
+  const int hid0 = split * p.chunks_per_cta * 128;     // first hidden unit of the slice
+  const bool producer = threadIdx.x == 128;            // first thread of warpgroup 1
 
   if (producer) {
     ptx::prefetch_tensormap(&tmX); ptx::prefetch_tensormap(&tmW1); ptx::prefetch_tensormap(&tmW2);
@@ -498,35 +508,28 @@ fused_mlp_fwd_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_const
   pdl_wait();
   pdl_trigger();
 
-  // Producer side (thread 0 only): ring item `it` goes to stage it % kMlpStages once all 8 warps have released the item
-  // kMlpStages before it.  Every warp waits only for items up to i + 2 before it releases item i, so this wait cannot
-  // depend on a load that has not been issued yet.
+  // Producer side: ring item `it` goes to stage it % kMlpStages once all 8 warps have released the item kMlpStages before
+  // it.  It is called from warpgroup 1's release of that item, and warpgroup 0 releases an item before it waits for any
+  // later one, so this wait never depends on a load that has not been issued yet.
   auto issue = [&](int it) {
-    if (it >= C * kItems) return;
-    const int st = it % kMlpStages, r = it % kItems;
-    const int n0 = (chunk0 + it / kItems) * 128;
+    if (it >= 2 * H) return;
+    const int st = it % kMlpStages;
+    const int h0 = hid0 + (it >> 1) * 64;              // first hidden unit of the item's half
     const uint32_t dst = sW + st * kMlpStageBytes;
     ptx::mbar_wait(w_empty(st), (((uint32_t)(it / kMlpStages)) & 1u) ^ 1u);
-    if (r < kW1Items) {
-      // GEMM1 B operand of the chunk: [K = d rows, N = 128 cols], k-blocks 2r and 2r + 1
-      ptx::mbar_arrive_expect_tx(w_full(st), 2u * 16384u);
-      for (int j = 0; j < 2; ++j) {
-        if (B_MN) {
-          for (int i = 0; i < 2; ++i)
-            ptx::tma_load_4d(dst + j * 16384 + i * 8192, &tmW1, w_full(st), n0 + i * 64, (2 * r + j) * BK, 0, 0);
-        } else {
-          ptx::tma_load_4d(dst + j * 16384, &tmW1, w_full(st), (2 * r + j) * BK, n0, 0, 0);      // [128 rows x 64 k]
-        }
+    ptx::mbar_arrive_expect_tx(w_full(st), kItemBytes);
+    if ((it & 1) == 0) {
+      // GEMM1 B operand of the half: [K = d, N = 64 hidden units], one 8 KB box per k-block
+      for (int kb = 0; kb < kbx; ++kb) {
+        if (B_MN) ptx::tma_load_4d(dst + kb * 8192, &tmW1, w_full(st), h0, kb * BK, 0, 0);
+        else ptx::tma_load_4d(dst + kb * 8192, &tmW1, w_full(st), kb * BK, h0, 0, 0);        // [64 hidden rows x 64 k]
       }
     } else {
-      // GEMM2 B operand of the chunk: [K = 128 hidden rows, N = d cols], k-block kb
-      const int kb = r - kW1Items;
-      ptx::mbar_arrive_expect_tx(w_full(st), (uint32_t)(D / 64) * 8192u);
+      // GEMM2 B operand of the half: [K = 64 hidden rows, N = d]
       if (B_MN) {
-        for (int i = 0; i < D / 64; ++i)
-          ptx::tma_load_4d(dst + i * 8192, &tmW2, w_full(st), i * 64, n0 + kb * BK, 0, 0);
+        for (int i = 0; i < D / 64; ++i) ptx::tma_load_4d(dst + i * 8192, &tmW2, w_full(st), i * 64, h0, 0, 0);
       } else {
-        ptx::tma_load_4d(dst, &tmW2, w_full(st), n0 + kb * BK, 0, 0, 0);                        // [d rows x 64 k]
+        ptx::tma_load_4d(dst, &tmW2, w_full(st), h0, 0, 0, 0);                                 // [d rows x 64 k]
       }
     }
   };
@@ -539,7 +542,8 @@ fused_mlp_fwd_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_const
 
   const int wg = warp >> 2, g = lane >> 2, q = lane & 3;
   const int m0 = m_blk * BM + wg * 64 + (warp & 3) * 16 + g;       // this thread's rows: m0 and m0 + 8
-  const bool use_bits = p.drop_ffn.p > 0.f;
+  const bool use_bits = B_MN && p.drop_ffn.p > 0.f;
+  const bool use_mask = !B_MN && p.mask_src != nullptr;
   const float dscale = use_bits ? p.drop_ffn.scale : 1.f;
   const float hidden_floor = p.relu ? 0.f : -INFINITY;
   auto stage_get = [&](int it) {
@@ -552,119 +556,141 @@ fused_mlp_fwd_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_const
     if (producer) issue(it + kMlpStages);
     __syncwarp();
   };
+  // The epilogue's inputs of half s that do not depend on the accumulator, loaded a step before they are folded into keep
+  // bits.  Forward: the dropout-bit bytes of columns n0 + 8 j (j < 8) of a row are 8 consecutive bytes, one 8-byte load;
+  // backward: the 16-bit F1 pairs at the thread's fragment positions.
+  uint32_t ew[2][8];
+  auto load_ew = [&](int s) {
+    const int n0 = hid0 + s * 64 + 2 * q;
+#pragma unroll
+    for (int hr = 0; hr < 2; ++hr) {
+      const int m = m0 + 8 * hr;
+#pragma unroll
+      for (int j = 0; j < 8; ++j) ew[hr][j] = 0u;
+      if (use_bits && m < p.M) {
+        const uint2 w = __ldg(reinterpret_cast<const uint2*>(p.drop_ffn.bits + (((int64_t)m * p.ffn + hid0 + s * 64) >> 3)));
+        ew[hr][0] = w.x; ew[hr][1] = w.y;
+      }
+      if (use_mask && m < p.M) {
+#pragma unroll
+        for (int j = 0; j < 8; ++j)
+          ew[hr][j] = __ldg(reinterpret_cast<const uint32_t*>(reinterpret_cast<const uint16_t*>(p.mask_src) + (int64_t)m * p.mask_ld + n0 + 8 * j));
+      }
+    }
+  };
+  // keep bits of element pair (row m0 + 8 hr, columns n0 + 8 j + {0, 1}): bits 16 hr + 2 j + {0, 1}
+  auto fold_keep = [&]() {
+    uint32_t keep = 0u;
+#pragma unroll
+    for (int hr = 0; hr < 2; ++hr) {
+#pragma unroll
+      for (int j = 0; j < 8; ++j) {
+        uint32_t k2;
+        if (B_MN) {
+          k2 = (ew[hr][j >> 2] >> (8 * (j & 3) + 2 * q)) & 3u;
+        } else {
+          // 16-bit mask source (bf16 / fp16): "> 0" <=> sign clear and magnitude bits non-zero
+          const uint32_t lo = ew[hr][j] & 0xffffu, hi = ew[hr][j] >> 16;
+          k2 = ((lo != 0u && lo < 0x8000u) ? 1u : 0u) | ((hi != 0u && hi < 0x8000u) ? 2u : 0u);
+        }
+        keep |= k2 << (16 * hr + 2 * j);
+      }
+    }
+    return keep;
+  };
+
   float out[D / 2];
 #pragma unroll
   for (int i = 0; i < D / 2; ++i) out[i] = 0.f;
-  ptx::mbar_wait(x_full, 0);
-  for (int c = 0; c < C; ++c) {
-    // The 128 hidden columns of chunk c go through the registers as two halves of 64 (GEMM1 half, epilogue, GEMM2 k-block),
-    // so that the [64 x D] output accumulator and the hidden fragments fit the register file; the W1 items are read by
-    // both halves and released after the second.
-    const int item0 = c * kItems;
-    uint32_t w1src[kW1Items];
+  float hid[32];
 #pragma unroll
-    for (int h = 0; h < 2; ++h) {
-      const int n0 = (chunk0 + c) * 128 + h * 64 + 2 * q;
-      // the epilogue's dropout-bit bytes (forward) / F1 mask words (backward) do not depend on the accumulator: they are
-      // loaded before GEMM1 is issued and folded into keep bits while it runs
-      uint32_t ew[2][8];
+  for (int i = 0; i < 32; ++i) hid[i] = 0.f;           // the first wgmma of every GEMM1 ignores the accumulator (scale-d 0)
+  uint32_t a16[4][4];
 #pragma unroll
-      for (int hr = 0; hr < 2; ++hr) {
-        const int m = m0 + 8 * hr;
+  for (int k = 0; k < 4; ++k)
 #pragma unroll
-        for (int j = 0; j < 8; ++j) {
-          const int n = n0 + 8 * j;
-          ew[hr][j] = 0u;
-          if (use_bits && m < p.M) ew[hr][j] = (uint32_t)__ldg(p.drop_ffn.bits + ((uint64_t)((int64_t)m * p.ffn + n) >> 3)) >> (2 * q);
-          if (!B_MN && p.mask_src && m < p.M)
-            ew[hr][j] = __ldg(reinterpret_cast<const uint32_t*>(reinterpret_cast<const uint16_t*>(p.mask_src) + (int64_t)m * p.mask_ld + n));
-        }
-      }
-      // ---- GEMM1: hidden accumulator [64 x 64] ----
-      float hid[32];
+    for (int i = 0; i < 4; ++i) a16[k][i] = 0u;
+  float2 bias[8];
 #pragma unroll
-      for (int i = 0; i < 32; ++i) hid[i] = 0.f;
-      if (h == 0) {
-#pragma unroll
-        for (int s2 = 0; s2 < kW1Items; ++s2) w1src[s2] = stage_get(item0 + s2);
-      }
-      ptx::fence_acc(hid);
-      ptx::wgmma_fence();
-#pragma unroll
-      for (int kb = 0; kb < kbx; ++kb) {
-        const uint32_t sa = sX + (uint32_t)kb * kABytes + (uint32_t)wg * 8192u;
-        const uint32_t sb = w1src[kb >> 1] + (uint32_t)(kb & 1) * 16384u + (uint32_t)h * 8192u;
-#pragma unroll
-        for (int k = 0; k < BK / 16; ++k)
-          ptx::WgmmaSS<64, BF, 0, B_MN>::mma(hid, ptx::desc_kmajor(sa, k), B_MN ? ptx::desc_mnmajor(sb, k) : ptx::desc_kmajor(sb, k),
-                                             (kb > 0 || k > 0) ? 1 : 0);
-      }
-      ptx::wgmma_commit();
-      // keep bits of element pair (row m0 + 8 hr, columns n0 + 8 j + {0, 1}): bits 16 hr + 2 j + {0, 1}
-      uint32_t keep = 0u;
-#pragma unroll
-      for (int hr = 0; hr < 2; ++hr) {
-#pragma unroll
-        for (int j = 0; j < 8; ++j) {
-          const uint32_t w = ew[hr][j];
-          uint32_t k2 = w & 3u;
-          if (!B_MN && p.mask_src) {
-            // 16-bit mask source (bf16 / fp16): "> 0" <=> sign clear and magnitude bits non-zero
-            const uint32_t lo = w & 0xffffu, hi = w >> 16;
-            k2 = ((lo != 0u && lo < 0x8000u) ? 1u : 0u) | ((hi != 0u && hi < 0x8000u) ? 2u : 0u);
-          }
-          keep |= k2 << (16 * hr + 2 * j);
-        }
-      }
-      asm volatile("" : "+r"(keep));            // computed before the wait, not after it
-      ptx::wgmma_wait<0>();
-      ptx::fence_acc(hid);
-      if (h == 1) {
-#pragma unroll
-        for (int s2 = 0; s2 < kW1Items; ++s2) release(item0 + s2);
-      }
-      // ---- hidden epilogue on the fragments: bias, ReLU, dropout (forward) / relu'-dropout' mask (backward); store; pack ----
-      uint32_t a16[4][4];
+  for (int j = 0; j < 8; ++j) bias[j] = make_float2(0.f, 0.f);
+  uint32_t keep = 0u;
+  // Step s; G2 / G1 are compile-time flags (false for the first / last step), so that no wgmma sits on a path the compiler
+  // must treat as divergent (ptxas would serialize them).
+  auto step = [&](const int s, auto G2, auto G1) {
+    if constexpr (decltype(G2)::value) {
+      // ---- hidden epilogue of half s - 1: bias, ReLU, dropout (forward) / relu'-dropout' mask (backward); store; pack ----
+      const int n0 = hid0 + (s - 1) * 64 + 2 * q;
 #pragma unroll
       for (int j = 0; j < 8; ++j) {
         const int n = n0 + 8 * j;
-        float2 bb = make_float2(0.f, 0.f);
-        if (p.b1) bb = __ldg(reinterpret_cast<const float2*>(p.b1 + n));
 #pragma unroll
         for (int hr = 0; hr < 2; ++hr) {
           const int m = m0 + 8 * hr;
           const bool row_ok = m < p.M;
-          float v0 = fmaxf(fmaf(hid[4 * j + 2 * hr], p.alpha, bb.x), hidden_floor);
-          float v1 = fmaxf(fmaf(hid[4 * j + 2 * hr + 1], p.alpha, bb.y), hidden_floor);
+          float v0 = fmaxf(fmaf(hid[4 * j + 2 * hr], p.alpha, bias[j].x), hidden_floor);
+          float v1 = fmaxf(fmaf(hid[4 * j + 2 * hr + 1], p.alpha, bias[j].y), hidden_floor);
           const uint32_t k2 = keep >> (16 * hr + 2 * j);
-          if (use_bits && row_ok) {
+          if ((use_bits || use_mask) && row_ok) {
             v0 = (k2 & 1u) ? v0 * dscale : 0.f;
             v1 = (k2 & 2u) ? v1 * dscale : 0.f;
-          }
-          if (!B_MN && p.mask_src && row_ok) {
-            if (!(k2 & 1u)) v0 = 0.f;
-            if (!(k2 & 2u)) v1 = 0.f;
           }
           const uint32_t pk = pack2_16(v0, v1, DT);
           if (row_ok) *reinterpret_cast<uint32_t*>(p.F1 + (int64_t)m * p.ffn + n) = pk;
           a16[j >> 1][(j & 1) * 2 + hr] = pk;
         }
       }
-      // ---- GEMM2: out[64 x D] += hidden half (registers) x the matching 64 rows of the W2 chunk ----
-      const int w2_item = item0 + kW1Items + h;
-      const uint32_t src = stage_get(w2_item);
-      ptx::fence_acc(out);
-      ptx::wgmma_fence();
+    }
+    // ---- step s, in this warpgroup's turn: GEMM2 of half s - 1 (out[64 x D] += hidden half x W2 rows), GEMM1 of half s ----
+    if (G2 || wg == 1) ptx::named_bar_sync(kOrderBar + wg, 256);
+    const uint32_t src = G2 ? stage_get(2 * s - 1) : 0u;          // both waits before the wgmmas: none sits between them
+    const uint32_t w1 = G1 ? stage_get(2 * s) : 0u;
+    ptx::fence_acc(out);
+    ptx::fence_acc(hid);
+    ptx::wgmma_fence();
+    if constexpr (decltype(G2)::value) {
 #pragma unroll
       for (int k = 0; k < BK / 16; ++k)
         ptx::WgmmaRS<D, BF, B_MN>::mma(out, a16[k], B_MN ? ptx::desc_mnmajor(src, k) : ptx::desc_kmajor(src, k),
-                                       (c > 0 || h > 0 || k > 0) ? 1 : 0);
+                                       (s > 1 || k > 0) ? 1 : 0);
       ptx::wgmma_commit();
-      ptx::wgmma_wait<0>();
-      ptx::fence_acc(out);
-      release(w2_item);
     }
-  }
+    if constexpr (decltype(G1)::value) {
+#pragma unroll
+      for (int kb = 0; kb < kbx; ++kb) {
+        const uint32_t sa = sX + (uint32_t)kb * kABytes + (uint32_t)wg * 8192u;
+        const uint32_t sb = w1 + (uint32_t)kb * 8192u;
+#pragma unroll
+        for (int k = 0; k < BK / 16; ++k)
+          ptx::WgmmaSS<64, BF, 0, B_MN>::mma(hid, ptx::desc_kmajor(sa, k), B_MN ? ptx::desc_mnmajor(sb, k) : ptx::desc_kmajor(sb, k),
+                                             (kb > 0 || k > 0) ? 1 : 0);
+      }
+      ptx::wgmma_commit();
+    }
+    if (G1 || wg == 0) ptx::named_bar_arrive(kOrderBar + (wg ^ 1), 256);
+    if constexpr (decltype(G1)::value) {
+      keep = fold_keep();
+      if (s + 1 < H) load_ew(s + 1);
+      if (B_MN && p.b1) {
+#pragma unroll
+        for (int j = 0; j < 8; ++j) bias[j] = __ldg(reinterpret_cast<const float2*>(p.b1 + hid0 + s * 64 + 8 * j + 2 * q));
+      }
+    }
+    asm volatile("" : "+r"(keep));            // folded while the wgmmas run, not after the wait
+    ptx::wgmma_wait<0>();
+    ptx::fence_acc(out);
+    ptx::fence_acc(hid);
+#pragma unroll
+    for (int k = 0; k < 4; ++k)
+#pragma unroll
+      for (int i = 0; i < 4; ++i) asm volatile("" : "+r"(a16[k][i]) :: "memory");   // GEMM2 reads them until the wait
+    if (G2) release(2 * s - 1);
+    if (G1) release(2 * s);
+  };
+  load_ew(0);
+  ptx::mbar_wait(x_full, 0);
+  step(0, std::false_type{}, std::true_type{});
+  for (int s = 1; s < H; ++s) step(s, std::true_type{}, std::true_type{});
+  step(H, std::true_type{}, std::false_type{});
   // ---- output rows: (+ b2 on slice 0) -> post dropout -> fp32 add into x_out ----
   const bool add_b2 = split == 0 && p.b2 != nullptr;
   const bool post = p.drop_post.p > 0.f;
@@ -1113,7 +1139,9 @@ static int mlp_splits(int m_tiles, int chunks, int* splits) {
 int fused_mlp_fwd(const void* X, int dtype, int M, int d, int ffn, const void* W1, const float* b1, const void* W2, const float* b2,
                   DropoutSpec drop_ffn, DropoutSpec drop_post, void* F1, float* x_out, cudaStream_t stream, int* tickets) {
   B200ST_CHECK(fused_mlp_supported(M, d, ffn, dtype), "fused MLP: unsupported shape / dtype");
-  if (drop_ffn.p > 0.f) B200ST_CHECK(drop_ffn.bits != nullptr, "fused MLP needs precomputed dropout bits");
+  if (drop_ffn.p > 0.f)
+    B200ST_CHECK(drop_ffn.bits != nullptr && (reinterpret_cast<uintptr_t>(drop_ffn.bits) & 7) == 0,
+                 "fused MLP needs precomputed, 8-byte aligned dropout bits");
   if (drop_post.p > 0.f) B200ST_CHECK(drop_post.bits != nullptr, "fused MLP needs precomputed dropout bits");
   const int m_tiles = ceil_div(M, BM), chunks = ffn / 128;
   int splits = 1;
@@ -1159,7 +1187,7 @@ int fused_mlp_bwd(const void* dY, int dtype, int M, int d, int ffn, const void* 
                (reinterpret_cast<uintptr_t>(F1) & 3) == 0, "fused MLP: unaligned buffer");
   CUtensorMap tx, tw1, tw2;
   B200ST_TRY(make_operand_map(GemmOperand{dY, dtype, 0, d, 0, 0}, M, d, 1, 1, BM, &tx));
-  B200ST_TRY(make_operand_map(GemmOperand{W2, dtype, 0, d, 0, 0}, ffn, d, 1, 1, 128, &tw1));     // G1: rows = hidden units, k = d
+  B200ST_TRY(make_operand_map(GemmOperand{W2, dtype, 0, d, 0, 0}, ffn, d, 1, 1, 64, &tw1));      // G1: rows = hidden units, k = d
   B200ST_TRY(make_operand_map(GemmOperand{W1, dtype, 0, ffn, 0, 0}, d, ffn, 1, 1, d, &tw2));      // G2: rows = model dims, k = hidden
   auto kern = d == 256 ? (dtype == F16 ? fused_mlp_fwd_kernel<F16, false, 256> : fused_mlp_fwd_kernel<BF16, false, 256>)
                        : (dtype == F16 ? fused_mlp_fwd_kernel<F16, false, 128> : fused_mlp_fwd_kernel<BF16, false, 128>);
