@@ -227,6 +227,39 @@ typedef struct {
 int64_t b200st_beam_state_bytes(b200st_handle h, int32_t B, int32_t beam_size, int32_t max_len);
 int b200st_beam_search(b200st_handle h, const b200st_buffers* buf, const b200st_decode_state* st, const b200st_beam_args* a,
                        void* stream);
+/* Top-k / nucleus sampling: sequence_sampling_search of TopSampling (neurst/layers/search/sampling.py:76-250).  Each utterance
+ * is tiled sample_num times (row b*sample_num + s is sample s of utterance b).  Per step and row: UNK is masked to FLOAT_MIN
+ * (unk_id < 0: not masked), EOS too while time < min_len - 1; the filter keeps the logits >= the k-th largest (top_k > 0,
+ * ties kept) or >= the largest value whose upper tail holds softmax mass >= top_p (top_p < 1; everything when no value
+ * reaches it); then one id is drawn.  The draw of global row g = row_offset + row at step t: x = the first word of
+ * Philox4x32-7(key seed, counter t, stream g) (the dropout generator), u = (x >> 8) * 2^-24, and the id is the first
+ * vocabulary index, in index order, whose running sum of kept weights exp(z - max) exceeds u * (their total).  A row that
+ * has emitted EOS emits EOS; the search stops when every row has, or after max_steps = max(min(T' + extra_decode_length,
+ * maximum_decode_length), minimum_decode_length).  out_logprob: the sum over the drawn ids of the masked, unfiltered
+ * log-softmax (the model's log-probability of the sample); out_len: the ids drawn up to and including the first EOS.
+ *   st as for b200st_beam_search with beam_size = sample_num (st->B counts utterances); sample_num <= 8; B*sample_num <= 8
+ *   with st->use_shadow 0, <= B200ST_DECODE_MAX_ROWS with use_shadow 1.  out_ids [B*sample_num][max_steps] padded with EOS.
+ *   state_words: b200st_beam_state_bytes(h, B, sample_num, st->max_len) bytes.  use_graph: 1 = captured step graph, 0 = eager.
+ * The selection uses fixed-order reductions only: on the wide step (above 8 rows) the ids are bit-reproducible and a row's
+ * ids do not depend on the other rows of the call.  Invalid arguments (top_k < 0 or > vocab, top_k > 0 with top_p < 1, a
+ * non-finite top_p, too many rows, max_steps > max_len, null buffers) fail before anything is launched. */
+typedef struct {
+  const int64_t* bos_ids;       /* [B] */
+  int32_t eos_id, unk_id, min_len, max_steps;
+  int32_t sample_num, top_k;
+  float top_p;
+  uint64_t seed;
+  int64_t row_offset;           /* global index of row 0 in the draws' key */
+  int64_t* out_ids; float* out_logprob; int32_t* out_len;
+  void* state_words;
+  int32_t use_graph;
+} b200st_sampling_args;
+int b200st_sampling_search(b200st_handle h, const b200st_buffers* buf, const b200st_decode_state* st, const b200st_sampling_args* a,
+                           void* stream);
+/* The same selection on caller logits fp32 [rows, V], without masks (top_k_logits / top_p_logits + one categorical draw):
+ * out_ids[r] draws with the key (seed, row_offset + r, step). */
+int b200st_sample_logits(const float* logits, int32_t rows, int32_t V, int32_t top_k, float top_p, uint64_t seed, int64_t row_offset,
+                         int32_t step, int64_t* out_ids, void* stream);
 /* Ensemble decoding: sequence_beam_search over EncoderDecoderEnsembleModel (neurst/models/encoder_decoder_ensemble_model.py;
  * neurst/layers/search/beam_search.py:97-115,486-515).  Per step every member runs its decoder step on the same rows, and the
  * search continues from log(sum_m w_m softmax(logits_m)) (evaluated as a log-sum-exp over the members) with the masks,

@@ -17,7 +17,9 @@ summary_steps, save_checkpoint_steps, update_cycle, clip_value, clip_norm, crite
 lr_schedule.params, pretrain_model}, dataset.class AudioTFRecordDataset / dataset.params, task.class SpeechToText /
 task.params, model.class / model.params / hparams_set, model_dir, dtype, and for `predict` the keys of the prediction
 recipes: `entry: predict` (the alias of entry.class) and search_method beam_search / search_method.params {beam_size,
-length_penalty, top_k, maximum_decode_length, extra_decode_length, minimum_decode_length, enable_unk}, and the top-level
+length_penalty, top_k, maximum_decode_length, extra_decode_length, minimum_decode_length, enable_unk} or search_method
+top_sampling / search_method.params {sample_num, top_k, top_p, maximum_decode_length, extra_decode_length,
+minimum_decode_length} (sample_num lines per utterance, drawn with entry.params random_seed), and the top-level
 batch_size (utterances per call; with a 16-bit dtype decoded from the 16-bit weights).  Several model_dirs (a yaml list or a
 comma-separated string) make `predict` decode with their ensemble, weighted by search_method.params / entry.params
 ensemble_weights ("average" or comma-separated numbers); each member is rebuilt from its model_configs.yml, which `train`
@@ -154,19 +156,38 @@ def _module_name(cfg, name):
 def resolve_search(cfg, ep, tp):
     """Search settings of `predict`.  Without search_method: greedy with the lengths of entry.params (as before).  With
     search_method BeamSearch: its parameters (search_method.params, then entry.params) with BeamSearch's defaults
-    (beam_search.py:465-490)."""
+    (beam_search.py:465-490).  With TopSampling (registered as TopSampling, topsampling and top_sampling): its parameters
+    from the same places with Sampling's defaults (sampling.py:290-313) and its two refusals."""
     length_default = int(ep.get("maximum_decode_length", tp.get("max_trg_len") or 256))
     method = _module_name(cfg, "search_method")
     if method is None:
         return None, {"maximum_decode_length": length_default, "extra_decode_length": int(ep.get("extra_decode_length", 50)),
                       "minimum_decode_length": int(ep.get("minimum_decode_length", 0))}
-    if str(method).lower().replace("_", "") != "beamsearch":
-        raise SystemExit("search_method %r is outside this path (beam_search only)" % method)
+    name = str(method).lower().replace("_", "")
+    if name not in ("beamsearch", "topsampling"):
+        raise SystemExit("search_method %r is outside this path (beam_search, top_sampling)" % method)
     sp = dict(cfg.get("search_method.params") or {})
 
     def get(key, default):
         v = sp.get(key, ep.get(key))
         return default if v is None else v
+
+    if name == "topsampling":
+        search = {"maximum_decode_length": int(get("maximum_decode_length", length_default)),
+                  "extra_decode_length": int(get("extra_decode_length", 50)),
+                  "minimum_decode_length": int(get("minimum_decode_length", 0) or 0),
+                  "sample_num": int(get("sample_num", 1)), "top_k": int(get("top_k", 0)), "top_p": float(get("top_p", 1.0))}
+        if search["top_k"] > 0 and search["top_p"] < 1:               # Sampling.__init__
+            raise SystemExit("top_sampling: Not implemented search logic when top_k > 0 and top_p < 1.")
+        if search["minimum_decode_length"] >= search["maximum_decode_length"]:       # Sampling.call
+            raise SystemExit("top_sampling: `minimum_decode_length` must be less than maximum decode length.")
+        if not 1 <= search["sample_num"] <= 8:
+            raise SystemExit("top_sampling: sample_num must be in 1..8 (the samples of an utterance share a decoding step), "
+                             "got %d" % search["sample_num"])
+        if search["top_k"] < 0 or search["top_p"] != search["top_p"] or abs(search["top_p"]) == float("inf"):
+            raise SystemExit("top_sampling: top_k must be >= 0 and top_p finite, got top_k %d, top_p %r"
+                             % (search["top_k"], search["top_p"]))
+        return "top_sampling", search
 
     lp = sp.get("length_penalty", ep.get("length_penalty", 0.6))
     return "beam_search", {"maximum_decode_length": int(get("maximum_decode_length", length_default)),
@@ -234,6 +255,8 @@ def resolve_validator(cfg, tp):
                              "is task.params' *_data_pipeline.params.language)" % ", ".join(sorted(metric_params)))
         if method is not None:
             plan["search_method"], plan["search"] = resolve_search({"search_method": method, "search_method.params": sp}, {}, tp)
+            if plan["search_method"] != "beam_search":
+                raise SystemExit("eval_search_method %r is outside this path for validation (beam_search only)" % method)
         language = "en"                     # the metric's language: the target data pipeline's (get_eval_metric)
         for k in ("transcript_data_pipeline.params", "trg_data_pipeline.params", "translation_data_pipeline.params"):
             if isinstance(tp.get(k), dict) and tp[k].get("language"):
@@ -325,6 +348,10 @@ def resolve(cfg, world=1):
             # eval_batch_size x beam_size must fit a decoding step: refused now, not at the first validation
             from neurst_b200.validation import generation_plan
             decode_settings(generation_plan(plan))
+    if len(model_dirs) > 1 and search_method == "top_sampling":
+        # EncoderDecoderEnsembleModel hands TopSampling one logits tensor per member, which its search cannot take
+        raise SystemExit("search_method top_sampling is outside this path for an ensemble of %d model_dirs (beam_search only)"
+                         % len(model_dirs))
     if len(model_dirs) > 1:
         # BeamSearch's ensemble_weights: search_method.params, then entry.params (where the flat --ensemble_weights lands)
         sp = cfg.get("search_method.params") or {}
@@ -567,10 +594,12 @@ def decode_settings(plan):
     to MAX_ROWS_SHADOW rows (utterances x beam) per step; the fp32 weights hold MAX_ROWS rows per step."""
     from neurst_b200.decode import MAX_ROWS, MAX_ROWS_SHADOW
     beam = plan.get("search_method") == "beam_search"
-    width = plan["search"]["beam_size"] if beam else 1
+    sampling = plan.get("search_method") == "top_sampling"
+    width = plan["search"]["beam_size"] if beam else plan["search"]["sample_num"] if sampling else 1
+    what = "sample_num" if sampling else "beam_size"
     per_call = MAX_ROWS // width
     if per_call < 1:
-        raise SystemExit("beam_size %d exceeds the %d rows a decoding step holds" % (plan["search"]["beam_size"], MAX_ROWS))
+        raise SystemExit("%s %d exceeds the %d rows a decoding step holds" % (what, width, MAX_ROWS))
     search_kw = dict(plan["search"])
     if plan.get("batch_size") is not None:
         if plan["precision"] == "fp32":
@@ -579,16 +608,23 @@ def decode_settings(plan):
             per_call = min(per_call, plan["batch_size"])
         else:
             if not 1 <= plan["batch_size"] * width <= MAX_ROWS_SHADOW:
-                raise SystemExit("batch_size %d x beam_size %d exceeds the %d rows a decoding step holds"
-                                 % (plan["batch_size"], width, MAX_ROWS_SHADOW))
+                raise SystemExit("batch_size %d x %s %d exceeds the %d rows a decoding step holds"
+                                 % (plan["batch_size"], what, width, MAX_ROWS_SHADOW))
             per_call = plan["batch_size"]
             search_kw["use_shadow"] = True
     return per_call, search_kw
 
 
-def decode_group(model, task, plan, group, search_kw):
-    """One search call over preprocessed samples -> [(ids_to_text hypothesis, score)], top_k rows per utterance,
-    consecutive (the reference's [B*top_k] order)."""
+def sampling_seed(seed, rank):
+    """The draws' seed of one rank: the run's random_seed with the rank folded in (rank 0 keeps it)."""
+    return (int(seed) + int(rank) * 0x9E3779B97F4A7C15) & 0xFFFFFFFFFFFFFFFF
+
+
+def decode_group(model, task, plan, group, search_kw, first=0):
+    """One search call over preprocessed samples -> [(ids_to_text hypothesis, score)], top_k (beam search) or sample_num
+    (top_sampling) rows per utterance, consecutive (the reference's [B*top_k] order).  `first`: the position of group[0] in
+    the rank's stream of utterances, which keys the samples' draws (row offset first * sample_num), so the samples do not
+    depend on how the stream is cut into calls."""
     tm = plan["trg_meta"]
     dim = plan["task"]["audio_feature_dim"] * plan["task"]["audio_feature_channels"]
     T = max(int(e["audio_length"]) for e in group)
@@ -596,7 +632,11 @@ def decode_group(model, task, plan, group, search_kw):
     for j, e in enumerate(group):
         src[j, :int(e["audio_length"])] = e["audio"]
     batch = task.example_to_input({"audio": src, "audio_length": torch.tensor([int(e["audio_length"]) for e in group])}, infer=True)
-    search = model.beam_search if plan.get("search_method") == "beam_search" else model.greedy_search
+    method = plan.get("search_method")
+    if method == "top_sampling":
+        search, search_kw = model.sampling_search, dict(search_kw, row_offset=int(first) * plan["search"]["sample_num"])
+    else:
+        search = model.beam_search if method == "beam_search" else model.greedy_search
     ids, score = search({"src": batch["src"], "src_length": batch["src_length"]}, **search_kw)
     return [(ids_to_text(row, tm["eos_id"], tm.get("tokens")), lp) for row, lp in zip(ids.cpu().tolist(), score.cpu().tolist())]
 
@@ -618,15 +658,19 @@ def predict(plan):
     per_call, search_kw = decode_settings(plan)
     if ensemble:
         search_kw["ensemble_weights"] = plan["ensemble_weights"]
+    if plan.get("search_method") == "top_sampling":
+        search_kw["seed"] = sampling_seed(plan["seed"], rank)
     hyps = []
     group = []
+    done = 0
     for ex in examples:
         group.append(ex)
         if len(group) == per_call:
-            hyps.extend(decode_group(model, task, plan, group, search_kw))
+            hyps.extend(decode_group(model, task, plan, group, search_kw, first=done))
+            done += len(group)
             group = []
     if group:
-        hyps.extend(decode_group(model, task, plan, group, search_kw))
+        hyps.extend(decode_group(model, task, plan, group, search_kw, first=done))
     out = plan["output_file"]
     if out and rank == 0:
         with open(out, "w", encoding="utf-8") as f:

@@ -29,6 +29,35 @@ struct EnsembleMix {
   int n;
 };
 
+// One step of the sampling search over `rows` rows (sampling.cu), or one draw per row of caller logits (step >= 0, no
+// masks, out[row]).  Row r draws with the key (seed, row_offset + r, step); the search reads the step from *time.
+struct SampleRows {
+  const float* logits;   // [rows, V]
+  int V;
+  int eos, unk, min_len; // UNK masked unless unk < 0; EOS masked while time < min_len - 1
+  int top_k;             // 0: no top-k filter
+  float top_p;           // < 1: the nucleus filter (top_k must be 0)
+  uint64_t seed;
+  int64_t row_offset;    // global index of row 0
+  int step;              // b200st_sample_logits: the step index of the key
+  int64_t* ids;          // [rows] current input ids
+  int32_t* finished;     // [rows]
+  int32_t* length;       // [rows]
+  float* logprob;        // [rows]
+  int64_t* out;          // [rows, max_steps] (b200st_sample_logits: [rows])
+  int max_steps;
+  int32_t* time;
+  int32_t* all_finished;
+  uint32_t* ticket;
+};
+// top_k / top_p as TopSampling takes them (finite top_p, 0 <= top_k <= V, not both filters)
+int check_sample_filter(int top_k, float top_p, int V);
+// sequence_sampling_search's initial state on rows = utterances x sample_num, the identity ancestry table and EOS-padded
+// output rows
+void sample_init(const BeamState& bs, const int64_t* bos, int rows, int sample_num, int max_len, int64_t* out, int max_steps,
+                 int eos, float* logprob, int32_t* length, cudaStream_t s);
+void sample_select(const SampleRows& a, int rows, cudaStream_t s);
+
 // lp[r, v] = log sum_m w_m softmax(z_m[r])[v], written over member 0's logits (one block per row, members in order)
 void ensemble_logprob(const EnsembleMix& mix, int rows, int V, cudaStream_t s);
 // beam_select_kernel on rows that already hold log-probabilities (the ensemble's mixture)

@@ -262,6 +262,20 @@ int b200st_beam_search(b200st_handle h, const b200st_buffers* buf, const b200st_
   if (!h || !buf || !st || !a) B200ST_FAIL("null argument");
   return beam_search(h->m, to_buffers(buf), to_state(st), to_beam_args(a), reinterpret_cast<cudaStream_t>(stream));
 }
+int b200st_sampling_search(b200st_handle h, const b200st_buffers* buf, const b200st_decode_state* st, const b200st_sampling_args* a,
+                           void* stream) {
+  if (!h || !buf || !st || !a) B200ST_FAIL("null argument");
+  SamplingArgs g{};
+  g.bos_ids = a->bos_ids; g.eos_id = a->eos_id; g.unk_id = a->unk_id; g.min_len = a->min_len; g.max_steps = a->max_steps;
+  g.sample_num = a->sample_num; g.top_k = a->top_k; g.top_p = a->top_p; g.seed = a->seed; g.row_offset = a->row_offset;
+  g.out_ids = a->out_ids; g.out_logprob = a->out_logprob; g.out_len = a->out_len; g.state_words = a->state_words;
+  g.use_graph = a->use_graph;
+  return sampling_search(h->m, to_buffers(buf), to_state(st), g, reinterpret_cast<cudaStream_t>(stream));
+}
+int b200st_sample_logits(const float* logits, int32_t rows, int32_t V, int32_t top_k, float top_p, uint64_t seed, int64_t row_offset,
+                         int32_t step, int64_t* out_ids, void* stream) {
+  return sample_logits(logits, rows, V, top_k, top_p, seed, row_offset, step, out_ids, reinterpret_cast<cudaStream_t>(stream));
+}
 static_assert(B200ST_ENSEMBLE_MAX_MODELS == kEnsembleMaxModels, "include/b200st.h and model.cuh disagree on the ensemble size");
 int b200st_ensemble_beam_search(const b200st_ensemble_member* members, int32_t n_members, const b200st_beam_args* a, void* stream) {
   if (n_members < 1 || n_members > B200ST_ENSEMBLE_MAX_MODELS)

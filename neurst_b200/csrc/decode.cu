@@ -1114,6 +1114,54 @@ int beam_search(const Model& m, const Buffers& buf, const DecodeState& st, const
   return 0;
 }
 
+// sequence_sampling_search (sampling.py:103-250) on B x sample_num rows: row u*sample_num + s is sample s of utterance u.
+// The rows never reorder, so the ancestry table stays the identity (each row reads its own self-attention cache) and the
+// beam variants of the step read the memory of utterance row / sample_num; sample_select_kernel (sampling.cu) draws.
+int sampling_search(const Model& m, const Buffers& buf, const DecodeState& st, const SamplingArgs& a, cudaStream_t s) {
+  B200ST_TRY(check_state(m, st));
+  const Config& cf = m.cfg;
+  const int n = a.sample_num;
+  B200ST_CHECK(n >= 1 && n <= KMAX, "sample_num must be in 1.." + std::to_string(KMAX) + ", got " + std::to_string(n));
+  B200ST_TRY(check_sample_filter(a.top_k, a.top_p, cf.vocab));
+  const int max_rows = st.use_shadow ? kDecodeMaxRows : MAXB;      // more than 8 rows: the wide step, 16-bit shadow only
+  B200ST_CHECK((int64_t)st.B * n <= max_rows, "sampling search decodes at most " + std::to_string(max_rows) +
+                                              " rows (utterances x sample_num) per call, got " + std::to_string(st.B) + " x " +
+                                              std::to_string(n));
+  B200ST_CHECK(a.max_steps >= 1 && a.max_steps <= st.max_len, "max_steps must be within the cache length");
+  B200ST_CHECK(a.row_offset >= 0, "row_offset must be >= 0");
+  B200ST_CHECK(a.bos_ids && a.out_ids && a.out_len && a.out_logprob && a.state_words, "sampling_search: null argument");
+  const int rows = st.B * n;
+  DecodeState rs = st;                    // the step runs on every sample row; cross_kv / memory_bias stay per utterance
+  rs.B = rows;
+  B200ST_TRY(check_state(m, rs));
+  if (rows > MAXB) B200ST_TRY(rows_check(m, buf, rs, n));
+  const size_t smem_self = self_attn_smem(cf, st.max_len, true);
+  B200ST_CHECK(smem_self <= 200 * 1024, "decode: too many keys for the shared-memory score buffer");
+  B200ST_TRY(raise_all_smem(cf, st));
+  B200ST_TRY(raise_beam_smem(smem_self, cross_attn_smem(cf, st.Tm)));
+  BeamState bs = beam_state_at(a.state_words, rows, st.max_len);
+  float* logits = rs.scratch + (rows > MAXB ? rows_logits_offset(cf, rows) : layout_of(cf, rows).logits);
+  sample_init(bs, a.bos_ids, rows, n, st.max_len, a.out_ids, a.max_steps, a.eos_id, a.out_logprob, a.out_len, s);
+  B200ST_CUDA(cudaGetLastError());
+  SampleRows sr{};
+  sr.logits = logits; sr.V = cf.vocab; sr.eos = a.eos_id; sr.unk = a.unk_id; sr.min_len = a.min_len;
+  sr.top_k = a.top_k; sr.top_p = a.top_p; sr.seed = a.seed; sr.row_offset = a.row_offset;
+  sr.ids = bs.ids; sr.finished = bs.finished; sr.length = a.out_len; sr.logprob = a.out_logprob;
+  sr.out = a.out_ids; sr.max_steps = a.max_steps;
+  sr.time = bs.time; sr.all_finished = bs.all_finished; sr.ticket = bs.ticket;
+  StepCtx c{m, buf, rs, s};
+  auto one_step = [&]() -> int {
+    B200ST_TRY(step_dispatch(c, bs.ids, bs.time, logits, bs.anc, n));
+    sample_select(sr, rows, s);
+    B200ST_LAUNCH_CHECK();
+    return 0;
+  };
+  bool graphed = false;
+  B200ST_TRY(run_token_loop(s, a.max_steps, a.use_graph != 0, bs.all_finished, one_step, &graphed));
+  B200ST_CHECK(graphed || !a.use_graph, "sampling search could not capture its step into a CUDA graph");
+  return 0;
+}
+
 // sequence_beam_search over EncoderDecoderEnsembleModel (encoder_decoder_ensemble_model.py, beam_search.py:97-115): per
 // token every member steps on the same B x beam rows (its own self-attention cache, cross K/V and scratch; the shared ids
 // and ancestry table of the one beam state), ensemble_logprob mixes their distributions over member 0's logits, and

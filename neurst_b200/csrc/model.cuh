@@ -154,6 +154,25 @@ struct BeamArgs {
 int64_t beam_state_bytes(int B, int beam, int max_len);
 // st.B counts utterances; self_kv and scratch are sized for B * beam_size rows, cross_kv / memory_bias for B
 int beam_search(const Model& m, const Buffers& buf, const DecodeState& st, const BeamArgs& a, cudaStream_t s);
+struct SamplingArgs {
+  const int64_t* bos_ids;        // [B] device, one per utterance
+  int eos_id, unk_id;            // unk_id < 0: UNK allowed
+  int min_len, max_steps;
+  int sample_num, top_k;         // top_k 0: no top-k filter
+  float top_p;                   // < 1: nucleus filter
+  uint64_t seed;
+  int64_t row_offset;            // global index of row 0 (the draws' key)
+  int64_t* out_ids;              // [B * sample_num, max_steps] device, padded with EOS
+  float* out_logprob;            // [B * sample_num]
+  int32_t* out_len;              // [B * sample_num]
+  void* state_words;             // >= beam_state_bytes(B, sample_num, max_len)
+  int use_graph;
+};
+// sequence_sampling_search (TopSampling) with the per-token step of beam_search on B x sample_num rows; st as beam_search's
+int sampling_search(const Model& m, const Buffers& buf, const DecodeState& st, const SamplingArgs& a, cudaStream_t s);
+// one draw per row of caller logits [rows, V], no masks: out[r] with the key (seed, row_offset + r, step) (sampling.cu)
+int sample_logits(const float* logits, int rows, int V, int top_k, float top_p, uint64_t seed, int64_t row_offset, int step,
+                  int64_t* out, cudaStream_t s);
 constexpr int kEnsembleMaxModels = 8;      // B200ST_ENSEMBLE_MAX_MODELS
 struct EnsembleMember {
   const Model* m;

@@ -4,10 +4,11 @@ Host mirror of
   EncoderDecoderModel.get_symbols_to_logits_fn      neurst/models/encoder_decoder_model.py:211-261
   TransformerDecoder.create_decoding_internal_cache neurst/layers/decoders/transformer_decoder.py:105-147
   sequence_beam_search                              neurst/layers/search/beam_search.py:254-439
+  sequence_sampling_search                          neurst/layers/search/sampling.py:103-250
   SequenceGenerator                                 neurst/exps/sequence_generator.py:62-86
 
 Everything numeric is a library call (b200st_encode / b200st_decode_init / b200st_decode_step / b200st_greedy_search /
-b200st_beam_search / b200st_ensemble_beam_search):
+b200st_beam_search / b200st_ensemble_beam_search / b200st_sampling_search):
 the key/value caches are preallocated device buffers owned by `DecodingCache`, the token ids and the position live on the
 device, and the greedy loop replays one captured CUDA graph per token inside the library.
 """
@@ -344,3 +345,91 @@ def ensemble_beam_search(rts, inputs, bos_id, eos_id, unk_id=None, weights="aver
     if steps < maximum_decode_length:      # padded to the fixed output length with EOS (beam_search.py:428-436)
         out = torch.cat([out, torch.full((k, maximum_decode_length - steps), int(eos_id), dtype=torch.int64, device=dev)], 1)
     return out, scores, logprob, length
+
+
+DEFAULT_SAMPLING_SEED = 1234      # the entries' default random_seed
+
+
+def _check_sampling_filter(top_k, top_p):
+    """Sampling.__init__'s refusal (sampling.py:313-314)."""
+    if top_k > 0 and top_p < 1:
+        raise NotImplementedError("Not implemented search logic when top_k > 0 and top_p < 1.")
+
+
+def sampling_search(rt, inputs, bos_id, eos_id, unk_id, sample_num=1, top_k=0, top_p=1.0, maximum_decode_length=256,
+                    extra_decode_length=50, minimum_decode_length=0, seed=DEFAULT_SAMPLING_SEED, row_offset=0, use_shadow=False,
+                    use_graph=True, cache=None):
+    """sequence_sampling_search of TopSampling (neurst/layers/search/sampling.py:103-250) on the device: each utterance is
+    decoded `sample_num` times (row b * sample_num + s is sample s of utterance b), every step masks UNK (unk_id None: not
+    masked) and, before minimum_decode_length, EOS; keeps the top_k logits (top_k > 0) or the nucleus of mass top_p
+    (top_p < 1); and draws one id per row with the keyed Philox draw of include/b200st.h (seed, global row
+    row_offset + row, step).  A row that has emitted EOS emits EOS.  Returns (ids int64 [B*sample_num, maximum_decode_length]
+    padded with EOS, log-probability fp32 [B*sample_num] of the drawn ids under the masked, unfiltered softmax, decoding
+    length int32 [B*sample_num]).  At most max_rows(use_shadow) // sample_num utterances per call, sample_num <= 8."""
+    sample_num, top_k, top_p = int(sample_num), int(top_k), float(top_p)
+    _check_sampling_filter(top_k, top_p)
+    if minimum_decode_length >= maximum_decode_length:          # Sampling.call (sampling.py:330-331)
+        raise ValueError("`minimum_decode_length` must be less than maximum decode length.")
+    if not 1 <= sample_num <= 8:
+        raise L.B200STError("sample_num must be in 1..8, got %d" % sample_num)
+    if cache is None:
+        B = int(inputs["src"].shape[0])
+        if B * sample_num > max_rows(use_shadow):
+            raise L.B200STError("sampling search decodes at most %d rows (utterances x sample_num) per call, got %d x %d"
+                                % (max_rows(use_shadow), B, sample_num))
+        enc, bias = encode(rt, inputs)
+        cache = create_decoding_cache(rt, enc, bias, maximum_decode_length, use_shadow, beam=sample_num)
+    elif cache.self_kv.shape[2] < cache.B * sample_num:
+        raise L.B200STError("the decoding cache holds %d rows, sampling needs %d" % (cache.self_kv.shape[2], cache.B * sample_num))
+    B, Tm = cache.B, cache.Tm
+    steps = _search_steps(Tm, maximum_decode_length, extra_decode_length, minimum_decode_length)
+    dev = rt.device
+    bos = torch.as_tensor(bos_id).to(device=dev, dtype=torch.int64).reshape(-1)
+    if bos.numel() == 1:
+        bos = bos.repeat(B)
+    bos = bos.contiguous()
+    n = B * sample_num
+    out = torch.empty(n, max(steps, 1), dtype=torch.int64, device=dev)
+    logprob = torch.zeros(n, dtype=torch.float32, device=dev)
+    length = torch.zeros(n, dtype=torch.int32, device=dev)
+    nbytes = int(rt.lib.b200st_beam_state_bytes(rt.handle, B, sample_num, cache.max_len))
+    if nbytes <= 0:
+        raise L.B200STError("sampling search state sizing failed: " + rt.lib.b200st_last_error().decode())
+    words = torch.zeros((nbytes + 7) // 8, dtype=torch.int64, device=dev)
+    a = L.SamplingArgs()
+    a.bos_ids, a.eos_id = bos.data_ptr(), int(eos_id)
+    a.unk_id = -1 if unk_id is None else int(unk_id)
+    a.min_len, a.max_steps = int(minimum_decode_length), int(steps)     # the library refuses steps beyond the cache
+    a.sample_num, a.top_k, a.top_p = sample_num, top_k, top_p
+    a.seed, a.row_offset = int(seed) & 0xFFFFFFFFFFFFFFFF, int(row_offset)
+    a.out_ids, a.out_logprob, a.out_len = out.data_ptr(), logprob.data_ptr(), length.data_ptr()
+    a.state_words, a.use_graph = words.data_ptr(), int(bool(use_graph))
+    bufs = _bufs(rt)
+    cur = torch.cuda.current_stream(dev)
+    side = getattr(rt, "_decode_stream", None)
+    if side is None:
+        side = rt._decode_stream = torch.cuda.Stream(device=dev)
+    side.wait_stream(cur)
+    with torch.cuda.stream(side):
+        L.check(rt.lib.b200st_sampling_search(rt.handle, C.byref(bufs), C.byref(cache.state), C.byref(a), L._stream()))
+    cur.wait_stream(side)
+    out = out[:, :steps]
+    if steps < maximum_decode_length:      # padded to the fixed output length with EOS (sampling.py:253-256)
+        out = torch.cat([out, torch.full((n, maximum_decode_length - steps), int(eos_id), dtype=torch.int64, device=dev)], 1)
+    return out, logprob, length
+
+
+def sample_logits(logits, top_k=0, top_p=1.0, seed=DEFAULT_SAMPLING_SEED, row_offset=0, step=0):
+    """top_k_logits / top_p_logits and one draw per row (sampling.py:76-100 + tf.random.categorical) on caller logits fp32
+    [rows, V] (CUDA), with the keyed draw of the sampling search: row r draws with (seed, row_offset + r, step).  No masks.
+    -> int64 [rows]."""
+    top_k, top_p = int(top_k), float(top_p)
+    _check_sampling_filter(top_k, top_p)
+    z = torch.as_tensor(logits)
+    if z.dim() != 2 or not z.is_cuda:
+        raise L.B200STError("sample_logits takes CUDA logits [rows, V]")
+    z = z.to(torch.float32).contiguous()
+    out = torch.empty(z.shape[0], dtype=torch.int64, device=z.device)
+    L.check(L.load().b200st_sample_logits(z.data_ptr(), z.shape[0], z.shape[1], top_k, top_p, int(seed) & 0xFFFFFFFFFFFFFFFF,
+                                          int(row_offset), int(step), out.data_ptr(), L._stream()))
+    return out

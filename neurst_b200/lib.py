@@ -211,6 +211,14 @@ class BeamArgs(C.Structure):
                 ("state_words", C.c_void_p), ("use_graph", C.c_int32)]
 
 
+class SamplingArgs(C.Structure):
+    _fields_ = [("bos_ids", C.c_void_p), ("eos_id", C.c_int32), ("unk_id", C.c_int32), ("min_len", C.c_int32),
+                ("max_steps", C.c_int32), ("sample_num", C.c_int32), ("top_k", C.c_int32), ("top_p", C.c_float),
+                ("seed", C.c_uint64), ("row_offset", C.c_int64),
+                ("out_ids", C.c_void_p), ("out_logprob", C.c_void_p), ("out_len", C.c_void_p),
+                ("state_words", C.c_void_p), ("use_graph", C.c_int32)]
+
+
 ENSEMBLE_MAX_MODELS = 8    # B200ST_ENSEMBLE_MAX_MODELS
 
 
@@ -226,7 +234,7 @@ EXPORTS = [
     "b200st_comm_unique_id", "b200st_comm_init", "b200st_comm_broadcast", "b200st_comm_destroy", "b200st_comm_stats", "b200st_train_step",
     "b200st_encode", "b200st_encode_workspace_bytes", "b200st_decode_scratch_floats", "b200st_decode_init", "b200st_decode_step",
     "b200st_greedy_search", "b200st_greedy_used_graph", "b200st_beam_state_bytes", "b200st_beam_search",
-    "b200st_ensemble_beam_search",
+    "b200st_ensemble_beam_search", "b200st_sampling_search", "b200st_sample_logits",
     "b200st_encoder_forward", "b200st_decoder_forward", "b200st_mha_forward", "b200st_lsce", "b200st_layernorm_fwd",
     "b200st_layernorm_bwd", "b200st_softmax_fwd", "b200st_conv1_ln_relu_fwd", "b200st_dropout_stream_id", "b200st_dropout_mask",
 ]
@@ -268,6 +276,10 @@ def _declare(lib):
     lib.b200st_beam_state_bytes.argtypes = [C.c_void_p, C.c_int32, C.c_int32, C.c_int32]
     lib.b200st_beam_search.argtypes = [C.c_void_p, C.POINTER(Buffers), C.POINTER(DecodeState), C.POINTER(BeamArgs), C.c_void_p]
     lib.b200st_ensemble_beam_search.argtypes = [C.POINTER(EnsembleMember), C.c_int32, C.POINTER(BeamArgs), C.c_void_p]
+    lib.b200st_sampling_search.argtypes = [C.c_void_p, C.POINTER(Buffers), C.POINTER(DecodeState), C.POINTER(SamplingArgs),
+                                           C.c_void_p]
+    lib.b200st_sample_logits.argtypes = [C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_float, C.c_uint64, C.c_int64, C.c_int32,
+                                         C.c_void_p, C.c_void_p]
     lib.b200st_adam_step.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64, C.c_float,
                                      C.c_float, C.c_float, C.c_float, C.c_int64, C.c_float, C.c_int32, C.c_void_p]
     lib.b200st_encoder_forward.argtypes = [C.c_void_p, C.POINTER(Buffers), C.c_void_p, C.c_void_p, C.c_int32, C.c_int32,

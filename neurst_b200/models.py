@@ -229,6 +229,24 @@ class _EncoderDecoder:
                                           maximum_decode_length, extra_decode_length, minimum_decode_length, enable_unk, use_shadow)
         return ids, scores
 
+    def sampling_search(self, inputs, sample_num=1, top_k=0, top_p=1.0, maximum_decode_length=256, extra_decode_length=50,
+                        minimum_decode_length=0, seed=1234, row_offset=0, use_shadow=False):
+        """SequenceGenerator with search_method TopSampling (neurst/layers/search/sampling.py:265-345) on the device:
+        -> (samples [B*sample_num, maximum_decode_length], their log-probabilities [B*sample_num]), row b * sample_num + s
+        being sample s of utterance b.  The draws are keyed by (seed, row_offset + row, step) (decode.sampling_search).
+        At most decode.MAX_ROWS // sample_num utterances per call with the fp32 weights, decode.MAX_ROWS_SHADOW // sample_num
+        with use_shadow; sample_num <= 8."""
+        from neurst_b200 import decode as D
+        tm = self._trg_meta
+        B = inputs["src"].shape[0]
+        bos = inputs.get("trg_input")
+        if bos is None:
+            bos = torch.full((B,), int(tm["bos_id"]), dtype=torch.long)
+        ids, logprob, _ = D.sampling_search(self._rt, inputs, bos, tm["eos_id"], tm.get("unk_id"), sample_num, top_k, top_p,
+                                            maximum_decode_length, extra_decode_length, minimum_decode_length, seed, row_offset,
+                                            use_shadow)
+        return ids, logprob
+
     def evaluate(self, inputs, is_training=False):
         """logits + criterion outputs (nll_sum [B], n_tokens [B], loss) in one call."""
         return self._rt.run(self._batch(inputs, is_training, want_logits=True), backward=False)
