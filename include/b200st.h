@@ -260,6 +260,26 @@ int b200st_sampling_search(b200st_handle h, const b200st_buffers* buf, const b20
  * out_ids[r] draws with the key (seed, row_offset + r, step). */
 int b200st_sample_logits(const float* logits, int32_t rows, int32_t V, int32_t top_k, float top_p, uint64_t seed, int64_t row_offset,
                          int32_t step, int64_t* out_ids, void* stream);
+/* Cascade ST handoff (ASR -> MT on the device): one block per utterance reads the ASR search's top-1 hypothesis ids
+ * hyp_ids [B][hyp_stride] (first hyp_len columns), truncates at the first asr_eos_id, maps each id through remap
+ * [asr_vocab] (int32, ASR target id -> MT source id; an ASR id outside 0..asr_vocab-1 maps to mt_unk_id), applies the MT
+ * side's truncation (max_src_len > 0: the first max_src_len - 1 ids and EOS; 0: none), appends mt_eos_id, and writes
+ * src_ids [B][out_stride] (padded with mt_pad_id), src_padding [B][out_stride] (1.0 beyond the length) and src_len [B].
+ * The remap values must lie in 0..mt_vocab-1 (the caller builds the table).  Bad sizes or ids (B, hyp_len > hyp_stride,
+ * table sizes < 1, eos / pad / unk ids outside their vocabulary, out_stride below the longest source) fail before anything is
+ * launched.  Integer work only: the outputs do not depend on the launch. */
+typedef struct {
+  const int64_t* hyp_ids;
+  int32_t B, hyp_len, hyp_stride;
+  int32_t asr_eos_id, asr_vocab;
+  const int32_t* remap;
+  int32_t mt_vocab, mt_eos_id, mt_pad_id, mt_unk_id;
+  int32_t max_src_len, out_stride;
+  int64_t* src_ids;
+  float* src_padding;
+  int32_t* src_len;
+} b200st_cascade_source_args;
+int b200st_cascade_source(const b200st_cascade_source_args* a, void* stream);
 /* Ensemble decoding: sequence_beam_search over EncoderDecoderEnsembleModel (neurst/models/encoder_decoder_ensemble_model.py;
  * neurst/layers/search/beam_search.py:97-115,486-515).  Per step every member runs its decoder step on the same rows, and the
  * search continues from log(sum_m w_m softmax(logits_m)) (evaluated as a log-sum-exp over the members) with the masks,

@@ -22,14 +22,32 @@ import numpy as np
 import torch
 
 MODEL_SCOPE = "SpeechTransformer"
+TEXT_MODEL_SCOPE = "Transformer"
 
 
-def tf_variable_names(table, scope=MODEL_SCOPE):
-    """{our parameter name: reference variable name} for every tensor of a SpeechTransformer parameter table."""
+def is_text_table(table):
+    """A text Transformer's table: no audio front-end (the source is the embedding table srcemb.emb or, tied, trg.emb)."""
+    return "src.conv1.kernel" not in table and "trg.emb" in table
+
+
+def model_scope(table):
+    """The reference model's name scope: `SpeechTransformer` or, for the text model, `Transformer`."""
+    return TEXT_MODEL_SCOPE if is_text_table(table) else MODEL_SCOPE
+
+
+def tf_variable_names(table, scope=None):
+    """{our parameter name: reference variable name} for every tensor of a SpeechTransformer or text Transformer parameter
+    table.  The text model's modalities are `input_symbol_modality` (source table, `emb/weights`) and
+    `target_symbol_modality` (`shared/{weights,bias}`), or one `shared_symbol_modality` when the source and target tables
+    are tied (encoder_decoder_model.py:148-178); each sits in its `_posenc_wrapper` (sinusoid timing)."""
+    scope = model_scope(table) if scope is None else scope
     out = {}
     src = scope + "/input_audio_modality_posenc_wrapper/input_audio_modality"
     trg = scope + "/target_symbol_modality_posenc_wrapper/target_symbol_modality"
+    if is_text_table(table) and "srcemb.emb" not in table:
+        trg = scope + "/shared_symbol_modality_posenc_wrapper/shared_symbol_modality"
     fixed = {
+        "srcemb.emb": scope + "/input_symbol_modality_posenc_wrapper/input_symbol_modality/emb/weights",
         "src.conv1.kernel": src + "/conv1/kernel", "src.conv1.bias": src + "/conv1/bias",
         "src.conv2.kernel": src + "/conv2/kernel", "src.conv2.bias": src + "/conv2/bias",
         "src.ln1.gamma": src + "/ln1/gamma", "src.ln1.beta": src + "/ln1/beta",
@@ -61,7 +79,7 @@ def tf_variable_names(table, scope=MODEL_SCOPE):
     return out
 
 
-def save_npz(rt, path, scope=MODEL_SCOPE, extra=None):
+def save_npz(rt, path, scope=None, extra=None):
     """Writes every parameter under its reference variable name (+ optional Adam slots as `<name>/.OPTIMIZER_SLOT/{m,v}`)."""
     names = tf_variable_names(rt.table, scope)
     arrays = {names[k]: rt.view(k).detach().cpu().numpy() for k in rt.table}
@@ -75,14 +93,21 @@ def save_npz(rt, path, scope=MODEL_SCOPE, extra=None):
     return sorted(arrays)
 
 
-def load_npz(rt, path, scope=None, strict=True):
-    """Restores by name.  `scope=None` uses the archive's own top-level scope (checkpoint_scope_name, checkpoints.py:322-338)."""
+def load_npz(rt, path, scope=None, strict=True, pattern=None, slots=True):
+    """Restores by name.  `scope=None` uses the archive's own top-level scope (checkpoint_scope_name, checkpoints.py:322-338).
+    `pattern`: restore only the variables whose name in THIS model (its own scope) matches the regular expression
+    (re.search), each read from the archive under the archive's scope (restore_checkpoint_if_possible,
+    checkpoints.py:340-360); the Adam slots are then left alone, as they are with `slots=False` (pretraining restores the
+    model's weights only)."""
     z = np.load(path)
     keys = [k for k in z.files if "/.OPTIMIZER_SLOT/" not in k]
     if scope is None:
         scopes = {k.split("/")[0] for k in keys if "/" in k}
-        scope = scopes.pop() if len(scopes) == 1 else MODEL_SCOPE
+        scope = scopes.pop() if len(scopes) == 1 else model_scope(rt.table)
     names = tf_variable_names(rt.table, scope)
+    if pattern is not None:
+        own = tf_variable_names(rt.table)
+        names = {k: v for k, v in names.items() if re.search(pattern, own[k]) is not None}
     missing = [v for v in names.values() if v not in z.files]
     if missing and strict:
         raise KeyError("checkpoint misses %d variables, e.g. %s" % (len(missing), missing[:3]))
@@ -92,7 +117,7 @@ def load_npz(rt, path, scope=None, strict=True):
             raise ValueError("shape mismatch for %s: checkpoint %s vs model %s" % (names[k], tuple(t.shape), rt.table[k][1]))
         rt.view(k).copy_(t.to(torch.float32))
     rt._shadow_stale = True
-    if all((names[k] + "/.OPTIMIZER_SLOT/m") in z.files for k in rt.table):
+    if slots and pattern is None and all((names[k] + "/.OPTIMIZER_SLOT/m") in z.files for k in rt.table):
         if rt.adam_m is None:
             rt.adam_m, rt.adam_v = torch.zeros_like(rt.params), torch.zeros_like(rt.params)
         for k in rt.table:

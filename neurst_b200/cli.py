@@ -44,6 +44,10 @@ SECTIONS = ("entry.params", "task.params", "dataset.params", "model.params", "se
 TOP_LEVEL = ("model_dir", "hparams_set", "dtype", "output_file", "entry", "search_method", "validator")
 # the validators' flags (neurst/training/validator.py, criterion_validator.py, seq_generation_validator.py): a flat
 # `--eval_steps 500` lands in validator.params, as the reference's registered flags do
+TEXT_TASKS = ("seqtoseq", "seq2seq")                       # registered as seq_to_seq and Seq2Seq
+TEXT_DATASETS = ("paralleltextdataset", "paralleltext")
+TEXT_MODELS = ("transformer",)
+SPEECH_MODELS = ("speechtransformer", "b200speechtransformer", "b200st")
 VALIDATOR_FLAGS = ("eval_steps", "eval_start_at", "eval_on_begin", "eval_dataset", "eval_dataset.params", "eval_batch_size",
                    "eval_task_args", "eval_criterion", "eval_criterion.params", "eval_search_method", "eval_search_method.params",
                    "eval_metric", "eval_metric.params", "eval_estop_patience", "eval_best_checkpoint_path",
@@ -88,6 +92,17 @@ def parse_command_line(argv):
             if i >= len(argv):
                 raise SystemExit("flag --%s needs a value" % key)
             val = argv[i]
+            # several values before the next flag make a list (`--pretrain_model asr/best_avg mt/best_avg`)
+            more = []
+            while i + 1 < len(argv) and not argv[i + 1].startswith("--"):
+                i += 1
+                more.append(argv[i])
+            if more:
+                if key == "config_paths":
+                    raise SystemExit("unexpected argument %r" % more[0])
+                overrides.append((key, [_coerce(v) for v in [val] + more]))
+                i += 1
+                continue
         if key == "config_paths":
             paths.extend(p for p in val.split(",") if p)
         else:
@@ -124,25 +139,46 @@ def load_config(paths, overrides=()):
     return cfg
 
 
-def target_meta(task_params):
-    """Vocabulary meta of the target side (text_data_pipeline.py:83-93, data/text/vocab.py): ids 0..n-1 are the file's
-    tokens, then <UNK>, <SEQ_BEG>, <SEQ_END>; padding = EOS."""
-    tp = task_params
-    n = tp.get("vocab_size")
+def _vocab_meta(n, path):
+    """Vocabulary meta (text_data_pipeline.py:83-93, data/text/vocab.py): ids 0..n-1 are the file's tokens, then <UNK>,
+    <SEQ_BEG>, <SEQ_END>; padding = EOS."""
     tokens = None
-    path = None
-    for k in ("transcript_data_pipeline.params", "trg_data_pipeline.params", "translation_data_pipeline.params"):
-        if isinstance(tp.get(k), dict) and tp[k].get("vocab_path"):
-            path = tp[k]["vocab_path"]
     if path and os.path.exists(path):
         with open(path, encoding="utf-8") as f:
             tokens = [l.rstrip("\n").split("\t")[0].split(" ")[0] for l in f if l.strip()]
         n = len(tokens) + 3
     if n is None:
-        raise SystemExit("the target vocabulary is unknown: give task.params.vocab_size or a readable *_data_pipeline.params.vocab_path")
+        return None
     n = int(n)
     return {"vocab_size": n, "unk_id": n - 3, "bos_id": n - 2, "eos_id": n - 1, "pad_id": n - 1, "padding_mode": "eos_as_padding",
             "tokens": tokens}
+
+
+def target_meta(task_params):
+    """Vocabulary meta of the target side: task.params.vocab_size, or the *_data_pipeline.params.vocab_path file."""
+    tp = task_params
+    path = None
+    for k in ("transcript_data_pipeline.params", "trg_data_pipeline.params", "translation_data_pipeline.params"):
+        if isinstance(tp.get(k), dict) and tp[k].get("vocab_path"):
+            path = tp[k]["vocab_path"]
+    meta = _vocab_meta(tp.get("vocab_size"), path)
+    if meta is None:
+        raise SystemExit("the target vocabulary is unknown: give task.params.vocab_size or a readable *_data_pipeline.params.vocab_path")
+    return meta
+
+
+def text_vocab_metas(task_params):
+    """(source, target) vocabulary metas of the seq2seq task, read from src_data_pipeline.params.vocab_path and
+    trg_data_pipeline.params.vocab_path: the text path maps tokens to ids itself, so both files must be readable."""
+    metas = []
+    for side in ("src", "trg"):
+        params = task_params.get(side + "_data_pipeline.params")
+        path = params.get("vocab_path") if isinstance(params, dict) else None
+        if not path or not os.path.isfile(path):
+            raise SystemExit("task.params.%s_data_pipeline.params.vocab_path must name a readable vocabulary file, got %r"
+                             % (side, path))
+        metas.append(_vocab_meta(None, path))
+    return tuple(metas)
 
 
 def _module_name(cfg, name):
@@ -205,9 +241,20 @@ def _as_dict(v, what):
     return dict(v)
 
 
-def resolve_validator(cfg, tp):
+def _text_dataset(dsp, what):
+    """dataset.params of a ParallelTextDataset: BPE'd, line-aligned source and target files."""
+    if not dsp.get("src_file"):
+        raise SystemExit("%s ParallelTextDataset needs src_file" % what)
+    if not dsp.get("data_is_processed"):
+        raise SystemExit("%s ParallelTextDataset with raw text is outside this path: the tokenizer and BPE (moses, "
+                         "subword-nmt, sentencepiece) are not applied here; give BPE'd files with data_is_processed: True" % what)
+    return {"src_file": dsp["src_file"], "trg_file": dsp.get("trg_file"), "data_is_processed": True}
+
+
+def resolve_validator(cfg, tp, text=False):
     """validator.class (or its alias `validator`) with validator.params, the flags and defaults of Validator,
-    CriterionValidator and SeqGenerationValidator; None without a validator."""
+    CriterionValidator and SeqGenerationValidator; None without a validator.  `text`: the seq2seq task, whose eval
+    dataset is a ParallelTextDataset."""
     cls = _module_name(cfg, "validator")
     if cls is None:
         return None
@@ -224,9 +271,14 @@ def resolve_validator(cfg, tp):
         return vp.get(key + ".class", vp.get(key)), _as_dict(vp.get(key + ".params"), "validator.params." + key + ".params")
 
     ds_cls, dsp = module("eval_dataset")
-    if ds_cls is None or not dsp.get("data_path"):
+    if text:
+        if str(ds_cls).lower().replace("_", "") not in TEXT_DATASETS:
+            raise SystemExit("eval_dataset %r is outside this path for the seq2seq task (ParallelTextDataset only)" % ds_cls)
+        if not dsp.get("trg_file"):
+            raise SystemExit("validator %s needs eval_dataset.params.trg_file" % name)
+    elif ds_cls is None or not dsp.get("data_path"):
         raise SystemExit("validator %s needs eval_dataset with eval_dataset.params.data_path" % name)
-    if str(ds_cls).lower().replace("_", "") not in ("audiotfrecorddataset", "audiotfrecord"):
+    elif str(ds_cls).lower().replace("_", "") not in ("audiotfrecorddataset", "audiotfrecord"):
         raise SystemExit("eval_dataset %r is outside this path (AudioTFRecordDataset only)" % ds_cls)
     task_args = _as_dict(vp.get("eval_task_args"), "eval_task_args")
     unknown = sorted(set(task_args) - {"batch_size", "truncate_src", "max_src_len"})
@@ -237,8 +289,9 @@ def resolve_validator(cfg, tp):
         raise SystemExit("eval_criterion %r is outside this path (label_smoothed_cross_entropy only)" % crit_cls)
     plan = {"class": name, "eval_steps": int(vp.get("eval_steps", 1000)), "eval_start_at": int(vp.get("eval_start_at", 0)),
             "eval_on_begin": bool(vp.get("eval_on_begin", False)),
-            "dataset": {"data_path": dsp["data_path"], "feature_key": dsp.get("feature_key", "audio"),
-                        "transcript_key": dsp.get("transcript_key", "transcript")},
+            "dataset": _text_dataset(dsp, "eval_dataset") if text else
+            {"data_path": dsp["data_path"], "feature_key": dsp.get("feature_key", "audio"),
+             "transcript_key": dsp.get("transcript_key", "transcript")},
             "batch_size": int(vp.get("eval_batch_size", 32)),
             "task_args": {k: v for k, v in task_args.items() if k != "batch_size"},
             # the reference builds the eval criterion from its own params: label_smoothing defaults to 0
@@ -278,20 +331,36 @@ def resolve_validator(cfg, tp):
 
 def resolve(cfg, world=1):
     """Everything the entries need, as plain dictionaries (also what the CPU test checks)."""
-    from neurst_b200.models import speech_transformer_hparams
+    from neurst_b200.models import speech_transformer_hparams, transformer_hparams
+    if str(_module_name(cfg, "entry") or "").lower().replace("_", "") == "cascadest":
+        return resolve_cascade(cfg, world)
     ep, tp = dict(cfg.get("entry.params") or {}), dict(cfg.get("task.params") or {})
     task_cls = str(cfg.get("task.class", "SpeechToText")).lower().replace("_", "")
-    if task_cls not in ("speechtotext", "speech2text"):
-        raise SystemExit("task.class %r is outside this path (SpeechToText only)" % cfg.get("task.class"))
-    ds_cls = str(cfg.get("dataset.class", "AudioTFRecordDataset")).lower().replace("_", "")
-    if ds_cls not in ("audiotfrecorddataset", "audiotfrecord"):
+    text = task_cls in TEXT_TASKS
+    if task_cls not in ("speechtotext", "speech2text") and not text:
+        raise SystemExit("task.class %r is outside this path (SpeechToText, Seq2Seq)" % cfg.get("task.class"))
+    ds_cls = str(cfg.get("dataset.class", "ParallelTextDataset" if text else "AudioTFRecordDataset")).lower().replace("_", "")
+    if text and ds_cls not in TEXT_DATASETS:
+        raise SystemExit("dataset.class %r is outside this path for the seq2seq task (ParallelTextDataset only)" % cfg.get("dataset.class"))
+    if not text and ds_cls not in ("audiotfrecorddataset", "audiotfrecord"):
         raise SystemExit("dataset.class %r is outside this path (AudioTFRecordDataset only)" % cfg.get("dataset.class"))
-    hp = speech_transformer_hparams(cfg.get("hparams_set") or "speech_transformer_s")
+    # the hparams_set's name picks the speech or the text table
+    hp_name = cfg.get("hparams_set") or ("transformer_s" if text else "speech_transformer_s")
+    try:
+        hp = speech_transformer_hparams(hp_name) or transformer_hparams(hp_name)
+    except ValueError as e:
+        raise SystemExit(str(e))
     if hp is None:
         raise SystemExit("unknown hparams_set %r" % cfg.get("hparams_set"))
+    if hp["model.class"] != ("Transformer" if text else "SpeechTransformer"):
+        raise SystemExit("hparams_set %r is a %s preset, outside this path for the %s task" % (
+            hp_name, hp["model.class"], "seq2seq" if text else "SpeechToText"))
     model_cls = str(cfg.get("model.class", hp["model.class"])).lower().replace("_", "")
-    if model_cls not in ("speechtransformer", "b200speechtransformer", "b200st"):
-        raise SystemExit("model.class %r is outside this path (SpeechTransformer only)" % cfg.get("model.class"))
+    if text and model_cls not in TEXT_MODELS:
+        raise SystemExit("model.class %r is outside this path for the seq2seq task (Transformer only)"
+                         % cfg.get("model.class", hp["model.class"]))
+    if not text and model_cls not in SPEECH_MODELS:
+        raise SystemExit("model.class %r is outside this path (SpeechTransformer only)" % cfg.get("model.class", hp["model.class"]))
     model_params = dict(hp["model.params"])
     model_params.update(cfg.get("model.params") or {})
     opt = dict(hp["optimizer.params"]); opt.update(ep.get("optimizer.params") or {})
@@ -299,6 +368,9 @@ def resolve(cfg, world=1):
     if str(ep.get("lr_schedule.class", "noam")).lower() != "noam" or str(ep.get("optimizer.class", "adam")).lower() != "adam":
         raise SystemExit("this path implements the presets' Adam + noam schedule")
     crit = ep.get("criterion.params") or {}
+    entry = str(_module_name(cfg, "entry") or "trainer").lower()
+    if text:
+        return _resolve_text(cfg, ep, tp, world, entry, model_params, opt, lr, crit)
     # batch_size counts frames when batch_by_frames (speech2text.py:296-310): per-GPU budget = batch_size // replicas
     per_gpu = tp.get("batch_size_per_gpu")
     if per_gpu is None:
@@ -315,14 +387,13 @@ def resolve(cfg, world=1):
     dataset = {"data_path": dsp.get("data_path"), "feature_key": dsp.get("feature_key", "audio"),
                "transcript_key": dsp.get("transcript_key", "transcript")}
     search_method, search = resolve_search(cfg, ep, tp)
-    entry = str(_module_name(cfg, "entry") or "trainer").lower()
     model_dirs = flatten_string_list(cfg.get("model_dir") or ep.get("model_dir") or "./b200st_model")
     if not model_dirs:
         raise SystemExit("model_dir names no directory")
     if len(model_dirs) > 1 and entry in ("trainer", "train"):
         raise SystemExit("training writes one model_dir, got %d: %s" % (len(model_dirs), ", ".join(model_dirs)))
     plan = {
-        "entry": entry,
+        "entry": entry, "model_class": "SpeechTransformer",
         # several directories: `predict` decodes with the ensemble of their models (SequenceGenerator._build_and_restore_model)
         "model_dir": model_dirs[0] if len(model_dirs) == 1 else model_dirs,
         "precision": {"float16": "fp16", "fp16": "fp16", "bfloat16": "bf16", "bf16": "bf16", "float32": "fp32", "fp32": "fp32"}[
@@ -337,11 +408,146 @@ def resolve(cfg, world=1):
         "search": search,
         "output_file": cfg.get("output_file") or ep.get("output_file"),
     }
+    return _finish_plan(plan, cfg, ep, tp, search_method, model_dirs)
+
+
+def _model_dir_configs(model_dir, what):
+    """model_configs.yml of a trained model directory: model class and parameters, and the task with its vocabularies."""
+    import yaml
+    path = os.path.join(model_dir, MODEL_CONFIGS)
+    if not os.path.isfile(path):
+        raise SystemExit("%s: %s has no %s" % (what, model_dir, MODEL_CONFIGS))
+    with open(path) as f:
+        configs = yaml.safe_load(f) or {}
+    if not isinstance(configs.get("task.params"), dict):
+        raise SystemExit("%s: %s records no task.params (the vocabularies); train it with this version or add them" % (what, path))
+    return configs
+
+
+def resolve_cascade(cfg, world=1):
+    """The `cascade_st` entry (neurst/cli/cascade_st.py): ASR search, then MT search on the ASR top-1 hypotheses.  Each
+    model is rebuilt from its directory's model_configs.yml (model and task, as ModelConfigs.load); the audio dataset is
+    AudioTripleTFRecordDataset (feature_key, transcript_key, translation_key)."""
+    if world > 1:
+        raise SystemExit("cascade_st runs on one device (WORLD_SIZE 1)")
+    ep = dict(cfg.get("entry.params") or {})
+
+    def get(key, default=None):
+        v = cfg.get(key, ep.get(key))
+        return default if v is None else v
+
+    dirs = {side: get(side + "_model_dir") for side in ("asr", "mt")}
+    for side, d in dirs.items():
+        if not d:
+            raise SystemExit("cascade_st needs %s_model_dir" % side)
+    ds_cls = str(cfg.get("dataset.class", "AudioTripleTFRecordDataset")).lower().replace("_", "")
+    if ds_cls not in ("audiotripletfrecorddataset", "audiotripletfrecord"):
+        raise SystemExit("dataset.class %r is outside this path for cascade_st (AudioTripleTFRecordDataset only)" % cfg.get("dataset.class"))
+    dsp = dict(cfg.get("dataset.params") or {})
+    if not dsp.get("data_path"):
+        raise SystemExit("cascade_st needs dataset.params.data_path")
+    batch_size = int(get("batch_size", 32))
+    plans = {}
+    for side, want in (("asr", "SpeechTransformer"), ("mt", "Transformer")):
+        configs = _model_dir_configs(dirs[side], side + "_model_dir")
+        if str(configs.get("model.class")) != want:
+            raise SystemExit("%s_model_dir %s holds a %s, not a %s" % (side, dirs[side], configs.get("model.class"), want))
+        method = cfg.get(side + "_search_method.class", cfg.get(side + "_search_method", "beam_search"))
+        sub = {"entry.class": "predict", "model_dir": dirs[side], "dtype": cfg.get("dtype", "float16"), "batch_size": batch_size,
+               "task.class": configs.get("task.class"), "task.params": configs["task.params"],
+               "model.class": want, "model.params": configs.get("model.params") or {},
+               "hparams_set": "speech_transformer_s" if side == "asr" else "transformer_s",
+               "search_method": method, "search_method.params": cfg.get(side + "_search_method.params") or {}}
+        if side == "asr":
+            sub["dataset.params"] = {"data_path": dsp["data_path"], "feature_key": dsp.get("feature_key", "audio"),
+                                     "transcript_key": dsp.get("transcript_key", "transcript")}
+        else:
+            sub["dataset.class"], sub["dataset.params"] = "ParallelTextDataset", {"src_file": "-", "data_is_processed": True}
+        plans[side] = resolve(sub)
+        if plans[side].get("search_method") not in ("beam_search", None):
+            raise SystemExit("%s_search_method %r is outside this path for cascade_st (beam_search)" % (side, method))
+    if plans["asr"]["search"].get("top_k", 1) != 1:
+        raise SystemExit("asr_search_method.params.top_k must be 1: the MT stage reads the ASR top-1 hypothesis")
+    metrics = {side: str(get(side + "_metric.class", get(side + "_metric", default))) for side, default in (("asr", "wer"), ("mt", "bleu"))}
+    from neurst_b200.metrics import build_metric
+    for side, m in metrics.items():
+        try:
+            build_metric(m, "en")
+        except ValueError as e:
+            raise SystemExit("%s_metric: %s" % (side, e))
+    return {"entry": "cascade_st", "asr": plans["asr"], "mt": plans["mt"], "batch_size": batch_size,
+            "translation_key": dsp.get("translation_key", "translation"), "metrics": metrics,
+            "asr_output_file": get("asr_output_file"), "mt_output_file": get("mt_output_file")}
+
+
+def _pretrain_patterns(ep):
+    """pretrain_variable_pattern beside pretrain_model (exps/trainer.py:52-72): one regular expression (or None) per
+    archive; None without patterns."""
+    patterns = ep.get("pretrain_variable_pattern")
+    if patterns is None:
+        return None
+    models = flatten_string_list(ep.get("pretrain_model"))
+    patterns = [patterns] if isinstance(patterns, str) else list(patterns)
+    if not models or len(models) != len(patterns):
+        raise SystemExit("`pretrain_variable_pattern` must match with `pretrain_model`: %d archive(s), %d pattern(s)"
+                         % (len(models or []), len(patterns)))
+    for p in patterns:
+        if p is not None:
+            try:
+                re.compile(p)
+            except re.error as e:
+                raise SystemExit("pretrain_variable_pattern %r: %s" % (p, e))
+    return [None if p is None else str(p) for p in patterns]
+
+
+def _resolve_text(cfg, ep, tp, world, entry, model_params, opt, lr, crit):
+    """The plan of the seq2seq task over a text Transformer (Seq2Seq, ParallelTextDataset)."""
+    src_meta, trg_meta = text_vocab_metas(tp)
+    if model_params.get("modality.share_source_target_embedding") and src_meta["tokens"] != trg_meta["tokens"]:
+        raise SystemExit("modality.share_source_target_embedding needs identical source and target vocabularies (%d vs %d "
+                         "entries)" % (src_meta["vocab_size"], trg_meta["vocab_size"]))
+    if entry in ("trainer", "train") and tp.get("batch_size") is None and tp.get("batch_size_per_gpu") is None:
+        raise SystemExit("task.params needs batch_size or batch_size_per_gpu (tokens with batch_by_tokens, else pairs)")
+    task = dict(max_src_len=tp.get("max_src_len"), max_trg_len=tp.get("max_trg_len"),
+                truncate_src=bool(tp.get("truncate_src") or False), truncate_trg=bool(tp.get("truncate_trg") or False),
+                batch_size=tp.get("batch_size"), batch_size_per_gpu=tp.get("batch_size_per_gpu"),
+                batch_by_tokens=bool(tp.get("batch_by_tokens") or False))
+    search_method, search = resolve_search(cfg, ep, tp)
+    model_dirs = flatten_string_list(cfg.get("model_dir") or ep.get("model_dir") or "./b200st_model")
+    if not model_dirs:
+        raise SystemExit("model_dir names no directory")
+    if len(model_dirs) > 1 and entry in ("trainer", "train"):
+        raise SystemExit("training writes one model_dir, got %d: %s" % (len(model_dirs), ", ".join(model_dirs)))
+    plan = {
+        "entry": entry, "model_class": "Transformer",
+        "model_dir": model_dirs[0] if len(model_dirs) == 1 else model_dirs,
+        "precision": {"float16": "fp16", "fp16": "fp16", "bfloat16": "bf16", "bf16": "bf16", "float32": "fp32", "fp32": "fp32"}[
+            str(cfg.get("dtype", "float16")).lower()],
+        "model_params": model_params, "optimizer": opt, "lr_schedule": lr,
+        "label_smoothing": float(crit.get("label_smoothing", 0.1)),
+        "train_steps": int(ep.get("train_steps", 10000000)), "summary_steps": int(ep.get("summary_steps", 200)),
+        "save_checkpoint_steps": int(ep.get("save_checkpoint_steps", 1000)), "update_cycle": int(ep.get("update_cycle", 1)),
+        "clip_value": ep.get("clip_value"), "clip_norm": ep.get("clip_norm"), "pretrain_model": ep.get("pretrain_model"),
+        "seed": int(ep.get("random_seed", 1234) or 1234), "max_to_keep": int(ep.get("checkpoints_max_to_keep", 8)),
+        "task": task, "dataset": _text_dataset(dict(cfg.get("dataset.params") or {}), "dataset"),
+        "src_meta": src_meta, "trg_meta": trg_meta,
+        "search": search,
+        "output_file": cfg.get("output_file") or ep.get("output_file"),
+    }
+    return _finish_plan(plan, cfg, ep, tp, search_method, model_dirs, text=True)
+
+
+def _finish_plan(plan, cfg, ep, tp, search_method, model_dirs, text=False):
+    """Prediction batch size, search, validator and ensemble settings shared by the speech and text plans."""
+    # the task's configuration, recorded in model_configs.yml so that a model directory names its vocabularies
+    plan["task_config"] = {"task.class": "Seq2Seq" if text else "SpeechToText", "task.params": dict(tp)}
+    if ep.get("pretrain_variable_pattern") is not None:
+        plan["pretrain_variable_pattern"] = _pretrain_patterns(ep)
     if cfg.get("batch_size") is not None:     # prediction recipes: utterances per batch (SequenceGenerator)
         plan["batch_size"] = int(cfg["batch_size"])
     if search_method:
         plan["search_method"] = search_method
-    validator = resolve_validator(cfg, tp)
+    validator = resolve_validator(cfg, tp, text=text)
     if validator is not None:
         plan["validator"] = validator
         if validator["search_method"]:
@@ -426,7 +632,9 @@ def write_model_configs(plan):
     os.makedirs(plan["model_dir"], exist_ok=True)
     path = os.path.join(plan["model_dir"], MODEL_CONFIGS)
     with open(path + ".tmp", "w") as f:
-        yaml.safe_dump({"model.class": "SpeechTransformer", "model.params": dict(plan["model_params"])}, f, default_flow_style=False)
+        configs = {"model.class": plan.get("model_class", "SpeechTransformer"), "model.params": dict(plan["model_params"])}
+        configs.update(plan.get("task_config") or {})
+        yaml.safe_dump(configs, f, default_flow_style=False)
     os.replace(path + ".tmp", path)
 
 
@@ -440,7 +648,11 @@ def member_model_params(plan, model_dir):
     with open(path) as f:
         cfg = yaml.safe_load(f) or {}
     cls = str(cfg.get("model.class", "SpeechTransformer")).lower().replace("_", "")
-    if cls not in ("speechtransformer", "b200speechtransformer", "b200st"):
+    if plan.get("model_class") == "Transformer":
+        if cls not in TEXT_MODELS:
+            raise SystemExit("%s: model.class %r is outside this path for the seq2seq task (Transformer only)"
+                             % (path, cfg.get("model.class")))
+    elif cls not in SPEECH_MODELS:
         raise SystemExit("%s: model.class %r is outside this path (SpeechTransformer only)" % (path, cfg.get("model.class")))
     return dict(cfg.get("model.params") or {})
 
@@ -458,19 +670,45 @@ def _dist_setup():
 
 
 def _build_model(plan):
-    from neurst_b200.models import SpeechTransformer
+    from neurst_b200.models import SpeechTransformer, Transformer
     tm = {k: v for k, v in plan["trg_meta"].items() if k != "tokens"}
+    # only the target table feeds the tensor cores (logits GEMM and its gradient); the source table is gathered and
+    # scatter-added in fp32, so a source vocabulary of any size runs on the 16-bit path
     if plan["precision"] != "fp32" and tm["vocab_size"] % 8 != 0:
         raise SystemExit("the 16-bit tensor-core path needs a target vocabulary size that is a multiple of 8 (TMA row alignment of the "
                          "logits gradient); this vocabulary has %d entries (tokens + <UNK>, <SEQ_BEG>, <SEQ_END>): pad the vocabulary file "
                          "with %d unused tokens or run with --dtype float32" % (tm["vocab_size"], -tm["vocab_size"] % 8))
+    if plan.get("model_class") == "Transformer":
+        sm = {k: v for k, v in plan["src_meta"].items() if k != "tokens"}
+        try:
+            return Transformer.new(plan["model_params"], sm, tm, precision=plan["precision"], label_smoothing=plan["label_smoothing"])
+        except (NotImplementedError, ValueError) as e:
+            raise SystemExit(str(e))
     src_meta = {"audio_feature_dim": plan["task"]["audio_feature_dim"], "audio_feature_channels": plan["task"]["audio_feature_channels"]}
     return SpeechTransformer.new(plan["model_params"], src_meta, tm, precision=plan["precision"], label_smoothing=plan["label_smoothing"])
 
 
 def _examples(plan, rank, world, training, with_label=None):
     """Endless (training) or single-pass stream of preprocessed samples of this rank's file shard (with the transcripts
-    when training or `with_label`)."""
+    when training or `with_label`).  The text task reads the whole corpus on every rank: its batches are global and
+    each rank takes its share of every one (Seq2Seq.train_batches), so all ranks run the same shape at each step.  Text
+    `predict` is single-rank: with WORLD_SIZE > 1 every rank decodes the whole file and rank 0 writes it."""
+    if plan.get("model_class") == "Transformer":
+        from neurst_b200.data import Seq2Seq
+        from neurst_b200.text import ParallelTextDataset
+        ds = ParallelTextDataset(plan["dataset"])
+        task = Seq2Seq(plan["src_meta"], plan["trg_meta"], world=world, **plan["task"])
+        proc = task.preprocess_fn(ds.status, training=training, with_label=training if with_label is None else with_label)
+
+        def text_stream():
+            while True:
+                n = 0
+                for ex in ds.build_iterator(map_func=proc)():
+                    n += 1
+                    yield ex
+                if not training or n == 0:
+                    return
+        return task, text_stream()
     from neurst_b200.data import SpeechToText
     from neurst_b200.tfrecord import AudioTFRecordDataset
     ds = AudioTFRecordDataset(plan["dataset"])
@@ -492,22 +730,38 @@ def _examples(plan, rank, world, training, with_label=None):
     return task, stream()
 
 
-def train(plan):
+def initialise(model, plan):
+    """The model's starting weights: the newest checkpoint of model_dir (resume), else pretrain_model, else its own
+    initialisation.  -> the step to resume from."""
     from neurst_b200 import checkpoints as CK
-    from neurst_b200.trainer import DataParallelTrainer, HostPipeline
-    world, rank, local = _dist_setup()
-    model = _build_model(plan)
     start_path, start_step = latest_checkpoint(plan["model_dir"])
     if start_path:
         CK.load_npz(model.runtime, start_path)
         LOG.info("restored %s", start_path)
+    elif plan["pretrain_model"] and plan.get("pretrain_variable_pattern"):
+        # restore_checkpoint_if_possible per (archive, pattern): the model's own initialisation stays everywhere else
+        model.init_parameters(plan["seed"])
+        for src, pattern in zip(flatten_string_list(plan["pretrain_model"]), plan["pretrain_variable_pattern"]):
+            src = restore_checkpoint(src)[0] if os.path.isdir(src) else src
+            if not src:
+                raise SystemExit("pretrain_model: no checkpoint to restore")
+            got = CK.load_npz(model.runtime, src, strict=False, pattern=pattern, slots=False)
+            LOG.info("initialised %d tensors from %s (pattern %r)", len(got), src, pattern)
     elif plan["pretrain_model"]:
         src = plan["pretrain_model"][0] if isinstance(plan["pretrain_model"], (list, tuple)) else plan["pretrain_model"]
         src = restore_checkpoint(src)[0] if os.path.isdir(src) else src
-        CK.load_npz(model.runtime, src, strict=False)
+        CK.load_npz(model.runtime, src, strict=False, slots=False)
         LOG.info("initialised from %s", src)
     else:
         model.init_parameters(plan["seed"])
+    return start_step
+
+
+def train(plan):
+    from neurst_b200.trainer import DataParallelTrainer, HostPipeline
+    world, rank, local = _dist_setup()
+    model = _build_model(plan)
+    start_step = initialise(model, plan)
     trainer = DataParallelTrainer(model, plan["optimizer"], plan["lr_schedule"], update_cycle=plan["update_cycle"],
                                   use_cuda_graph=True, clip_value=plan["clip_value"], clip_norm=plan["clip_norm"],
                                   summary_steps=plan["summary_steps"] if rank == 0 else 0, logger=LOG.info)
@@ -530,7 +784,8 @@ def train(plan):
     micro_target = (plan["train_steps"] - start_step) * plan["update_cycle"]
     if micro_target > 0:
         # reading, parsing, padding and pinning of the next batches run in a background thread (tf.data prefetch's role)
-        batches = Prefetcher(itertools.islice((per_rank[0] for per_rank in task.train_batches(examples, generator=gen, pin=True)),
+        share = rank if plan.get("model_class") == "Transformer" else 0      # the text task's batches are global
+        batches = Prefetcher(itertools.islice((per_rank[share] for per_rank in task.train_batches(examples, generator=gen, pin=True)),
                                               micro_target), depth=4, init=lambda: torch.cuda.set_device(local))
         try:
             pipeline = HostPipeline(trainer)
@@ -626,18 +881,23 @@ def decode_group(model, task, plan, group, search_kw, first=0):
     the rank's stream of utterances, which keys the samples' draws (row offset first * sample_num), so the samples do not
     depend on how the stream is cut into calls."""
     tm = plan["trg_meta"]
-    dim = plan["task"]["audio_feature_dim"] * plan["task"]["audio_feature_channels"]
-    T = max(int(e["audio_length"]) for e in group)
-    src = torch.zeros(len(group), T, dim)
-    for j, e in enumerate(group):
-        src[j, :int(e["audio_length"])] = e["audio"]
-    batch = task.example_to_input({"audio": src, "audio_length": torch.tensor([int(e["audio_length"]) for e in group])}, infer=True)
+    if plan.get("model_class") == "Transformer":
+        batch = task.group_to_input(group, infer=True)
+        inputs = {"src": batch["src"], "src_padding": batch["src_padding"]}
+    else:
+        dim = plan["task"]["audio_feature_dim"] * plan["task"]["audio_feature_channels"]
+        T = max(int(e["audio_length"]) for e in group)
+        src = torch.zeros(len(group), T, dim)
+        for j, e in enumerate(group):
+            src[j, :int(e["audio_length"])] = e["audio"]
+        batch = task.example_to_input({"audio": src, "audio_length": torch.tensor([int(e["audio_length"]) for e in group])}, infer=True)
+        inputs = {"src": batch["src"], "src_length": batch["src_length"]}
     method = plan.get("search_method")
     if method == "top_sampling":
         search, search_kw = model.sampling_search, dict(search_kw, row_offset=int(first) * plan["search"]["sample_num"])
     else:
         search = model.beam_search if method == "beam_search" else model.greedy_search
-    ids, score = search({"src": batch["src"], "src_length": batch["src_length"]}, **search_kw)
+    ids, score = search(inputs, **search_kw)
     return [(ids_to_text(row, tm["eos_id"], tm.get("tokens")), lp) for row, lp in zip(ids.cpu().tolist(), score.cpu().tolist())]
 
 
@@ -679,6 +939,82 @@ def predict(plan):
     return {"checkpoint_step": step, "hypotheses": hyps}
 
 
+def _cascade_references(plan, key, meta):
+    """The reference texts of one key of the audio records (ids -> text), or None when the records do not hold it."""
+    from neurst_b200.tfrecord import AudioTFRecordDataset, take_one_record
+    asr_ds = plan["asr"]["dataset"]
+    kind = take_one_record(asr_ds["data_path"]).get(key, (None, None))[0]
+    if kind is None:
+        return None
+    if kind != "int64":
+        raise SystemExit("the %r key holds raw text: the reference's text pipeline (tokenizer / BPE / vocabulary) is outside this "
+                         "path; write the TFRecords with projected (int64) ids" % key)
+    ds = AudioTFRecordDataset(dict(asr_ds, transcript_key=key))
+    return [ids_to_text(list(x["transcript"]), meta["eos_id"], meta.get("tokens")) for x in ds.build_iterator()()]
+
+
+def cascade_st(plan):
+    """ASR search, then, per group of utterances on the same stream, the handoff kernel (b200st_cascade_source: ASR top-1
+    ids -> MT source ids through the vocabulary remap table), one copy of the source lengths to the host, and the MT
+    encoder and search: no host text between the two models."""
+    from neurst_b200 import decode as D
+    from neurst_b200.metrics import build_metric
+    _dist_setup()
+    asr_plan, mt_plan = plan["asr"], plan["mt"]
+    asr, _ = _restore(asr_plan, asr_plan["model_dir"])
+    mt, _ = _restore(mt_plan, mt_plan["model_dir"])
+    task, examples = _examples(asr_plan, 0, 1, training=False, with_label=False)
+    asr_meta, src_meta, trg_meta = asr_plan["trg_meta"], mt_plan["src_meta"], mt_plan["trg_meta"]
+    if not asr_meta.get("tokens"):
+        raise SystemExit("cascade_st maps ASR tokens to MT tokens by string: the ASR model directory needs its vocab_path")
+    remap = D.cascade_remap(asr_meta["tokens"], src_meta["tokens"], src_meta["unk_id"], asr_meta["vocab_size"]).cuda()
+    asr_per_call, asr_kw = decode_settings(asr_plan)
+    mt_per_call, mt_kw = decode_settings(mt_plan)
+    per_call = min(asr_per_call, mt_per_call)
+    asr_search = asr.beam_search if asr_plan.get("search_method") == "beam_search" else asr.greedy_search
+    mt_search = mt.beam_search if mt_plan.get("search_method") == "beam_search" else mt.greedy_search
+    asr_hyps, mt_hyps = [], []
+
+    def run(group):
+        batch = task.example_to_input({"audio": _pad_audio(asr_plan, group), "audio_length": torch.tensor(
+            [int(e["audio_length"]) for e in group])}, infer=True)
+        ids, _ = asr_search({"src": batch["src"], "src_length": batch["src_length"]}, **asr_kw)
+        asr_hyps.extend(ids_to_text(r, asr_meta["eos_id"], asr_meta["tokens"]) for r in ids.cpu().tolist())
+        src, padding, _ = D.cascade_source(ids, remap, asr_meta["eos_id"], src_meta["vocab_size"], src_meta["eos_id"],
+                                           src_meta["pad_id"], src_meta["unk_id"])
+        out, _ = mt_search({"src": src, "src_padding": padding}, **mt_kw)
+        mt_hyps.extend(ids_to_text(r, trg_meta["eos_id"], trg_meta["tokens"]) for r in out.cpu().tolist())
+
+    group = []
+    for ex in examples:
+        group.append(ex)
+        if len(group) == per_call:
+            run(group)
+            group = []
+    if group:
+        run(group)
+    res = {"asr_hypotheses": asr_hyps, "mt_hypotheses": mt_hyps}
+    for side, key, meta, hyps in (("asr", asr_plan["dataset"]["transcript_key"], asr_meta, asr_hyps),
+                                  ("mt", plan["translation_key"], trg_meta, mt_hyps)):
+        out = plan[side + "_output_file"]
+        if out:
+            with open(out, "w", encoding="utf-8") as f:
+                f.write("".join(h + "\n" for h in hyps))
+        refs = _cascade_references(plan, key, meta)
+        if refs is not None:
+            res[side + "_metric"] = build_metric(plan["metrics"][side], "en")(hyps, refs)
+            LOG.info("Evaluation Result of %s: %s", side.upper(), res[side + "_metric"])
+    return res
+
+
+def _pad_audio(plan, group):
+    dim = plan["task"]["audio_feature_dim"] * plan["task"]["audio_feature_channels"]
+    src = torch.zeros(len(group), max(int(e["audio_length"]) for e in group), dim)
+    for j, e in enumerate(group):
+        src[j, :int(e["audio_length"])] = e["audio"]
+    return src
+
+
 def main(argv=None):
     logging.basicConfig(level=logging.INFO, format="%(asctime)s %(message)s")
     paths, overrides = parse_command_line(list(sys.argv[1:] if argv is None else argv))
@@ -688,6 +1024,9 @@ def main(argv=None):
         res = train(plan)
         if "validations" in res:
             res["validations"] = [{k: v for k, v in r.items() if k != "hypotheses"} for r in res["validations"]]
+    elif plan["entry"] == "cascade_st":
+        res = cascade_st(plan)
+        res = {k: v for k, v in res.items() if not k.endswith("_hypotheses")}
     elif plan["entry"] in ("predict", "sequencegenerator", "sequence_generator"):
         res = predict(plan)
         res = {"checkpoint_step": res["checkpoint_step"], "n_hypotheses": len(res["hypotheses"])}

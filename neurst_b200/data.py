@@ -1,7 +1,9 @@
-"""Input-pipeline edge of the speech-to-text task (SURVEY.md 8 f4): frame-budget length bucketing and SpecAugment.
+"""Input-pipeline edge of the speech-to-text task (SURVEY.md 8 f4): frame-budget length bucketing and SpecAugment; and of
+the seq2seq (text) task: vocabulary encoding of BPE'd text and token-budget bucketing.
 
   create_audio_bucket_boundaries / bucket table   neurst/tasks/speech2text.py:38-56,296-384
   SpecAugment                                      neurst/utils/audio_lib.py:24-257 (time warping is a documented no-op there too)
+  Seq2Seq / token buckets                          neurst/tasks/seq2seq.py:100-270, neurst/data/dataset_utils.py:125-178,435-560
 
 Bucketing is host logic (which utterance goes into which padded batch); SpecAugment runs on the GPU on the padded batch
 (the masks are sampled on the host exactly as `freq_or_time_masking_numpy`, the fill is one masked-select on the device),
@@ -216,6 +218,205 @@ class SpeechToText:
                 d["trg_length"] = (trg != pad).sum(1)
             else:                                                  # EOS_AS_PADDING: first pad (= eos) position + 1
                 d["trg_length"] = (trg != pad).to(torch.int32).argmin(-1) + 1
+            d["trg"] = trg
+            d["trg_input"] = torch.cat([bos[:, None], trg[:, :-1]], 1)
+        if pin and torch.cuda.is_available():
+            d = {k: v.contiguous().pin_memory() for k, v in d.items()}
+        return d
+
+
+# ------------------------------------------------------------------------------------------------ text (seq2seq) side
+_MIN_BUCKET_BOUNDARY = 8
+_BUCKET_BOUNDARY_SCALE = 1.1
+
+
+def create_batch_bucket_boundaries(max_length, min_boundary=_MIN_BUCKET_BOUNDARY, boundary_scale=_BUCKET_BOUNDARY_SCALE):
+    """neurst/data/dataset_utils.py:125-147: boundaries grown by `boundary_scale` (at least +1), closed by max_length + 1."""
+    bounds = []
+    x = min_boundary
+    while x < max_length:
+        bounds.append(x)
+        x = max(x + 1, int(x * boundary_scale))
+    if not bounds or bounds[-1] < max_length + 1:
+        bounds = bounds + [max_length + 1]
+    return bounds
+
+
+def associated_bucket_boundaries(a, b):
+    """dataset_utils.py:150-178: two boundary lists resampled to the shorter one's length."""
+    la, lb = len(a), len(b)
+    if la == lb:
+        return a, b
+    s1, s2 = (la * 1. / lb, 1) if la > lb else (1, lb * 1. / la)
+    return ([a[int(math.ceil(i * s1)) - 1] for i in range(1, min(la, lb) + 1)],
+            [b[int(math.ceil(i * s2)) - 1] for i in range(1, min(la, lb) + 1)])
+
+
+def adjust_batch_size(batch_size=None, batch_size_per_gpu=None, bucket_boundaries=None, num_replicas_in_sync=1):
+    """dataset_utils.py:435-464 -> the global batch size in samples (no boundaries) or, by tokens, the list of global
+    batch sizes per bucket: tokens // max(bucket boundaries), a multiple of the replica count."""
+    if batch_size is None and batch_size_per_gpu is None:
+        raise ValueError("At least one of the `batch_size` and `batch_size_per_gpu` should be provided.")
+    if batch_size_per_gpu is not None:
+        batch_size = int(batch_size_per_gpu * num_replicas_in_sync)
+    if bucket_boundaries is None:
+        return int(batch_size // num_replicas_in_sync * num_replicas_in_sync)
+    n = min(len(v) for v in bucket_boundaries.values())
+    return [int(batch_size // max(v[i] for v in bucket_boundaries.values()) // num_replicas_in_sync * num_replicas_in_sync)
+            for i in range(n)]
+
+
+class TokenBucketer:
+    """The TRAIN branch of Seq2Seq.create_and_batch_tfds (seq2seq.py:248-270) with batch_examples_by_token
+    (dataset_utils.py:467-560): bucket i holds the pairs with len(src) <= src_bounds[i] and len(trg) <= trg_bounds[i]
+    (the first such i), is padded to exactly (src_bounds[i], trg_bounds[i]) and leaves as a global batch of
+    batch_sizes[i] pairs, drop_remainder.  Each (bucket, per-replica batch) is one static shape, and every replica takes
+    the same bucket per step: `batches()` yields whole global batches split into `world` equal parts."""
+
+    def __init__(self, max_src_len, max_trg_len, batch_size=None, batch_size_per_gpu=None, batch_by_tokens=False, world=1):
+        if max_src_len is None:
+            raise RuntimeError("Must provide `max_src_len` for training.")
+        if max_trg_len is None:
+            raise RuntimeError("Must provide `max_trg_len` for training.")
+        self.world = int(world)
+        self.src_bounds, self.trg_bounds = associated_bucket_boundaries(create_batch_bucket_boundaries(int(max_src_len)),
+                                                                        create_batch_bucket_boundaries(int(max_trg_len)))
+        sizes = adjust_batch_size(batch_size, batch_size_per_gpu, num_replicas_in_sync=self.world,
+                                  bucket_boundaries={"feature": self.src_bounds, "label": self.trg_bounds} if batch_by_tokens else None)
+        self.batch_sizes = sizes if isinstance(sizes, list) else [sizes] * len(self.src_bounds)
+        bad = [i for i, s in enumerate(self.batch_sizes) if s < self.world]
+        if bad:
+            raise ValueError("batch size %s%s gives bucket (%d, %d) fewer than one pair per replica (%d replicas)" % (
+                batch_size if batch_size_per_gpu is None else batch_size_per_gpu,
+                " tokens" if batch_by_tokens else "", self.src_bounds[bad[0]], self.trg_bounds[bad[0]], self.world))
+
+    def bucket_of(self, n_src, n_trg):
+        for i, (s, t) in enumerate(zip(self.src_bounds, self.trg_bounds)):
+            if n_src <= s and n_trg <= t:
+                return i
+        return None
+
+    def shapes(self):
+        """[(T, B per replica, L)]: the static shapes (one captured CUDA graph each in the trainer)."""
+        return [(s, b // self.world, t) for s, t, b in zip(self.src_bounds, self.trg_bounds, self.batch_sizes)]
+
+    def batches(self, examples):
+        """examples: {feature: LongTensor, transcript: LongTensor} -> (bucket, [per-replica example lists])."""
+        pools = {}
+        for ex in examples:
+            key = self.bucket_of(ex["feature"].numel(), ex["transcript"].numel())
+            if key is None:
+                continue
+            pool = pools.setdefault(key, [])
+            pool.append(ex)
+            if len(pool) == self.batch_sizes[key]:
+                pools[key] = []
+                yield key, [pool[r::self.world] for r in range(self.world)]
+
+
+def _pad_ids(rows, length, pad):
+    out = torch.full((len(rows), length), int(pad), dtype=torch.long)
+    for j, r in enumerate(rows):
+        out[j, :r.numel()] = r
+    return out
+
+
+class Seq2Seq:
+    """Data side of the `Seq2Seq` task over BPE'd text (neurst/tasks/seq2seq.py): get_data_preprocess_fn (:165-190) with
+    TextDataPipeline.encode(is_processed=True) (tokens -> ids, UNK for a token outside the vocabulary, EOS appended), the
+    TRAIN batching of create_and_batch_tfds (TokenBucketer), the EVAL / INFER padded_batch (file order, padded to the
+    longest in the batch) and example_to_input (:130-155).  Both sides use EOS as padding.  Raw text needs the
+    reference's tokenizer and BPE and is refused."""
+
+    def __init__(self, src_meta, trg_meta, max_src_len=None, max_trg_len=None, truncate_src=False, truncate_trg=False,
+                 batch_size=None, batch_size_per_gpu=None, batch_by_tokens=False, world=1):
+        self.src_meta, self.meta = dict(src_meta), dict(trg_meta)
+        for m in (self.src_meta, self.meta):
+            if not m.get("tokens"):
+                raise RuntimeError("the text path needs the vocabulary file (*_data_pipeline.params.vocab_path)")
+        self._src_vocab = {w: i for i, w in enumerate(self.src_meta["tokens"])}
+        self._trg_vocab = {w: i for i, w in enumerate(self.meta["tokens"])}
+        self.max_src_len, self.max_trg_len = max_src_len, max_trg_len
+        self.truncate_src, self.truncate_trg = truncate_src, truncate_trg
+        self._batching = dict(batch_size=batch_size, batch_size_per_gpu=batch_size_per_gpu, batch_by_tokens=batch_by_tokens,
+                              world=world)
+        self._bucketer = None
+
+    @property
+    def bucketer(self):
+        if self._bucketer is None:
+            self._bucketer = TokenBucketer(self.max_src_len, self.max_trg_len, **self._batching)
+        return self._bucketer
+
+    @staticmethod
+    def encode(text, vocab, meta):
+        """TextDataPipeline.encode(is_processed=True): whitespace tokens -> ids (UNK when missing) + [EOS]."""
+        unk = int(meta["unk_id"])
+        return [vocab.get(w, unk) for w in text.split()] + [int(meta["eos_id"])]
+
+    @staticmethod
+    def truncate(ids, max_len):
+        """seq2seq.py:171-176: beyond max_len keep the first max_len - 1 tokens and the last one (EOS)."""
+        return ids[:max_len - 1] + ids[-1:] if len(ids) > max_len else ids
+
+    def preprocess_fn(self, data_status, training=True, with_label=True):
+        if data_status["feature"] != "processed" or (with_label and data_status.get("label") != "processed"):
+            raise RuntimeError("raw text needs the reference's text pipeline (tokenizer / BPE): give BPE'd files with "
+                               "dataset.params.data_is_processed: True")
+
+        def side(text, vocab, meta, trunc, max_len):
+            ids = self.encode(text, vocab, meta)
+            if training and trunc and max_len:
+                ids = self.truncate(ids, int(max_len))
+            return torch.tensor(ids, dtype=torch.long)
+
+        def proc(data):
+            ret = {"feature": side(data["feature"], self._src_vocab, self.src_meta, self.truncate_src, self.max_src_len)}
+            if with_label:
+                ret["transcript"] = side(data["label"], self._trg_vocab, self.meta, self.truncate_trg, self.max_trg_len)
+            return ret
+        return proc
+
+    def keep(self, ex):
+        """clean_dataset_by_length (dataset_utils.py:328-337): 1 < length <= the maximum, on both sides."""
+        s, t = ex["feature"].numel(), ex["transcript"].numel()
+        return 1 < s <= int(self.max_src_len) and 1 < t <= int(self.max_trg_len)
+
+    def train_batches(self, examples, generator=None, pin=False):
+        """Yields, per step, the list of per-replica model inputs (padded to the bucket's bounds)."""
+        b = self.bucketer
+        kept = (e for e in examples if self.keep(e))
+        for key, groups in b.batches(kept):
+            T, Lq = b.src_bounds[key], b.trg_bounds[key]
+            yield [self.example_to_input({"feature": _pad_ids([e["feature"] for e in g], T, self.src_meta["pad_id"]),
+                                          "transcript": _pad_ids([e["transcript"] for e in g], Lq, self.meta["pad_id"])},
+                                         pin=pin) for g in groups]
+
+    def group_to_input(self, group, infer=True):
+        """EVAL / INFER padded_batch of a list of samples: file order, padded to the longest source (and target)."""
+        batch = {"feature": _pad_ids([e["feature"] for e in group], max(e["feature"].numel() for e in group),
+                                     self.src_meta["pad_id"])}
+        if not infer:
+            batch["transcript"] = _pad_ids([e["transcript"] for e in group], max(e["transcript"].numel() for e in group),
+                                           self.meta["pad_id"])
+        return self.example_to_input(batch, infer=infer)
+
+    @staticmethod
+    def _eos_padded_length(x, pad):
+        # deduce_text_length with EOS_AS_PADDING (models/model_utils.py:23-41): first pad (= EOS) position + 1
+        return (x != pad).to(torch.int32).argmin(-1) + 1
+
+    def example_to_input(self, batch, infer=False, pin=False):
+        src = batch["feature"]
+        B, T = src.shape
+        src_length = self._eos_padded_length(src, int(self.src_meta["pad_id"])).to(torch.long)
+        d = {"src": src, "src_padding": (torch.arange(T)[None, :] >= src_length[:, None]).to(torch.float32)}
+        bos = torch.full((B,), int(self.meta["bos_id"]), dtype=torch.long)
+        if infer:
+            d["trg_input"] = bos
+        else:
+            trg = batch["transcript"]
+            d["trg_length"] = self._eos_padded_length(trg, int(self.meta["pad_id"])).to(torch.long)
             d["trg"] = trg
             d["trg_input"] = torch.cat([bos[:, None], trg[:, :-1]], 1)
         if pin and torch.cuda.is_available():

@@ -433,3 +433,40 @@ def sample_logits(logits, top_k=0, top_p=1.0, seed=DEFAULT_SAMPLING_SEED, row_of
     L.check(L.load().b200st_sample_logits(z.data_ptr(), z.shape[0], z.shape[1], top_k, top_p, int(seed) & 0xFFFFFFFFFFFFFFFF,
                                           int(row_offset), int(step), out.data_ptr(), L._stream()))
     return out
+
+
+def cascade_remap(asr_tokens, mt_src_tokens, mt_unk_id, asr_vocab_size):
+    """int32 [asr_vocab_size] table ASR target id -> MT source id, by token string (TextDataPipeline's vocabulary lookup:
+    a later duplicate wins); ids past the ASR token list (<UNK>, <SEQ_BEG>, <SEQ_END>) and tokens missing from the MT
+    vocabulary map to the MT UNK."""
+    index = {w: i for i, w in enumerate(mt_src_tokens)}
+    table = torch.full((int(asr_vocab_size),), int(mt_unk_id), dtype=torch.int32)
+    for i, w in enumerate(asr_tokens[:int(asr_vocab_size)]):
+        table[i] = index.get(w, int(mt_unk_id))
+    return table
+
+
+def cascade_source(hyp_ids, remap, asr_eos_id, mt_vocab, mt_eos_id, mt_pad_id, mt_unk_id, max_src_len=0):
+    """b200st_cascade_source: ASR top-1 hypotheses (device int64 [B, hyp_len]) -> the MT source batch on the device
+    (src_ids int64 [B, T], src_padding fp32 [B, T], src_len int32 [B]), T the longest source (one copy of the lengths to
+    the host sets it, as padded_batch pads to the longest of the batch)."""
+    dev = hyp_ids.device
+    hyp = hyp_ids.to(torch.int64).contiguous()
+    B, n = hyp.shape
+    remap = remap.to(device=dev, dtype=torch.int32).contiguous()
+    lo, hi = int(remap.min()), int(remap.max())                   # the table is the caller's: checked before the launch
+    if lo < 0 or hi >= int(mt_vocab):
+        raise L.B200STError("cascade remap table holds ids outside the MT vocabulary of %d (%d..%d)" % (mt_vocab, lo, hi))
+    width = min(n + 1, int(max_src_len)) if max_src_len else n + 1
+    src = torch.empty(B, width, dtype=torch.int64, device=dev)
+    pad = torch.empty(B, width, dtype=torch.float32, device=dev)
+    length = torch.empty(B, dtype=torch.int32, device=dev)
+    a = L.CascadeSourceArgs()
+    a.hyp_ids, a.B, a.hyp_len, a.hyp_stride = hyp.data_ptr(), B, n, n
+    a.asr_eos_id, a.asr_vocab, a.remap = int(asr_eos_id), remap.numel(), remap.data_ptr()
+    a.mt_vocab, a.mt_eos_id, a.mt_pad_id, a.mt_unk_id = int(mt_vocab), int(mt_eos_id), int(mt_pad_id), int(mt_unk_id)
+    a.max_src_len, a.out_stride = int(max_src_len or 0), width
+    a.src_ids, a.src_padding, a.src_len = src.data_ptr(), pad.data_ptr(), length.data_ptr()
+    L.check(L.load().b200st_cascade_source(C.byref(a), L._stream()))
+    T = int(length.max())
+    return src[:, :T], pad[:, :T], length

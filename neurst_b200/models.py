@@ -9,6 +9,8 @@
 `forward(inputs, is_training)` takes the reference's input dict (neurst/tasks/speech2text.py:135-161) and returns
 logits [B, L, V].  Training uses the fused `forward_backward(inputs)` entry (loss + all gradients in one C call).
 """
+import re
+
 import torch
 
 from neurst_b200 import lib as L
@@ -43,6 +45,41 @@ def speech_transformer_hparams(name):
         "lr_schedule.class": "noam",
         "lr_schedule.params": {"initial_factor": 5.0 if dmodel > 256 else 3.5, "end_factor": 2.0 if dmodel > 256 else 1.5,
                                "dmodel": dmodel, "warmup_steps": 25000, "start_decay_at": 50000, "decay_steps": 50000},
+    }
+
+
+def transformer_hparams(name):
+    """neurst/models/transformer.py:136-240 (`Transformer.build_model_args_by_name`): the text presets and the
+    `transformer_<d>_<n>e_<m>d[_<h>h][_dp0.x]` pattern, with their Adam and noam defaults; None for other names."""
+    table = {"transformer_toy": (8, 2, 2, 2, 10, 0.1), "transformer_base": (512, 8, 6, 6, 2048, 0.1),
+             "transformer_s": (256, 4, 6, 6, 2048, 0.1), "transformer_big": (1024, 16, 6, 6, 4096, 0.3),
+             "transformer_big_dp01": (1024, 16, 6, 6, 4096, 0.1)}
+    if name in table:
+        dmodel, heads, enc, dec, ffn, rate = table[name]
+    elif re.match(r"^transformer_\d+_\d+e_\d+d(_\d+h)?(_dp0\.\d+)?$", str(name)):
+        eles = name.split("_")
+        dmodel, enc, dec, heads, idx = int(eles[1]), int(eles[2][:-1]), int(eles[3][:-1]), 8, 4
+        if len(eles) > idx and eles[idx][-1] == "h":
+            heads = int(eles[idx][:-1])
+            idx += 1
+        if dmodel % heads != 0:
+            raise ValueError("Invalid arguments in hparams_set: dimension({}) must be divisible by head({})".format(dmodel, heads))
+        rate = float(eles[idx][2:]) if len(eles) > idx and eles[idx][0:2] == "dp" else 0.1
+        ffn = dmodel * 4
+    else:
+        return None
+    params = {"modality.share_source_target_embedding": False, "modality.share_embedding_and_softmax_weights": True,
+              "modality.dim": dmodel, "modality.timing": "sinusoids"}
+    for side, nl in (("encoder", enc), ("decoder", dec)):
+        params.update({side + ".num_layers": nl, side + ".hidden_size": dmodel, side + ".num_attention_heads": heads,
+                       side + ".filter_size": ffn, side + ".attention_dropout_rate": rate,
+                       side + ".attention_type": "dot_product", side + ".ffn_activation": "relu",
+                       side + ".ffn_dropout_rate": rate, side + ".post_normalize": False,
+                       side + ".layer_postprocess_dropout_rate": rate})
+    return {
+        "model.class": "Transformer", "model.params": params,
+        "optimizer.class": "Adam", "optimizer.params": {"epsilon": 1.e-9, "beta_1": 0.9, "beta_2": 0.98},
+        "lr_schedule.class": "noam", "lr_schedule.params": {"initial_factor": 1.0, "dmodel": dmodel, "warmup_steps": 4000},
     }
 
 
@@ -292,12 +329,17 @@ class Transformer(_EncoderDecoder):
 
     @classmethod
     def build_model_args_by_name(cls, name):
-        return None
+        return transformer_hparams(name)
 
     @classmethod
     def new(cls, args, src_meta, trg_meta, name=None, precision="fp32", label_smoothing=0.0, device="cuda"):
         _check_supported(args, False)
+        if args.get("encoder.post_normalize") or args.get("decoder.post_normalize"):
+            raise NotImplementedError("post_normalize=True is not supported by libb200st (all presets are pre-norm)")
         share = bool(args.get("modality.share_source_target_embedding", False))
+        if share and src_meta["vocab_size"] != trg_meta["vocab_size"]:
+            raise ValueError("Source vocab_size should be equal to target vocab_size when modality.share_source_target_embedding"
+                             "=True (%d vs %d)" % (src_meta["vocab_size"], trg_meta["vocab_size"]))
         cfg = make_config(
             L.MODEL_TEXT, args["encoder.hidden_size"], args["encoder.num_attention_heads"], args["encoder.filter_size"],
             args["encoder.num_layers"], args["decoder.num_layers"], trg_meta["vocab_size"], src_vocab=src_meta["vocab_size"],

@@ -283,12 +283,17 @@ class GraphedTrainStep:
     def __init__(self, rt, B, T, Lq, allreduce=False):
         self.allreduce = bool(allreduce)
         cfg = rt.config
-        if cfg.model_type != L.MODEL_SPEECH:
-            raise L.B200STError("GraphedTrainStep supports the SpeechTransformer handle")
+        if cfg.model_type not in (L.MODEL_SPEECH, L.MODEL_TEXT):
+            raise L.B200STError("GraphedTrainStep supports the SpeechTransformer and text Transformer handles")
         self.rt, self.B, self.T, self.L = rt, B, T, Lq
+        self.text = cfg.model_type == L.MODEL_TEXT
         dev = rt.device
-        self.src = torch.zeros(B, T, cfg.feat, cfg.in_channels, dtype=torch.float32, device=dev)
-        self.src_length = torch.zeros(B, dtype=torch.int64, device=dev)
+        if self.text:            # source ids and their padding (1.0 beyond the source length)
+            self.src = torch.zeros(B, T, dtype=torch.int64, device=dev)
+            self.src_padding = torch.zeros(B, T, dtype=torch.float32, device=dev)
+        else:
+            self.src = torch.zeros(B, T, cfg.feat, cfg.in_channels, dtype=torch.float32, device=dev)
+            self.src_length = torch.zeros(B, dtype=torch.int64, device=dev)
         self.trg_input = torch.zeros(B, Lq, dtype=torch.int64, device=dev)
         self.trg = torch.zeros(B, Lq, dtype=torch.int64, device=dev)
         self.trg_length = torch.ones(B, dtype=torch.int64, device=dev)
@@ -303,7 +308,10 @@ class GraphedTrainStep:
         self.workspace = torch.empty(need + 256, dtype=torch.uint8, device=dev)
         self.bufs = rt._buffers(need, True, ws=self.workspace)
         bt = L.Batch()
-        bt.src, bt.src_length = self.src.data_ptr(), self.src_length.data_ptr()
+        if self.text:
+            bt.src_ids, bt.src_padding = self.src.data_ptr(), self.src_padding.data_ptr()
+        else:
+            bt.src, bt.src_length = self.src.data_ptr(), self.src_length.data_ptr()
         bt.trg_input, bt.trg, bt.trg_length = self.trg_input.data_ptr(), self.trg.data_ptr(), self.trg_length.data_ptr()
         bt.B, bt.T, bt.L, bt.training = B, T, Lq, 1
         bt.seed, bt.seed_dev, bt.loss_scale = 0, self.seed.data_ptr(), 1.0
@@ -349,7 +357,10 @@ class GraphedTrainStep:
         if self.rt._shadow_stale:
             self.rt.refresh_shadow()
         self.src.copy_(batch["src"], non_blocking=True)
-        self.src_length.copy_(batch["src_length"], non_blocking=True)
+        if self.text:
+            self.src_padding.copy_(batch["src_padding"], non_blocking=True)
+        else:
+            self.src_length.copy_(batch["src_length"], non_blocking=True)
         self.trg_input.copy_(batch["trg_input"], non_blocking=True)
         self.trg.copy_(batch["trg"], non_blocking=True)
         self.trg_length.copy_(batch["trg_length"], non_blocking=True)

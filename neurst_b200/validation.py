@@ -197,6 +197,8 @@ class Validator:
         from neurst_b200.models import LabelSmoothedCrossEntropy
         crit = LabelSmoothedCrossEntropy({"label_smoothing": self.vp["label_smoothing"]})
         rt = self.model.runtime
+        if self.plan.get("model_class") == "Transformer":
+            return self._text_loss_sums(mine, crit)
         dim = self.plan["task"]["audio_feature_dim"] * self.plan["task"]["audio_feature_channels"]
         pad = int(self.plan["trg_meta"]["pad_id"])
         out = []
@@ -213,6 +215,19 @@ class Validator:
                                             "transcript": trg})
             b = {k: v.to(rt.device) for k, v in b.items()}
             logits = rt.run({"src": b["src"], "src_length": b["src_length"], "trg_input": b["trg_input"], "training": False,
+                             "seed": 0, "want_logits": True}, backward=False)["logits"]
+            nll, _, ntok = crit(b, logits)
+            out.append((bi, float(nll.double().sum()), float(len(group)), float(ntok.double().sum())))
+        return out
+
+    def _text_loss_sums(self, mine, crit):
+        """_loss_sums of the text model: EVAL-mode padded_batch (seq2seq.py:236-244, padded to the longest source and
+        target of the batch)."""
+        rt = self.model.runtime
+        out = []
+        for bi, group in mine:
+            b = {k: v.to(rt.device) for k, v in self.task.group_to_input(group, infer=False).items()}
+            logits = rt.run({"src": b["src"], "src_padding": b["src_padding"], "trg_input": b["trg_input"], "training": False,
                              "seed": 0, "want_logits": True}, backward=False)["logits"]
             nll, _, ntok = crit(b, logits)
             out.append((bi, float(nll.double().sum()), float(len(group)), float(ntok.double().sum())))
