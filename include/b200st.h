@@ -75,6 +75,8 @@ typedef struct {
   int32_t deterministic;             /* 1: the hidden-dimension slices of the fused FFN kernel reduce into the output in slice
                                       * order (ticket per row tile) instead of arrival order: bit-reproducible steps for a few
                                       * microseconds per FFN launch (default 0: fp32 sums in arrival order) */
+  int32_t encoder_monotonic;         /* 1: causal encoder self-attention, query i sees keys j <= i (transformer_encoder.py:119-123,
+                                      * the wait-k model's encoder).  Text model (model_type 1) only; other models refuse it. */
 } b200st_config;
 
 int b200st_create(const b200st_config* cfg, b200st_handle* out);   /* host object only; no device memory */
@@ -115,6 +117,11 @@ typedef struct {
   float* nll_sum;               /* out, optional: [B] */
   float* n_tokens;              /* out, optional: [B] */
   float* enc_out;               /* out, optional: fp32 [B,T',d] */
+  int32_t wait_k;               /* wait-k lag of the decoder's cross-attention (0: none): target position i (0-based) sees the
+                                 * memory keys j < i + wait_k (transformer_decoder.py:194-208).  < 0, or > 0 on a model without
+                                 * cross-attention, fails before anything is launched. */
+  const int32_t* wait_k_dev;    /* optional device int32 lag, read at kernel run time instead of wait_k (CUDA-graph replay with a
+                                 * fresh lag per step); a value < 1 there means no lag */
 } b200st_batch;
 
 int64_t b200st_workspace_bytes(b200st_handle h, int32_t B, int32_t T, int32_t L, int32_t training);
@@ -175,6 +182,9 @@ typedef struct {
   const float* memory_bias;
   float* scratch;
   int32_t use_shadow;
+  int32_t wait_k;               /* wait-k lag (0: none): decoding step t attends to the memory keys j < min(Tm, wait_k + t), the
+                                 * offline form of the streaming agent (waitk_transformer.py:102-110).  < 0, or > 0 on a model
+                                 * without cross-attention or in b200st_ensemble_beam_search, fails before anything is launched. */
 } b200st_decode_state;
 int64_t b200st_decode_scratch_floats(b200st_handle h, int32_t B);
 /* TransformerDecoder.create_decoding_internal_cache + memorize_memory (transformer_decoder.py:105-147) */

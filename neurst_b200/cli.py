@@ -45,8 +45,10 @@ TOP_LEVEL = ("model_dir", "hparams_set", "dtype", "output_file", "entry", "searc
 # the validators' flags (neurst/training/validator.py, criterion_validator.py, seq_generation_validator.py): a flat
 # `--eval_steps 500` lands in validator.params, as the reference's registered flags do
 TEXT_TASKS = ("seqtoseq", "seq2seq")                       # registered as seq_to_seq and Seq2Seq
+WAITK_TASKS = ("waitktranslation",)                        # registered as WaitkTranslation and waitk_translation
 TEXT_DATASETS = ("paralleltextdataset", "paralleltext")
 TEXT_MODELS = ("transformer",)
+WAITK_MODELS = ("waitktransformer",)
 SPEECH_MODELS = ("speechtransformer", "b200speechtransformer", "b200st")
 VALIDATOR_FLAGS = ("eval_steps", "eval_start_at", "eval_on_begin", "eval_dataset", "eval_dataset.params", "eval_batch_size",
                    "eval_task_args", "eval_criterion", "eval_criterion.params", "eval_search_method", "eval_search_method.params",
@@ -331,32 +333,41 @@ def resolve_validator(cfg, tp, text=False):
 
 def resolve(cfg, world=1):
     """Everything the entries need, as plain dictionaries (also what the CPU test checks)."""
-    from neurst_b200.models import speech_transformer_hparams, transformer_hparams
+    from neurst_b200.models import speech_transformer_hparams, transformer_hparams, waitk_transformer_hparams
     if str(_module_name(cfg, "entry") or "").lower().replace("_", "") == "cascadest":
         return resolve_cascade(cfg, world)
     ep, tp = dict(cfg.get("entry.params") or {}), dict(cfg.get("task.params") or {})
     task_cls = str(cfg.get("task.class", "SpeechToText")).lower().replace("_", "")
-    text = task_cls in TEXT_TASKS
+    waitk = task_cls in WAITK_TASKS
+    text = task_cls in TEXT_TASKS or waitk
     if task_cls not in ("speechtotext", "speech2text") and not text:
-        raise SystemExit("task.class %r is outside this path (SpeechToText, Seq2Seq)" % cfg.get("task.class"))
+        raise SystemExit("task.class %r is outside this path (SpeechToText, Seq2Seq, WaitkTranslation)" % cfg.get("task.class"))
+    if not text and (tp.get("wait_k") is not None or cfg.get("wait_k", ep.get("wait_k")) is not None):
+        raise SystemExit("wait_k is outside this path for the SpeechToText task: wait-k decoding is the text WaitkTranslation "
+                         "task's (the reference has no simultaneous speech model)")
     ds_cls = str(cfg.get("dataset.class", "ParallelTextDataset" if text else "AudioTFRecordDataset")).lower().replace("_", "")
     if text and ds_cls not in TEXT_DATASETS:
         raise SystemExit("dataset.class %r is outside this path for the seq2seq task (ParallelTextDataset only)" % cfg.get("dataset.class"))
     if not text and ds_cls not in ("audiotfrecorddataset", "audiotfrecord"):
         raise SystemExit("dataset.class %r is outside this path (AudioTFRecordDataset only)" % cfg.get("dataset.class"))
     # the hparams_set's name picks the speech or the text table
-    hp_name = cfg.get("hparams_set") or ("transformer_s" if text else "speech_transformer_s")
+    hp_name = cfg.get("hparams_set") or ("waitk_transformer_s" if waitk else "transformer_s" if text else "speech_transformer_s")
     try:
-        hp = speech_transformer_hparams(hp_name) or transformer_hparams(hp_name)
+        hp = speech_transformer_hparams(hp_name) or transformer_hparams(hp_name) or waitk_transformer_hparams(hp_name)
     except ValueError as e:
         raise SystemExit(str(e))
     if hp is None:
         raise SystemExit("unknown hparams_set %r" % cfg.get("hparams_set"))
-    if hp["model.class"] != ("Transformer" if text else "SpeechTransformer"):
+    if hp["model.class"] not in (("Transformer", "WaitkTransformer") if text else ("SpeechTransformer",)):
         raise SystemExit("hparams_set %r is a %s preset, outside this path for the %s task" % (
             hp_name, hp["model.class"], "seq2seq" if text else "SpeechToText"))
     model_cls = str(cfg.get("model.class", hp["model.class"])).lower().replace("_", "")
-    if text and model_cls not in TEXT_MODELS:
+    if waitk and model_cls not in WAITK_MODELS:
+        raise SystemExit("model.class %r is outside this path for the WaitkTranslation task (WaitkTransformer only)"
+                         % cfg.get("model.class", hp["model.class"]))
+    if text and not waitk and model_cls in WAITK_MODELS:
+        raise SystemExit("model.class WaitkTransformer needs task.class WaitkTranslation (the task supplies wait_k)")
+    if text and not waitk and model_cls not in TEXT_MODELS:
         raise SystemExit("model.class %r is outside this path for the seq2seq task (Transformer only)"
                          % cfg.get("model.class", hp["model.class"]))
     if not text and model_cls not in SPEECH_MODELS:
@@ -370,7 +381,7 @@ def resolve(cfg, world=1):
     crit = ep.get("criterion.params") or {}
     entry = str(_module_name(cfg, "entry") or "trainer").lower()
     if text:
-        return _resolve_text(cfg, ep, tp, world, entry, model_params, opt, lr, crit)
+        return _resolve_text(cfg, ep, tp, world, entry, model_params, opt, lr, crit, waitk)
     # batch_size counts frames when batch_by_frames (speech2text.py:296-310): per-GPU budget = batch_size // replicas
     per_gpu = tp.get("batch_size_per_gpu")
     if per_gpu is None:
@@ -446,6 +457,9 @@ def resolve_cascade(cfg, world=1):
     dsp = dict(cfg.get("dataset.params") or {})
     if not dsp.get("data_path"):
         raise SystemExit("cascade_st needs dataset.params.data_path")
+    if str(_model_dir_configs(dirs["mt"], "mt_model_dir").get("model.class")) == "WaitkTransformer":
+        raise SystemExit("mt_model_dir %s holds a wait-k model (WaitkTransformer): wait-k decoding in cascade_st is outside "
+                         "this path" % dirs["mt"])
     batch_size = int(get("batch_size", 32))
     plans = {}
     for side, want in (("asr", "SpeechTransformer"), ("mt", "Transformer")):
@@ -500,8 +514,29 @@ def _pretrain_patterns(ep):
     return [None if p is None else str(p) for p in patterns]
 
 
-def _resolve_text(cfg, ep, tp, world, entry, model_params, opt, lr, crit):
-    """The plan of the seq2seq task over a text Transformer (Seq2Seq, ParallelTextDataset)."""
+def _resolve_wait_k(cfg, ep, tp, entry, model_dirs):
+    """The lag of a WaitkTranslation run, parsed as WaitkTranslation does (an int, a list or a YAML string of either).
+    `predict` takes it from the model directory's model_configs.yml unless a command-line --wait_k or task.params.wait_k
+    overrides it (the reference's eval_task_args use); training takes task.params.wait_k."""
+    from neurst_b200.models import parse_wait_k
+    k = cfg.get("wait_k", ep.get("wait_k"))
+    if k is None:
+        k = tp.get("wait_k")
+    if k is None and entry not in ("trainer", "train") and len(model_dirs) == 1:
+        path = os.path.join(model_dirs[0], MODEL_CONFIGS)
+        if os.path.isfile(path):
+            k = (_model_dir_configs(model_dirs[0], "model_dir").get("task.params") or {}).get("wait_k")
+    if k is None:
+        raise SystemExit("WaitkTranslation needs wait_k (task.params.wait_k, or --wait_k): the decode lagging")
+    try:
+        return parse_wait_k(k)
+    except ValueError as e:
+        raise SystemExit(str(e))
+
+
+def _resolve_text(cfg, ep, tp, world, entry, model_params, opt, lr, crit, waitk=False):
+    """The plan of the seq2seq task over a text Transformer (Seq2Seq, ParallelTextDataset), or of the WaitkTranslation task
+    over a WaitkTransformer (plan["wait_k"] set)."""
     src_meta, trg_meta = text_vocab_metas(tp)
     if model_params.get("modality.share_source_target_embedding") and src_meta["tokens"] != trg_meta["tokens"]:
         raise SystemExit("modality.share_source_target_embedding needs identical source and target vocabularies (%d vs %d "
@@ -534,7 +569,16 @@ def _resolve_text(cfg, ep, tp, world, entry, model_params, opt, lr, crit):
         "search": search,
         "output_file": cfg.get("output_file") or ep.get("output_file"),
     }
-    return _finish_plan(plan, cfg, ep, tp, search_method, model_dirs, text=True)
+    if waitk:
+        if len(model_dirs) > 1:
+            raise SystemExit("an ensemble of %d model_dirs with a wait-k model is outside this path (one WaitkTransformer per "
+                             "predict)" % len(model_dirs))
+        plan["wait_k"] = _resolve_wait_k(cfg, ep, tp, entry, model_dirs)
+        tp = dict(tp, wait_k=plan["wait_k"])
+    plan = _finish_plan(plan, cfg, ep, tp, search_method, model_dirs, text=True)
+    if waitk:
+        plan["task_config"]["task.class"] = "WaitkTranslation"
+    return plan
 
 
 def _finish_plan(plan, cfg, ep, tp, search_method, model_dirs, text=False):
@@ -632,7 +676,8 @@ def write_model_configs(plan):
     os.makedirs(plan["model_dir"], exist_ok=True)
     path = os.path.join(plan["model_dir"], MODEL_CONFIGS)
     with open(path + ".tmp", "w") as f:
-        configs = {"model.class": plan.get("model_class", "SpeechTransformer"), "model.params": dict(plan["model_params"])}
+        cls = "WaitkTransformer" if plan.get("wait_k") is not None else plan.get("model_class", "SpeechTransformer")
+        configs = {"model.class": cls, "model.params": dict(plan["model_params"])}
         configs.update(plan.get("task_config") or {})
         yaml.safe_dump(configs, f, default_flow_style=False)
     os.replace(path + ".tmp", path)
@@ -648,6 +693,8 @@ def member_model_params(plan, model_dir):
     with open(path) as f:
         cfg = yaml.safe_load(f) or {}
     cls = str(cfg.get("model.class", "SpeechTransformer")).lower().replace("_", "")
+    if cls in WAITK_MODELS:
+        raise SystemExit("%s: a wait-k model (WaitkTransformer) in an ensemble of model_dirs is outside this path" % path)
     if plan.get("model_class") == "Transformer":
         if cls not in TEXT_MODELS:
             raise SystemExit("%s: model.class %r is outside this path for the seq2seq task (Transformer only)"
@@ -670,7 +717,7 @@ def _dist_setup():
 
 
 def _build_model(plan):
-    from neurst_b200.models import SpeechTransformer, Transformer
+    from neurst_b200.models import SpeechTransformer, Transformer, WaitkTransformer
     tm = {k: v for k, v in plan["trg_meta"].items() if k != "tokens"}
     # only the target table feeds the tensor cores (logits GEMM and its gradient); the source table is gathered and
     # scatter-added in fp32, so a source vocabulary of any size runs on the 16-bit path
@@ -681,6 +728,9 @@ def _build_model(plan):
     if plan.get("model_class") == "Transformer":
         sm = {k: v for k, v in plan["src_meta"].items() if k != "tokens"}
         try:
+            if plan.get("wait_k") is not None:
+                return WaitkTransformer.new(plan["model_params"], sm, tm, precision=plan["precision"],
+                                            label_smoothing=plan["label_smoothing"], wait_k=plan["wait_k"], random_seed=plan["seed"])
             return Transformer.new(plan["model_params"], sm, tm, precision=plan["precision"], label_smoothing=plan["label_smoothing"])
         except (NotImplementedError, ValueError) as e:
             raise SystemExit(str(e))
@@ -875,11 +925,12 @@ def sampling_seed(seed, rank):
     return (int(seed) + int(rank) * 0x9E3779B97F4A7C15) & 0xFFFFFFFFFFFFFFFF
 
 
-def decode_group(model, task, plan, group, search_kw, first=0):
+def decode_group(model, task, plan, group, search_kw, first=0, lengths=None):
     """One search call over preprocessed samples -> [(ids_to_text hypothesis, score)], top_k (beam search) or sample_num
     (top_sampling) rows per utterance, consecutive (the reference's [B*top_k] order).  `first`: the position of group[0] in
     the rank's stream of utterances, which keys the samples' draws (row offset first * sample_num), so the samples do not
-    depend on how the stream is cut into calls."""
+    depend on how the stream is cut into calls.  `lengths` (a list): receives (source tokens without EOS, hypothesis tokens
+    without EOS) per row, the model-token lengths of the wait-k latency."""
     tm = plan["trg_meta"]
     if plan.get("model_class") == "Transformer":
         batch = task.group_to_input(group, infer=True)
@@ -898,6 +949,11 @@ def decode_group(model, task, plan, group, search_kw, first=0):
     else:
         search = model.beam_search if method == "beam_search" else model.greedy_search
     ids, score = search(inputs, **search_kw)
+    if lengths is not None:
+        per = ids.shape[0] // len(group)
+        for r, row in enumerate(ids.cpu().tolist()):
+            n = next((i for i, x in enumerate(row) if x == tm["eos_id"]), len(row))
+            lengths.append((int(group[r // per]["feature"].numel()) - 1, n))
     return [(ids_to_text(row, tm["eos_id"], tm.get("tokens")), lp) for row, lp in zip(ids.cpu().tolist(), score.cpu().tolist())]
 
 
@@ -923,20 +979,30 @@ def predict(plan):
     hyps = []
     group = []
     done = 0
+    lengths = [] if plan.get("wait_k") is not None else None
     for ex in examples:
         group.append(ex)
         if len(group) == per_call:
-            hyps.extend(decode_group(model, task, plan, group, search_kw, first=done))
+            hyps.extend(decode_group(model, task, plan, group, search_kw, first=done, lengths=lengths))
             done += len(group)
             group = []
     if group:
-        hyps.extend(decode_group(model, task, plan, group, search_kw, first=done))
+        hyps.extend(decode_group(model, task, plan, group, search_kw, first=done, lengths=lengths))
     out = plan["output_file"]
     if out and rank == 0:
         with open(out, "w", encoding="utf-8") as f:
             for text, _ in hyps:
                 f.write(text + "\n")
-    return {"checkpoint_step": step, "hypotheses": hyps}
+    result = {"checkpoint_step": step, "hypotheses": hyps}
+    if lengths is not None:
+        # the offline wait-k schedule's latency, in model (BPE) tokens: not comparable with SimulEval's word-level numbers
+        from neurst_b200.metrics import corpus_waitk_latency
+        k = model.lag(False)
+        result["latency"] = corpus_waitk_latency(k, lengths)
+        if result["latency"] is not None:
+            LOG.info("predict: wait-k %d latency over %d hypotheses (BPE tokens): AL %.4f AP %.4f DAL %.4f", k, len(lengths),
+                     result["latency"]["AL"], result["latency"]["AP"], result["latency"]["DAL"])
+    return result
 
 
 def _cascade_references(plan, key, meta):

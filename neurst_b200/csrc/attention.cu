@@ -1,7 +1,7 @@
 // Fused multi-head attention for sm_90a (head dim 64): S = QK^T and O = PV on wgmma with fp32 accumulators in
 // registers, operands staged by TMA, online softmax on the accumulator fragments (a query row lives in the four lanes of a
-// quad), additive key bias / causal mask exactly as the reference (multi_head_attention.py:145-160: logits + bias,
-// FLOAT_MIN = -1e9), dropout on the probabilities (:207-208) from the precomputed keep-bit bitmap.  The [B,H,Tq,Tk] score /
+// quad), additive key bias / diagonal key mask (KeyMask: causal, monotonic or wait-k) exactly as the reference
+// (multi_head_attention.py:145-160: logits + bias, FLOAT_MIN = -1e9), dropout on the probabilities (:207-208) from the precomputed keep-bit bitmap.  The [B,H,Tq,Tk] score /
 // probability tensors never touch HBM: forward keeps only the per-row log-sum-exp; backward recomputes P from Q, K and the
 // LSE (flash-attention style).
 //
@@ -41,7 +41,7 @@ struct AttnParams {
   float alpha;                 // dh^-0.5
   const float* bias;           // [B, Tk] additive or null
   const int32_t* kv_len;       // [B] or null: keys >= kv_len[b] are padding (bias -1e9): their key blocks are skipped
-  int causal;
+  KeyMask mask;                // CAUSAL kernels: key k hidden from query q when k > q + key_mask_off(mask, Tk)
   DropoutSpec drop;
   uint16_t* ctx; int64_t ctx_ld;          // [B*Tq, H*64], 16-bit type DT (bf16 or fp16)
   float* lse;                  // [B, H, Tq]  (natural log)
@@ -171,6 +171,7 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__
     const float a2 = p.alpha * kLog2e;
     const float cmask = kMaskMin * kLog2e;
     const bool use_drop = p.drop.p > 0.f;
+    const int moff = CAUSAL ? key_mask_off(p.mask, p.Tk) : 0;
     {
       const float* bias_row = p.bias ? p.bias + (int64_t)b * p.Tk : nullptr;
       for (int k = threadIdx.x - 128; k < nblk * BKV; k += 256)
@@ -223,7 +224,7 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__
         for (int r = 0; r < 2; ++r) {
           float x0 = fmaf(s[4 * c8 + 2 * r], a2, bb.x), x1 = fmaf(s[4 * c8 + 2 * r + 1], a2, bb.y);
           if (CAUSAL) {
-            const int qlim = qrow[r] + (p.Tk - p.Tq);         // keys k > qlim get the additive FLOAT_MIN
+            const int qlim = qrow[r] + moff;                  // keys k > qlim get the additive FLOAT_MIN
             x0 = (kcol > qlim) ? x0 + cmask : x0;
             x1 = (kcol + 1 > qlim) ? x1 + cmask : x1;
           }
@@ -387,6 +388,7 @@ attn_bwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__
   const float cmask = kMaskMin * kLog2e;
   const bool use_drop = p.drop.p > 0.f;
   const float dscale = use_drop ? p.drop.scale : 1.0f;
+  const int moff = CAUSAL ? key_mask_off(p.mask, p.Tk) : 0;
   const float kbias[2] = {smem_f(sB)[krow0], smem_f(sB)[krow0 + 8]};
   const int key[2] = {jb * BKV + krow0, jb * BKV + krow0 + 8};
   const int key16 = key[0] & ~15;                           // key[0] & 7 == g, key[1] = key[0] + 8
@@ -442,7 +444,7 @@ attn_bwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__
 #pragma unroll
         for (int e = 0; e < 2; ++e) {
           float x = fmaf(st_[4 * c8 + 2 * r + e], a2, kbias[r]);
-          if (CAUSAL) x = (key[r] > q0 + e + (p.Tk - p.Tq)) ? x + cmask : x;
+          if (CAUSAL) x = (key[r] > q0 + e + moff) ? x + cmask : x;
           const float pr = ex2_approx(x - (e ? lse2.y : lse2.x));
           const bool kp = (kb[2 * c8 + e] >> (8 * r + g)) & 1u;
           const float dpv = kp ? dpt[4 * c8 + 2 * r + e] : 0.f;
@@ -601,7 +603,7 @@ constexpr size_t kFwdSmemFixed = 1024 + (size_t)(1 + 2 + 1) * kTile16K + 8 * 7 +
 
 // q/k/v: bf16 views [B*T, ld] with head h at columns [h*64, h*64+64)
 int attention_fwd_fused(int dt, const void* q, int64_t q_ld, const void* k, int64_t k_ld, const void* v, int64_t v_ld, int B, int H,
-                        int Tq, int Tk, const float* bias, int causal, DropoutSpec drop, void* ctx, int64_t ctx_ld, float* lse,
+                        int Tq, int Tk, const float* bias, KeyMask mask, DropoutSpec drop, void* ctx, int64_t ctx_ld, float* lse,
                         cudaStream_t s, const int32_t* kv_len) {
   B200ST_CHECK(Tq > 0 && Tk > 0 && B > 0 && H > 0, "empty attention");
   B200ST_CHECK(B <= 65535 && H <= 65535, "attention grid too large");
@@ -613,11 +615,12 @@ int attention_fwd_fused(int dt, const void* q, int64_t q_ld, const void* k, int6
   AttnParams p{};
   p.B = B; p.H = H; p.Tq = Tq; p.Tk = Tk; p.Tkp = (Tk + 7) / 8 * 8;
   p.alpha = 0.125f;                     // 64^-0.5 (multi_head_attention.py:203)
-  p.bias = bias; p.causal = causal; p.drop = drop; p.kv_len = kv_len;
+  p.bias = bias; p.mask = mask; p.drop = drop; p.kv_len = kv_len;
   p.ctx = reinterpret_cast<uint16_t*>(ctx); p.ctx_ld = ctx_ld; p.lse = lse;
   B200ST_CHECK((reinterpret_cast<uintptr_t>(ctx) & 15) == 0 && ctx_ld % 8 == 0, "ctx must be 16-byte aligned");
   const size_t smem = kFwdSmemFixed + (size_t)((Tk + BKV - 1) / BKV) * 512;
   B200ST_CHECK(smem <= 227 * 1024, "fused attention: Tk too large for the shared-memory bias table");
+  const bool causal = mask.on != 0;
   auto kern = causal ? (dt == F16 ? attn_fwd_kernel<true, F16> : attn_fwd_kernel<true, BF16>)
                      : (dt == F16 ? attn_fwd_kernel<false, F16> : attn_fwd_kernel<false, BF16>);
   static size_t attr[4] = {0, 0, 0, 0};
@@ -637,7 +640,7 @@ int attention_fwd_fused(int dt, const void* q, int64_t q_ld, const void* k, int6
 // dq_scratch: fp32 [B*Tq, H*64] (overwritten).  dq/dk/dv: bf16 views like q/k/v.  lse / ctx from the forward pass.
 int attention_bwd_fused(int dt, const void* q, int64_t q_ld, const void* k, int64_t k_ld, const void* v, int64_t v_ld, const void* ctx,
                         int64_t ctx_ld, const void* dctx, int64_t dctx_ld, const float* lse, int B, int H, int Tq, int Tk,
-                        const float* bias, int causal, DropoutSpec drop, float* dq_scratch, void* dq, int64_t dq_ld, void* dk,
+                        const float* bias, KeyMask mask, DropoutSpec drop, float* dq_scratch, void* dq, int64_t dq_ld, void* dk,
                         int64_t dk_ld, void* dv, int64_t dv_ld, cudaStream_t s, const int32_t* kv_len) {
   B200ST_CHECK(Tq > 0 && Tk > 0 && B > 0 && H > 0 && B <= 65535 && H <= 65535, "bad attention shape");
   B200ST_CHECK(is16(dt), "fused attention needs a 16-bit operand type");
@@ -649,7 +652,7 @@ int attention_bwd_fused(int dt, const void* q, int64_t q_ld, const void* k, int6
   AttnParams p{};
   p.B = B; p.H = H; p.Tq = Tq; p.Tk = Tk; p.Tkp = (Tk + 7) / 8 * 8;
   p.alpha = 0.125f;
-  p.bias = bias; p.causal = causal; p.drop = drop; p.kv_len = kv_len;
+  p.bias = bias; p.mask = mask; p.drop = drop; p.kv_len = kv_len;
   p.ctx = reinterpret_cast<uint16_t*>(const_cast<void*>(ctx)); p.ctx_ld = ctx_ld;
   p.lse = const_cast<float*>(lse);
   p.dctx = reinterpret_cast<const uint16_t*>(dctx); p.dctx_ld = dctx_ld;
@@ -680,6 +683,7 @@ int attention_bwd_fused(int dt, const void* q, int64_t q_ld, const void* k, int6
     B200ST_LAUNCH_CHECK();
   }
   dim3 grid((Tk + BKV - 1) / BKV, H, B);
+  const bool causal = mask.on != 0;
   auto kern = causal ? (dt == F16 ? attn_bwd_kernel<true, F16> : attn_bwd_kernel<true, BF16>)
                      : (dt == F16 ? attn_bwd_kernel<false, F16> : attn_bwd_kernel<false, BF16>);
   launch_pdl(kern, grid, kBwdThreads, kBwdSmem, s, tq, tk, tv, tdo, p);

@@ -109,7 +109,9 @@ int b200st_create(const b200st_config* cfg, b200st_handle* out) {
   c.with_cross_attention = cfg->with_cross_attention;
   c.disable_fused_attention = cfg->disable_fused_attention;
   c.deterministic = cfg->deterministic;
+  c.encoder_monotonic = cfg->encoder_monotonic;
   if (c.model_type < 0 || c.model_type > MODEL_MHA) { delete h; B200ST_FAIL("unknown model_type"); }
+  if (c.encoder_monotonic && c.model_type != MODEL_TEXT) { delete h; B200ST_FAIL("encoder_monotonic applies to the text model only"); }
   if (c.attention_dropout < 0 || c.attention_dropout >= 1 || c.ffn_dropout < 0 || c.ffn_dropout >= 1 ||
       c.postprocess_dropout < 0 || c.postprocess_dropout >= 1) { delete h; B200ST_FAIL("dropout rates must be in [0,1)"); }
   if (int r = build_param_table(h->m)) { delete h; return r; }
@@ -185,6 +187,7 @@ static Batch to_batch(const b200st_batch* b) {
   r.trg_input = b->trg_input; r.trg = b->trg; r.trg_length = b->trg_length;
   r.B = b->B; r.T = b->T; r.L = b->L; r.training = b->training; r.seed = b->seed; r.seed_dev = b->seed_dev; r.loss_scale = b->loss_scale; r.loss_scale_dev = b->loss_scale_dev;
   r.logits = b->logits; r.loss = b->loss; r.nll_sum = b->nll_sum; r.n_tokens = b->n_tokens; r.enc_out = b->enc_out;
+  r.wait_k = b->wait_k; r.wait_k_dev = b->wait_k_dev;
   return r;
 }
 
@@ -220,6 +223,7 @@ static DecodeState to_state(const b200st_decode_state* s) {
   d.B = s->B; d.Tm = s->Tm; d.max_len = s->max_len;
   d.cross_kv = s->cross_kv; d.self_kv = s->self_kv; d.memory_bias = s->memory_bias; d.scratch = s->scratch;
   d.use_shadow = s->use_shadow;
+  d.wait_k = s->wait_k;
   return d;
 }
 int64_t b200st_decode_scratch_floats(b200st_handle h, int32_t B) {
@@ -286,6 +290,7 @@ int b200st_ensemble_beam_search(const b200st_ensemble_member* members, int32_t n
     const b200st_ensemble_member& x = members[i];
     if (!x.h || !x.buf || !x.st) B200ST_FAIL("ensemble member " + std::to_string(i) + ": null argument");
     em[i] = EnsembleMember{&x.h->m, to_buffers(x.buf), to_state(x.st), x.weight};
+    if (em[i].st.wait_k != 0) B200ST_FAIL("ensemble member " + std::to_string(i) + ": wait_k is not supported in ensemble decoding");
   }
   return ensemble_beam_search(em, n_members, to_beam_args(a), reinterpret_cast<cudaStream_t>(stream));
 }
@@ -377,7 +382,7 @@ int b200st_layernorm_bwd(const void* dy, int32_t dy_dtype, const void* x, int32_
 int b200st_softmax_fwd(const float* S, int64_t ldS, const float* bias_2d, int32_t causal, void* P, int32_t p_dtype,
                        int64_t ldP, int32_t B, int32_t H, int32_t Tq, int32_t Tk, void* stream) {
   if (!S || !P) B200ST_FAIL("null argument");
-  return softmax_fwd(S, ldS, bias_2d, causal, P, nullptr, p_dtype, ldP, B, H, Tq, Tk, no_dropout(), reinterpret_cast<cudaStream_t>(stream));
+  return softmax_fwd(S, ldS, bias_2d, causal ? causal_mask(Tq, Tk) : no_key_mask(), P, nullptr, p_dtype, ldP, B, H, Tq, Tk, no_dropout(), reinterpret_cast<cudaStream_t>(stream));
 }
 int b200st_conv1_ln_relu_fwd(const float* src, const float* w, const float* b, const float* gamma, const float* beta,
                              void* y1, int32_t dtype, int32_t B, int32_t T, int32_t F, int32_t Cin, int32_t C,

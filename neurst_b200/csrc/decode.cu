@@ -123,19 +123,22 @@ __global__ void __launch_bounds__(128) gemv_kernel(const float* __restrict__ in,
 // slot of row anc[b][j] (the ancestry table kept by beam_select_kernel, so beams are reordered without copying the
 // cache); position `time` is always the row's own slot.  Cross-attention reads the memory of utterance b / beam, which
 // is projected once per utterance.
+// wait_k > 0 (cross-attention, wait-k decoding, waitk_transformer.py:102-110): step t attends to the memory keys
+// j < min(Tm, wait_k + t) only.  The hidden keys would carry FLOAT_MIN and contribute an exact 0 to the maximum, the sum and
+// the context, so scanning the visible prefix gives the masked result.
 template <typename TW, bool SELF, bool BEAM = false>
 __global__ void __launch_bounds__(256) attn_step_kernel(const float* __restrict__ qsrc, int q_ld, float* __restrict__ kcache,
                                                         float* __restrict__ vcache, int kv_ld, int cache_rows,
                                                         const float* __restrict__ mem_bias, const TW* __restrict__ Wo,
                                                         const float* __restrict__ bo, float* __restrict__ x, int d, int dh, int Tm,
-                                                        const int* __restrict__ time_dev, const int* __restrict__ anc = nullptr,
+                                                        int wait_k, const int* __restrict__ time_dev, const int* __restrict__ anc = nullptr,
                                                         int beam = 1) {
   pdl_wait();
   pdl_trigger();
   extern __shared__ float sm[];          // q[dh] | ctx[dh] | scores[nk] | red[8] (| BEAM && SELF: slot of each key [nk])
   const int h = blockIdx.x, b = blockIdx.y;
   const int t = *time_dev;
-  const int nk = SELF ? t + 1 : Tm;
+  const int nk = SELF ? t + 1 : (wait_k > 0 ? min(Tm, wait_k + t) : Tm);
   const int mb = (BEAM && !SELF) ? b / beam : b;      // memory row
   float* q = sm;
   float* ctx = sm + dh;
@@ -143,6 +146,7 @@ __global__ void __launch_bounds__(256) attn_step_kernel(const float* __restrict_
   float* red = sc + nk;
   int* slot = reinterpret_cast<int*>(red + 8);
   const float* qrow = qsrc + (int64_t)b * q_ld + h * dh;
+  const float* mbias = (!SELF && mem_bias) ? mem_bias + (int64_t)mb * Tm : nullptr;
   float* kbase = kcache + (int64_t)mb * cache_rows * kv_ld + h * dh;
   float* vbase = vcache + (int64_t)mb * cache_rows * kv_ld + h * dh;
   // key j is read at kb + koff(j): the own row's cache, or (BEAM && SELF) cache slot (anc[b][j], j) of the whole cache
@@ -174,7 +178,7 @@ __global__ void __launch_bounds__(256) attn_step_kernel(const float* __restrict_
     } else {
       for (int c = 0; c < dh; ++c) s = fmaf(q[c], kr[c], s);
     }
-    sc[j] = s + ((!SELF && mem_bias) ? mem_bias[(int64_t)mb * Tm + j] : 0.f);
+    sc[j] = s + (mbias ? mbias[j] : 0.f);
   }
   __syncthreads();
   float mx = -INFINITY;
@@ -396,6 +400,7 @@ struct PersistentArgs {
   LayerOffs layer[kMaxDecLayers];
   int64_t emb, emb_bias, out_lng, out_lnb;
   int n_layers, B, d, H, ffn, V, Tm, max_len, cross;
+  int wait_k;                     // cross-attention lag (0: none), as attn_step_kernel's
   float eps;
   const float* params;            // fp32 master arena (biases, LayerNorm parameters; weights too when TW = float)
   float* scratch;                 // layout_of(): x | qkv | qc | hid | logits
@@ -469,8 +474,8 @@ __device__ __forceinline__ void gemv_item(int item, const float* in, const float
 template <typename TW, bool SELF>
 __device__ __forceinline__ void attn_item(int h, int b, int t, const float* qsrc, int q_ld, float* kcache, float* vcache, int kv_ld,
                                           int cache_rows, const float* mem_bias, const TW* __restrict__ Wo, const float* bo, float* x, int d,
-                                          int dh, int Tm, float* sm) {
-  const int nk = SELF ? t + 1 : Tm;
+                                          int dh, int Tm, int wait_k, float* sm) {
+  const int nk = SELF ? t + 1 : (wait_k > 0 ? min(Tm, wait_k + t) : Tm);
   float* q = sm;
   float* ctx = sm + dh;
   float* sc = sm + 2 * dh;
@@ -577,7 +582,7 @@ __global__ void __launch_bounds__(256, 1) greedy_persistent_kernel(const __grid_
         float* sk = a.self_kv + (int64_t)l * 2 * B * a.max_len * d;
         float* sv = sk + (int64_t)B * a.max_len * d;
         for (int it = bid; it < H * B; it += nb)
-          attn_item<TW, true>(it % H, it / H, t, qkv, 3 * d, sk, sv, d, a.max_len, nullptr, wbase + L.s_out, P + L.s_outb, x, d, dh, 0, dsm);
+          attn_item<TW, true>(it % H, it / H, t, qkv, 3 * d, sk, sv, d, a.max_len, nullptr, wbase + L.s_out, P + L.s_outb, x, d, dh, 0, 0, dsm);
       }
       grid_barrier(a.barrier, target);
       if (a.cross) {
@@ -590,7 +595,7 @@ __global__ void __launch_bounds__(256, 1) greedy_persistent_kernel(const __grid_
         {
           float* ck = a.cross_kv + (int64_t)l * B * a.Tm * 2 * d;
           for (int it = bid; it < H * B; it += nb)
-            attn_item<TW, false>(it % H, it / H, t, qc, d, ck, ck + d, 2 * d, a.Tm, a.mem_bias, wbase + L.c_out, P + L.c_outb, x, d, dh, a.Tm, dsm);
+            attn_item<TW, false>(it % H, it / H, t, qc, d, ck, ck + d, 2 * d, a.Tm, a.mem_bias, wbase + L.c_out, P + L.c_outb, x, d, dh, a.Tm, a.wait_k, dsm);
         }
         grid_barrier(a.barrier, target);
       }
@@ -751,7 +756,7 @@ int step_launch(const StepCtx& c, const TW* wbase, const int64_t* ids, const int
     const size_t smem_self = self_attn_smem(cf, st.max_len, anc != nullptr);
     launch_pdl(anc ? attn_step_kernel<TW, true, true> : attn_step_kernel<TW, true>, dim3(H, B), 256, smem_self, c.s,
                (const float*)qkv, 3 * d, sk, sv, d, st.max_len, (const float*)nullptr, W(p + ".self.out.kernel"),
-               c.P(p + ".self.out.bias"), x, d, dh, 0, time_dev, anc, beam);
+               c.P(p + ".self.out.bias"), x, d, dh, 0, 0, time_dev, anc, beam);
     // encoder-decoder attention block over the pre-projected memory
     if (cf.with_cross_attention && st.Tm > 0) {
       launch_pdl(gemv_kernel<TW, 0>, dim3((d + 127) / 128, (d + 31) / 32), 128, 0, c.s, (const float*)x, c.P(p + ".cross.ln.gamma"),
@@ -760,7 +765,7 @@ int step_launch(const StepCtx& c, const TW* wbase, const int64_t* ids, const int
       const size_t smem_cross = sizeof(float) * (size_t)(2 * dh + st.Tm + 8);
       launch_pdl(anc ? attn_step_kernel<TW, false, true> : attn_step_kernel<TW, false>, dim3(H, B), 256, smem_cross, c.s,
                  (const float*)qc, d, ck, ck + d, 2 * d, st.Tm, st.memory_bias, W(p + ".cross.out.kernel"),
-                 c.P(p + ".cross.out.bias"), x, d, dh, st.Tm, time_dev, anc, beam);
+                 c.P(p + ".cross.out.bias"), x, d, dh, st.Tm, st.wait_k, time_dev, anc, beam);
     }
     // feed-forward block
     launch_pdl(gemv_kernel<TW, 0>, dim3((f + 127) / 128, (d + 31) / 32), 128, 0, c.s, (const float*)x, c.P(p + ".ffn.ln.gamma"),
@@ -865,6 +870,7 @@ int launch_persistent(const Model& m, const Buffers& buf, const DecodeState& st,
   a.emb = off("trg.emb"); a.emb_bias = off("trg.bias"); a.out_lng = off("dec.out_ln.gamma"); a.out_lnb = off("dec.out_ln.beta");
   a.n_layers = cf.dec_layers; a.B = st.B; a.d = cf.d; a.H = cf.heads; a.ffn = cf.ffn; a.V = cf.vocab; a.Tm = st.Tm; a.max_len = st.max_len;
   a.cross = (cf.with_cross_attention && st.Tm > 0) ? 1 : 0;
+  a.wait_k = st.wait_k;
   a.eps = cf.ln_eps;
   a.params = buf.params; a.scratch = st.scratch;
   const DecodeLayout lo = layout_of(cf, st.B);
@@ -901,6 +907,8 @@ int check_state(const Model& m, const DecodeState& st) {
   B200ST_CHECK(st.B >= 1 && st.B <= max_rows, "decode batch must be 1.." + std::to_string(max_rows));
   B200ST_CHECK(st.max_len >= 1 && st.Tm >= 0, "bad decode lengths");
   B200ST_CHECK(st.self_kv && st.scratch && (st.Tm == 0 || st.cross_kv), "decode state buffers missing");
+  B200ST_CHECK(st.wait_k >= 0, "wait_k must be >= 0 (0: no lag), got " + std::to_string(st.wait_k));
+  B200ST_CHECK(st.wait_k == 0 || cf.with_cross_attention, "wait_k needs a decoder with cross-attention");
   const int dh = cf.d / cf.heads;
   B200ST_CHECK(dh <= 256 && 256 % dh == 0, "decode kernels need a head dim that divides 256");
   const size_t smem = sizeof(float) * (size_t)(2 * dh + (st.Tm > st.max_len ? st.Tm : st.max_len) + 8);

@@ -320,15 +320,18 @@ __global__ void __launch_bounds__(kAttnThreads) rows_self_attn_kernel(const floa
 }
 
 // Cross-attention of the `beam` rows of utterance u, head h over the pre-projected memory ([u][Tm][2d]: keys | values) with
-// the additive memory bias: every key and value row is read once for all the utterance's rows.
+// the additive memory bias: every key and value row is read once for all the utterance's rows.  wait_k > 0: step t scans
+// the visible keys j < min(Tm, wait_k + t) only, as attn_step_kernel (decode.cu).
 // smem: q[beam][dh] | scores[beam][Tm] | partial context[beam][blockDim] | inv[beam] | red[32]
 __global__ void __launch_bounds__(kAttnThreads) rows_cross_attn_kernel(const float* __restrict__ qc, const float* __restrict__ mem,
                                                                       const float* __restrict__ mem_bias, int d, int dh, int Tm,
-                                                                      int beam, float* __restrict__ ctx) {
+                                                                      int wait_k, const int32_t* __restrict__ time_dev, int beam,
+                                                                      float* __restrict__ ctx) {
   pdl_wait();
   pdl_trigger();
   extern __shared__ float sm[];
   const int h = blockIdx.x, u = blockIdx.y, r0 = u * beam;
+  const int nk = wait_k > 0 ? min(Tm, wait_k + *time_dev) : Tm;
   float* q = sm;
   float* sc = q + beam * dh;
   float* part = sc + (int64_t)beam * Tm;
@@ -339,7 +342,7 @@ __global__ void __launch_bounds__(kAttnThreads) rows_cross_attn_kernel(const flo
   __syncthreads();
   const float* kb = mem + (int64_t)u * Tm * 2 * d + h * dh;
   const float* vb = kb + d;
-  for (int j = threadIdx.x; j < Tm; j += blockDim.x) {
+  for (int j = threadIdx.x; j < nk; j += blockDim.x) {
     const float* kr = kb + (int64_t)j * 2 * d;
     float s[kBeamMax];
 #pragma unroll
@@ -370,10 +373,10 @@ __global__ void __launch_bounds__(kAttnThreads) rows_cross_attn_kernel(const flo
   for (int r = 0; r < beam; ++r) {
     float* z = sc + (int64_t)r * Tm;
     float mx = -INFINITY;
-    for (int j = threadIdx.x; j < Tm; j += blockDim.x) mx = fmaxf(mx, z[j]);
+    for (int j = threadIdx.x; j < nk; j += blockDim.x) mx = fmaxf(mx, z[j]);
     mx = block_max(mx, red);
     float se = 0.f;
-    for (int j = threadIdx.x; j < Tm; j += blockDim.x) { const float e = expf(z[j] - mx); z[j] = e; se += e; }
+    for (int j = threadIdx.x; j < nk; j += blockDim.x) { const float e = expf(z[j] - mx); z[j] = e; se += e; }
     se = block_sum(se, red);
     if (threadIdx.x == 0) inv[r] = 1.f / se;
   }
@@ -382,7 +385,7 @@ __global__ void __launch_bounds__(kAttnThreads) rows_cross_attn_kernel(const flo
   float a[kBeamMax];
 #pragma unroll
   for (int r = 0; r < kBeamMax; ++r) a[r] = 0.f;
-  for (int j = pt; j < Tm; j += np) {
+  for (int j = pt; j < nk; j += np) {
     const float v = vb[(int64_t)j * 2 * d + c];
 #pragma unroll
     for (int r = 0; r < kBeamMax; ++r) if (r < beam) a[r] = fmaf(sc[(int64_t)r * Tm + j], v, a[r]);
@@ -565,7 +568,7 @@ int rows_step_t(const Model& m, const Buffers& buf, const DecodeState& st, const
       B200ST_TRY(rows_gemm(x, B, d, W(p + ".cross.q.kernel"), true, d, PRE_LN, P(p + ".cross.ln.gamma"), P(p + ".cross.ln.beta"),
                            cf.ln_eps, nullptr, P(p + ".cross.q.bias"), qc, EPI_STORE, lo, sc, s));
       launch_pdl(rows_cross_attn_kernel, dim3(H, B / beam), kAttnThreads, smem_cross, s, (const float*)qc,
-                 (const float*)(st.cross_kv + (int64_t)i * cross_layer), st.memory_bias, d, dh, st.Tm, beam, ctx);
+                 (const float*)(st.cross_kv + (int64_t)i * cross_layer), st.memory_bias, d, dh, st.Tm, st.wait_k, time_dev, beam, ctx);
       B200ST_TRY(rows_gemm(ctx, B, d, W(p + ".cross.out.kernel"), true, d, PRE_NONE, nullptr, nullptr, 0.f, nullptr,
                            P(p + ".cross.out.bias"), x, EPI_ADD, lo, sc, s));
     }

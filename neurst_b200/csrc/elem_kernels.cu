@@ -412,7 +412,7 @@ int layernorm_bwd_next(const void* dy, int dy_dtype, const void* x, int x_dtype,
 }
 
 // =============================================================================================
-// softmax (+ additive key bias, causal mask, dropout) : one warp per (b,h,q) row
+// softmax (+ additive key bias, diagonal key mask (KeyMask), dropout) : one warp per (b,h,q) row
 // =============================================================================================
 constexpr float kFloatMin = -1.0e9f;   // neurst/utils/compat.py:24
 
@@ -454,7 +454,7 @@ template <> __device__ __forceinline__ void load8<__half>(const __half* src, flo
 
 template <typename T, int STEPS>
 __global__ void __launch_bounds__(256) softmax_fwd_kernel(const float* __restrict__ S, int64_t ldS,
-                                                           const float* __restrict__ bias, int causal,
+                                                           const float* __restrict__ bias, KeyMask mask,
                                                            T* __restrict__ P_pre, T* __restrict__ P_drop, int64_t ldP,
                                                            int B, int H, int Tq, int Tk, DropoutSpec drop) {
   pdl_wait();
@@ -463,12 +463,13 @@ __global__ void __launch_bounds__(256) softmax_fwd_kernel(const float* __restric
   const int64_t rows = (int64_t)B * H * Tq;
   const int64_t warps_total = (int64_t)gridDim.x * (blockDim.x >> 5);
   const uint32_t thresh = dropout_thresh16(drop.p);
+  const int causal = mask.on, moff = mask.on ? key_mask_off(mask, Tk) : 0;
   for (int64_t row = (int64_t)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5); row < rows; row += warps_total) {
     const int q = (int)(row % Tq);
     const int b = (int)(row / ((int64_t)H * Tq));
     const float* sr = S + row * ldS;
     const float* br = bias ? bias + (int64_t)b * Tk : nullptr;
-    const int kmax_visible = q + (Tk - Tq);
+    const int kmax_visible = q + moff;
     float v[STEPS][8];
     float mx = -INFINITY;
 #pragma unroll
@@ -518,7 +519,7 @@ __global__ void __launch_bounds__(256) softmax_fwd_kernel(const float* __restric
   }
 }
 
-int softmax_fwd(const float* S, int64_t ldS, const float* bias, int causal, void* P_pre, void* P_drop, int p_dtype,
+int softmax_fwd(const float* S, int64_t ldS, const float* bias, KeyMask mask, void* P_pre, void* P_drop, int p_dtype,
                 int64_t ldP, int B, int H, int Tq, int Tk, DropoutSpec drop, cudaStream_t s) {
   const int64_t rows = (int64_t)B * H * Tq;
   if (rows == 0) return 0;
@@ -526,7 +527,7 @@ int softmax_fwd(const float* S, int64_t ldS, const float* bias, int causal, void
   B200ST_CHECK((reinterpret_cast<uintptr_t>(S) & 31) == 0 && (reinterpret_cast<uintptr_t>(P_pre) & 15) == 0, "softmax alignment");
   B200ST_CHECK(Tk <= 2048, "softmax supports up to 2048 keys");
   const int grid = grid_for(rows, 8);
-#define SM_FWD(ST) DISPATCH_DTYPE(p_dtype, T, (launch_pdl(softmax_fwd_kernel<T, ST>, grid, 256, 0, s, S, ldS, bias, causal, (T*)P_pre, \
+#define SM_FWD(ST) DISPATCH_DTYPE(p_dtype, T, (launch_pdl(softmax_fwd_kernel<T, ST>, grid, 256, 0, s, S, ldS, bias, mask, (T*)P_pre, \
                                                                                    (T*)P_drop, ldP, B, H, Tq, Tk, drop)))
   if (Tk <= 256) SM_FWD(1); else if (Tk <= 512) SM_FWD(2); else if (Tk <= 1024) SM_FWD(4); else SM_FWD(8);
 #undef SM_FWD

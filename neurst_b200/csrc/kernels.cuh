@@ -25,10 +25,35 @@ int layernorm_bwd_next(const void* dy, int dy_dtype, const void* x, int x_dtype,
                        float* dbeta, int64_t rows, int cols, int relu, void* dnext, int dnext_dtype, DropoutSpec ndrop,
                        cudaStream_t s);
 
-// P = softmax(S + bias[b, k] + causal) over k (multi_head_attention.py:147-160,207-208).
-// S fp32 [B,H,Tq,ldS]; bias fp32 [B,Tk] or null; causal: key k visible to query q iff k <= q + (Tk - Tq).
+// Diagonal key mask of an attention: when `on`, key k is hidden from query q (additive FLOAT_MIN, as the reference's
+// lower-triangle bias) when k > q + off, with off = *lag_dev - 1 when lag_dev is set (a wait-k lag read at kernel run
+// time, after griddepcontrol.wait, so that a replayed CUDA graph follows a fresh lag; a lag < 1 there hides nothing), else
+// `off`.  The decoder self-attention passes off = Tk - Tq (causal_mask), the monotonic encoder off = 0
+// (transformer_encoder.py:119-123), wait-k cross-attention with lag k off = k - 1: target i sees memory keys j < i + k
+// (transformer_decoder.py:194-208, layer_utils.py:56-78).
+// The reference combines this mask with the padding bias by `min`, the kernels here add both: a key masked twice gets -2e9
+// instead of -1e9.  Either way its probability is exactly 0 in fp32 unless every key of the row is masked, which cannot
+// happen: off >= 0 keeps key 0 visible to every query, and key 0 of a text source is never padding (a source holds at
+// least its EOS).
+struct KeyMask {
+  int on;
+  int off;
+  const int32_t* lag_dev;
+};
+inline KeyMask no_key_mask() { return KeyMask{0, 0, nullptr}; }
+inline KeyMask causal_mask(int Tq, int Tk) { return KeyMask{1, Tk - Tq, nullptr}; }
+#ifdef __CUDACC__
+__device__ __forceinline__ int key_mask_off(const KeyMask& m, int Tk) {
+  if (!m.lag_dev) return m.off;
+  const int lag = *m.lag_dev;
+  return lag > 0 ? lag - 1 : Tk;
+}
+#endif
+
+// P = softmax(S + bias[b, k] + mask) over k (multi_head_attention.py:147-160,207-208).
+// S fp32 [B,H,Tq,ldS]; bias fp32 [B,Tk] or null; mask: see KeyMask.
 // Writes P_pre and (if drop.p > 0) P_drop = dropout(P_pre), both `p_dtype` with row stride ldP.
-int softmax_fwd(const float* S, int64_t ldS, const float* bias, int causal, void* P_pre, void* P_drop, int p_dtype,
+int softmax_fwd(const float* S, int64_t ldS, const float* bias, KeyMask mask, void* P_pre, void* P_drop, int p_dtype,
                 int64_t ldP, int B, int H, int Tq, int Tk, DropoutSpec drop, cudaStream_t s);
 // dS = P * (dP' - sum_k dP' P), dP' = dropout'(dP); dP fp32 [rows, ldS], output `p_dtype` [rows, ldP].
 int softmax_bwd(const float* dP, int64_t ldS, const void* P_pre, void* dS, int p_dtype, int64_t ldP, int64_t rows,
@@ -108,11 +133,11 @@ int fill_f32(float* x, float v, int64_t n, cudaStream_t s);
 // kv_len (optional, int32 [B]): keys >= kv_len[b] all carry the -1e9 padding bias — their probabilities are exactly 0 in
 // fp32, so whole key blocks beyond it are skipped (bit-identical result; ragged batches of cfg-4)
 int attention_fwd_fused(int dt, const void* q, int64_t q_ld, const void* k, int64_t k_ld, const void* v, int64_t v_ld, int B, int H,
-                        int Tq, int Tk, const float* bias, int causal, DropoutSpec drop, void* ctx, int64_t ctx_ld, float* lse,
+                        int Tq, int Tk, const float* bias, KeyMask mask, DropoutSpec drop, void* ctx, int64_t ctx_ld, float* lse,
                         cudaStream_t s, const int32_t* kv_len = nullptr);
 int attention_bwd_fused(int dt, const void* q, int64_t q_ld, const void* k, int64_t k_ld, const void* v, int64_t v_ld, const void* ctx,
                         int64_t ctx_ld, const void* dctx, int64_t dctx_ld, const float* lse, int B, int H, int Tq, int Tk,
-                        const float* bias, int causal, DropoutSpec drop, float* dq_scratch, void* dq, int64_t dq_ld, void* dk,
+                        const float* bias, KeyMask mask, DropoutSpec drop, float* dq_scratch, void* dq, int64_t dq_ld, void* dk,
                         int64_t dk_ld, void* dv, int64_t dv_ld, cudaStream_t s, const int32_t* kv_len = nullptr);
 
 // ---- conv front-end (audio_modalities.py:84-109) ----

@@ -248,6 +248,7 @@ struct Ctx {
   bool training;
   uint64_t seed;
   const uint64_t* seed_dev = nullptr;
+  KeyMask cross_mask = no_key_mask();     // decoder cross-attention: the wait-k lag of the batch (KeyMask, kernels.cuh)
   Arena ar;
   int adt;
   Ctx(const Model& mm, const Buffers& b, cudaStream_t s, bool d) : m(mm), buf(b), st(s), dry(d), training(false), seed(0), adt(mm.adt) {
@@ -416,10 +417,10 @@ static bool use_fused_attention(const Ctx& c, const AttnDims& a) {
   return is16(c.adt) && a.units / a.H == 64 && !c.m.cfg.disable_fused_attention;
 }
 
-static int attention_fwd(Ctx& c, const AttnDims& a, View q, View k, View v, const float* bias, int causal, DropoutSpec drop,
+static int attention_fwd(Ctx& c, const AttnDims& a, View q, View k, View v, const float* bias, KeyMask mask, DropoutSpec drop,
                          float* S, void* p_pre, void* p_drop, void* ctx, float* lse) {
   if (use_fused_attention(c, a)) {
-    RUN(attention_fwd_fused(c.adt, q.ptr, q.ld, k.ptr, k.ld, v.ptr, v.ld, a.B, a.H, a.Tq, a.Tk, bias, causal, drop, ctx, a.units, lse, c.st,
+    RUN(attention_fwd_fused(c.adt, q.ptr, q.ld, k.ptr, k.ld, v.ptr, v.ld, a.B, a.H, a.Tq, a.Tk, bias, mask, drop, ctx, a.units, lse, c.st,
                             c.klen_for(bias)));
     return 0;
   }
@@ -431,7 +432,7 @@ static int attention_fwd(Ctx& c, const AttnDims& a, View q, View k, View v, cons
   g.C = S; g.c_dtype = F32; g.ldc = Tkp; g.c_sb1 = (int64_t)a.Tq * Tkp; g.c_sb2 = (int64_t)a.H * a.Tq * Tkp;
   g.epi.alpha = 1.0f / sqrtf((float)dh);     // q * dh^-0.5 (multi_head_attention.py:203)
   RUN(gemm(g, c.st));
-  RUN(softmax_fwd(S, Tkp, bias, causal, p_pre, drop.p > 0.f ? p_drop : nullptr, c.adt, Tkp, a.B, a.H, a.Tq, a.Tk, drop, c.st));
+  RUN(softmax_fwd(S, Tkp, bias, mask, p_pre, drop.p > 0.f ? p_drop : nullptr, c.adt, Tkp, a.B, a.H, a.Tq, a.Tk, drop, c.st));
   GemmArgs o = gemm_defaults();
   o.M = a.Tq; o.N = dh; o.K = a.Tk; o.nb1 = a.H; o.nb2 = a.B;
   o.A = GemmOperand{drop.p > 0.f ? p_drop : p_pre, c.adt, 0, Tkp, (int64_t)a.Tq * Tkp, (int64_t)a.H * a.Tq * Tkp};
@@ -444,9 +445,9 @@ static int attention_fwd(Ctx& c, const AttnDims& a, View q, View k, View v, cons
 // dctx (act dtype) [B*Tq, units]  ->  dq, dk, dv views (act dtype)
 static int attention_bwd(Ctx& c, const AttnDims& a, View q, View k, View v, const void* p_pre, const void* p_drop,
                          DropoutSpec drop, const void* dctx, float* dP, void* dS, View dq, View dk, View dv, const void* ctx,
-                         const float* lse, const float* bias, int causal, float* dq32) {
+                         const float* lse, const float* bias, KeyMask mask, float* dq32) {
   if (use_fused_attention(c, a)) {
-    RUN(attention_bwd_fused(c.adt, q.ptr, q.ld, k.ptr, k.ld, v.ptr, v.ld, ctx, a.units, dctx, a.units, lse, a.B, a.H, a.Tq, a.Tk, bias, causal,
+    RUN(attention_bwd_fused(c.adt, q.ptr, q.ld, k.ptr, k.ld, v.ptr, v.ld, ctx, a.units, dctx, a.units, lse, a.B, a.H, a.Tq, a.Tk, bias, mask,
                             drop, dq32, dq.ptr, dq.ld, dk.ptr, dk.ld, dv.ptr, dv.ld, c.st, c.klen_for(bias)));
     return 0;
   }
@@ -498,7 +499,7 @@ struct AttnSave {
   void* p_pre = nullptr; void* p_drop = nullptr; void* ctx = nullptr;
   float* lse = nullptr;     // fused attention: per-row log-sum-exp [B,H,Tq]
   const void* mem = nullptr; // cross: memory in act dtype [Mk, d]
-  const float* bias = nullptr; int causal = 0;
+  const float* bias = nullptr; KeyMask mask = no_key_mask();
   AttnDims dims{};
   uint64_t s_attn = 0, s_post = 0;
 };
@@ -542,12 +543,12 @@ static int block_ln_bwd(Ctx& c, Scratch& sc, const float* dh, const float* x_in,
 
 // x_out = x_in + dropout(Attn(LN(x_in)))  — pre-norm block (common_layers.py:73-85)
 static int self_attn_block_fwd(Ctx& c, const std::string& pre, const float* x_in, float* x_out, int B, int T, const float* bias,
-                               int causal, Scratch& sc, AttnSave& sv) {
+                               KeyMask mask, Scratch& sc, AttnSave& sv) {
   const Config& cf = c.m.cfg;
   const int d = cf.d, M = B * T, Tkp = round8(T);
   sv.x_in = x_in;
   sv.dims = AttnDims{B, cf.heads, T, T, d};
-  sv.bias = bias; sv.causal = causal;
+  sv.bias = bias; sv.mask = mask;
   sv.s_attn = dropout_stream_id(pre + ".attn_drop"); sv.s_post = dropout_stream_id(pre + ".post_drop");
   sv.h = c.act((int64_t)M * d); sv.mean = c.f32(M); sv.rstd = c.f32(M);
   sv.qkv = c.act((int64_t)M * 3 * d);
@@ -564,7 +565,7 @@ static int self_attn_block_fwd(Ctx& c, const std::string& pre, const float* x_in
   GemmEpilogue e0 = gemm_defaults().epi;
   B200ST_TRY(linear_fwd(c, sv.h, d, M, d, 3 * d, pre + ".qkv.kernel", pre + ".qkv.bias", e0, sv.qkv, c.adt, 3 * d));
   View q{sv.qkv, 3 * d}, k{c.act_off(sv.qkv, d), 3 * d}, v{c.act_off(sv.qkv, 2 * d), 3 * d};
-  B200ST_TRY(attention_fwd(c, sv.dims, q, k, v, bias, causal, adrop, sc.S, sv.p_pre, sv.p_drop, sv.ctx, sv.lse));
+  B200ST_TRY(attention_fwd(c, sv.dims, q, k, v, bias, mask, adrop, sc.S, sv.p_pre, sv.p_drop, sv.ctx, sv.lse));
   GemmEpilogue e1 = gemm_defaults().epi;
   e1.drop = c.drop(cf.postprocess_dropout, sv.s_post, (int64_t)M * d);
   e1.residual = x_in; e1.res_ld = d;
@@ -585,7 +586,7 @@ static int self_attn_block_bwd(Ctx& c, const std::string& pre, const float* dx_o
   View q{sv.qkv, 3 * d}, k{c.act_off(sv.qkv, d), 3 * d}, v{c.act_off(sv.qkv, 2 * d), 3 * d};
   View dq{sc.dqkv, 3 * d}, dk{c.act_off(sc.dqkv, d), 3 * d}, dv{c.act_off(sc.dqkv, 2 * d), 3 * d};
   B200ST_TRY(attention_bwd(c, sv.dims, q, k, v, sv.p_pre, sv.p_drop, c.drop(cf.attention_dropout, sv.s_attn), sc.dctx, sc.S, sc.dS,
-                           dq, dk, dv, sv.ctx, sv.lse, sv.bias, sv.causal, sc.dq32));
+                           dq, dk, dv, sv.ctx, sv.lse, sv.bias, sv.mask, sc.dq32));
   B200ST_TRY(linear_wgrad(c, sv.h, d, sc.dqkv, 3 * d, M, d, 3 * d, pre + ".qkv.kernel", pre + ".qkv.bias"));
   B200ST_TRY(wb.flush());      // every dY of the block exists: the side stream starts under the rest of the chain
   B200ST_TRY(linear_dgrad(c, sc.dqkv, 3 * d, M, 3 * d, d, pre + ".qkv.kernel", e0, sc.dh, F32, d));
@@ -600,7 +601,7 @@ static int cross_attn_block_fwd(Ctx& c, const std::string& pre, const float* x_i
   const int d = cf.d, M = B * L, Mk = B * Tm, Tkp = round8(Tm);
   sv.x_in = x_in; sv.mem = mem;
   sv.dims = AttnDims{B, cf.heads, L, Tm, d};
-  sv.bias = mem_bias; sv.causal = 0;
+  sv.bias = mem_bias; sv.mask = c.cross_mask;
   sv.s_attn = dropout_stream_id(pre + ".attn_drop"); sv.s_post = dropout_stream_id(pre + ".post_drop");
   sv.h = c.act((int64_t)M * d); sv.mean = c.f32(M); sv.rstd = c.f32(M);
   sv.qkv = c.act((int64_t)M * d);
@@ -619,7 +620,7 @@ static int cross_attn_block_fwd(Ctx& c, const std::string& pre, const float* x_i
   B200ST_TRY(linear_fwd(c, sv.h, d, M, d, d, pre + ".q.kernel", pre + ".q.bias", e0, sv.qkv, c.adt, d));
   B200ST_TRY(linear_fwd(c, mem, d, Mk, d, 2 * d, pre + ".kv.kernel", pre + ".kv.bias", e0, sv.kv, c.adt, 2 * d));
   View q{sv.qkv, d}, k{sv.kv, 2 * d}, v{c.act_off(sv.kv, d), 2 * d};
-  B200ST_TRY(attention_fwd(c, sv.dims, q, k, v, mem_bias, 0, adrop, sc.S, sv.p_pre, sv.p_drop, sv.ctx, sv.lse));
+  B200ST_TRY(attention_fwd(c, sv.dims, q, k, v, mem_bias, sv.mask, adrop, sc.S, sv.p_pre, sv.p_drop, sv.ctx, sv.lse));
   GemmEpilogue e1 = gemm_defaults().epi;
   e1.drop = c.drop(cf.postprocess_dropout, sv.s_post, (int64_t)M * d);
   e1.residual = x_in; e1.res_ld = d;
@@ -641,7 +642,7 @@ static int cross_attn_block_bwd(Ctx& c, const std::string& pre, const float* dx_
   View q{sv.qkv, d}, k{sv.kv, 2 * d}, v{c.act_off(sv.kv, d), 2 * d};
   View dq{sc.dqkv, d}, dk{sc.dkv, 2 * d}, dv{c.act_off(sc.dkv, d), 2 * d};
   B200ST_TRY(attention_bwd(c, sv.dims, q, k, v, sv.p_pre, sv.p_drop, c.drop(cf.attention_dropout, sv.s_attn), sc.dctx, sc.S, sc.dS,
-                           dq, dk, dv, sv.ctx, sv.lse, sv.bias, 0, sc.dq32));
+                           dq, dk, dv, sv.ctx, sv.lse, sv.bias, sv.mask, sc.dq32));
   B200ST_TRY(linear_wgrad(c, sv.h, d, sc.dqkv, d, M, d, d, pre + ".q.kernel", pre + ".q.bias"));
   B200ST_TRY(linear_wgrad(c, sv.mem, d, sc.dkv, 2 * d, Mk, d, 2 * d, pre + ".kv.kernel", pre + ".kv.bias"));
   B200ST_TRY(wb.flush());
@@ -759,10 +760,12 @@ static int encoder_fwd(Ctx& c, const float* x0, const float* bias, int B, int T,
   sv.B = B; sv.T = T;
   sv.att.resize(cf.enc_layers); sv.ffn.resize(cf.enc_layers);
   const float* x = x0;
+  // monotonic encoder (transformer_encoder.py:119-123): query i sees the non-padded keys j <= i
+  const KeyMask mask = cf.encoder_monotonic ? causal_mask(T, T) : no_key_mask();
   for (int i = 0; i < cf.enc_layers; ++i) {
     const std::string p = "enc." + std::to_string(i);
     float* x1 = c.f32((int64_t)M * d);
-    B200ST_TRY(self_attn_block_fwd(c, p + ".att", x, x1, B, T, bias, 0, sc, sv.att[i]));
+    B200ST_TRY(self_attn_block_fwd(c, p + ".att", x, x1, B, T, bias, mask, sc, sv.att[i]));
     float* x2 = c.f32((int64_t)M * d);
     B200ST_TRY(ffn_block_fwd(c, p + ".ffn", x1, x2, M, sv.ffn[i]));
     x = x2;
@@ -813,7 +816,7 @@ static int decoder_fwd(Ctx& c, const float* x0, int B, int L, const void* mem, i
   for (int i = 0; i < cf.dec_layers; ++i) {
     const std::string p = "dec." + std::to_string(i);
     float* x1 = c.f32((int64_t)M * d);
-    B200ST_TRY(self_attn_block_fwd(c, p + ".self", x, x1, B, L, nullptr, 1, sc, sv.self[i]));
+    B200ST_TRY(self_attn_block_fwd(c, p + ".self", x, x1, B, L, nullptr, causal_mask(L, L), sc, sv.self[i]));
     x = x1;
     if (cf.with_cross_attention && mem) {
       float* x2 = c.f32((int64_t)M * d);
@@ -978,6 +981,12 @@ static int model_run(Ctx& c, const Batch& b, bool backward) {
   c.training = b.training != 0;
   c.seed = b.seed;
   c.seed_dev = b.seed_dev;
+  B200ST_CHECK(b.wait_k >= 0, "wait_k must be >= 0 (0: no lag), got " + std::to_string(b.wait_k));
+  if (b.wait_k > 0 || b.wait_k_dev) {
+    B200ST_CHECK(cf.with_cross_attention, "wait_k needs a decoder with cross-attention");
+    // wait-k (transformer_decoder.py:194-208): target position i sees memory keys j < i + k
+    c.cross_mask = KeyMask{1, b.wait_k - 1, b.wait_k_dev};
+  }
   if (backward) B200ST_CHECK(c.buf.grads != nullptr && b.trg != nullptr && b.trg_length != nullptr, "backward needs grads and targets");
   if (is16(c.adt)) B200ST_CHECK(c.buf.shadow != nullptr, "16-bit precision needs the 16-bit shadow arena");
 
@@ -1237,7 +1246,7 @@ int mha_api_body(Ctx& c, const float* query, const float* memory, const float* b
     void* qkv = c.act(Mq * 3 * u);
     B200ST_TRY(linear_fwd(c, qin, cf.mha_din, (int)Mq, cf.mha_din, 3 * u, "att.qkv.kernel", "att.qkv.bias", e0, qkv, c.adt, 3 * u));
     View q{qkv, 3 * u}, k{c.act_off(qkv, u), 3 * u}, v{c.act_off(qkv, 2 * u), 3 * u};
-    B200ST_TRY(attention_fwd(c, dims, q, k, v, bias, 0, no_dropout(), S, p_pre, nullptr, ctx, lse));
+    B200ST_TRY(attention_fwd(c, dims, q, k, v, bias, no_key_mask(), no_dropout(), S, p_pre, nullptr, ctx, lse));
   } else {
     void* min = c.act(Mk * cf.mha_dmem);
     RUN(cast_dropout(memory, min, c.adt, Mk * cf.mha_dmem, no_dropout(), c.st));
@@ -1246,7 +1255,7 @@ int mha_api_body(Ctx& c, const float* query, const float* memory, const float* b
     B200ST_TRY(linear_fwd(c, qin, cf.mha_din, (int)Mq, cf.mha_din, u, "att.q.kernel", "att.q.bias", e0, qb, c.adt, u));
     B200ST_TRY(linear_fwd(c, min, cf.mha_dmem, (int)Mk, cf.mha_dmem, 2 * u, "att.kv.kernel", "att.kv.bias", e0, kv, c.adt, 2 * u));
     View q{qb, u}, k{kv, 2 * u}, v{c.act_off(kv, u), 2 * u};
-    B200ST_TRY(attention_fwd(c, dims, q, k, v, bias, 0, no_dropout(), S, p_pre, nullptr, ctx, lse));
+    B200ST_TRY(attention_fwd(c, dims, q, k, v, bias, no_key_mask(), no_dropout(), S, p_pre, nullptr, ctx, lse));
   }
   return linear_fwd(c, ctx, u, (int)Mq, u, cf.mha_dout, "att.out.kernel", "att.out.bias", e0, out, F32, cf.mha_dout);
 }

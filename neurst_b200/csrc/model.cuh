@@ -25,6 +25,7 @@ struct Config {
   int with_cross_attention;   // decoder stack: 1 (default)
   int disable_fused_attention; // tests: use the materialised (GEMM + softmax) attention path in bf16 mode
   int deterministic;           // fused FFN: slices reduce in slice order (bit-reproducible)
+  int encoder_monotonic;       // MODEL_TEXT: causal encoder self-attention (transformer_encoder.py:119-123)
 };
 
 struct ParamInfo {
@@ -87,6 +88,8 @@ struct Batch {
   const uint64_t* seed_dev;            // optional: device-resident seed (overrides `seed`)
   float loss_scale;                    // multiplies dlogits (1/world for DP mean, gradient-accumulation factor, ...)
   const float* loss_scale_dev;         // optional device word multiplied in as well (dynamic loss scale of the fp16 mode)
+  int wait_k;                          // decoder cross-attention lag k (0: none): target i sees memory keys j < i + k
+  const int32_t* wait_k_dev;           // optional device-resident lag, read at kernel run time (overrides wait_k)
   // outputs (device, optional)
   float* logits;                       // fp32 [B,L,V]
   float* loss;                         // [1]
@@ -121,6 +124,7 @@ struct DecodeState {
   const float* memory_bias;      // [B, Tm] additive (0 / -1e9) or null
   float* scratch;                // decode_scratch_floats(B) floats
   int use_shadow;                // 0: fp32 master weights, 1: the handle's 16-bit shadow
+  int wait_k;                    // wait-k lag (0: none): step t attends to the memory keys j < min(Tm, wait_k + t)
 };
 struct GreedyArgs {
   const int64_t* bos_ids;        // [B] device: first decoder input (generation_initializer["decoder_input"])

@@ -31,9 +31,12 @@ class DecodingCache:
     """`cache` argument of symbols_to_logits_fn: encoder memory (pre-projected per layer) + self-attention K/V.
 
     beam > 1 (beam search): the memory stays one copy per utterance, the self-attention cache and the step scratch hold
-    B * beam rows: at most MAX_ROWS with the fp32 weights, MAX_ROWS_SHADOW with use_shadow."""
+    B * beam rows: at most MAX_ROWS with the fp32 weights, MAX_ROWS_SHADOW with use_shadow.
 
-    def __init__(self, rt, B, Tm, max_len, memory_bias, use_shadow=False, beam=1):
+    wait_k > 0 (a WaitkTransformer): step t attends to the memory keys j < min(Tm, wait_k + t), the offline form of the
+    streaming wait-k agent (waitk_transformer.py:102-110); 0 attends to the whole memory."""
+
+    def __init__(self, rt, B, Tm, max_len, memory_bias, use_shadow=False, beam=1, wait_k=0):
         cfg = rt.config
         limit = max_rows(use_shadow)
         if beam < 1 or not 1 <= B * beam <= limit:
@@ -53,6 +56,7 @@ class DecodingCache:
         st.memory_bias = memory_bias.data_ptr() if memory_bias is not None else None
         st.scratch = self.scratch.data_ptr()
         st.use_shadow = int(bool(use_shadow))
+        st.wait_k = int(wait_k)
         self.state = st
 
     # reference-shaped view of the cache (transformer_decoder.py:119-147) for inspection / tests
@@ -106,10 +110,11 @@ def encode(rt, inputs):
     return enc, bias
 
 
-def create_decoding_cache(rt, encoder_outputs, memory_bias, max_len, use_shadow=False, beam=1):
+def create_decoding_cache(rt, encoder_outputs, memory_bias, max_len, use_shadow=False, beam=1, wait_k=0):
     """create_decoding_internal_cache(is_inference=True) + memorize_memory for every layer."""
     B, Tm, _ = encoder_outputs.shape
-    cache = DecodingCache(rt, B, Tm, max_len, memory_bias.contiguous() if memory_bias is not None else None, use_shadow, beam)
+    cache = DecodingCache(rt, B, Tm, max_len, memory_bias.contiguous() if memory_bias is not None else None, use_shadow, beam,
+                          wait_k)
     bufs = _bufs(rt)
     enc = encoder_outputs.to(torch.float32).contiguous()
     L.check(rt.lib.b200st_decode_init(rt.handle, C.byref(bufs), enc.data_ptr(), C.byref(cache.state), L._stream()))
@@ -131,13 +136,14 @@ def decoder_step_logits(rt, symbols, cache, time):
 
 
 def greedy_search(rt, inputs, bos_id, eos_id, unk_id=None, maximum_decode_length=256, extra_decode_length=50,
-                  minimum_decode_length=0, enable_unk=False, use_shadow=False, use_graph=True, cache=None, persistent=True):
+                  minimum_decode_length=0, enable_unk=False, use_shadow=False, use_graph=True, cache=None, persistent=True,
+                  wait_k=0):
     """sequence_beam_search(beam_size=1, top_k=1): returns (hypothesis int64 [B, maximum_decode_length] padded with EOS,
     log-probability [B], decoding length [B]).  `maximum_search_steps` = max(min(T' + extra, maximum), minimum)
     (beam_search.py:357-363)."""
     if cache is None:
         enc, bias = encode(rt, inputs)
-        cache = create_decoding_cache(rt, enc, bias, maximum_decode_length, use_shadow)
+        cache = create_decoding_cache(rt, enc, bias, maximum_decode_length, use_shadow, wait_k=wait_k)
     B, Tm = cache.B, cache.Tm
     steps = max(min(Tm + extra_decode_length, maximum_decode_length), minimum_decode_length)
     steps = min(steps, cache.max_len)
@@ -185,7 +191,8 @@ def _search_steps(Tm, maximum_decode_length, extra_decode_length, minimum_decode
 
 
 def beam_search(rt, inputs, bos_id, eos_id, unk_id=None, beam_size=4, length_penalty=0.6, top_k=1, maximum_decode_length=256,
-                extra_decode_length=50, minimum_decode_length=0, enable_unk=False, use_shadow=False, use_graph=True, cache=None):
+                extra_decode_length=50, minimum_decode_length=0, enable_unk=False, use_shadow=False, use_graph=True, cache=None,
+                wait_k=0):
     """sequence_beam_search (beam_search.py:254-439) on the device: returns (hypotheses int64 [B*top_k, maximum_decode_length]
     padded with EOS, scores fp32 [B*top_k] = logprob * length penalty, best first per utterance, accumulated log-probabilities
     [B*top_k], decoding lengths [B*top_k]).  length_penalty < 0 (or None) scores by 1/length.  At most
@@ -204,7 +211,7 @@ def beam_search(rt, inputs, bos_id, eos_id, unk_id=None, beam_size=4, length_pen
             raise L.B200STError("beam search decodes at most %d rows (utterances x beam_size) per call, got %d x %d"
                                 % (max_rows(use_shadow), B, beam_size))
         enc, bias = encode(rt, inputs)
-        cache = create_decoding_cache(rt, enc, bias, maximum_decode_length, use_shadow, beam=beam_size)
+        cache = create_decoding_cache(rt, enc, bias, maximum_decode_length, use_shadow, beam=beam_size, wait_k=wait_k)
     elif cache.self_kv.shape[2] < cache.B * beam_size:
         raise L.B200STError("the decoding cache holds %d rows, beam search needs %d" % (cache.self_kv.shape[2], cache.B * beam_size))
     B, Tm = cache.B, cache.Tm
@@ -358,7 +365,7 @@ def _check_sampling_filter(top_k, top_p):
 
 def sampling_search(rt, inputs, bos_id, eos_id, unk_id, sample_num=1, top_k=0, top_p=1.0, maximum_decode_length=256,
                     extra_decode_length=50, minimum_decode_length=0, seed=DEFAULT_SAMPLING_SEED, row_offset=0, use_shadow=False,
-                    use_graph=True, cache=None):
+                    use_graph=True, cache=None, wait_k=0):
     """sequence_sampling_search of TopSampling (neurst/layers/search/sampling.py:103-250) on the device: each utterance is
     decoded `sample_num` times (row b * sample_num + s is sample s of utterance b), every step masks UNK (unk_id None: not
     masked) and, before minimum_decode_length, EOS; keeps the top_k logits (top_k > 0) or the nucleus of mass top_p
@@ -378,7 +385,7 @@ def sampling_search(rt, inputs, bos_id, eos_id, unk_id, sample_num=1, top_k=0, t
             raise L.B200STError("sampling search decodes at most %d rows (utterances x sample_num) per call, got %d x %d"
                                 % (max_rows(use_shadow), B, sample_num))
         enc, bias = encode(rt, inputs)
-        cache = create_decoding_cache(rt, enc, bias, maximum_decode_length, use_shadow, beam=sample_num)
+        cache = create_decoding_cache(rt, enc, bias, maximum_decode_length, use_shadow, beam=sample_num, wait_k=wait_k)
     elif cache.self_kv.shape[2] < cache.B * sample_num:
         raise L.B200STError("the decoding cache holds %d rows, sampling needs %d" % (cache.self_kv.shape[2], cache.B * sample_num))
     B, Tm = cache.B, cache.Tm

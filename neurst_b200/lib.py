@@ -161,7 +161,8 @@ class Config(C.Structure):
                 ("postprocess_dropout", C.c_float), ("label_smoothing", C.c_float),
                 ("share_src_trg_embedding", C.c_int32),
                 ("mha_self", C.c_int32), ("mha_din", C.c_int32), ("mha_dmem", C.c_int32), ("mha_dout", C.c_int32),
-                ("with_cross_attention", C.c_int32), ("disable_fused_attention", C.c_int32), ("deterministic", C.c_int32)]
+                ("with_cross_attention", C.c_int32), ("disable_fused_attention", C.c_int32), ("deterministic", C.c_int32),
+                ("encoder_monotonic", C.c_int32)]
 
 
 class Buffers(C.Structure):
@@ -175,7 +176,7 @@ class Batch(C.Structure):
                 ("B", C.c_int32), ("T", C.c_int32), ("L", C.c_int32), ("training", C.c_int32),
                 ("seed", C.c_uint64), ("seed_dev", C.c_void_p), ("loss_scale", C.c_float), ("loss_scale_dev", C.c_void_p),
                 ("logits", C.c_void_p), ("loss", C.c_void_p), ("nll_sum", C.c_void_p), ("n_tokens", C.c_void_p),
-                ("enc_out", C.c_void_p)]
+                ("enc_out", C.c_void_p), ("wait_k", C.c_int32), ("wait_k_dev", C.c_void_p)]
 
 
 class OptimArgs(C.Structure):
@@ -195,7 +196,7 @@ class StepOpts(C.Structure):
 class DecodeState(C.Structure):
     _fields_ = [("B", C.c_int32), ("Tm", C.c_int32), ("max_len", C.c_int32),
                 ("cross_kv", C.c_void_p), ("self_kv", C.c_void_p), ("memory_bias", C.c_void_p), ("scratch", C.c_void_p),
-                ("use_shadow", C.c_int32)]
+                ("use_shadow", C.c_int32), ("wait_k", C.c_int32)]
 
 
 class GreedyArgs(C.Structure):

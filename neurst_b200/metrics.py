@@ -254,3 +254,45 @@ def build_metric(name, language="en"):
     m = Wer(language) if check_metric_name(name) == "wer" else BLEU(language)
     m.flag = str(name)
     return m
+
+
+# ------------------------------------------------------------------------------------------------ simultaneous latency
+# Latency of the offline wait-k schedule with SimulEval's definitions (AverageLagging, AverageProportion,
+# DifferentiableAverageLagging).  Units are model (BPE) tokens: |x| is the source without its EOS, |y| the hypothesis
+# without its EOS, and target token i (1-based) is written after g(i) = min(k + i - 1, |x|) source tokens.  SimulEval
+# reports detokenised words, so these numbers are not comparable with published word-level tables.
+def waitk_delays(k, src_len, hyp_len):
+    """g(i) = min(k + i - 1, |x|) for i = 1..|y|."""
+    return [min(int(k) + i - 1, int(src_len)) for i in range(1, int(hyp_len) + 1)]
+
+
+def simul_latency(delays, src_len):
+    """{"AL", "AP", "DAL"} of one sentence from its delays g(1..|y|) and |x|; None when either side is empty.
+      AL  = (1/tau) sum_{i<=tau} (g(i) - (i-1)|x|/|y|), tau the first i with g(i) = |x| (|y| when none)
+      AP  = sum_i g(i) / (|x||y|)
+      DAL = (1/|y|) sum_i (g'(i) - (i-1)|x|/|y|), g'(1) = g(1), g'(i) = max(g(i), g'(i-1) + |x|/|y|)"""
+    x, y = int(src_len), len(delays)
+    if x < 1 or y < 1:
+        return None
+    step = x / y
+    tau = next((i + 1 for i, g in enumerate(delays) if g >= x), y)
+    al = sum(delays[i] - i * step for i in range(tau)) / tau
+    ap = sum(delays) / (x * y)
+    dal, prev = 0.0, None
+    for i, g in enumerate(delays):
+        prev = g if prev is None else max(g, prev + step)
+        dal += prev - i * step
+    return {"AL": al, "AP": ap, "DAL": dal / y}
+
+
+def waitk_latency(k, src_len, hyp_len):
+    """simul_latency of the wait-k schedule (k source tokens read before the first target token, then one per token)."""
+    return simul_latency(waitk_delays(k, src_len, hyp_len), src_len)
+
+
+def corpus_waitk_latency(k, lengths):
+    """Means of AL / AP / DAL over (|x|, |y|) pairs, skipping sentences with an empty side; None when none is left."""
+    rows = [r for r in (waitk_latency(k, x, y) for x, y in lengths) if r is not None]
+    if not rows:
+        return None
+    return {m: sum(r[m] for r in rows) / len(rows) for m in ("AL", "AP", "DAL")}

@@ -2,6 +2,7 @@
 
   SpeechTransformer          neurst/models/speech_transformer.py:27-280  (PT twin neurst_pt/models/speech_transformer.py)
   Transformer                neurst/models/transformer.py:27-260         (cfg-1 plumbing model)
+  WaitkTransformer           neurst/models/waitk_transformer.py:23-144   (simultaneous translation, offline wait-k)
   EncoderDecoderEnsembleModel  neurst/models/encoder_decoder_ensemble_model.py  (generation only)
   LabelSmoothedCrossEntropy  neurst/criterions/label_smoothed_cross_entropy.py:26-157
 
@@ -83,6 +84,34 @@ def transformer_hparams(name):
     }
 
 
+def waitk_transformer_hparams(name):
+    """neurst/models/waitk_transformer.py:75-84: `waitk_transformer_<name>` and `waitktransformer_<name>` are the Transformer
+    preset `<name>` with model.class WaitkTransformer and a monotonic encoder; None for other names."""
+    name = str(name)
+    args = None
+    if name.startswith("waitk_transformer_"):
+        args = transformer_hparams(name[6:])
+    elif name.startswith("waitktransformer_"):
+        args = transformer_hparams(name[5:])
+    if args is not None:
+        args["model.class"] = "WaitkTransformer"
+        args["model.params"]["encoder.attention_monotonic"] = True
+    return args
+
+
+def parse_wait_k(value):
+    """WaitkTranslation's `wait_k` (waitk_translation.py:23-31): an int, a list of ints, or a YAML string of either."""
+    import yaml
+    k = yaml.safe_load(value) if isinstance(value, str) else value
+    if isinstance(k, bool) or not (isinstance(k, int) or (isinstance(k, (list, tuple)) and k)):
+        raise ValueError("wait_k must be an int or a non-empty list of ints, got %r" % (value,))
+    ks = list(k) if isinstance(k, (list, tuple)) else [k]
+    for x in ks:
+        if isinstance(x, bool) or not isinstance(x, int) or x < 1:
+            raise ValueError("wait_k must be >= 1 (a lag of k source tokens), got %r" % (value,))
+    return ks if isinstance(k, (list, tuple)) else k
+
+
 def _model_flags(speech):
     """(name, python type, default, help) of every `model.params` key — the flag list of the reference's
     `class_or_method_args()` (neurst_pt/models/speech_transformer.py:35-106, neurst/models/transformer.py:45-120):
@@ -102,7 +131,9 @@ def _model_flags(speech):
                ("modality.source.layer_norm", bool, False, "Whether to apply layer norm in convolution layers.")]
     else:
         fl += [("modality.share_source_target_embedding", bool, False,
-                "Whether to share source and target embedding table.")]
+                "Whether to share source and target embedding table."),
+               ("encoder.attention_monotonic", bool, False,
+                "Whether to apply a triangle mask to make the encoder self-attention monotonic (causal).")]
     for side in ("encoder", "decoder"):
         fl += [(side + ".num_layers", int, None, "The number of stacking layers of the %s." % side),
                (side + ".hidden_size", int, None, "The number of hidden units of the %s." % side),
@@ -157,6 +188,11 @@ class _EncoderDecoder:
 
     args = property(lambda self: self._args)
     runtime = property(lambda self: self._rt)
+    wait_k = None           # the WaitkTransformer's lag (an int or a list); None: no lag
+
+    def lag(self, is_training):
+        """The cross-attention lag of one call (0: none); see WaitkTransformer.lag."""
+        return 0
 
     def named_parameters(self):
         return self._rt.named_parameters()
@@ -189,6 +225,8 @@ class _EncoderDecoder:
             b["trg_length"] = (1.0 - torch.as_tensor(b["trg_padding"]).float()).sum(-1).long()
         self._step_seed += 1
         b.update(training=bool(is_training), seed=b.get("seed", self._step_seed))
+        if "wait_k" not in b:
+            b["wait_k"] = self.lag(is_training)
         b.update(extra)
         return b
 
@@ -226,7 +264,8 @@ class _EncoderDecoder:
         rt = self._rt
         enc, bias = D.encode(rt, inputs)
         max_len = int(decode_padded_length or self._args.get("maximum_decode_length", 256))
-        cache = D.create_decoding_cache(rt, enc, bias, max_len, use_shadow=bool(self._args.get("decode_with_shadow", False)))
+        cache = D.create_decoding_cache(rt, enc, bias, max_len, use_shadow=bool(self._args.get("decode_with_shadow", False)),
+                                        wait_k=self.lag(False))
 
         def symbols_to_logits_fn(symbols, cache, time=None):
             return D.decoder_step_logits(rt, symbols, cache, 0 if time is None else int(time))
@@ -247,7 +286,7 @@ class _EncoderDecoder:
         if bos is None:
             bos = torch.full((B,), int(tm["bos_id"]), dtype=torch.long)
         ids, logprob, _ = D.greedy_search(self._rt, inputs, bos, tm["eos_id"], tm.get("unk_id"), maximum_decode_length,
-                                          extra_decode_length, minimum_decode_length, enable_unk, use_shadow)
+                                          extra_decode_length, minimum_decode_length, enable_unk, use_shadow, wait_k=self.lag(False))
         return ids, logprob
 
     def beam_search(self, inputs, beam_size=4, length_penalty=0.6, top_k=1, maximum_decode_length=256, extra_decode_length=50,
@@ -263,7 +302,8 @@ class _EncoderDecoder:
         if bos is None:
             bos = torch.full((B,), int(tm["bos_id"]), dtype=torch.long)
         ids, scores, _, _ = D.beam_search(self._rt, inputs, bos, tm["eos_id"], tm.get("unk_id"), beam_size, length_penalty, top_k,
-                                          maximum_decode_length, extra_decode_length, minimum_decode_length, enable_unk, use_shadow)
+                                          maximum_decode_length, extra_decode_length, minimum_decode_length, enable_unk, use_shadow,
+                                          wait_k=self.lag(False))
         return ids, scores
 
     def sampling_search(self, inputs, sample_num=1, top_k=0, top_p=1.0, maximum_decode_length=256, extra_decode_length=50,
@@ -281,7 +321,7 @@ class _EncoderDecoder:
             bos = torch.full((B,), int(tm["bos_id"]), dtype=torch.long)
         ids, logprob, _ = D.sampling_search(self._rt, inputs, bos, tm["eos_id"], tm.get("unk_id"), sample_num, top_k, top_p,
                                             maximum_decode_length, extra_decode_length, minimum_decode_length, seed, row_offset,
-                                            use_shadow)
+                                            use_shadow, wait_k=self.lag(False))
         return ids, logprob
 
     def evaluate(self, inputs, is_training=False):
@@ -346,8 +386,41 @@ class Transformer(_EncoderDecoder):
             precision=precision, ln_eps=args.get("encoder.layer_postprocess_epsilon", 1e-6),
             attention_dropout=args.get("encoder.attention_dropout_rate", 0.), ffn_dropout=args.get("encoder.ffn_dropout_rate", 0.),
             postprocess_dropout=args.get("encoder.layer_postprocess_dropout_rate", 0.), label_smoothing=label_smoothing,
-            share_src_trg_embedding=share)
+            share_src_trg_embedding=share, encoder_monotonic=bool(args.get("encoder.attention_monotonic", False)))
         return cls(args, src_meta, trg_meta, Runtime(cfg, device))
+
+
+class WaitkTransformer(Transformer):
+    """ neurst/models/waitk_transformer.py: a Transformer (same variables) whose decoder cross-attention lags the source by
+    `wait_k` tokens: target position i sees the source keys j < i + k (transformer_decoder.py:194-208).  Its presets also make
+    the encoder monotonic, so that encoding the whole source once equals the streaming agent's incremental encoding. """
+
+    @classmethod
+    def build_model_args_by_name(cls, name):
+        return waitk_transformer_hparams(name)
+
+    @classmethod
+    def new(cls, args, src_meta, trg_meta, name=None, precision="fp32", label_smoothing=0.0, device="cuda", wait_k=None,
+            random_seed=0):
+        """wait_k: the task's lag (an int, a list, or a YAML string of either).  random_seed seeds the multi-path draw."""
+        if wait_k is None:
+            raise ValueError("WaitkTransformer needs wait_k (the decode lagging)")
+        model = super(WaitkTransformer, cls).new(args, src_meta, trg_meta, name=name, precision=precision,
+                                                 label_smoothing=label_smoothing, device=device)
+        model.wait_k = parse_wait_k(wait_k)
+        model._lag_gen = torch.Generator().manual_seed(int(random_seed))
+        return model
+
+    def lag(self, is_training):
+        """waitk_transformer.py:102-110: training with a list draws one k uniformly per call (multi-path); otherwise the first
+        k of the list.  The draw comes from a generator seeded by the run's random_seed, so that every replica draws the same
+        k at the same step (the reference draws with an unseeded tf.random.uniform on each replica)."""
+        ks = self.wait_k
+        if not isinstance(ks, list):
+            return int(ks)
+        if is_training and len(ks) > 1:
+            return int(ks[int(torch.randint(len(ks), (1,), generator=self._lag_gen))])
+        return int(ks[0])
 
 
 class EncoderDecoderEnsembleModel:

@@ -20,7 +20,8 @@ _TORCH16 = {L.BF16: torch.bfloat16, L.F16: torch.float16}
 def make_config(model_type, d, heads, ffn=0, enc_layers=0, dec_layers=0, vocab=0, src_vocab=0, feat=80, in_channels=1,
                 channels=0, conv_layer_norm=True, precision="bf16", ln_eps=1e-6, attention_dropout=0.0, ffn_dropout=0.0,
                 postprocess_dropout=0.0, label_smoothing=0.0, share_src_trg_embedding=False, mha_self=False, mha_din=0,
-                mha_dmem=0, mha_dout=0, with_cross_attention=True, disable_fused_attention=False, deterministic=False):
+                mha_dmem=0, mha_dout=0, with_cross_attention=True, disable_fused_attention=False, deterministic=False,
+                encoder_monotonic=False):
     c = L.Config()
     c.model_type = model_type
     c.d, c.heads, c.ffn, c.enc_layers, c.dec_layers = d, heads, ffn, enc_layers, dec_layers
@@ -35,6 +36,7 @@ def make_config(model_type, d, heads, ffn=0, enc_layers=0, dec_layers=0, vocab=0
     c.with_cross_attention = int(with_cross_attention)
     c.disable_fused_attention = int(disable_fused_attention)
     c.deterministic = int(deterministic)
+    c.encoder_monotonic = int(encoder_monotonic)
     return c
 
 
@@ -204,6 +206,7 @@ class Runtime:
         bt.training = int(batch.get("training", backward))
         bt.seed = int(batch.get("seed", 0))
         bt.loss_scale = float(batch.get("loss_scale", 1.0))
+        bt.wait_k = int(batch.get("wait_k", 0))
         if backward and self.fp16 and batch.get("dynamic_loss_scale", True):
             bt.loss_scale_dev = self.loss_scale_state.data_ptr()       # gradients come out multiplied by state[0]
         out = {}
@@ -278,9 +281,10 @@ class GraphedTrainStep:
 
     All launches of the step (~1800 kernels) are replayed from one graph; inputs live in static device buffers that
     `__call__` refreshes, and the dropout seed is read by the kernels from a device word (`seed_dev`), so every replay
-    draws fresh masks.  Gradients accumulate into the runtime's gradient arena exactly as in the eager path."""
+    draws fresh masks.  The wait-k lag of a wait-k model's cross-attention (`wait_k=True`) is a device word too (`wait_k_dev`), so a
+    multi-path model draws a fresh k per step and replays the same graph; other models capture no lag at all.  Gradients accumulate into the runtime's gradient arena exactly as in the eager path."""
 
-    def __init__(self, rt, B, T, Lq, allreduce=False):
+    def __init__(self, rt, B, T, Lq, allreduce=False, wait_k=False):
         self.allreduce = bool(allreduce)
         cfg = rt.config
         if cfg.model_type not in (L.MODEL_SPEECH, L.MODEL_TEXT):
@@ -298,6 +302,7 @@ class GraphedTrainStep:
         self.trg = torch.zeros(B, Lq, dtype=torch.int64, device=dev)
         self.trg_length = torch.ones(B, dtype=torch.int64, device=dev)
         self.seed = torch.zeros(1, dtype=torch.int64, device=dev)
+        self.wait_k = torch.zeros(1, dtype=torch.int32, device=dev) if wait_k else None
         self.loss = torch.zeros(1, dtype=torch.float32, device=dev)
         self.nll_sum = torch.zeros(B, dtype=torch.float32, device=dev)
         self.n_tokens = torch.zeros(B, dtype=torch.float32, device=dev)
@@ -315,6 +320,8 @@ class GraphedTrainStep:
         bt.trg_input, bt.trg, bt.trg_length = self.trg_input.data_ptr(), self.trg.data_ptr(), self.trg_length.data_ptr()
         bt.B, bt.T, bt.L, bt.training = B, T, Lq, 1
         bt.seed, bt.seed_dev, bt.loss_scale = 0, self.seed.data_ptr(), 1.0
+        if wait_k:
+            bt.wait_k_dev = self.wait_k.data_ptr()
         if rt.fp16:
             bt.loss_scale_dev = rt.loss_scale_state.data_ptr()
         bt.loss, bt.nll_sum, bt.n_tokens = self.loss.data_ptr(), self.nll_sum.data_ptr(), self.n_tokens.data_ptr()
@@ -351,7 +358,7 @@ class GraphedTrainStep:
         self.graph = g
         return self
 
-    def __call__(self, batch, seed):
+    def __call__(self, batch, seed, wait_k=0):
         if self.graph is None:
             self.capture()
         if self.rt._shadow_stale:
@@ -365,6 +372,10 @@ class GraphedTrainStep:
         self.trg.copy_(batch["trg"], non_blocking=True)
         self.trg_length.copy_(batch["trg_length"], non_blocking=True)
         self.seed.fill_(int(seed))
+        if self.wait_k is not None:
+            self.wait_k.fill_(int(wait_k))
+        elif wait_k:
+            raise L.B200STError("this GraphedTrainStep was captured without a wait-k lag (wait_k=False)")
         self.graph.replay()
         # fresh tensors, as the eager path returns: the persistent outputs are overwritten by the next replay
         return {"loss": self.loss.clone(), "nll_sum": self.nll_sum.clone(), "n_tokens": self.n_tokens.clone()}

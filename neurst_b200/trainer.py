@@ -109,13 +109,16 @@ class DataParallelTrainer:
             b["seed"] = int(seed) * self.world + self.rank
         last_micro = (self._micro + 1) % self.update_cycle == 0
         sync_now = self.lib_comm and last_micro          # gradients are all-reduced by the step that completes a cycle
+        waitk = getattr(self.model, "wait_k", None) is not None
+        if waitk:
+            b["wait_k"] = self.model.lag(True)           # the wait-k model's lag of this micro-batch (one draw per call)
         if self.use_cuda_graph:
             from neurst_b200.runtime import GraphedTrainStep
             key = (b["src"].shape[0], b["src"].shape[1], b["trg_input"].shape[1], sync_now)   # one graph per shape bucket
             if key not in self._graphs:
-                self._graphs[key] = GraphedTrainStep(self.rt, *key[:3], allreduce=sync_now).capture()
+                self._graphs[key] = GraphedTrainStep(self.rt, *key[:3], allreduce=sync_now, wait_k=waitk).capture()
             self._seed_ctr = getattr(self, "_seed_ctr", 0) + 1
-            out = self._graphs[key](b, b.get("seed", self._seed_ctr * self.world + self.rank))
+            out = self._graphs[key](b, b.get("seed", self._seed_ctr * self.world + self.rank), wait_k=b.get("wait_k", 0))
         else:
             if sync_now:
                 b["allreduce"] = True

@@ -222,13 +222,13 @@ class Validator:
 
     def _text_loss_sums(self, mine, crit):
         """_loss_sums of the text model: EVAL-mode padded_batch (seq2seq.py:236-244, padded to the longest source and
-        target of the batch)."""
+        target of the batch).  A wait-k model is evaluated with its first lag (waitk_transformer.py:106-107)."""
         rt = self.model.runtime
         out = []
         for bi, group in mine:
             b = {k: v.to(rt.device) for k, v in self.task.group_to_input(group, infer=False).items()}
             logits = rt.run({"src": b["src"], "src_padding": b["src_padding"], "trg_input": b["trg_input"], "training": False,
-                             "seed": 0, "want_logits": True}, backward=False)["logits"]
+                             "seed": 0, "want_logits": True, "wait_k": self.model.lag(False)}, backward=False)["logits"]
             nll, _, ntok = crit(b, logits)
             out.append((bi, float(nll.double().sum()), float(len(group)), float(ntok.double().sum())))
         return out
