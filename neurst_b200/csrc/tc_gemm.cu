@@ -435,7 +435,7 @@ __global__ void __launch_bounds__(kThreads, 1) tc_wgrad_group_kernel(const __gri
 // registers (GEMM1), get bias, ReLU and dropout there, are written to HBM only because the backward pass needs them, and
 // go, packed to 16 bits, straight back into the tensor cores as the register A operand of GEMM2, which accumulates the
 // [64 x D] output rows in registers across all halves.  Only the weights stream (L2 -> smem), and the [M, ffn] hidden
-// tensor is never read back.  Slices of the hidden dimension reduce into x_out with fp32 atomics (dropout is a mask: linear).
+// tensor is never read back.  Slices of the hidden dimension reduce into x_out with fp32 bulk reductions (dropout is a mask: linear).
 //   256 threads = the two consumer warpgroups and nothing else: a CTA of at most two warpgroups is compiled to a 255-register
 //   budget, which the [64 x 256] output accumulator plus the hidden fragments need for the wgmmas to stay asynchronous (with a
 //   third, producer warpgroup the budget is 168 and the d = 256 accumulators spill).
@@ -449,7 +449,7 @@ __global__ void __launch_bounds__(kThreads, 1) tc_wgrad_group_kernel(const __gri
 //   its first thread issues the TMA loads (X once, then the refill of a stage once all eight warps have released it) and
 //   warpgroup 0 never waits for a refill it did not need.  With 5 stages, the items of step s are requested when step
 //   s - 3 (item 2s - 1) and step s - 2 (item 2s) release theirs.
-//   smem: X 64 KB | weight ring 5 x 32 KB
+//   smem: X 64 KB | weight ring 5 x 32 KB (after the last step: the fp32 output rows on their way to x_out)
 // =============================================================================================================
 struct MlpParams {
   int M, d, ffn;
@@ -472,12 +472,37 @@ constexpr uint32_t kMlpXBytes = 65536;
 constexpr size_t kMlpSmem = 1024 + kMlpXBytes + kMlpStages * kMlpStageBytes + 256;
 static_assert(kMlpSmem <= (size_t)kSmemLimit, "fused MLP smem");
 
+// Timeline of the fused FFN kernel for tools/ffn_bench.py, compiled only into that tool's own library: the first thread of
+// each warpgroup writes clock64 stamps to g_mlp_timeline[(blockIdx.x * 2 + warpgroup) * kMlpTlSlots + slot].  Slots: 0 / 1
+// globaltimer / clock64 at entry, 2 after the X tile arrived, 3 tail start, 4 output rows staged in shared memory, 5 / 6
+// clock64 / globaltimer at exit (after the bulk reductions completed); step s (0 .. H) at 8 + 6 s + e: e = 0 entry, 1 hidden epilogue done, 2 turn taken (named barrier),
+// 3 ring items arrived, 4 wgmmas issued (before the wait), 5 wgmmas complete (after the W2 item's release).  No stamps are
+// written while the buffer pointer is null; without the macro nothing is emitted.
+#ifdef B200ST_MLP_TIMELINE
+constexpr int kMlpTlSlots = 256;
+__device__ unsigned long long* g_mlp_timeline;
+__device__ __forceinline__ unsigned long long mlp_globaltimer() {
+  unsigned long long t;
+  asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t));
+  return t;
+}
+#define MLP_STAMP_AT(slot, value)                                                                                       \
+  do {                                                                                                                  \
+    if ((threadIdx.x & 127) == 0 && g_mlp_timeline != nullptr)                                                          \
+      g_mlp_timeline[((size_t)blockIdx.x * 2 + (threadIdx.x >> 7)) * kMlpTlSlots + (slot)] = (value);                 \
+  } while (0)
+#define MLP_STAMP(slot) MLP_STAMP_AT(slot, (unsigned long long)clock64())
+#else
+#define MLP_STAMP_AT(slot, value) ((void)0)
+#define MLP_STAMP(slot) ((void)0)
+#endif
+
 // B_MN: weights as MN-major B operands (forward: W1 [d, ffn], W2 [ffn, d] in the TF [in, out] layout) or K-major (backward:
 // the same arrays read transposed: G1 uses W2 rows = hidden units, G2 uses W1 rows = model dims)
 template <int DT, bool B_MN, int D>
 __global__ void __launch_bounds__(kMlpThreads, 1)
 fused_mlp_fwd_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_constant__ CUtensorMap tmW1,
-                     const __grid_constant__ CUtensorMap tmW2, const MlpParams p) {
+                     const __grid_constant__ CUtensorMap tmW2, const __grid_constant__ CUtensorMap tmO, const MlpParams p) {
   extern __shared__ uint8_t smem_raw[];
   constexpr bool BF = DT == BF16;
   constexpr int kbx = D / BK;                  // k-blocks of GEMM1
@@ -497,9 +522,11 @@ fused_mlp_fwd_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_const
   const int H = 2 * p.chunks_per_cta;                  // 64-column hidden halves of this CTA's slice
   const int hid0 = split * p.chunks_per_cta * 128;     // first hidden unit of the slice
   const bool producer = threadIdx.x == 128;            // first thread of warpgroup 1
+  MLP_STAMP_AT(0, mlp_globaltimer());
+  MLP_STAMP(1);
 
   if (producer) {
-    ptx::prefetch_tensormap(&tmX); ptx::prefetch_tensormap(&tmW1); ptx::prefetch_tensormap(&tmW2);
+    ptx::prefetch_tensormap(&tmX); ptx::prefetch_tensormap(&tmW1); ptx::prefetch_tensormap(&tmW2); ptx::prefetch_tensormap(&tmO);
     ptx::mbar_init(x_full, 1);
     for (int s2 = 0; s2 < kMlpStages; ++s2) { ptx::mbar_init(w_full(s2), 1); ptx::mbar_init(w_empty(s2), kConsumerWarps); }
     ptx::fence_mbar_init();
@@ -617,6 +644,7 @@ fused_mlp_fwd_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_const
   // Step s; G2 / G1 are compile-time flags (false for the first / last step), so that no wgmma sits on a path the compiler
   // must treat as divergent (ptxas would serialize them).
   auto step = [&](const int s, auto G2, auto G1) {
+    MLP_STAMP(8 + 6 * s);
     if constexpr (decltype(G2)::value) {
       // ---- hidden epilogue of half s - 1: bias, ReLU, dropout (forward) / relu'-dropout' mask (backward); store; pack ----
       const int n0 = hid0 + (s - 1) * 64 + 2 * q;
@@ -641,9 +669,12 @@ fused_mlp_fwd_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_const
       }
     }
     // ---- step s, in this warpgroup's turn: GEMM2 of half s - 1 (out[64 x D] += hidden half x W2 rows), GEMM1 of half s ----
+    MLP_STAMP(8 + 6 * s + 1);
     if (G2 || wg == 1) ptx::named_bar_sync(kOrderBar + wg, 256);
+    MLP_STAMP(8 + 6 * s + 2);
     const uint32_t src = G2 ? stage_get(2 * s - 1) : 0u;          // both waits before the wgmmas: none sits between them
     const uint32_t w1 = G1 ? stage_get(2 * s) : 0u;
+    MLP_STAMP(8 + 6 * s + 3);
     ptx::fence_acc(out);
     ptx::fence_acc(hid);
     ptx::wgmma_fence();
@@ -676,7 +707,9 @@ fused_mlp_fwd_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_const
       }
     }
     asm volatile("" : "+r"(keep));            // folded while the wgmmas run, not after the wait
+    MLP_STAMP(8 + 6 * s + 4);
     ptx::wgmma_wait<0>();
+    MLP_STAMP(8 + 6 * s + 5);
     ptx::fence_acc(out);
     ptx::fence_acc(hid);
 #pragma unroll
@@ -688,22 +721,25 @@ fused_mlp_fwd_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_const
   };
   load_ew(0);
   ptx::mbar_wait(x_full, 0);
+  MLP_STAMP(2);
   step(0, std::false_type{}, std::true_type{});
   for (int s = 1; s < H; ++s) step(s, std::true_type{}, std::true_type{});
   step(H, std::true_type{}, std::false_type{});
-  // ---- output rows: (+ b2 on slice 0) -> post dropout -> fp32 add into x_out ----
+  MLP_STAMP(3);
+  // ---- output rows: (+ b2 on slice 0) -> post dropout -> shared memory -> TMA reduce-add into x_out ----
+  // Every CTA of the wave reaches this tail at about the same time.  Per-thread 8-byte atomics (each warp instruction
+  // touching 8 rows) ran at the L2's rate for such requests, about half the launch at M = 8000; staged through shared
+  // memory, the tile goes out as D / 32 bulk reductions per warpgroup of [64 rows x 32 columns] each, added at L2.
+  // Once both warpgroups are past their last wgmma wait no ring item is read any more, so the ring holds the staging:
+  // warpgroup wg's [64 x D] fp32 rows at sW + wg * 64 * D * 4, box b (columns 32 b ..) at + 8 KB * b, rows 128 B apart
+  // with the 16-byte chunks XOR-swizzled by row % 8 (the tensor map's 128B swizzle; a warp's stores hit 32 banks).
   const bool add_b2 = split == 0 && p.b2 != nullptr;
   const bool post = p.drop_post.p > 0.f;
   const float pscale = post ? p.drop_post.scale : 1.f;
-  if (p.tickets && p.splits > 1) {
-    // deterministic reduction order: slice s adds only after slices 0 .. s-1 of this row tile have completed theirs
-    if (lane == 0) {
-      const volatile int* tk = p.tickets + m_blk;
-      while (*tk != split) { }
-      __threadfence();
-    }
-    __syncwarp();
-  }
+  __syncthreads();
+  // this thread's rows (warp & 3) * 16 + g + 8 hr of the warpgroup's 64: row % 8 = g
+  const uint32_t row_base = sW + (uint32_t)wg * (64u * D * 4u) + (uint32_t)((warp & 3) * 16 + g) * 128u + (uint32_t)(q & 1) * 8u;
+  uint2 pbits[2];                              // post-dropout bytes of columns 8 j' .. 8 j' + 63 of the thread's two rows
 #pragma unroll
   for (int j = 0; j < D / 8; ++j) {
     const int n = 8 * j + 2 * q;
@@ -712,22 +748,48 @@ fused_mlp_fwd_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_const
 #pragma unroll
     for (int hr = 0; hr < 2; ++hr) {
       const int m = m0 + 8 * hr;
-      if (m < p.M) {
-        float v0 = out[4 * j + 2 * hr] + bb.x, v1 = out[4 * j + 2 * hr + 1] + bb.y;
-        if (post) {
-          const uint32_t kb = (uint32_t)__ldg(p.drop_post.bits + ((uint64_t)((int64_t)m * p.d + n) >> 3)) >> (2 * q);
-          v0 = (kb & 1u) ? v0 * pscale : 0.f;
-          v1 = (kb & 2u) ? v1 * pscale : 0.f;
-        }
-        atomicAdd(reinterpret_cast<float2*>(p.out + (int64_t)m * p.d + n), make_float2(v0, v1));
+      if ((j & 7) == 0)
+        pbits[hr] = post && m < p.M ? __ldg(reinterpret_cast<const uint2*>(p.drop_post.bits + (((int64_t)m * p.d + 8 * j) >> 3)))
+                                    : make_uint2(0u, 0u);
+      float v0 = out[4 * j + 2 * hr] + bb.x, v1 = out[4 * j + 2 * hr + 1] + bb.y;
+      if (post) {
+        const uint32_t kb = ((j & 4) ? pbits[hr].y : pbits[hr].x) >> (8 * (j & 3) + 2 * q);
+        v0 = (kb & 1u) ? v0 * pscale : 0.f;
+        v1 = (kb & 2u) ? v1 * pscale : 0.f;
       }
+      const uint32_t chunk = (uint32_t)(((j & 3) * 2 + (q >> 1)) ^ g);       // rows >= M are staged but not added
+      const uint32_t dst = row_base + (uint32_t)(j >> 2) * 8192u + (uint32_t)hr * 1024u + chunk * 16u;
+      asm volatile("st.shared.v2.f32 [%0], {%1, %2};" ::"r"(dst), "f"(v0), "f"(v1) : "memory");
     }
   }
-  if (p.tickets && p.splits > 1) {
-    __threadfence();
-    __syncthreads();                           // all 8 warps' additions have been performed
+  ptx::fence_proxy_async_smem();               // the generic-proxy stores, visible to the bulk reductions
+  ptx::named_bar_sync(kEpiBar + wg, 128);
+  MLP_STAMP(4);
+  const bool ordered = p.tickets && p.splits > 1;
+  if ((threadIdx.x & 127) == 0) {
+    if (ordered) {
+      // deterministic reduction order: slice s adds only after slices 0 .. s-1 of this row tile have completed theirs
+      const volatile int* tk = p.tickets + m_blk;
+      while (*tk != split) { }
+      __threadfence();
+      asm volatile("fence.proxy.async.global;" ::: "memory");
+    }
+#pragma unroll
+    for (int b = 0; b < D / 32; ++b)
+      ptx::tma_reduce_add_2d(&tmO, sW + (uint32_t)wg * (64u * D * 4u) + (uint32_t)b * 8192u, b * 32, m_blk * BM + wg * 64);
+    ptx::bulk_commit();
+    ptx::bulk_wait_all();                      // shared memory may be released, and the additions are performed
+    if (ordered) {
+      asm volatile("fence.proxy.async.global;" ::: "memory");
+      __threadfence();
+    }
+  }
+  if (ordered) {
+    __syncthreads();                           // both warpgroups' reductions have completed
     if (threadIdx.x == 0) atomicExch(p.tickets + m_blk, split + 1 == p.splits ? 0 : split + 1);
   }
+  MLP_STAMP(5);
+  MLP_STAMP_AT(6, mlp_globaltimer());
 }
 
 // -------------------------------------------------------------------------------------------
@@ -793,6 +855,30 @@ int make_operand_map(const GemmOperand& op, int rows, int K, int nb1, int nb2, i
                   const_cast<void*>(op.ptr), dims, strides, box, estr,
                   CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
                   CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+  if (r != CUDA_SUCCESS) B200ST_FAIL("cuTensorMapEncodeTiled failed with CUresult " + std::to_string((int)r));
+  std::lock_guard<std::mutex> lk(g_map_mu);
+  if (g_map_cache.size() > 65536) g_map_cache.clear();
+  g_map_cache.emplace(key, *out);
+  return 0;
+}
+
+// fp32 [M, d] row-major output of the fused FFN kernel: [64 rows x 32 columns] boxes, 128B swizzle (bulk reduce-add target)
+int make_out_map_f32(float* ptr, int M, int d, CUtensorMap* out) {
+  EncodeTiledFn fn = get_encode_fn();
+  B200ST_CHECK(fn != nullptr, "cuTensorMapEncodeTiled unavailable (no CUDA driver?)");
+  B200ST_CHECK((reinterpret_cast<uintptr_t>(ptr) & 15) == 0 && d % 32 == 0, "fp32 output map: unaligned base or width");
+  cuuint64_t dims[2] = {(cuuint64_t)d, (cuuint64_t)M};
+  cuuint64_t strides[1] = {(cuuint64_t)d * 4};
+  cuuint32_t box[2] = {32u, 64u};
+  cuuint32_t estr[2] = {1u, 1u};
+  MapKey key{{(uint64_t)(uintptr_t)ptr, (uint64_t)d, (uint64_t)M, 1, 1, strides[0], 0, 0, box[1], (uint64_t)F32 << 8 | 0x10000u}};
+  {
+    std::lock_guard<std::mutex> lk(g_map_mu);
+    auto it = g_map_cache.find(key);
+    if (it != g_map_cache.end()) { *out = it->second; return 0; }
+  }
+  CUresult r = fn(out, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 2, ptr, dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
+                  CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
   if (r != CUDA_SUCCESS) B200ST_FAIL("cuTensorMapEncodeTiled failed with CUresult " + std::to_string((int)r));
   std::lock_guard<std::mutex> lk(g_map_mu);
   if (g_map_cache.size() > 65536) g_map_cache.clear();
@@ -1142,7 +1228,9 @@ int fused_mlp_fwd(const void* X, int dtype, int M, int d, int ffn, const void* W
   if (drop_ffn.p > 0.f)
     B200ST_CHECK(drop_ffn.bits != nullptr && (reinterpret_cast<uintptr_t>(drop_ffn.bits) & 7) == 0,
                  "fused MLP needs precomputed, 8-byte aligned dropout bits");
-  if (drop_post.p > 0.f) B200ST_CHECK(drop_post.bits != nullptr, "fused MLP needs precomputed dropout bits");
+  if (drop_post.p > 0.f)
+    B200ST_CHECK(drop_post.bits != nullptr && (reinterpret_cast<uintptr_t>(drop_post.bits) & 7) == 0,
+                 "fused MLP needs precomputed, 8-byte aligned dropout bits");
   const int m_tiles = ceil_div(M, BM), chunks = ffn / 128;
   int splits = 1;
   B200ST_TRY(mlp_splits(m_tiles, chunks, &splits));
@@ -1151,11 +1239,13 @@ int fused_mlp_fwd(const void* X, int dtype, int M, int d, int ffn, const void* W
   p.b1 = b1; p.b2 = b2; p.drop_ffn = drop_ffn; p.drop_post = drop_post;
   p.relu = 1; p.alpha = 1.f; p.mask_src = nullptr; p.mask_ld = 0; p.tickets = tickets;
   p.F1 = reinterpret_cast<uint16_t*>(F1); p.out = x_out;
-  B200ST_CHECK((reinterpret_cast<uintptr_t>(F1) & 3) == 0 && (reinterpret_cast<uintptr_t>(x_out) & 7) == 0, "fused MLP: unaligned output");
+  B200ST_CHECK((reinterpret_cast<uintptr_t>(F1) & 3) == 0 && (reinterpret_cast<uintptr_t>(x_out) & 15) == 0, "fused MLP: unaligned output");
   CUtensorMap tx, tw1, tw2;
   B200ST_TRY(make_operand_map(GemmOperand{X, dtype, 0, d, 0, 0}, M, d, 1, 1, BM, &tx));
   B200ST_TRY(make_operand_map(GemmOperand{W1, dtype, 1, ffn, 0, 0}, ffn, d, 1, 1, 64, &tw1));
   B200ST_TRY(make_operand_map(GemmOperand{W2, dtype, 1, d, 0, 0}, d, ffn, 1, 1, 64, &tw2));
+  CUtensorMap to;
+  B200ST_TRY(make_out_map_f32(x_out, M, d, &to));
   auto kern = d == 256 ? (dtype == F16 ? fused_mlp_fwd_kernel<F16, true, 256> : fused_mlp_fwd_kernel<BF16, true, 256>)
                        : (dtype == F16 ? fused_mlp_fwd_kernel<F16, true, 128> : fused_mlp_fwd_kernel<BF16, true, 128>);
   static bool attr[4] = {false, false, false, false};
@@ -1164,7 +1254,7 @@ int fused_mlp_fwd(const void* X, int dtype, int M, int d, int ffn, const void* W
     B200ST_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kMlpSmem));
     attr[ai] = true;
   }
-  launch_pdl(kern, m_tiles * splits, kMlpThreads, kMlpSmem, stream, tx, tw1, tw2, p);
+  launch_pdl(kern, m_tiles * splits, kMlpThreads, kMlpSmem, stream, tx, tw1, tw2, to, p);
   ++g_launches;
   B200ST_LAUNCH_CHECK();
   return 0;
@@ -1183,12 +1273,14 @@ int fused_mlp_bwd(const void* dY, int dtype, int M, int d, int ffn, const void* 
   p.b1 = nullptr; p.b2 = nullptr; p.drop_ffn = no_dropout(); p.drop_post = no_dropout();
   p.relu = 0; p.alpha = scale; p.mask_src = F1; p.mask_ld = ffn; p.tickets = tickets;
   p.F1 = reinterpret_cast<uint16_t*>(dF1); p.out = dH;
-  B200ST_CHECK((reinterpret_cast<uintptr_t>(dF1) & 3) == 0 && (reinterpret_cast<uintptr_t>(dH) & 7) == 0 &&
+  B200ST_CHECK((reinterpret_cast<uintptr_t>(dF1) & 3) == 0 && (reinterpret_cast<uintptr_t>(dH) & 15) == 0 &&
                (reinterpret_cast<uintptr_t>(F1) & 3) == 0, "fused MLP: unaligned buffer");
   CUtensorMap tx, tw1, tw2;
   B200ST_TRY(make_operand_map(GemmOperand{dY, dtype, 0, d, 0, 0}, M, d, 1, 1, BM, &tx));
   B200ST_TRY(make_operand_map(GemmOperand{W2, dtype, 0, d, 0, 0}, ffn, d, 1, 1, 64, &tw1));      // G1: rows = hidden units, k = d
   B200ST_TRY(make_operand_map(GemmOperand{W1, dtype, 0, ffn, 0, 0}, d, ffn, 1, 1, d, &tw2));      // G2: rows = model dims, k = hidden
+  CUtensorMap to;
+  B200ST_TRY(make_out_map_f32(dH, M, d, &to));
   auto kern = d == 256 ? (dtype == F16 ? fused_mlp_fwd_kernel<F16, false, 256> : fused_mlp_fwd_kernel<BF16, false, 256>)
                        : (dtype == F16 ? fused_mlp_fwd_kernel<F16, false, 128> : fused_mlp_fwd_kernel<BF16, false, 128>);
   static bool attr[4] = {false, false, false, false};
@@ -1197,7 +1289,7 @@ int fused_mlp_bwd(const void* dY, int dtype, int M, int d, int ffn, const void* 
     B200ST_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kMlpSmem));
     attr[ai] = true;
   }
-  launch_pdl(kern, m_tiles * splits, kMlpThreads, kMlpSmem, stream, tx, tw1, tw2, p);
+  launch_pdl(kern, m_tiles * splits, kMlpThreads, kMlpSmem, stream, tx, tw1, tw2, to, p);
   ++g_launches;
   B200ST_LAUNCH_CHECK();
   return 0;
