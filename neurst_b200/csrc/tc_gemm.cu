@@ -57,6 +57,7 @@ struct TcParams {
   GemmEpilogue epi;
   int atomic;           // C += through fp32 atomics (split-K or accumulate)
   int vec2;             // C may be written two columns at a time (even N, ld and batch strides; 8-byte aligned base)
+  int plain16;          // 16-bit C, plain stores, epilogue = alpha (+ bias) only: the short epilogue loop applies
   // implicit transposed-convolution A operand (conv2 data gradient, see gemm_conv2_dgrad): A tile = a [conv_tu x conv_v]
   // patch of positions x 64 channels of dY[B, T2, F2, C], shifted by the tap; k-block kb = (tap, 64-channel chunk)
   int conv;             // 0 = off
@@ -299,7 +300,24 @@ tc_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
           *reinterpret_cast<float2*>(stg + (r + 8) * kLd + c) = make_float2(acc[h][4 * jj + 2], acc[h][4 * jj + 3]);
         }
         ptx::named_bar_sync(kEpiBar + wg, 128);
-        if (n < p.N) {
+        if (p.plain16 && n + 1 < p.N) {
+          // alpha (+ bias) into 16-bit C, a column pair per thread: the bias pair and the column offset are fixed for the
+          // tile, so a row costs one shared load, the arithmetic and one store (the general loop below re-derives every
+          // epilogue option per element, and its instruction count, not memory, bounded the short-K GEMMs)
+          const float b0 = ep.bias ? __ldg(ep.bias + n) : 0.f, b1 = ep.bias ? __ldg(ep.bias + n + 1) : 0.f;
+          uint32_t* c32 = reinterpret_cast<uint32_t*>(p.C);
+          const int64_t col = boff_c + n;
+#pragma unroll 8
+          for (int r = tid / kPairs; r < 64; r += kRowStep) {
+            const int m = t.m_blk * BM + h * 64 + r;
+            if (m < p.M) {
+              const float2 v = *reinterpret_cast<const float2*>(stg + r * kLd + 2 * cp);
+              float v0 = v.x * ep.alpha, v1 = v.y * ep.alpha;
+              if (ep.bias) { v0 += b0; v1 += b1; }
+              c32[(col + (int64_t)m * p.ldc) >> 1] = pack2_16(v0, v1, p.c_dtype);
+            }
+          }
+        } else if (n < p.N) {
 #pragma unroll 4
           for (int r = tid / kPairs; r < 64; r += kRowStep) {
             const int m = t.m_blk * BM + h * 64 + r;
@@ -1045,6 +1063,7 @@ int gemm_tc_impl(const GemmArgs& g, cudaStream_t stream, const ConvA* conv) {
   const uintptr_t pair_bytes = g.c_dtype == F32 ? 8 : 4;
   p.vec2 = ((reinterpret_cast<uintptr_t>(g.C) % pair_bytes) == 0 && g.ldc % 2 == 0 && (g.nb1 == 1 || g.c_sb1 % 2 == 0) &&
             (g.nb2 == 1 || g.c_sb2 % 2 == 0)) ? 1 : 0;
+  p.plain16 = (!p.atomic && g.c_dtype != F32 && p.vec2 && !g.epi.relu && !g.epi.mask_src && g.epi.drop.p == 0.f && !g.epi.residual) ? 1 : 0;
 
   CUtensorMap ta, tb;
   if (conv) {
