@@ -925,6 +925,12 @@ def sampling_seed(seed, rank):
     return (int(seed) + int(rank) * 0x9E3779B97F4A7C15) & 0xFFFFFFFFFFFFFFFF
 
 
+def search_fn(model, plan):
+    """The model's search for the plan's search_method: beam_search, top_sampling, or greedy without one."""
+    name = {"beam_search": "beam_search", "top_sampling": "sampling_search"}.get(plan.get("search_method"), "greedy_search")
+    return getattr(model, name)
+
+
 def decode_group(model, task, plan, group, search_kw, first=0, lengths=None):
     """One search call over preprocessed samples -> [(ids_to_text hypothesis, score)], top_k (beam search) or sample_num
     (top_sampling) rows per utterance, consecutive (the reference's [B*top_k] order).  `first`: the position of group[0] in
@@ -943,12 +949,9 @@ def decode_group(model, task, plan, group, search_kw, first=0, lengths=None):
             src[j, :int(e["audio_length"])] = e["audio"]
         batch = task.example_to_input({"audio": src, "audio_length": torch.tensor([int(e["audio_length"]) for e in group])}, infer=True)
         inputs = {"src": batch["src"], "src_length": batch["src_length"]}
-    method = plan.get("search_method")
-    if method == "top_sampling":
-        search, search_kw = model.sampling_search, dict(search_kw, row_offset=int(first) * plan["search"]["sample_num"])
-    else:
-        search = model.beam_search if method == "beam_search" else model.greedy_search
-    ids, score = search(inputs, **search_kw)
+    if plan.get("search_method") == "top_sampling":
+        search_kw = dict(search_kw, row_offset=int(first) * plan["search"]["sample_num"])
+    ids, score = search_fn(model, plan)(inputs, **search_kw)
     if lengths is not None:
         per = ids.shape[0] // len(group)
         for r, row in enumerate(ids.cpu().tolist()):
@@ -1037,8 +1040,7 @@ def cascade_st(plan):
     asr_per_call, asr_kw = decode_settings(asr_plan)
     mt_per_call, mt_kw = decode_settings(mt_plan)
     per_call = min(asr_per_call, mt_per_call)
-    asr_search = asr.beam_search if asr_plan.get("search_method") == "beam_search" else asr.greedy_search
-    mt_search = mt.beam_search if mt_plan.get("search_method") == "beam_search" else mt.greedy_search
+    asr_search, mt_search = search_fn(asr, asr_plan), search_fn(mt, mt_plan)
     asr_hyps, mt_hyps = [], []
 
     def run(group):

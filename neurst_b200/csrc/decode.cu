@@ -782,7 +782,7 @@ int step_launch(const StepCtx& c, const TW* wbase, const int64_t* ids, const int
 }
 
 // More than 8 rows: the embedding of the current symbols into x (scratch offset 0), then the wide step (decode_rows.cu).
-// rows_check has run before.
+// rows_check has run and the wide step's shared-memory limits are raised.
 int step_rows(const StepCtx& c, const int64_t* ids, const int32_t* time_dev, float* logits_out, const int* anc, int beam) {
   const Config& cf = c.m.cfg;
   const int n = c.st.B * cf.d;
@@ -961,6 +961,72 @@ BeamState beam_state_at(void* words, int rows, int max_len) {
   return bs;
 }
 
+// The logits [st.B, V] of a step in st's scratch: the GEMV step's layout up to 8 rows, the wide step's above.
+float* step_logits(const Config& cf, const DecodeState& st) {
+  return st.scratch + (st.B > MAXB ? rows_logits_offset(cf, st.B) : layout_of(cf, st.B).logits);
+}
+
+// What the beam, ensemble and sampling searches step: `width` rows per utterance (row u * width + k is beam or sample k of
+// utterance u) for each of n members, whose states hold the same B utterances.
+struct SearchRows {
+  int rows;
+  std::vector<StepCtx> ctx;      // per member, on every row; cross_kv / memory_bias stay per utterance
+  std::vector<float*> logits;    // per member: the logits [rows, V] of its step
+};
+
+// Checks everything the search needs before anything is launched, then raises the attention kernels' dynamic shared-memory
+// limits once, to the largest need over the members.  The limit is an attribute of the kernel, not of the launch: set
+// member after member, a member with a smaller head or model width would lower it below an earlier member's need.
+int prepare_search(const EnsembleMember* mem, int n, int width, int max_steps, const char* width_name, const char* search,
+                   cudaStream_t s, SearchRows* out) {
+  const DecodeState& st0 = mem[0].st;
+  const int V = mem[0].m->cfg.vocab;
+  const int64_t rows = (int64_t)st0.B * width;
+  B200ST_CHECK(width >= 1 && width <= KMAX,
+               std::string(width_name) + " must be in 1.." + std::to_string(KMAX) + ", got " + std::to_string(width));
+  B200ST_CHECK(max_steps >= 1 && max_steps <= st0.max_len, "max_steps must be within the cache length");
+  size_t smem_self = 0, smem_cross = 0, rows_self = 0, rows_cross = 0;
+  for (int i = 0; i < n; ++i) {
+    const Model& m = *mem[i].m;
+    const Config& cf = m.cfg;
+    const DecodeState& st = mem[i].st;
+    const std::string who = n > 1 ? "ensemble member " + std::to_string(i) + ": " : "";
+    if (n > 1) {
+      B200ST_CHECK(cf.vocab == V,
+                   who + "vocabulary of " + std::to_string(cf.vocab) + " differs from member 0's " + std::to_string(V));
+      B200ST_CHECK(st.B == st0.B && st.Tm == st0.Tm && st.max_len == st0.max_len,
+                   who + "decode state (B, Tm, max_len) = (" + std::to_string(st.B) + ", " + std::to_string(st.Tm) + ", " +
+                   std::to_string(st.max_len) + ") differs from member 0's (" + std::to_string(st0.B) + ", " +
+                   std::to_string(st0.Tm) + ", " + std::to_string(st0.max_len) + ")");
+    }
+    const int max_rows = st.use_shadow ? kDecodeMaxRows : MAXB;      // more than 8 rows: the wide step, 16-bit shadow only
+    B200ST_CHECK(rows <= max_rows, who + search + " decodes at most " + std::to_string(max_rows) + " rows (utterances x " +
+                                   width_name + ") per call" + (st.use_shadow ? "" : " without use_shadow") + ", got " +
+                                   std::to_string(st.B) + " x " + std::to_string(width));
+    B200ST_TRY(check_state(m, st));
+    if (st.use_shadow)
+      B200ST_CHECK(is16(m.adt) && mem[i].buf.shadow, who + "use_shadow needs a 16-bit precision handle and its shadow arena");
+    DecodeState rs = st;
+    rs.B = (int)rows;
+    B200ST_TRY(check_state(m, rs));
+    if (rows > MAXB) {
+      B200ST_TRY(rows_check(m, mem[i].buf, rs, width));
+      rows_self = std::max(rows_self, rows_self_smem(cf, st.max_len));
+      rows_cross = std::max(rows_cross, rows_cross_smem(cf, st.Tm, width));
+    }
+    const size_t ss = self_attn_smem(cf, st.max_len, true);
+    B200ST_CHECK(ss <= 200 * 1024, "decode: too many keys for the shared-memory score buffer");
+    smem_self = std::max(smem_self, ss);
+    smem_cross = std::max(smem_cross, cross_attn_smem(cf, st.Tm));
+    out->ctx.push_back(StepCtx{m, mem[i].buf, rs, s});
+    out->logits.push_back(step_logits(cf, rs));
+  }
+  out->rows = (int)rows;
+  B200ST_TRY(raise_beam_smem(smem_self, smem_cross));
+  if (rows > MAXB) B200ST_TRY(rows_raise_smem(rows_self, rows_cross));
+  return 0;
+}
+
 }  // namespace
 
 static int g_last_greedy_graph = -1;
@@ -995,7 +1061,10 @@ int decode_step(const Model& m, const Buffers& buf, const DecodeState& st, const
                 float* logits, cudaStream_t s) {
   B200ST_TRY(check_state(m, st));
   B200ST_CHECK(symbols && time_dev && logits, "decode_step: null argument");
-  if (st.B > MAXB) B200ST_TRY(rows_check(m, buf, st, 1));
+  if (st.B > MAXB) {
+    B200ST_TRY(rows_check(m, buf, st, 1));
+    B200ST_TRY(rows_raise_smem(rows_self_smem(m.cfg, st.max_len), rows_cross_smem(m.cfg, st.Tm, 1)));
+  }
   B200ST_TRY(raise_all_smem(m.cfg, st));
   StepCtx c{m, buf, st, s};
   return step_dispatch(c, symbols, time_dev, logits);
@@ -1009,7 +1078,10 @@ int greedy_search(const Model& m, const Buffers& buf, const DecodeState& st, con
   B200ST_CHECK(ga.max_steps >= 1 && ga.max_steps <= st.max_len, "max_steps must be within the cache length");
   B200ST_CHECK(ga.bos_ids && ga.out_ids && ga.out_len && ga.out_logprob && ga.state_words, "greedy_search: null argument");
   const bool wide = st.B > MAXB;
-  if (wide) B200ST_TRY(rows_check(m, buf, st, 1));
+  if (wide) {
+    B200ST_TRY(rows_check(m, buf, st, 1));
+    B200ST_TRY(rows_raise_smem(rows_self_smem(cf, st.max_len), rows_cross_smem(cf, st.Tm, 1)));
+  }
   B200ST_TRY(raise_all_smem(cf, st));
   // device words: [ids x int64][finished][time][all_finished] with 8 row slots, or B row slots and a [ticket] above 8 rows
   char* w = reinterpret_cast<char*>(ga.state_words);
@@ -1023,7 +1095,7 @@ int greedy_search(const Model& m, const Buffers& buf, const DecodeState& st, con
   g.time = reinterpret_cast<int32_t*>(w); w += sizeof(int32_t);
   g.all_finished = reinterpret_cast<int32_t*>(w); w += sizeof(int32_t);
   uint32_t* ticket = reinterpret_cast<uint32_t*>(w);
-  float* logits = st.scratch + (wide ? rows_logits_offset(cf, st.B) : layout_of(cf, st.B).logits);
+  float* logits = step_logits(cf, st);
   greedy_init_kernel<<<8, 256, 0, s>>>(g, ga.bos_ids, st.B, ga.max_steps, ga.eos_id);
   B200ST_CUDA(cudaGetLastError());
   if (wide) B200ST_CUDA(cudaMemsetAsync(ticket, 0, sizeof(uint32_t), s));
@@ -1067,99 +1139,34 @@ int64_t beam_state_bytes(int B, int beam, int max_len) {
 
 // sequence_beam_search (beam_search.py:254-439) with the per-token step of the greedy search on B x beam rows.
 int beam_search(const Model& m, const Buffers& buf, const DecodeState& st, const BeamArgs& a, cudaStream_t s) {
-  B200ST_TRY(check_state(m, st));
-  const Config& cf = m.cfg;
-  const int beam = a.beam_size;
-  B200ST_CHECK(beam >= 1, "beam_size must be >= 1");
-  B200ST_CHECK(a.top_k >= 1 && a.top_k <= beam, "top_k must be in 1..beam_size");
-  const int max_rows = st.use_shadow ? kDecodeMaxRows : MAXB;      // more than 8 rows: the wide step, 16-bit shadow only
-  B200ST_CHECK((int64_t)st.B * beam <= max_rows, "beam search decodes at most " + std::to_string(max_rows) +
-                                                 " rows (utterances x beam_size) per call, got " + std::to_string(st.B) + " x " +
-                                                 std::to_string(beam));
-  B200ST_CHECK(beam <= KMAX, "beam_size must be at most " + std::to_string(KMAX));
-  B200ST_CHECK(beam <= cf.vocab, "beam_size exceeds the vocabulary");
-  B200ST_CHECK(a.max_steps >= 1 && a.max_steps <= st.max_len, "max_steps must be within the cache length");
-  B200ST_CHECK(a.bos_ids && a.out_ids && a.out_scores && a.out_len && a.out_logprob && a.state_words, "beam_search: null argument");
-  if (beam == 1) {           // the reference's beam 1 is the greedy search
-    GreedyArgs ga{};
-    ga.bos_ids = a.bos_ids; ga.eos_id = a.eos_id; ga.unk_id = a.unk_id; ga.min_len = a.min_len; ga.max_steps = a.max_steps;
-    ga.out_ids = a.out_ids; ga.out_len = a.out_len; ga.out_logprob = a.out_logprob; ga.state_words = a.state_words;
-    ga.use_graph = a.use_graph;
-    B200ST_TRY(greedy_search(m, buf, st, ga, s));
-    beam1_score_kernel<<<(st.B + 255) / 256, 256, 0, s>>>(a.out_logprob, a.out_len, a.out_scores, st.B, a.length_penalty);
-    B200ST_CUDA(cudaGetLastError());
-    return 0;
-  }
-  const int rows = st.B * beam;
-  DecodeState rs = st;                    // the step runs on every beam row; cross_kv / memory_bias stay per utterance
-  rs.B = rows;
-  B200ST_TRY(check_state(m, rs));
-  if (rows > MAXB) B200ST_TRY(rows_check(m, buf, rs, beam));
-  const size_t smem_self = self_attn_smem(cf, st.max_len, true);
-  B200ST_CHECK(smem_self <= 200 * 1024, "decode: too many keys for the shared-memory score buffer");
-  B200ST_TRY(raise_all_smem(cf, st));
-  B200ST_TRY(raise_beam_smem(smem_self, cross_attn_smem(cf, st.Tm)));
-  const BeamState bs = beam_state_at(a.state_words, rows, st.max_len);
-  float* logits = rs.scratch + (rows > MAXB ? rows_logits_offset(cf, rows) : layout_of(cf, rows).logits);
-  beam_init_kernel<<<(rows + 255) / 256, 256, 0, s>>>(bs, a.bos_ids, rows, beam);
-  B200ST_CUDA(cudaGetLastError());
-  StepCtx c{m, buf, rs, s};
-  auto one_step = [&]() -> int {
-    B200ST_TRY(step_dispatch(c, bs.ids, bs.time, logits, bs.anc, beam));
-    launch_pdl(beam_select_kernel<false>, st.B, 1024, 0, s, (const float*)logits, bs, beam, cf.vocab, a.eos_id, a.unk_id, a.min_len,
-               a.length_penalty, st.max_len);
-    ++g_kernel_launches;
-    B200ST_LAUNCH_CHECK();
-    return 0;
-  };
-  bool graphed = false;
-  B200ST_TRY(run_token_loop(s, a.max_steps, a.use_graph != 0, bs.all_finished, one_step, &graphed));
-  B200ST_CHECK(graphed || !a.use_graph, "beam search could not capture its step into a CUDA graph");
-  beam_extract_kernel<<<st.B, 256, 0, s>>>(bs, beam, a.top_k, a.length_penalty, a.eos_id, st.max_len, a.max_steps, a.out_ids,
-                                           a.out_scores, a.out_logprob, a.out_len);
-  ++g_kernel_launches;
-  B200ST_CUDA(cudaGetLastError());
-  return 0;
+  const EnsembleMember one{&m, buf, st, 1.f};
+  return ensemble_beam_search(&one, 1, a, s);
 }
 
 // sequence_sampling_search (sampling.py:103-250) on B x sample_num rows: row u*sample_num + s is sample s of utterance u.
 // The rows never reorder, so the ancestry table stays the identity (each row reads its own self-attention cache) and the
 // beam variants of the step read the memory of utterance row / sample_num; sample_select_kernel (sampling.cu) draws.
 int sampling_search(const Model& m, const Buffers& buf, const DecodeState& st, const SamplingArgs& a, cudaStream_t s) {
-  B200ST_TRY(check_state(m, st));
   const Config& cf = m.cfg;
   const int n = a.sample_num;
-  B200ST_CHECK(n >= 1 && n <= KMAX, "sample_num must be in 1.." + std::to_string(KMAX) + ", got " + std::to_string(n));
   B200ST_TRY(check_sample_filter(a.top_k, a.top_p, cf.vocab));
-  const int max_rows = st.use_shadow ? kDecodeMaxRows : MAXB;      // more than 8 rows: the wide step, 16-bit shadow only
-  B200ST_CHECK((int64_t)st.B * n <= max_rows, "sampling search decodes at most " + std::to_string(max_rows) +
-                                              " rows (utterances x sample_num) per call, got " + std::to_string(st.B) + " x " +
-                                              std::to_string(n));
-  B200ST_CHECK(a.max_steps >= 1 && a.max_steps <= st.max_len, "max_steps must be within the cache length");
   B200ST_CHECK(a.row_offset >= 0, "row_offset must be >= 0");
   B200ST_CHECK(a.bos_ids && a.out_ids && a.out_len && a.out_logprob && a.state_words, "sampling_search: null argument");
-  const int rows = st.B * n;
-  DecodeState rs = st;                    // the step runs on every sample row; cross_kv / memory_bias stay per utterance
-  rs.B = rows;
-  B200ST_TRY(check_state(m, rs));
-  if (rows > MAXB) B200ST_TRY(rows_check(m, buf, rs, n));
-  const size_t smem_self = self_attn_smem(cf, st.max_len, true);
-  B200ST_CHECK(smem_self <= 200 * 1024, "decode: too many keys for the shared-memory score buffer");
-  B200ST_TRY(raise_all_smem(cf, st));
-  B200ST_TRY(raise_beam_smem(smem_self, cross_attn_smem(cf, st.Tm)));
+  const EnsembleMember one{&m, buf, st, 1.f};
+  SearchRows prep;
+  B200ST_TRY(prepare_search(&one, 1, n, a.max_steps, "sample_num", "sampling search", s, &prep));
+  const int rows = prep.rows;
   BeamState bs = beam_state_at(a.state_words, rows, st.max_len);
-  float* logits = rs.scratch + (rows > MAXB ? rows_logits_offset(cf, rows) : layout_of(cf, rows).logits);
   sample_init(bs, a.bos_ids, rows, n, st.max_len, a.out_ids, a.max_steps, a.eos_id, a.out_logprob, a.out_len, s);
   B200ST_CUDA(cudaGetLastError());
   SampleRows sr{};
-  sr.logits = logits; sr.V = cf.vocab; sr.eos = a.eos_id; sr.unk = a.unk_id; sr.min_len = a.min_len;
+  sr.logits = prep.logits[0]; sr.V = cf.vocab; sr.eos = a.eos_id; sr.unk = a.unk_id; sr.min_len = a.min_len;
   sr.top_k = a.top_k; sr.top_p = a.top_p; sr.seed = a.seed; sr.row_offset = a.row_offset;
   sr.ids = bs.ids; sr.finished = bs.finished; sr.length = a.out_len; sr.logprob = a.out_logprob;
   sr.out = a.out_ids; sr.max_steps = a.max_steps;
   sr.time = bs.time; sr.all_finished = bs.all_finished; sr.ticket = bs.ticket;
-  StepCtx c{m, buf, rs, s};
   auto one_step = [&]() -> int {
-    B200ST_TRY(step_dispatch(c, bs.ids, bs.time, logits, bs.anc, n));
+    B200ST_TRY(step_dispatch(prep.ctx[0], bs.ids, bs.time, prep.logits[0], bs.anc, n));
     sample_select(sr, rows, s);
     B200ST_LAUNCH_CHECK();
     return 0;
@@ -1170,11 +1177,12 @@ int sampling_search(const Model& m, const Buffers& buf, const DecodeState& st, c
   return 0;
 }
 
-// sequence_beam_search over EncoderDecoderEnsembleModel (encoder_decoder_ensemble_model.py, beam_search.py:97-115): per
-// token every member steps on the same B x beam rows (its own self-attention cache, cross K/V and scratch; the shared ids
-// and ancestry table of the one beam state), ensemble_logprob mixes their distributions over member 0's logits, and
-// beam_select_kernel<true> selects on the mixture.  beam_size 1 runs this same beam path, as the reference's greedy search
-// is sequence_beam_search(beam_size=1).  One member is the plain beam_search: the reference takes a plain log_softmax then.
+// The beam search of one model (beam_search) and of EncoderDecoderEnsembleModel (encoder_decoder_ensemble_model.py,
+// beam_search.py:97-115): per token every member steps on the same B x beam rows (its own self-attention cache, cross K/V
+// and scratch; the shared ids and ancestry table of the one beam state).  One member selects on its raw logits, as the
+// reference takes a plain log_softmax then; several are mixed by ensemble_logprob over member 0's logits and
+// beam_select_kernel<true> selects on the mixture.  One model's beam_size 1 is the greedy search; an ensemble's runs this
+// beam path, as the reference's greedy search is sequence_beam_search(beam_size=1).
 int ensemble_beam_search(const EnsembleMember* mem, int n, const BeamArgs& a, cudaStream_t s) {
   B200ST_CHECK(mem != nullptr && n >= 1 && n <= kEnsembleMaxModels,
                "an ensemble has 1.." + std::to_string(kEnsembleMaxModels) + " members, got " + std::to_string(n));
@@ -1187,76 +1195,49 @@ int ensemble_beam_search(const EnsembleMember* mem, int n, const BeamArgs& a, cu
     wsum += w;
   }
   B200ST_CHECK(wsum > 0.0, "ensemble weights must have a positive sum");
-  if (n == 1) return beam_search(*mem[0].m, mem[0].buf, mem[0].st, a, s);
   const DecodeState& st0 = mem[0].st;
   const int beam = a.beam_size, V = mem[0].m->cfg.vocab;
-  B200ST_CHECK(beam >= 1, "beam_size must be >= 1");
   B200ST_CHECK(a.top_k >= 1 && a.top_k <= beam, "top_k must be in 1..beam_size");
-  B200ST_CHECK(beam <= KMAX, "beam_size must be at most " + std::to_string(KMAX));
   B200ST_CHECK(beam <= V, "beam_size exceeds the vocabulary");
-  B200ST_CHECK(a.max_steps >= 1 && a.max_steps <= st0.max_len, "max_steps must be within the cache length");
-  B200ST_CHECK(a.bos_ids && a.out_ids && a.out_scores && a.out_len && a.out_logprob && a.state_words,
-               "ensemble_beam_search: null argument");
-  const int rows = st0.B * beam;
-  std::vector<StepCtx> ctx;
-  std::vector<float*> logits;
-  size_t smem_self = 0, smem_cross = 0, rows_self = 0, rows_cross = 0;
-  for (int i = 0; i < n; ++i) {
-    const Model& m = *mem[i].m;
-    const Config& cf = m.cfg;
-    const DecodeState& st = mem[i].st;
-    const std::string who = "ensemble member " + std::to_string(i) + ": ";
-    B200ST_CHECK(cf.model_type == MODEL_SPEECH || cf.model_type == MODEL_TEXT, who + "decoding needs an encoder-decoder handle");
-    B200ST_CHECK(cf.vocab == V, who + "vocabulary of " + std::to_string(cf.vocab) + " differs from member 0's " + std::to_string(V));
-    B200ST_CHECK(st.B == st0.B && st.Tm == st0.Tm && st.max_len == st0.max_len,
-                 who + "decode state (B, Tm, max_len) = (" + std::to_string(st.B) + ", " + std::to_string(st.Tm) + ", " +
-                 std::to_string(st.max_len) + ") differs from member 0's (" + std::to_string(st0.B) + ", " + std::to_string(st0.Tm) +
-                 ", " + std::to_string(st0.max_len) + ")");
-    const int max_rows = st.use_shadow ? kDecodeMaxRows : MAXB;      // more than 8 rows: the wide step, 16-bit shadow only
-    B200ST_CHECK(rows <= max_rows, who + "beam search decodes at most " + std::to_string(max_rows) + " rows (utterances x beam_size) per " +
-                                   "call" + (st.use_shadow ? "" : " without use_shadow") + ", got " + std::to_string(st.B) + " x " +
-                                   std::to_string(beam));
-    B200ST_TRY(check_state(m, st));
-    if (st.use_shadow) B200ST_CHECK(is16(m.adt) && mem[i].buf.shadow, who + "use_shadow needs a 16-bit precision handle and its shadow arena");
-    DecodeState rs = st;                  // the step runs on every beam row; cross_kv / memory_bias stay per utterance
-    rs.B = rows;
-    B200ST_TRY(check_state(m, rs));
-    if (rows > MAXB) {
-      B200ST_TRY(rows_check(m, mem[i].buf, rs, beam));
-      rows_self = std::max(rows_self, rows_self_smem(cf, st.max_len));
-      rows_cross = std::max(rows_cross, rows_cross_smem(cf, st.Tm, beam));
-    }
-    const size_t ss = self_attn_smem(cf, st.max_len, true);
-    B200ST_CHECK(ss <= 200 * 1024, "decode: too many keys for the shared-memory score buffer");
-    smem_self = std::max(smem_self, ss);
-    smem_cross = std::max(smem_cross, cross_attn_smem(cf, st.Tm));
-    ctx.push_back(StepCtx{m, mem[i].buf, rs, s});
-    logits.push_back(rs.scratch + (rows > MAXB ? rows_logits_offset(cf, rows) : layout_of(cf, rows).logits));
+  B200ST_CHECK(a.bos_ids && a.out_ids && a.out_scores && a.out_len && a.out_logprob && a.state_words, "beam_search: null argument");
+  if (n == 1 && beam == 1) {
+    GreedyArgs ga{};
+    ga.bos_ids = a.bos_ids; ga.eos_id = a.eos_id; ga.unk_id = a.unk_id; ga.min_len = a.min_len; ga.max_steps = a.max_steps;
+    ga.out_ids = a.out_ids; ga.out_len = a.out_len; ga.out_logprob = a.out_logprob; ga.state_words = a.state_words;
+    ga.use_graph = a.use_graph;
+    B200ST_TRY(greedy_search(*mem[0].m, mem[0].buf, st0, ga, s));
+    beam1_score_kernel<<<(st0.B + 255) / 256, 256, 0, s>>>(a.out_logprob, a.out_len, a.out_scores, st0.B, a.length_penalty);
+    B200ST_CUDA(cudaGetLastError());
+    return 0;
   }
-  // The dynamic shared-memory limit is an attribute of the kernel, not of the launch: set member after member, a member with
-  // a smaller head or model width would lower it below what an earlier member's attention launch needs.  So each attention
-  // kernel is raised once, to the largest need over the members, before the first step (and the capture).
-  B200ST_TRY(raise_beam_smem(smem_self, smem_cross));
-  if (rows > MAXB) B200ST_TRY(rows_raise_smem(rows_self, rows_cross));
+  SearchRows prep;
+  B200ST_TRY(prepare_search(mem, n, beam, a.max_steps, "beam_size", "beam search", s, &prep));
+  const int rows = prep.rows;
   EnsembleMix mix{};
   mix.n = n;
   for (int i = 0; i < n; ++i) {
-    mix.z[i] = logits[i];
+    mix.z[i] = prep.logits[i];
     mix.logw[i] = (float)std::log((double)mem[i].weight / wsum);       // a zero weight: -inf, which contributes nothing
   }
   const BeamState bs = beam_state_at(a.state_words, rows, st0.max_len);
   beam_init_kernel<<<(rows + 255) / 256, 256, 0, s>>>(bs, a.bos_ids, rows, beam);
   B200ST_CUDA(cudaGetLastError());
   auto one_step = [&]() -> int {
-    for (int i = 0; i < n; ++i) B200ST_TRY(step_dispatch(ctx[i], bs.ids, bs.time, logits[i], bs.anc, beam));
-    ensemble_logprob(mix, rows, V, s);
-    beam_select_logprobs(logits[0], bs, st0.B, beam, V, a.eos_id, a.unk_id, a.min_len, a.length_penalty, st0.max_len, s);
+    for (int i = 0; i < n; ++i) B200ST_TRY(step_dispatch(prep.ctx[i], bs.ids, bs.time, prep.logits[i], bs.anc, beam));
+    if (n > 1) {
+      ensemble_logprob(mix, rows, V, s);
+      beam_select_logprobs(prep.logits[0], bs, st0.B, beam, V, a.eos_id, a.unk_id, a.min_len, a.length_penalty, st0.max_len, s);
+    } else {
+      launch_pdl(beam_select_kernel<false>, st0.B, 1024, 0, s, (const float*)prep.logits[0], bs, beam, V, a.eos_id, a.unk_id,
+                 a.min_len, a.length_penalty, st0.max_len);
+      ++g_kernel_launches;
+    }
     B200ST_LAUNCH_CHECK();
     return 0;
   };
   bool graphed = false;
   B200ST_TRY(run_token_loop(s, a.max_steps, a.use_graph != 0, bs.all_finished, one_step, &graphed));
-  B200ST_CHECK(graphed || !a.use_graph, "ensemble beam search could not capture its step into a CUDA graph");
+  B200ST_CHECK(graphed || !a.use_graph, "beam search could not capture its step into a CUDA graph");
   beam_extract_kernel<<<st0.B, 256, 0, s>>>(bs, beam, a.top_k, a.length_penalty, a.eos_id, st0.max_len, a.max_steps, a.out_ids,
                                             a.out_scores, a.out_logprob, a.out_len);
   ++g_kernel_launches;

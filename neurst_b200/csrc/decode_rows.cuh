@@ -11,8 +11,9 @@ int64_t rows_scratch_floats(const Config& c, int B);
 int64_t rows_logits_offset(const Config& c, int B);
 // Checks what the wide step needs beyond check_state (shadow, dims, shared memory); nothing is launched.
 int rows_check(const Model& m, const Buffers& buf, const DecodeState& st, int beam);
-// Dynamic shared memory of the wide step's self- and cross-attention kernels, and the call that sets both kernels' limits
-// (rows_check sets them for its own model; an ensemble sets them once to the largest need of its members)
+// Dynamic shared memory of the wide step's self- and cross-attention kernels, and the call that sets both kernels' limits.
+// A caller of rows_check sets them once, to the largest need of the models it steps: the limit belongs to the kernel, so
+// setting it model after model could lower it below an earlier model's need.
 size_t rows_self_smem(const Config& c, int max_len);
 size_t rows_cross_smem(const Config& c, int Tm, int beam);
 int rows_raise_smem(size_t self_bytes, size_t cross_bytes);

@@ -135,6 +135,63 @@ def decoder_step_logits(rt, symbols, cache, time):
     return logits
 
 
+def _search_steps(Tm, maximum_decode_length, extra_decode_length, minimum_decode_length):
+    """maximum_search_steps = max(min(T' + extra, maximum), minimum) (beam_search.py:366-372)."""
+    return max(min(Tm + extra_decode_length, maximum_decode_length), minimum_decode_length)
+
+
+def _bos(rt, bos_id, B):
+    """The first decoder input of each utterance: one id for all, or one per utterance."""
+    bos = torch.as_tensor(bos_id).to(device=rt.device, dtype=torch.int64).reshape(-1)
+    return (bos.repeat(B) if bos.numel() == 1 else bos).contiguous()
+
+
+def _state_words(rt, B, width, max_len, search):
+    """The search's device state words, b200st_beam_state_bytes(B, width, max_len) of them (>= 512 bytes)."""
+    nbytes = int(rt.lib.b200st_beam_state_bytes(rt.handle, B, width, max_len))
+    if nbytes <= 0:
+        raise L.B200STError("%s state sizing failed: %s" % (search, rt.lib.b200st_last_error().decode()))
+    return torch.zeros((nbytes + 7) // 8, dtype=torch.int64, device=rt.device)
+
+
+def _on_decode_stream(rt, call):
+    """L.check(call()) on rt's side stream, ordered after and before the current stream's work: the library captures the
+    step into a CUDA graph, which needs a real (non-legacy-default) stream.  `call` reads L._stream() when it runs."""
+    cur = torch.cuda.current_stream(rt.device)
+    side = getattr(rt, "_decode_stream", None)
+    if side is None:
+        side = rt._decode_stream = torch.cuda.Stream(device=rt.device)
+    side.wait_stream(cur)
+    with torch.cuda.stream(side):
+        L.check(call())
+    cur.wait_stream(side)
+
+
+def _pad_with_eos(out, steps, maximum_decode_length, eos_id):
+    """The first `steps` columns, padded to the fixed output length with EOS (beam_search.py:428-436, sampling.py:253-256)."""
+    out = out[:, :steps]
+    if steps < maximum_decode_length:
+        out = torch.cat([out, torch.full((out.shape[0], maximum_decode_length - steps), int(eos_id), dtype=torch.int64,
+                                         device=out.device)], 1)
+    return out
+
+
+def _search_cache(rt, inputs, cache, width, width_name, search, maximum_decode_length, use_shadow, wait_k):
+    """The caller's cache, checked to hold B * width rows, or the encoder pass over `inputs` and a new cache of B * width
+    rows."""
+    if cache is not None:
+        if cache.self_kv.shape[2] < cache.B * width:
+            raise L.B200STError("the decoding cache holds %d rows, %s needs %d"
+                                % (cache.self_kv.shape[2], search, cache.B * width))
+        return cache
+    B = int(inputs["src"].shape[0])
+    if B * width > max_rows(use_shadow):
+        raise L.B200STError("%s decodes at most %d rows (utterances x %s) per call, got %d x %d"
+                            % (search, max_rows(use_shadow), width_name, B, width))
+    enc, bias = encode(rt, inputs)
+    return create_decoding_cache(rt, enc, bias, maximum_decode_length, use_shadow, beam=width, wait_k=wait_k)
+
+
 def greedy_search(rt, inputs, bos_id, eos_id, unk_id=None, maximum_decode_length=256, extra_decode_length=50,
                   minimum_decode_length=0, enable_unk=False, use_shadow=False, use_graph=True, cache=None, persistent=True,
                   wait_k=0):
@@ -144,21 +201,13 @@ def greedy_search(rt, inputs, bos_id, eos_id, unk_id=None, maximum_decode_length
     if cache is None:
         enc, bias = encode(rt, inputs)
         cache = create_decoding_cache(rt, enc, bias, maximum_decode_length, use_shadow, wait_k=wait_k)
-    B, Tm = cache.B, cache.Tm
-    steps = max(min(Tm + extra_decode_length, maximum_decode_length), minimum_decode_length)
-    steps = min(steps, cache.max_len)
-    dev = rt.device
-    bos = torch.as_tensor(bos_id).to(device=dev, dtype=torch.int64).reshape(-1)
-    if bos.numel() == 1:
-        bos = bos.repeat(B)
-    bos = bos.contiguous()
-    out = torch.empty(B, steps, dtype=torch.int64, device=dev)
-    length = torch.zeros(B, dtype=torch.int32, device=dev)
-    logprob = torch.zeros(B, dtype=torch.float32, device=dev)
-    nbytes = int(rt.lib.b200st_beam_state_bytes(rt.handle, B, 1, cache.max_len))    # >= 512; holds B rows' words
-    if nbytes <= 0:
-        raise L.B200STError("greedy search state sizing failed: " + rt.lib.b200st_last_error().decode())
-    words = torch.zeros((nbytes + 7) // 8, dtype=torch.int64, device=dev)
+    B = cache.B
+    steps = min(_search_steps(cache.Tm, maximum_decode_length, extra_decode_length, minimum_decode_length), cache.max_len)
+    bos = _bos(rt, bos_id, B)
+    out = torch.empty(B, steps, dtype=torch.int64, device=rt.device)
+    length = torch.zeros(B, dtype=torch.int32, device=rt.device)
+    logprob = torch.zeros(B, dtype=torch.float32, device=rt.device)
+    words = _state_words(rt, B, 1, cache.max_len, "greedy search")       # holds B rows' words
     a = L.GreedyArgs()
     a.bos_ids, a.eos_id = bos.data_ptr(), int(eos_id)
     a.unk_id = -1 if (enable_unk or unk_id is None) else int(unk_id)
@@ -169,25 +218,11 @@ def greedy_search(rt, inputs, bos_id, eos_id, unk_id=None, maximum_decode_length
     # rows there is no persistent kernel: the library replays the captured graph instead
     a.state_words, a.use_graph = words.data_ptr(), (2 if (persistent and use_graph) else int(bool(use_graph)))
     bufs = _bufs(rt)
-    # the library captures the step into a CUDA graph: that needs a real (non-legacy-default) stream
-    cur = torch.cuda.current_stream(dev)
-    side = getattr(rt, "_decode_stream", None)
-    if side is None:
-        side = rt._decode_stream = torch.cuda.Stream(device=dev)
-    side.wait_stream(cur)
-    with torch.cuda.stream(side):
-        L.check(rt.lib.b200st_greedy_search(rt.handle, C.byref(bufs), C.byref(cache.state), C.byref(a), L._stream()))
-    cur.wait_stream(side)
+    _on_decode_stream(rt, lambda: rt.lib.b200st_greedy_search(rt.handle, C.byref(bufs), C.byref(cache.state), C.byref(a),
+                                                              L._stream()))
     if use_graph and int(rt.lib.b200st_greedy_used_graph()) < 1:
         raise L.B200STError("greedy search could neither run its persistent kernel nor capture its step graph")
-    if steps < maximum_decode_length:      # padded to the fixed output length with EOS (beam_search.py:428-436)
-        out = torch.cat([out, torch.full((B, maximum_decode_length - steps), int(eos_id), dtype=torch.int64, device=dev)], 1)
-    return out, logprob, length
-
-
-def _search_steps(Tm, maximum_decode_length, extra_decode_length, minimum_decode_length):
-    """maximum_search_steps = max(min(T' + extra, maximum), minimum) (beam_search.py:366-372)."""
-    return max(min(Tm + extra_decode_length, maximum_decode_length), minimum_decode_length)
+    return _pad_with_eos(out, steps, maximum_decode_length, eos_id), logprob, length
 
 
 def beam_search(rt, inputs, bos_id, eos_id, unk_id=None, beam_size=4, length_penalty=0.6, top_k=1, maximum_decode_length=256,
@@ -197,62 +232,9 @@ def beam_search(rt, inputs, bos_id, eos_id, unk_id=None, beam_size=4, length_pen
     padded with EOS, scores fp32 [B*top_k] = logprob * length penalty, best first per utterance, accumulated log-probabilities
     [B*top_k], decoding lengths [B*top_k]).  length_penalty < 0 (or None) scores by 1/length.  At most
     max_rows(use_shadow) // beam_size utterances per call, and beam_size <= 8.  beam_size 1 is the greedy search (with its persistent kernel when use_graph)."""
-    beam_size, top_k = int(beam_size), int(top_k)
-    if beam_size < 1:
-        raise L.B200STError("beam_size must be >= 1, got %d" % beam_size)
-    if not 1 <= top_k <= beam_size:
-        raise L.B200STError("top_k must be in 1..beam_size (%d), got %d" % (beam_size, top_k))
-    if minimum_decode_length >= maximum_decode_length:          # BeamSearch.call (beam_search.py:531-532)
-        raise L.B200STError("minimum_decode_length must be less than maximum_decode_length")
-    alpha = -1.0 if length_penalty is None else float(length_penalty)
-    if cache is None:
-        B = int(inputs["src"].shape[0])
-        if B * beam_size > max_rows(use_shadow):
-            raise L.B200STError("beam search decodes at most %d rows (utterances x beam_size) per call, got %d x %d"
-                                % (max_rows(use_shadow), B, beam_size))
-        enc, bias = encode(rt, inputs)
-        cache = create_decoding_cache(rt, enc, bias, maximum_decode_length, use_shadow, beam=beam_size, wait_k=wait_k)
-    elif cache.self_kv.shape[2] < cache.B * beam_size:
-        raise L.B200STError("the decoding cache holds %d rows, beam search needs %d" % (cache.self_kv.shape[2], cache.B * beam_size))
-    B, Tm = cache.B, cache.Tm
-    steps = _search_steps(Tm, maximum_decode_length, extra_decode_length, minimum_decode_length)
-    dev = rt.device
-    bos = torch.as_tensor(bos_id).to(device=dev, dtype=torch.int64).reshape(-1)
-    if bos.numel() == 1:
-        bos = bos.repeat(B)
-    bos = bos.contiguous()
-    n = B * top_k
-    out = torch.empty(n, max(steps, 1), dtype=torch.int64, device=dev)
-    scores = torch.zeros(n, dtype=torch.float32, device=dev)
-    logprob = torch.zeros(n, dtype=torch.float32, device=dev)
-    length = torch.zeros(n, dtype=torch.int32, device=dev)
-    nbytes = int(rt.lib.b200st_beam_state_bytes(rt.handle, B, beam_size, cache.max_len))
-    if nbytes <= 0:
-        raise L.B200STError("beam search state sizing failed: " + rt.lib.b200st_last_error().decode())
-    words = torch.zeros((nbytes + 7) // 8, dtype=torch.int64, device=dev)
-    a = L.BeamArgs()
-    a.bos_ids, a.eos_id = bos.data_ptr(), int(eos_id)
-    a.unk_id = -1 if (enable_unk or unk_id is None) else int(unk_id)
-    a.min_len, a.max_steps = int(minimum_decode_length), int(steps)     # the library refuses steps beyond the cache
-    a.beam_size, a.top_k, a.length_penalty = beam_size, top_k, alpha
-    a.out_ids, a.out_scores, a.out_logprob, a.out_len = out.data_ptr(), scores.data_ptr(), logprob.data_ptr(), length.data_ptr()
-    a.state_words = words.data_ptr()
-    a.use_graph = (2 if beam_size == 1 else 1) if use_graph else 0
-    bufs = _bufs(rt)
-    cur = torch.cuda.current_stream(dev)
-    side = getattr(rt, "_decode_stream", None)
-    if side is None:
-        side = rt._decode_stream = torch.cuda.Stream(device=dev)
-    side.wait_stream(cur)
-    with torch.cuda.stream(side):
-        L.check(rt.lib.b200st_beam_search(rt.handle, C.byref(bufs), C.byref(cache.state), C.byref(a), L._stream()))
-    cur.wait_stream(side)
-    if beam_size == 1 and use_graph and int(rt.lib.b200st_greedy_used_graph()) < 1:
-        raise L.B200STError("greedy search could neither run its persistent kernel nor capture its step graph")
-    out = out[:, :steps]
-    if steps < maximum_decode_length:      # padded to the fixed output length with EOS (beam_search.py:428-436)
-        out = torch.cat([out, torch.full((n, maximum_decode_length - steps), int(eos_id), dtype=torch.int64, device=dev)], 1)
-    return out, scores, logprob, length
+    return _beam_search([rt], None, inputs, bos_id, eos_id, unk_id, beam_size, length_penalty, top_k, maximum_decode_length,
+                        extra_decode_length, minimum_decode_length, enable_unk, use_shadow, use_graph,
+                        None if cache is None else [cache], wait_k)
 
 
 def ensemble_weights(spec, n):
@@ -283,7 +265,14 @@ def ensemble_beam_search(rts, inputs, bos_id, eos_id, unk_id=None, weights="aver
     n = len(rts)
     if not 1 <= n <= L.ENSEMBLE_MAX_MODELS:
         raise L.B200STError("an ensemble has 1..%d members, got %d" % (L.ENSEMBLE_MAX_MODELS, n))
-    w = ensemble_weights(weights, n)
+    return _beam_search(rts, ensemble_weights(weights, n), inputs, bos_id, eos_id, unk_id, beam_size, length_penalty, top_k,
+                        maximum_decode_length, extra_decode_length, minimum_decode_length, enable_unk, use_shadow, use_graph,
+                        caches, 0)
+
+
+def _beam_search(rts, weights, inputs, bos_id, eos_id, unk_id, beam_size, length_penalty, top_k, maximum_decode_length,
+                 extra_decode_length, minimum_decode_length, enable_unk, use_shadow, use_graph, caches, wait_k):
+    """beam_search (weights None: b200st_beam_search of rts[0]) and ensemble_beam_search (b200st_ensemble_beam_search)."""
     beam_size, top_k = int(beam_size), int(top_k)
     if beam_size < 1:
         raise L.B200STError("beam_size must be >= 1, got %d" % beam_size)
@@ -291,67 +280,44 @@ def ensemble_beam_search(rts, inputs, bos_id, eos_id, unk_id=None, weights="aver
         raise L.B200STError("top_k must be in 1..beam_size (%d), got %d" % (beam_size, top_k))
     if minimum_decode_length >= maximum_decode_length:          # BeamSearch.call (beam_search.py:531-532)
         raise L.B200STError("minimum_decode_length must be less than maximum_decode_length")
-    alpha = -1.0 if length_penalty is None else float(length_penalty)
-    if caches is None:
-        B = int(inputs["src"].shape[0])
-        if B * beam_size > max_rows(use_shadow):
-            raise L.B200STError("beam search decodes at most %d rows (utterances x beam_size) per call, got %d x %d"
-                                % (max_rows(use_shadow), B, beam_size))
-        caches = []
-        for rt in rts:
-            enc, bias = encode(rt, inputs)
-            caches.append(create_decoding_cache(rt, enc, bias, maximum_decode_length, use_shadow, beam=beam_size))
-    caches = list(caches)
+    n = len(rts)
+    caches = [None] * n if caches is None else list(caches)
     if len(caches) != n:
         raise L.B200STError("%d decoding caches for %d ensemble members" % (len(caches), n))
-    for c in caches:
-        if c.self_kv.shape[2] < c.B * beam_size:
-            raise L.B200STError("the decoding cache holds %d rows, beam search needs %d" % (c.self_kv.shape[2], c.B * beam_size))
+    caches = [_search_cache(rt, inputs, c, beam_size, "beam_size", "beam search", maximum_decode_length, use_shadow, wait_k)
+              for rt, c in zip(rts, caches)]
     rt0, c0 = rts[0], caches[0]
-    B, Tm = c0.B, c0.Tm
-    steps = _search_steps(Tm, maximum_decode_length, extra_decode_length, minimum_decode_length)
-    dev = rt0.device
-    bos = torch.as_tensor(bos_id).to(device=dev, dtype=torch.int64).reshape(-1)
-    if bos.numel() == 1:
-        bos = bos.repeat(B)
-    bos = bos.contiguous()
+    B, dev = c0.B, rt0.device
+    steps = _search_steps(c0.Tm, maximum_decode_length, extra_decode_length, minimum_decode_length)
+    bos = _bos(rt0, bos_id, B)
     k = B * top_k
     out = torch.empty(k, max(steps, 1), dtype=torch.int64, device=dev)
     scores = torch.zeros(k, dtype=torch.float32, device=dev)
     logprob = torch.zeros(k, dtype=torch.float32, device=dev)
     length = torch.zeros(k, dtype=torch.int32, device=dev)
-    nbytes = int(rt0.lib.b200st_beam_state_bytes(rt0.handle, B, beam_size, c0.max_len))
-    if nbytes <= 0:
-        raise L.B200STError("beam search state sizing failed: " + rt0.lib.b200st_last_error().decode())
-    words = torch.zeros((nbytes + 7) // 8, dtype=torch.int64, device=dev)
+    words = _state_words(rt0, B, beam_size, c0.max_len, "beam search")
     a = L.BeamArgs()
     a.bos_ids, a.eos_id = bos.data_ptr(), int(eos_id)
     a.unk_id = -1 if (enable_unk or unk_id is None) else int(unk_id)
-    a.min_len, a.max_steps = int(minimum_decode_length), int(steps)
-    a.beam_size, a.top_k, a.length_penalty = beam_size, top_k, alpha
+    a.min_len, a.max_steps = int(minimum_decode_length), int(steps)     # the library refuses steps beyond the cache
+    a.beam_size, a.top_k, a.length_penalty = beam_size, top_k, -1.0 if length_penalty is None else float(length_penalty)
     a.out_ids, a.out_scores, a.out_logprob, a.out_len = out.data_ptr(), scores.data_ptr(), logprob.data_ptr(), length.data_ptr()
     a.state_words = words.data_ptr()
-    # one member is beam_search itself, whose beam 1 is the greedy search with its persistent kernel
+    # one model's beam 1 is the greedy search, with its persistent kernel
     a.use_graph = (2 if beam_size == 1 else 1) if use_graph else 0
     bufs = [_bufs(rt) for rt in rts]
-    members = (L.EnsembleMember * n)()
-    for i, (rt, c) in enumerate(zip(rts, caches)):
-        members[i].h, members[i].buf, members[i].st = rt.handle, C.pointer(bufs[i]), C.pointer(c.state)
-        members[i].weight = w[i]
-    cur = torch.cuda.current_stream(dev)
-    side = getattr(rt0, "_decode_stream", None)
-    if side is None:
-        side = rt0._decode_stream = torch.cuda.Stream(device=dev)
-    side.wait_stream(cur)
-    with torch.cuda.stream(side):
-        L.check(rt0.lib.b200st_ensemble_beam_search(members, n, C.byref(a), L._stream()))
-    cur.wait_stream(side)
+    if weights is None:
+        _on_decode_stream(rt0, lambda: rt0.lib.b200st_beam_search(rt0.handle, C.byref(bufs[0]), C.byref(c0.state), C.byref(a),
+                                                                  L._stream()))
+    else:
+        members = (L.EnsembleMember * n)()
+        for i, (rt, c) in enumerate(zip(rts, caches)):
+            members[i].h, members[i].buf, members[i].st = rt.handle, C.pointer(bufs[i]), C.pointer(c.state)
+            members[i].weight = weights[i]
+        _on_decode_stream(rt0, lambda: rt0.lib.b200st_ensemble_beam_search(members, n, C.byref(a), L._stream()))
     if n == 1 and beam_size == 1 and use_graph and int(rt0.lib.b200st_greedy_used_graph()) < 1:
         raise L.B200STError("greedy search could neither run its persistent kernel nor capture its step graph")
-    out = out[:, :steps]
-    if steps < maximum_decode_length:      # padded to the fixed output length with EOS (beam_search.py:428-436)
-        out = torch.cat([out, torch.full((k, maximum_decode_length - steps), int(eos_id), dtype=torch.int64, device=dev)], 1)
-    return out, scores, logprob, length
+    return _pad_with_eos(out, steps, maximum_decode_length, eos_id), scores, logprob, length
 
 
 DEFAULT_SAMPLING_SEED = 1234      # the entries' default random_seed
@@ -379,30 +345,16 @@ def sampling_search(rt, inputs, bos_id, eos_id, unk_id, sample_num=1, top_k=0, t
         raise ValueError("`minimum_decode_length` must be less than maximum decode length.")
     if not 1 <= sample_num <= 8:
         raise L.B200STError("sample_num must be in 1..8, got %d" % sample_num)
-    if cache is None:
-        B = int(inputs["src"].shape[0])
-        if B * sample_num > max_rows(use_shadow):
-            raise L.B200STError("sampling search decodes at most %d rows (utterances x sample_num) per call, got %d x %d"
-                                % (max_rows(use_shadow), B, sample_num))
-        enc, bias = encode(rt, inputs)
-        cache = create_decoding_cache(rt, enc, bias, maximum_decode_length, use_shadow, beam=sample_num, wait_k=wait_k)
-    elif cache.self_kv.shape[2] < cache.B * sample_num:
-        raise L.B200STError("the decoding cache holds %d rows, sampling needs %d" % (cache.self_kv.shape[2], cache.B * sample_num))
-    B, Tm = cache.B, cache.Tm
-    steps = _search_steps(Tm, maximum_decode_length, extra_decode_length, minimum_decode_length)
-    dev = rt.device
-    bos = torch.as_tensor(bos_id).to(device=dev, dtype=torch.int64).reshape(-1)
-    if bos.numel() == 1:
-        bos = bos.repeat(B)
-    bos = bos.contiguous()
+    cache = _search_cache(rt, inputs, cache, sample_num, "sample_num", "sampling search", maximum_decode_length, use_shadow,
+                          wait_k)
+    B, dev = cache.B, rt.device
+    steps = _search_steps(cache.Tm, maximum_decode_length, extra_decode_length, minimum_decode_length)
+    bos = _bos(rt, bos_id, B)
     n = B * sample_num
     out = torch.empty(n, max(steps, 1), dtype=torch.int64, device=dev)
     logprob = torch.zeros(n, dtype=torch.float32, device=dev)
     length = torch.zeros(n, dtype=torch.int32, device=dev)
-    nbytes = int(rt.lib.b200st_beam_state_bytes(rt.handle, B, sample_num, cache.max_len))
-    if nbytes <= 0:
-        raise L.B200STError("sampling search state sizing failed: " + rt.lib.b200st_last_error().decode())
-    words = torch.zeros((nbytes + 7) // 8, dtype=torch.int64, device=dev)
+    words = _state_words(rt, B, sample_num, cache.max_len, "sampling search")
     a = L.SamplingArgs()
     a.bos_ids, a.eos_id = bos.data_ptr(), int(eos_id)
     a.unk_id = -1 if unk_id is None else int(unk_id)
@@ -412,18 +364,9 @@ def sampling_search(rt, inputs, bos_id, eos_id, unk_id, sample_num=1, top_k=0, t
     a.out_ids, a.out_logprob, a.out_len = out.data_ptr(), logprob.data_ptr(), length.data_ptr()
     a.state_words, a.use_graph = words.data_ptr(), int(bool(use_graph))
     bufs = _bufs(rt)
-    cur = torch.cuda.current_stream(dev)
-    side = getattr(rt, "_decode_stream", None)
-    if side is None:
-        side = rt._decode_stream = torch.cuda.Stream(device=dev)
-    side.wait_stream(cur)
-    with torch.cuda.stream(side):
-        L.check(rt.lib.b200st_sampling_search(rt.handle, C.byref(bufs), C.byref(cache.state), C.byref(a), L._stream()))
-    cur.wait_stream(side)
-    out = out[:, :steps]
-    if steps < maximum_decode_length:      # padded to the fixed output length with EOS (sampling.py:253-256)
-        out = torch.cat([out, torch.full((n, maximum_decode_length - steps), int(eos_id), dtype=torch.int64, device=dev)], 1)
-    return out, logprob, length
+    _on_decode_stream(rt, lambda: rt.lib.b200st_sampling_search(rt.handle, C.byref(bufs), C.byref(cache.state), C.byref(a),
+                                                                L._stream()))
+    return _pad_with_eos(out, steps, maximum_decode_length, eos_id), logprob, length
 
 
 def sample_logits(logits, top_k=0, top_p=1.0, seed=DEFAULT_SAMPLING_SEED, row_offset=0, step=0):

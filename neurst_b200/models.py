@@ -274,6 +274,13 @@ class _EncoderDecoder:
                 "eos_id": trg_meta["eos_id"], "unk_id": trg_meta.get("unk_id")}
         return symbols_to_logits_fn, init
 
+    def _bos(self, inputs):
+        """The searches' first decoder input: trg_input when given, else BOS for every utterance."""
+        bos = inputs.get("trg_input")
+        if bos is None:
+            bos = torch.full((inputs["src"].shape[0],), int(self._trg_meta["bos_id"]), dtype=torch.long)
+        return bos
+
     def greedy_search(self, inputs, maximum_decode_length=256, extra_decode_length=50, minimum_decode_length=0, enable_unk=False,
                       use_shadow=False):
         """SequenceGenerator with search_method BeamSearch(beam_size=1) (neurst/exps/sequence_generator.py:62-86,
@@ -281,12 +288,9 @@ class _EncoderDecoder:
         At most decode.MAX_ROWS (8) utterances per call with the fp32 weights, decode.MAX_ROWS_SHADOW (256) with use_shadow."""
         from neurst_b200 import decode as D
         tm = self._trg_meta
-        B = inputs["src"].shape[0]
-        bos = inputs.get("trg_input")
-        if bos is None:
-            bos = torch.full((B,), int(tm["bos_id"]), dtype=torch.long)
-        ids, logprob, _ = D.greedy_search(self._rt, inputs, bos, tm["eos_id"], tm.get("unk_id"), maximum_decode_length,
-                                          extra_decode_length, minimum_decode_length, enable_unk, use_shadow, wait_k=self.lag(False))
+        ids, logprob, _ = D.greedy_search(self._rt, inputs, self._bos(inputs), tm["eos_id"], tm.get("unk_id"),
+                                          maximum_decode_length, extra_decode_length, minimum_decode_length, enable_unk,
+                                          use_shadow, wait_k=self.lag(False))
         return ids, logprob
 
     def beam_search(self, inputs, beam_size=4, length_penalty=0.6, top_k=1, maximum_decode_length=256, extra_decode_length=50,
@@ -297,13 +301,9 @@ class _EncoderDecoder:
         use_shadow (the 16-bit weights; beam_size <= 8)."""
         from neurst_b200 import decode as D
         tm = self._trg_meta
-        B = inputs["src"].shape[0]
-        bos = inputs.get("trg_input")
-        if bos is None:
-            bos = torch.full((B,), int(tm["bos_id"]), dtype=torch.long)
-        ids, scores, _, _ = D.beam_search(self._rt, inputs, bos, tm["eos_id"], tm.get("unk_id"), beam_size, length_penalty, top_k,
-                                          maximum_decode_length, extra_decode_length, minimum_decode_length, enable_unk, use_shadow,
-                                          wait_k=self.lag(False))
+        ids, scores, _, _ = D.beam_search(self._rt, inputs, self._bos(inputs), tm["eos_id"], tm.get("unk_id"), beam_size,
+                                          length_penalty, top_k, maximum_decode_length, extra_decode_length,
+                                          minimum_decode_length, enable_unk, use_shadow, wait_k=self.lag(False))
         return ids, scores
 
     def sampling_search(self, inputs, sample_num=1, top_k=0, top_p=1.0, maximum_decode_length=256, extra_decode_length=50,
@@ -315,13 +315,9 @@ class _EncoderDecoder:
         with use_shadow; sample_num <= 8."""
         from neurst_b200 import decode as D
         tm = self._trg_meta
-        B = inputs["src"].shape[0]
-        bos = inputs.get("trg_input")
-        if bos is None:
-            bos = torch.full((B,), int(tm["bos_id"]), dtype=torch.long)
-        ids, logprob, _ = D.sampling_search(self._rt, inputs, bos, tm["eos_id"], tm.get("unk_id"), sample_num, top_k, top_p,
-                                            maximum_decode_length, extra_decode_length, minimum_decode_length, seed, row_offset,
-                                            use_shadow, wait_k=self.lag(False))
+        ids, logprob, _ = D.sampling_search(self._rt, inputs, self._bos(inputs), tm["eos_id"], tm.get("unk_id"), sample_num,
+                                            top_k, top_p, maximum_decode_length, extra_decode_length, minimum_decode_length,
+                                            seed, row_offset, use_shadow, wait_k=self.lag(False))
         return ids, logprob
 
     def evaluate(self, inputs, is_training=False):
@@ -460,10 +456,7 @@ class EncoderDecoderEnsembleModel:
         return symbols_to_logits_fn, init
 
     def _bos(self, inputs):
-        bos = inputs.get("trg_input")
-        if bos is None:
-            bos = torch.full((inputs["src"].shape[0],), int(self._encoder_decoder_models[0]._trg_meta["bos_id"]), dtype=torch.long)
-        return bos
+        return self._encoder_decoder_models[0]._bos(inputs)
 
     def beam_search(self, inputs, beam_size=4, length_penalty=0.6, top_k=1, maximum_decode_length=256, extra_decode_length=50,
                     minimum_decode_length=0, enable_unk=False, ensemble_weights="average", use_shadow=False):
