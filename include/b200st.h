@@ -337,6 +337,44 @@ typedef struct b200st_optim_args_ {
   float growth_steps, multiplier;   /* 0 => 2000, 2 */
 } b200st_optim_args;
 int b200st_optimizer_step(b200st_handle h, const b200st_optim_args* a, void* stream);
+/* Weight pruning during training: the reference's pruning optimizer (neurst/sparsity/pruning_optimizer.py, built with
+ * keep_prune_property=True) around b200st_optimizer_step, with its schedules (neurst/sparsity/pruning_schedule.py).
+ * state[0] counts the updates applied in this run (the optimizer's iterations, from 1; a step the dynamic loss scale skips
+ * does not count).  A pruning turn is an applied update with step >= begin_step, (step <= end_step or end_step < 0) and
+ * (step - begin_step) % frequency == 0.  Off a turn: Adam, then w *= mask.  On a turn: Adam without the old mask, then per
+ * pruned tensor k = round(size * (1 - sparsity)) in float32 (half to even), threshold = the k-th largest |w| counting
+ * duplicates, mask = |w| >= threshold and w *= mask.  The sparsity is target_sparsity (B200ST_PRUNE_CONSTANT) or
+ * (initial - target) * (1 - clip((step - begin) / (end - begin), 0, 1)) ** polynomial_power + target (B200ST_PRUNE_POLYNOMIAL),
+ * in float32.  Masked weights are written as zero in the parameter and shadow arenas; their Adam moments keep moving, so a
+ * later turn can bring them back.  Gradients are never masked.  Nothing synchronises with the host. */
+#define B200ST_PRUNE_CONSTANT 0
+#define B200ST_PRUNE_POLYNOMIAL 1
+#define B200ST_PRUNE_MAX_TENSORS 512
+typedef struct {
+  uint8_t* mask;                /* device, numel / 8 bytes: bit j of byte b = 1 keeps element 8b + j; 1 outside the pruned
+                                 * tensors.  The owner derives it from weight != 0 when a run starts (masks are not checkpointed) */
+  const int32_t* tensor_ids;    /* host: the pruned tensors' indices (b200st_param_info order), each once */
+  int32_t n_tensors;            /* 1..B200ST_PRUNE_MAX_TENSORS */
+  int32_t schedule;             /* B200ST_PRUNE_CONSTANT or B200ST_PRUNE_POLYNOMIAL */
+  double initial_sparsity, target_sparsity;   /* float32(initial - target), taken in double, and float32(target) enter the
+                                               * float32 formula, as the reference's Python floats do */
+  float polynomial_power;
+  int64_t begin_step, end_step, frequency;
+  int32_t* state;               /* device int32[4], zero when a run starts: {applied updates, this update was a pruning turn,
+                                 * pruning turns so far, float bits of the last turn's sparsity} */
+  float* thresholds;            /* device float[n_tensors] or NULL: each tensor's |w| threshold at the last turn */
+  void* scratch;                /* device, b200st_prune_scratch_bytes(n_tensors) bytes, zero-filled once before the first call */
+} b200st_prune_args;
+int64_t b200st_prune_scratch_bytes(int32_t n_tensors);
+/* b200st_optimizer_step with pruning; the schedule is refused as the reference's constructors refuse it (and
+ * PolynomialDecay with end_step == begin_step), and so is a sparsity that leaves some pruned tensor with k == 0. */
+int b200st_optimizer_step_pruned(b200st_handle h, const b200st_optim_args* a, const b200st_prune_args* p, void* stream);
+/* The selection alone on n tensors of an arena: tensor i = params[offsets[i], offsets[i] + sizes[i]), offsets multiples of 8,
+ * each tensor's slot padded to a multiple of 8 elements.  k: device int64[n], 1 <= k[i] <= sizes[i].  Writes the mask bytes of
+ * the tensors, the thresholds (device float[n] or NULL) and zeroes the pruned elements of params and of the 16-bit shadow
+ * (or NULL).  scratch as for b200st_prune_args. */
+int b200st_prune_select(float* params, void* shadow, const int64_t* offsets, const int64_t* sizes, const int64_t* k, int32_t n,
+                        uint8_t* mask, float* thresholds, void* scratch, void* stream);
 /* legacy form: plain Keras Adam with a bf16 shadow, epsilon-hat form (neurst/optimizers/__init__.py:21; hparams speech_transformer.py:265-270):
  * g' = g*grad_scale; m,v update; p -= lr*sqrt(1-b2^t)/(1-b1^t) * m/(sqrt(v)+eps); optional bf16 shadow refresh + g=0 */
 int b200st_adam_step(float* params, float* grads, float* m, float* v, void* shadow, int64_t numel, float lr, float beta1,

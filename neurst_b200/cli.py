@@ -14,7 +14,9 @@ Host mirror of
 
 Keys understood (the ones of examples/speech_transformer/*/st_training_args.yml): entry.class / entry.params {train_steps,
 summary_steps, save_checkpoint_steps, update_cycle, clip_value, clip_norm, criterion.params.label_smoothing, optimizer.params,
-lr_schedule.params, pretrain_model}, dataset.class AudioTFRecordDataset / dataset.params, task.class SpeechToText /
+lr_schedule.params, pretrain_model, initial_global_step, pruning_schedule / pruning_schedule.params {initial_sparsity,
+target_sparsity, begin_pruning_step, end_pruning_step, pruning_frequency, polynomial_power} (or the same names as flat
+flags), pruning_variable_pattern, nopruning_variable_pattern}, dataset.class AudioTFRecordDataset / dataset.params, task.class SpeechToText /
 task.params, model.class / model.params / hparams_set, model_dir, dtype, and for `predict` the keys of the prediction
 recipes: `entry: predict` (the alias of entry.class) and search_method beam_search / search_method.params {beam_size,
 length_penalty, top_k, maximum_decode_length, extra_decode_length, minimum_decode_length, enable_unk} or search_method
@@ -581,8 +583,56 @@ def _resolve_text(cfg, ep, tp, world, entry, model_params, opt, lr, crit, waitk=
     return plan
 
 
+def _entry_key(cfg, ep, key):
+    """A trainer flag from entry.params, else from the top level of the configuration."""
+    v = ep.get(key)
+    return cfg.get(key) if v is None else v
+
+
+def resolve_pruning(cfg, ep):
+    """The trainer's weight pruning (exps/trainer.py:91-93,102-103,136-140): pruning_schedule (class, PolynomialDecay by
+    default) with pruning_schedule.params or the flat flags --initial_sparsity --target_sparsity --begin_pruning_step
+    --end_pruning_step --pruning_frequency --polynomial_power (a flat flag wins over the same key of the params), and
+    pruning_variable_pattern / nopruning_variable_pattern.  None when target_sparsity is 0 (PruningSchedule.new): the
+    trainer then runs the plain optimizer step."""
+    from neurst_b200 import pruning as PR
+    name = _entry_key(cfg, ep, "pruning_schedule.class") or _entry_key(cfg, ep, "pruning_schedule")
+    params = _entry_key(cfg, ep, "pruning_schedule.params")
+    if isinstance(name, dict):                 # pruning_schedule: {class: ..., params: {...}}
+        params = dict(name.get("params") or {}, **(params or {}))
+        name = name.get("class")
+    params = _as_dict(params, "pruning_schedule.params")
+    for k in PR.SCHEDULE_FLAGS:
+        v = _entry_key(cfg, ep, k)
+        if v is not None:
+            params[k] = v
+    try:
+        cls = PR.schedule_class(name or "PolynomialDecay")
+        if cls is PR.ConstantSparsity:
+            params = {k: v for k, v in params.items() if k not in ("initial_sparsity", "polynomial_power")}
+        schedule = PR.build_schedule(cls.__name__, params)
+    except (ValueError, TypeError) as e:
+        raise SystemExit("pruning_schedule: %s" % e)
+    if schedule is None:
+        return None
+    patterns = {k: _entry_key(cfg, ep, k) for k in ("pruning_variable_pattern", "nopruning_variable_pattern")}
+    for k, p in patterns.items():
+        if p is not None:
+            try:
+                re.compile(p)
+            except re.error as e:
+                raise SystemExit("%s %r: %s" % (k, p, e))
+    return dict(schedule=schedule, **patterns)
+
+
 def _finish_plan(plan, cfg, ep, tp, search_method, model_dirs, text=False):
-    """Prediction batch size, search, validator and ensemble settings shared by the speech and text plans."""
+    """Prediction batch size, search, validator and ensemble settings shared by the speech and text plans, and the trainer's
+    weight pruning and initial_global_step."""
+    plan["pruning"] = resolve_pruning(cfg, ep)
+    igs = _entry_key(cfg, ep, "initial_global_step")
+    plan["initial_global_step"] = None if igs is None else int(igs)
+    if plan["initial_global_step"] is not None and plan["initial_global_step"] < 0:
+        raise SystemExit("initial_global_step must be >= 0")
     # the task's configuration, recorded in model_configs.yml so that a model directory names its vocabularies
     plan["task_config"] = {"task.class": "Seq2Seq" if text else "SpeechToText", "task.params": dict(tp)}
     if ep.get("pretrain_variable_pattern") is not None:
@@ -812,10 +862,38 @@ def train(plan):
     world, rank, local = _dist_setup()
     model = _build_model(plan)
     start_step = initialise(model, plan)
+    # initial_global_step wins over a restored checkpoint's step (exps/trainer.py:172-178): the noam position, the checkpoint
+    # numbers and the validation steps count from it, and the run makes train_steps updates (the reference's steps_per_epoch)
+    igs = plan.get("initial_global_step")
+    end_step = plan["train_steps"] if igs is None else igs + plan["train_steps"]
+    if igs is not None:
+        start_step = igs
+    pruning = plan.get("pruning")
+    schedule = names = None
+    if pruning:
+        from neurst_b200.pruning import pruned_parameters
+        schedule = pruning["schedule"]
+        names = pruned_parameters(model.runtime.table, pruning["pruning_variable_pattern"], pruning["nopruning_variable_pattern"])
+        if not names:
+            raise SystemExit("pruning: the variable patterns select no parameter tensor")
+        LOG.info("Pruning: %s, %d of %d parameter tensors will be pruned", type(schedule).__name__, len(names),
+                 len(model.runtime.table))
     trainer = DataParallelTrainer(model, plan["optimizer"], plan["lr_schedule"], update_cycle=plan["update_cycle"],
                                   use_cuda_graph=True, clip_value=plan["clip_value"], clip_norm=plan["clip_norm"],
-                                  summary_steps=plan["summary_steps"] if rank == 0 else 0, logger=LOG.info)
+                                  summary_steps=plan["summary_steps"] if rank == 0 else 0, logger=LOG.info,
+                                  pruning_schedule=schedule, pruning_variables=names)
     trainer.global_step = start_step
+    if igs is not None:
+        # only the lr schedule, the checkpoints and validation read the initial step (compat.register_initial_step); the
+        # optimizer's iterations start at 0 in this run, so Adam's bias correction counts this run's updates from t = 1
+        trainer.adam_step_base = igs
+
+    def log_sparsity():
+        if schedule is not None and trainer._pruning_ready:
+            zeros, total = model.runtime.prune_sparsity()
+            LOG.info("Pruning: %d of %d weights of the pruned tensors are zero (sparsity %.4f)", zeros, total, zeros / total)
+            return zeros, total
+        return None
     trainer.broadcast_parameters()
     if rank == 0:
         write_model_configs(plan)
@@ -831,7 +909,7 @@ def train(plan):
     import itertools
     last = None
     early_stopped = False
-    micro_target = (plan["train_steps"] - start_step) * plan["update_cycle"]
+    micro_target = (end_step - start_step) * plan["update_cycle"]
     if micro_target > 0:
         # reading, parsing, padding and pinning of the next batches run in a background thread (tf.data prefetch's role)
         share = rank if plan.get("model_class") == "Transformer" else 0      # the text task's batches are global
@@ -849,6 +927,7 @@ def train(plan):
                     torch.cuda.synchronize()
                     save_checkpoint(model.runtime, plan["model_dir"], step, plan["max_to_keep"])
                     saved_at = step
+                    log_sparsity()
                 # the step's kernels (and its optimizer update) are done once validate() synchronises; the next step is
                 # launched only when this generator resumes, so every rank validates the same weights
                 if validator is not None and step > validated_at and validator.due(step):
@@ -862,10 +941,18 @@ def train(plan):
     torch.cuda.synchronize()
     if rank == 0 and trainer.global_step > start_step:
         save_checkpoint(model.runtime, plan["model_dir"], trainer.global_step, plan["max_to_keep"])
+    sparsity = log_sparsity() if rank == 0 else None
     if world > 1:
         trainer.close()
         torch.distributed.barrier()
     res = {"global_step": trainer.global_step, "loss": last}
+    if sparsity is not None:
+        # the schedule's device state: updates applied in this run, pruning turns, the last turn's sparsity
+        import struct
+        st = [int(x) for x in model.runtime.prune_state.cpu()]
+        res["pruning"] = {"zeros": sparsity[0], "weights": sparsity[1], "sparsity": sparsity[0] / sparsity[1],
+                          "updates": st[0], "turns": st[2], "turn_sparsity": struct.unpack("<f", struct.pack("<i", st[3]))[0],
+                          "tensors": len(names)}
     if validator is not None:
         res.update(early_stopped=early_stopped, validations=validator.history)
     return res

@@ -7,7 +7,9 @@
 #include <cstring>
 #include <cstdlib>
 #include "pdl.cuh"
+#include <algorithm>
 #include <cmath>
+#include <vector>
 
 namespace b200st {
 static thread_local std::string g_last_error;
@@ -325,6 +327,94 @@ int b200st_optimizer_step(b200st_handle h, const b200st_optim_args* a, void* str
     tt.n = 1; tt.off8[0] = 0; tt.off8[1] = (uint32_t)((a->numel + 7) >> 3);
   }
   return optimizer_step(o, tt, reinterpret_cast<cudaStream_t>(stream));
+}
+int64_t b200st_prune_scratch_bytes(int32_t n_tensors) {
+  if (n_tensors < 1 || n_tensors > B200ST_PRUNE_MAX_TENSORS) return -1;
+  return (int64_t)prune_scratch_bytes(n_tensors);
+}
+static_assert(B200ST_PRUNE_MAX_TENSORS == kPruneMaxTensors, "include/b200st.h and kernels.cuh disagree on the pruning table");
+// tensor i of the table: arena offset off[i] (a multiple of 8), size[i] elements
+static int fill_prune_table(const int64_t* off, const int64_t* size, int n, PruneTable& pt) {
+  if (n < 1 || n > kPruneMaxTensors) B200ST_FAIL("pruning takes 1.." + std::to_string(kPruneMaxTensors) + " tensors, got " + std::to_string(n));
+  pt.n = n;
+  uint32_t chunks = 0;
+  for (int i = 0; i < n; ++i) {
+    if (off[i] < 0 || off[i] % 8 != 0 || (off[i] >> 3) > 0xffffffffll) B200ST_FAIL("pruned tensor " + std::to_string(i) + ": offset must be a multiple of 8");
+    if (size[i] < 1 || size[i] > 0xffffffffll) B200ST_FAIL("pruned tensor " + std::to_string(i) + ": size must be 1..2^32-1");
+    pt.off8[i] = (uint32_t)(off[i] >> 3);
+    pt.size[i] = (uint32_t)size[i];
+    pt.cbase[i] = chunks;
+    const int64_t c = (size[i] + kPruneChunk - 1) / kPruneChunk;
+    if ((int64_t)chunks + c > 0xffffffffll) B200ST_FAIL("pruned tensors too large");
+    chunks += (uint32_t)c;
+  }
+  pt.cbase[n] = chunks;
+  return 0;
+}
+int b200st_optimizer_step_pruned(b200st_handle h, const b200st_optim_args* a, const b200st_prune_args* p, void* stream) {
+  if (!h || !a || !p) B200ST_FAIL("null argument");
+  if (!a->params || !a->grads || !a->m || !a->v) B200ST_FAIL("bad optimizer arguments");
+  if (!a->loss_scale_state && a->step_t < 1) B200ST_FAIL("step_t counts from 1");
+  if (a->numel != h->m.arena_numel) B200ST_FAIL("numel does not match the handle's parameter arena");
+  if (!p->mask || !p->state || !p->scratch || !p->tensor_ids) B200ST_FAIL("pruning needs mask, tensor_ids, state and scratch");
+  // the reference's constructors (pruning_schedule.py:48-57,152-157); end == begin would divide by zero in PolynomialDecay
+  if (p->schedule != B200ST_PRUNE_CONSTANT && p->schedule != B200ST_PRUNE_POLYNOMIAL) B200ST_FAIL("unknown pruning schedule");
+  if (p->begin_step < 0) B200ST_FAIL("begin_pruning_step should be >= 0");
+  if (p->end_step != -1 && p->end_step < p->begin_step) B200ST_FAIL("begin_pruning_step should be <= end_pruning_step if end_pruning_step != -1");
+  if (p->frequency <= 0) B200ST_FAIL("pruning_frequency should be > 0");
+  if (!(p->target_sparsity >= 0.0 && p->target_sparsity < 1.0)) B200ST_FAIL("target_sparsity must be in range [0,1)");
+  const bool poly = p->schedule == B200ST_PRUNE_POLYNOMIAL;
+  if (poly && !(p->initial_sparsity >= 0.0 && p->initial_sparsity < 1.0)) B200ST_FAIL("initial_sparsity must be in range [0,1)");
+  if (poly && p->end_step < 0) B200ST_FAIL("end_pruning_step must > 0 when using PolynomialDecay.");
+  if (poly && p->end_step == p->begin_step) B200ST_FAIL("PolynomialDecay needs end_pruning_step > begin_pruning_step");
+  const int n = p->n_tensors;
+  if (n < 1 || n > kPruneMaxTensors) B200ST_FAIL("pruning takes 1.." + std::to_string(kPruneMaxTensors) + " tensors, got " + std::to_string(n));
+  std::vector<int64_t> off(n), size(n);
+  std::vector<char> seen(h->m.params.size(), 0);
+  // the largest sparsity the schedule reaches (PolynomialDecay moves monotonically from initial to target)
+  const float smax = (float)(poly ? std::max(p->initial_sparsity, p->target_sparsity) : p->target_sparsity);
+  for (int i = 0; i < n; ++i) {
+    const int id = p->tensor_ids[i];
+    if (id < 0 || id >= (int)h->m.params.size() || seen[id]) B200ST_FAIL("tensor_ids: bad or repeated index " + std::to_string(id));
+    seen[id] = 1;
+    const ParamInfo& pi = h->m.params[id];
+    off[i] = pi.offset;
+    size[i] = pi.numel;
+    if (std::nearbyint((float)pi.numel * (1.f - smax)) < 1.f)
+      B200ST_FAIL("pruning " + pi.name + " (" + std::to_string(pi.numel) + " elements) at sparsity " + std::to_string(smax) +
+                  " keeps k = 0 weights: lower the sparsity or leave the tensor out");
+  }
+  PruneTable pt{};
+  B200ST_TRY(fill_prune_table(off.data(), size.data(), n, pt));
+  PruneSchedule sc{};
+  sc.polynomial = poly ? 1 : 0;
+  // pruning_schedule.py:173-174: the Python floats' difference, then float32 (a float32 subtraction can differ by an ulp)
+  sc.delta = poly ? (float)(p->initial_sparsity - p->target_sparsity) : 0.f;
+  sc.target = (float)p->target_sparsity;
+  sc.power = p->polynomial_power;
+  sc.begin = p->begin_step; sc.end = p->end_step; sc.frequency = p->frequency;
+  PruneDev pd{p->mask, p->state, p->thresholds, reinterpret_cast<uint32_t*>(p->scratch)};
+  OptimArgs o{};
+  o.p = a->params; o.g = a->grads; o.m = a->m; o.v = a->v;
+  o.shadow = a->shadow; o.shadow_dtype = a->shadow_dtype;
+  o.n = a->numel;
+  o.lr = a->lr; o.beta1 = a->beta1; o.beta2 = a->beta2; o.eps = a->eps; o.step_t = a->step_t;
+  o.grad_scale = a->grad_scale; o.zero_grad = a->zero_grad;
+  o.clip_value = a->clip_value; o.clip_norm = a->clip_norm;
+  o.tensor_sumsq = a->tensor_sumsq; o.ctl = a->loss_scale_state;
+  o.growth_steps = a->growth_steps; o.multiplier = a->multiplier;
+  TensorTable tt{};
+  fill_tensor_table(h->m, tt);
+  return optimizer_step_pruned(o, tt, pt, sc, pd, reinterpret_cast<cudaStream_t>(stream));
+}
+int b200st_prune_select(float* params, void* shadow, const int64_t* offsets, const int64_t* sizes, const int64_t* k, int32_t n,
+                        uint8_t* mask, float* thresholds, void* scratch, void* stream) {
+  if (!params || !offsets || !sizes || !k || !mask || !scratch) B200ST_FAIL("null argument");
+  if ((reinterpret_cast<uintptr_t>(params) & 31) != 0) B200ST_FAIL("params must be 32-byte aligned");
+  PruneTable pt{};
+  B200ST_TRY(fill_prune_table(offsets, sizes, n, pt));
+  PruneDev pd{mask, nullptr, thresholds, reinterpret_cast<uint32_t*>(scratch)};
+  return prune_select(params, shadow, pt, k, pd, reinterpret_cast<cudaStream_t>(stream));
 }
 int b200st_adam_step(float* params, float* grads, float* m, float* v, void* shadow, int64_t numel, float lr, float beta1,
                      float beta2, float eps, int64_t step_t, float grad_scale, int32_t zero_grad, void* stream) {

@@ -1,5 +1,5 @@
 // Host launchers of the non-GEMM kernels (LayerNorm, softmax, dropout casts, reductions, positions,
-// embedding, label-smoothed CE, Adam, conv front-end).  All activations are `dtype`-tagged raw pointers
+// embedding, label-smoothed CE, Adam, weight pruning, conv front-end).  All activations are `dtype`-tagged raw pointers
 // (F32 in the fp32 parity mode, BF16 in the wgmma mode); statistics, residual stream, gradients of
 // parameters and the loss are always fp32.
 #pragma once
@@ -113,6 +113,48 @@ struct OptimArgs {
   float growth_steps, multiplier;     // revised_dynamic_loss_scale.py:82-107 (2000, 2)
 };
 int optimizer_step(const OptimArgs& a, const TensorTable& tt, cudaStream_t s);
+
+// ---- weight pruning (prune.cu) ----------------------------------------------------------------------------------------
+// The pruned tensors travel as a kernel argument like TensorTable.  The selection works in chunks of kPruneChunk elements
+// that never straddle two tensors: tensor i owns chunks [cbase[i], cbase[i+1]).
+constexpr int kPruneMaxTensors = 512;
+constexpr int kPruneChunk = 16384;
+constexpr int kPruneBins = 2048;          // histogram bins of the widest radix digit (11 bits)
+constexpr int kPruneScratchHead = 1152;   // uint32 words before the histograms: rank[512], prefix[512], turn word
+struct PruneTable {
+  int n;
+  uint32_t off8[kPruneMaxTensors];        // arena offset / 8
+  uint32_t size[kPruneMaxTensors];        // elements (the alignment padding after a tensor is not part of it)
+  uint32_t cbase[kPruneMaxTensors + 1];
+};
+struct PruneSchedule {                    // neurst/sparsity/pruning_schedule.py
+  int polynomial;
+  float delta, target, power;             // delta = float32(initial - target) with the difference taken in double
+  int64_t begin, end, frequency;
+};
+// Device words of the pruned step.  state: int32[4] = {updates applied in this run (the schedule's step), this update is a
+// pruning turn, pruning turns so far, float bits of the last turn's sparsity}.  scratch: uint32 words, zero-filled once by the
+// owner: rank[512] (remaining rank of the k-th largest inside the digits chosen so far), prefix[512] (those digits: at the
+// end of a turn the threshold's bit pattern), turn word of prune_select, then n x kPruneBins histogram counts, which every
+// pass leaves zeroed for the next one.
+struct PruneDev {
+  uint8_t* mask;                          // bit j of byte b: element 8b + j is kept
+  int32_t* state;
+  float* thresholds;                      // [n] or null
+  uint32_t* scratch;
+};
+size_t prune_scratch_bytes(int n);
+int check_prune_table(const PruneTable& pt);
+// control step after the loss-scale control: advances the schedule's step on an applied update (ctl null: every update),
+// decides the turn and, on a turn, each tensor's k = round(size * (1 - sparsity)) in float32
+int prune_control(const PruneTable& pt, const PruneSchedule& sc, const float* ctl, const PruneDev& pd, cudaStream_t s);
+// when *turn != 0: the k-th largest |w| of every tensor (radix select, 3 digit passes), then mask = |w| >= threshold and the
+// pruned elements of p and of the 16-bit shadow (or null) set to zero.  Off-turn every kernel exits at once.
+int prune_select_apply(float* p, void* shadow, const PruneTable& pt, const PruneDev& pd, const int32_t* turn, cudaStream_t s);
+// the selection with host-given k (tests, bench): seeds rank / prefix / the turn word, then prune_select_apply
+int prune_select(float* p, void* shadow, const PruneTable& pt, const int64_t* k, const PruneDev& pd, cudaStream_t s);
+int optimizer_step_pruned(const OptimArgs& a, const TensorTable& tt, const PruneTable& pt, const PruneSchedule& sc,
+                          const PruneDev& pd, cudaStream_t s);
 int cast_f32_to_16(const float* x, void* y, int y_dtype, int64_t n, cudaStream_t s);
 // out[g] = keep-bits of elements [8g, 8g+8) of the dropout site (identical to the on-the-fly Philox decisions)
 int dropout_bits(DropoutSpec drop, int64_t n_elems, uint8_t* out, cudaStream_t s);

@@ -1,6 +1,7 @@
 // Optimizer step of the training loop: gradient statistics (per-tensor sum of squares + finite check), dynamic loss-scale
 // control, clip-by-value / per-tensor clip-by-norm and the Keras Adam update with the 16-bit shadow refresh — HBM-bound
-// streaming kernels over the flat arenas (34 B per parameter for Adam, 4 B for the statistics pass).
+// streaming kernels over the flat arenas (34 B per parameter for Adam, 4 B for the statistics pass); the pruned step adds
+// the weight mask (1 bit per parameter) to the Adam pass and the selection kernels of prune.cu.
 //
 // Reference: GradAccumKerasModel.train_step (neurst/training/gradaccum_keras_model.py:222-240): unscale -> clip_by_value
 // or clip_by_norm per gradient tensor -> apply_gradients; Keras Adam, epsilon-hat form (neurst/optimizers/__init__.py:21,
@@ -83,10 +84,16 @@ __global__ void step_control_kernel(float* __restrict__ sumsq, int n_tensors, fl
   }
 }
 
-template <bool CLIP_NORM>
-__global__ void __launch_bounds__(256) adam_kernel(const OptimArgs a, const __grid_constant__ TensorTable tt, float unscale_host) {
+// MASK (the pruned step): off a pruning turn, the elements whose bit of `mask` is 0 are written as zero in the master and
+// shadow arenas after their update (their Adam moments still move, so a later turn can bring them back); on a turn
+// (*turn != 0) the mask is not applied, the selection that follows sets the new one.
+template <bool CLIP_NORM, bool MASK>
+__global__ void __launch_bounds__(256) adam_kernel(const OptimArgs a, const __grid_constant__ TensorTable tt, float unscale_host,
+                                                   const uint8_t* __restrict__ mask, const int32_t* __restrict__ turn) {
   pdl_wait();
   pdl_trigger();
+  bool apply_mask = false;
+  if constexpr (MASK) apply_mask = *turn == 0;
   float gs = a.grad_scale * unscale_host;
   float t = (float)a.step_t;
   bool skip = false;
@@ -125,6 +132,13 @@ __global__ void __launch_bounds__(256) adam_kernel(const OptimArgs a, const __gr
       mi[j] = b1 * mo[j] + (1.f - b1) * gi[j];
       vi[j] = b2 * vo[j] + (1.f - b2) * gi[j] * gi[j];
       pi[j] = po[j] - lr_t * mi[j] / (sqrtf(vi[j]) + a.eps);
+    }
+    if constexpr (MASK) {
+      if (apply_mask) {
+        const uint32_t bits = mask[i >> 1] >> ((i & 1) * 4);     // the 4 elements of vector i: bits 4(i&1) .. 4(i&1)+3
+#pragma unroll
+        for (int j = 0; j < 4; ++j) if (!((bits >> j) & 1u)) pi[j] = 0.f;
+      }
     }
     reinterpret_cast<float4*>(a.m)[i] = make_float4(mi[0], mi[1], mi[2], mi[3]);
     reinterpret_cast<float4*>(a.v)[i] = make_float4(vi[0], vi[1], vi[2], vi[3]);
@@ -171,32 +185,65 @@ int cast_f32_to_16(const float* x, void* y, int y_dtype, int64_t n, cudaStream_t
   return 0;
 }
 
-int optimizer_step(const OptimArgs& a, const TensorTable& tt, cudaStream_t s) {
-  if (a.n == 0) return 0;
+// gradient statistics + loss-scale control when clip_norm or the dynamic loss scale needs them
+static int step_stats(const OptimArgs& a, const TensorTable& tt, cudaStream_t s) {
+  const bool need_stats = a.clip_norm > 0.f || a.ctl != nullptr;
+  if (!need_stats) return 0;
+  B200ST_CHECK(a.tensor_sumsq != nullptr, "clip_norm / dynamic loss scale need the tensor_sumsq scratch [n_tensors + 1]");
+  B200ST_CHECK(tt.n > 0 && tt.n <= 512, "clip_norm / dynamic loss scale support up to 512 parameter tensors");
+  B200ST_CHECK(a.n % 8 == 0, "clip_norm / dynamic loss scale need an arena padded to a multiple of 8 elements");
+  B200ST_CUDA(cudaMemsetAsync(a.tensor_sumsq, 0, sizeof(float) * (size_t)(tt.n + 1), s));
+  launch_pdl(grad_stats_kernel, grid_for(a.n, 8192, 132 * 8), 256, 0, s, (const float*)a.g, a.n, tt, a.tensor_sumsq);
+  ++g_kernel_launches;
+  if (a.ctl) { launch_pdl(latch_unscale_kernel, 1, 32, 0, s, a.ctl); ++g_kernel_launches; }
+  launch_pdl(step_control_kernel, 1, 32, 0, s, a.tensor_sumsq, tt.n, a.ctl, a.grad_scale, a.growth_steps > 0.f ? a.growth_steps : 2000.f,
+             a.multiplier > 1.f ? a.multiplier : 2.f);
+  ++g_kernel_launches;
+  B200ST_LAUNCH_CHECK();
+  return 0;
+}
+
+static int check_arenas(const OptimArgs& a) {
   B200ST_CHECK(((reinterpret_cast<uintptr_t>(a.p) | reinterpret_cast<uintptr_t>(a.g) | reinterpret_cast<uintptr_t>(a.m) |
                  reinterpret_cast<uintptr_t>(a.v)) & 15) == 0 && (reinterpret_cast<uintptr_t>(a.shadow) & 7) == 0,
                "optimizer: arenas must be 16-byte aligned");
   B200ST_CHECK(!a.shadow || is16(a.shadow_dtype), "optimizer: the shadow arena must be a 16-bit type");
-  const bool need_stats = a.clip_norm > 0.f || a.ctl != nullptr;
-  if (need_stats) {
-    B200ST_CHECK(a.tensor_sumsq != nullptr, "clip_norm / dynamic loss scale need the tensor_sumsq scratch [n_tensors + 1]");
-    B200ST_CHECK(tt.n > 0 && tt.n <= 512, "clip_norm / dynamic loss scale support up to 512 parameter tensors");
-    B200ST_CHECK(a.n % 8 == 0, "clip_norm / dynamic loss scale need an arena padded to a multiple of 8 elements");
-    B200ST_CUDA(cudaMemsetAsync(a.tensor_sumsq, 0, sizeof(float) * (size_t)(tt.n + 1), s));
-    launch_pdl(grad_stats_kernel, grid_for(a.n, 8192, 132 * 8), 256, 0, s, (const float*)a.g, a.n, tt, a.tensor_sumsq);
-    ++g_kernel_launches;
-    if (a.ctl) { launch_pdl(latch_unscale_kernel, 1, 32, 0, s, a.ctl); ++g_kernel_launches; }
-    launch_pdl(step_control_kernel, 1, 32, 0, s, a.tensor_sumsq, tt.n, a.ctl, a.grad_scale, a.growth_steps > 0.f ? a.growth_steps : 2000.f,
-               a.multiplier > 1.f ? a.multiplier : 2.f);
-    ++g_kernel_launches;
-    B200ST_LAUNCH_CHECK();
-  }
+  return 0;
+}
+
+int optimizer_step(const OptimArgs& a, const TensorTable& tt, cudaStream_t s) {
+  if (a.n == 0) return 0;
+  B200ST_TRY(check_arenas(a));
+  B200ST_TRY(step_stats(a, tt, s));
   const int grid = grid_for(a.n, 256 * 4 * 4);
-  if (a.clip_norm > 0.f) launch_pdl(adam_kernel<true>, grid, 256, 0, s, a, tt, 1.f);
-  else launch_pdl(adam_kernel<false>, grid, 256, 0, s, a, tt, 1.f);
+  const uint8_t* no_mask = nullptr;
+  const int32_t* no_turn = nullptr;
+  if (a.clip_norm > 0.f) launch_pdl(adam_kernel<true, false>, grid, 256, 0, s, a, tt, 1.f, no_mask, no_turn);
+  else launch_pdl(adam_kernel<false, false>, grid, 256, 0, s, a, tt, 1.f, no_mask, no_turn);
   ++g_kernel_launches;
   B200ST_LAUNCH_CHECK();
   return 0;
+}
+
+// The reference's pruning optimizer (neurst/sparsity/pruning_optimizer.py) inside the loss-scale optimizer: statistics and
+// loss-scale control, the pruning control (which sees whether this update is applied), Adam with the mask off-turn, and
+// the selection + new mask on a turn.  No host synchronisation: the turn is a device word every kernel reads.
+int optimizer_step_pruned(const OptimArgs& a, const TensorTable& tt, const PruneTable& pt, const PruneSchedule& sc,
+                          const PruneDev& pd, cudaStream_t s) {
+  B200ST_CHECK(a.n > 0 && a.n % 8 == 0, "the pruned step needs an arena padded to a multiple of 8 elements");
+  B200ST_CHECK(pd.mask && pd.state && pd.scratch, "the pruned step needs the mask, the state words and the scratch");
+  B200ST_TRY(check_arenas(a));
+  B200ST_TRY(check_prune_table(pt));
+  B200ST_TRY(step_stats(a, tt, s));
+  B200ST_TRY(prune_control(pt, sc, a.ctl, pd, s));
+  const int grid = grid_for(a.n, 256 * 4 * 4);
+  const uint8_t* mask = pd.mask;
+  const int32_t* turn = pd.state + 1;
+  if (a.clip_norm > 0.f) launch_pdl(adam_kernel<true, true>, grid, 256, 0, s, a, tt, 1.f, mask, turn);
+  else launch_pdl(adam_kernel<false, true>, grid, 256, 0, s, a, tt, 1.f, mask, turn);
+  ++g_kernel_launches;
+  B200ST_LAUNCH_CHECK();
+  return prune_select_apply(a.p, a.shadow, pt, pd, turn, s);
 }
 
 }  // namespace b200st

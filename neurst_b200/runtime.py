@@ -237,11 +237,12 @@ class Runtime:
         return out
 
     def adam_step(self, lr, step_t, beta1=0.9, beta2=0.98, eps=1e-9, grad_scale=1.0, zero_grad=True, clip_value=None,
-                  clip_norm=None, dynamic_loss_scale=None, growth_steps=2000, multiplier=2.0):
+                  clip_norm=None, dynamic_loss_scale=None, growth_steps=2000, multiplier=2.0, prune=None):
         """One optimizer step over the flat arenas (b200st_optimizer_step): unscale -> clip (per gradient tensor, as
         tf.clip_by_value / tf.clip_by_norm in gradaccum_keras_model.py:228-233) -> Keras Adam -> shadow refresh -> g = 0.
         fp16 precision: the gradients carry the dynamic loss scale; a step with non-finite gradients is skipped on the
-        device (state in `self.loss_scale_state`)."""
+        device (state in `self.loss_scale_state`).  `prune`: the schedule given to prune_setup(); the step is then
+        b200st_optimizer_step_pruned (mask off-turn, selection and new mask on a turn)."""
         if self.adam_m is None:
             self.adam_m = torch.zeros_like(self.params)
             self.adam_v = torch.zeros_like(self.params)
@@ -266,8 +267,94 @@ class Runtime:
                 self.loss_scale_state[0] = 1.0
             a.loss_scale_state = self.loss_scale_state.data_ptr()
             a.growth_steps, a.multiplier = float(growth_steps), float(multiplier)
-        L.check(self.lib.b200st_optimizer_step(self.handle, C.byref(a), L._stream()))
+        if prune is not None:
+            L.check(self.lib.b200st_optimizer_step_pruned(self.handle, C.byref(a), C.byref(self._prune_args(prune)), L._stream()))
+        else:
+            L.check(self.lib.b200st_optimizer_step(self.handle, C.byref(a), L._stream()))
         self._shadow_stale = False
+
+    # ---- weight pruning (b200st_optimizer_step_pruned) -----------------------------------------------------------------
+    def prune_setup(self, schedule, names):
+        """Pruning of the parameters `names` under `schedule` (neurst_b200.pruning) for the steps that follow: a fresh device
+        state (the schedule's step restarts at 0, as the reference's optimizer iterations do in a new run) and the mask
+        derived from the weights now in the arena (weight != 0, keep_prune_property=True): masks are not checkpointed, so
+        a resumed or pretrained run finds its pruned weights as zeros."""
+        from neurst_b200 import pruning as PR
+        if not names:
+            raise L.B200STError("pruning selects no parameter tensor")
+        if len(names) > L.PRUNE_MAX_TENSORS:
+            raise L.B200STError("pruning takes at most %d tensors, got %d" % (L.PRUNE_MAX_TENSORS, len(names)))
+        if self.numel % 8:
+            raise L.B200STError("pruning needs an arena padded to a multiple of 8 elements")
+        index = {k: i for i, k in enumerate(self.table)}
+        smax = schedule.max_sparsity()
+        for k in names:
+            size = self._numel_of(k)
+            if PR.k_of(size, smax) < 1:
+                raise L.B200STError("pruning %s (%d elements) at sparsity %g keeps no weight (k = 0): lower the sparsity or leave "
+                                    "the tensor out" % (k, size, float(smax)))
+        self.prune_names = list(names)
+        self.prune_schedule = schedule
+        self.prune_ids = (C.c_int32 * len(names))(*[index[k] for k in names])
+        self.prune_state = torch.zeros(4, dtype=torch.int32, device=self.device)
+        self.prune_thresholds = torch.zeros(len(names), dtype=torch.float32, device=self.device)
+        nbytes = int(self.lib.b200st_prune_scratch_bytes(len(names)))
+        self.prune_scratch = torch.zeros(nbytes, dtype=torch.uint8, device=self.device)
+        self.prune_mask = self.derive_prune_mask()
+        return self
+
+    def _numel_of(self, name):
+        n = 1
+        for s in self.table[name][1]:
+            n *= s
+        return n
+
+    def derive_prune_mask(self):
+        """Mask bitmap of the pruned set from the current weights: bit j of byte b keeps element 8b + j; 1 outside the pruned
+        tensors (and in the alignment padding after each), weight != 0 inside them.  Built tensor by tensor in uint8, so
+        the temporaries are the size of the largest pruned tensor's slot."""
+        mask = torch.full((self.numel // 8,), 0xFF, dtype=torch.uint8, device=self.device)
+        for k in self.prune_names:
+            off, _ = self.table[k]
+            n = self._numel_of(k)
+            n8 = (n + 7) // 8 * 8                        # the tensor's slot in the arena
+            nz = (self.params[off:off + n8] != 0).view(-1, 8)
+            if n8 > n:
+                nz[-1, n - n8 + 8:] = True
+            byte = torch.zeros(n8 // 8, dtype=torch.uint8, device=self.device)
+            for j in range(8):
+                byte |= nz[:, j].to(torch.uint8) << j
+            mask[off // 8:(off + n8) // 8] = byte
+        return mask
+
+    def _prune_args(self, prune):
+        from neurst_b200 import pruning as PR
+        if getattr(self, "prune_schedule", None) is not prune:
+            raise L.B200STError("adam_step(prune=...) needs prune_setup() with that schedule first")
+        sc = prune
+        p = L.PruneArgs()
+        p.mask = self.prune_mask.data_ptr()
+        p.tensor_ids = self.prune_ids
+        p.n_tensors = len(self.prune_names)
+        poly = isinstance(sc, PR.PolynomialDecay)
+        p.schedule = L.PRUNE_POLYNOMIAL if poly else L.PRUNE_CONSTANT
+        p.initial_sparsity = sc.initial_sparsity if poly else 0.0
+        p.target_sparsity = sc.target_sparsity
+        p.polynomial_power = sc.polynomial_power if poly else 0.0
+        p.begin_step, p.end_step, p.frequency = sc.begin_pruning_step, sc.end_pruning_step, sc.pruning_frequency
+        p.state = self.prune_state.data_ptr()
+        p.thresholds = self.prune_thresholds.data_ptr()
+        p.scratch = self.prune_scratch.data_ptr()
+        return p
+
+    def prune_sparsity(self):
+        """(zeros, elements) over the pruned tensors: a host reduction, for a point that is already synchronised."""
+        zeros = total = 0
+        for k in self.prune_names:
+            v = self.view(k)
+            zeros += int((v == 0).sum())
+            total += v.numel()
+        return zeros, total
 
     def dropout_mask(self, site, n, p, seed):
         sid = int(self.lib.b200st_dropout_stream_id(site.encode()))

@@ -50,7 +50,11 @@ class DataParallelTrainer:
     initial parameter broadcast and scalar metric reduction."""
 
     def __init__(self, model, optimizer_params=None, lr_schedule_params=None, update_cycle=1, grad_buckets=1,
-                 use_cuda_graph=False, clip_value=None, clip_norm=None, summary_steps=0, logger=None):
+                 use_cuda_graph=False, clip_value=None, clip_norm=None, summary_steps=0, logger=None, pruning_schedule=None,
+                 pruning_variables=None):
+        """`pruning_schedule` (neurst_b200.pruning, or None): prune the parameters `pruning_variables` (our names; all of them
+        when None) during training, as the reference's pruning optimizer does; a schedule with target_sparsity 0 prunes nothing.  The mask is derived from the weights at the
+        first update, after the rank-0 broadcast."""
         self.model = model
         self.rt = model.runtime
         op = optimizer_params or {}
@@ -58,6 +62,9 @@ class DataParallelTrainer:
         self.lr_params = lr_schedule_params or dict(dmodel=model.runtime.config.d, warmup_steps=4000, initial_factor=1.0)
         self.update_cycle = int(update_cycle)
         self.global_step = 0
+        # the global step at which the optimizer's iterations (Adam's t) count from 0: a run started at initial_global_step
+        # sets it, as the reference's optimizer starts its own iterations at 0 whatever the registered initial step
+        self.adam_step_base = 0
         self._micro = 0
         self.dist = torch.distributed if torch.distributed.is_available() and torch.distributed.is_initialized() else None
         self.world = self.dist.get_world_size() if self.dist else 1
@@ -74,6 +81,10 @@ class DataParallelTrainer:
         if self.lib_comm:
             self.rt.comm_init(self.dist)
         self.meter = ThroughputMeter(summary_steps, self.world, logger) if summary_steps else None
+        # target_sparsity 0 is no pruning (PruningSchedule.new returns None): the plain optimizer step
+        self.pruning_schedule = pruning_schedule if pruning_schedule is not None and pruning_schedule.target_sparsity > 0 else None
+        self.pruning_variables = None if pruning_variables is None else list(pruning_variables)
+        self._pruning_ready = False
 
     def close(self):
         """Collective-ordered shutdown of the in-library communicator (call on every rank before leaving the job)."""
@@ -135,7 +146,13 @@ class DataParallelTrainer:
             kw = {}
             if self.clip_value or self.clip_norm:
                 kw = dict(clip_value=self.clip_value, clip_norm=self.clip_norm)
-            self.rt.adam_step(lr, self.global_step, self.beta1, self.beta2, self.eps, grad_scale=scale, zero_grad=True, **kw)
+            if self.pruning_schedule is not None:
+                if not self._pruning_ready:
+                    names = list(self.rt.table) if self.pruning_variables is None else self.pruning_variables
+                    self.rt.prune_setup(self.pruning_schedule, names)
+                    self._pruning_ready = True
+                kw["prune"] = self.pruning_schedule
+            self.rt.adam_step(lr, self.global_step - self.adam_step_base, self.beta1, self.beta2, self.eps, grad_scale=scale, zero_grad=True, **kw)
             if self.meter is not None:
                 self.meter.step_end(self.global_step, out["loss"], lr)
         return out["loss"]
