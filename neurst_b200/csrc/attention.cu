@@ -630,10 +630,7 @@ int attention_fwd_fused(int dt, const void* q, int64_t q_ld, const void* k, int6
     attr[ai] = smem;
   }
   dim3 grid((Tq + BQ - 1) / BQ, H, B);
-  launch_pdl(kern, grid, kAttnThreads, smem, s, tq, tk, tv, p);
-  tc_count_launch();
-  B200ST_LAUNCH_CHECK();
-  return 0;
+  return launch(kern, grid, kAttnThreads, smem, s, tq, tk, tv, p);
 }
 
 
@@ -677,26 +674,19 @@ int attention_bwd_fused(int dt, const void* q, int64_t q_ld, const void* k, int6
   {
     int64_t gp = (rows + 7) / 8;
     if (gp > 132 * 8) gp = 132 * 8;
-    launch_pdl(dt == F16 ? attn_bwd_prep_kernel<F16> : attn_bwd_prep_kernel<BF16>, (int)gp, 256, 0, s,
-               reinterpret_cast<const uint16_t*>(ctx), ctx_ld, reinterpret_cast<const uint16_t*>(dctx), dctx_ld, dq_scratch, dvec, B, H, Tq);
-    g_kernel_launches += 1;
-    B200ST_LAUNCH_CHECK();
+    B200ST_TRY(launch(dt == F16 ? attn_bwd_prep_kernel<F16> : attn_bwd_prep_kernel<BF16>, (int)gp, 256, 0, s,
+                      reinterpret_cast<const uint16_t*>(ctx), ctx_ld, reinterpret_cast<const uint16_t*>(dctx), dctx_ld, dq_scratch, dvec, B, H, Tq));
   }
   dim3 grid((Tk + BKV - 1) / BKV, H, B);
   const bool causal = mask.on != 0;
   auto kern = causal ? (dt == F16 ? attn_bwd_kernel<true, F16> : attn_bwd_kernel<true, BF16>)
                      : (dt == F16 ? attn_bwd_kernel<false, F16> : attn_bwd_kernel<false, BF16>);
-  launch_pdl(kern, grid, kBwdThreads, kBwdSmem, s, tq, tk, tv, tdo, p);
-  B200ST_LAUNCH_CHECK();
+  B200ST_TRY(launch(kern, grid, kBwdThreads, kBwdSmem, s, tq, tk, tv, tdo, p));
   const int64_t n8 = rows * (H * DH / 8);
   int64_t g = (n8 + 255) / 256;
   if (g > 132 * 8) g = 132 * 8;
-  launch_pdl(dt == F16 ? cast_rows_kernel<F16> : cast_rows_kernel<BF16>, (int)g, 256, 0, s, dq_scratch, (int64_t)H * DH,
-             reinterpret_cast<uint16_t*>(dq), dq_ld, rows, H * DH);
-  tc_count_launch();
-  g_kernel_launches += 1;
-  B200ST_LAUNCH_CHECK();
-  return 0;
+  return launch(dt == F16 ? cast_rows_kernel<F16> : cast_rows_kernel<BF16>, (int)g, 256, 0, s, dq_scratch, (int64_t)H * DH,
+                reinterpret_cast<uint16_t*>(dq), dq_ld, rows, H * DH);
 }
 
 }  // namespace b200st

@@ -54,15 +54,15 @@ struct SampleRows {
 int check_sample_filter(int top_k, float top_p, int V);
 // sequence_sampling_search's initial state on rows = utterances x sample_num, the identity ancestry table and EOS-padded
 // output rows
-void sample_init(const BeamState& bs, const int64_t* bos, int rows, int sample_num, int max_len, int64_t* out, int max_steps,
-                 int eos, float* logprob, int32_t* length, cudaStream_t s);
-void sample_select(const SampleRows& a, int rows, cudaStream_t s);
+int sample_init(const BeamState& bs, const int64_t* bos, int rows, int sample_num, int max_len, int64_t* out, int max_steps,
+                int eos, float* logprob, int32_t* length, cudaStream_t s);
+int sample_select(const SampleRows& a, int rows, cudaStream_t s);
 
 // lp[r, v] = log sum_m w_m softmax(z_m[r])[v], written over member 0's logits (one block per row, members in order)
-void ensemble_logprob(const EnsembleMix& mix, int rows, int V, cudaStream_t s);
+int ensemble_logprob(const EnsembleMix& mix, int rows, int V, cudaStream_t s);
 // beam_select_kernel on rows that already hold log-probabilities (the ensemble's mixture)
-void beam_select_logprobs(const float* logprobs, const BeamState& bs, int utterances, int beam, int V, int eos, int unk, int min_len,
-                          float alpha, int max_len, cudaStream_t s);
+int beam_select_logprobs(const float* logprobs, const BeamState& bs, int utterances, int beam, int V, int eos, int unk, int min_len,
+                         float alpha, int max_len, cudaStream_t s);
 
 namespace {
 

@@ -6,7 +6,6 @@
 #include "model.cuh"
 #include <cstring>
 #include <cstdlib>
-#include "pdl.cuh"
 #include <algorithm>
 #include <cmath>
 #include <vector>
@@ -14,8 +13,13 @@
 namespace b200st {
 static thread_local std::string g_last_error;
 void set_last_error(const std::string& s) { g_last_error = s; }
-int64_t g_kernel_launches = 0;
-cudaError_t& pdl_launch_error() { static thread_local cudaError_t e = cudaSuccess; return e; }
+static int64_t n_launches = 0;
+void count_launch() { ++n_launches; }
+int launch_failed(cudaError_t e) {
+  cudaGetLastError();
+  set_last_error(std::string("kernel launch failed: ") + cudaGetErrorString(e));
+  return 1;
+}
 // B200ST_NO_PDL only drops the launch attribute (every kernel computes the same thing), so that torch.profiler kernel
 // times do not include the griddepcontrol.wait of a kernel launched early under its predecessor
 bool pdl_enabled() { static const bool on = getenv("B200ST_NO_PDL") == nullptr; return on; }
@@ -27,7 +31,7 @@ extern "C" {
 
 const char* b200st_last_error(void) { return g_last_error.c_str(); }
 int b200st_version(void) { return 202; }
-int64_t b200st_launch_count(void) { return g_kernel_launches + tc_launch_count(); }
+int64_t b200st_launch_count(void) { return n_launches; }
 
 static GemmOperand to_operand(const b200st_operand& o) {
   GemmOperand r;
@@ -498,8 +502,6 @@ extern "C" int b200st_dropout_mask(uint64_t seed, uint64_t stream_id, int64_t n,
   if (n == 0) return 0;
   int64_t g = (n + 255) / 256;
   if (g > 132 * 16) g = 132 * 16;
-  launch_pdl(b200st::dropout_mask_kernel, (int)g, 256, 0, reinterpret_cast<cudaStream_t>(stream), seed, stream_id, n, p, out);
-  B200ST_LAUNCH_CHECK();
-  return 0;
+  return launch(b200st::dropout_mask_kernel, (int)g, 256, 0, reinterpret_cast<cudaStream_t>(stream), seed, stream_id, n, p, out);
 }
 

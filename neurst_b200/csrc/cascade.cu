@@ -9,6 +9,7 @@
 #include "../../include/b200st.h"
 #include "common.cuh"
 #include "kernels.cuh"
+#include "pdl.cuh"
 
 #include <string>
 
@@ -64,10 +65,7 @@ static int cascade_source(const b200st_cascade_source_args& a, cudaStream_t s) {
   const int need = a.max_src_len > 0 && a.max_src_len < a.hyp_len + 1 ? a.max_src_len : a.hyp_len + 1;
   B200ST_CHECK(a.out_stride >= need, "cascade_source: out_stride " + std::to_string(a.out_stride) + " < the longest source " +
                std::to_string(need));
-  cascade_source_kernel<<<a.B, kCascadeThreads, 0, s>>>(a);
-  ++g_kernel_launches;
-  B200ST_CUDA(cudaGetLastError());
-  return 0;
+  return launch_serial(cascade_source_kernel, a.B, kCascadeThreads, 0, s, a);
 }
 
 }  // namespace b200st

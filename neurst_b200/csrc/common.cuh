@@ -37,15 +37,14 @@ void set_last_error(const std::string& s);
     int _r = (expr);                                                                       \
     if (_r != 0) return _r;                                                                \
   } while (0)
-cudaError_t& pdl_launch_error();
-#define B200ST_LAUNCH_CHECK()                                                              \
-  do {                                                                                     \
-    if (::b200st::pdl_launch_error() != cudaSuccess) {                                     \
-      cudaError_t _pe = ::b200st::pdl_launch_error();                                      \
-      ::b200st::pdl_launch_error() = cudaSuccess;                                          \
-      B200ST_FAIL(std::string("kernel launch failed: ") + cudaGetErrorString(_pe));        \
-    }                                                                                      \
-    B200ST_CUDA(cudaGetLastError());                                                       \
+// Runs the launch expression (0 or 1, as launch() in pdl.cuh returns) with T bound to the C++ type of dtype `dt`, and
+// returns from the caller when it fails.
+#define DISPATCH_DTYPE(dt, T, ...)                                                    \
+  do {                                                                                \
+    if ((dt) == F32) { using T = float; B200ST_TRY(__VA_ARGS__); }                    \
+    else if ((dt) == BF16) { using T = __nv_bfloat16; B200ST_TRY(__VA_ARGS__); }      \
+    else if ((dt) == F16) { using T = __half; B200ST_TRY(__VA_ARGS__); }              \
+    else B200ST_FAIL("bad dtype");                                                    \
   } while (0)
 
 // ---- dtype helpers -----------------------------------------------------------------------
@@ -72,6 +71,25 @@ __device__ __forceinline__ float2 unpack2_16(uint32_t u, int dt) {
   if (dt == F16) return __half22float2(*reinterpret_cast<const __half2*>(&u));
   return __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162*>(&u));
 }
+// 8 consecutive elements: 16 bytes of a 16-bit type `DT` -> fp32, and fp32 -> 32 bytes of fp32 / 16 bytes of a 16-bit type
+template <int DT> __device__ __forceinline__ void unpack8_16(const uint4& pk, float (&v)[8]) {
+  const uint32_t w[4] = {pk.x, pk.y, pk.z, pk.w};
+#pragma unroll
+  for (int i = 0; i < 4; ++i) { const float2 f = unpack2_16(w[i], DT); v[2 * i] = f.x; v[2 * i + 1] = f.y; }
+}
+template <typename T> __device__ __forceinline__ void store8(T* dst, const float (&v)[8]);
+template <> __device__ __forceinline__ void store8<float>(float* dst, const float (&v)[8]) {
+  *reinterpret_cast<float4*>(dst) = make_float4(v[0], v[1], v[2], v[3]);
+  *reinterpret_cast<float4*>(dst + 4) = make_float4(v[4], v[5], v[6], v[7]);
+}
+template <int DT> __device__ __forceinline__ void store8_16(void* dst, const float (&v)[8]) {
+  uint4 pk;
+  pk.x = pack2_16(v[0], v[1], DT); pk.y = pack2_16(v[2], v[3], DT);
+  pk.z = pack2_16(v[4], v[5], DT); pk.w = pack2_16(v[6], v[7], DT);
+  *reinterpret_cast<uint4*>(dst) = pk;
+}
+template <> __device__ __forceinline__ void store8<__nv_bfloat16>(__nv_bfloat16* dst, const float (&v)[8]) { store8_16<BF16>(dst, v); }
+template <> __device__ __forceinline__ void store8<__half>(__half* dst, const float (&v)[8]) { store8_16<F16>(dst, v); }
 
 __device__ __forceinline__ float load_as_f32(const void* p, int dtype, int64_t idx) {
   return dtype == F32 ? reinterpret_cast<const float*>(p)[idx]
@@ -184,5 +202,11 @@ __device__ __forceinline__ bool drop_keep1(const DropoutSpec& d, uint64_t e) {
 }
 
 static inline int ceil_div(int64_t a, int64_t b) { return (int)((a + b - 1) / b); }
+// blocks for `work` items at `per_block` items per block, clamped to [1, cap] (grid-stride kernels loop over the rest)
+static inline int grid_for(int64_t work, int per_block, int cap = 132 * 16) {
+  int64_t g = (work + per_block - 1) / per_block;
+  if (g < 1) g = 1;
+  return (int)(g > cap ? cap : g);
+}
 
 }  // namespace b200st

@@ -14,14 +14,6 @@
 
 namespace b200st {
 
-#define DISPATCH_DTYPE(dt, T, ...)                                   \
-  do {                                                               \
-    if ((dt) == F32) { using T = float; __VA_ARGS__; }               \
-    else if ((dt) == BF16) { using T = __nv_bfloat16; __VA_ARGS__; } \
-    else if ((dt) == F16) { using T = __half; __VA_ARGS__; }         \
-    else B200ST_FAIL("bad dtype");                                   \
-  } while (0)
-
 namespace {
 
 template <typename T> __device__ __forceinline__ void ld8(const T* src, float (&v)[8]);
@@ -29,30 +21,12 @@ template <> __device__ __forceinline__ void ld8<float>(const float* src, float (
   const float4 a = __ldg(reinterpret_cast<const float4*>(src)), b = __ldg(reinterpret_cast<const float4*>(src) + 1);
   v[0] = a.x; v[1] = a.y; v[2] = a.z; v[3] = a.w; v[4] = b.x; v[5] = b.y; v[6] = b.z; v[7] = b.w;
 }
-template <int DT> __device__ __forceinline__ void unpack8_16(const uint4& pk, float (&v)[8]) {
-  const uint32_t w[4] = {pk.x, pk.y, pk.z, pk.w};
-#pragma unroll
-  for (int i = 0; i < 4; ++i) { const float2 f = unpack2_16(w[i], DT); v[2 * i] = f.x; v[2 * i + 1] = f.y; }
-}
 template <> __device__ __forceinline__ void ld8<__nv_bfloat16>(const __nv_bfloat16* src, float (&v)[8]) {
   unpack8_16<BF16>(__ldg(reinterpret_cast<const uint4*>(src)), v);
 }
 template <> __device__ __forceinline__ void ld8<__half>(const __half* src, float (&v)[8]) {
   unpack8_16<F16>(__ldg(reinterpret_cast<const uint4*>(src)), v);
 }
-template <typename T> __device__ __forceinline__ void st8(T* dst, const float (&v)[8]);
-template <> __device__ __forceinline__ void st8<float>(float* dst, const float (&v)[8]) {
-  *reinterpret_cast<float4*>(dst) = make_float4(v[0], v[1], v[2], v[3]);
-  *reinterpret_cast<float4*>(dst + 4) = make_float4(v[4], v[5], v[6], v[7]);
-}
-template <int DT> __device__ __forceinline__ void st8_16(void* dst, const float (&v)[8]) {
-  uint4 pk;
-  pk.x = pack2_16(v[0], v[1], DT); pk.y = pack2_16(v[2], v[3], DT);
-  pk.z = pack2_16(v[4], v[5], DT); pk.w = pack2_16(v[6], v[7], DT);
-  *reinterpret_cast<uint4*>(dst) = pk;
-}
-template <> __device__ __forceinline__ void st8<__nv_bfloat16>(__nv_bfloat16* dst, const float (&v)[8]) { st8_16<BF16>(dst, v); }
-template <> __device__ __forceinline__ void st8<__half>(__half* dst, const float (&v)[8]) { st8_16<F16>(dst, v); }
 
 // 8 consecutive elements held in raw form (prefetch registers: 16 B for bf16, 32 B for fp32)
 template <typename T> struct Vec8;
@@ -117,7 +91,7 @@ __device__ __forceinline__ void store_row(T* p, int lane, int C, const float (&v
         float t[8];
 #pragma unroll
         for (int j = 0; j < 8; ++j) t[j] = v[8 * g + j];
-        st8<T>(p + c0, t);
+        store8<T>(p + c0, t);
       }
     }
   } else {
@@ -321,7 +295,7 @@ __global__ void __launch_bounds__(256, 2) conv1_fwd_c256_kernel(const float* __r
 #pragma unroll
       for (int i = 0; i < 8; ++i) z[i] = fmaxf(fmaf(z[i] * rstd, greg[i], bereg[i]), 0.f);
     }
-    st8<T>(y + pp * C + 8 * lane, z);
+    store8<T>(y + pp * C + 8 * lane, z);
   };
   float ring[RING];
 #pragma unroll
@@ -538,7 +512,7 @@ __global__ void __launch_bounds__(256, 2) conv1_bwd_xhat_c256_kernel(
       c1 *= (1.0f / C); c2s *= (1.0f / C);
 #pragma unroll
       for (int i = 0; i < 8; ++i) { d[i] = rs * (d[i] * greg[i] - c1 - xh[i] * c2s); a_db[i] += d[i]; }
-      st8<T>(dz1 + pp * C + 8 * lane, d);
+      store8<T>(dz1 + pp * C + 8 * lane, d);
       if (lane < K1p) col1[pp * K1p + lane] = from_f32<T>(lane < 9 ? cur.xv : 0.f);
     };
     // issue cursor (position whose loads are issued next) runs RING-1 positions ahead of the compute cursor `pos`
@@ -721,11 +695,6 @@ __global__ void __launch_bounds__(256) im2col_row_kernel(const T* __restrict__ y
 
 }  // namespace
 
-static int pick_grid(int64_t npos, int per_block, int cap) {
-  int64_t g = (npos + per_block - 1) / per_block;
-  return (int)(g < 1 ? 1 : (g > cap ? cap : g));
-}
-
 static int conv1_fwd_launch(const float* src, const float* w, const float* b, const float* gamma, const float* beta, float eps,
                             void* y1, int y_dtype, int B, int T, int F, int Cin, int C, int use_ln, float* rstd_out, cudaStream_t s);
 
@@ -746,29 +715,25 @@ static int conv1_fwd_launch(const float* src, const float* w, const float* b, co
   const int T1 = (T + 1) / 2, F1 = (F + 1) / 2;
   const int64_t npos = (int64_t)B * T1 * F1;
   if (npos == 0) return 0;
-  const int grid = pick_grid(npos, 8 * 4, 132 * 12);
+  const int grid = grid_for(npos, 8 * 4, 132 * 12);
   const bool vec = (C % 8 == 0) && ((reinterpret_cast<uintptr_t>(y1) & 15) == 0);
   if (vec && C == 256 && Cin == 1 && (use_ln || rstd_out) && ((reinterpret_cast<uintptr_t>(w) & 15) == 0) &&
       ((reinterpret_cast<uintptr_t>(b) & 15) == 0) && (rstd_out || (((reinterpret_cast<uintptr_t>(gamma) | reinterpret_cast<uintptr_t>(beta)) & 15) == 0))) {
-    const int grid1 = pick_grid(npos, 8 * 16, 132 * 2);
-    if (rstd_out) DISPATCH_DTYPE(y_dtype, TT, (launch_pdl(conv1_fwd_c256_kernel<TT, true>, grid1, 256, 0, s, src, w, b, gamma, beta, eps, (TT*)y1, rstd_out, B, T, F, T1, F1)));
-    else DISPATCH_DTYPE(y_dtype, TT, (launch_pdl(conv1_fwd_c256_kernel<TT, false>, grid1, 256, 0, s, src, w, b, gamma, beta, eps, (TT*)y1, rstd_out, B, T, F, T1, F1)));
-    ++g_kernel_launches;
-    B200ST_LAUNCH_CHECK();
+    const int grid1 = grid_for(npos, 8 * 16, 132 * 2);
+    if (rstd_out) DISPATCH_DTYPE(y_dtype, TT, (launch(conv1_fwd_c256_kernel<TT, true>, grid1, 256, 0, s, src, w, b, gamma, beta, eps, (TT*)y1, rstd_out, B, T, F, T1, F1)));
+    else DISPATCH_DTYPE(y_dtype, TT, (launch(conv1_fwd_c256_kernel<TT, false>, grid1, 256, 0, s, src, w, b, gamma, beta, eps, (TT*)y1, rstd_out, B, T, F, T1, F1)));
     return 0;
   }
   const size_t smem = (size_t)(9 * Cin + 1) * ((C + 255) & ~255) * sizeof(float);
   B200ST_CHECK(smem <= 48 * 1024, "conv1 filter does not fit the default shared memory");
 #define FWD(VEC, CPL, CIN1)                                                                                             \
-  DISPATCH_DTYPE(y_dtype, TT, (launch_pdl(conv1_fwd_kernel<TT, VEC, CPL, CIN1>, grid, 256, smem, s, src, w, b, gamma, beta, eps, (TT*)y1, \
+  DISPATCH_DTYPE(y_dtype, TT, (launch(conv1_fwd_kernel<TT, VEC, CPL, CIN1>, grid, 256, smem, s, src, w, b, gamma, beta, eps, (TT*)y1, \
                                                                                         B, T, F, Cin, C, T1, F1, use_ln, rstd_out)))
   if (vec && C <= 256) { if (Cin == 1) FWD(true, 8, true); else FWD(true, 8, false); }
   else if (vec) { if (Cin == 1) FWD(true, 16, true); else FWD(true, 16, false); }
   else if (C <= 256) { if (Cin == 1) FWD(false, 8, true); else FWD(false, 8, false); }
   else { if (Cin == 1) FWD(false, 16, true); else FWD(false, 16, false); }
 #undef FWD
-  ++g_kernel_launches;
-  B200ST_LAUNCH_CHECK();
   return 0;
 }
 
@@ -780,13 +745,13 @@ int conv1_bwd_fused(const float* src, const float* w, const float* b, const floa
   const int T1 = (T + 1) / 2, F1 = (F + 1) / 2, T2 = (T1 + 1) / 2, F2 = (F1 + 1) / 2;
   const int64_t npos = (int64_t)B * T1 * F1;
   if (npos == 0) return 0;
-  const int grid = pick_grid(npos, 8 * 4, 132 * 8);
+  const int grid = grid_for(npos, 8 * 4, 132 * 8);
   const size_t smem = (size_t)(9 * Cin + 1 + 3) * ((C + 255) & ~255) * sizeof(float);
   B200ST_CHECK(smem <= 48 * 1024, "conv1 filter does not fit the default shared memory");
   const bool vec = (C % 8 == 0) && ((reinterpret_cast<uintptr_t>(y1) & 15) == 0) && ((reinterpret_cast<uintptr_t>(dcol) & 15) == 0) &&
                    ((reinterpret_cast<uintptr_t>(dz1) & 15) == 0);
 #define BWD(VEC, CPL, CIN1)                                                                                             \
-  DISPATCH_DTYPE(dtype, TT, (launch_pdl(conv1_bwd_fused_kernel<TT, VEC, CPL, CIN1>, grid, 256, smem, s,                           \
+  DISPATCH_DTYPE(dtype, TT, (launch(conv1_bwd_fused_kernel<TT, VEC, CPL, CIN1>, grid, 256, smem, s,                           \
       src, w, b, gamma, beta, eps, (const TT*)y1, (const TT*)dcol, (TT*)dz1, (TT*)col1, K1p, db, dgamma, dbeta, B, T, F, Cin, C, \
       T1, F1, T2, F2, use_ln)))
   if (vec && C <= 256) { if (Cin == 1) BWD(true, 8, true); else BWD(true, 8, false); }
@@ -794,8 +759,6 @@ int conv1_bwd_fused(const float* src, const float* w, const float* b, const floa
   else if (C <= 256) { if (Cin == 1) BWD(false, 8, true); else BWD(false, 8, false); }
   else { if (Cin == 1) BWD(false, 16, true); else BWD(false, 16, false); }
 #undef BWD
-  ++g_kernel_launches;
-  B200ST_LAUNCH_CHECK();
   return 0;
 }
 
@@ -809,18 +772,16 @@ int conv1_bwd_from_xhat(const float* src, const void* gamma, const void* beta, c
   const int T1 = (T + 1) / 2, F1 = (F + 1) / 2, T2 = (T1 + 1) / 2, F2 = (F1 + 1) / 2;
   const int64_t npos = (int64_t)B * T1 * F1;
   if (npos == 0) return 0;
-  const int grid = pick_grid(npos, 8 * 16, 132 * 2);
+  const int grid = grid_for(npos, 8 * 16, 132 * 2);
   const int tu = F2 > 0 && F2 <= 128 ? 128 / F2 : 1, ub = (T2 + tu - 1) / tu;
   if (implicit_tiles) {
     B200ST_CHECK(F2 <= 128, "implicit conv2 dgrad layout needs F2 <= 128");
-    DISPATCH_DTYPE(dtype, TT, (launch_pdl(conv1_bwd_xhat_c256_kernel<TT, true>, grid, 256, 0, s, src, (const TT*)gamma, (const TT*)beta, (const TT*)xhat, rstd,
+    DISPATCH_DTYPE(dtype, TT, (launch(conv1_bwd_xhat_c256_kernel<TT, true>, grid, 256, 0, s, src, (const TT*)gamma, (const TT*)beta, (const TT*)xhat, rstd,
                                           (const TT*)dcol, (TT*)dz1, (TT*)col1, K1p, db, dgamma, dbeta, B, T, F, T1, F1, T2, F2, tu, ub)));
   } else {
-    DISPATCH_DTYPE(dtype, TT, (launch_pdl(conv1_bwd_xhat_c256_kernel<TT, false>, grid, 256, 0, s, src, (const TT*)gamma, (const TT*)beta, (const TT*)xhat, rstd,
+    DISPATCH_DTYPE(dtype, TT, (launch(conv1_bwd_xhat_c256_kernel<TT, false>, grid, 256, 0, s, src, (const TT*)gamma, (const TT*)beta, (const TT*)xhat, rstd,
                                           (const TT*)dcol, (TT*)dz1, (TT*)col1, K1p, db, dgamma, dbeta, B, T, F, T1, F1, T2, F2, tu, ub)));
   }
-  ++g_kernel_launches;
-  B200ST_LAUNCH_CHECK();
   return 0;
 }
 
@@ -834,19 +795,17 @@ int im2col_3x3s2_affine(const void* y1, void* col, int dtype, int B, int T1, int
   const int T2 = (T1 + 1) / 2, F2 = (F1 + 1) / 2;
   const int64_t nchunks = (int64_t)B * T2 * F2 * 9;
   if (nchunks == 0) return 0;
-  const int grid = pick_grid(nchunks, 8 * 8, 132 * 16);
+  const int grid = grid_for(nchunks, 8 * 8, 132 * 16);
   const int esz = dtype_size(dtype);
   const bool vec = ((C * esz) % 16 == 0) && ((reinterpret_cast<uintptr_t>(y1) & 15) == 0) && ((reinterpret_cast<uintptr_t>(col) & 15) == 0) &&
                    ((reinterpret_cast<uintptr_t>(gamma) & 15) == 0) && ((reinterpret_cast<uintptr_t>(beta) & 15) == 0);
   const bool one = vec && C * esz == 32 * 16;
   if (one) {
-    const int grid_r = pick_grid(nchunks / 9, 8 * 4, 132 * 8);
-    DISPATCH_DTYPE(dtype, TT, (launch_pdl(im2col_row_kernel<TT>, grid_r, 256, 0, s, (const TT*)y1, (TT*)col, B, T1, F1, T2, F2, (const TT*)gamma, (const TT*)beta)));
+    const int grid_r = grid_for(nchunks / 9, 8 * 4, 132 * 8);
+    DISPATCH_DTYPE(dtype, TT, (launch(im2col_row_kernel<TT>, grid_r, 256, 0, s, (const TT*)y1, (TT*)col, B, T1, F1, T2, F2, (const TT*)gamma, (const TT*)beta)));
   }
-  else if (vec) DISPATCH_DTYPE(dtype, TT, (launch_pdl(im2col_kernel<TT, true, false>, grid, 256, 0, s, (const TT*)y1, (TT*)col, B, T1, F1, C, T2, F2, (const TT*)gamma, (const TT*)beta)));
-  else DISPATCH_DTYPE(dtype, TT, (launch_pdl(im2col_kernel<TT, false, false>, grid, 256, 0, s, (const TT*)y1, (TT*)col, B, T1, F1, C, T2, F2, (const TT*)gamma, (const TT*)beta)));
-  ++g_kernel_launches;
-  B200ST_LAUNCH_CHECK();
+  else if (vec) DISPATCH_DTYPE(dtype, TT, (launch(im2col_kernel<TT, true, false>, grid, 256, 0, s, (const TT*)y1, (TT*)col, B, T1, F1, C, T2, F2, (const TT*)gamma, (const TT*)beta)));
+  else DISPATCH_DTYPE(dtype, TT, (launch(im2col_kernel<TT, false, false>, grid, 256, 0, s, (const TT*)y1, (TT*)col, B, T1, F1, C, T2, F2, (const TT*)gamma, (const TT*)beta)));
   return 0;
 }
 

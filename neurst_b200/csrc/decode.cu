@@ -741,7 +741,7 @@ int step_launch(const StepCtx& c, const TW* wbase, const int64_t* ids, const int
   // zero every accumulator of the step in one node (qkv / q / ffn hidden of all layers; logits are plain stores)
   B200ST_CUDA(cudaMemsetAsync(st.scratch + lo.qkv, 0, sizeof(float) * (size_t)(lo.logits - lo.qkv), c.s));
   auto W = [&](const std::string& n) { return wbase + c.off(n); };
-  launch_pdl(embed_step_kernel<TW>, (B * d + 255) / 256, 256, 0, c.s, ids, W("trg.emb"), x, B, d, V, time_dev);
+  B200ST_TRY(launch(embed_step_kernel<TW>, (B * d + 255) / 256, 256, 0, c.s, ids, W("trg.emb"), x, B, d, V, time_dev));
   const int64_t self_layer = 2 * (int64_t)B * st.max_len * d, cross_layer = (int64_t)(B / beam) * st.Tm * 2 * d;
   for (int i = 0; i < cf.dec_layers; ++i) {
     const std::string p = "dec." + std::to_string(i);
@@ -749,36 +749,32 @@ int step_launch(const StepCtx& c, const TW* wbase, const int64_t* ids, const int
     float* qc = st.scratch + lo.qc + (int64_t)i * B * d;
     float* hid = st.scratch + lo.hid + (int64_t)i * B * f;
     // self attention block
-    launch_pdl(gemv_kernel<TW, 0>, dim3((3 * d + 127) / 128, (d + 31) / 32), 128, 0, c.s, (const float*)x, c.P(p + ".self.ln.gamma"),
-               c.P(p + ".self.ln.beta"), (const float*)nullptr, cf.ln_eps, W(p + ".self.qkv.kernel"), c.P(p + ".self.qkv.bias"), qkv, B, d, 3 * d);
+    B200ST_TRY(launch(gemv_kernel<TW, 0>, dim3((3 * d + 127) / 128, (d + 31) / 32), 128, 0, c.s, (const float*)x, c.P(p + ".self.ln.gamma"),
+                      c.P(p + ".self.ln.beta"), (const float*)nullptr, cf.ln_eps, W(p + ".self.qkv.kernel"), c.P(p + ".self.qkv.bias"), qkv, B, d, 3 * d));
     float* sk = st.self_kv + (int64_t)i * self_layer;
     float* sv = sk + (int64_t)B * st.max_len * d;
     const size_t smem_self = self_attn_smem(cf, st.max_len, anc != nullptr);
-    launch_pdl(anc ? attn_step_kernel<TW, true, true> : attn_step_kernel<TW, true>, dim3(H, B), 256, smem_self, c.s,
-               (const float*)qkv, 3 * d, sk, sv, d, st.max_len, (const float*)nullptr, W(p + ".self.out.kernel"),
-               c.P(p + ".self.out.bias"), x, d, dh, 0, 0, time_dev, anc, beam);
+    B200ST_TRY(launch(anc ? attn_step_kernel<TW, true, true> : attn_step_kernel<TW, true>, dim3(H, B), 256, smem_self, c.s,
+                      (const float*)qkv, 3 * d, sk, sv, d, st.max_len, (const float*)nullptr, W(p + ".self.out.kernel"),
+                      c.P(p + ".self.out.bias"), x, d, dh, 0, 0, time_dev, anc, beam));
     // encoder-decoder attention block over the pre-projected memory
     if (cf.with_cross_attention && st.Tm > 0) {
-      launch_pdl(gemv_kernel<TW, 0>, dim3((d + 127) / 128, (d + 31) / 32), 128, 0, c.s, (const float*)x, c.P(p + ".cross.ln.gamma"),
-                 c.P(p + ".cross.ln.beta"), (const float*)nullptr, cf.ln_eps, W(p + ".cross.q.kernel"), c.P(p + ".cross.q.bias"), qc, B, d, d);
+      B200ST_TRY(launch(gemv_kernel<TW, 0>, dim3((d + 127) / 128, (d + 31) / 32), 128, 0, c.s, (const float*)x, c.P(p + ".cross.ln.gamma"),
+                        c.P(p + ".cross.ln.beta"), (const float*)nullptr, cf.ln_eps, W(p + ".cross.q.kernel"), c.P(p + ".cross.q.bias"), qc, B, d, d));
       float* ck = st.cross_kv + (int64_t)i * cross_layer;
       const size_t smem_cross = sizeof(float) * (size_t)(2 * dh + st.Tm + 8);
-      launch_pdl(anc ? attn_step_kernel<TW, false, true> : attn_step_kernel<TW, false>, dim3(H, B), 256, smem_cross, c.s,
-                 (const float*)qc, d, ck, ck + d, 2 * d, st.Tm, st.memory_bias, W(p + ".cross.out.kernel"),
-                 c.P(p + ".cross.out.bias"), x, d, dh, st.Tm, st.wait_k, time_dev, anc, beam);
+      B200ST_TRY(launch(anc ? attn_step_kernel<TW, false, true> : attn_step_kernel<TW, false>, dim3(H, B), 256, smem_cross, c.s,
+                        (const float*)qc, d, ck, ck + d, 2 * d, st.Tm, st.memory_bias, W(p + ".cross.out.kernel"),
+                        c.P(p + ".cross.out.bias"), x, d, dh, st.Tm, st.wait_k, time_dev, anc, beam));
     }
     // feed-forward block
-    launch_pdl(gemv_kernel<TW, 0>, dim3((f + 127) / 128, (d + 31) / 32), 128, 0, c.s, (const float*)x, c.P(p + ".ffn.ln.gamma"),
-               c.P(p + ".ffn.ln.beta"), (const float*)nullptr, cf.ln_eps, W(p + ".ffn.w1"), (const float*)nullptr, hid, B, d, f);
-    launch_pdl(gemv_kernel<TW, 1>, dim3((d + 127) / 128, (f + 31) / 32), 128, 0, c.s, (const float*)hid, (const float*)nullptr,
-               (const float*)nullptr, c.P(p + ".ffn.b1"), 0.f, W(p + ".ffn.w2"), c.P(p + ".ffn.b2"), x, B, f, d);
-    g_kernel_launches += cf.with_cross_attention && st.Tm > 0 ? 6 : 4;
+    B200ST_TRY(launch(gemv_kernel<TW, 0>, dim3((f + 127) / 128, (d + 31) / 32), 128, 0, c.s, (const float*)x, c.P(p + ".ffn.ln.gamma"),
+                      c.P(p + ".ffn.ln.beta"), (const float*)nullptr, cf.ln_eps, W(p + ".ffn.w1"), (const float*)nullptr, hid, B, d, f));
+    B200ST_TRY(launch(gemv_kernel<TW, 1>, dim3((d + 127) / 128, (f + 31) / 32), 128, 0, c.s, (const float*)hid, (const float*)nullptr,
+                      (const float*)nullptr, c.P(p + ".ffn.b1"), 0.f, W(p + ".ffn.w2"), c.P(p + ".ffn.b2"), x, B, f, d));
   }
-  launch_pdl(logits_step_kernel<TW>, 132 * 2, 256, sizeof(float) * (size_t)B * d, c.s, (const float*)x, c.P("dec.out_ln.gamma"),
-             c.P("dec.out_ln.beta"), cf.ln_eps, W("trg.emb"), c.P("trg.bias"), logits_out, B, d, V);
-  g_kernel_launches += 2;
-  B200ST_LAUNCH_CHECK();
-  return 0;
+  return launch(logits_step_kernel<TW>, 132 * 2, 256, sizeof(float) * (size_t)B * d, c.s, (const float*)x, c.P("dec.out_ln.gamma"),
+                c.P("dec.out_ln.beta"), cf.ln_eps, W("trg.emb"), c.P("trg.bias"), logits_out, B, d, V);
 }
 
 // More than 8 rows: the embedding of the current symbols into x (scratch offset 0), then the wide step (decode_rows.cu).
@@ -787,12 +783,11 @@ int step_rows(const StepCtx& c, const int64_t* ids, const int32_t* time_dev, flo
   const Config& cf = c.m.cfg;
   const int n = c.st.B * cf.d;
   if (c.m.adt == F16)
-    launch_pdl(embed_step_kernel<__half>, (n + 255) / 256, 256, 0, c.s, ids, reinterpret_cast<const __half*>(c.buf.shadow) + c.off("trg.emb"),
-               c.st.scratch, c.st.B, cf.d, cf.vocab, time_dev);
+    B200ST_TRY(launch(embed_step_kernel<__half>, (n + 255) / 256, 256, 0, c.s, ids, reinterpret_cast<const __half*>(c.buf.shadow) + c.off("trg.emb"),
+                      c.st.scratch, c.st.B, cf.d, cf.vocab, time_dev));
   else
-    launch_pdl(embed_step_kernel<__nv_bfloat16>, (n + 255) / 256, 256, 0, c.s, ids,
-               reinterpret_cast<const __nv_bfloat16*>(c.buf.shadow) + c.off("trg.emb"), c.st.scratch, c.st.B, cf.d, cf.vocab, time_dev);
-  ++g_kernel_launches;
+    B200ST_TRY(launch(embed_step_kernel<__nv_bfloat16>, (n + 255) / 256, 256, 0, c.s, ids,
+                      reinterpret_cast<const __nv_bfloat16*>(c.buf.shadow) + c.off("trg.emb"), c.st.scratch, c.st.B, cf.d, cf.vocab, time_dev));
   return rows_step(c.m, c.buf, c.st, time_dev, logits_out, anc, beam, c.s);
 }
 
@@ -822,7 +817,7 @@ int run_token_loop(cudaStream_t s, int max_steps, bool use_graph, const int32_t*
       const int rc = one_step();
       cudaError_t e = cudaStreamEndCapture(s, &graph);
       if (rc == 0 && e == cudaSuccess && graph && cudaGraphInstantiate(&exec, graph, 0) == cudaSuccess) graphed = true;
-      else { cudaGetLastError(); pdl_launch_error() = cudaSuccess; }
+      else cudaGetLastError();
     } else {
       cudaGetLastError();
     }
@@ -895,7 +890,7 @@ int launch_persistent(const Model& m, const Buffers& buf, const DecodeState& st,
   void* args[2] = {(void*)&a, (void*)&wbase};
   const cudaError_t e = cudaLaunchCooperativeKernel((const void*)kern, dim3(sms), dim3(256), args, smem, s);
   if (e != cudaSuccess) { cudaGetLastError(); return 0; }
-  ++g_kernel_launches;
+  count_launch();
   *done = true;
   return 0;
 }
@@ -1052,7 +1047,6 @@ int decode_init(const Model& m, const Buffers& buf, const float* enc_out, const 
     g.C = st.cross_kv + (int64_t)i * st.B * st.Tm * 2 * d; g.c_dtype = F32; g.ldc = 2 * d;
     g.epi.bias = buf.params + m.params[bi].offset;
     B200ST_TRY(gemm_simt_f32(g, s));
-    ++g_kernel_launches;
   }
   return 0;
 }
@@ -1096,8 +1090,7 @@ int greedy_search(const Model& m, const Buffers& buf, const DecodeState& st, con
   g.all_finished = reinterpret_cast<int32_t*>(w); w += sizeof(int32_t);
   uint32_t* ticket = reinterpret_cast<uint32_t*>(w);
   float* logits = step_logits(cf, st);
-  greedy_init_kernel<<<8, 256, 0, s>>>(g, ga.bos_ids, st.B, ga.max_steps, ga.eos_id);
-  B200ST_CUDA(cudaGetLastError());
+  B200ST_TRY(launch_serial(greedy_init_kernel, 8, 256, 0, s, g, ga.bos_ids, st.B, ga.max_steps, ga.eos_id));
   if (wide) B200ST_CUDA(cudaMemsetAsync(ticket, 0, sizeof(uint32_t), s));
   if (ga.use_graph == 2 && !wide) {       // persistent mode: one cooperative launch for the whole search
     bool done = false;
@@ -1113,15 +1106,10 @@ int greedy_search(const Model& m, const Buffers& buf, const DecodeState& st, con
   StepCtx c{m, buf, st, s};
   auto one_step = [&]() -> int {
     B200ST_TRY(step_dispatch(c, g.ids, g.time, logits));
-    if (wide) {
-      rows_greedy_pick(logits, g.ids, g.finished, g.length, g.logprob, g.out, g.time, g.all_finished, ticket, st.B, cf.vocab, ga.eos_id,
-                       ga.unk_id, ga.min_len, ga.max_steps, s);
-    } else {
-      launch_pdl(greedy_pick_kernel, 1, 1024, 0, s, (const float*)logits, g, st.B, cf.vocab, ga.eos_id, ga.unk_id, ga.min_len, ga.max_steps);
-      ++g_kernel_launches;
-    }
-    B200ST_LAUNCH_CHECK();
-    return 0;
+    if (wide)
+      return rows_greedy_pick(logits, g.ids, g.finished, g.length, g.logprob, g.out, g.time, g.all_finished, ticket, st.B, cf.vocab,
+                              ga.eos_id, ga.unk_id, ga.min_len, ga.max_steps, s);
+    return launch(greedy_pick_kernel, 1, 1024, 0, s, (const float*)logits, g, st.B, cf.vocab, ga.eos_id, ga.unk_id, ga.min_len, ga.max_steps);
   };
   bool graphed = false;
   const int rc = run_token_loop(s, ga.max_steps, ga.use_graph != 0, g.all_finished, one_step, &graphed);
@@ -1157,8 +1145,7 @@ int sampling_search(const Model& m, const Buffers& buf, const DecodeState& st, c
   B200ST_TRY(prepare_search(&one, 1, n, a.max_steps, "sample_num", "sampling search", s, &prep));
   const int rows = prep.rows;
   BeamState bs = beam_state_at(a.state_words, rows, st.max_len);
-  sample_init(bs, a.bos_ids, rows, n, st.max_len, a.out_ids, a.max_steps, a.eos_id, a.out_logprob, a.out_len, s);
-  B200ST_CUDA(cudaGetLastError());
+  B200ST_TRY(sample_init(bs, a.bos_ids, rows, n, st.max_len, a.out_ids, a.max_steps, a.eos_id, a.out_logprob, a.out_len, s));
   SampleRows sr{};
   sr.logits = prep.logits[0]; sr.V = cf.vocab; sr.eos = a.eos_id; sr.unk = a.unk_id; sr.min_len = a.min_len;
   sr.top_k = a.top_k; sr.top_p = a.top_p; sr.seed = a.seed; sr.row_offset = a.row_offset;
@@ -1167,9 +1154,7 @@ int sampling_search(const Model& m, const Buffers& buf, const DecodeState& st, c
   sr.time = bs.time; sr.all_finished = bs.all_finished; sr.ticket = bs.ticket;
   auto one_step = [&]() -> int {
     B200ST_TRY(step_dispatch(prep.ctx[0], bs.ids, bs.time, prep.logits[0], bs.anc, n));
-    sample_select(sr, rows, s);
-    B200ST_LAUNCH_CHECK();
-    return 0;
+    return sample_select(sr, rows, s);
   };
   bool graphed = false;
   B200ST_TRY(run_token_loop(s, a.max_steps, a.use_graph != 0, bs.all_finished, one_step, &graphed));
@@ -1206,9 +1191,8 @@ int ensemble_beam_search(const EnsembleMember* mem, int n, const BeamArgs& a, cu
     ga.out_ids = a.out_ids; ga.out_len = a.out_len; ga.out_logprob = a.out_logprob; ga.state_words = a.state_words;
     ga.use_graph = a.use_graph;
     B200ST_TRY(greedy_search(*mem[0].m, mem[0].buf, st0, ga, s));
-    beam1_score_kernel<<<(st0.B + 255) / 256, 256, 0, s>>>(a.out_logprob, a.out_len, a.out_scores, st0.B, a.length_penalty);
-    B200ST_CUDA(cudaGetLastError());
-    return 0;
+    return launch_serial(beam1_score_kernel, (st0.B + 255) / 256, 256, 0, s, a.out_logprob, a.out_len, a.out_scores, st0.B,
+                         a.length_penalty);
   }
   SearchRows prep;
   B200ST_TRY(prepare_search(mem, n, beam, a.max_steps, "beam_size", "beam search", s, &prep));
@@ -1220,29 +1204,21 @@ int ensemble_beam_search(const EnsembleMember* mem, int n, const BeamArgs& a, cu
     mix.logw[i] = (float)std::log((double)mem[i].weight / wsum);       // a zero weight: -inf, which contributes nothing
   }
   const BeamState bs = beam_state_at(a.state_words, rows, st0.max_len);
-  beam_init_kernel<<<(rows + 255) / 256, 256, 0, s>>>(bs, a.bos_ids, rows, beam);
-  B200ST_CUDA(cudaGetLastError());
+  B200ST_TRY(launch_serial(beam_init_kernel, (rows + 255) / 256, 256, 0, s, bs, a.bos_ids, rows, beam));
   auto one_step = [&]() -> int {
     for (int i = 0; i < n; ++i) B200ST_TRY(step_dispatch(prep.ctx[i], bs.ids, bs.time, prep.logits[i], bs.anc, beam));
     if (n > 1) {
-      ensemble_logprob(mix, rows, V, s);
-      beam_select_logprobs(prep.logits[0], bs, st0.B, beam, V, a.eos_id, a.unk_id, a.min_len, a.length_penalty, st0.max_len, s);
-    } else {
-      launch_pdl(beam_select_kernel<false>, st0.B, 1024, 0, s, (const float*)prep.logits[0], bs, beam, V, a.eos_id, a.unk_id,
-                 a.min_len, a.length_penalty, st0.max_len);
-      ++g_kernel_launches;
+      B200ST_TRY(ensemble_logprob(mix, rows, V, s));
+      return beam_select_logprobs(prep.logits[0], bs, st0.B, beam, V, a.eos_id, a.unk_id, a.min_len, a.length_penalty, st0.max_len, s);
     }
-    B200ST_LAUNCH_CHECK();
-    return 0;
+    return launch(beam_select_kernel<false>, st0.B, 1024, 0, s, (const float*)prep.logits[0], bs, beam, V, a.eos_id, a.unk_id,
+                  a.min_len, a.length_penalty, st0.max_len);
   };
   bool graphed = false;
   B200ST_TRY(run_token_loop(s, a.max_steps, a.use_graph != 0, bs.all_finished, one_step, &graphed));
   B200ST_CHECK(graphed || !a.use_graph, "beam search could not capture its step into a CUDA graph");
-  beam_extract_kernel<<<st0.B, 256, 0, s>>>(bs, beam, a.top_k, a.length_penalty, a.eos_id, st0.max_len, a.max_steps, a.out_ids,
-                                            a.out_scores, a.out_logprob, a.out_len);
-  ++g_kernel_launches;
-  B200ST_CUDA(cudaGetLastError());
-  return 0;
+  return launch_serial(beam_extract_kernel, st0.B, 256, 0, s, bs, beam, a.top_k, a.length_penalty, a.eos_id, st0.max_len, a.max_steps,
+                       a.out_ids, a.out_scores, a.out_logprob, a.out_len);
 }
 
 }  // namespace b200st

@@ -485,9 +485,7 @@ RowsLayout rows_layout(const Config& c, int B) {
 
 template <bool BF, bool B_MN, int PRE, int EPI>
 int launch_rows_gemm(const CUtensorMap& tm, const RowsParams& p, dim3 grid, cudaStream_t s) {
-  launch_pdl(rows_gemm_kernel<BF, B_MN, PRE, EPI>, grid, kRowsThreads, kRowsSmem, s, tm, p);
-  ++g_kernel_launches;
-  return 0;
+  return launch(rows_gemm_kernel<BF, B_MN, PRE, EPI>, grid, kRowsThreads, kRowsSmem, s, tm, p);
 }
 
 // K slices of one rows GEMM.  Only the products into the d-wide residual stream (N <= d: the output projections and the
@@ -560,15 +558,15 @@ int rows_step_t(const Model& m, const Buffers& buf, const DecodeState& st, const
     B200ST_TRY(rows_gemm(x, B, d, W(p + ".self.qkv.kernel"), true, 3 * d, PRE_LN, P(p + ".self.ln.gamma"), P(p + ".self.ln.beta"),
                          cf.ln_eps, nullptr, P(p + ".self.qkv.bias"), qkv, EPI_STORE, lo, sc, s));
     float* sk = st.self_kv + (int64_t)i * self_layer;
-    launch_pdl(rows_self_attn_kernel, dim3(H, B), kAttnThreads, smem_self, s, (const float*)qkv, sk, sk + (int64_t)B * st.max_len * d,
-               d, dh, st.max_len, time_dev, anc, ctx);
+    B200ST_TRY(launch(rows_self_attn_kernel, dim3(H, B), kAttnThreads, smem_self, s, (const float*)qkv, sk, sk + (int64_t)B * st.max_len * d,
+                      d, dh, st.max_len, time_dev, anc, ctx));
     B200ST_TRY(rows_gemm(ctx, B, d, W(p + ".self.out.kernel"), true, d, PRE_NONE, nullptr, nullptr, 0.f, nullptr,
                          P(p + ".self.out.bias"), x, EPI_ADD, lo, sc, s));
     if (cross) {
       B200ST_TRY(rows_gemm(x, B, d, W(p + ".cross.q.kernel"), true, d, PRE_LN, P(p + ".cross.ln.gamma"), P(p + ".cross.ln.beta"),
                            cf.ln_eps, nullptr, P(p + ".cross.q.bias"), qc, EPI_STORE, lo, sc, s));
-      launch_pdl(rows_cross_attn_kernel, dim3(H, B / beam), kAttnThreads, smem_cross, s, (const float*)qc,
-                 (const float*)(st.cross_kv + (int64_t)i * cross_layer), st.memory_bias, d, dh, st.Tm, st.wait_k, time_dev, beam, ctx);
+      B200ST_TRY(launch(rows_cross_attn_kernel, dim3(H, B / beam), kAttnThreads, smem_cross, s, (const float*)qc,
+                        (const float*)(st.cross_kv + (int64_t)i * cross_layer), st.memory_bias, d, dh, st.Tm, st.wait_k, time_dev, beam, ctx));
       B200ST_TRY(rows_gemm(ctx, B, d, W(p + ".cross.out.kernel"), true, d, PRE_NONE, nullptr, nullptr, 0.f, nullptr,
                            P(p + ".cross.out.bias"), x, EPI_ADD, lo, sc, s));
     }
@@ -576,11 +574,9 @@ int rows_step_t(const Model& m, const Buffers& buf, const DecodeState& st, const
                          nullptr, nullptr, hid, EPI_STORE, lo, sc, s));
     B200ST_TRY(rows_gemm(hid, B, f, W(p + ".ffn.w2"), true, d, PRE_RELU_BIAS, nullptr, nullptr, 0.f, P(p + ".ffn.b1"),
                          P(p + ".ffn.b2"), x, EPI_ADD, lo, sc, s));
-    g_kernel_launches += cross ? 2 : 1;
   }
   B200ST_TRY(rows_gemm(x, B, d, W("trg.emb"), false, V, PRE_LN, P("dec.out_ln.gamma"), P("dec.out_ln.beta"), cf.ln_eps, nullptr,
                        P("trg.bias"), logits, EPI_STORE, lo, sc, s));
-  B200ST_LAUNCH_CHECK();
   return 0;
 }
 
@@ -626,12 +622,11 @@ int rows_step(const Model& m, const Buffers& buf, const DecodeState& st, const i
   return rows_step_t(m, buf, st, reinterpret_cast<const __nv_bfloat16*>(buf.shadow), time_dev, logits, anc, beam, s);
 }
 
-void rows_greedy_pick(const float* logits, int64_t* ids, int32_t* finished, int32_t* length, float* logprob, int64_t* out,
-                      int32_t* time, int32_t* all_finished, uint32_t* ticket, int B, int V, int eos, int unk, int min_len,
-                      int max_steps, cudaStream_t s) {
-  launch_pdl(rows_greedy_pick_kernel, B, 1024, 0, s, logits, ids, finished, length, logprob, out, time, all_finished, ticket, V, eos,
-             unk, min_len, max_steps);
-  ++g_kernel_launches;
+int rows_greedy_pick(const float* logits, int64_t* ids, int32_t* finished, int32_t* length, float* logprob, int64_t* out,
+                     int32_t* time, int32_t* all_finished, uint32_t* ticket, int B, int V, int eos, int unk, int min_len,
+                     int max_steps, cudaStream_t s) {
+  return launch(rows_greedy_pick_kernel, B, 1024, 0, s, logits, ids, finished, length, logprob, out, time, all_finished, ticket, V, eos,
+                unk, min_len, max_steps);
 }
 
 }  // namespace b200st

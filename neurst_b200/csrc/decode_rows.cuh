@@ -21,8 +21,8 @@ int rows_raise_smem(size_t self_bytes, size_t cross_bytes);
 int rows_step(const Model& m, const Buffers& buf, const DecodeState& st, const int32_t* time_dev, float* logits, const int* anc,
               int beam, cudaStream_t s);
 // greedy_pick_kernel's selection rules with one block per row; the last block to finish publishes time / all_finished
-void rows_greedy_pick(const float* logits, int64_t* ids, int32_t* finished, int32_t* length, float* logprob, int64_t* out,
-                      int32_t* time, int32_t* all_finished, uint32_t* ticket, int B, int V, int eos, int unk, int min_len,
-                      int max_steps, cudaStream_t s);
+int rows_greedy_pick(const float* logits, int64_t* ids, int32_t* finished, int32_t* length, float* logprob, int64_t* out,
+                     int32_t* time, int32_t* all_finished, uint32_t* ticket, int B, int V, int eos, int unk, int min_len,
+                     int max_steps, cudaStream_t s);
 
 }  // namespace b200st

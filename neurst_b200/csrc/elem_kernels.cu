@@ -6,25 +6,12 @@
 
 namespace b200st {
 
-#define DISPATCH_DTYPE(dt, T, ...)                                   \
-  do {                                                               \
-    if ((dt) == F32) { using T = float; __VA_ARGS__; }               \
-    else if ((dt) == BF16) { using T = __nv_bfloat16; __VA_ARGS__; } \
-    else if ((dt) == F16) { using T = __half; __VA_ARGS__; }         \
-    else B200ST_FAIL("bad dtype");                                   \
-  } while (0)
 // three tensors that are either all fp32 or all the same 16-bit type (keeps the instantiation count linear)
 #define DISPATCH_UNIFORM3(d0, d1, d2, T, ...)                                                 \
   do {                                                                                        \
     if ((d0) != (d1) || (d1) != (d2)) B200ST_FAIL("the three tensors must share one dtype"); \
     DISPATCH_DTYPE(d0, T, __VA_ARGS__);                                                       \
   } while (0)
-
-static inline int grid_for(int64_t work, int per_block, int cap = 132 * 16) {
-  int64_t g = (work + per_block - 1) / per_block;
-  if (g < 1) g = 1;
-  return (int)(g > cap ? cap : g);
-}
 
 
 // ---- 4-wide vector access along the feature axis (16-byte fp32 / 8-byte bf16) ------------------------------------
@@ -158,19 +145,17 @@ int layernorm_fwd_copy(const void* x, int x_dtype, const float* gamma, const flo
   const bool vec = (cols % 4 == 0) && cols <= 1024 && ((reinterpret_cast<uintptr_t>(x) & 15) == 0) &&
                    ((reinterpret_cast<uintptr_t>(y) & 15) == 0) && ((reinterpret_cast<uintptr_t>(gamma) & 15) == 0) &&
                    ((reinterpret_cast<uintptr_t>(beta) & 15) == 0) && (!y32 || (reinterpret_cast<uintptr_t>(y32) & 15) == 0);
+  // x and y dtypes are independent: the inner dispatch runs in a lambda so that the outer one gets its result
+#define LN_FWD(...) DISPATCH_DTYPE(x_dtype, TX, [&] { DISPATCH_DTYPE(y_dtype, TY, __VA_ARGS__); return 0; }())
 #define LN_FWD_VEC(NV)                                                                                                  \
-  DISPATCH_DTYPE(x_dtype, TX, DISPATCH_DTYPE(y_dtype, TY,                                                               \
-      (launch_pdl(ln_fwd_vec_kernel<TX, TY, NV>, grid, 256, 0, s, (const TX*)x, gamma, beta, eps, (TY*)y, y32, mean, rstd, rows, cols, relu, \
-                  (vec && x_dtype == F32 && (reinterpret_cast<uintptr_t>(xcopy) & 15) == 0) ? xcopy : (float*)nullptr))))
+  LN_FWD(launch(ln_fwd_vec_kernel<TX, TY, NV>, grid, 256, 0, s, (const TX*)x, gamma, beta, eps, (TY*)y, y32, mean, rstd, rows, cols, relu, \
+                (vec && x_dtype == F32 && (reinterpret_cast<uintptr_t>(xcopy) & 15) == 0) ? xcopy : (float*)nullptr))
   if (vec && cols <= 256) LN_FWD_VEC(2);
   else if (vec && cols <= 512) LN_FWD_VEC(4);
   else if (vec) LN_FWD_VEC(8);
-  else
-    DISPATCH_DTYPE(x_dtype, TX, DISPATCH_DTYPE(y_dtype, TY,
-        (launch_pdl(ln_fwd_kernel<TX, TY>, grid, 256, 0, s, (const TX*)x, gamma, beta, eps, (TY*)y, y32, mean, rstd, rows, cols, relu))));
+  else LN_FWD(launch(ln_fwd_kernel<TX, TY>, grid, 256, 0, s, (const TX*)x, gamma, beta, eps, (TY*)y, y32, mean, rstd, rows, cols, relu));
 #undef LN_FWD_VEC
-  ++g_kernel_launches;
-  B200ST_LAUNCH_CHECK();
+#undef LN_FWD
   if (xcopy && !(vec && x_dtype == F32 && (reinterpret_cast<uintptr_t>(xcopy) & 15) == 0)) {
     B200ST_CHECK(x_dtype == F32, "layernorm_fwd_copy needs fp32 input rows");
     B200ST_CUDA(cudaMemcpyAsync(xcopy, x, sizeof(float) * (size_t)rows * cols, cudaMemcpyDeviceToDevice, s));
@@ -381,14 +366,14 @@ int layernorm_bwd_next(const void* dy, int dy_dtype, const void* x, int x_dtype,
   const size_t smem = 2 * (size_t)cols * sizeof(float);
 #define LN_BWD_LAUNCH(CPL)                                                                                              \
   DISPATCH_UNIFORM3(dy_dtype, x_dtype, dx_dtype, TT,                                                                    \
-      (launch_pdl(ln_bwd_kernel<TT, TT, TT, CPL>, grid, 256, smem, s, (const TT*)dy, (const TT*)x, mean, rstd, gamma, beta, dres, \
+      (launch(ln_bwd_kernel<TT, TT, TT, CPL>, grid, 256, smem, s, (const TT*)dy, (const TT*)x, mean, rstd, gamma, beta, dres, \
                                                                 (TT*)dx, dgamma, dbeta, rows, cols, relu)))
   const bool vec = (cols % 4 == 0) && ((reinterpret_cast<uintptr_t>(x) & 15) == 0) && ((reinterpret_cast<uintptr_t>(dy) & 15) == 0) &&
                    ((reinterpret_cast<uintptr_t>(dx) & 15) == 0) && ((reinterpret_cast<uintptr_t>(gamma) & 15) == 0) &&
                    ((reinterpret_cast<uintptr_t>(beta) & 15) == 0) && (!dres || (reinterpret_cast<uintptr_t>(dres) & 15) == 0);
 #define LN_BWD_VEC(NV, RR)                                                                                                \
   DISPATCH_UNIFORM3(dy_dtype, x_dtype, dx_dtype, TT,                                                                    \
-      (launch_pdl(ln_bwd_vec_kernel<TT, TT, TT, NV, RR>, grid, 256, smem * 8, s, (const TT*)dy, (const TT*)x, mean, rstd, gamma, beta, dres, \
+      (launch(ln_bwd_vec_kernel<TT, TT, TT, NV, RR>, grid, 256, smem * 8, s, (const TT*)dy, (const TT*)x, mean, rstd, gamma, beta, dres, \
                                                                    (TT*)dx, dgamma, dbeta, rows, cols, relu, fused_next ? dnext : nullptr, dnext_dtype, ndrop)))
   const bool vec_ok = vec && ((reinterpret_cast<uintptr_t>(dgamma) & 15) == 0) && ((reinterpret_cast<uintptr_t>(dbeta) & 15) == 0);
   const bool fused_next = dnext && vec_ok && cols <= 512 && ((reinterpret_cast<uintptr_t>(dnext) & 15) == 0) &&
@@ -402,8 +387,6 @@ int layernorm_bwd_next(const void* dy, int dy_dtype, const void* x, int x_dtype,
   else LN_BWD_LAUNCH(32);
 #undef LN_BWD_VEC
 #undef LN_BWD_LAUNCH
-  ++g_kernel_launches;
-  B200ST_LAUNCH_CHECK();
   if (dnext && !fused_next) {         // shapes outside the vector kernel: the separate kernel the fusion replaces
     B200ST_CHECK(dx_dtype == F32, "layernorm_bwd_next fallback needs an fp32 dx");
     B200ST_TRY(cast_dropout(reinterpret_cast<const float*>(dx), dnext, dnext_dtype, rows * cols, ndrop, s));
@@ -425,19 +408,6 @@ __device__ __forceinline__ float masked_logit(float v, const float* br, int k, i
   return v;
 }
 
-template <typename T> __device__ __forceinline__ void store8(T* dst, const float (&v)[8]);
-template <> __device__ __forceinline__ void store8<float>(float* dst, const float (&v)[8]) {
-  *reinterpret_cast<float4*>(dst) = make_float4(v[0], v[1], v[2], v[3]);
-  *reinterpret_cast<float4*>(dst + 4) = make_float4(v[4], v[5], v[6], v[7]);
-}
-template <int DT> __device__ __forceinline__ void store8_16(void* dst, const float (&v)[8]) {
-  uint4 pk;
-  pk.x = pack2_16(v[0], v[1], DT); pk.y = pack2_16(v[2], v[3], DT);
-  pk.z = pack2_16(v[4], v[5], DT); pk.w = pack2_16(v[6], v[7], DT);
-  *reinterpret_cast<uint4*>(dst) = pk;
-}
-template <> __device__ __forceinline__ void store8<__nv_bfloat16>(__nv_bfloat16* dst, const float (&v)[8]) { store8_16<BF16>(dst, v); }
-template <> __device__ __forceinline__ void store8<__half>(__half* dst, const float (&v)[8]) { store8_16<F16>(dst, v); }
 template <typename T> __device__ __forceinline__ void load8(const T* src, float (&v)[8]);
 template <> __device__ __forceinline__ void load8<float>(const float* src, float (&v)[8]) {
   const float4 a = *reinterpret_cast<const float4*>(src), b = *reinterpret_cast<const float4*>(src + 4);
@@ -445,9 +415,7 @@ template <> __device__ __forceinline__ void load8<float>(const float* src, float
 }
 template <int DT> __device__ __forceinline__ void load8_16(const void* src, float (&v)[8]) {
   const uint4 pk = *reinterpret_cast<const uint4*>(src);
-  const uint32_t w[4] = {pk.x, pk.y, pk.z, pk.w};
-#pragma unroll
-  for (int i = 0; i < 4; ++i) { const float2 f = unpack2_16(w[i], DT); v[2 * i] = f.x; v[2 * i + 1] = f.y; }
+  unpack8_16<DT>(pk, v);
 }
 template <> __device__ __forceinline__ void load8<__nv_bfloat16>(const __nv_bfloat16* src, float (&v)[8]) { load8_16<BF16>(src, v); }
 template <> __device__ __forceinline__ void load8<__half>(const __half* src, float (&v)[8]) { load8_16<F16>(src, v); }
@@ -527,12 +495,10 @@ int softmax_fwd(const float* S, int64_t ldS, const float* bias, KeyMask mask, vo
   B200ST_CHECK((reinterpret_cast<uintptr_t>(S) & 31) == 0 && (reinterpret_cast<uintptr_t>(P_pre) & 15) == 0, "softmax alignment");
   B200ST_CHECK(Tk <= 2048, "softmax supports up to 2048 keys");
   const int grid = grid_for(rows, 8);
-#define SM_FWD(ST) DISPATCH_DTYPE(p_dtype, T, (launch_pdl(softmax_fwd_kernel<T, ST>, grid, 256, 0, s, S, ldS, bias, mask, (T*)P_pre, \
+#define SM_FWD(ST) DISPATCH_DTYPE(p_dtype, T, (launch(softmax_fwd_kernel<T, ST>, grid, 256, 0, s, S, ldS, bias, mask, (T*)P_pre, \
                                                                                    (T*)P_drop, ldP, B, H, Tq, Tk, drop)))
   if (Tk <= 256) SM_FWD(1); else if (Tk <= 512) SM_FWD(2); else if (Tk <= 1024) SM_FWD(4); else SM_FWD(8);
 #undef SM_FWD
-  ++g_kernel_launches;
-  B200ST_LAUNCH_CHECK();
   return 0;
 }
 
@@ -583,12 +549,10 @@ int softmax_bwd(const float* dP, int64_t ldS, const void* P_pre, void* dS, int p
   if (rows == 0) return 0;
   B200ST_CHECK(ldS % 8 == 0 && ldP % 8 == 0 && Tk <= 2048, "softmax_bwd needs row strides padded to 8 and Tk <= 2048");
   const int grid = grid_for(rows, 8);
-#define SM_BWD(ST) DISPATCH_DTYPE(p_dtype, T, (launch_pdl(softmax_bwd_kernel<T, ST>, grid, 256, 0, s, dP, ldS, (const T*)P_pre, (T*)dS, \
+#define SM_BWD(ST) DISPATCH_DTYPE(p_dtype, T, (launch(softmax_bwd_kernel<T, ST>, grid, 256, 0, s, dP, ldS, (const T*)P_pre, (T*)dS, \
                                                                                    ldP, rows, Tk, drop)))
   if (Tk <= 256) SM_BWD(1); else if (Tk <= 512) SM_BWD(2); else if (Tk <= 1024) SM_BWD(4); else SM_BWD(8);
 #undef SM_BWD
-  ++g_kernel_launches;
-  B200ST_LAUNCH_CHECK();
   return 0;
 }
 
@@ -619,9 +583,7 @@ __global__ void __launch_bounds__(256) cast_dropout_kernel(const float* __restri
 }
 int cast_dropout(const float* x, void* y, int y_dtype, int64_t n, DropoutSpec drop, cudaStream_t s) {
   if (n == 0) return 0;
-  DISPATCH_DTYPE(y_dtype, T, (launch_pdl(cast_dropout_kernel<T>, grid_for((n + 7) / 8, 256), 256, 0, s, x, (T*)y, n, drop)));
-  ++g_kernel_launches;
-  B200ST_LAUNCH_CHECK();
+  DISPATCH_DTYPE(y_dtype, T, (launch(cast_dropout_kernel<T>, grid_for((n + 7) / 8, 256), 256, 0, s, x, (T*)y, n, drop)));
   return 0;
 }
 
@@ -687,17 +649,15 @@ int colsum_accum(const void* dY, int dtype, int64_t M, int N, int64_t ld, float*
     const int cap = (132 * 4 + gx - 1) / gx;
     if (gy > cap) gy = cap;
     if (gy < 1) gy = 1;
-    DISPATCH_DTYPE(dtype, T, (launch_pdl(colsum_vec_kernel<T>, dim3(gx, gy), 256, 0, s, (const T*)dY, M, N, ld, db)));
+    DISPATCH_DTYPE(dtype, T, (launch(colsum_vec_kernel<T>, dim3(gx, gy), 256, 0, s, (const T*)dY, M, N, ld, db)));
   } else {
     dim3 block(32, 8);
     int gy = (int)((M + 255) / 256);
     if (gy > 64) gy = 64;
     if (gy < 1) gy = 1;
     dim3 grid(ceil_div(N, 32), gy);
-    DISPATCH_DTYPE(dtype, T, (launch_pdl(colsum_kernel<T>, grid, block, 0, s, (const T*)dY, M, N, ld, db)));
+    DISPATCH_DTYPE(dtype, T, (launch(colsum_kernel<T>, grid, block, 0, s, (const T*)dY, M, N, ld, db)));
   }
-  ++g_kernel_launches;
-  B200ST_LAUNCH_CHECK();
   return 0;
 }
 
@@ -727,10 +687,7 @@ __global__ void posenc_fwd_kernel(const float* __restrict__ v, float* __restrict
 int posenc_fwd(const float* v, float* x, int B, int T, int d, float scale, int t0, DropoutSpec drop, cudaStream_t s) {
   const int64_t n = (int64_t)B * T * d;
   if (n == 0) return 0;
-  launch_pdl(posenc_fwd_kernel, grid_for(n, 256 * 2), 256, 0, s, v, x, B, T, d, scale, t0, drop);
-  ++g_kernel_launches;
-  B200ST_LAUNCH_CHECK();
-  return 0;
+  return launch(posenc_fwd_kernel, grid_for(n, 256 * 2), 256, 0, s, v, x, B, T, d, scale, t0, drop);
 }
 
 template <typename T>
@@ -745,9 +702,7 @@ __global__ void posenc_bwd_kernel(const float* __restrict__ dx, T* __restrict__ 
 }
 int posenc_bwd(const float* dx, void* dv, int dv_dtype, int64_t n, float scale, DropoutSpec drop, cudaStream_t s) {
   if (n == 0) return 0;
-  DISPATCH_DTYPE(dv_dtype, T, (launch_pdl(posenc_bwd_kernel<T>, grid_for(n, 256 * 4), 256, 0, s, dx, (T*)dv, n, scale, drop)));
-  ++g_kernel_launches;
-  B200ST_LAUNCH_CHECK();
+  DISPATCH_DTYPE(dv_dtype, T, (launch(posenc_bwd_kernel<T>, grid_for(n, 256 * 4), 256, 0, s, dx, (T*)dv, n, scale, drop)));
   return 0;
 }
 
@@ -771,10 +726,7 @@ int embed_fwd(const int64_t* ids, const float* E, float* x, int B, int L, int d,
               cudaStream_t s) {
   const int64_t n = (int64_t)B * L * d;
   if (n == 0) return 0;
-  launch_pdl(embed_fwd_kernel, grid_for(n, 256 * 2), 256, 0, s, ids, E, x, B, L, d, V, t0, sqrtf((float)d), drop);
-  ++g_kernel_launches;
-  B200ST_LAUNCH_CHECK();
-  return 0;
+  return launch(embed_fwd_kernel, grid_for(n, 256 * 2), 256, 0, s, ids, E, x, B, L, d, V, t0, sqrtf((float)d), drop);
 }
 __global__ void embed_bwd_kernel(const int64_t* __restrict__ ids, const float* __restrict__ dx, float* __restrict__ dE,
                                  int B, int L, int d, int V, float scale, DropoutSpec drop) {
@@ -794,10 +746,7 @@ __global__ void embed_bwd_kernel(const int64_t* __restrict__ ids, const float* _
 int embed_bwd(const int64_t* ids, const float* dx, float* dE, int B, int L, int d, int V, DropoutSpec drop, cudaStream_t s) {
   const int64_t n = (int64_t)B * L * d;
   if (n == 0) return 0;
-  launch_pdl(embed_bwd_kernel, grid_for(n, 256 * 2), 256, 0, s, ids, dx, dE, B, L, d, V, sqrtf((float)d), drop);
-  ++g_kernel_launches;
-  B200ST_LAUNCH_CHECK();
-  return 0;
+  return launch(embed_bwd_kernel, grid_for(n, 256 * 2), 256, 0, s, ids, dx, dE, B, L, d, V, sqrtf((float)d), drop);
 }
 
 __global__ void length_to_bias_kernel(const int64_t* __restrict__ lengths, float* __restrict__ bias, int B, int T, int n_halvings,
@@ -815,10 +764,7 @@ __global__ void length_to_bias_kernel(const int64_t* __restrict__ lengths, float
 }
 int length_to_bias(const int64_t* lengths, float* bias, int B, int T, int n_halvings, cudaStream_t s, int32_t* klen) {
   if ((int64_t)B * T == 0) return 0;
-  launch_pdl(length_to_bias_kernel, grid_for((int64_t)B * T, 256), 256, 0, s, lengths, bias, B, T, n_halvings, klen);
-  ++g_kernel_launches;
-  B200ST_LAUNCH_CHECK();
-  return 0;
+  return launch(length_to_bias_kernel, grid_for((int64_t)B * T, 256), 256, 0, s, lengths, bias, B, T, n_halvings, klen);
 }
 __global__ void padding_to_bias_kernel(const float* __restrict__ padding, float* __restrict__ bias, int64_t n) {
   pdl_wait();
@@ -828,10 +774,7 @@ __global__ void padding_to_bias_kernel(const float* __restrict__ padding, float*
 }
 int padding_to_bias(const float* padding, float* bias, int64_t n, cudaStream_t s) {
   if (n == 0) return 0;
-  launch_pdl(padding_to_bias_kernel, grid_for(n, 256), 256, 0, s, padding, bias, n);
-  ++g_kernel_launches;
-  B200ST_LAUNCH_CHECK();
-  return 0;
+  return launch(padding_to_bias_kernel, grid_for(n, 256), 256, 0, s, padding, bias, n);
 }
 
 // =============================================================================================
@@ -991,19 +934,15 @@ int lsce_fwd_bwd(const float* logits, const int64_t* trg, const int64_t* trg_len
   B200ST_CUDA(cudaMemsetAsync(nll_sum, 0, sizeof(float) * B, s));
   const bool vec = (V % 4 == 0) && ((reinterpret_cast<uintptr_t>(logits) & 15) == 0) && (!dlogits || (reinterpret_cast<uintptr_t>(dlogits) & 15) == 0);
   if (vec && V <= 8192)
-    DISPATCH_DTYPE(d_dtype, T, (launch_pdl(lsce_vec_kernel<T, 8>, B * L, 256, 0, s, logits, trg, trg_length, B, L, V, label_smoothing,
+    DISPATCH_DTYPE(d_dtype, T, (launch(lsce_vec_kernel<T, 8>, B * L, 256, 0, s, logits, trg, trg_length, B, L, V, label_smoothing,
                                            nll_sum, (T*)dlogits, loss_scale, loss_scale_dev)));
   else if (vec && V <= 32768)
-    DISPATCH_DTYPE(d_dtype, T, (launch_pdl(lsce_vec_kernel<T, 32>, B * L, 256, 0, s, logits, trg, trg_length, B, L, V, label_smoothing,
+    DISPATCH_DTYPE(d_dtype, T, (launch(lsce_vec_kernel<T, 32>, B * L, 256, 0, s, logits, trg, trg_length, B, L, V, label_smoothing,
                                            nll_sum, (T*)dlogits, loss_scale, loss_scale_dev)));
   else
-    DISPATCH_DTYPE(d_dtype, T, (launch_pdl(lsce_kernel<T>, B * L, 256, 0, s, logits, trg, trg_length, B, L, V, label_smoothing, nll_sum,
+    DISPATCH_DTYPE(d_dtype, T, (launch(lsce_kernel<T>, B * L, 256, 0, s, logits, trg, trg_length, B, L, V, label_smoothing, nll_sum,
                                            (T*)dlogits, loss_scale, loss_scale_dev)));
-  B200ST_LAUNCH_CHECK();
-  launch_pdl(lsce_finalize_kernel, 1, 256, 0, s, nll_sum, trg_length, B, L, n_tokens, loss);
-  g_kernel_launches += 2;
-  B200ST_LAUNCH_CHECK();
-  return 0;
+  return launch(lsce_finalize_kernel, 1, 256, 0, s, nll_sum, trg_length, B, L, n_tokens, loss);
 }
 
 __global__ void dropout_bits_kernel(DropoutSpec drop, int64_t ngroups, uint8_t* __restrict__ out) {
@@ -1017,10 +956,7 @@ __global__ void dropout_bits_kernel(DropoutSpec drop, int64_t ngroups, uint8_t* 
 int dropout_bits(DropoutSpec drop, int64_t n_elems, uint8_t* out, cudaStream_t s) {
   const int64_t ng = (n_elems + 7) / 8;
   if (ng == 0) return 0;
-  launch_pdl(dropout_bits_kernel, grid_for(ng, 256), 256, 0, s, drop, ng, out);
-  ++g_kernel_launches;
-  B200ST_LAUNCH_CHECK();
-  return 0;
+  return launch(dropout_bits_kernel, grid_for(ng, 256), 256, 0, s, drop, ng, out);
 }
 __global__ void __launch_bounds__(256) dropout_bits_multi_kernel(const DropBitsTable t, uint64_t seed, const uint64_t* seed_ptr,
                                                                   uint8_t* __restrict__ base) {
@@ -1053,10 +989,7 @@ __global__ void __launch_bounds__(256) dropout_bits_multi_kernel(const DropBitsT
 }
 int dropout_bits_multi(const DropBitsTable& t, uint64_t seed, const uint64_t* seed_ptr, uint8_t* base, cudaStream_t s) {
   if (t.n == 0 || t.goff[t.n] == 0) return 0;
-  launch_pdl(dropout_bits_multi_kernel, grid_for((t.goff[t.n] + 3) / 4, 256, 132 * 8), 256, 0, s, t, seed, seed_ptr, base);
-  ++g_kernel_launches;
-  B200ST_LAUNCH_CHECK();
-  return 0;
+  return launch(dropout_bits_multi_kernel, grid_for((t.goff[t.n] + 3) / 4, 256, 132 * 8), 256, 0, s, t, seed, seed_ptr, base);
 }
 __global__ void fill_kernel(float* __restrict__ x, float v, int64_t n) {
   pdl_wait();
@@ -1065,10 +998,7 @@ __global__ void fill_kernel(float* __restrict__ x, float v, int64_t n) {
 }
 int fill_f32(float* x, float v, int64_t n, cudaStream_t s) {
   if (n == 0) return 0;
-  launch_pdl(fill_kernel, grid_for(n, 256 * 4), 256, 0, s, x, v, n);
-  ++g_kernel_launches;
-  B200ST_LAUNCH_CHECK();
-  return 0;
+  return launch(fill_kernel, grid_for(n, 256 * 4), 256, 0, s, x, v, n);
 }
 
 }  // namespace b200st

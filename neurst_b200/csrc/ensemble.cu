@@ -54,15 +54,13 @@ __global__ void __launch_bounds__(kMixThreads) ensemble_logprob_kernel(const __g
 
 }  // namespace
 
-void ensemble_logprob(const EnsembleMix& mix, int rows, int V, cudaStream_t s) {
-  launch_pdl(ensemble_logprob_kernel, rows, kMixThreads, 0, s, mix, V);
-  ++g_kernel_launches;
+int ensemble_logprob(const EnsembleMix& mix, int rows, int V, cudaStream_t s) {
+  return launch(ensemble_logprob_kernel, rows, kMixThreads, 0, s, mix, V);
 }
 
-void beam_select_logprobs(const float* logprobs, const BeamState& bs, int utterances, int beam, int V, int eos, int unk, int min_len,
-                          float alpha, int max_len, cudaStream_t s) {
-  launch_pdl(beam_select_kernel<true>, utterances, 1024, 0, s, logprobs, bs, beam, V, eos, unk, min_len, alpha, max_len);
-  ++g_kernel_launches;
+int beam_select_logprobs(const float* logprobs, const BeamState& bs, int utterances, int beam, int V, int eos, int unk, int min_len,
+                         float alpha, int max_len, cudaStream_t s) {
+  return launch(beam_select_kernel<true>, utterances, 1024, 0, s, logprobs, bs, beam, V, eos, unk, min_len, alpha, max_len);
 }
 
 }  // namespace b200st

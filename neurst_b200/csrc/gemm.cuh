@@ -88,8 +88,6 @@ int fused_mlp_bwd(const void* dY, int dtype, int M, int d, int ffn, const void* 
 // SMs left to concurrent communication kernels: the persistent GEMM and fused-FFN grids are sized to the rest of the
 // device.  The model sets it while gradient all-reduces overlap the backward pass; 0 = none.
 void set_reserved_sms(int n);
-int64_t tc_launch_count();
-void tc_count_launch();
 void tc_profile_begin();
 bool tc_profile_active();   // per-launch event timing on: the model keeps every launch on one stream
 int tc_profile_end(double* ms, double* flops, int64_t* launches);

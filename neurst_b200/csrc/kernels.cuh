@@ -7,8 +7,6 @@
 
 namespace b200st {
 
-extern int64_t g_kernel_launches;
-
 // y = LN(x) (* gamma + beta) [relu]; x: [rows, cols] in x_dtype; y in y_dtype; optional fp32 copy y32.
 // mean / rstd (fp32 [rows]) may be null.  (neurst/layers/common_layers.py:64-65,77; audio_modalities.py:73-74,103-104)
 int layernorm_fwd(const void* x, int x_dtype, const float* gamma, const float* beta, float eps, void* y, int y_dtype,

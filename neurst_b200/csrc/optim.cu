@@ -167,22 +167,13 @@ __global__ void cast16_kernel(const float* __restrict__ x, T* __restrict__ y, in
     y[i] = from_f32<T>(x[i]);
 }
 
-int grid_for(int64_t work, int per_block, int cap = 132 * 16) {
-  int64_t g = (work + per_block - 1) / per_block;
-  if (g < 1) g = 1;
-  return (int)(g > cap ? cap : g);
-}
-
 }  // namespace
 
 int cast_f32_to_16(const float* x, void* y, int y_dtype, int64_t n, cudaStream_t s) {
   if (n == 0) return 0;
   B200ST_CHECK(is16(y_dtype), "cast_f32_to_16 needs a 16-bit destination type");
-  if (y_dtype == F16) launch_pdl(cast16_kernel<__half>, grid_for(n, 256 * 4), 256, 0, s, x, reinterpret_cast<__half*>(y), n);
-  else launch_pdl(cast16_kernel<__nv_bfloat16>, grid_for(n, 256 * 4), 256, 0, s, x, reinterpret_cast<__nv_bfloat16*>(y), n);
-  ++g_kernel_launches;
-  B200ST_LAUNCH_CHECK();
-  return 0;
+  if (y_dtype == F16) return launch(cast16_kernel<__half>, grid_for(n, 256 * 4), 256, 0, s, x, reinterpret_cast<__half*>(y), n);
+  return launch(cast16_kernel<__nv_bfloat16>, grid_for(n, 256 * 4), 256, 0, s, x, reinterpret_cast<__nv_bfloat16*>(y), n);
 }
 
 // gradient statistics + loss-scale control when clip_norm or the dynamic loss scale needs them
@@ -193,14 +184,10 @@ static int step_stats(const OptimArgs& a, const TensorTable& tt, cudaStream_t s)
   B200ST_CHECK(tt.n > 0 && tt.n <= 512, "clip_norm / dynamic loss scale support up to 512 parameter tensors");
   B200ST_CHECK(a.n % 8 == 0, "clip_norm / dynamic loss scale need an arena padded to a multiple of 8 elements");
   B200ST_CUDA(cudaMemsetAsync(a.tensor_sumsq, 0, sizeof(float) * (size_t)(tt.n + 1), s));
-  launch_pdl(grad_stats_kernel, grid_for(a.n, 8192, 132 * 8), 256, 0, s, (const float*)a.g, a.n, tt, a.tensor_sumsq);
-  ++g_kernel_launches;
-  if (a.ctl) { launch_pdl(latch_unscale_kernel, 1, 32, 0, s, a.ctl); ++g_kernel_launches; }
-  launch_pdl(step_control_kernel, 1, 32, 0, s, a.tensor_sumsq, tt.n, a.ctl, a.grad_scale, a.growth_steps > 0.f ? a.growth_steps : 2000.f,
-             a.multiplier > 1.f ? a.multiplier : 2.f);
-  ++g_kernel_launches;
-  B200ST_LAUNCH_CHECK();
-  return 0;
+  B200ST_TRY(launch(grad_stats_kernel, grid_for(a.n, 8192, 132 * 8), 256, 0, s, (const float*)a.g, a.n, tt, a.tensor_sumsq));
+  if (a.ctl) B200ST_TRY(launch(latch_unscale_kernel, 1, 32, 0, s, a.ctl));
+  return launch(step_control_kernel, 1, 32, 0, s, a.tensor_sumsq, tt.n, a.ctl, a.grad_scale, a.growth_steps > 0.f ? a.growth_steps : 2000.f,
+                a.multiplier > 1.f ? a.multiplier : 2.f);
 }
 
 static int check_arenas(const OptimArgs& a) {
@@ -218,11 +205,8 @@ int optimizer_step(const OptimArgs& a, const TensorTable& tt, cudaStream_t s) {
   const int grid = grid_for(a.n, 256 * 4 * 4);
   const uint8_t* no_mask = nullptr;
   const int32_t* no_turn = nullptr;
-  if (a.clip_norm > 0.f) launch_pdl(adam_kernel<true, false>, grid, 256, 0, s, a, tt, 1.f, no_mask, no_turn);
-  else launch_pdl(adam_kernel<false, false>, grid, 256, 0, s, a, tt, 1.f, no_mask, no_turn);
-  ++g_kernel_launches;
-  B200ST_LAUNCH_CHECK();
-  return 0;
+  if (a.clip_norm > 0.f) return launch(adam_kernel<true, false>, grid, 256, 0, s, a, tt, 1.f, no_mask, no_turn);
+  return launch(adam_kernel<false, false>, grid, 256, 0, s, a, tt, 1.f, no_mask, no_turn);
 }
 
 // The reference's pruning optimizer (neurst/sparsity/pruning_optimizer.py) inside the loss-scale optimizer: statistics and
@@ -239,10 +223,8 @@ int optimizer_step_pruned(const OptimArgs& a, const TensorTable& tt, const Prune
   const int grid = grid_for(a.n, 256 * 4 * 4);
   const uint8_t* mask = pd.mask;
   const int32_t* turn = pd.state + 1;
-  if (a.clip_norm > 0.f) launch_pdl(adam_kernel<true, true>, grid, 256, 0, s, a, tt, 1.f, mask, turn);
-  else launch_pdl(adam_kernel<false, true>, grid, 256, 0, s, a, tt, 1.f, mask, turn);
-  ++g_kernel_launches;
-  B200ST_LAUNCH_CHECK();
+  if (a.clip_norm > 0.f) B200ST_TRY(launch(adam_kernel<true, true>, grid, 256, 0, s, a, tt, 1.f, mask, turn));
+  else B200ST_TRY(launch(adam_kernel<false, true>, grid, 256, 0, s, a, tt, 1.f, mask, turn));
   return prune_select_apply(a.p, a.shadow, pt, pd, turn, s);
 }
 

@@ -216,10 +216,7 @@ int check_prune_table(const PruneTable& pt) {
 }
 
 int prune_control(const PruneTable& pt, const PruneSchedule& sc, const float* ctl, const PruneDev& pd, cudaStream_t s) {
-  launch_pdl(prune_control_kernel, 1, 256, 0, s, pt, sc, ctl, pd.state, pd.scratch, pd.scratch + kPruneMaxTensors);
-  ++g_kernel_launches;
-  B200ST_LAUNCH_CHECK();
-  return 0;
+  return launch(prune_control_kernel, 1, 256, 0, s, pt, sc, ctl, pd.state, pd.scratch, pd.scratch + kPruneMaxTensors);
 }
 
 int prune_select_apply(float* p, void* shadow, const PruneTable& pt, const PruneDev& pd, const int32_t* turn, cudaStream_t s) {
@@ -227,23 +224,18 @@ int prune_select_apply(float* p, void* shadow, const PruneTable& pt, const Prune
   uint32_t* prefix = pd.scratch + kPruneMaxTensors;
   uint32_t* counts = pd.scratch + kPruneScratchHead;
   const int grid = grid_chunks(pt);
-  launch_pdl(prune_hist_kernel<21, 11>, grid, 256, 0, s, (const float*)p, pt, turn, (const uint32_t*)prefix, counts);
-  launch_pdl(prune_pick_kernel<21, 11, false>, pt.n, 256, 0, s, turn, rank, prefix, counts, pd.thresholds);
-  launch_pdl(prune_hist_kernel<10, 11>, grid, 256, 0, s, (const float*)p, pt, turn, (const uint32_t*)prefix, counts);
-  launch_pdl(prune_pick_kernel<10, 11, false>, pt.n, 256, 0, s, turn, rank, prefix, counts, pd.thresholds);
-  launch_pdl(prune_hist_kernel<0, 10>, grid, 256, 0, s, (const float*)p, pt, turn, (const uint32_t*)prefix, counts);
-  launch_pdl(prune_pick_kernel<0, 10, true>, pt.n, 256, 0, s, turn, rank, prefix, counts, pd.thresholds);
-  launch_pdl(prune_apply_kernel, grid, 256, 0, s, p, reinterpret_cast<uint16_t*>(shadow), pt, turn, (const uint32_t*)prefix, pd.mask);
-  g_kernel_launches += 7;
-  B200ST_LAUNCH_CHECK();
-  return 0;
+  B200ST_TRY(launch(prune_hist_kernel<21, 11>, grid, 256, 0, s, (const float*)p, pt, turn, (const uint32_t*)prefix, counts));
+  B200ST_TRY(launch(prune_pick_kernel<21, 11, false>, pt.n, 256, 0, s, turn, rank, prefix, counts, pd.thresholds));
+  B200ST_TRY(launch(prune_hist_kernel<10, 11>, grid, 256, 0, s, (const float*)p, pt, turn, (const uint32_t*)prefix, counts));
+  B200ST_TRY(launch(prune_pick_kernel<10, 11, false>, pt.n, 256, 0, s, turn, rank, prefix, counts, pd.thresholds));
+  B200ST_TRY(launch(prune_hist_kernel<0, 10>, grid, 256, 0, s, (const float*)p, pt, turn, (const uint32_t*)prefix, counts));
+  B200ST_TRY(launch(prune_pick_kernel<0, 10, true>, pt.n, 256, 0, s, turn, rank, prefix, counts, pd.thresholds));
+  return launch(prune_apply_kernel, grid, 256, 0, s, p, reinterpret_cast<uint16_t*>(shadow), pt, turn, (const uint32_t*)prefix, pd.mask);
 }
 
 int prune_select(float* p, void* shadow, const PruneTable& pt, const int64_t* k, const PruneDev& pd, cudaStream_t s) {
   B200ST_TRY(check_prune_table(pt));
-  launch_pdl(prune_seed_kernel, 1, 256, 0, s, pt, k, pd.scratch);
-  ++g_kernel_launches;
-  B200ST_LAUNCH_CHECK();
+  B200ST_TRY(launch(prune_seed_kernel, 1, 256, 0, s, pt, k, pd.scratch));
   return prune_select_apply(p, shadow, pt, pd, reinterpret_cast<const int32_t*>(pd.scratch + 2 * kPruneMaxTensors), s);
 }
 

@@ -242,17 +242,15 @@ int check_sample_filter(int top_k, float top_p, int V) {
   return 0;
 }
 
-void sample_init(const BeamState& bs, const int64_t* bos, int rows, int sample_num, int max_len, int64_t* out, int max_steps,
-                 int eos, float* logprob, int32_t* length, cudaStream_t s) {
+int sample_init(const BeamState& bs, const int64_t* bos, int rows, int sample_num, int max_len, int64_t* out, int max_steps,
+                int eos, float* logprob, int32_t* length, cudaStream_t s) {
   const int64_t work = (int64_t)rows * (max_len > max_steps ? max_len : max_steps);
   const int grid = (int)std::min<int64_t>((work + 255) / 256, 132 * 8);
-  sample_init_kernel<<<grid, 256, 0, s>>>(bs, bos, rows, sample_num, max_len, out, max_steps, eos, logprob, length);
-  ++g_kernel_launches;
+  return launch_serial(sample_init_kernel, grid, 256, 0, s, bs, bos, rows, sample_num, max_len, out, max_steps, eos, logprob, length);
 }
 
-void sample_select(const SampleRows& a, int rows, cudaStream_t s) {
-  launch_pdl(sample_select_kernel<true>, rows, kSampleThreads, 0, s, a);
-  ++g_kernel_launches;
+int sample_select(const SampleRows& a, int rows, cudaStream_t s) {
+  return launch(sample_select_kernel<true>, rows, kSampleThreads, 0, s, a);
 }
 
 int sample_logits(const float* logits, int rows, int V, int top_k, float top_p, uint64_t seed, int64_t row_offset, int step,
@@ -265,10 +263,7 @@ int sample_logits(const float* logits, int rows, int V, int top_k, float top_p, 
   a.logits = logits; a.V = V; a.eos = -1; a.unk = -1; a.min_len = 0;
   a.top_k = top_k; a.top_p = top_p; a.seed = seed; a.row_offset = row_offset; a.step = step;
   a.out = out; a.max_steps = 1;
-  launch_pdl(sample_select_kernel<false>, rows, kSampleThreads, 0, s, a);
-  ++g_kernel_launches;
-  B200ST_LAUNCH_CHECK();
-  return 0;
+  return launch(sample_select_kernel<false>, rows, kSampleThreads, 0, s, a);
 }
 
 }  // namespace b200st

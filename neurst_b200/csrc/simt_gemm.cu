@@ -82,9 +82,7 @@ int gemm_simt_f32(const GemmArgs& g, cudaStream_t stream) {
   const int64_t nb = (int64_t)g.nb1 * g.nb2;
   B200ST_CHECK(nb <= 65535 && ceil_div(g.M, TM) <= 65535, "grid too large for SIMT GEMM");
   dim3 grid(ceil_div(g.N, TN), ceil_div(g.M, TM), (unsigned)nb);
-  launch_pdl(simt_gemm_kernel, grid, 256, 0, stream, g);
-  B200ST_LAUNCH_CHECK();
-  return 0;
+  return launch(simt_gemm_kernel, grid, 256, 0, stream, g);
 }
 
 int gemm(const GemmArgs& g, cudaStream_t stream) {

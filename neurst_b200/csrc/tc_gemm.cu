@@ -906,7 +906,6 @@ int make_out_map_f32(float* ptr, int M, int d, CUtensorMap* out) {
 
 int g_num_sms = 0;
 int g_reserved_sms = 0;
-int64_t g_launches = 0;
 
 // SMs a persistent grid may fill: the device's, less those reserved for communication kernels (set_reserved_sms)
 int usable_sms(int* out) {
@@ -926,7 +925,6 @@ int make_tma_map_16(const void* ptr, int dtype, uint64_t inner, uint64_t rows, i
   GemmOperand op{ptr, dtype, 0, ld, sb1, sb2};
   return make_operand_map(op, (int)rows, (int)inner, nb1, nb2, (int)box_rows, out);
 }
-void tc_count_launch() { ++g_launches; }
 
 namespace {
 
@@ -952,9 +950,7 @@ int launch_kernel(const CUtensorMap& ta, const CUtensorMap& tb, const TcParams& 
     B200ST_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemLimit));
     attr_set = true;
   }
-  launch_pdl(kern, grid, kThreads, smem, stream, ta, tb, p);
-  B200ST_LAUNCH_CHECK();
-  return 0;
+  return launch(kern, grid, kThreads, smem, stream, ta, tb, p);
 }
 
 template <int BN, bool A_MN, bool B_MN>
@@ -975,7 +971,6 @@ int launch_bn(bool a_mn, bool b_mn, bool bf, const CUtensorMap& ta, const CUtens
 }  // namespace
 
 void set_reserved_sms(int n) { g_reserved_sms = n; }
-int64_t tc_launch_count() { return g_launches; }
 
 namespace {
 int gemm_tc_impl(const GemmArgs& g, cudaStream_t stream, const ConvA* conv);
@@ -1094,7 +1089,6 @@ int gemm_tc_impl(const GemmArgs& g, cudaStream_t stream, const ConvA* conv) {
 
   const int max_grid = num_sms;
   const int grid = (int)(p.num_tiles < max_grid ? p.num_tiles : max_grid);
-  ++g_launches;
   if (g_prof) {
     ProfRec r{g, stream, bn, splitk};
     if (conv) { r.has_conv = true; r.conv = *conv; }
@@ -1214,16 +1208,13 @@ int gemm_wgrad_group(const GemmArgs* gs, int n, cudaStream_t stream) {
     attr_set[gs[0].A.dtype == BF16] = true;
   }
   const int grid = grp.num_tiles < num_sms ? grp.num_tiles : num_sms;
-  ++g_launches;
   if (g_prof) {
     ProfRec r{gs[0], stream, 256, grp.prob[0].splitk};
     r.group_n = n;
     for (int i = 1; i < n; ++i) r.rest[i - 1] = gs[i];
     g_prof_recs.push_back(r);
   }
-  launch_pdl(kern, grid, kThreads, smem, stream, grp);
-  B200ST_LAUNCH_CHECK();
-  return 0;
+  return launch(kern, grid, kThreads, smem, stream, grp);
 }
 
 
@@ -1273,10 +1264,7 @@ int fused_mlp_fwd(const void* X, int dtype, int M, int d, int ffn, const void* W
     B200ST_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kMlpSmem));
     attr[ai] = true;
   }
-  launch_pdl(kern, m_tiles * splits, kMlpThreads, kMlpSmem, stream, tx, tw1, tw2, to, p);
-  ++g_launches;
-  B200ST_LAUNCH_CHECK();
-  return 0;
+  return launch(kern, m_tiles * splits, kMlpThreads, kMlpSmem, stream, tx, tw1, tw2, to, p);
 }
 
 // Fused FFN backward, data-gradient chain: dF1 = scale * (dY W2^T) masked by (F1 > 0)  [written for the W1 weight gradient],
@@ -1308,10 +1296,7 @@ int fused_mlp_bwd(const void* dY, int dtype, int M, int d, int ffn, const void* 
     B200ST_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kMlpSmem));
     attr[ai] = true;
   }
-  launch_pdl(kern, m_tiles * splits, kMlpThreads, kMlpSmem, stream, tx, tw1, tw2, to, p);
-  ++g_launches;
-  B200ST_LAUNCH_CHECK();
-  return 0;
+  return launch(kern, m_tiles * splits, kMlpThreads, kMlpSmem, stream, tx, tw1, tw2, to, p);
 }
 
 void tc_profile_begin() {
