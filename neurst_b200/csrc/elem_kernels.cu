@@ -315,8 +315,11 @@ __global__ void __launch_bounds__(256, 2) ln_bwd_vec_kernel(const TDY* __restric
           if (dnext) {
             // the consumer block's first op fused here: dY = cast(dropout'(dx)) in the activation dtype
             const float nscale = ndrop.p > 0.f ? ndrop.scale : 1.f;
+            // element e = row * cols + c + j keeps bit e & 7 of byte e >> 3; c % 4 == 0, so that bit is
+            // ((row * cols + c) & 4) + j (not (c & 4) + j: row * cols need not be a multiple of 8, e.g. cols % 8 == 4)
+            const int bit0 = (int)((row * cols + c) & 4);
 #pragma unroll
-            for (int j = 0; j < 4; ++j) o[j] = ((kb[r][i] >> ((c & 4) + j)) & 1u) ? o[j] * nscale : 0.f;
+            for (int j = 0; j < 4; ++j) o[j] = ((kb[r][i] >> (bit0 + j)) & 1u) ? o[j] * nscale : 0.f;
             if (dnext_dt == BF16) store4<__nv_bfloat16>(reinterpret_cast<__nv_bfloat16*>(dnext) + row * cols + c, o);
             else if (dnext_dt == F16) store4<__half>(reinterpret_cast<__half*>(dnext) + row * cols + c, o);
             else store4<float>(reinterpret_cast<float*>(dnext) + row * cols + c, o);

@@ -36,13 +36,13 @@ def test_forward_bf16_vs_reference_fixture():
     assert err < 5e-2, err
 
 
-@pytest.mark.parametrize("precision,tol_logits,tol_grad", [("fp32", 1e-4, 2e-4), ("fp16", 8e-3, 5e-2), ("bf16", 6e-2, 1e-1)])
-@pytest.mark.parametrize("dropout", [0.0, 0.1])
-@pytest.mark.parametrize("channels", [64, 256])      # 256 = the production front-end kernels (normalised-save conv1 path)
-def test_forward_backward_vs_oracle(precision, tol_logits, tol_grad, dropout, channels):
-    cfg = dict(model="speech", d=64, heads=4, enc_layers=2, dec_layers=2, ffn=128, channels=channels, feat=80, in_channels=1, vocab=96)
+TOL = {"fp32": (1e-4, 2e-4), "fp16": (8e-3, 5e-2), "bf16": (6e-2, 1e-1)}     # logits max-abs, gradient relative L2
+
+
+def check_step_vs_oracle(cfg, precision, dropout, B, T, Lq, tol_logits, tol_grad):
+    """One training step (forward, label-smoothed loss, backward) through the C ABI against the fp64 oracle with the
+    library's own dropout masks: logits, loss, token counts and every gradient tensor."""
     P = R.init_params(cfg, seed=7, random_bias=True)
-    B, T, Lq = 3, 61, 9
     batch = U.synthetic_speech_batch(cfg, B, T, Lq, seed=3)
     rt = U.speech_runtime(cfg, precision, dropout=dropout, label_smoothing=0.1)
     rt.load_parameters(P)
@@ -54,17 +54,68 @@ def test_forward_backward_vs_oracle(precision, tol_logits, tol_grad, dropout, ch
     T2 = R.length_after_conv(T)
     masks = U.dropout_masks(rt, cfg, B, T2, Lq, dropout, seed) if dropout > 0 else R.NO_DROPOUT
     logits, loss, grads = U.oracle_loss_and_grads(P, cfg, batch, 0.1, masks)
-    assert float((out["logits"].cpu().double() - logits).abs().max()) < tol_logits
-    assert abs(float(out["loss"]) - float(loss)) < tol_logits * max(1.0, abs(float(loss)))
-    nt = batch["trg_length"].clamp(max=Lq).float()
-    assert torch.equal(out["n_tokens"].cpu(), nt)
+    e_logits = float((out["logits"].cpu().double() - logits).abs().max())
     worst = ("", 0.0)
     S = float(rt.loss_scale_state[0]) if rt.fp16 else 1.0      # fp16: gradients carry the dynamic loss scale
     for k, g in grads.items():
         e = U.rel_err(rt.grad_view(k) / S, g)
         if e > worst[1]:
             worst = (k, e)
+    print("\n[%s d=%d H=%d ffn=%d V=%d B=%d T=%d (T2=%d) L=%d p=%.1f] logits max-abs %.3e | loss %.6f vs %.6f | worst grad %s %.2e"
+          % (precision, cfg["d"], cfg["heads"], cfg["ffn"], cfg["vocab"], B, T, T2, Lq, dropout, e_logits, float(out["loss"]),
+             float(loss), worst[0], worst[1]))
+    assert e_logits < tol_logits
+    assert abs(float(out["loss"]) - float(loss)) < tol_logits * max(1.0, abs(float(loss)))
+    nt = batch["trg_length"].clamp(max=Lq).float()
+    assert torch.equal(out["n_tokens"].cpu(), nt)
     assert worst[1] < tol_grad, worst
+
+
+@pytest.mark.parametrize("precision,tol_logits,tol_grad", [(p,) + TOL[p] for p in ("fp32", "fp16", "bf16")])
+@pytest.mark.parametrize("dropout", [0.0, 0.1])
+@pytest.mark.parametrize("channels", [64, 256])      # 256 = the production front-end kernels (normalised-save conv1 path)
+def test_forward_backward_vs_oracle(precision, tol_logits, tol_grad, dropout, channels):
+    cfg = dict(model="speech", d=64, heads=4, enc_layers=2, dec_layers=2, ffn=128, channels=channels, feat=80, in_channels=1, vocab=96)
+    check_step_vs_oracle(cfg, precision, dropout, 3, 61, 9, tol_logits, tol_grad)
+
+
+def speech_cfg(d, heads, ffn, vocab, channels=8):
+    return dict(model="speech", d=d, heads=heads, enc_layers=2, dec_layers=2, ffn=ffn, channels=channels, feat=80, in_channels=1,
+                vocab=vocab)
+
+
+# Shapes that select the row kernels' other branches (neurst_b200/csrc/elem_kernels.cu).  The unfused attention path (fp32, or
+# 16-bit with head dim != 64) runs softmax_fwd/bwd with STEPS = ceil(Tk / 256) rounded up to 1, 2, 4 or 8; T2 is the key
+# length after the two stride-2 convolutions, R.length_after_conv(T): T = 1204 -> 301, 3028 -> 757, 4804 -> 1201.
+BRANCH_CASES = [
+    # d % 8 == 4: ln_bwd_vec_kernel hands dY to the next backward block through the dropout bitmap at rows whose first
+    # element is not on a byte boundary; V = 97: the scalar lsce_kernel (V % 4 != 0) and scalar colsum_kernel (V % 8 != 0)
+    pytest.param(speech_cfg(12, 3, 20, 97), "fp32", 0.1, 3, 61, 9, id="d12-fp32-p0.1"),
+    pytest.param(speech_cfg(12, 3, 20, 97), "fp32", 0.0, 3, 61, 9, id="d12-fp32-p0"),
+    # d % 4 != 0: ln_fwd_kernel and ln_bwd_kernel, then the separate cast_dropout for the next block's dY
+    pytest.param(speech_cfg(10, 2, 14, 96), "fp32", 0.1, 3, 61, 9, id="d10-fp32-p0.1"),
+    # long keys on the unfused path: encoder self-attention and cross-attention at Tk = T2 (STEPS 2, 4, 8, Tk % 8 != 0),
+    # decoder self-attention at Tk = Lq = 261 (causal, STEPS 2)
+    pytest.param(speech_cfg(16, 2, 24, 96), "fp32", 0.1, 2, 1204, 261, id="T2_301-L261-fp32"),
+    pytest.param(speech_cfg(16, 2, 24, 96), "fp32", 0.1, 2, 3028, 9, id="T2_757-fp32"),
+    pytest.param(speech_cfg(16, 2, 24, 96), "fp32", 0.1, 2, 4804, 9, id="T2_1201-fp32"),
+    # 16-bit P (dropout on the rounded probabilities), head dim 32: not the fused kernel
+    pytest.param(speech_cfg(64, 2, 128, 96), "bf16", 0.1, 2, 1204, 9, id="T2_301-bf16"),
+    pytest.param(speech_cfg(64, 2, 128, 96), "fp16", 0.1, 2, 1204, 9, id="T2_301-fp16"),
+    pytest.param(speech_cfg(64, 2, 128, 96), "bf16", 0.1, 2, 3028, 9, id="T2_757-bf16"),
+    pytest.param(speech_cfg(64, 2, 128, 96), "fp16", 0.1, 2, 3028, 9, id="T2_757-fp16"),
+    # vocabulary: 8200 -> lsce_vec_kernel<32> and the vector colsum; above 32768 -> the scalar lsce_kernel (bf16: 16-bit
+    # dlogits)
+    pytest.param(speech_cfg(16, 2, 24, 8200), "fp32", 0.1, 2, 61, 9, id="V8200-fp32"),
+    pytest.param(speech_cfg(16, 2, 24, 8200), "bf16", 0.1, 2, 61, 9, id="V8200-bf16"),
+    pytest.param(speech_cfg(16, 2, 24, 32776), "bf16", 0.1, 2, 61, 9, id="V32776-bf16"),
+    pytest.param(speech_cfg(16, 2, 24, 40000), "fp32", 0.1, 2, 61, 9, id="V40000-fp32"),
+]
+
+
+@pytest.mark.parametrize("cfg,precision,dropout,B,T,Lq", BRANCH_CASES)
+def test_row_kernel_branches_vs_oracle(cfg, precision, dropout, B, T, Lq):
+    check_step_vs_oracle(cfg, precision, dropout, B, T, Lq, *TOL[precision])
 
 
 def test_kat_text_transformer_toy_fp32():
