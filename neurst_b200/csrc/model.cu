@@ -166,14 +166,17 @@ struct Ctx {
   bool side_pending[2] = {false, false};
   int bwd_blocks = 0;
   int cur_par = 0;
-  // Start of a backward block: picks the gradient-scratch parity and waits for the side-stream readers of that parity
-  // (issued two blocks ago) before the block overwrites it.
+  // waits on `st` for the side-stream readers of gradient-scratch parity `par` (issued two blocks ago)
+  void wait_side(int par) {
+    if (side && !dry && side_pending[par]) {
+      if (cudaStreamWaitEvent(st, side->done[par], 0) != cudaSuccess) launch_failed = true;
+      side_pending[par] = false;
+    }
+  }
+  // Start of a backward block: picks the gradient-scratch parity; its readers must be done before the block overwrites it.
   int begin_bwd_block() {
     cur_par = (bwd_blocks++) & 1;
-    if (side && !dry && side_pending[cur_par]) {
-      if (cudaStreamWaitEvent(st, side->done[cur_par], 0) != cudaSuccess) launch_failed = true;
-      side_pending[cur_par] = false;
-    }
+    wait_side(cur_par);
     return cur_par;
   }
   // stream for a weight-gradient launch whose inputs were produced on `st` so far
@@ -191,26 +194,17 @@ struct Ctx {
     side_pending[cur_par] = true;
   }
   // Fused hand-over between backward blocks: the final LayerNorm-backward of a block also writes the NEXT block's
-  // dY = cast(dropout'(dx)) into that block's parity buffer (set by the stack loop through `next_drop`).
-  const DropoutSpec* next_drop = nullptr;   // post-dropout site of the block that runs next (null: no fused hand-over)
+  // dY = cast(dropout'(dx)) into that block's parity buffer (set by the stack walk through `next_drop`).
+  DropoutSpec next_drop = no_dropout();     // post-dropout site of the block that runs next
+  bool has_next_drop = false;               // next_drop is set: the fused hand-over is on
   bool dy_ready = false;                    // the previous block already produced this block's dY
-  // parity the next block will select; its side-stream readers (two blocks ago) must be done before it is overwritten
+  // parity the next block will select; its side-stream readers must be done before it is overwritten
   int next_parity_ready() {
     const int par = bwd_blocks & 1;
-    if (side && !dry && side_pending[par]) {
-      if (cudaStreamWaitEvent(st, side->done[par], 0) != cudaSuccess) launch_failed = true;
-      side_pending[par] = false;
-    }
+    wait_side(par);
     return par;
   }
-  void join_side() {
-    if (!side || dry) return;
-    for (int i = 0; i < 2; ++i)
-      if (side_pending[i]) {
-        if (cudaStreamWaitEvent(st, side->done[i], 0) != cudaSuccess) launch_failed = true;
-        side_pending[i] = false;
-      }
-  }
+  void join_side() { wait_side(0); wait_side(1); }
   // ---- data-parallel gradient buckets (comm.cu): [lo, hi) of the arena is final -> all-reduce it on the comm stream ----
   GradSync* sync = nullptr;
   int64_t sync_hi = 0;       // everything at or above this arena offset has already been handed to NCCL
@@ -318,11 +312,6 @@ static int need_param(const Ctx& c, const std::string& n) {
   return 0;
 }
 
-struct Scratch;
-// final LayerNorm-backward of a block (+ fused production of the next block's dY when the stack loop announced one)
-static int block_ln_bwd(Ctx& c, Scratch& sc, const float* dh, const float* x_in, const float* mean, const float* rstd,
-                        const std::string& pre, const float* dx_out, float* dx_in, int M, int d);
-
 // ---- dense layers:  weights stored [K_in, N_out] (TF layout) -----------------------------------
 // Y[M,N] = epi(X[M,K] W)
 static int linear_fwd(Ctx& c, const void* X, int64_t ldx, int M, int K, int N, const std::string& w, const std::string& b,
@@ -397,16 +386,17 @@ static int flush_wgrads(Ctx& c) {
   c.wgrad_done(ws);
   return 0;
 }
-struct WgradBlock {          // scope of one backward block: defers linear_wgrad launches until flush()
-  Ctx& c;
-  explicit WgradBlock(Ctx& cc) : c(cc) { c.defer_wgrads = true; }
-  int flush() { c.defer_wgrads = false; return flush_wgrads(c); }
-  ~WgradBlock() { c.defer_wgrads = false; }
-};
 
 // ---- attention core on projected q/k/v views ----------------------------------------------------
 struct View { void* ptr; int64_t ld; };   // [B*T, ld] row-major, heads at column offset h*dh
 struct AttnDims { int B, H, Tq, Tk, units; };
+
+struct QkvViews { View q, k, v; };
+// self-attention (kv null): q/k/v side by side in one [M,3u] projection; cross-attention: q [M,u], k/v side by side in kv [Mk,2u]
+static QkvViews qkv_views(const Ctx& c, void* qkv, void* kv, int u) {
+  if (!kv) return {{qkv, 3 * u}, {c.act_off(qkv, u), 3 * u}, {c.act_off(qkv, 2 * u), 3 * u}};
+  return {{qkv, u}, {kv, 2 * u}, {c.act_off(kv, u), 2 * u}};
+}
 
 static GemmOperand head_op(const Ctx& c, View v, int T, int dh, int mn_major) {
   return GemmOperand{v.ptr, c.adt, mn_major, v.ld, dh, (int64_t)T * v.ld};
@@ -491,9 +481,13 @@ static int attention_bwd(Ctx& c, const AttnDims& a, View q, View k, View v, cons
 }
 
 // ---- saved activations ---------------------------------------------------------------------------
-struct AttnSave {
+struct PrenormSave {        // what every pre-norm block saves: its input, LN(input) and the LayerNorm statistics
   const float* x_in = nullptr;
   void* h = nullptr; float* mean = nullptr; float* rstd = nullptr;
+  int M = 0;
+  uint64_t s_post = 0;
+};
+struct AttnSave : PrenormSave {
   void* qkv = nullptr;      // self: [M,3u]; cross: q [M,u]
   void* kv = nullptr;       // cross: [Mk,2u]
   void* p_pre = nullptr; void* p_drop = nullptr; void* ctx = nullptr;
@@ -501,14 +495,11 @@ struct AttnSave {
   const void* mem = nullptr; // cross: memory in act dtype [Mk, d]
   const float* bias = nullptr; KeyMask mask = no_key_mask();
   AttnDims dims{};
-  uint64_t s_attn = 0, s_post = 0;
+  uint64_t s_attn = 0;
 };
-struct FfnSave {
-  const float* x_in = nullptr;
-  void* h = nullptr; float* mean = nullptr; float* rstd = nullptr;
+struct FfnSave : PrenormSave {
   void* f1 = nullptr;
-  int M = 0;
-  uint64_t s_ffn = 0, s_post = 0;
+  uint64_t s_ffn = 0;
 };
 
 struct Scratch {   // shared transient buffers (sized for the largest sublayer)
@@ -526,132 +517,110 @@ struct Scratch {   // shared transient buffers (sized for the largest sublayer)
   float* dq32 = nullptr;    // [M,d] fp32 (fused attention: dQ reduction across kv blocks)
 };
 
-static int block_ln_bwd(Ctx& c, Scratch& sc, const float* dh, const float* x_in, const float* mean, const float* rstd,
-                        const std::string& pre, const float* dx_out, float* dx_in, int M, int d) {
-  void* dnext = nullptr;
-  DropoutSpec nd = no_dropout();
-  if (c.next_drop) {
-    dnext = sc.dY2[c.next_parity_ready()];
-    nd = *c.next_drop;
-    c.next_drop = nullptr;
-    c.dy_ready = true;
-  }
-  RUN(layernorm_bwd_next(dh, F32, x_in, F32, mean, rstd, c.P(pre + ".ln.gamma"), c.P(pre + ".ln.beta"), dx_out, dx_in, F32,
-                         c.G(pre + ".ln.gamma"), c.G(pre + ".ln.beta"), M, d, 0, dnext, c.adt, nd, c.st));
+// First step of a pre-norm block's forward: LN(x_in) and its statistics come first in the block's workspace; the block
+// allocates the rest before prenorm_fwd() launches the LayerNorm.
+static void prenorm_alloc(Ctx& c, const std::string& pre, const float* x_in, int M, PrenormSave& sv) {
+  sv.x_in = x_in; sv.M = M;
+  sv.s_post = dropout_stream_id(pre + ".post_drop");
+  sv.h = c.act((int64_t)M * c.m.cfg.d); sv.mean = c.f32(M); sv.rstd = c.f32(M);
+}
+// h = LN(x_in); xcopy (the fused FFN's residual seed, else null) also receives x_in
+static int prenorm_fwd(Ctx& c, const std::string& pre, const PrenormSave& sv, float* xcopy) {
+  const Config& cf = c.m.cfg;
+  RUN(layernorm_fwd_copy(sv.x_in, F32, c.P(pre + ".ln.gamma"), c.P(pre + ".ln.beta"), cf.ln_eps, sv.h, c.adt, nullptr, sv.mean,
+                         sv.rstd, sv.M, cf.d, 0, xcopy, c.st));
   return 0;
 }
 
-// x_out = x_in + dropout(Attn(LN(x_in)))  — pre-norm block (common_layers.py:73-85)
-static int self_attn_block_fwd(Ctx& c, const std::string& pre, const float* x_in, float* x_out, int B, int T, const float* bias,
-                               KeyMask mask, Scratch& sc, AttnSave& sv) {
+// Scope of one backward block.  The constructor selects the gradient-scratch parity, defers the block's linear_wgrad
+// launches until flush(), and puts the block's dY = cast(dropout'(dx_out)) in sc.dY unless the previous block's
+// LayerNorm-backward already wrote it there; `rc` is that launch's result.  finish() runs the block's LayerNorm-backward,
+// which also writes the next block's dY when the stack walk handed one over, and flushes.
+struct BwdBlock {
+  Ctx& c; Scratch& sc; const std::string& pre; const PrenormSave& sv; const float* dx_out; float* dx_in;
+  int rc = 0;
+  BwdBlock(Ctx& cc, Scratch& s, const std::string& p, const PrenormSave& v, const float* dxo, float* dxi)
+      : c(cc), sc(s), pre(p), sv(v), dx_out(dxo), dx_in(dxi) {
+    sc.select(c.begin_bwd_block());
+    c.defer_wgrads = true;
+    if (c.dy_ready) c.dy_ready = false;
+    else if (!c.dry)
+      rc = cast_dropout(dx_out, sc.dY, c.adt, (int64_t)sv.M * c.m.cfg.d, c.drop(c.m.cfg.postprocess_dropout, sv.s_post), c.st);
+  }
+  ~BwdBlock() { c.defer_wgrads = false; }
+  int flush() { c.defer_wgrads = false; return flush_wgrads(c); }
+  int finish() {
+    void* dnext = nullptr;
+    DropoutSpec nd = no_dropout();
+    if (c.has_next_drop) {
+      dnext = sc.dY2[c.next_parity_ready()];
+      nd = c.next_drop;
+      c.has_next_drop = false;
+      c.dy_ready = true;
+    }
+    RUN(layernorm_bwd_next(sc.dh, F32, sv.x_in, F32, sv.mean, sv.rstd, c.P(pre + ".ln.gamma"), c.P(pre + ".ln.beta"), dx_out, dx_in,
+                           F32, c.G(pre + ".ln.gamma"), c.G(pre + ".ln.beta"), sv.M, c.m.cfg.d, 0, dnext, c.adt, nd, c.st));
+    return flush();
+  }
+};
+
+// x_out = x_in + dropout(Attn(LN(x_in)))  — pre-norm block (common_layers.py:73-85).  mem == nullptr: self-attention over
+// LN(x_in) (Tk = Tq); else cross-attention with q from LN(x_in) and k/v from the memory (act dtype [B*Tk, d]).
+static int attn_block_fwd(Ctx& c, const std::string& pre, const float* x_in, float* x_out, int B, int Tq, const void* mem, int Tk,
+                          const float* bias, KeyMask mask, Scratch& sc, AttnSave& sv) {
   const Config& cf = c.m.cfg;
-  const int d = cf.d, M = B * T, Tkp = round8(T);
-  sv.x_in = x_in;
-  sv.dims = AttnDims{B, cf.heads, T, T, d};
+  const int d = cf.d, M = B * Tq, Mk = B * Tk, Tkp = round8(Tk), nq = mem ? d : 3 * d;
+  const std::string q = pre + (mem ? ".q" : ".qkv");
+  sv.mem = mem;
+  sv.dims = AttnDims{B, cf.heads, Tq, Tk, d};
   sv.bias = bias; sv.mask = mask;
-  sv.s_attn = dropout_stream_id(pre + ".attn_drop"); sv.s_post = dropout_stream_id(pre + ".post_drop");
-  sv.h = c.act((int64_t)M * d); sv.mean = c.f32(M); sv.rstd = c.f32(M);
-  sv.qkv = c.act((int64_t)M * 3 * d);
-  const DropoutSpec adrop = c.drop(cf.attention_dropout, sv.s_attn, (int64_t)B * cf.heads * T * Tkp);
+  sv.s_attn = dropout_stream_id(pre + ".attn_drop");
+  prenorm_alloc(c, pre, x_in, M, sv);
+  sv.qkv = c.act((int64_t)M * nq);
+  if (mem) sv.kv = c.act((int64_t)Mk * 2 * d);
+  const DropoutSpec adrop = c.drop(cf.attention_dropout, sv.s_attn, (int64_t)B * cf.heads * Tq * Tkp);
   if (use_fused_attention(c, sv.dims)) {
-    sv.lse = c.f32((int64_t)B * cf.heads * T);
+    sv.lse = c.f32((int64_t)B * cf.heads * Tq);
   } else {
-    sv.p_pre = c.act((int64_t)B * cf.heads * T * Tkp);
-    sv.p_drop = adrop.p > 0.f ? c.act((int64_t)B * cf.heads * T * Tkp) : nullptr;
+    sv.p_pre = c.act((int64_t)B * cf.heads * Tq * Tkp);
+    sv.p_drop = adrop.p > 0.f ? c.act((int64_t)B * cf.heads * Tq * Tkp) : nullptr;
   }
   sv.ctx = c.act((int64_t)M * d);
-  RUN(layernorm_fwd(x_in, F32, c.P(pre + ".ln.gamma"), c.P(pre + ".ln.beta"), cf.ln_eps, sv.h, c.adt, nullptr, sv.mean, sv.rstd,
-                    M, d, 0, c.st));
+  B200ST_TRY(prenorm_fwd(c, pre, sv, nullptr));
   GemmEpilogue e0 = gemm_defaults().epi;
-  B200ST_TRY(linear_fwd(c, sv.h, d, M, d, 3 * d, pre + ".qkv.kernel", pre + ".qkv.bias", e0, sv.qkv, c.adt, 3 * d));
-  View q{sv.qkv, 3 * d}, k{c.act_off(sv.qkv, d), 3 * d}, v{c.act_off(sv.qkv, 2 * d), 3 * d};
-  B200ST_TRY(attention_fwd(c, sv.dims, q, k, v, bias, mask, adrop, sc.S, sv.p_pre, sv.p_drop, sv.ctx, sv.lse));
+  B200ST_TRY(linear_fwd(c, sv.h, d, M, d, nq, q + ".kernel", q + ".bias", e0, sv.qkv, c.adt, nq));
+  if (mem) B200ST_TRY(linear_fwd(c, mem, d, Mk, d, 2 * d, pre + ".kv.kernel", pre + ".kv.bias", e0, sv.kv, c.adt, 2 * d));
+  const QkvViews a = qkv_views(c, sv.qkv, sv.kv, d);
+  B200ST_TRY(attention_fwd(c, sv.dims, a.q, a.k, a.v, bias, mask, adrop, sc.S, sv.p_pre, sv.p_drop, sv.ctx, sv.lse));
   GemmEpilogue e1 = gemm_defaults().epi;
   e1.drop = c.drop(cf.postprocess_dropout, sv.s_post, (int64_t)M * d);
   e1.residual = x_in; e1.res_ld = d;
-  B200ST_TRY(linear_fwd(c, sv.ctx, d, M, d, d, pre + ".out.kernel", pre + ".out.bias", e1, x_out, F32, d));
-  return 0;
+  return linear_fwd(c, sv.ctx, d, M, d, d, pre + ".out.kernel", pre + ".out.bias", e1, x_out, F32, d);
 }
 
-static int self_attn_block_bwd(Ctx& c, const std::string& pre, const float* dx_out, float* dx_in, Scratch& sc, const AttnSave& sv) {
-  sc.select(c.begin_bwd_block());
-  WgradBlock wb(c);
+// dmem: fp32 [Mk,d] memory gradient, accumulated by cross-attention (unused by self-attention)
+static int attn_block_bwd(Ctx& c, const std::string& pre, const float* dx_out, float* dx_in, float* dmem, Scratch& sc,
+                          const AttnSave& sv) {
+  BwdBlock bb(c, sc, pre, sv, dx_out, dx_in);
+  B200ST_TRY(bb.rc);
   const Config& cf = c.m.cfg;
-  const int d = cf.d, M = sv.dims.B * sv.dims.Tq;
-  if (c.dy_ready) c.dy_ready = false;      // produced by the previous block's LayerNorm-backward
-  else RUN(cast_dropout(dx_out, sc.dY, c.adt, (int64_t)M * d, c.drop(cf.postprocess_dropout, sv.s_post), c.st));
+  const int d = cf.d, M = sv.M, Mk = sv.dims.B * sv.dims.Tk, nq = sv.mem ? d : 3 * d;
+  const std::string q = pre + (sv.mem ? ".q" : ".qkv");
   B200ST_TRY(linear_wgrad(c, sv.ctx, d, sc.dY, d, M, d, d, pre + ".out.kernel", pre + ".out.bias"));
   GemmEpilogue e0 = gemm_defaults().epi;
   B200ST_TRY(linear_dgrad(c, sc.dY, d, M, d, d, pre + ".out.kernel", e0, sc.dctx, c.adt, d));
-  View q{sv.qkv, 3 * d}, k{c.act_off(sv.qkv, d), 3 * d}, v{c.act_off(sv.qkv, 2 * d), 3 * d};
-  View dq{sc.dqkv, 3 * d}, dk{c.act_off(sc.dqkv, d), 3 * d}, dv{c.act_off(sc.dqkv, 2 * d), 3 * d};
-  B200ST_TRY(attention_bwd(c, sv.dims, q, k, v, sv.p_pre, sv.p_drop, c.drop(cf.attention_dropout, sv.s_attn), sc.dctx, sc.S, sc.dS,
-                           dq, dk, dv, sv.ctx, sv.lse, sv.bias, sv.mask, sc.dq32));
-  B200ST_TRY(linear_wgrad(c, sv.h, d, sc.dqkv, 3 * d, M, d, 3 * d, pre + ".qkv.kernel", pre + ".qkv.bias"));
-  B200ST_TRY(wb.flush());      // every dY of the block exists: the side stream starts under the rest of the chain
-  B200ST_TRY(linear_dgrad(c, sc.dqkv, 3 * d, M, 3 * d, d, pre + ".qkv.kernel", e0, sc.dh, F32, d));
-  B200ST_TRY(block_ln_bwd(c, sc, sc.dh, sv.x_in, sv.mean, sv.rstd, pre, dx_out, dx_in, M, d));
-  return wb.flush();
-}
-
-// cross attention: q from LN(x), k/v from memory (act dtype, [B*Tm, d]); memory_bias [B,Tm]
-static int cross_attn_block_fwd(Ctx& c, const std::string& pre, const float* x_in, float* x_out, int B, int L, const void* mem,
-                                int Tm, const float* mem_bias, Scratch& sc, AttnSave& sv) {
-  const Config& cf = c.m.cfg;
-  const int d = cf.d, M = B * L, Mk = B * Tm, Tkp = round8(Tm);
-  sv.x_in = x_in; sv.mem = mem;
-  sv.dims = AttnDims{B, cf.heads, L, Tm, d};
-  sv.bias = mem_bias; sv.mask = c.cross_mask;
-  sv.s_attn = dropout_stream_id(pre + ".attn_drop"); sv.s_post = dropout_stream_id(pre + ".post_drop");
-  sv.h = c.act((int64_t)M * d); sv.mean = c.f32(M); sv.rstd = c.f32(M);
-  sv.qkv = c.act((int64_t)M * d);
-  sv.kv = c.act((int64_t)Mk * 2 * d);
-  const DropoutSpec adrop = c.drop(cf.attention_dropout, sv.s_attn, (int64_t)B * cf.heads * L * Tkp);
-  if (use_fused_attention(c, sv.dims)) {
-    sv.lse = c.f32((int64_t)B * cf.heads * L);
-  } else {
-    sv.p_pre = c.act((int64_t)B * cf.heads * L * Tkp);
-    sv.p_drop = adrop.p > 0.f ? c.act((int64_t)B * cf.heads * L * Tkp) : nullptr;
-  }
-  sv.ctx = c.act((int64_t)M * d);
-  RUN(layernorm_fwd(x_in, F32, c.P(pre + ".ln.gamma"), c.P(pre + ".ln.beta"), cf.ln_eps, sv.h, c.adt, nullptr, sv.mean, sv.rstd,
-                    M, d, 0, c.st));
-  GemmEpilogue e0 = gemm_defaults().epi;
-  B200ST_TRY(linear_fwd(c, sv.h, d, M, d, d, pre + ".q.kernel", pre + ".q.bias", e0, sv.qkv, c.adt, d));
-  B200ST_TRY(linear_fwd(c, mem, d, Mk, d, 2 * d, pre + ".kv.kernel", pre + ".kv.bias", e0, sv.kv, c.adt, 2 * d));
-  View q{sv.qkv, d}, k{sv.kv, 2 * d}, v{c.act_off(sv.kv, d), 2 * d};
-  B200ST_TRY(attention_fwd(c, sv.dims, q, k, v, mem_bias, sv.mask, adrop, sc.S, sv.p_pre, sv.p_drop, sv.ctx, sv.lse));
-  GemmEpilogue e1 = gemm_defaults().epi;
-  e1.drop = c.drop(cf.postprocess_dropout, sv.s_post, (int64_t)M * d);
-  e1.residual = x_in; e1.res_ld = d;
-  B200ST_TRY(linear_fwd(c, sv.ctx, d, M, d, d, pre + ".out.kernel", pre + ".out.bias", e1, x_out, F32, d));
-  return 0;
-}
-
-static int cross_attn_block_bwd(Ctx& c, const std::string& pre, const float* dx_out, float* dx_in, float* dmem, Scratch& sc,
-                                const AttnSave& sv) {
-  sc.select(c.begin_bwd_block());
-  WgradBlock wb(c);
-  const Config& cf = c.m.cfg;
-  const int d = cf.d, M = sv.dims.B * sv.dims.Tq, Mk = sv.dims.B * sv.dims.Tk;
-  if (c.dy_ready) c.dy_ready = false;      // produced by the previous block's LayerNorm-backward
-  else RUN(cast_dropout(dx_out, sc.dY, c.adt, (int64_t)M * d, c.drop(cf.postprocess_dropout, sv.s_post), c.st));
-  B200ST_TRY(linear_wgrad(c, sv.ctx, d, sc.dY, d, M, d, d, pre + ".out.kernel", pre + ".out.bias"));
-  GemmEpilogue e0 = gemm_defaults().epi;
-  B200ST_TRY(linear_dgrad(c, sc.dY, d, M, d, d, pre + ".out.kernel", e0, sc.dctx, c.adt, d));
-  View q{sv.qkv, d}, k{sv.kv, 2 * d}, v{c.act_off(sv.kv, d), 2 * d};
-  View dq{sc.dqkv, d}, dk{sc.dkv, 2 * d}, dv{c.act_off(sc.dkv, d), 2 * d};
-  B200ST_TRY(attention_bwd(c, sv.dims, q, k, v, sv.p_pre, sv.p_drop, c.drop(cf.attention_dropout, sv.s_attn), sc.dctx, sc.S, sc.dS,
-                           dq, dk, dv, sv.ctx, sv.lse, sv.bias, sv.mask, sc.dq32));
-  B200ST_TRY(linear_wgrad(c, sv.h, d, sc.dqkv, d, M, d, d, pre + ".q.kernel", pre + ".q.bias"));
-  B200ST_TRY(linear_wgrad(c, sv.mem, d, sc.dkv, 2 * d, Mk, d, 2 * d, pre + ".kv.kernel", pre + ".kv.bias"));
-  B200ST_TRY(wb.flush());
-  B200ST_TRY(linear_dgrad(c, sc.dqkv, d, M, d, d, pre + ".q.kernel", e0, sc.dh, F32, d));
-  B200ST_TRY(block_ln_bwd(c, sc, sc.dh, sv.x_in, sv.mean, sv.rstd, pre, dx_out, dx_in, M, d));
+  const QkvViews a = qkv_views(c, sv.qkv, sv.kv, d), da = qkv_views(c, sc.dqkv, sv.mem ? sc.dkv : nullptr, d);
+  B200ST_TRY(attention_bwd(c, sv.dims, a.q, a.k, a.v, sv.p_pre, sv.p_drop, c.drop(cf.attention_dropout, sv.s_attn), sc.dctx, sc.S,
+                           sc.dS, da.q, da.k, da.v, sv.ctx, sv.lse, sv.bias, sv.mask, sc.dq32));
+  B200ST_TRY(linear_wgrad(c, sv.h, d, sc.dqkv, nq, M, d, nq, q + ".kernel", q + ".bias"));
+  if (sv.mem) B200ST_TRY(linear_wgrad(c, sv.mem, d, sc.dkv, 2 * d, Mk, d, 2 * d, pre + ".kv.kernel", pre + ".kv.bias"));
+  B200ST_TRY(bb.flush());      // every dY of the block exists: the side stream starts under the rest of the chain
+  B200ST_TRY(linear_dgrad(c, sc.dqkv, nq, M, nq, d, q + ".kernel", e0, sc.dh, F32, d));
+  B200ST_TRY(bb.finish());
+  if (!sv.mem) return 0;
   GemmEpilogue ea = gemm_defaults().epi;
   ea.accumulate = 1;                              // memory gradient accumulates over decoder layers
-  B200ST_TRY(linear_dgrad(c, sc.dkv, 2 * d, Mk, 2 * d, d, pre + ".kv.kernel", ea, dmem, F32, d));
-  return wb.flush();
+  return linear_dgrad(c, sc.dkv, 2 * d, Mk, 2 * d, d, pre + ".kv.kernel", ea, dmem, F32, d);
 }
 
 // FFN block path, one choice for its forward and its backward: the fused kernel where it supports the shape and dtype, else
@@ -664,16 +633,14 @@ static bool use_fused_ffn(const Ctx& c, int M) {
 static int ffn_block_fwd(Ctx& c, const std::string& pre, const float* x_in, float* x_out, int M, FfnSave& sv) {
   const Config& cf = c.m.cfg;
   const int d = cf.d, f = cf.ffn;
-  sv.x_in = x_in; sv.M = M;
-  sv.s_ffn = dropout_stream_id(pre + ".ffn_drop"); sv.s_post = dropout_stream_id(pre + ".post_drop");
-  sv.h = c.act((int64_t)M * d); sv.mean = c.f32(M); sv.rstd = c.f32(M);
+  sv.s_ffn = dropout_stream_id(pre + ".ffn_drop");
+  prenorm_alloc(c, pre, x_in, M, sv);
   sv.f1 = c.act((int64_t)M * f);
   if (use_fused_ffn(c, M)) {
     // one kernel for FFN1 -> ReLU -> dropout -> FFN2 -> dropout -> +residual (SURVEY K11): the LayerNorm kernel also seeds
     // x_out with the residual, the fused kernel reduce-adds the rest
     B200ST_TRY(need_param(c, pre + ".w1")); B200ST_TRY(need_param(c, pre + ".w2"));
-    RUN(layernorm_fwd_copy(x_in, F32, c.P(pre + ".ln.gamma"), c.P(pre + ".ln.beta"), cf.ln_eps, sv.h, c.adt, nullptr, sv.mean, sv.rstd,
-                           M, d, 0, x_out, c.st));
+    B200ST_TRY(prenorm_fwd(c, pre, sv, x_out));
     const DropoutSpec d1 = c.drop(cf.ffn_dropout, sv.s_ffn, (int64_t)M * f);
     const DropoutSpec d2 = c.drop(cf.postprocess_dropout, sv.s_post, (int64_t)M * d);
     int* tk = c.mlp_tickets(M);
@@ -681,8 +648,7 @@ static int ffn_block_fwd(Ctx& c, const std::string& pre, const float* x_in, floa
                       d1, d2, sv.f1, x_out, c.st, tk));
     return 0;
   }
-  RUN(layernorm_fwd(x_in, F32, c.P(pre + ".ln.gamma"), c.P(pre + ".ln.beta"), cf.ln_eps, sv.h, c.adt, nullptr, sv.mean, sv.rstd,
-                    M, d, 0, c.st));
+  B200ST_TRY(prenorm_fwd(c, pre, sv, nullptr));
   GemmEpilogue e1 = gemm_defaults().epi;
   e1.relu = 1;
   e1.drop = c.drop(cf.ffn_dropout, sv.s_ffn, (int64_t)M * f);
@@ -690,48 +656,51 @@ static int ffn_block_fwd(Ctx& c, const std::string& pre, const float* x_in, floa
   GemmEpilogue e2 = gemm_defaults().epi;
   e2.drop = c.drop(cf.postprocess_dropout, sv.s_post, (int64_t)M * d);
   e2.residual = x_in; e2.res_ld = d;
-  B200ST_TRY(linear_fwd(c, sv.f1, f, M, f, d, pre + ".w2", pre + ".b2", e2, x_out, F32, d));
-  return 0;
+  return linear_fwd(c, sv.f1, f, M, f, d, pre + ".w2", pre + ".b2", e2, x_out, F32, d);
 }
 
 static int ffn_block_bwd(Ctx& c, const std::string& pre, const float* dx_out, float* dx_in, Scratch& sc, const FfnSave& sv) {
-  sc.select(c.begin_bwd_block());
-  WgradBlock wb(c);
+  BwdBlock bb(c, sc, pre, sv, dx_out, dx_in);
+  B200ST_TRY(bb.rc);
   const Config& cf = c.m.cfg;
   const int d = cf.d, f = cf.ffn, M = sv.M;
-  if (c.dy_ready) c.dy_ready = false;      // produced by the previous block's LayerNorm-backward
-  else RUN(cast_dropout(dx_out, sc.dY, c.adt, (int64_t)M * d, c.drop(cf.postprocess_dropout, sv.s_post), c.st));
+  const DropoutSpec fd = c.drop(cf.ffn_dropout, sv.s_ffn);
   B200ST_TRY(linear_wgrad(c, sv.f1, f, sc.dY, d, M, f, d, pre + ".w2", pre + ".b2"));
   if (use_fused_ffn(c, M)) {
     // data-gradient chain in one kernel: dF1 = (dY W2^T) * relu'/dropout' (written for the W1 weight gradient), dh = dF1 W1^T
-    const DropoutSpec fd = c.drop(cf.ffn_dropout, sv.s_ffn);
     RUN(cudaMemsetAsync(sc.dh, 0, sizeof(float) * (size_t)M * d, c.st) == cudaSuccess ? 0 : 1);
     int* tk = c.mlp_tickets(M);
     RUN(fused_mlp_bwd(sc.dY, c.adt, M, d, f, c.W(pre + ".w1", 0, f).ptr, c.W(pre + ".w2", 0, d).ptr, sv.f1,
                       fd.p > 0.f ? fd.scale : 1.f, sc.dF1, sc.dh, c.st, tk));
     B200ST_TRY(linear_wgrad(c, sv.h, d, sc.dF1, f, M, d, f, pre + ".w1", pre + ".b1"));
-    B200ST_TRY(wb.flush());
-    B200ST_TRY(block_ln_bwd(c, sc, sc.dh, sv.x_in, sv.mean, sv.rstd, pre, dx_out, dx_in, M, d));
-    return wb.flush();
+    B200ST_TRY(bb.flush());
+    return bb.finish();
   }
   GemmEpilogue e1 = gemm_defaults().epi;
   e1.mask_src = sv.f1; e1.mask_dtype = c.adt; e1.mask_ld = f;      // relu' and ffn-dropout mask: stored f1 > 0
-  const DropoutSpec fd = c.drop(cf.ffn_dropout, sv.s_ffn);
   e1.alpha = fd.p > 0.f ? fd.scale : 1.f;
   B200ST_TRY(linear_dgrad(c, sc.dY, d, M, d, f, pre + ".w2", e1, sc.dF1, c.adt, f));
   B200ST_TRY(linear_wgrad(c, sv.h, d, sc.dF1, f, M, d, f, pre + ".w1", pre + ".b1"));
   GemmEpilogue e0 = gemm_defaults().epi;
   B200ST_TRY(linear_dgrad(c, sc.dF1, f, M, f, d, pre + ".w1", e0, sc.dh, F32, d));
-  B200ST_TRY(block_ln_bwd(c, sc, sc.dh, sv.x_in, sv.mean, sv.rstd, pre, dx_out, dx_in, M, d));
-  return wb.flush();
+  return bb.finish();
 }
 
 // ---- stacks ----------------------------------------------------------------------------------------
-struct EncoderSave {
-  std::vector<AttnSave> att; std::vector<FfnSave> ffn;
+// A stack's blocks in forward order (encoder: self -> ffn per layer; decoder: self -> [cross] -> ffn) and its final LayerNorm
+struct StackSave {
+  struct Block {
+    std::string pre;        // parameter prefix, e.g. "dec.3.cross"
+    bool ffn;               // FFN block (f), else attention (att)
+    AttnSave att; FfnSave f;
+    const PrenormSave& save() const { return ffn ? static_cast<const PrenormSave&>(f) : att; }
+  };
+  std::vector<Block> blocks;
+  std::string name;          // "enc" / "dec"
   const float* x_last = nullptr; float* mean = nullptr; float* rstd = nullptr;
   void* out = nullptr;       // act dtype [M,d]
-  int B = 0, T = 0;
+  int M = 0;
+  Block& add(const std::string& pre, bool ffn) { blocks.push_back(Block{pre, ffn, {}, {}}); return blocks.back(); }
 };
 
 static void alloc_scratch(Ctx& c, Scratch& sc, int B, int Tq_max, int Tk_max, int Mq_max, int Mk_max, bool backward) {
@@ -753,114 +722,84 @@ static void alloc_scratch(Ctx& c, Scratch& sc, int B, int Tq_max, int Tk_max, in
   }
 }
 
+// the stack's final LayerNorm: out (act dtype) and out32 (optional fp32 copy) = LN(x)
+static int stack_out_fwd(Ctx& c, const char* name, const float* x, int M, StackSave& sv, float* out32) {
+  const Config& cf = c.m.cfg;
+  const std::string ln = std::string(name) + ".out_ln";
+  sv.name = name; sv.M = M; sv.x_last = x;
+  sv.mean = c.f32(M); sv.rstd = c.f32(M);
+  sv.out = c.act((int64_t)M * cf.d);
+  RUN(layernorm_fwd(x, F32, c.P(ln + ".gamma"), c.P(ln + ".beta"), cf.ln_eps, sv.out, c.adt, out32, sv.mean, sv.rstd, M, cf.d, 0, c.st));
+  return 0;
+}
+
 // x0: embedded input fp32 [B*T,d] (dropout already applied); bias [B,T]; out: act-dtype (+ optional fp32 copy)
-static int encoder_fwd(Ctx& c, const float* x0, const float* bias, int B, int T, Scratch& sc, EncoderSave& sv, float* out32) {
+static int encoder_fwd(Ctx& c, const float* x0, const float* bias, int B, int T, Scratch& sc, StackSave& sv, float* out32) {
   const Config& cf = c.m.cfg;
   const int M = B * T, d = cf.d;
-  sv.B = B; sv.T = T;
-  sv.att.resize(cf.enc_layers); sv.ffn.resize(cf.enc_layers);
   const float* x = x0;
   // monotonic encoder (transformer_encoder.py:119-123): query i sees the non-padded keys j <= i
   const KeyMask mask = cf.encoder_monotonic ? causal_mask(T, T) : no_key_mask();
   for (int i = 0; i < cf.enc_layers; ++i) {
     const std::string p = "enc." + std::to_string(i);
     float* x1 = c.f32((int64_t)M * d);
-    B200ST_TRY(self_attn_block_fwd(c, p + ".att", x, x1, B, T, bias, mask, sc, sv.att[i]));
+    StackSave::Block& a = sv.add(p + ".att", false);
+    B200ST_TRY(attn_block_fwd(c, a.pre, x, x1, B, T, nullptr, T, bias, mask, sc, a.att));
     float* x2 = c.f32((int64_t)M * d);
-    B200ST_TRY(ffn_block_fwd(c, p + ".ffn", x1, x2, M, sv.ffn[i]));
+    StackSave::Block& f = sv.add(p + ".ffn", true);
+    B200ST_TRY(ffn_block_fwd(c, f.pre, x1, x2, M, f.f));
     x = x2;
   }
-  sv.x_last = x;
-  sv.mean = c.f32(M); sv.rstd = c.f32(M);
-  sv.out = c.act((int64_t)M * d);
-  RUN(layernorm_fwd(x, F32, c.P("enc.out_ln.gamma"), c.P("enc.out_ln.beta"), cf.ln_eps, sv.out, c.adt, out32, sv.mean, sv.rstd, M, d, 0,
-                    c.st));
-  return 0;
+  return stack_out_fwd(c, "enc", x, M, sv, out32);
 }
-
-// d_out: fp32 [M,d] gradient wrt encoder output; returns gradient wrt x0 in dx (fp32 [M,d])
-static int encoder_bwd(Ctx& c, const float* d_out, float* dx, float* dx_tmp, Scratch& sc, const EncoderSave& sv, bool buckets = false) {
-  const Config& cf = c.m.cfg;
-  const int M = sv.B * sv.T, d = cf.d;
-  RUN(layernorm_bwd(d_out, F32, sv.x_last, F32, sv.mean, sv.rstd, c.P("enc.out_ln.gamma"), c.P("enc.out_ln.beta"), nullptr, dx, F32,
-                    c.G("enc.out_ln.gamma"), c.G("enc.out_ln.beta"), M, d, 0, c.st));
-  for (int i = cf.enc_layers - 1; i >= 0; --i) {
-    const std::string p = "enc." + std::to_string(i);
-    // each block's LayerNorm-backward also emits the next block's dY = cast(dropout'(dx)) (same M for the whole stack)
-    const DropoutSpec nd_att = c.drop(cf.postprocess_dropout, sv.att[i].s_post);
-    c.next_drop = &nd_att;
-    B200ST_TRY(ffn_block_bwd(c, p + ".ffn", dx, dx_tmp, sc, sv.ffn[i]));
-    DropoutSpec nd_ffn = no_dropout();
-    if (i > 0) { nd_ffn = c.drop(cf.postprocess_dropout, sv.ffn[i - 1].s_post); c.next_drop = &nd_ffn; }
-    B200ST_TRY(self_attn_block_bwd(c, p + ".att", dx_tmp, dx, sc, sv.att[i]));
-    // gradient bucket: the upper half of the encoder stack (+ its final LayerNorm) is final after layer enc_layers / 2
-    if (buckets && i == cf.enc_layers / 2 && i > 0) B200ST_TRY(c.reduce_down_to(p + ".att.ln.gamma"));
-  }
-  return 0;
-}
-
-struct DecoderSave {
-  std::vector<AttnSave> self, cross; std::vector<FfnSave> ffn;
-  const float* x_last = nullptr; float* mean = nullptr; float* rstd = nullptr;
-  void* out = nullptr;
-  int B = 0, L = 0, Tm = 0;
-};
 
 static int decoder_fwd(Ctx& c, const float* x0, int B, int L, const void* mem, int Tm, const float* mem_bias, Scratch& sc,
-                       DecoderSave& sv, float* out32) {
+                       StackSave& sv, float* out32) {
   const Config& cf = c.m.cfg;
   const int M = B * L, d = cf.d;
-  sv.B = B; sv.L = L; sv.Tm = Tm;
-  sv.self.resize(cf.dec_layers); sv.cross.resize(cf.dec_layers); sv.ffn.resize(cf.dec_layers);
   const float* x = x0;
   for (int i = 0; i < cf.dec_layers; ++i) {
     const std::string p = "dec." + std::to_string(i);
     float* x1 = c.f32((int64_t)M * d);
-    B200ST_TRY(self_attn_block_fwd(c, p + ".self", x, x1, B, L, nullptr, causal_mask(L, L), sc, sv.self[i]));
+    StackSave::Block& s = sv.add(p + ".self", false);
+    B200ST_TRY(attn_block_fwd(c, s.pre, x, x1, B, L, nullptr, L, nullptr, causal_mask(L, L), sc, s.att));
     x = x1;
     if (cf.with_cross_attention && mem) {
       float* x2 = c.f32((int64_t)M * d);
-      B200ST_TRY(cross_attn_block_fwd(c, p + ".cross", x, x2, B, L, mem, Tm, mem_bias, sc, sv.cross[i]));
+      StackSave::Block& a = sv.add(p + ".cross", false);
+      B200ST_TRY(attn_block_fwd(c, a.pre, x, x2, B, L, mem, Tm, mem_bias, c.cross_mask, sc, a.att));
       x = x2;
     }
     float* x3 = c.f32((int64_t)M * d);
-    B200ST_TRY(ffn_block_fwd(c, p + ".ffn", x, x3, M, sv.ffn[i]));
+    StackSave::Block& f = sv.add(p + ".ffn", true);
+    B200ST_TRY(ffn_block_fwd(c, f.pre, x, x3, M, f.f));
     x = x3;
   }
-  sv.x_last = x;
-  sv.mean = c.f32(M); sv.rstd = c.f32(M);
-  sv.out = c.act((int64_t)M * d);
-  RUN(layernorm_fwd(x, F32, c.P("dec.out_ln.gamma"), c.P("dec.out_ln.beta"), cf.ln_eps, sv.out, c.adt, out32, sv.mean, sv.rstd, M, d, 0,
-                    c.st));
-  return 0;
+  return stack_out_fwd(c, "dec", x, M, sv, out32);
 }
 
-static int decoder_bwd(Ctx& c, const float* d_out, float* dx, float* dx_tmp, float* dmem, bool has_mem, Scratch& sc,
-                       const DecoderSave& sv) {
+// d_out: fp32 [M,d] gradient wrt the stack output; returns the gradient wrt its input in dx (fp32 [M,d]).  dmem accumulates
+// the cross-attention blocks' memory gradient.  After block `bucket` (-1: none) the gradients of every block above it and of
+// the final LayerNorm are final: they are all-reduced under the rest of the backward pass.
+static int stack_bwd(Ctx& c, const float* d_out, float* dx, float* dx_tmp, float* dmem, Scratch& sc, const StackSave& sv,
+                     int bucket) {
   const Config& cf = c.m.cfg;
-  const int M = sv.B * sv.L, d = cf.d;
-  RUN(layernorm_bwd(d_out, F32, sv.x_last, F32, sv.mean, sv.rstd, c.P("dec.out_ln.gamma"), c.P("dec.out_ln.beta"), nullptr, dx, F32,
-                    c.G("dec.out_ln.gamma"), c.G("dec.out_ln.beta"), M, d, 0, c.st));
+  const std::string ln = sv.name + ".out_ln";
+  RUN(layernorm_bwd(d_out, F32, sv.x_last, F32, sv.mean, sv.rstd, c.P(ln + ".gamma"), c.P(ln + ".beta"), nullptr, dx, F32,
+                    c.G(ln + ".gamma"), c.G(ln + ".beta"), sv.M, cf.d, 0, c.st));
   float* a = dx; float* b = dx_tmp;
-  for (int i = cf.dec_layers - 1; i >= 0; --i) {
-    const std::string p = "dec." + std::to_string(i);
-    const bool cross = cf.with_cross_attention && has_mem;
-    const DropoutSpec nd1 = c.drop(cf.postprocess_dropout, cross ? sv.cross[i].s_post : sv.self[i].s_post);
-    c.next_drop = &nd1;
-    B200ST_TRY(ffn_block_bwd(c, p + ".ffn", a, b, sc, sv.ffn[i]));
-    std::swap(a, b);
-    if (cross) {
-      const DropoutSpec nd2 = c.drop(cf.postprocess_dropout, sv.self[i].s_post);
-      c.next_drop = &nd2;
-      B200ST_TRY(cross_attn_block_bwd(c, p + ".cross", a, b, dmem, sc, sv.cross[i]));
-      std::swap(a, b);
+  for (int k = (int)sv.blocks.size() - 1; k >= 0; --k) {
+    const StackSave::Block& blk = sv.blocks[k];
+    // the block's LayerNorm-backward also emits the dY of the block that ran before it in the forward pass
+    if (k > 0) {
+      c.next_drop = c.drop(cf.postprocess_dropout, sv.blocks[k - 1].save().s_post);
+      c.has_next_drop = true;
     }
-    DropoutSpec nd3 = no_dropout();
-    if (i > 0) { nd3 = c.drop(cf.postprocess_dropout, sv.ffn[i - 1].s_post); c.next_drop = &nd3; }
-    B200ST_TRY(self_attn_block_bwd(c, p + ".self", a, b, sc, sv.self[i]));
+    B200ST_TRY(blk.ffn ? ffn_block_bwd(c, blk.pre, a, b, sc, blk.f) : attn_block_bwd(c, blk.pre, a, b, dmem, sc, blk.att));
     std::swap(a, b);
+    if (k == bucket) B200ST_TRY(c.reduce_down_to(blk.pre + ".ln.gamma"));
   }
-  if (a != dx) RUN(cudaMemcpyAsync(dx, a, sizeof(float) * (size_t)M * d, cudaMemcpyDeviceToDevice, c.st) == cudaSuccess ? 0 : 1);
+  if (a != dx) RUN(cudaMemcpyAsync(dx, a, sizeof(float) * (size_t)sv.M * cf.d, cudaMemcpyDeviceToDevice, c.st) == cudaSuccess ? 0 : 1);
   return 0;
 }
 
@@ -1010,7 +949,7 @@ static int model_run(Ctx& c, const Batch& b, bool backward) {
     RUN(embed_fwd(b.src_ids, c.P(tab), x0, B, Ts, d, cf.share_src_trg_embedding ? V : cf.src_vocab, 0,
                   c.drop(cf.postprocess_dropout, dropout_stream_id("enc.in_drop")), c.st));
   }
-  EncoderSave es;
+  StackSave es;
   B200ST_TRY(encoder_fwd(c, x0, enc_bias, B, Ts, sc, es, b.enc_out));
   if (b.stop_after_encoder) {
     if (b.enc_bias_out)
@@ -1021,7 +960,7 @@ static int model_run(Ctx& c, const Batch& b, bool backward) {
   // ---- decoder side ----
   float* y0 = c.f32((int64_t)Md * d);
   RUN(embed_fwd(b.trg_input, c.P("trg.emb"), y0, B, L, d, V, 0, c.drop(cf.postprocess_dropout, dropout_stream_id("dec.in_drop")), c.st));
-  DecoderSave ds;
+  StackSave ds;
   B200ST_TRY(decoder_fwd(c, y0, B, L, es.out, Ts, enc_bias, sc, ds, nullptr));
 
   // ---- logits + loss ----
@@ -1095,12 +1034,15 @@ static int model_run(Ctx& c, const Batch& b, bool backward) {
   float* dy_tmp = c.f32((int64_t)Md * d);
   float* d_enc = c.f32((int64_t)Ms * d);
   RUN(fill_f32(d_enc, 0.f, (int64_t)Ms * d, c.st));
-  B200ST_TRY(decoder_bwd(c, d_dec, dy, dy_tmp, d_enc, true, sc, ds));
+  B200ST_TRY(stack_bwd(c, d_dec, dy, dy_tmp, d_enc, sc, ds, -1));
   RUN(embed_bwd(b.trg_input, dy, c.G("trg.emb"), B, L, d, V, c.drop(cf.postprocess_dropout, dropout_stream_id("dec.in_drop")), c.st));
   if (buckets) B200ST_TRY(c.reduce_down_to("dec.0.self.ln.gamma"));     // decoder + output layer: ~40 MB under the encoder backward
   float* dx = c.f32((int64_t)Ms * d);
   float* dx_tmp = c.f32((int64_t)Ms * d);
-  B200ST_TRY(encoder_bwd(c, d_enc, dx, dx_tmp, sc, es, buckets));
+  // gradient bucket: the upper half of the encoder stack (+ its final LayerNorm) is final after the attention block of layer
+  // enc_layers / 2
+  const int half = cf.enc_layers / 2;
+  B200ST_TRY(stack_bwd(c, d_enc, dx, dx_tmp, nullptr, sc, es, buckets && half > 0 ? 2 * half : -1));
   if (buckets) B200ST_TRY(c.reduce_down_to("enc.0.att.ln.gamma"));
   if (speech) {
     B200ST_TRY(speech_front_bwd(c, b.src, dx, fs));
@@ -1205,7 +1147,7 @@ int encoder_api_body(Ctx& c, const float* x, const float* padding, int B, int T,
   float* x0 = c.f32((int64_t)B * T * cf.d);
   // encoder input dropout (transformer_encoder.py:125-127)
   RUN(cast_dropout(x, x0, F32, (int64_t)B * T * cf.d, c.drop(cf.postprocess_dropout, dropout_stream_id("enc.in_drop")), c.st));
-  EncoderSave es;
+  StackSave es;
   return encoder_fwd(c, x0, bias, B, T, sc, es, out);
 }
 
@@ -1226,7 +1168,7 @@ int decoder_api_body(Ctx& c, const float* x, const float* memory, const float* m
     mbias = c.f32((int64_t)B * Tm);
     RUN(padding_to_bias(memory_padding, mbias, (int64_t)B * Tm, c.st));
   }
-  DecoderSave ds;
+  StackSave ds;
   return decoder_fwd(c, x0, B, L, mem, Tm, mbias, sc, ds, out);
 }
 
@@ -1242,21 +1184,20 @@ int mha_api_body(Ctx& c, const float* query, const float* memory, const float* b
   float* lse = c.f32((int64_t)B * cf.heads * Tq);
   GemmEpilogue e0 = gemm_defaults().epi;
   AttnDims dims{B, cf.heads, Tq, Tk, u};
+  void* qkv; void* kv = nullptr;
   if (cf.mha_self) {
-    void* qkv = c.act(Mq * 3 * u);
+    qkv = c.act(Mq * 3 * u);
     B200ST_TRY(linear_fwd(c, qin, cf.mha_din, (int)Mq, cf.mha_din, 3 * u, "att.qkv.kernel", "att.qkv.bias", e0, qkv, c.adt, 3 * u));
-    View q{qkv, 3 * u}, k{c.act_off(qkv, u), 3 * u}, v{c.act_off(qkv, 2 * u), 3 * u};
-    B200ST_TRY(attention_fwd(c, dims, q, k, v, bias, no_key_mask(), no_dropout(), S, p_pre, nullptr, ctx, lse));
   } else {
     void* min = c.act(Mk * cf.mha_dmem);
     RUN(cast_dropout(memory, min, c.adt, Mk * cf.mha_dmem, no_dropout(), c.st));
-    void* qb = c.act(Mq * u);
-    void* kv = c.act(Mk * 2 * u);
-    B200ST_TRY(linear_fwd(c, qin, cf.mha_din, (int)Mq, cf.mha_din, u, "att.q.kernel", "att.q.bias", e0, qb, c.adt, u));
+    qkv = c.act(Mq * u);
+    kv = c.act(Mk * 2 * u);
+    B200ST_TRY(linear_fwd(c, qin, cf.mha_din, (int)Mq, cf.mha_din, u, "att.q.kernel", "att.q.bias", e0, qkv, c.adt, u));
     B200ST_TRY(linear_fwd(c, min, cf.mha_dmem, (int)Mk, cf.mha_dmem, 2 * u, "att.kv.kernel", "att.kv.bias", e0, kv, c.adt, 2 * u));
-    View q{qb, u}, k{kv, 2 * u}, v{c.act_off(kv, u), 2 * u};
-    B200ST_TRY(attention_fwd(c, dims, q, k, v, bias, no_key_mask(), no_dropout(), S, p_pre, nullptr, ctx, lse));
   }
+  const QkvViews a = qkv_views(c, qkv, kv, u);
+  B200ST_TRY(attention_fwd(c, dims, a.q, a.k, a.v, bias, no_key_mask(), no_dropout(), S, p_pre, nullptr, ctx, lse));
   return linear_fwd(c, ctx, u, (int)Mq, u, cf.mha_dout, "att.out.kernel", "att.out.bias", e0, out, F32, cf.mha_dout);
 }
 

@@ -90,6 +90,20 @@ def test_transformer_decoder():
     assert _sq(sa["values"].reshape(2, 1, 4), k["expect:3"]) < 1e-9
 
 
+def test_transformer_decoder_without_cross_attention():
+    """with_encoder_decoder_attention=False: every layer is self-attention -> FFN, against the fp64 decoder without memory."""
+    torch.manual_seed(0)
+    cfg = dict(model="none", d=16, heads=4, enc_layers=0, dec_layers=2, ffn=24, vocab=1)
+    P = R.init_params(cfg, seed=9, random_bias=True)
+    decoder = TransformerDecoder(num_layers=2, num_attention_heads=4, hidden_size=16, filter_size=24,
+                                 with_encoder_decoder_attention=False)
+    decoder.load_parameters(P)
+    x = torch.randn(3, 7, 16)
+    out = decoder(x, decoder.create_decoding_internal_cache(None, None), is_training=False).cpu().double()
+    expect = R.decoder({k: v.double() for k, v in P.items()}, x.double(), None, None, 2, 4)
+    assert float((out - expect).abs().max()) < 1e-5
+
+
 def test_incremental_decode_matches_full_decode():
     """cached steps reproduce the full (training-mode) decoder outputs position by position."""
     torch.manual_seed(0)
