@@ -6,9 +6,14 @@
 // NORMALISED activation xhat + 1/sigma ("normalised-save"): gamma/beta/ReLU are applied by the im2col in flight and the
 // backward reads xhat back, so it needs neither the convolution recompute nor the statistics.  Other shapes use the
 // generic kernels (filter in shared memory, post-ReLU activation stored, z1 recomputed in the backward).
-// conv2 is lowered to wgmma GEMMs through im2col (forward / wgrad) and a dcol GEMM (dgrad); the dgrad's col2im
-// gather is fused with the ReLU mask, the LayerNorm backward of conv1 and the parameter-gradient partial sums.
-// conv1's filter gradient is one more split-K GEMM over the tiny im2col of the fbank (written by the same kernel).
+// conv2, 16-bit normalised-save front-end with F2 <= 128 (the training path): conv1's forward also writes the post-activation
+// split by parity class, and conv2's forward, filter gradient and data gradient are implicit wgmma GEMMs over those planes
+// (tc_gemm.cu) — no column matrix.  conv1's backward reads the data gradient's class-major tiles, applies the ReLU mask and
+// the LayerNorm backward and accumulates every parameter gradient of conv1, its filter gradient included.
+// Otherwise (fp32, other shapes, F2 > 128): conv2 is lowered to wgmma GEMMs through im2col (forward / wgrad) and a dcol GEMM
+// (dgrad); the dgrad's col2im gather is fused with the ReLU mask, the LayerNorm backward of conv1 and the parameter-gradient
+// partial sums, and conv1's filter gradient is one more split-K GEMM over the tiny im2col of the fbank (written by the same
+// kernel).
 #include "kernels.cuh"
 #include "pdl.cuh"
 
@@ -214,17 +219,70 @@ __global__ void __launch_bounds__(256, (CPL <= 8 ? 3 : 1)) conv1_fwd_kernel(cons
   }
 }
 
+// y = relu(x * gamma + beta) on one 16-byte vector (affine parameters in the activation dtype: for bf16 they come from
+// the bf16 shadow arena and the math is packed HFMA2.BF16 / HMNMX2 — the same rounding the backward's ReLU mask assumes)
+__device__ __forceinline__ uint4 affine_relu_vec(uint4 v, const __nv_bfloat162 (&g)[4], const __nv_bfloat162 (&b)[4]) {
+  __nv_bfloat162* h = reinterpret_cast<__nv_bfloat162*>(&v);
+  const __nv_bfloat162 zero = __floats2bfloat162_rn(0.f, 0.f);
+#pragma unroll
+  for (int j = 0; j < 4; ++j) h[j] = __hmax2(__hfma2(h[j], g[j], b[j]), zero);
+  return v;
+}
+__device__ __forceinline__ uint4 affine_relu_vec(uint4 v, const __half2 (&g)[4], const __half2 (&b)[4]) {
+  __half2* h = reinterpret_cast<__half2*>(&v);
+  const __half2 zero = __floats2half2_rn(0.f, 0.f);
+#pragma unroll
+  for (int j = 0; j < 4; ++j) h[j] = __hmax2(__hfma2(h[j], g[j], b[j]), zero);
+  return v;
+}
+__device__ __forceinline__ uint4 affine_relu_vec(uint4 v, const float (&g)[4], const float (&b)[4]) {
+  float* f = reinterpret_cast<float*>(&v);
+#pragma unroll
+  for (int j = 0; j < 4; ++j) f[j] = fmaxf(fmaf(f[j], g[j], b[j]), 0.f);
+  return v;
+}
+template <typename T> struct AffineRegs;
+template <> struct AffineRegs<__nv_bfloat16> {
+  __nv_bfloat162 g[4], b[4];
+  __device__ __forceinline__ void load(const __nv_bfloat16* gamma, const __nv_bfloat16* beta, int c) {
+    const uint4 gv = __ldg(reinterpret_cast<const uint4*>(gamma + c)), bv = __ldg(reinterpret_cast<const uint4*>(beta + c));
+#pragma unroll
+    for (int j = 0; j < 4; ++j) { g[j] = reinterpret_cast<const __nv_bfloat162*>(&gv)[j]; b[j] = reinterpret_cast<const __nv_bfloat162*>(&bv)[j]; }
+  }
+};
+template <> struct AffineRegs<__half> {
+  __half2 g[4], b[4];
+  __device__ __forceinline__ void load(const __half* gamma, const __half* beta, int c) {
+    const uint4 gv = __ldg(reinterpret_cast<const uint4*>(gamma + c)), bv = __ldg(reinterpret_cast<const uint4*>(beta + c));
+#pragma unroll
+    for (int j = 0; j < 4; ++j) { g[j] = reinterpret_cast<const __half2*>(&gv)[j]; b[j] = reinterpret_cast<const __half2*>(&bv)[j]; }
+  }
+};
+template <> struct AffineRegs<float> {
+  float g[4], b[4];
+  __device__ __forceinline__ void load(const float* gamma, const float* beta, int c) {
+    const float4 gv = __ldg(reinterpret_cast<const float4*>(gamma + c)), bv = __ldg(reinterpret_cast<const float4*>(beta + c));
+    g[0] = gv.x; g[1] = gv.y; g[2] = gv.z; g[3] = gv.w; b[0] = bv.x; b[1] = bv.y; b[2] = bv.z; b[3] = bv.w;
+  }
+};
+
 // ---------------------------------------------------------------------------------------------
 // conv1 forward, production shape (C == 256, Cin == 1): the lane's 9 x 8 filter taps live in registers (no shared-memory
 // traffic: the generic kernel is LDS-bound), the 9 fbank taps of a position are fetched by lanes 0..8 one position
 // ahead and broadcast with shuffles, each warp walks a contiguous range of positions.
 // SAVE: store xhat + 1/sigma (normalised-save mode); else y = relu(LN(z) * gamma + beta).
+// SAVE with a1 != null (16-bit): also the post-activation a1 = relu(xhat * g16 + b16), computed from the stored (rounded)
+// xhat with the packed arithmetic of the backward's ReLU mask, into the parity-class planes of the implicit conv2 GEMMs:
+//   a1[cls][b][t1 >> 1][f1 >> 1][C],  cls = ((t1 & 1) << 1) | (f1 & 1),  each plane T2 x F2 positions;
+// the class positions past an odd T1 / F1 (the conv2 border) are written as zeros by the last row / column.
 // ---------------------------------------------------------------------------------------------
 template <typename T, bool SAVE>
 __global__ void __launch_bounds__(256, 2) conv1_fwd_c256_kernel(const float* __restrict__ src, const float* __restrict__ w,
                                                                 const float* __restrict__ bias, const float* __restrict__ gamma,
                                                                 const float* __restrict__ beta, float eps, T* __restrict__ y,
-                                                                float* __restrict__ rstd_out, int B, int Tn, int F, int T1, int F1) {
+                                                                float* __restrict__ rstd_out, const T* __restrict__ g16,
+                                                                const T* __restrict__ b16, T* __restrict__ a1, int B, int Tn,
+                                                                int F, int T1, int F1) {
   pdl_wait();
   pdl_trigger();
   constexpr int C = 256;
@@ -246,6 +304,9 @@ __global__ void __launch_bounds__(256, 2) conv1_fwd_c256_kernel(const float* __r
   int f1 = (int)(pos % F1);
   int t1 = (int)((pos / F1) % T1);
   int b = (int)(pos / ((int64_t)F1 * T1));
+  const int T2 = (T1 + 1) / 2, F2 = (F1 + 1) / 2;
+  AffineRegs<T> ar;
+  if (SAVE && a1) ar.load(g16, b16, 8 * lane);
   const int tap_dt = lane / 3 - 1, tap_df = lane % 3 - 1;      // lanes 0..8 own one fbank tap each
   auto load_tap = [&](int bb, int tt1, int ff1) {
     float v = 0.f;
@@ -296,6 +357,22 @@ __global__ void __launch_bounds__(256, 2) conv1_fwd_c256_kernel(const float* __r
       for (int i = 0; i < 8; ++i) z[i] = fmaxf(fmaf(z[i] * rstd, greg[i], bereg[i]), 0.f);
     }
     store8<T>(y + pp * C + 8 * lane, z);
+    if constexpr (SAVE && sizeof(T) == 2) {
+      if (a1) {
+        uint4 pk;
+        pk.x = pack2_16(z[0], z[1], DTypeOf<T>::value); pk.y = pack2_16(z[2], z[3], DTypeOf<T>::value);
+        pk.z = pack2_16(z[4], z[5], DTypeOf<T>::value); pk.w = pack2_16(z[6], z[7], DTypeOf<T>::value);
+        const int cls = ((t1 & 1) << 1) | (f1 & 1);
+        T* dst = a1 + ((((int64_t)cls * B + b) * T2 + (t1 >> 1)) * F2 + (f1 >> 1)) * C + 8 * lane;
+        const int64_t plane = (int64_t)B * T2 * F2 * C;
+        *reinterpret_cast<uint4*>(dst) = affine_relu_vec(pk, ar.g, ar.b);
+        const bool tpad = !(t1 & 1) && t1 + 1 == T1, fpad = !(f1 & 1) && f1 + 1 == F1;
+        const uint4 zero = make_uint4(0, 0, 0, 0);
+        if (tpad) *reinterpret_cast<uint4*>(dst + 2 * plane) = zero;
+        if (fpad) *reinterpret_cast<uint4*>(dst + plane) = zero;
+        if (tpad && fpad) *reinterpret_cast<uint4*>(dst + 3 * plane) = zero;
+      }
+    }
   };
   float ring[RING];
 #pragma unroll
@@ -307,6 +384,7 @@ __global__ void __launch_bounds__(256, 2) conv1_fwd_c256_kernel(const float* __r
         ring[(j + RING - 1) % RING] = issue_next();
         process(pos, ring[j]);
         ++pos;
+        if (++f1 == F1) { f1 = 0; if (++t1 == T1) { t1 = 0; ++b; } }
       }
     }
   }
@@ -420,28 +498,38 @@ __global__ void __launch_bounds__(256, (CPL <= 8 ? 2 : 1)) conv1_bwd_fused_kerne
 
 // ---------------------------------------------------------------------------------------------
 // Backward from the saved normalised activations (C == 256, Cin == 1): col2im gather of dcol + ReLU' + LN' with xhat and
-// 1/sigma read back (no convolution recompute, no statistics), db/dgamma/dbeta partials, fbank im2col rows for dW1.
+// 1/sigma read back (no convolution recompute, no statistics), db/dgamma/dbeta partials, and dz1 + fbank im2col rows for the
+// dW1 GEMM (or, IMPLICIT, dW1 itself).
 // ---------------------------------------------------------------------------------------------
 // IMPLICIT: `dcol` is the class-major tiled input gradient written by the implicit conv2 data-gradient GEMMs
-// (tc_gemm.cu: conv2_dgrad_implicit) — one row per position instead of up to four tap rows to gather.
+// (tc_gemm.cu: conv2_dgrad_implicit) — one row per position instead of up to four tap rows to gather — and conv1's filter
+// gradient dW1[tap][c] += src_tap * dz1[c] is accumulated here (fp32, with the 16-bit rounding of both factors that the
+// explicit GEMM over col1 / dz1 applied), so neither dz1 nor col1 is written.  Its 72 accumulators per lane do not fit the
+// 128-register budget of two CTAs per SM: one CTA per SM, with a twice deeper load ring to keep the same bytes in flight.
 template <typename T, bool IMPLICIT>
-__global__ void __launch_bounds__(256, 2) conv1_bwd_xhat_c256_kernel(
+__global__ void __launch_bounds__(256, IMPLICIT ? 1 : 2) conv1_bwd_xhat_c256_kernel(
     const float* __restrict__ src, const T* __restrict__ gamma, const T* __restrict__ beta, const T* __restrict__ xhat,
     const float* __restrict__ rstd, const T* __restrict__ dcol, T* __restrict__ dz1, T* __restrict__ col1, int K1p,
-    float* __restrict__ db, float* __restrict__ dgamma, float* __restrict__ dbeta, int B, int Tn, int F, int T1, int F1, int T2,
-    int F2, int tu, int ub) {
+    float* __restrict__ dw1, float* __restrict__ db, float* __restrict__ dgamma, float* __restrict__ dbeta, int B, int Tn, int F,
+    int T1, int F1, int T2, int F2, int tu, int ub) {
   pdl_wait();
   pdl_trigger();
   constexpr int C = 256;
-  __shared__ float sacc[3 * C];
-  for (int i = threadIdx.x; i < 3 * C; i += blockDim.x) sacc[i] = 0.f;
+  constexpr int NACC = IMPLICIT ? 12 : 3;      // db | dgamma | dbeta (| dW1, 9 taps)
+  __shared__ float sacc[NACC * C];
+  for (int i = threadIdx.x; i < NACC * C; i += blockDim.x) sacc[i] = 0.f;
   __syncthreads();
   const int lane = threadIdx.x & 31;
   float greg[8], breg[8], a_db[8], a_dg[8], a_dbe[8];
+  float a_dw[IMPLICIT ? 9 : 1][8];
   ld8<T>(gamma + 8 * lane, greg);       // affine parameters exactly as the forward used them (bf16 shadow in bf16 mode)
   ld8<T>(beta + 8 * lane, breg);
 #pragma unroll
   for (int i = 0; i < 8; ++i) a_db[i] = a_dg[i] = a_dbe[i] = 0.f;
+#pragma unroll
+  for (int tp = 0; tp < (IMPLICIT ? 9 : 1); ++tp)
+#pragma unroll
+    for (int i = 0; i < 8; ++i) a_dw[tp][i] = 0.f;
   const int64_t npos = (int64_t)B * T1 * F1;
   const int64_t nwarps = (int64_t)gridDim.x * (blockDim.x >> 5);
   const int64_t wid = (int64_t)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
@@ -457,7 +545,7 @@ __global__ void __launch_bounds__(256, 2) conv1_bwd_xhat_c256_kernel(
     // bound by bytes in flight, not by bandwidth — the implicit variant loads
     // one gradient row instead of four and spends the freed registers on a deeper ring
     constexpr int NDC = IMPLICIT ? 1 : 4;
-    constexpr int RING = IMPLICIT ? 4 : 2;
+    constexpr int RING = IMPLICIT ? 6 : 2;
     struct Loads { Vec8<T> xh, dc[NDC]; float rs, xv; };
     auto issue = [&](int64_t p, int bb, int tt1, int ff1, Loads& L) {
       L.xv = 0.f;
@@ -487,6 +575,19 @@ __global__ void __launch_bounds__(256, 2) conv1_bwd_xhat_c256_kernel(
         }
       }
     };
+    // IMPLICIT: the filter-gradient update of a position is made during the next position's statistics reductions (shuffle
+    // chains that would otherwise leave the scheduler idle at one CTA per SM)
+    float prev_d[8], prev_x = 0.f;
+#pragma unroll
+    for (int i = 0; i < 8; ++i) prev_d[i] = 0.f;
+    auto dw_update = [&]() {
+#pragma unroll
+      for (int tp = 0; tp < 9; ++tp) {
+        const float x = __shfl_sync(0xffffffffu, prev_x, tp);
+#pragma unroll
+        for (int i = 0; i < 8; ++i) a_dw[tp][i] = fmaf(x, prev_d[i], a_dw[tp][i]);
+      }
+    };
     auto process = [&](int64_t pp, const Loads& cur) {
       float xh[8], d[8];
       cur.xh.get(xh);
@@ -507,13 +608,20 @@ __global__ void __launch_bounds__(256, 2) conv1_bwd_xhat_c256_kernel(
         c1 += g; c2s = fmaf(g, xh[i], c2s);
         a_dg[i] = fmaf(d[i], xh[i], a_dg[i]); a_dbe[i] += d[i];
       }
+      if constexpr (IMPLICIT) dw_update();
 #pragma unroll
       for (int o = 16; o > 0; o >>= 1) { c1 += __shfl_xor_sync(0xffffffffu, c1, o); c2s += __shfl_xor_sync(0xffffffffu, c2s, o); }
       c1 *= (1.0f / C); c2s *= (1.0f / C);
 #pragma unroll
       for (int i = 0; i < 8; ++i) { d[i] = rs * (d[i] * greg[i] - c1 - xh[i] * c2s); a_db[i] += d[i]; }
-      store8<T>(dz1 + pp * C + 8 * lane, d);
-      if (lane < K1p) col1[pp * K1p + lane] = from_f32<T>(lane < 9 ? cur.xv : 0.f);
+      if constexpr (IMPLICIT) {
+        prev_x = to_f32(from_f32<T>(cur.xv));
+#pragma unroll
+        for (int i = 0; i < 8; ++i) prev_d[i] = to_f32(from_f32<T>(d[i]));
+      } else {
+        store8<T>(dz1 + pp * C + 8 * lane, d);
+        if (lane < K1p) col1[pp * K1p + lane] = from_f32<T>(lane < 9 ? cur.xv : 0.f);
+      }
     };
     // issue cursor (position whose loads are issued next) runs RING-1 positions ahead of the compute cursor `pos`
     int64_t ipos = pos;
@@ -540,68 +648,28 @@ __global__ void __launch_bounds__(256, 2) conv1_bwd_xhat_c256_kernel(
         }
       }
     }
+    if constexpr (IMPLICIT) dw_update();      // the last position
   }
 #pragma unroll
   for (int i = 0; i < 8; ++i) {
     const int c = 8 * lane + i;
     atomicAdd(&sacc[c], a_db[i]); atomicAdd(&sacc[C + c], a_dg[i]); atomicAdd(&sacc[2 * C + c], a_dbe[i]);
+    if constexpr (IMPLICIT) {
+#pragma unroll
+      for (int tp = 0; tp < 9; ++tp) atomicAdd(&sacc[(3 + tp) * C + c], a_dw[tp][i]);
+    }
   }
   __syncthreads();
   for (int i = threadIdx.x; i < C; i += blockDim.x) {
     atomicAdd(&db[i], sacc[i]); atomicAdd(&dgamma[i], sacc[C + i]); atomicAdd(&dbeta[i], sacc[2 * C + i]);
   }
+  if constexpr (IMPLICIT)
+    for (int i = threadIdx.x; i < 9 * C; i += blockDim.x) atomicAdd(&dw1[i], sacc[3 * C + i]);
 }
 
 // ---------------------------------------------------------------------------------------------
 // im2col for the 3x3 stride-2 pad-1 conv2 (NHWC): one warp per (row, tap) chunk of C channels
 // ---------------------------------------------------------------------------------------------
-// y = relu(x * gamma + beta) on one 16-byte vector (affine parameters in the activation dtype: for bf16 they come from
-// the bf16 shadow arena and the math is packed HFMA2.BF16 / HMNMX2 — the same rounding the backward's ReLU mask assumes)
-__device__ __forceinline__ uint4 affine_relu_vec(uint4 v, const __nv_bfloat162 (&g)[4], const __nv_bfloat162 (&b)[4]) {
-  __nv_bfloat162* h = reinterpret_cast<__nv_bfloat162*>(&v);
-  const __nv_bfloat162 zero = __floats2bfloat162_rn(0.f, 0.f);
-#pragma unroll
-  for (int j = 0; j < 4; ++j) h[j] = __hmax2(__hfma2(h[j], g[j], b[j]), zero);
-  return v;
-}
-__device__ __forceinline__ uint4 affine_relu_vec(uint4 v, const __half2 (&g)[4], const __half2 (&b)[4]) {
-  __half2* h = reinterpret_cast<__half2*>(&v);
-  const __half2 zero = __floats2half2_rn(0.f, 0.f);
-#pragma unroll
-  for (int j = 0; j < 4; ++j) h[j] = __hmax2(__hfma2(h[j], g[j], b[j]), zero);
-  return v;
-}
-__device__ __forceinline__ uint4 affine_relu_vec(uint4 v, const float (&g)[4], const float (&b)[4]) {
-  float* f = reinterpret_cast<float*>(&v);
-#pragma unroll
-  for (int j = 0; j < 4; ++j) f[j] = fmaxf(fmaf(f[j], g[j], b[j]), 0.f);
-  return v;
-}
-template <typename T> struct AffineRegs;
-template <> struct AffineRegs<__nv_bfloat16> {
-  __nv_bfloat162 g[4], b[4];
-  __device__ __forceinline__ void load(const __nv_bfloat16* gamma, const __nv_bfloat16* beta, int c) {
-    const uint4 gv = __ldg(reinterpret_cast<const uint4*>(gamma + c)), bv = __ldg(reinterpret_cast<const uint4*>(beta + c));
-#pragma unroll
-    for (int j = 0; j < 4; ++j) { g[j] = reinterpret_cast<const __nv_bfloat162*>(&gv)[j]; b[j] = reinterpret_cast<const __nv_bfloat162*>(&bv)[j]; }
-  }
-};
-template <> struct AffineRegs<__half> {
-  __half2 g[4], b[4];
-  __device__ __forceinline__ void load(const __half* gamma, const __half* beta, int c) {
-    const uint4 gv = __ldg(reinterpret_cast<const uint4*>(gamma + c)), bv = __ldg(reinterpret_cast<const uint4*>(beta + c));
-#pragma unroll
-    for (int j = 0; j < 4; ++j) { g[j] = reinterpret_cast<const __half2*>(&gv)[j]; b[j] = reinterpret_cast<const __half2*>(&bv)[j]; }
-  }
-};
-template <> struct AffineRegs<float> {
-  float g[4], b[4];
-  __device__ __forceinline__ void load(const float* gamma, const float* beta, int c) {
-    const float4 gv = __ldg(reinterpret_cast<const float4*>(gamma + c)), bv = __ldg(reinterpret_cast<const float4*>(beta + c));
-    g[0] = gv.x; g[1] = gv.y; g[2] = gv.z; g[3] = gv.w; b[0] = bv.x; b[1] = bv.y; b[2] = bv.z; b[3] = bv.w;
-  }
-};
-
 // gamma != null: the source holds the normalised conv1 activations; y = relu(x * gamma + beta) is applied in flight.
 // ONE: C == 32 vectors, i.e. each lane owns exactly one 16-byte vector of the row (affine parameters stay in registers).
 template <typename T, bool VEC, bool ONE>
@@ -708,6 +776,21 @@ int conv1_norm_fwd(const float* src, const float* w, const float* b, float eps, 
   B200ST_CHECK(rstd != nullptr, "conv1_norm_fwd needs the rstd buffer");
   return conv1_fwd_launch(src, w, b, nullptr, nullptr, eps, xhat, dtype, B, T, F, Cin, C, 0, rstd, s);
 }
+// ... and the post-activation into the parity-class planes of the implicit conv2 GEMMs (16-bit, C == 256, Cin == 1)
+int conv1_norm_fwd_planes(const float* src, const float* w, const float* b, float eps, void* xhat, int dtype, float* rstd,
+                          const void* g16, const void* b16, void* a1, int B, int T, int F, int C, cudaStream_t s) {
+  B200ST_CHECK(is16(dtype) && C == 256, "conv1_norm_fwd_planes: 16-bit, C == 256, Cin == 1");
+  B200ST_CHECK(((reinterpret_cast<uintptr_t>(xhat) | reinterpret_cast<uintptr_t>(a1) | reinterpret_cast<uintptr_t>(w) |
+                 reinterpret_cast<uintptr_t>(b) | reinterpret_cast<uintptr_t>(g16) | reinterpret_cast<uintptr_t>(b16)) & 15) == 0,
+               "conv1 forward buffers must be 16-byte aligned");
+  const int T1 = (T + 1) / 2, F1 = (F + 1) / 2;
+  const int64_t npos = (int64_t)B * T1 * F1;
+  if (npos == 0) return 0;
+  const int grid1 = grid_for(npos, 8 * 16, 132 * 2);
+  DISPATCH_DTYPE(dtype, TT, (launch(conv1_fwd_c256_kernel<TT, true>, grid1, 256, 0, s, src, w, b, nullptr, nullptr, eps, (TT*)xhat, rstd,
+                                    (const TT*)g16, (const TT*)b16, (TT*)a1, B, T, F, T1, F1)));
+  return 0;
+}
 
 static int conv1_fwd_launch(const float* src, const float* w, const float* b, const float* gamma, const float* beta, float eps,
                             void* y1, int y_dtype, int B, int T, int F, int Cin, int C, int use_ln, float* rstd_out, cudaStream_t s) {
@@ -720,8 +803,10 @@ static int conv1_fwd_launch(const float* src, const float* w, const float* b, co
   if (vec && C == 256 && Cin == 1 && (use_ln || rstd_out) && ((reinterpret_cast<uintptr_t>(w) & 15) == 0) &&
       ((reinterpret_cast<uintptr_t>(b) & 15) == 0) && (rstd_out || (((reinterpret_cast<uintptr_t>(gamma) | reinterpret_cast<uintptr_t>(beta)) & 15) == 0))) {
     const int grid1 = grid_for(npos, 8 * 16, 132 * 2);
-    if (rstd_out) DISPATCH_DTYPE(y_dtype, TT, (launch(conv1_fwd_c256_kernel<TT, true>, grid1, 256, 0, s, src, w, b, gamma, beta, eps, (TT*)y1, rstd_out, B, T, F, T1, F1)));
-    else DISPATCH_DTYPE(y_dtype, TT, (launch(conv1_fwd_c256_kernel<TT, false>, grid1, 256, 0, s, src, w, b, gamma, beta, eps, (TT*)y1, rstd_out, B, T, F, T1, F1)));
+    if (rstd_out) DISPATCH_DTYPE(y_dtype, TT, (launch(conv1_fwd_c256_kernel<TT, true>, grid1, 256, 0, s, src, w, b, gamma, beta, eps, (TT*)y1, rstd_out,
+                                                      (const TT*)nullptr, (const TT*)nullptr, (TT*)nullptr, B, T, F, T1, F1)));
+    else DISPATCH_DTYPE(y_dtype, TT, (launch(conv1_fwd_c256_kernel<TT, false>, grid1, 256, 0, s, src, w, b, gamma, beta, eps, (TT*)y1, rstd_out,
+                                             (const TT*)nullptr, (const TT*)nullptr, (TT*)nullptr, B, T, F, T1, F1)));
     return 0;
   }
   const size_t smem = (size_t)(9 * Cin + 1) * ((C + 255) & ~255) * sizeof(float);
@@ -762,25 +847,32 @@ int conv1_bwd_fused(const float* src, const float* w, const float* b, const floa
   return 0;
 }
 
-// backward of the normalised-save front-end (C == 256, Cin == 1, 16-byte aligned rows)
+// backward of the normalised-save front-end (C == 256, Cin == 1, 16-byte aligned rows).  implicit_tiles: dcol holds the
+// class-major tiles of conv2_dgrad_implicit and conv1's filter gradient is accumulated into dw1 (dz1 / col1 unused); else
+// dcol is the explicit column gradient and dz1 / col1 are written for the filter-gradient GEMM.
 int conv1_bwd_from_xhat(const float* src, const void* gamma, const void* beta, const void* xhat, const float* rstd,
-                        const void* dcol, int dtype, void* dz1, void* col1, int K1p, float* db, float* dgamma, float* dbeta, int B,
-                        int T, int F, int C, cudaStream_t s, int implicit_tiles) {
+                        const void* dcol, int dtype, void* dz1, void* col1, int K1p, float* dw1, float* db, float* dgamma,
+                        float* dbeta, int B, int T, int F, int C, cudaStream_t s, int implicit_tiles) {
   B200ST_CHECK(C == 256 && K1p >= 9 && K1p <= 32, "conv1_bwd_from_xhat supports C == 256, Cin == 1");
   B200ST_CHECK(((reinterpret_cast<uintptr_t>(xhat) | reinterpret_cast<uintptr_t>(dcol) | reinterpret_cast<uintptr_t>(dz1) |
                  reinterpret_cast<uintptr_t>(gamma) | reinterpret_cast<uintptr_t>(beta)) & 15) == 0, "conv1 backward buffers must be 16-byte aligned");
   const int T1 = (T + 1) / 2, F1 = (F + 1) / 2, T2 = (T1 + 1) / 2, F2 = (F1 + 1) / 2;
   const int64_t npos = (int64_t)B * T1 * F1;
   if (npos == 0) return 0;
-  const int grid = grid_for(npos, 8 * 16, 132 * 2);
   const int tu = F2 > 0 && F2 <= 128 ? 128 / F2 : 1, ub = (T2 + tu - 1) / tu;
   if (implicit_tiles) {
-    B200ST_CHECK(F2 <= 128, "implicit conv2 dgrad layout needs F2 <= 128");
-    DISPATCH_DTYPE(dtype, TT, (launch(conv1_bwd_xhat_c256_kernel<TT, true>, grid, 256, 0, s, src, (const TT*)gamma, (const TT*)beta, (const TT*)xhat, rstd,
-                                          (const TT*)dcol, (TT*)dz1, (TT*)col1, K1p, db, dgamma, dbeta, B, T, F, T1, F1, T2, F2, tu, ub)));
+    B200ST_CHECK(F2 <= 128 && dw1 != nullptr, "implicit conv2 dgrad layout needs F2 <= 128 and the dW1 accumulator");
+    const int grid = grid_for(npos, 8 * 16, 132);
+    B200ST_CHECK(is16(dtype), "implicit conv2 dgrad layout is 16-bit");
+#define BWD_IMPLICIT(TT)                                                                                                          \
+  launch(conv1_bwd_xhat_c256_kernel<TT, true>, grid, 256, 0, s, src, (const TT*)gamma, (const TT*)beta, (const TT*)xhat, rstd,   \
+         (const TT*)dcol, (TT*)nullptr, (TT*)nullptr, K1p, dw1, db, dgamma, dbeta, B, T, F, T1, F1, T2, F2, tu, ub)
+    B200ST_TRY(dtype == F16 ? BWD_IMPLICIT(__half) : BWD_IMPLICIT(__nv_bfloat16));
+#undef BWD_IMPLICIT
   } else {
+    const int grid = grid_for(npos, 8 * 16, 132 * 2);
     DISPATCH_DTYPE(dtype, TT, (launch(conv1_bwd_xhat_c256_kernel<TT, false>, grid, 256, 0, s, src, (const TT*)gamma, (const TT*)beta, (const TT*)xhat, rstd,
-                                          (const TT*)dcol, (TT*)dz1, (TT*)col1, K1p, db, dgamma, dbeta, B, T, F, T1, F1, T2, F2, tu, ub)));
+                                          (const TT*)dcol, (TT*)dz1, (TT*)col1, K1p, (float*)nullptr, db, dgamma, dbeta, B, T, F, T1, F1, T2, F2, tu, ub)));
   }
   return 0;
 }

@@ -192,16 +192,26 @@ int conv1_bwd_fused(const float* src, const float* w, const float* b, const floa
                     float* dbeta, int B, int T, int F, int Cin, int C, int use_ln, cudaStream_t s);
 // col[(b,t2,f2), (kh,kw,c)] = y1[b, 2*t2+kh-1, 2*f2+kw-1, c] (zero outside)
 int im2col_3x3s2(const void* y1, void* col, int dtype, int B, int T1, int F1, int C, cudaStream_t s);
-// normalised-save front-end (training path at C == 256, Cin == 1): conv1 stores xhat + 1/sigma, the im2col applies
+// normalised-save front-end (C == 256, Cin == 1): conv1 stores xhat + 1/sigma, the im2col (fp32, F2 > 128) applies
 // gamma / beta / ReLU in flight, the backward reads xhat back instead of recomputing the convolution
 int conv1_norm_fwd(const float* src, const float* w, const float* b, float eps, void* xhat, int dtype, float* rstd, int B, int T,
                    int F, int Cin, int C, cudaStream_t s);
 int im2col_3x3s2_affine(const void* y1, void* col, int dtype, int B, int T1, int F1, int C, const void* gamma, const void* beta,
                         cudaStream_t s);   // gamma / beta in the activation dtype (bf16 shadow or fp32 master)
+// ... which also writes a1 = relu(xhat * g16 + b16) (16-bit affine parameters) as the parity-class planes
+// a1[4][B][T2][F2][C] that the implicit conv2 forward and filter-gradient GEMMs read
+int conv1_norm_fwd_planes(const float* src, const float* w, const float* b, float eps, void* xhat, int dtype, float* rstd,
+                          const void* g16, const void* b16, void* a1, int B, int T, int F, int C, cudaStream_t s);
+// implicit_tiles: dcol = conv2_dgrad_implicit's tiles and dW1 += src_tap * dz1 is accumulated into dw1 (dz1 / col1 unused)
 int conv1_bwd_from_xhat(const float* src, const void* gamma, const void* beta, const void* xhat, const float* rstd,
-                        const void* dcol, int dtype, void* dz1, void* col1, int K1p, float* db, float* dgamma, float* dbeta, int B,
-                        int T, int F, int C, cudaStream_t s, int implicit_tiles = 0);
-// conv2 data gradient as four implicit GEMMs (tc_gemm.cu); da = class-major padded tiles, conv2_dgrad_implicit_elems() elements
+                        const void* dcol, int dtype, void* dz1, void* col1, int K1p, float* dw1, float* db, float* dgamma,
+                        float* dbeta, int B, int T, int F, int C, cudaStream_t s, int implicit_tiles);
+// conv2 as implicit GEMMs over the parity-class planes of conv1_norm_fwd_planes (tc_gemm.cu): forward z2 [B, T2, F2, C] =
+// conv(a1) + bias; filter gradient dw [9C, C] += a1_tap^T dz2 (fp32 split-K); data gradient into class-major padded tiles,
+// conv2_dgrad_implicit_elems() elements
+int conv2_fwd_implicit(const void* a1, const void* w16, const float* bias, void* z2, int dtype, int B, int T2, int F2, int C,
+                       cudaStream_t stream);
+int conv2_wgrad_implicit(const void* a1, const void* dz2, float* dw, int dtype, int B, int T2, int F2, int C, cudaStream_t stream);
 int conv2_dgrad_implicit(const void* dy, const void* w16, void* da, int dtype, int B, int T2, int F2, int C, cudaStream_t stream);
 int64_t conv2_dgrad_implicit_elems(int B, int T2, int F2, int C);
 

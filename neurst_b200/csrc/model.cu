@@ -808,12 +808,18 @@ struct FrontSave {
   void* y1 = nullptr; void* col = nullptr; void* z2 = nullptr; void* y2 = nullptr;
   float* mean2 = nullptr; float* rstd2 = nullptr;
   float* rstd1 = nullptr;    // normalised-save mode: y1 holds xhat of conv1's LayerNorm, rstd1 its 1/sigma
+  void* a1 = nullptr;        // implicit mode: conv1's post-activation as parity-class planes (no column matrix `col`)
+  bool implicit = false;
   int B = 0, T = 0, T1 = 0, F1 = 0, T2 = 0, F2 = 0;
   uint64_t s_in = 0;
 };
 
 // conv1's LayerNorm output is saved normalised (xhat + 1/sigma) instead of post-ReLU when the fast kernels apply
 static bool front_saves_xhat(const Config& cf) { return cf.conv_layer_norm && cf.channels == 256 && cf.in_channels == 1; }
+// conv2 as implicit GEMMs over parity-split planes in all three products (forward, filter and data gradient) and conv1's
+// filter gradient inside its backward kernel; otherwise the explicit column matrix and GEMMs.  One decision for the forward
+// and the backward.
+static bool front_implicit(const Ctx& c, int F2) { return front_saves_xhat(c.m.cfg) && is16(c.adt) && F2 <= 128; }
 
 // src fp32 [B,T,F,Cin] -> x0 fp32 [B*T2, d] = dropout((dense(flatten(conv stack))) * sqrt(d) + pos)
 static int speech_front_fwd(Ctx& c, const float* src, int B, int T, float* x0, FrontSave& sv) {
@@ -823,13 +829,21 @@ static int speech_front_fwd(Ctx& c, const float* src, int B, int T, float* x0, F
   sv.B = B; sv.T = T; sv.T1 = T1; sv.F1 = F1; sv.T2 = T2; sv.F2 = F2;
   sv.s_in = dropout_stream_id("enc.in_drop");
   const int64_t R1 = (int64_t)B * T1 * F1, R2 = (int64_t)B * T2 * F2;
+  sv.implicit = front_implicit(c, F2);
   sv.y1 = c.act(R1 * C);
-  sv.col = c.act(R2 * 9 * C);
+  if (sv.implicit) sv.a1 = c.act(4 * (int64_t)B * T2 * F2 * C);
+  else sv.col = c.act(R2 * 9 * C);
   sv.z2 = c.act(R2 * C);
   sv.y2 = c.act(R2 * C);
   sv.mean2 = c.f32(R2); sv.rstd2 = c.f32(R2);
   float* e0 = c.f32((int64_t)B * T2 * d);
-  if (front_saves_xhat(cf)) {
+  if (sv.implicit) {
+    sv.rstd1 = c.f32(R1);
+    RUN(conv1_norm_fwd_planes(src, c.P("src.conv1.kernel"), c.P("src.conv1.bias"), 1e-6f, sv.y1, c.adt, sv.rstd1,
+                              c.W("src.ln1.gamma", 0, C).ptr, c.W("src.ln1.beta", 0, C).ptr, sv.a1, B, T, F, C, c.st));
+    B200ST_TRY(need_param(c, "src.conv2.kernel"));
+    RUN(conv2_fwd_implicit(sv.a1, c.W("src.conv2.kernel", 1, C).ptr, c.P("src.conv2.bias"), sv.z2, c.adt, B, T2, F2, C, c.st));
+  } else if (front_saves_xhat(cf)) {
     sv.rstd1 = c.f32(R1);
     RUN(conv1_norm_fwd(src, c.P("src.conv1.kernel"), c.P("src.conv1.bias"), 1e-6f, sv.y1, c.adt, sv.rstd1, B, T, F, cf.in_channels, C,
                        c.st));
@@ -841,7 +855,8 @@ static int speech_front_fwd(Ctx& c, const float* src, int B, int T, float* x0, F
   }
   GemmEpilogue ez = gemm_defaults().epi;
   if (cf.conv_layer_norm) {
-    B200ST_TRY(linear_fwd(c, sv.col, 9 * C, (int)R2, 9 * C, C, "src.conv2.kernel", "src.conv2.bias", ez, sv.z2, c.adt, C));
+    if (!sv.implicit)
+      B200ST_TRY(linear_fwd(c, sv.col, 9 * C, (int)R2, 9 * C, C, "src.conv2.kernel", "src.conv2.bias", ez, sv.z2, c.adt, C));
     RUN(layernorm_fwd(sv.z2, c.adt, c.P("src.ln2.gamma"), c.P("src.ln2.beta"), 1e-6f, sv.y2, c.adt, nullptr, sv.mean2, sv.rstd2, R2, C,
                       1, c.st));
   } else {
@@ -865,11 +880,11 @@ static int speech_front_bwd(Ctx& c, const float* src, const float* dx0, const Fr
   void* dz2 = c.act(R2 * C);
   // conv2's data gradient: implicit GEMMs straight from dz2 into class-major tiles (no [rows, 9C] column gradient), or the
   // explicit dcol = dz2 W^T + gather in conv1's backward
-  const bool implicit_dgrad = front_saves_xhat(cf) && is16(c.adt) && C == 256 && sv.F2 <= 128;
-  void* dcol = c.act(implicit_dgrad ? conv2_dgrad_implicit_elems(B, sv.T2, sv.F2, C) : R2 * 9 * C);
-  void* dz1 = c.act(R1 * C);
+  const bool implicit = sv.implicit;
+  void* dcol = c.act(implicit ? conv2_dgrad_implicit_elems(B, sv.T2, sv.F2, C) : R2 * 9 * C);
   const int K1p = (9 * cf.in_channels + 7) / 8 * 8;
-  void* col1 = c.act(R1 * K1p);
+  void* dz1 = implicit ? nullptr : c.act(R1 * C);
+  void* col1 = implicit ? nullptr : c.act(R1 * K1p);
   RUN(posenc_bwd(dx0, de0, c.adt, (int64_t)Mx * d, sqrtf((float)d), c.drop(cf.postprocess_dropout, sv.s_in), c.st));
   B200ST_TRY(linear_wgrad(c, sv.y2, (int64_t)sv.F2 * C, de0, d, Mx, sv.F2 * C, d, "src.dense.kernel", "src.dense.bias"));
   GemmEpilogue e0 = gemm_defaults().epi;
@@ -880,19 +895,29 @@ static int speech_front_bwd(Ctx& c, const float* src, const float* dx0, const Fr
   } else {
     B200ST_FAIL("training without conv layer norm is not implemented");
   }
-  B200ST_TRY(linear_wgrad(c, sv.col, 9 * C, dz2, C, (int)R2, 9 * C, C, "src.conv2.kernel", "src.conv2.bias"));
-  if (implicit_dgrad) RUN(conv2_dgrad_implicit(dz2, c.W("src.conv2.kernel", 0, C).ptr, dcol, c.adt, B, sv.T2, sv.F2, C, c.st));
-  else B200ST_TRY(linear_dgrad(c, dz2, C, (int)R2, C, 9 * C, "src.conv2.kernel", e0, dcol, c.adt, 9 * C));
-  // fused: col2im gather + ReLU' + LN' -> dz1, fbank im2col rows, db/dgamma/dbeta (xhat read back, or z1 recomputed)
+  if (implicit) {
+    B200ST_TRY(need_param(c, "src.conv2.kernel"));
+    cudaStream_t ws = c.wgrad_stream();
+    RUN(conv2_wgrad_implicit(sv.a1, dz2, c.G("src.conv2.kernel"), c.adt, B, sv.T2, sv.F2, C, ws));
+    RUN(colsum_accum(dz2, c.adt, (int)R2, C, C, c.G("src.conv2.bias"), ws));
+    c.wgrad_done(ws);
+    RUN(conv2_dgrad_implicit(dz2, c.W("src.conv2.kernel", 0, C).ptr, dcol, c.adt, B, sv.T2, sv.F2, C, c.st));
+  } else {
+    B200ST_TRY(linear_wgrad(c, sv.col, 9 * C, dz2, C, (int)R2, 9 * C, C, "src.conv2.kernel", "src.conv2.bias"));
+    B200ST_TRY(linear_dgrad(c, dz2, C, (int)R2, C, 9 * C, "src.conv2.kernel", e0, dcol, c.adt, 9 * C));
+  }
+  // fused: col2im gather + ReLU' + LN' -> dz1, fbank im2col rows, db/dgamma/dbeta (xhat read back, or z1 recomputed); in
+  // implicit mode conv1's filter gradient too
   if (front_saves_xhat(cf)) {
     RUN(conv1_bwd_from_xhat(src, c.W("src.ln1.gamma", 0, C).ptr, c.W("src.ln1.beta", 0, C).ptr, sv.y1, sv.rstd1, dcol, c.adt, dz1, col1, K1p,
-                            c.G("src.conv1.bias"), c.G("src.ln1.gamma"), c.G("src.ln1.beta"), B, sv.T, F, C, c.st, implicit_dgrad ? 1 : 0));
+                            implicit ? c.G("src.conv1.kernel") : nullptr, c.G("src.conv1.bias"), c.G("src.ln1.gamma"), c.G("src.ln1.beta"),
+                            B, sv.T, F, C, c.st, implicit ? 1 : 0));
   } else {
     RUN(conv1_bwd_fused(src, c.P("src.conv1.kernel"), c.P("src.conv1.bias"), c.P("src.ln1.gamma"), c.P("src.ln1.beta"), 1e-6f, sv.y1,
                         dcol, c.adt, dz1, col1, K1p, c.G("src.conv1.bias"), c.G("src.ln1.gamma"), c.G("src.ln1.beta"), B, sv.T, F,
                         cf.in_channels, C, cf.conv_layer_norm, c.st));
   }
-  {
+  if (!implicit) {
     // dW1[9*Cin, C] += col1^T dz1   (split-K wgmma GEMM over all B*T1*F1 positions)
     GemmArgs g = gemm_defaults();
     g.M = 9 * cf.in_channels; g.N = C; g.K = (int)R1;

@@ -58,15 +58,19 @@ struct TcParams {
   int atomic;           // C += through fp32 atomics (split-K or accumulate)
   int vec2;             // C may be written two columns at a time (even N, ld and batch strides; 8-byte aligned base)
   int plain16;          // 16-bit C, plain stores, epilogue = alpha (+ bias) only: the short epilogue loop applies
-  // implicit transposed-convolution A operand (conv2 data gradient, see gemm_conv2_dgrad): A tile = a [conv_tu x conv_v]
-  // patch of positions x 64 channels of dY[B, T2, F2, C], shifted by the tap; k-block kb = (tap, 64-channel chunk)
-  int conv;             // 0 = off
+  // Implicit convolution A operand (tc_gemm_kernel<..., CONV = true>; conv2 of the speech front-end, see ConvA): A tile = conv_tu time rows x F2 positions of
+  // one plane x 64 channels, read as a 4-D box (channels, F2, time rows, plane) shifted by the tap — coordinates outside the
+  // tensor are zero-filled by the TMA unit, which is the convolution's pad-1 border; k-block kb = (tap, 64-channel chunk).
+  // The data gradient writes the tiles as they are (class-major tiles); the forward (conv_remap) sends tile rows to the
+  // dense [B, T2, F2] rows of its output and drops the rows past the image.
   int conv_ub;          // row tiles per utterance
   int conv_tu;          // time rows per tile
   int conv_kpc;         // k-blocks per tap (C / 64)
-  int conv_dt[4], conv_df[4], conv_wrow[4];   // per tap: time / frequency shift into dY, first row of the tap in the weight matrix
-  uint32_t conv_a_bytes;                      // bytes one A box delivers (64 ch x conv_v x conv_tu x 2)
+  int conv_remap, conv_T2, conv_F2;
+  int conv_dt[9], conv_df[9], conv_wrow[9], conv_plane[9];   // per tap: time / frequency shift, first weight row, first plane
+  uint32_t conv_a_bytes;                      // bytes one A box delivers (64 ch x F2 x conv_tu x 2)
 };
+constexpr int kConvRows = 1, kConvWgrad = 2;   // ConvA::mode: tc_gemm_kernel's A operand, or tc_wgrad_group_kernel's operands
 
 struct TileCoord { int b2, b1, m_blk, n_blk, split; };
 
@@ -188,10 +192,12 @@ __device__ __forceinline__ void consume_tile(float (&acc)[2][BN / 2], Ring& r, i
   if (prev >= 0 && lane == 0) ptx::mbar_arrive(r.empty(prev));
 }
 
-template <int BN, bool A_MN, bool B_MN, bool BF>
-__global__ void __launch_bounds__(kThreads, 1)
-tc_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, const TcParams p) {
+// CONV: implicit conv2 A operand (TcParams conv fields; K-major A only), compiled into an entry point of its own
+// (tc_gemm_conv_kernel) so that the plain GEMMs carry none of its code.
+template <int BN, bool A_MN, bool B_MN, bool BF, bool CONV>
+__device__ __forceinline__ void tc_gemm_body(const CUtensorMap& tmA, const CUtensorMap& tmB, const TcParams& p) {
   static_assert(BN <= 128, "a consumer warpgroup holds the whole 128 x BN accumulator");
+  static_assert(!CONV || !A_MN, "the implicit conv A operand is K-major");
   extern __shared__ uint8_t smem_raw[];
   constexpr uint32_t kBBytes = BN * BK * 2;
   constexpr uint32_t kStageBytes = kABytes + kBBytes;
@@ -229,16 +235,20 @@ tc_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
           ptx::mbar_wait(ring.empty(ring.stage), ring.phase ^ 1u);
           const uint32_t sa = ring.slot();
           const uint32_t sb = sa + kABytes;
-          if constexpr (!A_MN && !B_MN) {
-            if (p.conv) {
-              const int tap = kb / p.conv_kpc, c0 = (kb - tap * p.conv_kpc) * BK;
-              ptx::mbar_arrive_expect_tx(ring.full(), p.conv_a_bytes + kBBytes);
-              ptx::tma_load_4d(sa, &tmA, ring.full(), c0, p.conv_df[tap], (t.m_blk % p.conv_ub) * p.conv_tu + p.conv_dt[tap],
-                               t.m_blk / p.conv_ub);
+          if constexpr (CONV) {
+            const int tap = kb / p.conv_kpc, c0 = (kb - tap * p.conv_kpc) * BK;
+            ptx::mbar_arrive_expect_tx(ring.full(), p.conv_a_bytes + kBBytes);
+            ptx::tma_load_4d(sa, &tmA, ring.full(), c0, p.conv_df[tap], (t.m_blk % p.conv_ub) * p.conv_tu + p.conv_dt[tap],
+                             p.conv_plane[tap] + t.m_blk / p.conv_ub);
+            if (B_MN) {
+#pragma unroll
+              for (int c = 0; c < BN / 64; ++c)
+                ptx::tma_load_4d(sb + c * (64 * BK * 2), &tmB, ring.full(), t.n_blk * BN + c * 64, p.conv_wrow[tap] + c0, 0, 0);
+            } else {
               ptx::tma_load_4d(sb, &tmB, ring.full(), c0, p.conv_wrow[tap] + t.n_blk * BN, 0, 0);
-              ring.advance();
-              continue;
             }
+            ring.advance();
+            continue;
           }
           ptx::mbar_arrive_expect_tx(ring.full(), kStageBytes);
           if (A_MN) {
@@ -307,14 +317,28 @@ tc_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
           const float b0 = ep.bias ? __ldg(ep.bias + n) : 0.f, b1 = ep.bias ? __ldg(ep.bias + n + 1) : 0.f;
           uint32_t* c32 = reinterpret_cast<uint32_t*>(p.C);
           const int64_t col = boff_c + n;
+          auto store = [&](int r, int m) {
+            const float2 v = *reinterpret_cast<const float2*>(stg + r * kLd + 2 * cp);
+            float v0 = v.x * ep.alpha, v1 = v.y * ep.alpha;
+            if (ep.bias) { v0 += b0; v1 += b1; }
+            c32[(col + (int64_t)m * p.ldc) >> 1] = pack2_16(v0, v1, p.c_dtype);
+          };
+          bool remap = false;
+          if constexpr (CONV) remap = p.conv_remap;
+          if (remap) {
+            // implicit conv2 forward: tile row rr is position (rr / F2, rr % F2) of the tile's conv_tu time rows; rows past the
+            // tile's positions or past T2 are dropped (a loop of its own: the plain loop's instruction count sets short-K GEMMs)
+            const int u0 = (t.m_blk % p.conv_ub) * p.conv_tu, b = t.m_blk / p.conv_ub;
+#pragma unroll 4
+            for (int r = tid / kPairs; r < 64; r += kRowStep) {
+              const int rr = h * 64 + r, tr = rr / p.conv_F2, t2 = u0 + tr;
+              if (tr < p.conv_tu && t2 < p.conv_T2) store(r, (b * p.conv_T2 + t2) * p.conv_F2 + (rr - tr * p.conv_F2));
+            }
+          } else {
 #pragma unroll 8
-          for (int r = tid / kPairs; r < 64; r += kRowStep) {
-            const int m = t.m_blk * BM + h * 64 + r;
-            if (m < p.M) {
-              const float2 v = *reinterpret_cast<const float2*>(stg + r * kLd + 2 * cp);
-              float v0 = v.x * ep.alpha, v1 = v.y * ep.alpha;
-              if (ep.bias) { v0 += b0; v1 += b1; }
-              c32[(col + (int64_t)m * p.ldc) >> 1] = pack2_16(v0, v1, p.c_dtype);
+            for (int r = tid / kPairs; r < 64; r += kRowStep) {
+              const int m = t.m_blk * BM + h * 64 + r;
+              if (m < p.M) store(r, m);
             }
           }
         } else if (n < p.N) {
@@ -333,6 +357,18 @@ tc_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
 }
 
 
+template <int BN, bool A_MN, bool B_MN, bool BF>
+__global__ void __launch_bounds__(kThreads, 1)
+tc_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, const TcParams p) {
+  tc_gemm_body<BN, A_MN, B_MN, BF, false>(tmA, tmB, p);
+}
+// the implicit conv2 GEMMs (conv2_fwd_implicit: MN-major weights, conv2_dgrad_implicit: K-major weights)
+template <bool B_MN, bool BF>
+__global__ void __launch_bounds__(kThreads, 1)
+tc_gemm_conv_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, const TcParams p) {
+  tc_gemm_body<128, false, B_MN, BF, true>(tmA, tmB, p);
+}
+
 // =============================================================================================================
 // Grouped weight-gradient GEMM: up to kMaxGroup products  dW_g[K_in, N_out] += X_g^T dY_g  of one backward block in ONE
 // persistent launch (TF autodiff of the Dense / einsum sites of a sublayer: neurst/layers/common_layers.py:270-288,
@@ -350,9 +386,17 @@ struct TcGroupProb {
   float alpha;
   int pad_;
 };
+// Implicit conv2 filter gradient (conv2_wgrad_implicit, one product): m = (tap, input channel), k-block kb = (utterance, chunk
+// of kt time rows x fw frequencies); A = the tap's parity-class plane shifted by the tap, B = dZ2 at the same positions, both
+// MN-major 4-D boxes.  Both deliver krows of the 64 k rows; the rest stay zero (set up at kernel start).
+struct ConvWgrad {
+  int on, kpc, kc, fc, kt, fw, krows;     // m tiles per tap, k-blocks per utterance, frequency chunks per row group
+  int dt[9], df[9], plane[9];
+};
 struct TcGroup {
   TcGroupProb prob[kMaxGroup];
   int n, num_tiles, stages;
+  ConvWgrad cw;
 };
 struct GroupTile { int gi, m_blk, n_blk, kb0, kb1; };
 __device__ __forceinline__ GroupTile group_tile(const TcGroup& g, int tile) {
@@ -395,6 +439,18 @@ __global__ void __launch_bounds__(kThreads, 1) tc_wgrad_group_kernel(const __gri
     ring.init(kConsumerWarps);
     ptx::fence_mbar_init();
   }
+  if (grp.cw.on && grp.cw.krows < BK) {
+    // k rows krows..63 of every 64 x 64 operand block are never written by the TMA unit: zero them once in every stage, in
+    // both operands (a stale value times zero can still be NaN)
+    constexpr int kBlocks = (BM + BN) / 64;
+    const int tail16 = (BK - grp.cw.krows) * 8;           // 16-byte words per block tail
+    uint8_t* ring0 = smem_raw + (ring.smem - ptx::smem_u32(smem_raw));
+    for (int i = threadIdx.x; i < grp.stages * kBlocks * tail16; i += blockDim.x) {
+      const int blk = i / tail16, w = i - blk * tail16;
+      reinterpret_cast<uint4*>(ring0 + (uint32_t)blk * (64 * BK * 2) + grp.cw.krows * 128)[w] = make_uint4(0, 0, 0, 0);
+    }
+    ptx::fence_proxy_async_smem();
+  }
   __syncthreads();
   pdl_wait();
   pdl_trigger();
@@ -410,6 +466,21 @@ __global__ void __launch_bounds__(kThreads, 1) tc_wgrad_group_kernel(const __gri
           ptx::mbar_wait(ring.empty(ring.stage), ring.phase ^ 1u);
           const uint32_t sa = ring.slot();
           const uint32_t sb = sa + kABytes;
+          if (grp.cw.on) {
+            const ConvWgrad& cw = grp.cw;
+            const int tap = t.m_blk / cw.kpc, ci0 = (t.m_blk - tap * cw.kpc) * BM;
+            const int b = kb / cw.kc, ch = kb - b * cw.kc;
+            const int t0 = (ch / cw.fc) * cw.kt, f0 = (ch % cw.fc) * cw.fw;
+            ptx::mbar_arrive_expect_tx(ring.full(), (uint32_t)((BM + BN) * cw.krows * 2));
+#pragma unroll
+            for (int c = 0; c < BM / 64; ++c)
+              ptx::tma_load_4d(sa + c * (64 * BK * 2), ma, ring.full(), ci0 + c * 64, f0 + cw.df[tap], t0 + cw.dt[tap], cw.plane[tap] + b);
+#pragma unroll
+            for (int c = 0; c < BN / 64; ++c)
+              ptx::tma_load_4d(sb + c * (64 * BK * 2), mb, ring.full(), t.n_blk * BN + c * 64, f0, t0, b);
+            ring.advance();
+            continue;
+          }
           ptx::mbar_arrive_expect_tx(ring.full(), kStageBytes);
 #pragma unroll
           for (int c = 0; c < BM / 64; ++c)
@@ -904,6 +975,23 @@ int make_out_map_f32(float* ptr, int M, int d, CUtensorMap* out) {
   return 0;
 }
 
+// [planes][T2][F2][C] 16-bit activation as a 4-D tensor (C, F2, T2, planes) with a {64, box_f, box_t, 1} box, 128B swizzle.
+// Boxes that reach outside the tensor (negative or past-the-end shifted coordinates) are zero-filled: the conv's border.
+int make_conv_map(const void* ptr, int dtype, int C, int F2, int T2, int planes, int box_f, int box_t, CUtensorMap* out) {
+  EncodeTiledFn fn = get_encode_fn();
+  B200ST_CHECK(fn != nullptr, "cuTensorMapEncodeTiled unavailable (no CUDA driver?)");
+  B200ST_CHECK((reinterpret_cast<uintptr_t>(ptr) & 15) == 0, "TMA operand base must be 16-byte aligned");
+  cuuint64_t dims[4] = {(cuuint64_t)C, (cuuint64_t)F2, (cuuint64_t)T2, (cuuint64_t)planes};
+  cuuint64_t strides[3] = {(cuuint64_t)C * 2, (cuuint64_t)F2 * C * 2, (cuuint64_t)T2 * F2 * C * 2};
+  cuuint32_t box[4] = {(cuuint32_t)BK, (cuuint32_t)box_f, (cuuint32_t)box_t, 1u};
+  cuuint32_t estr[4] = {1u, 1u, 1u, 1u};
+  CUresult r = fn(out, dtype == F16 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT16 : CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 4, const_cast<void*>(ptr),
+                  dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
+                  CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+  if (r != CUDA_SUCCESS) B200ST_FAIL("cuTensorMapEncodeTiled (conv operand) failed with CUresult " + std::to_string((int)r));
+  return 0;
+}
+
 int g_num_sms = 0;
 int g_reserved_sms = 0;
 
@@ -932,19 +1020,26 @@ namespace {
 // end is RECORDED (arguments only); tc_profile_end() then replays each recorded GEMM back to back (1 warm-up + kReps timed
 // launches bracketed by one event pair, no host gap between them) and reports the per-launch average.  The buffers of the
 // step are still alive (same workspace), accumulate / reduce epilogues only add into gradients nobody reads afterwards.
-// conv2 data gradient as an implicit GEMM (see conv2_dgrad_implicit): replaces the A tensor map and the k-block -> coordinates rule
+// Implicit conv2 GEMM (conv2_fwd_implicit, conv2_dgrad_implicit, conv2_wgrad_implicit): replaces the operand tensor maps and
+// the k-block -> coordinates rule.  x: [planes][T2][F2][C] (dY: one plane per utterance; the parity-split activation: 4 B
+// planes, class-major); dy: the wgrad's B operand dZ2 [B, T2, F2, C].
 struct ConvA {
-  const void* dy; int B, T2, F2, C;     // dY [B, T2, F2, C]
-  int tu, ub, ntaps;
-  int dt[4], df[4], wrow[4];
+  int mode;                              // kConvRows or kConvWgrad
+  const void* x; int planes, T2, F2, C;
+  const void* dy; int B;
+  int tu, ub, remap;                     // kConvRows
+  int ntaps;
+  int dt[9], df[9], wrow[9], plane[9];
 };
 struct ProfRec { GemmArgs g; cudaStream_t stream; int bn, splitk; int group_n = 0; GemmArgs rest[3]; bool has_conv = false; ConvA conv; };   // group_n > 1: grouped weight-gradient launch (g + rest)
 bool g_prof = false;
 std::vector<ProfRec> g_prof_recs;
 
-template <int BN, bool A_MN, bool B_MN, bool BF>
+template <int BN, bool A_MN, bool B_MN, bool BF, bool CONV>
 int launch_kernel(const CUtensorMap& ta, const CUtensorMap& tb, const TcParams& p, int grid, size_t smem, cudaStream_t stream) {
-  auto kern = tc_gemm_kernel<BN, A_MN, B_MN, BF>;
+  void (*kern)(const CUtensorMap, const CUtensorMap, const TcParams);
+  if constexpr (CONV) kern = tc_gemm_conv_kernel<B_MN, BF>;
+  else kern = tc_gemm_kernel<BN, A_MN, B_MN, BF>;
   static bool attr_set = false;
   if (!attr_set) {
     B200ST_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemLimit));
@@ -953,10 +1048,10 @@ int launch_kernel(const CUtensorMap& ta, const CUtensorMap& tb, const TcParams& 
   return launch(kern, grid, kThreads, smem, stream, ta, tb, p);
 }
 
-template <int BN, bool A_MN, bool B_MN>
+template <int BN, bool A_MN, bool B_MN, bool CONV = false>
 int launch_variant(bool bf, const CUtensorMap& ta, const CUtensorMap& tb, const TcParams& p, int grid, size_t smem, cudaStream_t stream) {
-  if (bf) return launch_kernel<BN, A_MN, B_MN, true>(ta, tb, p, grid, smem, stream);
-  return launch_kernel<BN, A_MN, B_MN, false>(ta, tb, p, grid, smem, stream);
+  if (bf) return launch_kernel<BN, A_MN, B_MN, true, CONV>(ta, tb, p, grid, smem, stream);
+  return launch_kernel<BN, A_MN, B_MN, false, CONV>(ta, tb, p, grid, smem, stream);
 }
 
 template <int BN>
@@ -1062,26 +1157,21 @@ int gemm_tc_impl(const GemmArgs& g, cudaStream_t stream, const ConvA* conv) {
 
   CUtensorMap ta, tb;
   if (conv) {
-    B200ST_CHECK(bn == 128 && splitk == 1 && !g.A.mn_major && !g.B.mn_major && g.nb1 == 1 && g.nb2 == 1 && conv->C % BK == 0 &&
-                     g.K == conv->ntaps * conv->C && g.M == conv->B * conv->ub * BM && conv->F2 * conv->tu <= BM && conv->ntaps <= 4,
-                 "implicit conv dgrad: unsupported shape");
-    p.conv = 1; p.conv_ub = conv->ub; p.conv_tu = conv->tu; p.conv_kpc = conv->C / BK;
-    for (int i = 0; i < conv->ntaps; ++i) { p.conv_dt[i] = conv->dt[i]; p.conv_df[i] = conv->df[i]; p.conv_wrow[i] = conv->wrow[i]; }
+    B200ST_CHECK(conv->mode == kConvRows && bn == 128 && splitk == 1 && !g.A.mn_major && g.nb1 == 1 && g.nb2 == 1 && conv->C % BK == 0 && conv->ntaps <= 9 &&
+                     g.K == conv->ntaps * conv->C && g.M == conv->B * conv->ub * BM && conv->F2 * conv->tu <= BM &&
+                     (!conv->remap || p.plain16),
+                 "implicit conv2 GEMM: unsupported shape");
+    p.conv_ub = conv->ub; p.conv_tu = conv->tu; p.conv_kpc = conv->C / BK;
+    p.conv_remap = conv->remap; p.conv_T2 = conv->T2; p.conv_F2 = conv->F2;
+    for (int i = 0; i < conv->ntaps; ++i) {
+      p.conv_dt[i] = conv->dt[i]; p.conv_df[i] = conv->df[i]; p.conv_wrow[i] = conv->wrow[i]; p.conv_plane[i] = conv->plane[i];
+    }
     p.conv_a_bytes = (uint32_t)(BK * conv->F2 * conv->tu * 2);
-    // A: dY as a 4-D tensor (C, F2, T2, B); one box = 64 channels x all F2 frequencies x tu time rows of one utterance — rows
-    // beyond the tensor (the shifted taps at the far edge) are zero-filled by the TMA unit, i.e. the convolution's border
-    EncodeTiledFn fn = get_encode_fn();
-    B200ST_CHECK(fn != nullptr, "cuTensorMapEncodeTiled unavailable (no CUDA driver?)");
-    B200ST_CHECK((reinterpret_cast<uintptr_t>(conv->dy) & 15) == 0, "TMA operand base must be 16-byte aligned");
-    cuuint64_t dims[4] = {(cuuint64_t)conv->C, (cuuint64_t)conv->F2, (cuuint64_t)conv->T2, (cuuint64_t)conv->B};
-    cuuint64_t strides[3] = {(cuuint64_t)conv->C * 2, (cuuint64_t)conv->F2 * conv->C * 2, (cuuint64_t)conv->T2 * conv->F2 * conv->C * 2};
-    cuuint32_t box[4] = {(cuuint32_t)BK, (cuuint32_t)conv->F2, (cuuint32_t)conv->tu, 1u};
-    cuuint32_t estr[4] = {1u, 1u, 1u, 1u};
-    CUresult r = fn(&ta, g.A.dtype == F16 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT16 : CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 4, const_cast<void*>(conv->dy),
-                    dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
-                    CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-    if (r != CUDA_SUCCESS) B200ST_FAIL("cuTensorMapEncodeTiled (conv dY) failed with CUresult " + std::to_string((int)r));
-    B200ST_TRY(make_operand_map(g.B, 9 * conv->C, conv->C, 1, 1, bn, &tb));      // all 9 taps of the [9C, C] weight matrix
+    // A: one box = 64 channels x all F2 frequencies x tu time rows of one plane
+    B200ST_TRY(make_conv_map(conv->x, g.A.dtype, conv->C, conv->F2, conv->T2, conv->planes, conv->F2, conv->tu, &ta));
+    // B: all 9 taps of the [9C, C] weight matrix (K-major for the data gradient, MN-major for the forward)
+    if (g.B.mn_major) B200ST_TRY(make_operand_map(g.B, conv->C, 9 * conv->C, 1, 1, bn, &tb));
+    else B200ST_TRY(make_operand_map(g.B, 9 * conv->C, conv->C, 1, 1, bn, &tb));
   } else {
     B200ST_TRY(make_operand_map(g.A, g.M, g.K, g.nb1, g.nb2, BM, &ta));
     B200ST_TRY(make_operand_map(g.B, g.N, g.K, g.nb1, g.nb2, bn, &tb));
@@ -1096,6 +1186,10 @@ int gemm_tc_impl(const GemmArgs& g, cudaStream_t stream, const ConvA* conv) {
   }
   int rc = 0;
   const bool bf = g.A.dtype == BF16;
+  if (conv) {
+    if (g.B.mn_major) return launch_variant<128, false, true, true>(bf, ta, tb, p, grid, smem, stream);
+    return launch_variant<128, false, false, true>(bf, ta, tb, p, grid, smem, stream);
+  }
   switch (bn) {
     case 64: rc = launch_bn<64>(g.A.mn_major, g.B.mn_major, bf, ta, tb, p, grid, smem, stream); break;
     case 128: rc = launch_bn<128>(g.A.mn_major, g.B.mn_major, bf, ta, tb, p, grid, smem, stream); break;
@@ -1105,18 +1199,72 @@ int gemm_tc_impl(const GemmArgs& g, cudaStream_t stream, const ConvA* conv) {
 }
 }  // namespace
 
-// Data gradient of the 3x3 / stride-2 / pad-1 convolution (Conv2D#2 of AudioConv2dSubsamplingLayer,
-// neurst/layers/modalities/audio_modalities.py:96-104) as four implicit GEMMs, one per parity class (t1 & 1, f1 & 1) of the
-// input position: dA[b, t1, f1, :] = sum over the taps (kh, kw) with t1 = 2 t2 + kh - 1, f1 = 2 f2 + kw - 1 of
-// dY[b, t2, f2, :] W[kh, kw]^T — 1 tap for (even, even), 2 for the mixed classes, 4 for (odd, odd).  The A operand is read
-// straight out of dY by 4-D TMA boxes shifted by the tap (zero fill = border), so neither the [rows, 9C] column gradient
-// (737 MB at cfg-2) nor its col2im gather exist.  Output: class-major padded tiles
+// Conv2D#2 of AudioConv2dSubsamplingLayer (neurst/layers/modalities/audio_modalities.py:96-104): 3x3, stride 2, pad 1, as
+// implicit GEMMs.  Tap (kh, kw) of output position (t2, f2) reads input position (2 t2 + kh - 1, 2 f2 + kw - 1); stored split
+// by parity class cls = ((t1 & 1) << 1) | (f1 & 1) at plane position (t1 >> 1, f1 >> 1), that is plane position
+// (t2 + dt, f2 + df) of class plane cls with dt = -1 for kh = 0 and 0 otherwise (df alike) — dense unit-stride boxes
+// shifted per tap.  conv1's forward writes the activation in that layout (conv_kernels.cu), zero at the class positions
+// past the image.
+static void conv2_fwd_taps(ConvA& ca, int B, int C) {
+  ca.ntaps = 9;
+  for (int kh = 0; kh < 3; ++kh)
+    for (int kw = 0; kw < 3; ++kw) {
+      const int tap = kh * 3 + kw, cls = ((kh != 1) << 1) | (kw != 1);
+      ca.dt[tap] = kh == 0 ? -1 : 0; ca.df[tap] = kw == 0 ? -1 : 0;
+      ca.wrow[tap] = tap * C; ca.plane[tap] = cls * B;
+    }
+}
+
+// z2[b, t2, f2, :] = bias + sum over taps of a1_tap W[tap]: a 128-row tile = tu = 128 / F2 time rows of one utterance, k-blocks
+// in the (kh, kw, channel) order of the explicit column matrix, so every output element sums the same products in the same
+// order as the explicit GEMM did.
+int conv2_fwd_implicit(const void* a1, const void* w16, const float* bias, void* z2, int dtype, int B, int T2, int F2, int C,
+                       cudaStream_t stream) {
+  B200ST_CHECK(is16(dtype) && C == 256 && F2 >= 1 && F2 <= BM, "implicit conv2 forward: 16-bit, C == 256, F2 <= 128");
+  ConvA ca{};
+  ca.mode = kConvRows; ca.x = a1; ca.planes = 4 * B; ca.T2 = T2; ca.F2 = F2; ca.C = C; ca.B = B;
+  ca.tu = BM / F2; ca.ub = ceil_div(T2, ca.tu); ca.remap = 1;
+  conv2_fwd_taps(ca, B, C);
+  GemmArgs g = gemm_defaults();
+  g.M = B * ca.ub * BM; g.N = C; g.K = 9 * C;
+  g.A = GemmOperand{a1, dtype, 0, C, 0, 0};
+  g.B = GemmOperand{w16, dtype, 1, C, 0, 0};
+  g.C = z2; g.c_dtype = dtype; g.ldc = C;
+  g.epi.bias = bias;
+  return gemm_tc_impl(g, stream, &ca);
+}
+
+// dW[(kh, kw, ci), co] += sum over positions p of a1_tap(p)[ci] dZ2[p][co]: both operands MN-major, a k-block = a chunk of whole
+// time rows x F2 frequencies of one utterance (F2 <= 64: 64 / F2 rows; 64 < F2 <= 128: one row in two halves of 64).
+// Split-K with fp32 atomics; all work units run in one wave and walk their k ranges in step, so the 18 m tiles (9 taps x 2
+// channel halves) of a k range read the four class planes of the same positions at about the same time, from L2.
+namespace { int conv_wgrad_launch(const GemmArgs& g, const ConvA& ca, cudaStream_t stream); }
+int conv2_wgrad_implicit(const void* a1, const void* dz2, float* dw, int dtype, int B, int T2, int F2, int C, cudaStream_t stream) {
+  B200ST_CHECK(is16(dtype) && C == 256 && F2 >= 1 && F2 <= BM, "implicit conv2 filter gradient: 16-bit, C == 256, F2 <= 128");
+  ConvA ca{};
+  ca.mode = kConvWgrad; ca.x = a1; ca.planes = 4 * B; ca.T2 = T2; ca.F2 = F2; ca.C = C; ca.dy = dz2; ca.B = B;
+  conv2_fwd_taps(ca, B, C);
+  const int kt = F2 < BK ? BK / F2 : 1, fc = F2 <= BK ? 1 : 2;
+  GemmArgs g = gemm_defaults();
+  g.M = 9 * C; g.N = C; g.K = B * ceil_div(T2, kt) * fc * BK;
+  g.A = GemmOperand{a1, dtype, 1, 9 * C, 0, 0};
+  g.B = GemmOperand{dz2, dtype, 1, C, 0, 0};
+  g.C = dw; g.c_dtype = F32; g.ldc = C;
+  g.epi.accumulate = 1;
+  return conv_wgrad_launch(g, ca, stream);
+}
+
+// Data gradient of the same convolution as four implicit GEMMs, one per parity class (t1 & 1, f1 & 1) of the input position:
+// dA[b, t1, f1, :] = sum over the taps (kh, kw) with t1 = 2 t2 + kh - 1, f1 = 2 f2 + kw - 1 of dY[b, t2, f2, :] W[kh, kw]^T —
+// 1 tap for (even, even), 2 for the mixed classes, 4 for (odd, odd).  The A operand is read straight out of dY by 4-D TMA
+// boxes shifted by the tap (zero fill = border), so neither the [rows, 9C] column gradient (737 MB at cfg-2) nor its col2im
+// gather exist.  Output: class-major padded tiles
 //   dA[cls][b][tile][128 rows = tu x F2 positions (+ unused rows)][C],   tile = (t1 >> 1) / tu,   row = ((t1 >> 1) % tu) * F2 + (f1 >> 1)
 // which conv1's backward kernel reads back with the same arithmetic.
 int conv2_dgrad_implicit(const void* dy, const void* w16, void* da, int dtype, int B, int T2, int F2, int C, cudaStream_t stream) {
   B200ST_CHECK(is16(dtype) && C == 256 && F2 >= 1 && F2 <= BM, "implicit conv2 dgrad: 16-bit, C == 256, F2 <= 128");
   ConvA ca{};
-  ca.dy = dy; ca.B = B; ca.T2 = T2; ca.F2 = F2; ca.C = C;
+  ca.mode = kConvRows; ca.x = dy; ca.planes = B; ca.B = B; ca.T2 = T2; ca.F2 = F2; ca.C = C;
   ca.tu = BM / F2;
   ca.ub = ceil_div(T2, ca.tu);
   const int64_t cls_elems = (int64_t)B * ca.ub * BM * C;
@@ -1130,7 +1278,7 @@ int conv2_dgrad_implicit(const void* dy, const void* w16, void* da, int dtype, i
     for (int a = 0; a < nt; ++a)
       for (int b2 = 0; b2 < nf; ++b2) {
         const int i = a * nf + b2;
-        ca.dt[i] = dt_of[a]; ca.df[i] = df_of[b2]; ca.wrow[i] = (kh_of[a] * 3 + kw_of[b2]) * C;
+        ca.dt[i] = dt_of[a]; ca.df[i] = df_of[b2]; ca.wrow[i] = (kh_of[a] * 3 + kw_of[b2]) * C; ca.plane[i] = 0;
       }
     GemmArgs g = gemm_defaults();
     g.M = B * ca.ub * BM; g.N = C; g.K = ca.ntaps * C;
@@ -1150,6 +1298,46 @@ int64_t conv2_dgrad_implicit_elems(int B, int T2, int F2, int C) {
 // One launch for the weight gradients of a backward block (see tc_wgrad_group_kernel).  Every product must be a plain
 // fp32-accumulate MN-major x MN-major 16-bit GEMM with M % 128 == 0 and N % 256 == 0; returns 2 (nothing launched) when the
 // group does not qualify, so that the caller issues the products one by one.
+// Splits the products of `grp` (tensor maps, C, ldc and alpha set; m_tiles, n_tiles and kb_total given) into work units of
+// one common k-range length and launches them as one wave.
+static int launch_wgrad_group(TcGroup& grp, bool bf, cudaStream_t stream) {
+  int num_sms = 0;
+  B200ST_TRY(usable_sms(&num_sms));
+  int64_t work = 0;
+  for (int i = 0; i < grp.n; ++i) work += (int64_t)grp.prob[i].m_tiles * grp.prob[i].n_tiles * grp.prob[i].kb_total;
+  // smallest common k-range L (in 64-row blocks) whose work units fit one wave of `num_sms` CTAs
+  int L = (int)((work + num_sms - 1) / num_sms);
+  if (L < 2) L = 2;
+  for (;; ++L) {
+    int64_t units = 0;
+    for (int i = 0; i < grp.n; ++i) units += (int64_t)grp.prob[i].m_tiles * grp.prob[i].n_tiles * ceil_div(grp.prob[i].kb_total, L);
+    if (units <= num_sms || L >= 4096) break;
+  }
+  int tile = 0;
+  for (int i = 0; i < grp.n; ++i) {
+    TcGroupProb& q = grp.prob[i];
+    q.kb_per_split = L < q.kb_total ? L : q.kb_total;
+    q.splitk = ceil_div(q.kb_total, q.kb_per_split);
+    q.tile_begin = tile;
+    tile += q.m_tiles * q.n_tiles * q.splitk;
+  }
+  grp.num_tiles = tile;
+  const uint32_t stage_bytes = kABytes + 256u * BK * 2;
+  int stages = (int)((kSmemLimit - 2048) / stage_bytes);
+  if (stages > 8) stages = 8;
+  grp.stages = stages;
+  const size_t smem = 1024 + (size_t)stages * stage_bytes + 16 * stages + 16;
+  B200ST_CHECK(smem <= (size_t)kSmemLimit, "smem budget exceeded");
+  auto kern = bf ? tc_wgrad_group_kernel<true> : tc_wgrad_group_kernel<false>;
+  static bool attr_set[2] = {false, false};
+  if (!attr_set[bf]) {
+    B200ST_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemLimit));
+    attr_set[bf] = true;
+  }
+  const int grid = grp.num_tiles < num_sms ? grp.num_tiles : num_sms;
+  return launch(kern, grid, kThreads, smem, stream, grp);
+}
+
 int gemm_wgrad_group(const GemmArgs* gs, int n, cudaStream_t stream) {
   if (n < 2 || n > kMaxGroup) return 2;
   for (int i = 0; i < n; ++i) {
@@ -1160,62 +1348,61 @@ int gemm_wgrad_group(const GemmArgs* gs, int n, cudaStream_t stream) {
           (reinterpret_cast<uintptr_t>(g.C) & 7) == 0 && g.ldc % 2 == 0))
       return 2;
   }
-  int num_sms = 0;
-  B200ST_TRY(usable_sms(&num_sms));
   TcGroup grp;
   std::memset(&grp, 0, sizeof(grp));
   grp.n = n;
-  int64_t work = 0;
-  int tiles0[kMaxGroup], kbt[kMaxGroup];
-  for (int i = 0; i < n; ++i) {
-    tiles0[i] = (gs[i].M / BM) * (gs[i].N / 256);
-    kbt[i] = ceil_div(gs[i].K, BK);
-    work += (int64_t)tiles0[i] * kbt[i];
-  }
-  // smallest common k-range L (in 64-row blocks) whose work units fit one wave of `num_sms` CTAs
-  int L = (int)((work + num_sms - 1) / num_sms);
-  if (L < 2) L = 2;
-  for (;; ++L) {
-    int64_t units = 0;
-    for (int i = 0; i < n; ++i) units += (int64_t)tiles0[i] * ceil_div(kbt[i], L);
-    if (units <= num_sms || L >= 4096) break;
-  }
-  int tile = 0;
   for (int i = 0; i < n; ++i) {
     const GemmArgs& g = gs[i];
     TcGroupProb& q = grp.prob[i];
-    q.m_tiles = g.M / BM; q.n_tiles = g.N / 256; q.kb_total = kbt[i];
-    q.kb_per_split = L < kbt[i] ? L : kbt[i];
-    q.splitk = ceil_div(kbt[i], q.kb_per_split);
-    q.tile_begin = tile;
+    q.m_tiles = g.M / BM; q.n_tiles = g.N / 256; q.kb_total = ceil_div(g.K, BK);
     q.alpha = g.epi.alpha;
-    tile += q.m_tiles * q.n_tiles * q.splitk;
     B200ST_TRY(make_operand_map(g.A, g.M, g.K, 1, 1, BM, &q.ta));
     B200ST_TRY(make_operand_map(g.B, g.N, g.K, 1, 1, 256, &q.tb));
     q.C = reinterpret_cast<float*>(g.C); q.ldc = g.ldc;
   }
-  grp.num_tiles = tile;
-  const uint32_t stage_bytes = kABytes + 256u * BK * 2;
-  int stages = (int)((kSmemLimit - 2048) / stage_bytes);
-  if (stages > 8) stages = 8;
-  grp.stages = stages;
-  const size_t smem = 1024 + (size_t)stages * stage_bytes + 16 * stages + 16;
-  B200ST_CHECK(smem <= (size_t)kSmemLimit, "smem budget exceeded");
-  auto kern = gs[0].A.dtype == BF16 ? tc_wgrad_group_kernel<true> : tc_wgrad_group_kernel<false>;
-  static bool attr_set[2] = {false, false};
-  if (!attr_set[gs[0].A.dtype == BF16]) {
-    B200ST_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemLimit));
-    attr_set[gs[0].A.dtype == BF16] = true;
-  }
-  const int grid = grp.num_tiles < num_sms ? grp.num_tiles : num_sms;
+  B200ST_TRY(launch_wgrad_group(grp, gs[0].A.dtype == BF16, stream));
   if (g_prof) {
     ProfRec r{gs[0], stream, 256, grp.prob[0].splitk};
     r.group_n = n;
     for (int i = 1; i < n; ++i) r.rest[i - 1] = gs[i];
     g_prof_recs.push_back(r);
   }
-  return launch(kern, grid, kThreads, smem, stream, grp);
+  return 0;
 }
+
+namespace {
+// dW[(kh, kw, ci), co] += sum over positions of a1_tap[ci] dZ2[co] as one tc_wgrad_group_kernel product (128 x 256 tiles: each
+// k-block of the two operands feeds twice the MMA work of a 128 x 128 tile, which sets this GEMM's time: it is bound by
+// operand traffic from L2, not by HBM)
+int conv_wgrad_launch(const GemmArgs& g, const ConvA& ca, cudaStream_t stream) {
+  B200ST_CHECK(ca.mode == kConvWgrad && is16(g.A.dtype) && g.A.dtype == g.B.dtype && ca.C % BM == 0 && ca.ntaps == 9 &&
+                   g.M == 9 * ca.C && g.N == ca.C && ca.C % 256 == 0 && ca.F2 >= 1 && ca.F2 <= 2 * BK && g.c_dtype == F32 &&
+                   (reinterpret_cast<uintptr_t>(g.C) & 7) == 0 && g.ldc % 2 == 0,
+               "implicit conv2 filter gradient: unsupported shape");
+  const int fw = ca.F2 < BK ? ca.F2 : BK, kt = ca.F2 < BK ? BK / ca.F2 : 1;
+  TcGroup grp;
+  std::memset(&grp, 0, sizeof(grp));
+  grp.n = 1;
+  ConvWgrad& cw = grp.cw;
+  cw.on = 1; cw.kpc = ca.C / BM; cw.fw = fw; cw.kt = kt; cw.fc = ceil_div(ca.F2, fw); cw.krows = fw * kt;
+  cw.kc = ceil_div(ca.T2, kt) * cw.fc;
+  for (int i = 0; i < 9; ++i) { cw.dt[i] = ca.dt[i]; cw.df[i] = ca.df[i]; cw.plane[i] = ca.plane[i]; }
+  TcGroupProb& q = grp.prob[0];
+  q.m_tiles = g.M / BM; q.n_tiles = g.N / 256; q.kb_total = ca.B * cw.kc;
+  B200ST_CHECK(ceil_div(g.K, BK) == q.kb_total, "implicit conv2 filter gradient: k-blocks do not match the chunking");
+  q.alpha = g.epi.alpha;
+  q.C = reinterpret_cast<float*>(g.C); q.ldc = g.ldc;
+  B200ST_TRY(make_conv_map(ca.x, g.A.dtype, ca.C, ca.F2, ca.T2, ca.planes, fw, kt, &q.ta));
+  B200ST_TRY(make_conv_map(ca.dy, g.B.dtype, ca.C, ca.F2, ca.T2, ca.B, fw, kt, &q.tb));
+  B200ST_TRY(launch_wgrad_group(grp, g.A.dtype == BF16, stream));
+  if (g_prof) {
+    ProfRec r{g, stream, 256, q.splitk};
+    r.has_conv = true; r.conv = ca;
+    g_prof_recs.push_back(r);
+  }
+  return 0;
+}
+}  // namespace
 
 
 // Fused FFN forward (see fused_mlp_fwd_kernel).  X: 16-bit [M, d] (LayerNorm output); W1 [d, ffn], W2 [ffn, d] in the same
@@ -1322,7 +1509,7 @@ int tc_profile_end(double* ms, double* flops, int64_t* launches) {
     grp_args[0] = r.g;
     for (int i = 1; i < r.group_n; ++i) grp_args[i] = r.rest[i - 1];
     auto run = [&]() -> int {
-      if (r.has_conv) return gemm_tc_impl(r.g, st, &r.conv);
+      if (r.has_conv) return r.conv.mode == kConvWgrad ? conv_wgrad_launch(r.g, r.conv, st) : gemm_tc_impl(r.g, st, &r.conv);
       return r.group_n > 1 ? gemm_wgrad_group(grp_args, r.group_n, st) : gemm_tc_bf16(r.g, st);
     };
     B200ST_TRY(run());                                          // warm-up (tensor maps, instruction cache)
