@@ -76,9 +76,16 @@ __device__ __forceinline__ void tma_reduce_add_2d(const void* tmap, uint32_t src
   asm volatile("cp.reduce.async.bulk.tensor.2d.global.shared::cta.add.tile.bulk_group [%0, {%2, %3}], [%1];"
                ::"l"(tmap), "r"(src_smem), "r"(c0), "r"(c1) : "memory");
 }
+// global[box at (c0, c1)] = smem box (elements outside the tensor are not written)
+__device__ __forceinline__ void tma_store_2d(const void* tmap, uint32_t src_smem, int c0, int c1) {
+  asm volatile("cp.async.bulk.tensor.2d.global.shared::cta.bulk_group [%0, {%2, %3}], [%1];"
+               ::"l"(tmap), "r"(src_smem), "r"(c0), "r"(c1) : "memory");
+}
 __device__ __forceinline__ void bulk_commit() { asm volatile("cp.async.bulk.commit_group;" ::: "memory"); }
 // all committed bulk operations of this thread have completed (their global writes performed)
 __device__ __forceinline__ void bulk_wait_all() { asm volatile("cp.async.bulk.wait_group 0;" ::: "memory"); }
+// all committed bulk operations of this thread have finished reading their shared-memory source (it may be overwritten)
+__device__ __forceinline__ void bulk_wait_read_all() { asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory"); }
 
 // ---- named barriers (ids 1..15; 0 is __syncthreads) -------------------------------------------
 // `threads` counts every thread of both sides (a multiple of 32): sync blocks until it is reached, arrive does not block.

@@ -58,6 +58,7 @@ struct TcParams {
   int atomic;           // C += through fp32 atomics (split-K or accumulate)
   int vec2;             // C may be written two columns at a time (even N, ld and batch strides; 8-byte aligned base)
   int plain16;          // 16-bit C, plain stores, epilogue = alpha (+ bias) only: the short epilogue loop applies
+  int c_reduce;         // tc_gemm_f32_kernel: bulk reduce-adds (split-K / accumulate) instead of bulk stores
   // Implicit convolution A operand (tc_gemm_kernel<..., CONV = true>; conv2 of the speech front-end, see ConvA): A tile = conv_tu time rows x F2 positions of
   // one plane x 64 channels, read as a 4-D box (channels, F2, time rows, plane) shifted by the tap — coordinates outside the
   // tensor are zero-filled by the TMA unit, which is the convolution's pad-1 border; k-block kb = (tap, 64-channel chunk).
@@ -105,6 +106,38 @@ struct Ring {
     for (int s = 0; s < stages; ++s) { ptx::mbar_init(bars + 8u * s, 1); ptx::mbar_init(empty(s), releasers); }
   }
 };
+
+// fp32 output rows of one consumer warpgroup on their way to global memory through a 128B-swizzled fp32 tensor map
+// (make_out_map_f32): [64 rows x 32 columns] boxes, box b (columns 32 b ..) at base + 8 KB * b, rows 128 B apart, the
+// 16-byte chunks XOR-swizzled by row % 8 as the map's 128B swizzle expects (a warp's fragment stores hit all 32 banks).
+// base must be 1024-byte aligned.  Stores the warpgroup's [64 x N] wgmma accumulator fragment (layout: ptx.cuh) times alpha.
+template <int N>
+__device__ __forceinline__ void stage_rows_sw128(uint32_t base, const float (&acc)[N / 2], float alpha, int warp, int lane) {
+  const int g = lane >> 2, q = lane & 3;
+  // this thread's rows (warp & 3) * 16 + g + 8 hr of the warpgroup's 64: row % 8 = g
+  const uint32_t row = base + (uint32_t)((warp & 3) * 16 + g) * 128u + (uint32_t)(q & 1) * 8u;
+#pragma unroll
+  for (int j = 0; j < N / 8; ++j) {
+#pragma unroll
+    for (int hr = 0; hr < 2; ++hr) {
+      const uint32_t chunk = (uint32_t)(((j & 3) * 2 + (q >> 1)) ^ g);
+      const uint32_t dst = row + (uint32_t)(j >> 2) * 8192u + (uint32_t)hr * 1024u + chunk * 16u;
+      asm volatile("st.shared.v2.f32 [%0], {%1, %2};" ::"r"(dst), "f"(acc[4 * j + 2 * hr] * alpha), "f"(acc[4 * j + 2 * hr + 1] * alpha)
+                   : "memory");
+    }
+  }
+}
+// One thread, after the warpgroup's stage_rows_sw128 stores, fence_proxy_async_smem and a warpgroup barrier:
+// C[row0 .., col0 .. col0 + N) += the staged rows as N / 32 bulk reduce-adds (fp32 adds performed at L2, element-wise atomic
+// with respect to other writers; rows and columns outside the map are skipped).  Returns once they are performed, so the
+// staging may be reused and the sums are visible to whatever runs after the kernel.
+template <int N>
+__device__ __forceinline__ void reduce_add_rows_sw128(const CUtensorMap* tm, uint32_t base, int col0, int row0) {
+#pragma unroll
+  for (int b = 0; b < N / 32; ++b) ptx::tma_reduce_add_2d(tm, base + (uint32_t)b * 8192u, col0 + b * 32, row0);
+  ptx::bulk_commit();
+  ptx::bulk_wait_all();
+}
 
 // Consumer warpgroup `wg`: acc[64 x BN] = sum over the next nkb ring slots of A_slot[64 wg .. 64 wg + 64, :] B_slot^T.
 // The wgmma group of slot i stays in flight while slot i + 1 is issued; a slot is released once its group has retired.
@@ -194,8 +227,10 @@ __device__ __forceinline__ void consume_tile(float (&acc)[2][BN / 2], Ring& r, i
 
 // CONV: implicit conv2 A operand (TcParams conv fields; K-major A only), compiled into an entry point of its own
 // (tc_gemm_conv_kernel) so that the plain GEMMs carry none of its code.
-template <int BN, bool A_MN, bool B_MN, bool BF, bool CONV>
-__device__ __forceinline__ void tc_gemm_body(const CUtensorMap& tmA, const CUtensorMap& tmB, const TcParams& p) {
+// F32C: fp32 C written through the tensor map tmC (bulk stores, or reduce-adds when p.c_reduce), epilogue alpha (+ bias);
+// an entry point of its own (tc_gemm_f32_kernel): next to the general loop, its code spilled the BN = 128 accumulators.
+template <int BN, bool A_MN, bool B_MN, bool BF, bool CONV, bool F32C = false>
+__device__ __forceinline__ void tc_gemm_body(const CUtensorMap& tmA, const CUtensorMap& tmB, const CUtensorMap& tmC, const TcParams& p) {
   static_assert(BN <= 128, "a consumer warpgroup holds the whole 128 x BN accumulator");
   static_assert(!CONV || !A_MN, "the implicit conv A operand is K-major");
   extern __shared__ uint8_t smem_raw[];
@@ -216,6 +251,7 @@ __device__ __forceinline__ void tc_gemm_body(const CUtensorMap& tmA, const CUten
   if (warp == 0 && lane == 0) {
     ptx::prefetch_tensormap(&tmA);
     ptx::prefetch_tensormap(&tmB);
+    if constexpr (F32C) ptx::prefetch_tensormap(&tmC);
     ring.init(4);         // a slot is read by the 4 warps of the warpgroup that owns its tile
     ptx::fence_mbar_init();
   }
@@ -302,6 +338,46 @@ __device__ __forceinline__ void tc_gemm_body(const CUtensorMap& tmA, const CUten
       const int cp = tid % kPairs, n = t.n_blk * BN + 2 * cp;
 #pragma unroll
       for (int h = 0; h < 2; ++h) {
+        if constexpr (F32C) {
+          // the half's raw accumulators go to the staging buffer as swizzled [64 x 32] boxes; alpha (+ bias) is applied
+          // there as gemm_epilogue_value computes it, and one thread issues a bulk store or reduce-add per box that starts
+          // inside C (the map clips rows past M and columns past N).  The buffer is refilled only after that thread has
+          // seen the previous half's bulk operations finish reading it.
+          const uint32_t sbuf = staging + (uint32_t)wg * staging_bytes(BN);
+          if (tid == 0) ptx::bulk_wait_read_all();
+          ptx::named_bar_sync(kEpiBar + wg, 128);
+          stage_rows_sw128<BN>(sbuf, acc[h], 1.f, warp, lane);
+          if (ep.alpha != 1.f || ep.bias) {
+            ptx::named_bar_sync(kEpiBar + wg, 128);
+            const int c = 2 * cp;                            // a column pair per thread, its bias pair loaded once per tile
+            const float b0 = ep.bias && n < p.N ? __ldg(ep.bias + n) : 0.f, b1 = ep.bias && n + 1 < p.N ? __ldg(ep.bias + n + 1) : 0.f;
+            const uint32_t col = sbuf + (uint32_t)(c >> 5) * 8192u + (uint32_t)(c & 3) * 4u;
+#pragma unroll 4
+            for (int r = tid / kPairs; r < 64; r += kRowStep) {
+              const uint32_t a = col + (uint32_t)r * 128u + ((uint32_t)(((c & 31) >> 2) ^ (r & 7)) << 4);
+              float v0, v1;
+              asm volatile("ld.shared.v2.f32 {%0, %1}, [%2];" : "=f"(v0), "=f"(v1) : "r"(a) : "memory");
+              v0 = v0 * ep.alpha;
+              v1 = v1 * ep.alpha;
+              if (ep.bias) { v0 += b0; v1 += b1; }
+              asm volatile("st.shared.v2.f32 [%0], {%1, %2};" ::"r"(a), "f"(v0), "f"(v1) : "memory");
+            }
+          }
+          ptx::fence_proxy_async_smem();               // the generic-proxy stores, visible to the bulk operations
+          ptx::named_bar_sync(kEpiBar + wg, 128);
+          const int r0 = t.m_blk * BM + h * 64;
+          if (tid == 0 && r0 < p.M) {
+#pragma unroll
+            for (int b = 0; b < BN / 32; ++b) {
+              const int c0 = t.n_blk * BN + b * 32;
+              if (c0 >= p.N) break;
+              if (p.c_reduce) ptx::tma_reduce_add_2d(&tmC, sbuf + (uint32_t)b * 8192u, c0, r0);
+              else ptx::tma_store_2d(&tmC, sbuf + (uint32_t)b * 8192u, c0, r0);
+            }
+            ptx::bulk_commit();
+          }
+          continue;
+        }
         ptx::named_bar_sync(kEpiBar + wg, 128);          // the previous half's reads are done
 #pragma unroll
         for (int jj = 0; jj < BN / 8; ++jj) {
@@ -353,6 +429,9 @@ __device__ __forceinline__ void tc_gemm_body(const CUtensorMap& tmA, const CUten
         }
       }
     }
+    if constexpr (F32C) {
+      if (tid == 0) ptx::bulk_wait_all();      // the staging stays allocated until the last bulk operations are done
+    }
   }
 }
 
@@ -360,13 +439,20 @@ __device__ __forceinline__ void tc_gemm_body(const CUtensorMap& tmA, const CUten
 template <int BN, bool A_MN, bool B_MN, bool BF>
 __global__ void __launch_bounds__(kThreads, 1)
 tc_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, const TcParams p) {
-  tc_gemm_body<BN, A_MN, B_MN, BF, false>(tmA, tmB, p);
+  tc_gemm_body<BN, A_MN, B_MN, BF, false>(tmA, tmB, tmA, p);
+}
+// non-batched GEMMs with fp32 C that fits a tensor map and an alpha (+ bias) epilogue (gemm_tc_impl: TcParams::c_reduce)
+template <int BN, bool A_MN, bool B_MN, bool BF>
+__global__ void __launch_bounds__(kThreads, 1)
+tc_gemm_f32_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
+                   const __grid_constant__ CUtensorMap tmC, const TcParams p) {
+  tc_gemm_body<BN, A_MN, B_MN, BF, false, true>(tmA, tmB, tmC, p);
 }
 // the implicit conv2 GEMMs (conv2_fwd_implicit: MN-major weights, conv2_dgrad_implicit: K-major weights)
 template <bool B_MN, bool BF>
 __global__ void __launch_bounds__(kThreads, 1)
 tc_gemm_conv_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, const TcParams p) {
-  tc_gemm_body<128, false, B_MN, BF, true>(tmA, tmB, p);
+  tc_gemm_body<128, false, B_MN, BF, true>(tmA, tmB, tmA, p);
 }
 
 // =============================================================================================================
@@ -375,16 +461,16 @@ tc_gemm_conv_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_consta
 // multi_head_attention.py:145-215).  Each product alone has 2..16 output tiles and needs split-K over the B*T rows to fill
 // the SMs, i.e. every CTA reduce-adds a full 128 x 256 fp32 tile for a handful of k-blocks of MMA work and every launch pays
 // its fixed cost; together the products of a block give one wave of work units with k-ranges several times longer.
-// Same pipeline as tc_gemm_kernel<256, true, true>; a work unit = (product, m tile, n tile, k split).
+// Same pipeline as tc_gemm_kernel<256, true, true>; a work unit = (product, m tile, n tile, k split), exactly one per CTA
+// (launch_wgrad_group).  Every CTA of the wave finishes at about the same time, so the units' fp32 tiles leave as bulk
+// reduce-adds staged in the drained operand ring, not as per-thread atomics (see the fused FFN kernel's tail).
 // =============================================================================================================
 constexpr int kMaxGroup = 4;
 struct TcGroupProb {
   CUtensorMap ta, tb;
-  float* C;
-  int64_t ldc;
+  CUtensorMap tc;           // fp32 C (make_out_map_f32), the bulk reduce-add target
   int m_tiles, n_tiles, splitk, kb_total, kb_per_split, tile_begin;
   float alpha;
-  int pad_;
 };
 // Implicit conv2 filter gradient (conv2_wgrad_implicit, one product): m = (tap, input channel), k-block kb = (utterance, chunk
 // of kt time rows x fw frequencies); A = the tap's parity-class plane shifted by the tap, B = dZ2 at the same positions, both
@@ -435,6 +521,7 @@ __global__ void __launch_bounds__(kThreads, 1) tc_wgrad_group_kernel(const __gri
     for (int i = 0; i < grp.n; ++i) {
       ptx::prefetch_tensormap(&grp.prob[i].ta);
       ptx::prefetch_tensormap(&grp.prob[i].tb);
+      ptx::prefetch_tensormap(&grp.prob[i].tc);
     }
     ring.init(kConsumerWarps);
     ptx::fence_mbar_init();
@@ -455,62 +542,57 @@ __global__ void __launch_bounds__(kThreads, 1) tc_wgrad_group_kernel(const __gri
   pdl_wait();
   pdl_trigger();
 
+  const GroupTile t = group_tile(grp, blockIdx.x);         // the CTA's one work unit (gridDim.x == grp.num_tiles)
   if (warp < 4) {
     ptx::reg_dealloc<kProducerRegs>();
     if (warp == 0 && lane == 0) {
-      for (int tile = blockIdx.x; tile < grp.num_tiles; tile += gridDim.x) {
-        const GroupTile t = group_tile(grp, tile);
-        const CUtensorMap* ma = &grp.prob[t.gi].ta;
-        const CUtensorMap* mb = &grp.prob[t.gi].tb;
-        for (int kb = t.kb0; kb < t.kb1; ++kb) {
-          ptx::mbar_wait(ring.empty(ring.stage), ring.phase ^ 1u);
-          const uint32_t sa = ring.slot();
-          const uint32_t sb = sa + kABytes;
-          if (grp.cw.on) {
-            const ConvWgrad& cw = grp.cw;
-            const int tap = t.m_blk / cw.kpc, ci0 = (t.m_blk - tap * cw.kpc) * BM;
-            const int b = kb / cw.kc, ch = kb - b * cw.kc;
-            const int t0 = (ch / cw.fc) * cw.kt, f0 = (ch % cw.fc) * cw.fw;
-            ptx::mbar_arrive_expect_tx(ring.full(), (uint32_t)((BM + BN) * cw.krows * 2));
-#pragma unroll
-            for (int c = 0; c < BM / 64; ++c)
-              ptx::tma_load_4d(sa + c * (64 * BK * 2), ma, ring.full(), ci0 + c * 64, f0 + cw.df[tap], t0 + cw.dt[tap], cw.plane[tap] + b);
-#pragma unroll
-            for (int c = 0; c < BN / 64; ++c)
-              ptx::tma_load_4d(sb + c * (64 * BK * 2), mb, ring.full(), t.n_blk * BN + c * 64, f0, t0, b);
-            ring.advance();
-            continue;
-          }
-          ptx::mbar_arrive_expect_tx(ring.full(), kStageBytes);
+      const CUtensorMap* ma = &grp.prob[t.gi].ta;
+      const CUtensorMap* mb = &grp.prob[t.gi].tb;
+      for (int kb = t.kb0; kb < t.kb1; ++kb) {
+        ptx::mbar_wait(ring.empty(ring.stage), ring.phase ^ 1u);
+        const uint32_t sa = ring.slot();
+        const uint32_t sb = sa + kABytes;
+        if (grp.cw.on) {
+          const ConvWgrad& cw = grp.cw;
+          const int tap = t.m_blk / cw.kpc, ci0 = (t.m_blk - tap * cw.kpc) * BM;
+          const int b = kb / cw.kc, ch = kb - b * cw.kc;
+          const int t0 = (ch / cw.fc) * cw.kt, f0 = (ch % cw.fc) * cw.fw;
+          ptx::mbar_arrive_expect_tx(ring.full(), (uint32_t)((BM + BN) * cw.krows * 2));
 #pragma unroll
           for (int c = 0; c < BM / 64; ++c)
-            ptx::tma_load_4d(sa + c * (64 * BK * 2), ma, ring.full(), t.m_blk * BM + c * 64, kb * BK, 0, 0);
+            ptx::tma_load_4d(sa + c * (64 * BK * 2), ma, ring.full(), ci0 + c * 64, f0 + cw.df[tap], t0 + cw.dt[tap], cw.plane[tap] + b);
 #pragma unroll
           for (int c = 0; c < BN / 64; ++c)
-            ptx::tma_load_4d(sb + c * (64 * BK * 2), mb, ring.full(), t.n_blk * BN + c * 64, kb * BK, 0, 0);
+            ptx::tma_load_4d(sb + c * (64 * BK * 2), mb, ring.full(), t.n_blk * BN + c * 64, f0, t0, b);
           ring.advance();
+          continue;
         }
+        ptx::mbar_arrive_expect_tx(ring.full(), kStageBytes);
+#pragma unroll
+        for (int c = 0; c < BM / 64; ++c)
+          ptx::tma_load_4d(sa + c * (64 * BK * 2), ma, ring.full(), t.m_blk * BM + c * 64, kb * BK, 0, 0);
+#pragma unroll
+        for (int c = 0; c < BN / 64; ++c)
+          ptx::tma_load_4d(sb + c * (64 * BK * 2), mb, ring.full(), t.n_blk * BN + c * 64, kb * BK, 0, 0);
+        ring.advance();
       }
     }
   } else {
     ptx::reg_alloc<kConsumerRegs>();
-    const int wg = (warp >> 2) - 1, g = lane >> 2, q = lane & 3;
+    const int wg = (warp >> 2) - 1;
     float acc[BN / 2];
 #pragma unroll
     for (int i = 0; i < BN / 2; ++i) acc[i] = 0.f;
-    for (int tile = blockIdx.x; tile < grp.num_tiles; tile += gridDim.x) {
-      const GroupTile t = group_tile(grp, tile);
-      const float alpha = grp.prob[t.gi].alpha;
-      consume_kblocks<BN, true, true, BF>(acc, ring, t.kb1 - t.kb0, wg, lane);
-      // M % 128 == 0 and N % 256 == 0 (gemm_wgrad_group): no edge tiles
-      float* c = grp.prob[t.gi].C + (int64_t)(t.m_blk * BM + wg * 64 + (warp & 3) * 16 + g) * grp.prob[t.gi].ldc + t.n_blk * BN + 2 * q;
-      const int64_t row8 = 8 * grp.prob[t.gi].ldc;
-#pragma unroll
-      for (int j = 0; j < BN / 8; ++j) {
-        atomicAdd(reinterpret_cast<float2*>(c + 8 * j), make_float2(acc[4 * j] * alpha, acc[4 * j + 1] * alpha));
-        atomicAdd(reinterpret_cast<float2*>(c + row8 + 8 * j), make_float2(acc[4 * j + 2] * alpha, acc[4 * j + 3] * alpha));
-      }
-    }
+    consume_kblocks<BN, true, true, BF>(acc, ring, t.kb1 - t.kb0, wg, lane);
+    // Both warpgroups read every slot, so the ring is free once both are past their last wgmma wait (all TMA loads of the
+    // unit have landed by then).  Warpgroup wg's [64 x 256] fp32 rows go to ring.smem + 64 KB * wg (launch_wgrad_group
+    // sizes the ring for both); M % 128 == 0 and N % 256 == 0 (gemm_wgrad_group): no edge tiles.
+    ptx::named_bar_sync(kOrderBar, 256);
+    const uint32_t stg = ring.smem + (uint32_t)wg * (64u * BN * 4u);
+    stage_rows_sw128<BN>(stg, acc, grp.prob[t.gi].alpha, warp, lane);
+    ptx::fence_proxy_async_smem();             // the generic-proxy stores, visible to the bulk reductions
+    ptx::named_bar_sync(kEpiBar + wg, 128);
+    if ((threadIdx.x & 127) == 0) reduce_add_rows_sw128<BN>(&grp.prob[t.gi].tc, stg, t.n_blk * BN, t.m_blk * BM + wg * 64);
   }
 }
 
@@ -820,14 +902,12 @@ fused_mlp_fwd_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_const
   // touching 8 rows) ran at the L2's rate for such requests, about half the launch at M = 8000; staged through shared
   // memory, the tile goes out as D / 32 bulk reductions per warpgroup of [64 rows x 32 columns] each, added at L2.
   // Once both warpgroups are past their last wgmma wait no ring item is read any more, so the ring holds the staging:
-  // warpgroup wg's [64 x D] fp32 rows at sW + wg * 64 * D * 4, box b (columns 32 b ..) at + 8 KB * b, rows 128 B apart
-  // with the 16-byte chunks XOR-swizzled by row % 8 (the tensor map's 128B swizzle; a warp's stores hit 32 banks).
+  // warpgroup wg's [64 x D] fp32 rows at sW + wg * 64 * D * 4 (stage_rows_sw128).
   const bool add_b2 = split == 0 && p.b2 != nullptr;
   const bool post = p.drop_post.p > 0.f;
   const float pscale = post ? p.drop_post.scale : 1.f;
   __syncthreads();
-  // this thread's rows (warp & 3) * 16 + g + 8 hr of the warpgroup's 64: row % 8 = g
-  const uint32_t row_base = sW + (uint32_t)wg * (64u * D * 4u) + (uint32_t)((warp & 3) * 16 + g) * 128u + (uint32_t)(q & 1) * 8u;
+  const uint32_t stg = sW + (uint32_t)wg * (64u * D * 4u);
   uint2 pbits[2];                              // post-dropout bytes of columns 8 j' .. 8 j' + 63 of the thread's two rows
 #pragma unroll
   for (int j = 0; j < D / 8; ++j) {
@@ -846,11 +926,11 @@ fused_mlp_fwd_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_const
         v0 = (kb & 1u) ? v0 * pscale : 0.f;
         v1 = (kb & 2u) ? v1 * pscale : 0.f;
       }
-      const uint32_t chunk = (uint32_t)(((j & 3) * 2 + (q >> 1)) ^ g);       // rows >= M are staged but not added
-      const uint32_t dst = row_base + (uint32_t)(j >> 2) * 8192u + (uint32_t)hr * 1024u + chunk * 16u;
-      asm volatile("st.shared.v2.f32 [%0], {%1, %2};" ::"r"(dst), "f"(v0), "f"(v1) : "memory");
+      out[4 * j + 2 * hr] = v0;
+      out[4 * j + 2 * hr + 1] = v1;
     }
   }
+  stage_rows_sw128<D>(stg, out, 1.f, warp, lane);   // rows >= M are staged but not added
   ptx::fence_proxy_async_smem();               // the generic-proxy stores, visible to the bulk reductions
   ptx::named_bar_sync(kEpiBar + wg, 128);
   MLP_STAMP(4);
@@ -863,11 +943,7 @@ fused_mlp_fwd_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_const
       __threadfence();
       asm volatile("fence.proxy.async.global;" ::: "memory");
     }
-#pragma unroll
-    for (int b = 0; b < D / 32; ++b)
-      ptx::tma_reduce_add_2d(&tmO, sW + (uint32_t)wg * (64u * D * 4u) + (uint32_t)b * 8192u, b * 32, m_blk * BM + wg * 64);
-    ptx::bulk_commit();
-    ptx::bulk_wait_all();                      // shared memory may be released, and the additions are performed
+    reduce_add_rows_sw128<D>(&tmO, stg, 0, m_blk * BM + wg * 64);
     if (ordered) {
       asm volatile("fence.proxy.async.global;" ::: "memory");
       __threadfence();
@@ -951,13 +1027,14 @@ int make_operand_map(const GemmOperand& op, int rows, int K, int nb1, int nb2, i
   return 0;
 }
 
-// fp32 [M, d] row-major output of the fused FFN kernel: [64 rows x 32 columns] boxes, 128B swizzle (bulk reduce-add target)
-int make_out_map_f32(float* ptr, int M, int d, CUtensorMap* out) {
+// fp32 [M, d] row-major output (rows ld floats apart) of the fused FFN, grouped weight-gradient and fp32 GEMM kernels: [64 rows
+// x 32 columns] boxes, 128B swizzle (bulk store / reduce-add target; stage_rows_sw128 writes the layout; boxes are clipped)
+int make_out_map_f32(float* ptr, int M, int d, int64_t ld, CUtensorMap* out) {
   EncodeTiledFn fn = get_encode_fn();
   B200ST_CHECK(fn != nullptr, "cuTensorMapEncodeTiled unavailable (no CUDA driver?)");
-  B200ST_CHECK((reinterpret_cast<uintptr_t>(ptr) & 15) == 0 && d % 32 == 0, "fp32 output map: unaligned base or width");
+  B200ST_CHECK((reinterpret_cast<uintptr_t>(ptr) & 15) == 0 && ld >= d && ld % 4 == 0, "fp32 output map: unaligned base or row stride");
   cuuint64_t dims[2] = {(cuuint64_t)d, (cuuint64_t)M};
-  cuuint64_t strides[1] = {(cuuint64_t)d * 4};
+  cuuint64_t strides[1] = {(cuuint64_t)ld * 4};
   cuuint32_t box[2] = {32u, 64u};
   cuuint32_t estr[2] = {1u, 1u};
   MapKey key{{(uint64_t)(uintptr_t)ptr, (uint64_t)d, (uint64_t)M, 1, 1, strides[0], 0, 0, box[1], (uint64_t)F32 << 8 | 0x10000u}};
@@ -1035,8 +1112,21 @@ struct ProfRec { GemmArgs g; cudaStream_t stream; int bn, splitk; int group_n = 
 bool g_prof = false;
 std::vector<ProfRec> g_prof_recs;
 
+// tc: the fp32 C map of a tc_gemm_f32_kernel launch, or null
 template <int BN, bool A_MN, bool B_MN, bool BF, bool CONV>
-int launch_kernel(const CUtensorMap& ta, const CUtensorMap& tb, const TcParams& p, int grid, size_t smem, cudaStream_t stream) {
+int launch_kernel(const CUtensorMap& ta, const CUtensorMap& tb, const CUtensorMap* tc, const TcParams& p, int grid, size_t smem,
+                  cudaStream_t stream) {
+  if constexpr (!CONV) {
+    if (tc) {
+      auto kf = tc_gemm_f32_kernel<BN, A_MN, B_MN, BF>;
+      static bool attr_f32 = false;
+      if (!attr_f32) {
+        B200ST_CUDA(cudaFuncSetAttribute(kf, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemLimit));
+        attr_f32 = true;
+      }
+      return launch(kf, grid, kThreads, smem, stream, ta, tb, *tc, p);
+    }
+  }
   void (*kern)(const CUtensorMap, const CUtensorMap, const TcParams);
   if constexpr (CONV) kern = tc_gemm_conv_kernel<B_MN, BF>;
   else kern = tc_gemm_kernel<BN, A_MN, B_MN, BF>;
@@ -1049,18 +1139,19 @@ int launch_kernel(const CUtensorMap& ta, const CUtensorMap& tb, const TcParams& 
 }
 
 template <int BN, bool A_MN, bool B_MN, bool CONV = false>
-int launch_variant(bool bf, const CUtensorMap& ta, const CUtensorMap& tb, const TcParams& p, int grid, size_t smem, cudaStream_t stream) {
-  if (bf) return launch_kernel<BN, A_MN, B_MN, true, CONV>(ta, tb, p, grid, smem, stream);
-  return launch_kernel<BN, A_MN, B_MN, false, CONV>(ta, tb, p, grid, smem, stream);
+int launch_variant(bool bf, const CUtensorMap& ta, const CUtensorMap& tb, const CUtensorMap* tc, const TcParams& p, int grid, size_t smem,
+                   cudaStream_t stream) {
+  if (bf) return launch_kernel<BN, A_MN, B_MN, true, CONV>(ta, tb, tc, p, grid, smem, stream);
+  return launch_kernel<BN, A_MN, B_MN, false, CONV>(ta, tb, tc, p, grid, smem, stream);
 }
 
 template <int BN>
-int launch_bn(bool a_mn, bool b_mn, bool bf, const CUtensorMap& ta, const CUtensorMap& tb, const TcParams& p, int grid, size_t smem,
-              cudaStream_t stream) {
-  if (!a_mn && !b_mn) return launch_variant<BN, false, false>(bf, ta, tb, p, grid, smem, stream);
-  if (!a_mn && b_mn) return launch_variant<BN, false, true>(bf, ta, tb, p, grid, smem, stream);
-  if (a_mn && !b_mn) return launch_variant<BN, true, false>(bf, ta, tb, p, grid, smem, stream);
-  return launch_variant<BN, true, true>(bf, ta, tb, p, grid, smem, stream);
+int launch_bn(bool a_mn, bool b_mn, bool bf, const CUtensorMap& ta, const CUtensorMap& tb, const CUtensorMap* tc, const TcParams& p, int grid,
+              size_t smem, cudaStream_t stream) {
+  if (!a_mn && !b_mn) return launch_variant<BN, false, false>(bf, ta, tb, tc, p, grid, smem, stream);
+  if (!a_mn && b_mn) return launch_variant<BN, false, true>(bf, ta, tb, tc, p, grid, smem, stream);
+  if (a_mn && !b_mn) return launch_variant<BN, true, false>(bf, ta, tb, tc, p, grid, smem, stream);
+  return launch_variant<BN, true, true>(bf, ta, tb, tc, p, grid, smem, stream);
 }
 
 }  // namespace
@@ -1154,8 +1245,15 @@ int gemm_tc_impl(const GemmArgs& g, cudaStream_t stream, const ConvA* conv) {
   p.vec2 = ((reinterpret_cast<uintptr_t>(g.C) % pair_bytes) == 0 && g.ldc % 2 == 0 && (g.nb1 == 1 || g.c_sb1 % 2 == 0) &&
             (g.nb2 == 1 || g.c_sb2 % 2 == 0)) ? 1 : 0;
   p.plain16 = (!p.atomic && g.c_dtype != F32 && p.vec2 && !g.epi.relu && !g.epi.mask_src && g.epi.drop.p == 0.f && !g.epi.residual) ? 1 : 0;
+  // fp32 C of a non-batched GEMM that fits a tensor map, epilogue alpha (+ bias unless added): tc_gemm_f32_kernel's bulk
+  // stores or, for split-K / accumulate, bulk reduce-adds instead of the general loop's per-element stores and atomics
+  const bool f32c = g.c_dtype == F32 && !conv && g.nb1 == 1 && g.nb2 == 1 && (reinterpret_cast<uintptr_t>(g.C) & 15) == 0 &&
+                    g.ldc >= g.N && g.ldc % 4 == 0 && !g.epi.relu && !g.epi.mask_src && g.epi.drop.p == 0.f && !g.epi.residual &&
+                    !(p.atomic && g.epi.bias);
+  p.c_reduce = p.atomic;
 
-  CUtensorMap ta, tb;
+  CUtensorMap ta, tb, tc;
+  if (f32c) B200ST_TRY(make_out_map_f32(reinterpret_cast<float*>(g.C), g.M, g.N, g.ldc, &tc));
   if (conv) {
     B200ST_CHECK(conv->mode == kConvRows && bn == 128 && splitk == 1 && !g.A.mn_major && g.nb1 == 1 && g.nb2 == 1 && conv->C % BK == 0 && conv->ntaps <= 9 &&
                      g.K == conv->ntaps * conv->C && g.M == conv->B * conv->ub * BM && conv->F2 * conv->tu <= BM &&
@@ -1187,12 +1285,12 @@ int gemm_tc_impl(const GemmArgs& g, cudaStream_t stream, const ConvA* conv) {
   int rc = 0;
   const bool bf = g.A.dtype == BF16;
   if (conv) {
-    if (g.B.mn_major) return launch_variant<128, false, true, true>(bf, ta, tb, p, grid, smem, stream);
-    return launch_variant<128, false, false, true>(bf, ta, tb, p, grid, smem, stream);
+    if (g.B.mn_major) return launch_variant<128, false, true, true>(bf, ta, tb, nullptr, p, grid, smem, stream);
+    return launch_variant<128, false, false, true>(bf, ta, tb, nullptr, p, grid, smem, stream);
   }
   switch (bn) {
-    case 64: rc = launch_bn<64>(g.A.mn_major, g.B.mn_major, bf, ta, tb, p, grid, smem, stream); break;
-    case 128: rc = launch_bn<128>(g.A.mn_major, g.B.mn_major, bf, ta, tb, p, grid, smem, stream); break;
+    case 64: rc = launch_bn<64>(g.A.mn_major, g.B.mn_major, bf, ta, tb, f32c ? &tc : nullptr, p, grid, smem, stream); break;
+    case 128: rc = launch_bn<128>(g.A.mn_major, g.B.mn_major, bf, ta, tb, f32c ? &tc : nullptr, p, grid, smem, stream); break;
     default: B200ST_FAIL("unsupported BN");
   }
   return rc;
@@ -1296,22 +1394,32 @@ int64_t conv2_dgrad_implicit_elems(int B, int T2, int F2, int C) {
 
 
 // One launch for the weight gradients of a backward block (see tc_wgrad_group_kernel).  Every product must be a plain
-// fp32-accumulate MN-major x MN-major 16-bit GEMM with M % 128 == 0 and N % 256 == 0; returns 2 (nothing launched) when the
-// group does not qualify, so that the caller issues the products one by one.
-// Splits the products of `grp` (tensor maps, C, ldc and alpha set; m_tiles, n_tiles and kb_total given) into work units of
-// one common k-range length and launches them as one wave.
+// fp32-accumulate MN-major x MN-major 16-bit GEMM with M % 128 == 0 and N % 256 == 0, whose C fits an fp32 tensor map, and
+// the group's output tiles must fit one wave; gemm_wgrad_group returns 2 (nothing launched) when the group does not
+// qualify, so that the caller issues the products one by one.
+// Output tiles of the group's products: at most one wave, since every tile is at least one work unit.
+static int64_t wgrad_group_tiles(const TcGroup& grp) {
+  int64_t tiles = 0;
+  for (int i = 0; i < grp.n; ++i) tiles += (int64_t)grp.prob[i].m_tiles * grp.prob[i].n_tiles;
+  return tiles;
+}
+// Splits the products of `grp` (tensor maps and alpha set; m_tiles, n_tiles and kb_total given) into work units of one
+// common k-range length and launches them as one wave, one unit per CTA: the kernel's tail stages the unit's sums in the
+// operand ring, which is only drained for good when no further unit follows.
 static int launch_wgrad_group(TcGroup& grp, bool bf, cudaStream_t stream) {
   int num_sms = 0;
   B200ST_TRY(usable_sms(&num_sms));
+  B200ST_CHECK(wgrad_group_tiles(grp) <= num_sms, "grouped weight gradient: more output tiles than SMs");
   int64_t work = 0;
   for (int i = 0; i < grp.n; ++i) work += (int64_t)grp.prob[i].m_tiles * grp.prob[i].n_tiles * grp.prob[i].kb_total;
-  // smallest common k-range L (in 64-row blocks) whose work units fit one wave of `num_sms` CTAs
+  // smallest common k-range L (in 64-row blocks) whose work units fit one wave of `num_sms` CTAs; it exists (at the longest
+  // product's kb_total every product is one unit per tile)
   int L = (int)((work + num_sms - 1) / num_sms);
   if (L < 2) L = 2;
   for (;; ++L) {
     int64_t units = 0;
     for (int i = 0; i < grp.n; ++i) units += (int64_t)grp.prob[i].m_tiles * grp.prob[i].n_tiles * ceil_div(grp.prob[i].kb_total, L);
-    if (units <= num_sms || L >= 4096) break;
+    if (units <= num_sms) break;
   }
   int tile = 0;
   for (int i = 0; i < grp.n; ++i) {
@@ -1322,20 +1430,21 @@ static int launch_wgrad_group(TcGroup& grp, bool bf, cudaStream_t stream) {
     tile += q.m_tiles * q.n_tiles * q.splitk;
   }
   grp.num_tiles = tile;
+  B200ST_CHECK(grp.num_tiles <= num_sms, "grouped weight gradient: one work unit per CTA");
   const uint32_t stage_bytes = kABytes + 256u * BK * 2;
   int stages = (int)((kSmemLimit - 2048) / stage_bytes);
   if (stages > 8) stages = 8;
   grp.stages = stages;
   const size_t smem = 1024 + (size_t)stages * stage_bytes + 16 * stages + 16;
   B200ST_CHECK(smem <= (size_t)kSmemLimit, "smem budget exceeded");
+  B200ST_CHECK((size_t)stages * stage_bytes >= 2 * 64 * 256 * 4, "grouped weight gradient: the ring holds both warpgroups' output rows");
   auto kern = bf ? tc_wgrad_group_kernel<true> : tc_wgrad_group_kernel<false>;
   static bool attr_set[2] = {false, false};
   if (!attr_set[bf]) {
     B200ST_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemLimit));
     attr_set[bf] = true;
   }
-  const int grid = grp.num_tiles < num_sms ? grp.num_tiles : num_sms;
-  return launch(kern, grid, kThreads, smem, stream, grp);
+  return launch(kern, grp.num_tiles, kThreads, smem, stream, grp);
 }
 
 int gemm_wgrad_group(const GemmArgs* gs, int n, cudaStream_t stream) {
@@ -1345,20 +1454,27 @@ int gemm_wgrad_group(const GemmArgs* gs, int n, cudaStream_t stream) {
     const bool plain = !g.epi.relu && !g.epi.mask_src && g.epi.drop.p == 0.f && !g.epi.residual && !g.epi.bias && g.epi.accumulate;
     if (!(is16(g.A.dtype) && g.A.dtype == g.B.dtype && g.A.dtype == gs[0].A.dtype && g.A.mn_major && g.B.mn_major && plain &&
           g.c_dtype == F32 && g.nb1 == 1 && g.nb2 == 1 && g.M % BM == 0 && g.N % 256 == 0 && g.K > 0 && g.splitk <= 1 &&
-          (reinterpret_cast<uintptr_t>(g.C) & 7) == 0 && g.ldc % 2 == 0))
+          (reinterpret_cast<uintptr_t>(g.C) & 15) == 0 && g.ldc >= g.N && g.ldc % 4 == 0))     // C fits an fp32 tensor map
       return 2;
   }
   TcGroup grp;
   std::memset(&grp, 0, sizeof(grp));
   grp.n = n;
   for (int i = 0; i < n; ++i) {
+    grp.prob[i].m_tiles = gs[i].M / BM;
+    grp.prob[i].n_tiles = gs[i].N / 256;
+  }
+  int num_sms = 0;
+  B200ST_TRY(usable_sms(&num_sms));
+  if (wgrad_group_tiles(grp) > num_sms) return 2;
+  for (int i = 0; i < n; ++i) {
     const GemmArgs& g = gs[i];
     TcGroupProb& q = grp.prob[i];
-    q.m_tiles = g.M / BM; q.n_tiles = g.N / 256; q.kb_total = ceil_div(g.K, BK);
+    q.kb_total = ceil_div(g.K, BK);
     q.alpha = g.epi.alpha;
     B200ST_TRY(make_operand_map(g.A, g.M, g.K, 1, 1, BM, &q.ta));
     B200ST_TRY(make_operand_map(g.B, g.N, g.K, 1, 1, 256, &q.tb));
-    q.C = reinterpret_cast<float*>(g.C); q.ldc = g.ldc;
+    B200ST_TRY(make_out_map_f32(reinterpret_cast<float*>(g.C), g.M, g.N, g.ldc, &q.tc));
   }
   B200ST_TRY(launch_wgrad_group(grp, gs[0].A.dtype == BF16, stream));
   if (g_prof) {
@@ -1376,8 +1492,7 @@ namespace {
 // operand traffic from L2, not by HBM)
 int conv_wgrad_launch(const GemmArgs& g, const ConvA& ca, cudaStream_t stream) {
   B200ST_CHECK(ca.mode == kConvWgrad && is16(g.A.dtype) && g.A.dtype == g.B.dtype && ca.C % BM == 0 && ca.ntaps == 9 &&
-                   g.M == 9 * ca.C && g.N == ca.C && ca.C % 256 == 0 && ca.F2 >= 1 && ca.F2 <= 2 * BK && g.c_dtype == F32 &&
-                   (reinterpret_cast<uintptr_t>(g.C) & 7) == 0 && g.ldc % 2 == 0,
+                   g.M == 9 * ca.C && g.N == ca.C && ca.C % 256 == 0 && ca.F2 >= 1 && ca.F2 <= 2 * BK && g.c_dtype == F32,
                "implicit conv2 filter gradient: unsupported shape");
   const int fw = ca.F2 < BK ? ca.F2 : BK, kt = ca.F2 < BK ? BK / ca.F2 : 1;
   TcGroup grp;
@@ -1391,7 +1506,7 @@ int conv_wgrad_launch(const GemmArgs& g, const ConvA& ca, cudaStream_t stream) {
   q.m_tiles = g.M / BM; q.n_tiles = g.N / 256; q.kb_total = ca.B * cw.kc;
   B200ST_CHECK(ceil_div(g.K, BK) == q.kb_total, "implicit conv2 filter gradient: k-blocks do not match the chunking");
   q.alpha = g.epi.alpha;
-  q.C = reinterpret_cast<float*>(g.C); q.ldc = g.ldc;
+  B200ST_TRY(make_out_map_f32(reinterpret_cast<float*>(g.C), g.M, g.N, g.ldc, &q.tc));
   B200ST_TRY(make_conv_map(ca.x, g.A.dtype, ca.C, ca.F2, ca.T2, ca.planes, fw, kt, &q.ta));
   B200ST_TRY(make_conv_map(ca.dy, g.B.dtype, ca.C, ca.F2, ca.T2, ca.B, fw, kt, &q.tb));
   B200ST_TRY(launch_wgrad_group(grp, g.A.dtype == BF16, stream));
@@ -1442,7 +1557,7 @@ int fused_mlp_fwd(const void* X, int dtype, int M, int d, int ffn, const void* W
   B200ST_TRY(make_operand_map(GemmOperand{W1, dtype, 1, ffn, 0, 0}, ffn, d, 1, 1, 64, &tw1));
   B200ST_TRY(make_operand_map(GemmOperand{W2, dtype, 1, d, 0, 0}, d, ffn, 1, 1, 64, &tw2));
   CUtensorMap to;
-  B200ST_TRY(make_out_map_f32(x_out, M, d, &to));
+  B200ST_TRY(make_out_map_f32(x_out, M, d, d, &to));
   auto kern = d == 256 ? (dtype == F16 ? fused_mlp_fwd_kernel<F16, true, 256> : fused_mlp_fwd_kernel<BF16, true, 256>)
                        : (dtype == F16 ? fused_mlp_fwd_kernel<F16, true, 128> : fused_mlp_fwd_kernel<BF16, true, 128>);
   static bool attr[4] = {false, false, false, false};
@@ -1474,7 +1589,7 @@ int fused_mlp_bwd(const void* dY, int dtype, int M, int d, int ffn, const void* 
   B200ST_TRY(make_operand_map(GemmOperand{W2, dtype, 0, d, 0, 0}, ffn, d, 1, 1, 64, &tw1));      // G1: rows = hidden units, k = d
   B200ST_TRY(make_operand_map(GemmOperand{W1, dtype, 0, ffn, 0, 0}, d, ffn, 1, 1, d, &tw2));      // G2: rows = model dims, k = hidden
   CUtensorMap to;
-  B200ST_TRY(make_out_map_f32(dH, M, d, &to));
+  B200ST_TRY(make_out_map_f32(dH, M, d, d, &to));
   auto kern = d == 256 ? (dtype == F16 ? fused_mlp_fwd_kernel<F16, false, 256> : fused_mlp_fwd_kernel<BF16, false, 256>)
                        : (dtype == F16 ? fused_mlp_fwd_kernel<F16, false, 128> : fused_mlp_fwd_kernel<BF16, false, 128>);
   static bool attr[4] = {false, false, false, false};
