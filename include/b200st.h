@@ -375,6 +375,16 @@ int b200st_optimizer_step_pruned(b200st_handle h, const b200st_optim_args* a, co
  * (or NULL).  scratch as for b200st_prune_args. */
 int b200st_prune_select(float* params, void* shadow, const int64_t* offsets, const int64_t* sizes, const int64_t* k, int32_t n,
                         uint8_t* mask, float* thresholds, void* scratch, void* stream);
+/* Partial tuning of a pruned model (Prune-Tune, examples/prune_tune/src/partial_tuning_optimizer.py): b200st_optimizer_step,
+ * after which every element whose bit of `frozen` is 1 keeps the weight it had before the step, in the parameter arena and
+ * in the 16-bit shadow (w = w_orig * original_mask + w * tuning_mask).  frozen: device, numel / 8 bytes, bit j of byte b is
+ * element 8b + j (the pruning mask's layout); 1 in the alignment padding.  The Adam moments, the gradient statistics and
+ * the loss-scale state advance exactly as in b200st_optimizer_step, and the free elements get its weights bit for bit.
+ * numel must be the handle's arena, padded to a multiple of 8. */
+int b200st_optimizer_step_partial(b200st_handle h, const b200st_optim_args* a, const uint8_t* frozen, void* stream);
+/* params[i] = 0 (and shadow[i] = +0 when shadow is not NULL; shadow_dtype B200ST_F16 or B200ST_BF16) for every element whose
+ * bit of `keep` (same layout) is 0.  n: a multiple of 8. */
+int b200st_apply_mask(float* params, void* shadow, int shadow_dtype, const uint8_t* keep, int64_t n, void* stream);
 /* legacy form: plain Keras Adam with a bf16 shadow, epsilon-hat form (neurst/optimizers/__init__.py:21; hparams speech_transformer.py:265-270):
  * g' = g*grad_scale; m,v update; p -= lr*sqrt(1-b2^t)/(1-b1^t) * m/(sqrt(v)+eps); optional bf16 shadow refresh + g=0 */
 int b200st_adam_step(float* params, float* grads, float* m, float* v, void* shadow, int64_t numel, float lr, float beta1,

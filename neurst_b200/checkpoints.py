@@ -79,6 +79,12 @@ def tf_variable_names(table, scope=None):
     return out
 
 
+def archive_scope(keys, table):
+    """The top-level scope of an archive's variable names when they share one, else the model's own scope."""
+    scopes = {k.split("/")[0] for k in keys if "/" in k}
+    return scopes.pop() if len(scopes) == 1 else model_scope(table)
+
+
 def save_npz(rt, path, scope=None, extra=None):
     """Writes every parameter under its reference variable name (+ optional Adam slots as `<name>/.OPTIMIZER_SLOT/{m,v}`)."""
     names = tf_variable_names(rt.table, scope)
@@ -102,8 +108,7 @@ def load_npz(rt, path, scope=None, strict=True, pattern=None, slots=True):
     z = np.load(path)
     keys = [k for k in z.files if "/.OPTIMIZER_SLOT/" not in k]
     if scope is None:
-        scopes = {k.split("/")[0] for k in keys if "/" in k}
-        scope = scopes.pop() if len(scopes) == 1 else model_scope(rt.table)
+        scope = archive_scope(keys, rt.table)
     names = tf_variable_names(rt.table, scope)
     if pattern is not None:
         own = tf_variable_names(rt.table)

@@ -16,7 +16,10 @@ Keys understood (the ones of examples/speech_transformer/*/st_training_args.yml)
 summary_steps, save_checkpoint_steps, update_cycle, clip_value, clip_norm, criterion.params.label_smoothing, optimizer.params,
 lr_schedule.params, pretrain_model, initial_global_step, pruning_schedule / pruning_schedule.params {initial_sparsity,
 target_sparsity, begin_pruning_step, end_pruning_step, pruning_frequency, polynomial_power} (or the same names as flat
-flags), pruning_variable_pattern, nopruning_variable_pattern}, dataset.class AudioTFRecordDataset / dataset.params, task.class SpeechToText /
+flags), pruning_variable_pattern, nopruning_variable_pattern}, `entry: prune_tune_train` (`train` with the Prune-Tune recipe's
+partial_tuning (a bare --partial_tuning) and mask_pkl, and <model_dir>/mask.pkl written after a pruning or partial-tuning
+run; --include is accepted and ignored), `entry: mask_predict` / `mask_generation` (`predict` with the weights multiplied
+by the masks of mask_pkl), dataset.class AudioTFRecordDataset / dataset.params, task.class SpeechToText /
 task.params, model.class / model.params / hparams_set, model_dir, dtype, and for `predict` the keys of the prediction
 recipes: `entry: predict` (the alias of entry.class) and search_method beam_search / search_method.params {beam_size,
 length_penalty, top_k, maximum_decode_length, extra_decode_length, minimum_decode_length, enable_unk} or search_method
@@ -52,6 +55,14 @@ TEXT_DATASETS = ("paralleltextdataset", "paralleltext")
 TEXT_MODELS = ("transformer",)
 WAITK_MODELS = ("waitktransformer",)
 SPEECH_MODELS = ("speechtransformer", "b200speechtransformer", "b200st")
+# the reference's boolean flags that stand alone on its command lines (`--partial_tuning`, examples/prune_tune/README.md):
+# they take no value unless written `--flag=value`; every other flag takes the values that follow it
+BARE_FLAGS = ("partial_tuning",)
+# flags of the reference's launcher that have nothing to do here (`--include examples/prune_tune/src/` loads its plugins)
+IGNORED_FLAGS = ("include",)
+TRAIN_ENTRIES = ("trainer", "train", "prune_tune_train")
+MASK_PREDICT_ENTRIES = ("mask_predict", "mask_generation")
+PREDICT_ENTRIES = ("predict", "sequencegenerator", "sequence_generator") + MASK_PREDICT_ENTRIES
 VALIDATOR_FLAGS = ("eval_steps", "eval_start_at", "eval_on_begin", "eval_dataset", "eval_dataset.params", "eval_batch_size",
                    "eval_task_args", "eval_criterion", "eval_criterion.params", "eval_search_method", "eval_search_method.params",
                    "eval_metric", "eval_metric.params", "eval_estop_patience", "eval_best_checkpoint_path",
@@ -91,6 +102,10 @@ def parse_command_line(argv):
         key = a[2:]
         if "=" in key:
             key, val = key.split("=", 1)
+        elif key in BARE_FLAGS:
+            overrides.append((key, True))
+            i += 1
+            continue
         else:
             i += 1
             if i >= len(argv):
@@ -112,7 +127,7 @@ def parse_command_line(argv):
         else:
             overrides.append((key, _coerce(val)))
         i += 1
-    return paths, overrides
+    return paths, [(k, v) for k, v in overrides if k not in IGNORED_FLAGS]
 
 
 def _set_dotted(cfg, key, val):
@@ -131,6 +146,10 @@ def load_config(paths, overrides=()):
         with open(p) as f:
             cfg = deep_merge(cfg, yaml.safe_load(f) or {})
     for key, val in overrides:
+        if key in ("entry", "search_method", "validator") and (key + ".class") in cfg:
+            # `--entry` is the command-line alias of `entry.class` (flags_core.py: ModuleFlag): it overrides the file's class
+            cfg[key + ".class"] = val
+            continue
         if "." in key or key in TOP_LEVEL:
             _set_dotted(cfg, key, val)
             continue
@@ -403,7 +422,7 @@ def resolve(cfg, world=1):
     model_dirs = flatten_string_list(cfg.get("model_dir") or ep.get("model_dir") or "./b200st_model")
     if not model_dirs:
         raise SystemExit("model_dir names no directory")
-    if len(model_dirs) > 1 and entry in ("trainer", "train"):
+    if len(model_dirs) > 1 and entry in TRAIN_ENTRIES:
         raise SystemExit("training writes one model_dir, got %d: %s" % (len(model_dirs), ", ".join(model_dirs)))
     plan = {
         "entry": entry, "model_class": "SpeechTransformer",
@@ -524,7 +543,7 @@ def _resolve_wait_k(cfg, ep, tp, entry, model_dirs):
     k = cfg.get("wait_k", ep.get("wait_k"))
     if k is None:
         k = tp.get("wait_k")
-    if k is None and entry not in ("trainer", "train") and len(model_dirs) == 1:
+    if k is None and entry not in TRAIN_ENTRIES and len(model_dirs) == 1:
         path = os.path.join(model_dirs[0], MODEL_CONFIGS)
         if os.path.isfile(path):
             k = (_model_dir_configs(model_dirs[0], "model_dir").get("task.params") or {}).get("wait_k")
@@ -543,7 +562,7 @@ def _resolve_text(cfg, ep, tp, world, entry, model_params, opt, lr, crit, waitk=
     if model_params.get("modality.share_source_target_embedding") and src_meta["tokens"] != trg_meta["tokens"]:
         raise SystemExit("modality.share_source_target_embedding needs identical source and target vocabularies (%d vs %d "
                          "entries)" % (src_meta["vocab_size"], trg_meta["vocab_size"]))
-    if entry in ("trainer", "train") and tp.get("batch_size") is None and tp.get("batch_size_per_gpu") is None:
+    if entry in TRAIN_ENTRIES and tp.get("batch_size") is None and tp.get("batch_size_per_gpu") is None:
         raise SystemExit("task.params needs batch_size or batch_size_per_gpu (tokens with batch_by_tokens, else pairs)")
     task = dict(max_src_len=tp.get("max_src_len"), max_trg_len=tp.get("max_trg_len"),
                 truncate_src=bool(tp.get("truncate_src") or False), truncate_trg=bool(tp.get("truncate_trg") or False),
@@ -553,7 +572,7 @@ def _resolve_text(cfg, ep, tp, world, entry, model_params, opt, lr, crit, waitk=
     model_dirs = flatten_string_list(cfg.get("model_dir") or ep.get("model_dir") or "./b200st_model")
     if not model_dirs:
         raise SystemExit("model_dir names no directory")
-    if len(model_dirs) > 1 and entry in ("trainer", "train"):
+    if len(model_dirs) > 1 and entry in TRAIN_ENTRIES:
         raise SystemExit("training writes one model_dir, got %d: %s" % (len(model_dirs), ", ".join(model_dirs)))
     plan = {
         "entry": entry, "model_class": "Transformer",
@@ -625,10 +644,32 @@ def resolve_pruning(cfg, ep):
     return dict(schedule=schedule, **patterns)
 
 
+def resolve_prune_tune(cfg, ep, entry, pruning, model_dirs):
+    """The Prune-Tune entries' flags (examples/prune_tune/src/partial_trainer.py:50-58, mask_sequence_generator.py:40-45):
+    prune_tune_train's partial_tuning and mask_pkl, mask_predict's / mask_generation's mask_pkl; None for the other entries."""
+    mask_pkl = _entry_key(cfg, ep, "mask_pkl") or None
+    if entry not in ("prune_tune_train",) + MASK_PREDICT_ENTRIES:
+        return None
+    if mask_pkl is not None and not os.path.isfile(str(mask_pkl)):
+        raise SystemExit("mask_pkl %s: no such file" % mask_pkl)
+    if entry in MASK_PREDICT_ENTRIES:
+        if mask_pkl is not None and len(model_dirs) > 1:
+            # the reference zips one model's masks against the ensemble's weights
+            raise SystemExit("%s with mask_pkl takes one model_dir, got %d: the masks belong to one model" % (entry, len(model_dirs)))
+        return {"mask_pkl": mask_pkl}
+    partial = bool(_entry_key(cfg, ep, "partial_tuning") or False)
+    if partial and pruning is not None:
+        # the recipe prunes in one run and tunes in the next; in one run the two writes of mask.pkl would collide
+        raise SystemExit("prune_tune_train: partial_tuning together with a pruning schedule is outside this path (prune in one run, "
+                         "tune the pruned weights in the next)")
+    return {"partial_tuning": partial, "mask_pkl": mask_pkl}
+
+
 def _finish_plan(plan, cfg, ep, tp, search_method, model_dirs, text=False):
     """Prediction batch size, search, validator and ensemble settings shared by the speech and text plans, and the trainer's
-    weight pruning and initial_global_step."""
+    weight pruning, Prune-Tune flags and initial_global_step."""
     plan["pruning"] = resolve_pruning(cfg, ep)
+    plan["prune_tune"] = resolve_prune_tune(cfg, ep, plan["entry"], plan["pruning"], model_dirs)
     igs = _entry_key(cfg, ep, "initial_global_step")
     plan["initial_global_step"] = None if igs is None else int(igs)
     if plan["initial_global_step"] is not None and plan["initial_global_step"] < 0:
@@ -858,9 +899,11 @@ def initialise(model, plan):
 
 
 def train(plan):
+    from neurst_b200 import prune_tune as PT
     from neurst_b200.trainer import DataParallelTrainer, HostPipeline
     world, rank, local = _dist_setup()
     model = _build_model(plan)
+    resumed = latest_checkpoint(plan["model_dir"])[0] is not None
     start_step = initialise(model, plan)
     # initial_global_step wins over a restored checkpoint's step (exps/trainer.py:172-178): the noam position, the checkpoint
     # numbers and the validation steps count from it, and the run makes train_steps updates (the reference's steps_per_epoch)
@@ -878,10 +921,12 @@ def train(plan):
             raise SystemExit("pruning: the variable patterns select no parameter tensor")
         LOG.info("Pruning: %s, %d of %d parameter tensors will be pruned", type(schedule).__name__, len(names),
                  len(model.runtime.table))
+    prune_tune = plan.get("prune_tune") or {}
+    partial = _partial_tuning_masks(model, plan, resumed) if prune_tune.get("partial_tuning") else None
     trainer = DataParallelTrainer(model, plan["optimizer"], plan["lr_schedule"], update_cycle=plan["update_cycle"],
                                   use_cuda_graph=True, clip_value=plan["clip_value"], clip_norm=plan["clip_norm"],
                                   summary_steps=plan["summary_steps"] if rank == 0 else 0, logger=LOG.info,
-                                  pruning_schedule=schedule, pruning_variables=names)
+                                  pruning_schedule=schedule, pruning_variables=names, partial_tuning_mask=partial)
     trainer.global_step = start_step
     if igs is not None:
         # only the lr schedule, the checkpoints and validation read the initial step (compat.register_initial_step); the
@@ -897,6 +942,16 @@ def train(plan):
     trainer.broadcast_parameters()
     if rank == 0:
         write_model_configs(plan)
+    mask_path = os.path.join(plan["model_dir"], PT.MASK_FILE)
+    if partial is not None:
+        tuned, frozen = trainer.setup_partial_tuning()
+        LOG.info("Partial tuning: %d weights are tuned, %d frozen (masks from %s)", tuned, frozen,
+                 "the non-zero weights" if isinstance(partial, str) else prune_tune.get("mask_pkl") or mask_path)
+        if rank == 0:
+            # the reference writes the loaded masks (None without mask_pkl) at the end only; this path writes the masks it
+            # tunes with before the first update, so that a resumed run finds them, and again at the end
+            os.makedirs(plan["model_dir"], exist_ok=True)
+            PT.save_masks(model.runtime, mask_path, model.runtime.partial_frozen)
     validator = None
     if plan.get("validator"):
         from neurst_b200.validation import Validator
@@ -941,11 +996,18 @@ def train(plan):
     torch.cuda.synchronize()
     if rank == 0 and trainer.global_step > start_step:
         save_checkpoint(model.runtime, plan["model_dir"], trainer.global_step, plan["max_to_keep"])
+    if rank == 0 and plan["entry"] == "prune_tune_train" and (partial is not None or schedule is not None):
+        # partial_trainer.py:188-206: after a pruning run weight != 0 over every variable, after a partial tuning its masks
+        rt = model.runtime
+        PT.save_masks(rt, mask_path, rt.partial_frozen if partial is not None else rt.derive_prune_mask(list(rt.table)))
+        LOG.info("wrote the masks to %s", mask_path)
     sparsity = log_sparsity() if rank == 0 else None
     if world > 1:
         trainer.close()
         torch.distributed.barrier()
     res = {"global_step": trainer.global_step, "loss": last}
+    if partial is not None:
+        res["partial_tuning"] = {"tuned": trainer.partial_counts[0], "frozen": trainer.partial_counts[1]}
     if sparsity is not None:
         # the schedule's device state: updates applied in this run, pruning turns, the last turn's sparsity
         import struct
@@ -956,6 +1018,26 @@ def train(plan):
     if validator is not None:
         res.update(early_stopped=early_stopped, validations=validator.history)
     return res
+
+
+def _partial_tuning_masks(model, plan, resumed):
+    """The masks of a partial-tuning run (partial_tuning_optimizer.py:50-80): those of mask_pkl; else "weights", i.e.
+    weight != 0 of the restored or pretrained weights.  One deliberate deviation: a run that resumes from a checkpoint of its
+    own model_dir without mask_pkl reads <model_dir>/mask.pkl, which the run wrote before its first update: the reference
+    would re-derive the masks from the tuned weights, in which nearly every weight is non-zero, and freeze them all."""
+    from neurst_b200 import prune_tune as PT
+    path = plan["prune_tune"]["mask_pkl"]
+    if path is None and resumed:
+        path = os.path.join(plan["model_dir"], PT.MASK_FILE)
+        if not os.path.isfile(path):
+            raise SystemExit("partial tuning resumes from a checkpoint of %s, which holds no %s: give --mask_pkl (masks "
+                             "derived from the tuned weights would freeze nearly every weight)" % (plan["model_dir"], PT.MASK_FILE))
+    if path is None:
+        return "weights"
+    try:
+        return PT.load_masks(model.runtime, path)
+    except PT.MaskFileError as e:
+        raise SystemExit(str(e))
 
 
 def ids_to_text(ids, eos_id, tokens):
@@ -1060,6 +1142,16 @@ def predict(plan):
                  plan["ensemble_weights"])
     else:
         model, step = _restore(plan, plan["model_dir"])
+        mask_pkl = (plan.get("prune_tune") or {}).get("mask_pkl")
+        if mask_pkl:
+            # mask_sequence_generator.py:74-84: every weight times its mask, on the device, before the search
+            from neurst_b200 import prune_tune as PT
+            try:
+                masks = PT.load_masks(model.runtime, mask_pkl)
+            except PT.MaskFileError as e:
+                raise SystemExit(str(e))
+            model.runtime.apply_mask(PT.mask_bitmap(model.runtime, masks))
+            LOG.info("%s: weights masked with %s", plan["entry"], mask_pkl)
     task, examples = _examples(plan, rank, world, training=False)
     per_call, search_kw = decode_settings(plan)
     if ensemble:
@@ -1175,18 +1267,18 @@ def main(argv=None):
     paths, overrides = parse_command_line(list(sys.argv[1:] if argv is None else argv))
     cfg = load_config(paths, overrides)
     plan = resolve(cfg, world=int(os.environ.get("WORLD_SIZE", "1")))
-    if plan["entry"] in ("trainer", "train"):
+    if plan["entry"] in TRAIN_ENTRIES:
         res = train(plan)
         if "validations" in res:
             res["validations"] = [{k: v for k, v in r.items() if k != "hypotheses"} for r in res["validations"]]
     elif plan["entry"] == "cascade_st":
         res = cascade_st(plan)
         res = {k: v for k, v in res.items() if not k.endswith("_hypotheses")}
-    elif plan["entry"] in ("predict", "sequencegenerator", "sequence_generator"):
+    elif plan["entry"] in PREDICT_ENTRIES:
         res = predict(plan)
         res = {"checkpoint_step": res["checkpoint_step"], "n_hypotheses": len(res["hypotheses"])}
     else:
-        raise SystemExit("entry.class %r is outside this path (trainer / predict)" % plan["entry"])
+        raise SystemExit("entry.class %r is outside this path (trainer, prune_tune_train, predict, mask_predict)" % plan["entry"])
     LOG.info("%s", json.dumps(res))
     return res
 

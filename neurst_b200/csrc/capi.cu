@@ -411,6 +411,29 @@ int b200st_optimizer_step_pruned(b200st_handle h, const b200st_optim_args* a, co
   fill_tensor_table(h->m, tt);
   return optimizer_step_pruned(o, tt, pt, sc, pd, reinterpret_cast<cudaStream_t>(stream));
 }
+int b200st_optimizer_step_partial(b200st_handle h, const b200st_optim_args* a, const uint8_t* frozen, void* stream) {
+  if (!h || !a || !frozen) B200ST_FAIL("null argument");
+  if (!a->params || !a->grads || !a->m || !a->v) B200ST_FAIL("bad optimizer arguments");
+  if (!a->loss_scale_state && a->step_t < 1) B200ST_FAIL("step_t counts from 1");
+  if (a->numel != h->m.arena_numel) B200ST_FAIL("numel does not match the handle's parameter arena");
+  OptimArgs o{};
+  o.p = a->params; o.g = a->grads; o.m = a->m; o.v = a->v;
+  o.shadow = a->shadow; o.shadow_dtype = a->shadow_dtype;
+  o.n = a->numel;
+  o.lr = a->lr; o.beta1 = a->beta1; o.beta2 = a->beta2; o.eps = a->eps; o.step_t = a->step_t;
+  o.grad_scale = a->grad_scale; o.zero_grad = a->zero_grad;
+  o.clip_value = a->clip_value; o.clip_norm = a->clip_norm;
+  o.tensor_sumsq = a->tensor_sumsq; o.ctl = a->loss_scale_state;
+  o.growth_steps = a->growth_steps; o.multiplier = a->multiplier;
+  TensorTable tt{};
+  fill_tensor_table(h->m, tt);
+  return optimizer_step_partial(o, tt, frozen, reinterpret_cast<cudaStream_t>(stream));
+}
+int b200st_apply_mask(float* params, void* shadow, int shadow_dtype, const uint8_t* keep, int64_t n, void* stream) {
+  if (!params || !keep) B200ST_FAIL("null argument");
+  if (shadow && shadow_dtype != B200ST_F16 && shadow_dtype != B200ST_BF16) B200ST_FAIL("apply_mask: the shadow must be a 16-bit type");
+  return apply_mask(params, shadow, keep, n, reinterpret_cast<cudaStream_t>(stream));
+}
 int b200st_prune_select(float* params, void* shadow, const int64_t* offsets, const int64_t* sizes, const int64_t* k, int32_t n,
                         uint8_t* mask, float* thresholds, void* scratch, void* stream) {
   if (!params || !offsets || !sizes || !k || !mask || !scratch) B200ST_FAIL("null argument");

@@ -1,7 +1,8 @@
 // Optimizer step of the training loop: gradient statistics (per-tensor sum of squares + finite check), dynamic loss-scale
 // control, clip-by-value / per-tensor clip-by-norm and the Keras Adam update with the 16-bit shadow refresh — HBM-bound
 // streaming kernels over the flat arenas (34 B per parameter for Adam, 4 B for the statistics pass); the pruned step adds
-// the weight mask (1 bit per parameter) to the Adam pass and the selection kernels of prune.cu.
+// the weight mask (1 bit per parameter) to the Adam pass and the selection kernels of prune.cu, the partial-tuning step
+// the frozen-element bitmap (1 bit per parameter) to the Adam pass.
 //
 // Reference: GradAccumKerasModel.train_step (neurst/training/gradaccum_keras_model.py:222-240): unscale -> clip_by_value
 // or clip_by_norm per gradient tensor -> apply_gradients; Keras Adam, epsilon-hat form (neurst/optimizers/__init__.py:21,
@@ -84,16 +85,23 @@ __global__ void step_control_kernel(float* __restrict__ sumsq, int n_tensors, fl
   }
 }
 
-// MASK (the pruned step): off a pruning turn, the elements whose bit of `mask` is 0 are written as zero in the master and
-// shadow arenas after their update (their Adam moments still move, so a later turn can bring them back); on a turn
-// (*turn != 0) the mask is not applied, the selection that follows sets the new one.
-template <bool CLIP_NORM, bool MASK>
+// What the Adam pass does with the 1-bit-per-parameter `mask` (bit j of byte b is element 8b + j):
+//   NONE    no mask.
+//   PRUNE   the pruned step: off a pruning turn, the elements whose bit is 0 are written as zero in the master and shadow
+//           arenas after their update (their Adam moments still move, so a later turn can bring them back); on a turn
+//           (*turn != 0) the mask is not applied, the selection that follows sets the new one.
+//   FREEZE  the partial-tuning step: the elements whose bit is 1 keep their old weight in the master and shadow arenas
+//           (the shadow is the rounding of the master, so rounding the old weight rewrites the old 16-bit value); their
+//           Adam moments still move, as the reference's Keras Adam updates every slot before the restore.  `turn` unused.
+enum class MaskMode { NONE, PRUNE, FREEZE };
+
+template <bool CLIP_NORM, MaskMode MODE>
 __global__ void __launch_bounds__(256) adam_kernel(const OptimArgs a, const __grid_constant__ TensorTable tt, float unscale_host,
                                                    const uint8_t* __restrict__ mask, const int32_t* __restrict__ turn) {
   pdl_wait();
   pdl_trigger();
   bool apply_mask = false;
-  if constexpr (MASK) apply_mask = *turn == 0;
+  if constexpr (MODE == MaskMode::PRUNE) apply_mask = *turn == 0;
   float gs = a.grad_scale * unscale_host;
   float t = (float)a.step_t;
   bool skip = false;
@@ -133,12 +141,17 @@ __global__ void __launch_bounds__(256) adam_kernel(const OptimArgs a, const __gr
       vi[j] = b2 * vo[j] + (1.f - b2) * gi[j] * gi[j];
       pi[j] = po[j] - lr_t * mi[j] / (sqrtf(vi[j]) + a.eps);
     }
-    if constexpr (MASK) {
+    if constexpr (MODE == MaskMode::PRUNE) {
       if (apply_mask) {
         const uint32_t bits = mask[i >> 1] >> ((i & 1) * 4);     // the 4 elements of vector i: bits 4(i&1) .. 4(i&1)+3
 #pragma unroll
         for (int j = 0; j < 4; ++j) if (!((bits >> j) & 1u)) pi[j] = 0.f;
       }
+    }
+    if constexpr (MODE == MaskMode::FREEZE) {
+      const uint32_t bits = mask[i >> 1] >> ((i & 1) * 4);
+#pragma unroll
+      for (int j = 0; j < 4; ++j) if ((bits >> j) & 1u) pi[j] = po[j];
     }
     reinterpret_cast<float4*>(a.m)[i] = make_float4(mi[0], mi[1], mi[2], mi[3]);
     reinterpret_cast<float4*>(a.v)[i] = make_float4(vi[0], vi[1], vi[2], vi[3]);
@@ -205,8 +218,8 @@ int optimizer_step(const OptimArgs& a, const TensorTable& tt, cudaStream_t s) {
   const int grid = grid_for(a.n, 256 * 4 * 4);
   const uint8_t* no_mask = nullptr;
   const int32_t* no_turn = nullptr;
-  if (a.clip_norm > 0.f) return launch(adam_kernel<true, false>, grid, 256, 0, s, a, tt, 1.f, no_mask, no_turn);
-  return launch(adam_kernel<false, false>, grid, 256, 0, s, a, tt, 1.f, no_mask, no_turn);
+  if (a.clip_norm > 0.f) return launch(adam_kernel<true, MaskMode::NONE>, grid, 256, 0, s, a, tt, 1.f, no_mask, no_turn);
+  return launch(adam_kernel<false, MaskMode::NONE>, grid, 256, 0, s, a, tt, 1.f, no_mask, no_turn);
 }
 
 // The reference's pruning optimizer (neurst/sparsity/pruning_optimizer.py) inside the loss-scale optimizer: statistics and
@@ -223,9 +236,23 @@ int optimizer_step_pruned(const OptimArgs& a, const TensorTable& tt, const Prune
   const int grid = grid_for(a.n, 256 * 4 * 4);
   const uint8_t* mask = pd.mask;
   const int32_t* turn = pd.state + 1;
-  if (a.clip_norm > 0.f) B200ST_TRY(launch(adam_kernel<true, true>, grid, 256, 0, s, a, tt, 1.f, mask, turn));
-  else B200ST_TRY(launch(adam_kernel<false, true>, grid, 256, 0, s, a, tt, 1.f, mask, turn));
+  if (a.clip_norm > 0.f) B200ST_TRY(launch(adam_kernel<true, MaskMode::PRUNE>, grid, 256, 0, s, a, tt, 1.f, mask, turn));
+  else B200ST_TRY(launch(adam_kernel<false, MaskMode::PRUNE>, grid, 256, 0, s, a, tt, 1.f, mask, turn));
   return prune_select_apply(a.p, a.shadow, pt, pd, turn, s);
+}
+
+// The reference's partial-tuning optimizer (examples/prune_tune/src/partial_tuning_optimizer.py:79-88): the plain step, then
+// w = w_orig * original_mask + w * tuning_mask, i.e. the elements whose bit of `frozen` is 1 keep their weight.  Same
+// statistics, loss-scale control and launches as optimizer_step; the Adam pass reads numel / 8 bytes more.
+int optimizer_step_partial(const OptimArgs& a, const TensorTable& tt, const uint8_t* frozen, cudaStream_t s) {
+  B200ST_CHECK(a.n > 0 && a.n % 8 == 0, "the partial-tuning step needs an arena padded to a multiple of 8 elements");
+  B200ST_CHECK(frozen != nullptr, "the partial-tuning step needs the frozen-element bitmap");
+  B200ST_TRY(check_arenas(a));
+  B200ST_TRY(step_stats(a, tt, s));
+  const int grid = grid_for(a.n, 256 * 4 * 4);
+  const int32_t* no_turn = nullptr;
+  if (a.clip_norm > 0.f) return launch(adam_kernel<true, MaskMode::FREEZE>, grid, 256, 0, s, a, tt, 1.f, frozen, no_turn);
+  return launch(adam_kernel<false, MaskMode::FREEZE>, grid, 256, 0, s, a, tt, 1.f, frozen, no_turn);
 }
 
 }  // namespace b200st

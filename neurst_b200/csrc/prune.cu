@@ -197,6 +197,23 @@ __global__ void __launch_bounds__(256) prune_apply_kernel(float* __restrict__ p,
   }
 }
 
+// one thread per mask byte: the elements of its 8 whose bit is 0 -> +0 in the master and the 16-bit shadow (or null)
+__global__ void __launch_bounds__(256) apply_mask_kernel(float* __restrict__ p, uint16_t* __restrict__ shadow,
+                                                         const uint8_t* __restrict__ keep, int64_t n_bytes) {
+  pdl_wait();
+  pdl_trigger();
+  for (int64_t b = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; b < n_bytes; b += (int64_t)gridDim.x * blockDim.x) {
+    const uint32_t bits = keep[b];
+    if (bits == 0xFFu) continue;
+#pragma unroll
+    for (int j = 0; j < 8; ++j) {
+      if ((bits >> j) & 1u) continue;
+      p[b * 8 + j] = 0.f;
+      if (shadow) shadow[b * 8 + j] = 0;
+    }
+  }
+}
+
 int grid_chunks(const PruneTable& pt) {
   const uint32_t n = pt.cbase[pt.n];
   return (int)(n < 1 ? 1 : n > 132 * 8 ? 132 * 8 : n);
@@ -237,6 +254,12 @@ int prune_select(float* p, void* shadow, const PruneTable& pt, const int64_t* k,
   B200ST_TRY(check_prune_table(pt));
   B200ST_TRY(launch(prune_seed_kernel, 1, 256, 0, s, pt, k, pd.scratch));
   return prune_select_apply(p, shadow, pt, pd, reinterpret_cast<const int32_t*>(pd.scratch + 2 * kPruneMaxTensors), s);
+}
+
+int apply_mask(float* p, void* shadow, const uint8_t* keep, int64_t n, cudaStream_t s) {
+  if (n == 0) return 0;
+  B200ST_CHECK(n > 0 && n % 8 == 0, "apply_mask: the arena must be padded to a multiple of 8 elements");
+  return launch(apply_mask_kernel, grid_for(n / 8, 256, 132 * 8), 256, 0, s, p, reinterpret_cast<uint16_t*>(shadow), keep, n / 8);
 }
 
 }  // namespace b200st

@@ -251,7 +251,8 @@ EXPORTS = [
     "b200st_last_error", "b200st_version", "b200st_launch_count", "b200st_gemm", "b200st_gemm_bench", "b200st_profile_begin", "b200st_profile_end",
     "b200st_create", "b200st_destroy", "b200st_param_arena_numel", "b200st_param_count", "b200st_param_info",
     "b200st_workspace_bytes", "b200st_forward", "b200st_forward_backward", "b200st_refresh_shadow", "b200st_adam_step", "b200st_optimizer_step",
-    "b200st_prune_scratch_bytes", "b200st_optimizer_step_pruned", "b200st_prune_select",
+    "b200st_prune_scratch_bytes", "b200st_optimizer_step_pruned", "b200st_prune_select", "b200st_optimizer_step_partial",
+    "b200st_apply_mask",
     "b200st_comm_unique_id", "b200st_comm_init", "b200st_comm_broadcast", "b200st_comm_destroy", "b200st_comm_stats", "b200st_train_step",
     "b200st_encode", "b200st_encode_workspace_bytes", "b200st_decode_scratch_floats", "b200st_decode_init", "b200st_decode_step",
     "b200st_greedy_search", "b200st_greedy_used_graph", "b200st_beam_state_bytes", "b200st_beam_search",
@@ -282,6 +283,8 @@ def _declare(lib):
     lib.b200st_optimizer_step_pruned.argtypes = [C.c_void_p, C.POINTER(OptimArgs), C.POINTER(PruneArgs), C.c_void_p]
     lib.b200st_prune_select.argtypes = [C.c_void_p, C.c_void_p, C.POINTER(C.c_int64), C.POINTER(C.c_int64), C.c_void_p, C.c_int32,
                                         C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]
+    lib.b200st_optimizer_step_partial.argtypes = [C.c_void_p, C.POINTER(OptimArgs), C.c_void_p, C.c_void_p]
+    lib.b200st_apply_mask.argtypes = [C.c_void_p, C.c_void_p, C.c_int32, C.c_void_p, C.c_int64, C.c_void_p]
     lib.b200st_comm_unique_id.argtypes = [C.c_char_p]
     lib.b200st_comm_init.argtypes = [C.c_void_p, C.c_char_p, C.c_int32, C.c_int32]
     lib.b200st_comm_broadcast.argtypes = [C.c_void_p, C.c_void_p, C.c_int64, C.c_int32, C.c_void_p]

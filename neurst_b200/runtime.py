@@ -237,12 +237,15 @@ class Runtime:
         return out
 
     def adam_step(self, lr, step_t, beta1=0.9, beta2=0.98, eps=1e-9, grad_scale=1.0, zero_grad=True, clip_value=None,
-                  clip_norm=None, dynamic_loss_scale=None, growth_steps=2000, multiplier=2.0, prune=None):
+                  clip_norm=None, dynamic_loss_scale=None, growth_steps=2000, multiplier=2.0, prune=None, frozen=None):
         """One optimizer step over the flat arenas (b200st_optimizer_step): unscale -> clip (per gradient tensor, as
         tf.clip_by_value / tf.clip_by_norm in gradaccum_keras_model.py:228-233) -> Keras Adam -> shadow refresh -> g = 0.
         fp16 precision: the gradients carry the dynamic loss scale; a step with non-finite gradients is skipped on the
         device (state in `self.loss_scale_state`).  `prune`: the schedule given to prune_setup(); the step is then
-        b200st_optimizer_step_pruned (mask off-turn, selection and new mask on a turn)."""
+        b200st_optimizer_step_pruned (mask off-turn, selection and new mask on a turn).  `frozen`: the bitmap given to
+        partial_setup(); the step is then b200st_optimizer_step_partial (the elements whose bit is 1 keep their weight)."""
+        if prune is not None and frozen is not None:
+            raise L.B200STError("adam_step takes a pruning schedule or a frozen-element bitmap, not both")
         if self.adam_m is None:
             self.adam_m = torch.zeros_like(self.params)
             self.adam_v = torch.zeros_like(self.params)
@@ -269,6 +272,10 @@ class Runtime:
             a.growth_steps, a.multiplier = float(growth_steps), float(multiplier)
         if prune is not None:
             L.check(self.lib.b200st_optimizer_step_pruned(self.handle, C.byref(a), C.byref(self._prune_args(prune)), L._stream()))
+        elif frozen is not None:
+            if getattr(self, "partial_frozen", None) is not frozen:
+                raise L.B200STError("adam_step(frozen=...) needs partial_setup() with that bitmap first")
+            L.check(self.lib.b200st_optimizer_step_partial(self.handle, C.byref(a), _ptr(frozen), L._stream()))
         else:
             L.check(self.lib.b200st_optimizer_step(self.handle, C.byref(a), L._stream()))
         self._shadow_stale = False
@@ -309,16 +316,22 @@ class Runtime:
             n *= s
         return n
 
-    def derive_prune_mask(self):
-        """Mask bitmap of the pruned set from the current weights: bit j of byte b keeps element 8b + j; 1 outside the pruned
-        tensors (and in the alignment padding after each), weight != 0 inside them.  Built tensor by tensor in uint8, so
-        the temporaries are the size of the largest pruned tensor's slot."""
+    def derive_prune_mask(self, names=None, source=None):
+        """Mask bitmap of the tensors `names` (the pruned set when None) from the current weights: bit j of byte b keeps
+        element 8b + j; 1 outside those tensors (and in the alignment padding after each), weight != 0 inside them.  With
+        `source` ({name: array in the tensor's shape}, e.g. the masks of a mask file) the bits are source != 0 instead.
+        Built tensor by tensor in uint8, so the temporaries are the size of the largest tensor's slot."""
         mask = torch.full((self.numel // 8,), 0xFF, dtype=torch.uint8, device=self.device)
-        for k in self.prune_names:
+        for k in (self.prune_names if names is None else names):
             off, _ = self.table[k]
             n = self._numel_of(k)
             n8 = (n + 7) // 8 * 8                        # the tensor's slot in the arena
-            nz = (self.params[off:off + n8] != 0).view(-1, 8)
+            if source is None:
+                nz = (self.params[off:off + n8] != 0).view(-1, 8)
+            else:
+                nz = torch.empty(n8, dtype=torch.bool, device=self.device)
+                nz[:n] = torch.as_tensor(source[k]).to(self.device).reshape(-1) != 0
+                nz = nz.view(-1, 8)
             if n8 > n:
                 nz[-1, n - n8 + 8:] = True
             byte = torch.zeros(n8 // 8, dtype=torch.uint8, device=self.device)
@@ -355,6 +368,37 @@ class Runtime:
             zeros += int((v == 0).sum())
             total += v.numel()
         return zeros, total
+
+    # ---- partial tuning of a pruned model (b200st_optimizer_step_partial, b200st_apply_mask) ---------------------------
+    def partial_setup(self, mask_bitmap):
+        """Partial tuning for the steps that follow (adam_step(frozen=self.partial_frozen)): `mask_bitmap` (device uint8
+        [numel / 8], derive_prune_mask's layout over every tensor) holds 1 where the weight stays frozen, 0 where it is
+        tuned.  -> (tuned, frozen) element counts over the parameter tensors."""
+        if self.numel % 8:
+            raise L.B200STError("partial tuning needs an arena padded to a multiple of 8 elements")
+        m = mask_bitmap
+        if not (torch.is_tensor(m) and m.dtype == torch.uint8 and m.device == self.params.device and m.is_contiguous()
+                and m.numel() == self.numel // 8):
+            raise L.B200STError("partial_setup needs a contiguous uint8 bitmap of %d bytes on %s" % (self.numel // 8, self.device))
+        self.partial_frozen = m
+        return self.mask_counts(m)
+
+    def mask_counts(self, bitmap):
+        """(bits 0, bits 1) over the elements of the parameter tensors of a derive_prune_mask bitmap over every tensor (whose
+        bits outside the tensors are 1)."""
+        popcount = torch.tensor([bin(i).count("1") for i in range(256)], dtype=torch.int64, device=self.device)
+        ones = int(popcount[bitmap.long()].sum())
+        elements = sum(self._numel_of(k) for k in self.table)
+        frozen = ones - (self.numel - elements)
+        return elements - frozen, frozen
+
+    def apply_mask(self, keep):
+        """The weights whose bit of `keep` (derive_prune_mask's layout) is 0 -> 0, in the master arena and in the 16-bit
+        shadow (b200st_apply_mask)."""
+        if not (torch.is_tensor(keep) and keep.dtype == torch.uint8 and keep.numel() == self.numel // 8):
+            raise L.B200STError("apply_mask needs a uint8 bitmap of %d bytes" % (self.numel // 8))
+        L.check(self.lib.b200st_apply_mask(_ptr(self.params), _ptr(self.shadow), self.prec if self.bf16 else L.BF16, _ptr(keep),
+                                           self.numel, L._stream()))
 
     def dropout_mask(self, site, n, p, seed):
         sid = int(self.lib.b200st_dropout_stream_id(site.encode()))

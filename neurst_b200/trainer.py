@@ -51,10 +51,14 @@ class DataParallelTrainer:
 
     def __init__(self, model, optimizer_params=None, lr_schedule_params=None, update_cycle=1, grad_buckets=1,
                  use_cuda_graph=False, clip_value=None, clip_norm=None, summary_steps=0, logger=None, pruning_schedule=None,
-                 pruning_variables=None):
+                 pruning_variables=None, partial_tuning_mask=None):
         """`pruning_schedule` (neurst_b200.pruning, or None): prune the parameters `pruning_variables` (our names; all of them
         when None) during training, as the reference's pruning optimizer does; a schedule with target_sparsity 0 prunes nothing.  The mask is derived from the weights at the
-        first update, after the rank-0 broadcast."""
+        first update, after the rank-0 broadcast.
+        `partial_tuning_mask` (Prune-Tune's partial tuning, or None): "weights" freezes every weight that is not zero, a
+        {our name: 0/1 array} (neurst_b200.prune_tune.load_masks) every element whose mask is 1; only the others are tuned.
+        Like the pruning mask it is set up after the rank-0 broadcast (setup_partial_tuning, at the latest at the first
+        update), so every rank freezes the same elements.  It cannot be combined with a pruning schedule."""
         self.model = model
         self.rt = model.runtime
         op = optimizer_params or {}
@@ -85,6 +89,13 @@ class DataParallelTrainer:
         self.pruning_schedule = pruning_schedule if pruning_schedule is not None and pruning_schedule.target_sparsity > 0 else None
         self.pruning_variables = None if pruning_variables is None else list(pruning_variables)
         self._pruning_ready = False
+        if partial_tuning_mask is not None and not (isinstance(partial_tuning_mask, dict) or partial_tuning_mask == "weights"):
+            raise ValueError("partial_tuning_mask is \"weights\" or a {name: 0/1 array} mapping, got %r" % type(partial_tuning_mask))
+        if partial_tuning_mask is not None and self.pruning_schedule is not None:
+            # the recipe prunes first and tunes afterwards; together, the pruning would re-mask the tuned positions
+            raise ValueError("partial tuning cannot be combined with a pruning schedule")
+        self.partial_tuning_mask = partial_tuning_mask
+        self.partial_counts = None
 
     def close(self):
         """Collective-ordered shutdown of the in-library communicator (call on every rank before leaving the job)."""
@@ -107,6 +118,16 @@ class DataParallelTrainer:
         elif self.dist:
             self.dist.broadcast(self.rt.params, src=0)
             self.rt._shadow_stale = True
+
+    def setup_partial_tuning(self):
+        """Builds the frozen-element bitmap from the current weights or the given masks (once) -> (tuned, frozen) element
+        counts, or None without partial tuning.  Call it after broadcast_parameters."""
+        if self.partial_tuning_mask is None:
+            return None
+        if self.partial_counts is None:
+            source = None if isinstance(self.partial_tuning_mask, str) else self.partial_tuning_mask
+            self.partial_counts = self.rt.partial_setup(self.rt.derive_prune_mask(list(self.rt.table), source))
+        return self.partial_counts
 
     def _allreduce_grads(self):
         if self.dist and not self.lib_comm:        # lib_comm: already reduced inside b200st_train_step, overlapped
@@ -152,6 +173,9 @@ class DataParallelTrainer:
                     self.rt.prune_setup(self.pruning_schedule, names)
                     self._pruning_ready = True
                 kw["prune"] = self.pruning_schedule
+            if self.partial_tuning_mask is not None:
+                self.setup_partial_tuning()
+                kw["frozen"] = self.rt.partial_frozen
             self.rt.adam_step(lr, self.global_step - self.adam_step_base, self.beta1, self.beta2, self.eps, grad_scale=scale, zero_grad=True, **kw)
             if self.meter is not None:
                 self.meter.step_end(self.global_step, out["loss"], lr)
