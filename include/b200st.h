@@ -322,7 +322,9 @@ int b200st_refresh_shadow(const float* params, void* shadow, int32_t shadow_dtyp
  * (neurst/training/revised_dynamic_loss_scale.py:60-107): device float[8] = {scale, finite steps in a row, last step skipped,
  * skipped steps, applied steps, global gradient norm, 1/scale latch, reserved}; a step whose gradients are not all finite
  * is skipped (parameters untouched, gradients zeroed) and halves the scale; `growth_steps` finite steps double it.
- * h may be NULL (whole arena = one tensor). tensor_sumsq: device float[param_count + 1] scratch (clip_norm / loss scale). */
+ * h may be NULL (whole arena = one tensor); numel must then be a multiple of 8, as every arena the library lays out is
+ * (refused otherwise, before any launch).  clip_value keeps a NaN gradient NaN, as tf.clip_by_value does.
+ * tensor_sumsq: device float[param_count + 1] scratch (clip_norm / loss scale). */
 typedef struct b200st_optim_args_ {
   float* params; float* grads; float* m; float* v;
   void* shadow; int32_t shadow_dtype;
@@ -386,7 +388,8 @@ int b200st_optimizer_step_partial(b200st_handle h, const b200st_optim_args* a, c
  * bit of `keep` (same layout) is 0.  n: a multiple of 8. */
 int b200st_apply_mask(float* params, void* shadow, int shadow_dtype, const uint8_t* keep, int64_t n, void* stream);
 /* legacy form: plain Keras Adam with a bf16 shadow, epsilon-hat form (neurst/optimizers/__init__.py:21; hparams speech_transformer.py:265-270):
- * g' = g*grad_scale; m,v update; p -= lr*sqrt(1-b2^t)/(1-b1^t) * m/(sqrt(v)+eps); optional bf16 shadow refresh + g=0 */
+ * g' = g*grad_scale; m,v update; p -= lr*sqrt(1-b2^t)/(1-b1^t) * m/(sqrt(v)+eps); optional bf16 shadow refresh + g=0.
+ * numel: a multiple of 8. */
 int b200st_adam_step(float* params, float* grads, float* m, float* v, void* shadow, int64_t numel, float lr, float beta1,
                      float beta2, float eps, int64_t step_t, float grad_scale, int32_t zero_grad, void* stream);
 

@@ -85,8 +85,18 @@ def archive_scope(keys, table):
     return scopes.pop() if len(scopes) == 1 else model_scope(table)
 
 
+# The dynamic loss scale's state beside the Adam slots (the reference checkpoints the LossScaleOptimizer's loss-scale
+# variables and its iterations with the model): {archive key: word of Runtime.loss_scale_state}.  Word 4, the updates
+# applied on the device, is Adam's t under the dynamic loss scale.  The keys carry `/.OPTIMIZER_SLOT/`, so every reader
+# that tells optimizer state from variables by it (archive_scope, strict and pattern restores) skips them.
+LOSS_SCALE_KEYS = {"optimizer/.OPTIMIZER_SLOT/loss_scale/current_loss_scale": 0,
+                   "optimizer/.OPTIMIZER_SLOT/loss_scale/good_steps": 1,
+                   "optimizer/.OPTIMIZER_SLOT/iterations": 4}
+
+
 def save_npz(rt, path, scope=None, extra=None):
-    """Writes every parameter under its reference variable name (+ optional Adam slots as `<name>/.OPTIMIZER_SLOT/{m,v}`)."""
+    """Writes every parameter under its reference variable name (+ optional Adam slots as `<name>/.OPTIMIZER_SLOT/{m,v}`,
+    + the dynamic loss scale's state under LOSS_SCALE_KEYS when the runtime has one)."""
     names = tf_variable_names(rt.table, scope)
     arrays = {names[k]: rt.view(k).detach().cpu().numpy() for k in rt.table}
     if extra:
@@ -95,6 +105,11 @@ def save_npz(rt, path, scope=None, extra=None):
         for k in rt.table:
             arrays[names[k] + "/.OPTIMIZER_SLOT/m"] = rt.view(k, rt.adam_m).detach().cpu().numpy()
             arrays[names[k] + "/.OPTIMIZER_SLOT/v"] = rt.view(k, rt.adam_v).detach().cpu().numpy()
+    state = getattr(rt, "loss_scale_state", None)
+    if state is not None:
+        words = state.detach().cpu().numpy()
+        for key, i in LOSS_SCALE_KEYS.items():
+            arrays[key] = words[i:i + 1].copy()
     np.savez(path, **arrays)
     return sorted(arrays)
 
@@ -104,7 +119,8 @@ def load_npz(rt, path, scope=None, strict=True, pattern=None, slots=True):
     `pattern`: restore only the variables whose name in THIS model (its own scope) matches the regular expression
     (re.search), each read from the archive under the archive's scope (restore_checkpoint_if_possible,
     checkpoints.py:340-360); the Adam slots are then left alone, as they are with `slots=False` (pretraining restores the
-    model's weights only)."""
+    model's weights only).  The loss-scale state is restored with the slots, into the runtime's existing tensor in place
+    (captured CUDA graphs hold its pointer); an archive without it leaves the runtime's state as it is."""
     z = np.load(path)
     keys = [k for k in z.files if "/.OPTIMIZER_SLOT/" not in k]
     if scope is None:
@@ -128,6 +144,10 @@ def load_npz(rt, path, scope=None, strict=True, pattern=None, slots=True):
         for k in rt.table:
             rt.view(k, rt.adam_m).copy_(torch.from_numpy(z[names[k] + "/.OPTIMIZER_SLOT/m"]))
             rt.view(k, rt.adam_v).copy_(torch.from_numpy(z[names[k] + "/.OPTIMIZER_SLOT/v"]))
+    state = getattr(rt, "loss_scale_state", None)
+    if slots and pattern is None and state is not None and all(key in z.files for key in LOSS_SCALE_KEYS):
+        for key, i in LOSS_SCALE_KEYS.items():
+            state[i:i + 1].copy_(torch.from_numpy(np.asarray(z[key], dtype=np.float32).reshape(1)))
     return sorted(P)
 
 

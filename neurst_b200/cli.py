@@ -932,6 +932,8 @@ def train(plan):
         # only the lr schedule, the checkpoints and validation read the initial step (compat.register_initial_step); the
         # optimizer's iterations start at 0 in this run, so Adam's bias correction counts this run's updates from t = 1
         trainer.adam_step_base = igs
+        if model.runtime.loss_scale_state is not None:
+            model.runtime.loss_scale_state[4] = 0.0       # the dynamic loss scale's t: the updates applied in this run
 
     def log_sparsity():
         if schedule is not None and trainer._pruning_ready:

@@ -326,6 +326,10 @@ int b200st_optimizer_step(b200st_handle h, const b200st_optim_args* a, void* str
   if (h) {
     if (a->numel != h->m.arena_numel) B200ST_FAIL("numel does not match the handle's parameter arena");
     fill_tensor_table(h->m, tt);
+  } else if (a->numel % 8 != 0) {
+    // the Adam pass moves 4-element vectors and the statistics pass assumes 8-element tensor slots: an unpadded tail
+    // would be left without its update
+    B200ST_FAIL("numel must be a multiple of 8 (pad the arena)");
   } else if (a->clip_norm > 0.f || a->loss_scale_state) {
     // no handle: the whole arena is one tensor
     tt.n = 1; tt.off8[0] = 0; tt.off8[1] = (uint32_t)((a->numel + 7) >> 3);

@@ -130,8 +130,9 @@ __global__ void __launch_bounds__(256) adam_kernel(const OptimArgs a, const __gr
     }
     float gi[4] = {g4.x * sc, g4.y * sc, g4.z * sc, g4.w * sc};
     if (a.clip_value > 0.f) {
+      // tf.clip_by_value keeps a NaN (its minimum / maximum propagate it); fminf / fmaxf would return the bound instead
 #pragma unroll
-      for (int j = 0; j < 4; ++j) gi[j] = fminf(fmaxf(gi[j], -a.clip_value), a.clip_value);
+      for (int j = 0; j < 4; ++j) gi[j] = gi[j] > a.clip_value ? a.clip_value : (gi[j] < -a.clip_value ? -a.clip_value : gi[j]);
     }
     const float mo[4] = {m4.x, m4.y, m4.z, m4.w}, vo[4] = {v4.x, v4.y, v4.z, v4.w}, po[4] = {p4.x, p4.y, p4.z, p4.w};
     float mi[4], vi[4], pi[4];

@@ -258,7 +258,7 @@ class Runtime:
         a.numel = self.numel
         a.lr, a.beta1, a.beta2, a.eps = lr, beta1, beta2, eps
         a.step_t, a.grad_scale, a.zero_grad = int(step_t), grad_scale, int(zero_grad)
-        a.clip_value = float(clip_value or 0.0)
+        a.clip_value = abs(float(clip_value or 0.0))      # GradAccumKerasModel takes abs(clip_value)
         a.clip_norm = float(clip_norm or 0.0)
         if dyn or a.clip_norm > 0:
             if self.tensor_sumsq is None:

@@ -113,7 +113,17 @@ def _write_dataset(root, n_shards=3, per_shard=70, vocab=90):
 
 
 @pytest.mark.gpu
-def test_train_resume_predict_through_the_entry(tmp_path):
+def test_train_resume_predict_through_the_entry(tmp_path, monkeypatch):
+    from neurst_b200 import checkpoints as CK
+    from neurst_b200.runtime import Runtime
+    states = []              # the fp16 loss-scale state (scale, finite steps, last skipped, skips, applied updates) around each update
+    adam_step = Runtime.adam_step
+
+    def recording(rt, *a, **kw):
+        before = rt.loss_scale_state[:5].tolist()
+        adam_step(rt, *a, **kw)
+        states.append((before, rt.loss_scale_state[:5].tolist()))
+    monkeypatch.setattr(Runtime, "adam_step", recording)
     n = _write_dataset(tmp_path, vocab=93)                          # 93 tokens + 3 symbols = 96: the 16-bit path needs vocab % 8 == 0
     y = _write_yaml(tmp_path, data=str(tmp_path / "train.tfrecords"), n_tokens=93)
     model_dir = str(tmp_path / "model")
@@ -132,8 +142,12 @@ def test_train_resume_predict_through_the_entry(tmp_path):
     assert idx["model_checkpoint_path"] == "ckpt-6.npz"
     z = np.load(os.path.join(model_dir, "ckpt-6.npz"))
     assert any(k.startswith("SpeechTransformer/TransformerEncoder/layer_0/") for k in z.files) and any("/.OPTIMIZER_SLOT/m" in k for k in z.files)
+    saved = [float(z[k][0]) for k in CK.LOSS_SCALE_KEYS]         # the default dtype float16: scale, finite steps, applied updates
+    assert len(states) == 6 and [states[5][1][i] for i in (0, 1, 4)] == saved
     res = cli.main(common + ["--train_steps", "8"])                 # resumes at 6 (parameters, Adam slots, schedule position)
     assert res["global_step"] == 8 and os.path.exists(os.path.join(model_dir, "ckpt-8.npz"))
+    # ... and the loss-scale state: the resumed run's first update starts from the one ckpt-6 saved
+    assert len(states) == 8 and [states[6][0][i] for i in (0, 1, 4)] == saved, (states[6][0], saved)
     out = str(tmp_path / "hyp.txt")
     one = tmp_path / "one"
     one.mkdir()

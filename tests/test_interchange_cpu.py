@@ -62,6 +62,42 @@ def test_npz_round_trip(tmp_path):
         CK.load_npz(b, str(tmp_path / "bad.npz"))
 
 
+def test_npz_round_trip_of_the_loss_scale_state(tmp_path):
+    """The dynamic loss scale's scale, finite-step count and applied-update count (Adam's t) travel with the Adam slots,
+    into the runtime's own state tensor in place; they are no variables (scope detection, strict and pattern restores are
+    unchanged), and a restore without slots, by pattern, or from an archive without them keeps the runtime's state."""
+    cfg = R.CONFIGS["speech_transformer_toy"]
+    a = _FakeRT(cfg, 1)
+    a.adam_m, a.adam_v = torch.rand_like(a.params), torch.rand_like(a.params)
+    a.loss_scale_state = torch.tensor([2.0 ** 13, 5, 0, 2, 41, 3.5, 2.0 ** -13, 0])
+    p = str(tmp_path / "ckpt.npz")
+    keys = CK.save_npz(a, p, scope="MyScope")
+    z = np.load(p)
+    assert sorted(CK.LOSS_SCALE_KEYS) == sorted(k for k in keys if not k.startswith("MyScope/"))
+    assert [float(z[k][0]) for k in CK.LOSS_SCALE_KEYS] == [2.0 ** 13, 5.0, 41.0]
+
+    def fresh():
+        b = _FakeRT(cfg, 2)
+        b.loss_scale_state = torch.tensor([2.0 ** 15, 0, 0, 0, 0, 0, 0, 0])
+        return b
+    b = fresh()
+    state = b.loss_scale_state
+    assert CK.load_npz(b, p) == sorted(a.table)               # strict: every variable, nothing else
+    assert b.loss_scale_state is state
+    assert state.tolist() == [2.0 ** 13, 5, 0, 0, 41, 0, 0, 0]
+    for kw in (dict(slots=False), dict(pattern="TransformerEncoder", strict=False)):
+        b = fresh()
+        CK.load_npz(b, p, **kw)
+        assert b.loss_scale_state.tolist() == [2.0 ** 15, 0, 0, 0, 0, 0, 0, 0], kw
+    a.loss_scale_state = None                                   # bf16 / fp32 runtimes have no such state
+    CK.save_npz(a, p)
+    assert not set(CK.LOSS_SCALE_KEYS) & set(np.load(p).files)
+    b = fresh()
+    CK.load_npz(b, p)
+    assert b.loss_scale_state.tolist() == [2.0 ** 15, 0, 0, 0, 0, 0, 0, 0]
+    assert torch.equal(b.view("enc.0.ffn.w1", b.adam_m), a.view("enc.0.ffn.w1", a.adam_m))
+
+
 def _reference_root():
     """The reference tree when it is installed, else the copy staged under oracle/_ref by build(), else None."""
     if os.path.isdir(REF):
