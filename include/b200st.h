@@ -313,6 +313,53 @@ typedef struct {
 } b200st_ensemble_member;
 int b200st_ensemble_beam_search(const b200st_ensemble_member* members, int32_t n_members, const b200st_beam_args* a, void* stream);
 
+/* Streaming simultaneous translation: the wait-k agent's read / write loop on one source stream (SimulTransTextAgent,
+ * neurst/utils/simuleval_agents/simul_trans_text_agent.py; WaitkTransformer.incremental_encode / incremental_decode,
+ * neurst/models/waitk_transformer.py:119-140).  A session decodes one stream with 1..B200ST_ENSEMBLE_MAX_MODELS text
+ * Transformer members with a monotonic encoder (encoder_monotonic = 1), sharing the target vocabulary and d.
+ *   Per member, caller-owned device buffers (nothing is allocated on the device after set-up):
+ *     enc_kv   fp32 [enc_layers][2][max_src][d]: each encoder layer's self-attention keys / values
+ *     cross_kv fp32 [dec_layers][max_src][2d]: the memory keys | values, appended as the source grows
+ *     self_kv  fp32 [dec_layers][2][max_trg][d]
+ *     enc_out  optional fp32 [max_src][d]: the encoder output rows (after its final LayerNorm), NULL: not written
+ *     scratch  b200st_stream_scratch_floats(h) floats
+ *   use_shadow as for b200st_decode_state: 1 reads the embeddings, the attention projections (qkv / q / out) and the FFN
+ *   kernels of both stacks from the 16-bit shadow; the cross K/V projection, biases and LayerNorm parameters always come from
+ *   the master arena, and all arithmetic is fp32.
+ *   lens_dev: device int32[2] = {src_len (source ids encoded), trg_len (decoder positions used)}, caller-owned; the session
+ *   keeps host mirrors of both to check calls before anything is launched.
+ * b200st_stream_read appends n >= 1 source ids (device int64 [n]) at positions src_len .. src_len + n - 1 for every member:
+ *   embedding + sinusoid at the absolute positions, each encoder layer (the new rows attend causally to the cached keys and
+ *   to each other), the final LayerNorm, and each decoder layer's cross K/V of the new rows; then src_len += n.
+ * b200st_stream_write runs one decoder step per member at position trg_len on the symbol in *out_id_dev, attending to the
+ *   memory [0, src_len) with no lag mask; mixes the members' log-probabilities (weights NULL: equal, the agent's
+ *   logsumexp_m(log_softmax_m) - log n; otherwise normalised to sum 1; one member: log_softmax); takes the argmax (lower index
+ *   on ties, no UNK or minimum-length mask); writes the id to *out_id_dev (the next step's symbol) and sets trg_len += 1.  The
+ *   step is captured once into a CUDA graph (again when out_id_dev or the weights change) and replayed: `stream` must be a
+ *   stream that can capture (not capturing already, not the legacy default stream).
+ * Invalid calls fail before anything is launched: src_len + n > max_src, trg_len == max_trg, a write before any read,
+ * members with different vocabularies or d, a handle without a monotonic encoder. */
+typedef struct {
+  int32_t max_src, max_trg;
+  float* enc_kv; float* cross_kv; float* self_kv; float* enc_out;
+  float* scratch;
+  int32_t use_shadow;
+} b200st_stream_state;
+typedef struct {
+  b200st_handle h; const b200st_buffers* buf; const b200st_stream_state* st;
+} b200st_stream_member;
+typedef struct b200st_stream_session* b200st_stream;
+int64_t b200st_stream_scratch_floats(b200st_handle h);
+/* host object only; the members' buffers must outlive it */
+int b200st_stream_create(const b200st_stream_member* members, int32_t n_members, int32_t* lens_dev, b200st_stream* out);
+int b200st_stream_destroy(b200st_stream s);
+/* zeroes src_len and trg_len (the caches need no clearing: the lengths bound every read of them) */
+int b200st_stream_reset(b200st_stream s, void* stream);
+int b200st_stream_read(b200st_stream s, int32_t n, const int64_t* ids, void* stream);
+int b200st_stream_write(b200st_stream s, const float* weights, int64_t* out_id_dev, void* stream);
+/* the host mirrors of src_len and trg_len */
+int b200st_stream_lengths(b200st_stream s, int32_t* src_len, int32_t* trg_len);
+
 /* 16-bit shadow of the parameter arena (wgmma operands); shadow_dtype = B200ST_BF16 or B200ST_F16 */
 int b200st_refresh_shadow(const float* params, void* shadow, int32_t shadow_dtype, int64_t numel, void* stream);
 

@@ -40,6 +40,7 @@ import logging
 import os
 import re
 import sys
+import time
 
 import torch
 
@@ -357,6 +358,8 @@ def resolve(cfg, world=1):
     from neurst_b200.models import speech_transformer_hparams, transformer_hparams, waitk_transformer_hparams
     if str(_module_name(cfg, "entry") or "").lower().replace("_", "") == "cascadest":
         return resolve_cascade(cfg, world)
+    if str(_module_name(cfg, "entry") or "").lower().replace("_", "") == "simuleval":
+        return resolve_simuleval(cfg, world)
     ep, tp = dict(cfg.get("entry.params") or {}), dict(cfg.get("task.params") or {})
     task_cls = str(cfg.get("task.class", "SpeechToText")).lower().replace("_", "")
     waitk = task_cls in WAITK_TASKS
@@ -513,6 +516,59 @@ def resolve_cascade(cfg, world=1):
     return {"entry": "cascade_st", "asr": plans["asr"], "mt": plans["mt"], "batch_size": batch_size,
             "translation_key": dsp.get("translation_key", "translation"), "metrics": metrics,
             "asr_output_file": get("asr_output_file"), "mt_output_file": get("mt_output_file")}
+
+
+def resolve_simuleval(cfg, world=1):
+    """The `simuleval` entry: SimulEval's text-to-text evaluation of SimulTransTextAgent, replayed offline on the device
+    (neurst/utils/simuleval_agents/simul_trans_text_agent.py; examples/iwslt21/SIMUL_TRANS.md).  model_dir: one or more
+    WaitkTransformer directories (an ensemble mixed as the agent mixes it); wait_k (source words) from the command line
+    overrides model_configs.yml, as build_task_and_model does; source: pre-tokenised (BPE) source lines; target: reference
+    lines; output: the directory of instances.log and scores."""
+    if world > 1:
+        raise SystemExit("simuleval runs on one device (WORLD_SIZE 1)")
+    ep = dict(cfg.get("entry.params") or {})
+
+    def get(key, default=None):
+        v = cfg.get(key, ep.get(key))
+        return default if v is None else v
+
+    model_dirs = flatten_string_list(get("model_dir"))
+    if not model_dirs:
+        raise SystemExit("simuleval needs --model_dir (one or more WaitkTransformer directories)")
+    if len(model_dirs) > 8:
+        raise SystemExit("simuleval mixes at most 8 models, got %d" % len(model_dirs))
+    k = get("wait_k")
+    if k is None or isinstance(k, bool) or not str(k).strip().isdigit() or int(k) < 1:
+        raise SystemExit("simuleval needs --wait_k, a positive number of source words, got %r" % (k,))
+    for key in ("source", "output"):
+        if not get(key):
+            raise SystemExit("simuleval needs --%s" % key)
+    members, trg_tokens = [], None
+    for d in model_dirs:
+        configs = _model_dir_configs(d, "model_dir")
+        if str(configs.get("model.class")) != "WaitkTransformer":
+            raise SystemExit("model_dir %s holds a %s, not a wait-k model (WaitkTransformer): the agent streams a monotonic "
+                             "encoder" % (d, configs.get("model.class")))
+        tp = dict(configs["task.params"], wait_k=int(k))
+        lang = (tp.get("trg_data_pipeline.params") or {}).get("language")
+        if str(lang).lower() == "ja":
+            raise SystemExit("simuleval: the agent's Japanese target branch (one character per segment) is outside this path")
+        sub = {"entry.class": "predict", "model_dir": d, "dtype": get("dtype", "float32"), "task.class": "WaitkTranslation",
+               "task.params": tp, "model.class": "WaitkTransformer", "model.params": configs.get("model.params") or {},
+               "hparams_set": "waitk_transformer_s", "wait_k": int(k),
+               "dataset.params": {"src_file": get("source"), "data_is_processed": True}}
+        plan = resolve(sub)
+        if trg_tokens is None:
+            trg_tokens = plan["trg_meta"]["tokens"]
+        elif plan["trg_meta"]["tokens"] != trg_tokens:
+            raise SystemExit("model_dir %s has a target vocabulary that differs from %s's: the agent mixes the members' "
+                             "distributions over one vocabulary" % (d, model_dirs[0]))
+        members.append(plan)
+    force = get("force_segment", False)
+    if isinstance(force, str):
+        force = force.strip().lower() in ("1", "true", "yes", "on")
+    return {"entry": "simuleval", "members": members, "wait_k": int(k), "force_segment": bool(force),
+            "max_len": int(get("max_len", 200)), "source": get("source"), "target": get("target"), "output": get("output")}
 
 
 def _pretrain_patterns(ep):
@@ -1256,6 +1312,59 @@ def cascade_st(plan):
     return res
 
 
+def simuleval(plan):
+    """Streams every source line through SimulTransTextAgent word by word on the device (simultaneous.py) and writes
+    <output>/instances.log (one JSON line per sentence: prediction, delays in source words, the device time of each action)
+    and <output>/scores (BLEU from metrics, and AL / AP / DAL of the measured delays from metrics.simul_latency)."""
+    from neurst_b200.metrics import build_metric, simul_latency
+    from neurst_b200.simultaneous import SimulTransTextAgent, StreamingSession, words_of
+    _dist_setup()
+    models = [_restore(p, p["model_dir"])[0] for p in plan["members"]]
+    first = plan["members"][0]
+    with open(plan["source"], encoding="utf-8") as f:
+        sources = [l.rstrip("\n") for l in f]
+    # the source with the EOS of a forced segment and the final one; the target up to the agent's max_len + 1 units
+    max_src = max([len(l.split()) for l in sources] + [1]) + 2
+    session = StreamingSession(models, use_shadow=first["precision"] != "fp32", max_src=max_src, max_trg=plan["max_len"] + 2)
+    agent = SimulTransTextAgent(session, first["src_meta"], first["trg_meta"], plan["wait_k"], plan["force_segment"], plan["max_len"])
+    bow = any(t.startswith("\u2581") for t in first["src_meta"]["tokens"] or [])
+    refs = None
+    if plan.get("target"):
+        with open(plan["target"], encoding="utf-8") as f:
+            refs = [l.rstrip("\n") for l in f]
+
+    def clock():
+        torch.cuda.synchronize()
+        return time.perf_counter()
+
+    os.makedirs(plan["output"], exist_ok=True)
+    hyps, lat = [], []
+    with open(os.path.join(plan["output"], "instances.log"), "w", encoding="utf-8") as f:
+        for i, line in enumerate(sources):
+            words = words_of(line, bow)
+            r = agent.translate(words, clock=clock)
+            hyp = " ".join(r["prediction"])
+            hyps.append(hyp)
+            row = {"index": i, "prediction": hyp, "delays": r["delays"], "source_length": len(words),
+                   "action_seconds": [[a, round(t, 7)] for a, t in r["actions"]]}
+            if refs is not None:
+                row["reference"] = refs[i]
+            m = simul_latency(r["delays"], len(words))
+            if m is not None:
+                lat.append(m)
+                row.update(m)
+            f.write(json.dumps(row) + "\n")
+    scores = {"n_sentences": len(hyps)}
+    for key in ("AL", "AP", "DAL"):
+        scores[key] = sum(m[key] for m in lat) / len(lat) if lat else None
+    if refs is not None:
+        scores["BLEU"] = build_metric("bleu", "en")(hyps, refs)
+    with open(os.path.join(plan["output"], "scores"), "w", encoding="utf-8") as f:
+        f.write(json.dumps(scores, indent=2) + "\n")
+    LOG.info("simuleval: %s", json.dumps(scores))
+    return dict(scores, hypotheses=hyps)
+
+
 def _pad_audio(plan, group):
     dim = plan["task"]["audio_feature_dim"] * plan["task"]["audio_feature_channels"]
     src = torch.zeros(len(group), max(int(e["audio_length"]) for e in group), dim)
@@ -1273,6 +1382,8 @@ def main(argv=None):
         res = train(plan)
         if "validations" in res:
             res["validations"] = [{k: v for k, v in r.items() if k != "hypotheses"} for r in res["validations"]]
+    elif plan["entry"] == "simuleval":
+        res = {k: v for k, v in simuleval(plan).items() if k != "hypotheses"}
     elif plan["entry"] == "cascade_st":
         res = cascade_st(plan)
         res = {k: v for k, v in res.items() if not k.endswith("_hypotheses")}

@@ -300,6 +300,53 @@ int b200st_ensemble_beam_search(const b200st_ensemble_member* members, int32_t n
   }
   return ensemble_beam_search(em, n_members, to_beam_args(a), reinterpret_cast<cudaStream_t>(stream));
 }
+struct b200st_stream_session { StreamSession* s; };
+int64_t b200st_stream_scratch_floats(b200st_handle h) { return h ? stream_scratch_floats(h->m) : -1; }
+int b200st_stream_create(const b200st_stream_member* members, int32_t n_members, int32_t* lens_dev, b200st_stream* out) {
+  if (!members || !out || !lens_dev) B200ST_FAIL("null argument");
+  if (n_members < 1 || n_members > B200ST_ENSEMBLE_MAX_MODELS)
+    B200ST_FAIL("a streaming session has 1.." + std::to_string(B200ST_ENSEMBLE_MAX_MODELS) + " members, got " + std::to_string(n_members));
+  StreamMember sm[B200ST_ENSEMBLE_MAX_MODELS];
+  for (int i = 0; i < n_members; ++i) {
+    const b200st_stream_member& x = members[i];
+    if (!x.h || !x.buf || !x.st) B200ST_FAIL("stream member " + std::to_string(i) + ": null argument");
+    StreamState st{};
+    st.max_src = x.st->max_src; st.max_trg = x.st->max_trg;
+    st.enc_kv = x.st->enc_kv; st.cross_kv = x.st->cross_kv; st.self_kv = x.st->self_kv; st.enc_out = x.st->enc_out;
+    st.scratch = x.st->scratch; st.use_shadow = x.st->use_shadow;
+    sm[i] = StreamMember{&x.h->m, to_buffers(x.buf), st};
+  }
+  StreamSession* s = nullptr;
+  B200ST_TRY(stream_create(sm, n_members, lens_dev, &s));
+  *out = new b200st_stream_session{s};
+  return 0;
+}
+int b200st_stream_destroy(b200st_stream s) {
+  if (!s) B200ST_FAIL("null argument");
+  stream_destroy(s->s);
+  delete s;
+  return 0;
+}
+int b200st_stream_reset(b200st_stream s, void* stream) {
+  if (!s) B200ST_FAIL("null argument");
+  return stream_reset(s->s, reinterpret_cast<cudaStream_t>(stream));
+}
+int b200st_stream_read(b200st_stream s, int32_t n, const int64_t* ids, void* stream) {
+  if (!s) B200ST_FAIL("null argument");
+  return stream_read(s->s, n, ids, reinterpret_cast<cudaStream_t>(stream));
+}
+int b200st_stream_write(b200st_stream s, const float* weights, int64_t* out_id_dev, void* stream) {
+  if (!s) B200ST_FAIL("null argument");
+  return stream_write(s->s, weights, out_id_dev, reinterpret_cast<cudaStream_t>(stream));
+}
+int b200st_stream_lengths(b200st_stream s, int32_t* src_len, int32_t* trg_len) {
+  if (!s) B200ST_FAIL("null argument");
+  int a = 0, b = 0;
+  stream_lengths(s->s, &a, &b);
+  if (src_len) *src_len = a;
+  if (trg_len) *trg_len = b;
+  return 0;
+}
 int b200st_refresh_shadow(const float* params, void* shadow, int32_t shadow_dtype, int64_t numel, void* stream) {
   if (!params || !shadow) B200ST_FAIL("null argument");
   return cast_f32_to_16(params, shadow, shadow_dtype, numel, reinterpret_cast<cudaStream_t>(stream));

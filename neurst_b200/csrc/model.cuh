@@ -187,4 +187,28 @@ struct EnsembleMember {
 // beam_search over the weighted mixture of n members' next-token distributions, one beam state for all members
 int ensemble_beam_search(const EnsembleMember* members, int n, const BeamArgs& a, cudaStream_t s);
 
+// ---- streaming simultaneous translation (stream.cu) ------------------------------------------------------------------
+struct StreamState {
+  int max_src, max_trg;
+  float* enc_kv;                 // [enc_layers][2][max_src][d] fp32: each encoder layer's self-attention keys / values
+  float* cross_kv;               // [dec_layers][max_src][2d] fp32: memory keys | values
+  float* self_kv;                // [dec_layers][2][max_trg][d] fp32
+  float* enc_out;                // optional [max_src][d] fp32: the encoder output rows (final LayerNorm)
+  float* scratch;                // stream_scratch_floats() floats
+  int use_shadow;
+};
+struct StreamMember {
+  const Model* m;
+  Buffers buf;
+  StreamState st;
+};
+struct StreamSession;
+int64_t stream_scratch_floats(const Model& m);
+int stream_create(const StreamMember* members, int n, int32_t* lens_dev, StreamSession** out);
+void stream_destroy(StreamSession* s);
+int stream_reset(StreamSession* s, cudaStream_t st);
+int stream_read(StreamSession* s, int n, const int64_t* ids, cudaStream_t st);
+int stream_write(StreamSession* s, const float* weights, int64_t* out_id, cudaStream_t st);
+void stream_lengths(const StreamSession* s, int* src_len, int* trg_len);
+
 }  // namespace b200st

@@ -234,6 +234,16 @@ class SamplingArgs(C.Structure):
 ENSEMBLE_MAX_MODELS = 8    # B200ST_ENSEMBLE_MAX_MODELS
 
 
+class StreamState(C.Structure):
+    _fields_ = [("max_src", C.c_int32), ("max_trg", C.c_int32),
+                ("enc_kv", C.c_void_p), ("cross_kv", C.c_void_p), ("self_kv", C.c_void_p), ("enc_out", C.c_void_p),
+                ("scratch", C.c_void_p), ("use_shadow", C.c_int32)]
+
+
+class StreamMember(C.Structure):
+    _fields_ = [("h", C.c_void_p), ("buf", C.POINTER(Buffers)), ("st", C.POINTER(StreamState))]
+
+
 class CascadeSourceArgs(C.Structure):
     _fields_ = [("hyp_ids", C.c_void_p), ("B", C.c_int32), ("hyp_len", C.c_int32), ("hyp_stride", C.c_int32),
                 ("asr_eos_id", C.c_int32), ("asr_vocab", C.c_int32), ("remap", C.c_void_p),
@@ -256,7 +266,9 @@ EXPORTS = [
     "b200st_comm_unique_id", "b200st_comm_init", "b200st_comm_broadcast", "b200st_comm_destroy", "b200st_comm_stats", "b200st_train_step",
     "b200st_encode", "b200st_encode_workspace_bytes", "b200st_decode_scratch_floats", "b200st_decode_init", "b200st_decode_step",
     "b200st_greedy_search", "b200st_greedy_used_graph", "b200st_beam_state_bytes", "b200st_beam_search",
-    "b200st_ensemble_beam_search", "b200st_sampling_search", "b200st_sample_logits", "b200st_cascade_source",
+    "b200st_ensemble_beam_search", "b200st_sampling_search",
+    "b200st_stream_scratch_floats", "b200st_stream_create", "b200st_stream_destroy", "b200st_stream_reset", "b200st_stream_read",
+    "b200st_stream_write", "b200st_stream_lengths", "b200st_sample_logits", "b200st_cascade_source",
     "b200st_encoder_forward", "b200st_decoder_forward", "b200st_mha_forward", "b200st_lsce", "b200st_layernorm_fwd",
     "b200st_layernorm_bwd", "b200st_softmax_fwd", "b200st_conv1_ln_relu_fwd", "b200st_dropout_stream_id", "b200st_dropout_mask",
 ]
@@ -309,6 +321,14 @@ def _declare(lib):
                                            C.c_void_p]
     lib.b200st_sample_logits.argtypes = [C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_float, C.c_uint64, C.c_int64, C.c_int32,
                                          C.c_void_p, C.c_void_p]
+    lib.b200st_stream_scratch_floats.restype = C.c_int64
+    lib.b200st_stream_scratch_floats.argtypes = [C.c_void_p]
+    lib.b200st_stream_create.argtypes = [C.POINTER(StreamMember), C.c_int32, C.c_void_p, C.POINTER(C.c_void_p)]
+    lib.b200st_stream_destroy.argtypes = [C.c_void_p]
+    lib.b200st_stream_reset.argtypes = [C.c_void_p, C.c_void_p]
+    lib.b200st_stream_read.argtypes = [C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p]
+    lib.b200st_stream_write.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]
+    lib.b200st_stream_lengths.argtypes = [C.c_void_p, C.POINTER(C.c_int32), C.POINTER(C.c_int32)]
     lib.b200st_cascade_source.argtypes = [C.POINTER(CascadeSourceArgs), C.c_void_p]
     lib.b200st_adam_step.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64, C.c_float,
                                      C.c_float, C.c_float, C.c_float, C.c_int64, C.c_float, C.c_int32, C.c_void_p]
