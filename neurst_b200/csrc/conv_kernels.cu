@@ -17,6 +17,8 @@
 #include "kernels.cuh"
 #include "pdl.cuh"
 
+#include <type_traits>
+
 namespace b200st {
 
 namespace {
@@ -501,65 +503,252 @@ __global__ void __launch_bounds__(256, (CPL <= 8 ? 2 : 1)) conv1_bwd_fused_kerne
 // 1/sigma read back (no convolution recompute, no statistics), db/dgamma/dbeta partials, and dz1 + fbank im2col rows for the
 // dW1 GEMM (or, IMPLICIT, dW1 itself).
 // ---------------------------------------------------------------------------------------------
-// IMPLICIT: `dcol` is the class-major tiled input gradient written by the implicit conv2 data-gradient GEMMs
+// m16n8k16 tensor-core product of 16-bit operands with fp32 accumulation: d += a b (a: 16 x 16 row-major fragment, b: 16 x 8
+// column fragment, layouts of the PTX ISA).
+template <typename T>
+__device__ __forceinline__ void mma_16816(float (&d)[4], const uint32_t (&a)[4], uint32_t b0, uint32_t b1) {
+  if constexpr (std::is_same<T, __half>::value)
+    asm volatile("mma.sync.aligned.m16n8k16.row.col.f32.f16.f16.f32 {%0, %1, %2, %3}, {%4, %5, %6, %7}, {%8, %9}, {%0, %1, %2, %3};"
+                 : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]) : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "r"(b0), "r"(b1));
+  else
+    asm volatile("mma.sync.aligned.m16n8k16.row.col.f32.bf16.bf16.f32 {%0, %1, %2, %3}, {%4, %5, %6, %7}, {%8, %9}, {%0, %1, %2, %3};"
+                 : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]) : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "r"(b0), "r"(b1));
+}
+__device__ __forceinline__ void ldmatrix_x4(uint32_t (&r)[4], const void* p) {
+  asm volatile("ldmatrix.sync.aligned.m8n8.x4.shared.b16 {%0, %1, %2, %3}, [%4];"
+               : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]) : "r"((uint32_t)__cvta_generic_to_shared(p)));
+}
+__device__ __forceinline__ void ldmatrix_x4_trans(uint32_t (&r)[4], const void* p) {
+  asm volatile("ldmatrix.sync.aligned.m8n8.x4.trans.shared.b16 {%0, %1, %2, %3}, [%4];"
+               : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]) : "r"((uint32_t)__cvta_generic_to_shared(p)));
+}
+
+// IMPLICIT: `dcol` is the class-major tiled input gradient written by the implicit conv2 data-gradient GEMM
 // (tc_gemm.cu: conv2_dgrad_implicit) — one row per position instead of up to four tap rows to gather — and conv1's filter
-// gradient dW1[tap][c] += src_tap * dz1[c] is accumulated here (fp32, with the 16-bit rounding of both factors that the
-// explicit GEMM over col1 / dz1 applied), so neither dz1 nor col1 is written.  Its 72 accumulators per lane do not fit the
-// 128-register budget of two CTAs per SM: one CTA per SM, with a twice deeper load ring to keep the same bytes in flight.
+// gradient dW1[tap][c] = sum over positions of src_tap * dz1[c] is computed here, with the 16-bit rounding of both factors
+// that the explicit GEMM over col1 / dz1 applied, so neither dz1 nor col1 is written.
+//
+// The kernel moves ~1.1 KB per position and is meant to run at HBM bandwidth, so it needs many positions in flight and few
+// instructions per position: 8 warps per CTA and 2 CTAs per SM (<= 128 registers, no stack; the 64 of 4 CTAs per SM
+// spill).  A warp takes R positions at a time (their loads issued one group ahead), lane l owning channels 8 l .. 8 l + 7,
+// and interleaves the R LayerNorm-statistics reductions.  The filter gradient is a tensor-core product per
+// phase of KP positions (NP per warp): each warp stages its rounded dz1 rows and fbank taps in shared memory, and after
+// one barrier warp w contracts the phase's taps (M: 9 padded to 16) x channels 32 w .. 32 w + 31 (N) over the KP positions
+// (K) with mma.sync, adding its result into the CTA's dW1 partial.  The staging is double-buffered, so the barrier of
+// phase i also orders phase i - 1's products before phase i + 1 refills that buffer.
+template <typename T>
+__device__ __forceinline__ void conv1_bwd_implicit_body(const float* __restrict__ src, const T* __restrict__ gamma,
+                                                        const T* __restrict__ beta, const T* __restrict__ xhat,
+                                                        const float* __restrict__ rstd, const T* __restrict__ dcol,
+                                                        float* __restrict__ dw1, float* __restrict__ db, float* __restrict__ dgamma,
+                                                        float* __restrict__ dbeta, int B, int Tn, int F, int T1, int F1, int F2,
+                                                        int tu, int ub) {
+  constexpr int C = 256, WARPS = 8, R = 2, NP = 4, KP = WARPS * NP;
+  static_assert(NP % (2 * R) == 0 && KP % 16 == 0, "a phase is whole pairs of load groups and whole k16 steps");
+  // row strides in elements: 528-byte dz1 rows and 80-byte tap rows put the 8 rows of every ldmatrix 8x8 matrix in distinct
+  // banks
+  constexpr int DS = C + 8, XS = KP + 8;
+  struct Stage { T dz[KP][DS]; T x[16][XS]; };
+  __shared__ __align__(16) Stage stage[2];
+  // db | dgamma | dbeta | dW1 (9 taps); until the end, the first two rows hold gamma | beta (read per position, not kept in
+  // registers: registers are the budget)
+  __shared__ __align__(16) float sacc[12 * C];
+  float* sgb = sacc;
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  for (int i = 2 * C + threadIdx.x; i < 12 * C; i += blockDim.x) sacc[i] = 0.f;
+  for (int i = threadIdx.x; i < 2 * 16 * XS; i += blockDim.x) (&stage[i / (16 * XS)].x[0][0])[i % (16 * XS)] = from_f32<T>(0.f);
+  // affine parameters exactly as the forward used them (bf16 shadow in bf16 mode)
+  for (int i = threadIdx.x; i < C; i += blockDim.x) { sgb[i] = to_f32(gamma[i]); sgb[C + i] = to_f32(beta[i]); }
+  float a_db[8], a_dg[8], a_dbe[8];
+#pragma unroll
+  for (int i = 0; i < 8; ++i) a_db[i] = a_dg[i] = a_dbe[i] = 0.f;
+
+  // warp wid takes positions wid, wid + nwarps, ...; every warp of a CTA runs as many phases as the CTA's first warp needs
+  // (positions past the end are zero and add nothing)
+  // (positions are int: the host checks B T1 F1 < 2^31)
+  const int npos = B * T1 * F1;
+  const int nwarps = gridDim.x * WARPS;
+  const int wid0 = blockIdx.x * WARPS;
+  const int nfirst = npos > wid0 ? (npos - wid0 + nwarps - 1) / nwarps : 0;
+  const int nphase = (nfirst + NP - 1) / NP;
+  const int step_f = nwarps % F1, step_t = (nwarps / F1) % T1, step_b = nwarps / (F1 * T1);
+  int ipos = wid0 + warp;                        // position whose loads are issued next
+  int ib = ipos / (F1 * T1), it1 = (ipos / F1) % T1, if1 = ipos % F1;
+  const int tap_dt = lane / 3 - 1, tap_df = lane % 3 - 1;      // lanes 0..8 own one fbank tap each
+  struct Loads { Vec8<T> xh, dc; float rs, xv; };
+  auto issue_next = [&](Loads& L) {
+    L.xv = 0.f;
+    if (ipos < npos) {
+      if (lane < 9) {
+        const int t = 2 * it1 + tap_dt, f = 2 * if1 + tap_df;
+        if (t >= 0 && t < Tn && f >= 0 && f < F) L.xv = __ldg(&src[((int64_t)ib * Tn + t) * F + f]);
+      }
+      L.xh.load(xhat + (int64_t)ipos * C + 8 * lane);
+      L.rs = __ldg(rstd + ipos);
+      const int cls = ((it1 & 1) << 1) | (if1 & 1), u = it1 >> 1, v = if1 >> 1;
+      const int64_t row = (((int64_t)cls * B + ib) * ub + u / tu) * 128 + (u % tu) * F2 + v;
+      L.dc.load(dcol + row * C + 8 * lane);
+    } else {
+      L.xh.zero(); L.dc.zero(); L.rs = 0.f;
+    }
+    ipos += nwarps;
+    if1 += step_f; if (if1 >= F1) { if1 -= F1; ++it1; }
+    it1 += step_t; if (it1 >= T1) { it1 -= T1; ++ib; }
+    ib += step_b;
+  };
+  // ReLU' and LayerNorm backward of R positions, their statistics reductions interleaved; the rounded dz1 rows and fbank taps
+  // go to stage rows k0 .. k0 + R - 1
+  auto process = [&](const Loads (&L)[R], uint32_t sdz, uint32_t sx) {
+    float greg[8], breg[8];
+    *reinterpret_cast<float4*>(greg) = *reinterpret_cast<const float4*>(&sgb[8 * lane]);
+    *reinterpret_cast<float4*>(greg + 4) = *reinterpret_cast<const float4*>(&sgb[8 * lane + 4]);
+    *reinterpret_cast<float4*>(breg) = *reinterpret_cast<const float4*>(&sgb[C + 8 * lane]);
+    *reinterpret_cast<float4*>(breg + 4) = *reinterpret_cast<const float4*>(&sgb[C + 8 * lane + 4]);
+    float xh[R][8], d[R][8], c1[R], c2s[R];
+#pragma unroll
+    for (int r = 0; r < R; ++r) {
+      L[r].xh.get(xh[r]);
+      L[r].dc.get(d[r]);
+      c1[r] = 0.f; c2s[r] = 0.f;
+#pragma unroll
+      for (int i = 0; i < 8; ++i) {
+        if (!(fmaf(xh[r][i], greg[i], breg[i]) > 0.f)) d[r][i] = 0.f;      // ReLU' on y = xhat * gamma + beta
+        const float g = d[r][i] * greg[i];
+        c1[r] += g; c2s[r] = fmaf(g, xh[r][i], c2s[r]);
+        a_dg[i] = fmaf(d[r][i], xh[r][i], a_dg[i]); a_dbe[i] += d[r][i];
+      }
+    }
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) {
+#pragma unroll
+      for (int r = 0; r < R; ++r) {
+        c1[r] += __shfl_xor_sync(0xffffffffu, c1[r], o);
+        c2s[r] += __shfl_xor_sync(0xffffffffu, c2s[r], o);
+      }
+    }
+#pragma unroll
+    for (int r = 0; r < R; ++r) {
+      c1[r] *= (1.0f / C); c2s[r] *= (1.0f / C);
+#pragma unroll
+      for (int i = 0; i < 8; ++i) { d[r][i] = L[r].rs * (d[r][i] * greg[i] - c1[r] - xh[r][i] * c2s[r]); a_db[i] += d[r][i]; }
+      constexpr int DT = std::is_same<T, __half>::value ? F16 : BF16;
+      asm volatile("st.shared.v4.b32 [%0], {%1, %2, %3, %4};" ::"r"(sdz + (uint32_t)(r * DS * 2)), "r"(pack2_16(d[r][0], d[r][1], DT)),
+                   "r"(pack2_16(d[r][2], d[r][3], DT)), "r"(pack2_16(d[r][4], d[r][5], DT)), "r"(pack2_16(d[r][6], d[r][7], DT)) : "memory");
+      if (lane < 9) {
+        const T xv = from_f32<T>(L[r].xv);
+        asm volatile("st.shared.b16 [%0], %1;" ::"r"(sx + (uint32_t)(r * 2)), "h"(*reinterpret_cast<const unsigned short*>(&xv)) : "memory");
+      }
+    }
+  };
+  Loads ring[2][R];
+#pragma unroll
+  for (int r = 0; r < R; ++r) issue_next(ring[0][r]);
+  __syncthreads();
+  // this lane's stage addresses: dz1 row warp * NP, channels 8 lane ..; tap row lane, position warp * NP
+  const uint32_t sdz0 = (uint32_t)__cvta_generic_to_shared(&stage[0].dz[warp * NP][8 * lane]);
+  const uint32_t sx0 = (uint32_t)__cvta_generic_to_shared(&stage[0].x[lane < 16 ? lane : 0][warp * NP]);
+  for (int ph = 0; ph < nphase; ++ph) {
+    Stage& S = stage[ph & 1];
+    const uint32_t soff = (uint32_t)((ph & 1) * sizeof(Stage));
+#pragma unroll
+    for (int j = 0; j < NP / R; ++j) {
+#pragma unroll
+      for (int r = 0; r < R; ++r) issue_next(ring[(j + 1) & 1][r]);
+      process(ring[j & 1], sdz0 + soff + (uint32_t)(j * R * DS * 2), sx0 + soff + (uint32_t)(j * R * 2));
+    }
+    __syncthreads();
+    // dW1 partial of this phase: taps x channels 32 warp .. 32 warp + 31, as two halves of 2 n8 tiles (fragment rows g: taps
+    // 0..7; g + 8: tap 8 for g == 0, padding otherwise); each element of the partial has one owner in the CTA
+    const int mr = (lane & 7) + 8 * ((lane >> 3) & 1), mc = 8 * (lane >> 4);   // this lane's ldmatrix row / column offset
+    const int g = lane >> 2, q = lane & 3;
+#pragma unroll
+    for (int np = 0; np < 2; ++np) {
+      float acc[2][4] = {};
+#pragma unroll
+      for (int ks = 0; ks < KP / 16; ++ks) {
+        uint32_t a[4], b[4];
+        ldmatrix_x4(a, &S.x[mr][16 * ks + mc]);
+        ldmatrix_x4_trans(b, &S.dz[16 * ks + mr][32 * warp + 16 * np + mc]);
+        mma_16816<T>(acc[0], a, b[0], b[1]);
+        mma_16816<T>(acc[1], a, b[2], b[3]);
+      }
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        const int c = 32 * warp + 16 * np + 8 * h + 2 * q;
+        float2* p0 = reinterpret_cast<float2*>(&sacc[(3 + g) * C + c]);
+        const float2 v0 = *p0;
+        *p0 = make_float2(v0.x + acc[h][0], v0.y + acc[h][1]);
+        if (g == 0) {
+          float2* p8 = reinterpret_cast<float2*>(&sacc[11 * C + c]);
+          const float2 v8 = *p8;
+          *p8 = make_float2(v8.x + acc[h][2], v8.y + acc[h][3]);
+        }
+      }
+    }
+  }
+  __syncthreads();                               // gamma | beta read for the last time
+  for (int i = threadIdx.x; i < 2 * C; i += blockDim.x) sacc[i] = 0.f;
+  __syncthreads();
+#pragma unroll
+  for (int i = 0; i < 8; ++i) {
+    const int c = 8 * lane + i;
+    atomicAdd(&sacc[c], a_db[i]); atomicAdd(&sacc[C + c], a_dg[i]); atomicAdd(&sacc[2 * C + c], a_dbe[i]);
+  }
+  __syncthreads();
+  // one vector reduction per 4 floats: 768 per CTA
+  for (int i = threadIdx.x; i < 3 * C; i += blockDim.x) {
+    const int a = i / (C / 4), e = 4 * (i % (C / 4));
+    float* dst = a == 0 ? db + e : a == 1 ? dgamma + e : a == 2 ? dbeta + e : dw1 + (a - 3) * C + e;
+    const float4 v = *reinterpret_cast<const float4*>(&sacc[4 * i]);
+    asm volatile("red.global.add.v4.f32 [%0], {%1, %2, %3, %4};" ::"l"(dst), "f"(v.x), "f"(v.y), "f"(v.z), "f"(v.w) : "memory");
+  }
+}
+
 template <typename T, bool IMPLICIT>
-__global__ void __launch_bounds__(256, IMPLICIT ? 1 : 2) conv1_bwd_xhat_c256_kernel(
+__global__ void __launch_bounds__(256, 2) conv1_bwd_xhat_c256_kernel(
     const float* __restrict__ src, const T* __restrict__ gamma, const T* __restrict__ beta, const T* __restrict__ xhat,
     const float* __restrict__ rstd, const T* __restrict__ dcol, T* __restrict__ dz1, T* __restrict__ col1, int K1p,
     float* __restrict__ dw1, float* __restrict__ db, float* __restrict__ dgamma, float* __restrict__ dbeta, int B, int Tn, int F,
     int T1, int F1, int T2, int F2, int tu, int ub) {
   pdl_wait();
   pdl_trigger();
-  constexpr int C = 256;
-  constexpr int NACC = IMPLICIT ? 12 : 3;      // db | dgamma | dbeta (| dW1, 9 taps)
-  __shared__ float sacc[NACC * C];
-  for (int i = threadIdx.x; i < NACC * C; i += blockDim.x) sacc[i] = 0.f;
-  __syncthreads();
-  const int lane = threadIdx.x & 31;
-  float greg[8], breg[8], a_db[8], a_dg[8], a_dbe[8];
-  float a_dw[IMPLICIT ? 9 : 1][8];
-  ld8<T>(gamma + 8 * lane, greg);       // affine parameters exactly as the forward used them (bf16 shadow in bf16 mode)
-  ld8<T>(beta + 8 * lane, breg);
+  if constexpr (IMPLICIT) {
+    conv1_bwd_implicit_body<T>(src, gamma, beta, xhat, rstd, dcol, dw1, db, dgamma, dbeta, B, Tn, F, T1, F1, F2, tu, ub);
+  } else {
+    constexpr int C = 256;
+    __shared__ float sacc[3 * C];      // db | dgamma | dbeta
+    for (int i = threadIdx.x; i < 3 * C; i += blockDim.x) sacc[i] = 0.f;
+    __syncthreads();
+    const int lane = threadIdx.x & 31;
+    float greg[8], breg[8], a_db[8], a_dg[8], a_dbe[8];
+    ld8<T>(gamma + 8 * lane, greg);       // affine parameters exactly as the forward used them (bf16 shadow in bf16 mode)
+    ld8<T>(beta + 8 * lane, breg);
 #pragma unroll
-  for (int i = 0; i < 8; ++i) a_db[i] = a_dg[i] = a_dbe[i] = 0.f;
-#pragma unroll
-  for (int tp = 0; tp < (IMPLICIT ? 9 : 1); ++tp)
-#pragma unroll
-    for (int i = 0; i < 8; ++i) a_dw[tp][i] = 0.f;
-  const int64_t npos = (int64_t)B * T1 * F1;
-  const int64_t nwarps = (int64_t)gridDim.x * (blockDim.x >> 5);
-  const int64_t wid = (int64_t)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
-  int64_t pos = wid;                       // warp-interleaved positions: the grid sweeps one contiguous window of xhat / dz1
-  const int64_t pos_end = npos;
-  const int step_f = (int)(nwarps % F1), step_t = (int)((nwarps / F1) % T1), step_b = (int)(nwarps / ((int64_t)F1 * T1));
-  if (pos < pos_end) {
-    int f1 = (int)(pos % F1);
-    int t1 = (int)((pos / F1) % T1);
-    int b = (int)(pos / ((int64_t)F1 * T1));
-    const int tap_dt = lane / 3 - 1, tap_df = lane % 3 - 1;      // lanes 0..8 own one fbank tap each
-    // every global load of a position (fbank tap, xhat row, 1/sigma, dcol rows) is issued RING-1 positions ahead: the kernel is
-    // bound by bytes in flight, not by bandwidth — the implicit variant loads
-    // one gradient row instead of four and spends the freed registers on a deeper ring
-    constexpr int NDC = IMPLICIT ? 1 : 4;
-    constexpr int RING = IMPLICIT ? 6 : 2;
-    struct Loads { Vec8<T> xh, dc[NDC]; float rs, xv; };
-    auto issue = [&](int64_t p, int bb, int tt1, int ff1, Loads& L) {
-      L.xv = 0.f;
-      if (lane < 9) {
-        const int t = 2 * tt1 + tap_dt, f = 2 * ff1 + tap_df;
-        if (t >= 0 && t < Tn && f >= 0 && f < F) L.xv = __ldg(&src[((int64_t)bb * Tn + t) * F + f]);
-      }
-      L.xh.load(xhat + p * C + 8 * lane);
-      L.rs = __ldg(rstd + p);
-      if constexpr (IMPLICIT) {
-        const int cls = ((tt1 & 1) << 1) | (ff1 & 1), u = tt1 >> 1, v = ff1 >> 1;
-        const int64_t row = (((int64_t)cls * B + bb) * ub + u / tu) * 128 + (u % tu) * F2 + v;
-        L.dc[0].load(dcol + row * C + 8 * lane);
-      } else {
+    for (int i = 0; i < 8; ++i) a_db[i] = a_dg[i] = a_dbe[i] = 0.f;
+    const int64_t npos = (int64_t)B * T1 * F1;
+    const int64_t nwarps = (int64_t)gridDim.x * (blockDim.x >> 5);
+    const int64_t wid = (int64_t)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
+    int64_t pos = wid;                       // warp-interleaved positions: the grid sweeps one contiguous window of xhat / dz1
+    const int64_t pos_end = npos;
+    const int step_f = (int)(nwarps % F1), step_t = (int)((nwarps / F1) % T1), step_b = (int)(nwarps / ((int64_t)F1 * T1));
+    if (pos < pos_end) {
+      int f1 = (int)(pos % F1);
+      int t1 = (int)((pos / F1) % T1);
+      int b = (int)(pos / ((int64_t)F1 * T1));
+      const int tap_dt = lane / 3 - 1, tap_df = lane % 3 - 1;      // lanes 0..8 own one fbank tap each
+      // every global load of a position (fbank tap, xhat row, 1/sigma, dcol rows) is issued RING-1 positions ahead: the
+      // kernel is bound by bytes in flight, not by bandwidth
+      constexpr int NDC = 4;
+      constexpr int RING = 2;
+      struct Loads { Vec8<T> xh, dc[NDC]; float rs, xv; };
+      auto issue = [&](int64_t p, int bb, int tt1, int ff1, Loads& L) {
+        L.xv = 0.f;
+        if (lane < 9) {
+          const int t = 2 * tt1 + tap_dt, f = 2 * ff1 + tap_df;
+          if (t >= 0 && t < Tn && f >= 0 && f < F) L.xv = __ldg(&src[((int64_t)bb * Tn + t) * F + f]);
+        }
+        L.xh.load(xhat + p * C + 8 * lane);
+        L.rs = __ldg(rstd + p);
         // col2im: t1 even -> kh = 1 ; t1 odd -> kh in {0, 2} (same along f); slot = 2 * a + c2
         const int kh0 = (tt1 & 1) ? 0 : 1, kw0 = (ff1 & 1) ? 0 : 1;
 #pragma unroll
@@ -573,98 +762,71 @@ __global__ void __launch_bounds__(256, IMPLICIT ? 1 : 2) conv1_bwd_xhat_c256_ker
             else L.dc[2 * a + c2].zero();
           }
         }
-      }
-    };
-    // IMPLICIT: the filter-gradient update of a position is made during the next position's statistics reductions (shuffle
-    // chains that would otherwise leave the scheduler idle at one CTA per SM)
-    float prev_d[8], prev_x = 0.f;
+      };
+      auto process = [&](int64_t pp, const Loads& cur) {
+        float xh[8], d[8];
+        cur.xh.get(xh);
+        cur.dc[0].get(d);
 #pragma unroll
-    for (int i = 0; i < 8; ++i) prev_d[i] = 0.f;
-    auto dw_update = [&]() {
+        for (int k = 1; k < NDC; ++k) {
+          float t8[8];
+          cur.dc[k].get(t8);
 #pragma unroll
-      for (int tp = 0; tp < 9; ++tp) {
-        const float x = __shfl_sync(0xffffffffu, prev_x, tp);
+          for (int i = 0; i < 8; ++i) d[i] += t8[i];
+        }
+        const float rs = cur.rs;
+        float c1 = 0.f, c2s = 0.f;
 #pragma unroll
-        for (int i = 0; i < 8; ++i) a_dw[tp][i] = fmaf(x, prev_d[i], a_dw[tp][i]);
-      }
-    };
-    auto process = [&](int64_t pp, const Loads& cur) {
-      float xh[8], d[8];
-      cur.xh.get(xh);
-      cur.dc[0].get(d);
+        for (int i = 0; i < 8; ++i) {
+          if (!(fmaf(xh[i], greg[i], breg[i]) > 0.f)) d[i] = 0.f;      // ReLU' on y = xhat * gamma + beta
+          const float g = d[i] * greg[i];
+          c1 += g; c2s = fmaf(g, xh[i], c2s);
+          a_dg[i] = fmaf(d[i], xh[i], a_dg[i]); a_dbe[i] += d[i];
+        }
 #pragma unroll
-      for (int k = 1; k < NDC; ++k) {
-        float t8[8];
-        cur.dc[k].get(t8);
+        for (int o = 16; o > 0; o >>= 1) { c1 += __shfl_xor_sync(0xffffffffu, c1, o); c2s += __shfl_xor_sync(0xffffffffu, c2s, o); }
+        c1 *= (1.0f / C); c2s *= (1.0f / C);
 #pragma unroll
-        for (int i = 0; i < 8; ++i) d[i] += t8[i];
-      }
-      const float rs = cur.rs;
-      float c1 = 0.f, c2s = 0.f;
-#pragma unroll
-      for (int i = 0; i < 8; ++i) {
-        if (!(fmaf(xh[i], greg[i], breg[i]) > 0.f)) d[i] = 0.f;      // ReLU' on y = xhat * gamma + beta
-        const float g = d[i] * greg[i];
-        c1 += g; c2s = fmaf(g, xh[i], c2s);
-        a_dg[i] = fmaf(d[i], xh[i], a_dg[i]); a_dbe[i] += d[i];
-      }
-      if constexpr (IMPLICIT) dw_update();
-#pragma unroll
-      for (int o = 16; o > 0; o >>= 1) { c1 += __shfl_xor_sync(0xffffffffu, c1, o); c2s += __shfl_xor_sync(0xffffffffu, c2s, o); }
-      c1 *= (1.0f / C); c2s *= (1.0f / C);
-#pragma unroll
-      for (int i = 0; i < 8; ++i) { d[i] = rs * (d[i] * greg[i] - c1 - xh[i] * c2s); a_db[i] += d[i]; }
-      if constexpr (IMPLICIT) {
-        prev_x = to_f32(from_f32<T>(cur.xv));
-#pragma unroll
-        for (int i = 0; i < 8; ++i) prev_d[i] = to_f32(from_f32<T>(d[i]));
-      } else {
+        for (int i = 0; i < 8; ++i) { d[i] = rs * (d[i] * greg[i] - c1 - xh[i] * c2s); a_db[i] += d[i]; }
         store8<T>(dz1 + pp * C + 8 * lane, d);
         if (lane < K1p) col1[pp * K1p + lane] = from_f32<T>(lane < 9 ? cur.xv : 0.f);
-      }
-    };
-    // issue cursor (position whose loads are issued next) runs RING-1 positions ahead of the compute cursor `pos`
-    int64_t ipos = pos;
-    int ib = b, it1 = t1, if1 = f1;
-    auto issue_next = [&](Loads& L) {
-      if (ipos < pos_end) {
-        issue(ipos, ib, it1, if1, L);
-        ipos += nwarps;
-        if1 += step_f; if (if1 >= F1) { if1 -= F1; ++it1; }
-        it1 += step_t; if (it1 >= T1) { it1 -= T1; ++ib; }
-        ib += step_b;
-      }
-    };
-    Loads ring[RING];
+      };
+      // issue cursor (position whose loads are issued next) runs RING-1 positions ahead of the compute cursor `pos`
+      int64_t ipos = pos;
+      int ib = b, it1 = t1, if1 = f1;
+      auto issue_next = [&](Loads& L) {
+        if (ipos < pos_end) {
+          issue(ipos, ib, it1, if1, L);
+          ipos += nwarps;
+          if1 += step_f; if (if1 >= F1) { if1 -= F1; ++it1; }
+          it1 += step_t; if (it1 >= T1) { it1 -= T1; ++ib; }
+          ib += step_b;
+        }
+      };
+      Loads ring[RING];
 #pragma unroll
-    for (int j = 0; j < RING - 1; ++j) issue_next(ring[j]);
-    while (pos < pos_end) {
+      for (int j = 0; j < RING - 1; ++j) issue_next(ring[j]);
+      while (pos < pos_end) {
 #pragma unroll
-      for (int j = 0; j < RING; ++j) {
-        if (pos < pos_end) {
-          issue_next(ring[(j + RING - 1) % RING]);
-          process(pos, ring[j]);
-          pos += nwarps;
+        for (int j = 0; j < RING; ++j) {
+          if (pos < pos_end) {
+            issue_next(ring[(j + RING - 1) % RING]);
+            process(pos, ring[j]);
+            pos += nwarps;
+          }
         }
       }
     }
-    if constexpr (IMPLICIT) dw_update();      // the last position
-  }
 #pragma unroll
-  for (int i = 0; i < 8; ++i) {
-    const int c = 8 * lane + i;
-    atomicAdd(&sacc[c], a_db[i]); atomicAdd(&sacc[C + c], a_dg[i]); atomicAdd(&sacc[2 * C + c], a_dbe[i]);
-    if constexpr (IMPLICIT) {
-#pragma unroll
-      for (int tp = 0; tp < 9; ++tp) atomicAdd(&sacc[(3 + tp) * C + c], a_dw[tp][i]);
+    for (int i = 0; i < 8; ++i) {
+      const int c = 8 * lane + i;
+      atomicAdd(&sacc[c], a_db[i]); atomicAdd(&sacc[C + c], a_dg[i]); atomicAdd(&sacc[2 * C + c], a_dbe[i]);
+    }
+    __syncthreads();
+    for (int i = threadIdx.x; i < C; i += blockDim.x) {
+      atomicAdd(&db[i], sacc[i]); atomicAdd(&dgamma[i], sacc[C + i]); atomicAdd(&dbeta[i], sacc[2 * C + i]);
     }
   }
-  __syncthreads();
-  for (int i = threadIdx.x; i < C; i += blockDim.x) {
-    atomicAdd(&db[i], sacc[i]); atomicAdd(&dgamma[i], sacc[C + i]); atomicAdd(&dbeta[i], sacc[2 * C + i]);
-  }
-  if constexpr (IMPLICIT)
-    for (int i = threadIdx.x; i < 9 * C; i += blockDim.x) atomicAdd(&dw1[i], sacc[3 * C + i]);
 }
 
 // ---------------------------------------------------------------------------------------------
@@ -862,7 +1024,10 @@ int conv1_bwd_from_xhat(const float* src, const void* gamma, const void* beta, c
   const int tu = F2 > 0 && F2 <= 128 ? 128 / F2 : 1, ub = (T2 + tu - 1) / tu;
   if (implicit_tiles) {
     B200ST_CHECK(F2 <= 128 && dw1 != nullptr, "implicit conv2 dgrad layout needs F2 <= 128 and the dW1 accumulator");
-    const int grid = grid_for(npos, 8 * 16, 132);
+    B200ST_CHECK(npos < ((int64_t)1 << 31), "conv1 backward: more than 2^31 positions");
+    B200ST_CHECK(((reinterpret_cast<uintptr_t>(dw1) | reinterpret_cast<uintptr_t>(db) | reinterpret_cast<uintptr_t>(dgamma) |
+                   reinterpret_cast<uintptr_t>(dbeta)) & 15) == 0, "conv1 parameter gradients must be 16-byte aligned");
+    const int grid = grid_for(npos, 8 * 16, 132 * 2);      // 2 CTAs per SM (the kernel's register budget)
     B200ST_CHECK(is16(dtype), "implicit conv2 dgrad layout is 16-bit");
 #define BWD_IMPLICIT(TT)                                                                                                          \
   launch(conv1_bwd_xhat_c256_kernel<TT, true>, grid, 256, 0, s, src, (const TT*)gamma, (const TT*)beta, (const TT*)xhat, rstd,   \

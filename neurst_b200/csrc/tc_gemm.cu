@@ -70,6 +70,11 @@ struct TcParams {
   int conv_remap, conv_T2, conv_F2;
   int conv_dt[9], conv_df[9], conv_wrow[9], conv_plane[9];   // per tap: time / frequency shift, first weight row, first plane
   uint32_t conv_a_bytes;                      // bytes one A box delivers (64 ch x F2 x conv_tu x 2)
+  // Data gradient (tc_gemm_conv_kernel<B_MN = false>): the four parity classes in one launch.  Tile = unit * 4 + cls, unit =
+  // (row tile, n tile); class cls has the taps conv_tap0[cls] .. conv_tap0[cls] + conv_ntap[cls] - 1 (the classes' taps
+  // follow each other, 9 in all) and writes C + cls * conv_cls_elems.  See dgrad_first_tile.
+  int conv_tap0[4], conv_ntap[4];
+  int64_t conv_cls_elems;
 };
 constexpr int kConvRows = 1, kConvWgrad = 2;   // ConvA::mode: tc_gemm_kernel's A operand, or tc_wgrad_group_kernel's operands
 
@@ -82,6 +87,36 @@ __device__ __forceinline__ TileCoord decode_tile(const TcParams& p, int64_t tile
   t.m_blk = (int)(tile % p.m_tiles); tile /= p.m_tiles;
   t.b1 = (int)(tile % p.nb1);
   t.b2 = (int)(tile / p.nb1);
+  return t;
+}
+
+// Static schedule of the conv2 data gradient's tiles over its persistent CTAs.  The tiles, in (unit, class) order, form one
+// sequence of W = units * 9 * conv_kpc k-blocks; CTA c owns the tiles whose first k-block lies in [ceil(c W / G),
+// ceil((c + 1) W / G)) for a grid of G CTAs.  Each CTA's k-blocks therefore differ from the mean W / G by less than one tile
+// (at most 4 taps * conv_kpc k-blocks), and the four class tiles of a unit, which read the same dZ2 rows, run back to back on
+// one SM.  Returns the first tile of CTA c (c = G: the tile count).
+__device__ __forceinline__ int64_t dgrad_first_tile(const TcParams& p, int c) {
+  const int64_t per_unit = 9 * p.conv_kpc;
+  const int64_t s = ((int64_t)c * (p.num_tiles / 4) * per_unit + gridDim.x - 1) / gridDim.x;
+  int64_t unit = s / per_unit;
+  const int rem = (int)(s - unit * per_unit);
+  int cls = 0;
+  while (cls < 4 && p.conv_tap0[cls] * p.conv_kpc < rem) ++cls;
+  if (cls == 4) { ++unit; cls = 0; }
+  return unit * 4 + cls;
+}
+
+// Coordinates of data-gradient tile `tile` (parity class tile & 3): its row / n tile and its k-blocks [kb0, kb1) in the
+// 9-tap k-block numbering (k-block kb is tap kb / conv_kpc).
+__device__ __forceinline__ TileCoord decode_dgrad_tile(const TcParams& p, int64_t tile, int& kb0, int& kb1) {
+  const int cls = (int)(tile & 3);
+  const int64_t unit = tile >> 2;
+  TileCoord t;
+  t.split = 0; t.b1 = 0; t.b2 = 0;
+  t.n_blk = (int)(unit % p.n_tiles);
+  t.m_blk = (int)(unit / p.n_tiles);
+  kb0 = p.conv_tap0[cls] * p.conv_kpc;
+  kb1 = kb0 + p.conv_ntap[cls] * p.conv_kpc;
   return t;
 }
 
@@ -247,6 +282,11 @@ __device__ __forceinline__ void tc_gemm_body(const CUtensorMap& tmA, const CUten
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
+  // the CTA's tiles: blockIdx.x, + gridDim.x, ... (the conv2 data gradient: a contiguous run, dgrad_first_tile)
+  constexpr bool DGRAD = CONV && !B_MN;
+  auto first_tile = [&]() -> int64_t { if constexpr (DGRAD) return dgrad_first_tile(p, blockIdx.x); else return blockIdx.x; };
+  auto end_tile = [&]() -> int64_t { if constexpr (DGRAD) return dgrad_first_tile(p, blockIdx.x + 1); else return p.num_tiles; };
+  auto next_tile = [&](int64_t tile) -> int64_t { if constexpr (DGRAD) return tile + 1; else return tile + gridDim.x; };
 
   if (warp == 0 && lane == 0) {
     ptx::prefetch_tensormap(&tmA);
@@ -263,10 +303,16 @@ __device__ __forceinline__ void tc_gemm_body(const CUtensorMap& tmA, const CUten
     // ===================== TMA producer =====================
     ptx::reg_dealloc<kProducerRegs>();
     if (warp == 0 && lane == 0) {
-      for (int64_t tile = blockIdx.x; tile < p.num_tiles; tile += gridDim.x) {
-        const TileCoord t = decode_tile(p, tile);
-        const int kb0 = t.split * p.kb_per_split;
-        const int kb1 = min(p.kb_total, kb0 + p.kb_per_split);
+      for (int64_t tile = first_tile(), end = end_tile(); tile < end; tile = next_tile(tile)) {
+        TileCoord t;
+        int kb0, kb1;
+        if constexpr (DGRAD) {
+          t = decode_dgrad_tile(p, tile, kb0, kb1);
+        } else {
+          t = decode_tile(p, tile);
+          kb0 = t.split * p.kb_per_split;
+          kb1 = min(p.kb_total, kb0 + p.kb_per_split);
+        }
         for (int kb = kb0; kb < kb1; ++kb) {
           ptx::mbar_wait(ring.empty(ring.stage), ring.phase ^ 1u);
           const uint32_t sa = ring.slot();
@@ -319,19 +365,27 @@ __device__ __forceinline__ void tc_gemm_body(const CUtensorMap& tmA, const CUten
 #pragma unroll
     for (int i = 0; i < BN / 2; ++i) acc[0][i] = acc[1][i] = 0.f;
     int j = 0;
-    for (int64_t tile = blockIdx.x; tile < p.num_tiles; tile += gridDim.x, ++j) {
-      const TileCoord t = decode_tile(p, tile);
-      const int kb0 = t.split * p.kb_per_split;
-      const int kb1 = min(p.kb_total, kb0 + p.kb_per_split);
+    for (int64_t tile = first_tile(), end = end_tile(); tile < end; tile = next_tile(tile), ++j) {
+      TileCoord t;
+      int kb0, kb1;
+      if constexpr (DGRAD) {
+        t = decode_dgrad_tile(p, tile, kb0, kb1);
+      } else {
+        t = decode_tile(p, tile);
+        kb0 = t.split * p.kb_per_split;
+        kb1 = min(p.kb_total, kb0 + p.kb_per_split);
+      }
       if ((j & 1) != wg) {
         ring.skip(kb1 - kb0);
         continue;
       }
       if (j > 0) ptx::named_bar_sync(kOrderBar + wg, 256);
-      const int handoff = tile + gridDim.x < p.num_tiles ? kOrderBar + (wg ^ 1) : -1;
+      const int handoff = next_tile(tile) < end ? kOrderBar + (wg ^ 1) : -1;
       consume_tile<BN, A_MN, B_MN, BF>(acc, ring, kb1 - kb0, lane, handoff);
       const int64_t bidx = (int64_t)t.b2 * p.nb1 + t.b1;
-      const int64_t boff_c = (int64_t)t.b2 * p.c_sb2 + (int64_t)t.b1 * p.c_sb1;
+      int64_t boff_c;
+      if constexpr (DGRAD) boff_c = (tile & 3) * p.conv_cls_elems;      // the tile's parity class
+      else boff_c = (int64_t)t.b2 * p.c_sb2 + (int64_t)t.b1 * p.c_sb1;
       const int64_t boff_mask = (int64_t)t.b2 * ep.mask_sb2 + (int64_t)t.b1 * ep.mask_sb1;
       const int64_t boff_res = (int64_t)t.b2 * ep.res_sb2 + (int64_t)t.b1 * ep.res_sb1;
       constexpr int kLd = BN + 8, kPairs = BN / 2, kRowStep = 128 / kPairs;
@@ -1107,6 +1161,8 @@ struct ConvA {
   int tu, ub, remap;                     // kConvRows
   int ntaps;
   int dt[9], df[9], wrow[9], plane[9];
+  int tap0[4], ntap[4];                  // data gradient: each parity class's taps (TcParams::conv_tap0 ...)
+  int64_t cls_elems;
 };
 struct ProfRec { GemmArgs g; cudaStream_t stream; int bn, splitk; int group_n = 0; GemmArgs rest[3]; bool has_conv = false; ConvA conv; };   // group_n > 1: grouped weight-gradient launch (g + rest)
 bool g_prof = false;
@@ -1265,6 +1321,12 @@ int gemm_tc_impl(const GemmArgs& g, cudaStream_t stream, const ConvA* conv) {
       p.conv_dt[i] = conv->dt[i]; p.conv_df[i] = conv->df[i]; p.conv_wrow[i] = conv->wrow[i]; p.conv_plane[i] = conv->plane[i];
     }
     p.conv_a_bytes = (uint32_t)(BK * conv->F2 * conv->tu * 2);
+    if (!g.B.mn_major) {
+      // data gradient: g.K is the four classes' K together (9 C), the tiles are the four class tiles of every unit
+      for (int c = 0; c < 4; ++c) { p.conv_tap0[c] = conv->tap0[c]; p.conv_ntap[c] = conv->ntap[c]; }
+      p.conv_cls_elems = conv->cls_elems;
+      p.num_tiles = 4 * (int64_t)p.m_tiles * p.n_tiles;
+    }
     // A: one box = 64 channels x all F2 frequencies x tu time rows of one plane
     B200ST_TRY(make_conv_map(conv->x, g.A.dtype, conv->C, conv->F2, conv->T2, conv->planes, conv->F2, conv->tu, &ta));
     // B: all 9 taps of the [9C, C] weight matrix (K-major for the data gradient, MN-major for the forward)
@@ -1352,11 +1414,12 @@ int conv2_wgrad_implicit(const void* a1, const void* dz2, float* dw, int dtype, 
   return conv_wgrad_launch(g, ca, stream);
 }
 
-// Data gradient of the same convolution as four implicit GEMMs, one per parity class (t1 & 1, f1 & 1) of the input position:
-// dA[b, t1, f1, :] = sum over the taps (kh, kw) with t1 = 2 t2 + kh - 1, f1 = 2 f2 + kw - 1 of dY[b, t2, f2, :] W[kh, kw]^T —
-// 1 tap for (even, even), 2 for the mixed classes, 4 for (odd, odd).  The A operand is read straight out of dY by 4-D TMA
-// boxes shifted by the tap (zero fill = border), so neither the [rows, 9C] column gradient (737 MB at cfg-2) nor its col2im
-// gather exist.  Output: class-major padded tiles
+// Data gradient of the same convolution as one implicit GEMM launch over the four parity classes (t1 & 1, f1 & 1) of the input
+// position: dA[b, t1, f1, :] = sum over the taps (kh, kw) with t1 = 2 t2 + kh - 1, f1 = 2 f2 + kw - 1 of dY[b, t2, f2, :]
+// W[kh, kw]^T — 1 tap for (even, even), 2 for the mixed classes, 4 for (odd, odd), 9 in all.  The A operand is read straight
+// out of dY by 4-D TMA boxes shifted by the tap (zero fill = border), so neither the [rows, 9C] column gradient (737 MB at
+// cfg-2) nor its col2im gather exist.  The four class tiles of one (row tile, n tile) are consecutive tiles of one CTA
+// (dgrad_first_tile), so they share their dY rows in L2.  Output: class-major padded tiles
 //   dA[cls][b][tile][128 rows = tu x F2 positions (+ unused rows)][C],   tile = (t1 >> 1) / tu,   row = ((t1 >> 1) % tu) * F2 + (f1 >> 1)
 // which conv1's backward kernel reads back with the same arithmetic.
 int conv2_dgrad_implicit(const void* dy, const void* w16, void* da, int dtype, int B, int T2, int F2, int C, cudaStream_t stream) {
@@ -1365,27 +1428,28 @@ int conv2_dgrad_implicit(const void* dy, const void* w16, void* da, int dtype, i
   ca.mode = kConvRows; ca.x = dy; ca.planes = B; ca.B = B; ca.T2 = T2; ca.F2 = F2; ca.C = C;
   ca.tu = BM / F2;
   ca.ub = ceil_div(T2, ca.tu);
-  const int64_t cls_elems = (int64_t)B * ca.ub * BM * C;
+  ca.cls_elems = (int64_t)B * ca.ub * BM * C;
+  ca.ntaps = 0;
   for (int cls = 0; cls < 4; ++cls) {
     const int pt = cls >> 1, pf = cls & 1;
     // per axis: even position -> centre tap, same index; odd position -> tap 2 at the same index and tap 0 at index + 1
     const int nt = pt ? 2 : 1, nf = pf ? 2 : 1;
     const int kh_of[2] = {pt ? 2 : 1, 0}, dt_of[2] = {0, 1};
     const int kw_of[2] = {pf ? 2 : 1, 0}, df_of[2] = {0, 1};
-    ca.ntaps = nt * nf;
+    ca.tap0[cls] = ca.ntaps;
+    ca.ntap[cls] = nt * nf;
     for (int a = 0; a < nt; ++a)
       for (int b2 = 0; b2 < nf; ++b2) {
-        const int i = a * nf + b2;
+        const int i = ca.ntaps++;
         ca.dt[i] = dt_of[a]; ca.df[i] = df_of[b2]; ca.wrow[i] = (kh_of[a] * 3 + kw_of[b2]) * C; ca.plane[i] = 0;
       }
-    GemmArgs g = gemm_defaults();
-    g.M = B * ca.ub * BM; g.N = C; g.K = ca.ntaps * C;
-    g.A = GemmOperand{dy, dtype, 0, C, 0, 0};
-    g.B = GemmOperand{w16, dtype, 0, C, 0, 0};
-    g.C = reinterpret_cast<char*>(da) + (size_t)cls * cls_elems * 2; g.c_dtype = dtype; g.ldc = C;
-    B200ST_TRY(gemm_tc_impl(g, stream, &ca));
   }
-  return 0;
+  GemmArgs g = gemm_defaults();
+  g.M = B * ca.ub * BM; g.N = C; g.K = ca.ntaps * C;      // M per class; K = the classes' K together (profile FLOPs 2 M N K)
+  g.A = GemmOperand{dy, dtype, 0, C, 0, 0};
+  g.B = GemmOperand{w16, dtype, 0, C, 0, 0};
+  g.C = da; g.c_dtype = dtype; g.ldc = C;
+  return gemm_tc_impl(g, stream, &ca);
 }
 int64_t conv2_dgrad_implicit_elems(int B, int T2, int F2, int C) {
   const int tu = BM / F2;

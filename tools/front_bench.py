@@ -6,11 +6,14 @@ by kernel name and by their place in the step:
   conv1 forward        conv1_fwd_c256_kernel
   im2col               im2col_row_kernel (explicit front-end only)
   conv2 forward        the first GEMM (tc_gemm_kernel / tc_gemm_conv_kernel) after conv1's forward on its stream
-  conv2 data gradient  the GEMM launches right before conv1's backward on its stream (4 implicit, or 1 explicit)
+  conv2 data gradient  the GEMM launches right before conv1's backward on its stream (1 implicit launch over the four
+                       parity classes, or 1 explicit)
   conv2 filter grad.   the last tc_wgrad_group_kernel or MN-major x MN-major tc_gemm_kernel on the side stream before
                        conv1's backward
   conv1 backward       conv1_bwd_xhat_c256_kernel
   conv1 filter grad.   the first GEMM after conv1's backward on its stream (explicit front-end only)
+Also the front-end backward span: from the start of the last LayerNorm backward (LN2's) before conv1's backward on its
+stream to the end of conv1's backward — the stretch of the step's critical path the lines above share.
 With --compare DIR, also the whole step: bench.py in this tree and in DIR (another checkout, built), alternated --rounds
 times per workload, median and range of ms_per_step.  Prints the card's name, power limit and clocks; writes
 bench_out/front_bench.json.  Run from the repository root on a machine with an H100."""
@@ -98,6 +101,9 @@ def classify(ev):
             add("im2col", e)
         elif "conv1_bwd_xhat_c256_kernel" in n:
             add("conv1 backward", e)
+            ln2 = next((x for x in reversed(ev[:i]) if stream(x) == stream(e) and re.search(r"\bln_bwd(_vec)?_kernel", x["name"])), None)
+            if ln2:
+                out.setdefault("front-end backward span", []).append(e["ts"] + e["dur"] - ln2["ts"])
             j, dg = i - 1, 0.0
             while j >= 0:
                 if stream(ev[j]) == stream(e):
@@ -165,6 +171,9 @@ def main():
         mb = nbytes[k] / 1e6
         res["launches"][k] = {"us": us, "bytes": nbytes[k], "GB/s": nbytes[k] / (us * 1e-6) / 1e9, "samples": len(times[k])}
         print("%-24s %10.1f %10.1f %8.0f" % (k, us, mb, res["launches"][k]["GB/s"]))
+    if times.get("front-end backward span"):
+        res["front_backward_span_us"] = statistics.mean(times["front-end backward span"])
+        print("%-24s %10.1f   (LN2 backward start -> conv1 backward end, main stream)" % ("front-end bwd span", res["front_backward_span_us"]))
 
     if args.compare:
         res["step"] = {}
