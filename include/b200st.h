@@ -371,31 +371,27 @@ int b200st_refresh_shadow(const float* params, void* shadow, int32_t shadow_dtyp
  * is skipped (parameters untouched, gradients zeroed) and halves the scale; `growth_steps` finite steps double it.
  * h may be NULL (whole arena = one tensor); numel must then be a multiple of 8, as every arena the library lays out is
  * (refused otherwise, before any launch).  clip_value keeps a NaN gradient NaN, as tf.clip_by_value does.
- * tensor_sumsq: device float[param_count + 1] scratch (clip_norm / loss scale). */
-typedef struct b200st_optim_args_ {
-  float* params; float* grads; float* m; float* v;
-  void* shadow; int32_t shadow_dtype;
-  int64_t numel;
-  float lr, beta1, beta2, eps;
-  int64_t step_t;               /* Adam's t (from 1) when loss_scale_state is NULL; else t = applied steps on the device */
-  float grad_scale;             /* 1 / (replicas * update_cycle) */
-  int32_t zero_grad;
-  float clip_value, clip_norm;  /* <= 0: off */
-  float* tensor_sumsq;
-  float* loss_scale_state;
-  float growth_steps, multiplier;   /* 0 => 2000, 2 */
-} b200st_optim_args;
-int b200st_optimizer_step(b200st_handle h, const b200st_optim_args* a, void* stream);
-/* Weight pruning during training: the reference's pruning optimizer (neurst/sparsity/pruning_optimizer.py, built with
- * keep_prune_property=True) around b200st_optimizer_step, with its schedules (neurst/sparsity/pruning_schedule.py).
- * state[0] counts the updates applied in this run (the optimizer's iterations, from 1; a step the dynamic loss scale skips
- * does not count).  A pruning turn is an applied update with step >= begin_step, (step <= end_step or end_step < 0) and
- * (step - begin_step) % frequency == 0.  Off a turn: Adam, then w *= mask.  On a turn: Adam without the old mask, then per
- * pruned tensor k = round(size * (1 - sparsity)) in float32 (half to even), threshold = the k-th largest |w| counting
- * duplicates, mask = |w| >= threshold and w *= mask.  The sparsity is target_sparsity (B200ST_PRUNE_CONSTANT) or
- * (initial - target) * (1 - clip((step - begin) / (end - begin), 0, 1)) ** polynomial_power + target (B200ST_PRUNE_POLYNOMIAL),
- * in float32.  Masked weights are written as zero in the parameter and shadow arenas; their Adam moments keep moving, so a
- * later turn can bring them back.  Gradients are never masked.  Nothing synchronises with the host. */
+ * tensor_sumsq: device float[param_count + 1] scratch (clip_norm / loss scale).
+ *
+ * An optional per-element mask makes it one of two other steps; setting both, or either without a handle, is refused
+ * before any launch.  Their bitmaps are device, numel / 8 bytes, bit j of byte b is element 8b + j.
+ *
+ * prune: weight pruning during training, the reference's pruning optimizer (neurst/sparsity/pruning_optimizer.py, built
+ *   with keep_prune_property=True), with its schedules (neurst/sparsity/pruning_schedule.py).  state[0] counts the updates
+ *   applied in this run (the optimizer's iterations, from 1; a step the dynamic loss scale skips does not count).  A pruning
+ *   turn is an applied update with step >= begin_step, (step <= end_step or end_step < 0) and
+ *   (step - begin_step) % frequency == 0.  Off a turn: Adam, then w *= mask.  On a turn: Adam without the old mask, then per
+ *   pruned tensor k = round(size * (1 - sparsity)) in float32 (half to even), threshold = the k-th largest |w| counting
+ *   duplicates, mask = |w| >= threshold and w *= mask.  The sparsity is target_sparsity (B200ST_PRUNE_CONSTANT) or
+ *   (initial - target) * (1 - clip((step - begin) / (end - begin), 0, 1)) ** polynomial_power + target
+ *   (B200ST_PRUNE_POLYNOMIAL), in float32.  Masked weights are written as zero in the parameter and shadow arenas; their Adam
+ *   moments keep moving, so a later turn can bring them back.  Gradients are never masked.  Nothing synchronises with the
+ *   host.  The schedule is refused as the reference's constructors refuse it (and PolynomialDecay with
+ *   end_step == begin_step), and so is a sparsity that leaves some pruned tensor with k == 0.
+ * frozen: partial tuning of a pruned model (Prune-Tune, examples/prune_tune/src/partial_tuning_optimizer.py): every element
+ *   whose bit is 1 keeps the weight it had before the step, in the parameter arena and in the 16-bit shadow
+ *   (w = w_orig * original_mask + w * tuning_mask); 1 in the alignment padding.  The Adam moments, the gradient statistics
+ *   and the loss-scale state advance exactly as in the plain step, and the free elements get its weights bit for bit. */
 #define B200ST_PRUNE_CONSTANT 0
 #define B200ST_PRUNE_POLYNOMIAL 1
 #define B200ST_PRUNE_MAX_TENSORS 512
@@ -414,31 +410,32 @@ typedef struct {
   float* thresholds;            /* device float[n_tensors] or NULL: each tensor's |w| threshold at the last turn */
   void* scratch;                /* device, b200st_prune_scratch_bytes(n_tensors) bytes, zero-filled once before the first call */
 } b200st_prune_args;
+typedef struct b200st_optim_args_ {
+  float* params; float* grads; float* m; float* v;
+  void* shadow; int32_t shadow_dtype;
+  int64_t numel;
+  float lr, beta1, beta2, eps;
+  int64_t step_t;               /* Adam's t (from 1) when loss_scale_state is NULL; else t = applied steps on the device */
+  float grad_scale;             /* 1 / (replicas * update_cycle) */
+  int32_t zero_grad;
+  float clip_value, clip_norm;  /* <= 0: off */
+  float* tensor_sumsq;
+  float* loss_scale_state;
+  float growth_steps, multiplier;   /* 0 => 2000, 2 */
+  const b200st_prune_args* prune;   /* NULL: no pruning */
+  const uint8_t* frozen;            /* NULL: no frozen elements */
+} b200st_optim_args;
+int b200st_optimizer_step(b200st_handle h, const b200st_optim_args* a, void* stream);
 int64_t b200st_prune_scratch_bytes(int32_t n_tensors);
-/* b200st_optimizer_step with pruning; the schedule is refused as the reference's constructors refuse it (and
- * PolynomialDecay with end_step == begin_step), and so is a sparsity that leaves some pruned tensor with k == 0. */
-int b200st_optimizer_step_pruned(b200st_handle h, const b200st_optim_args* a, const b200st_prune_args* p, void* stream);
 /* The selection alone on n tensors of an arena: tensor i = params[offsets[i], offsets[i] + sizes[i]), offsets multiples of 8,
  * each tensor's slot padded to a multiple of 8 elements.  k: device int64[n], 1 <= k[i] <= sizes[i].  Writes the mask bytes of
  * the tensors, the thresholds (device float[n] or NULL) and zeroes the pruned elements of params and of the 16-bit shadow
  * (or NULL).  scratch as for b200st_prune_args. */
 int b200st_prune_select(float* params, void* shadow, const int64_t* offsets, const int64_t* sizes, const int64_t* k, int32_t n,
                         uint8_t* mask, float* thresholds, void* scratch, void* stream);
-/* Partial tuning of a pruned model (Prune-Tune, examples/prune_tune/src/partial_tuning_optimizer.py): b200st_optimizer_step,
- * after which every element whose bit of `frozen` is 1 keeps the weight it had before the step, in the parameter arena and
- * in the 16-bit shadow (w = w_orig * original_mask + w * tuning_mask).  frozen: device, numel / 8 bytes, bit j of byte b is
- * element 8b + j (the pruning mask's layout); 1 in the alignment padding.  The Adam moments, the gradient statistics and
- * the loss-scale state advance exactly as in b200st_optimizer_step, and the free elements get its weights bit for bit.
- * numel must be the handle's arena, padded to a multiple of 8. */
-int b200st_optimizer_step_partial(b200st_handle h, const b200st_optim_args* a, const uint8_t* frozen, void* stream);
 /* params[i] = 0 (and shadow[i] = +0 when shadow is not NULL; shadow_dtype B200ST_F16 or B200ST_BF16) for every element whose
  * bit of `keep` (same layout) is 0.  n: a multiple of 8. */
 int b200st_apply_mask(float* params, void* shadow, int shadow_dtype, const uint8_t* keep, int64_t n, void* stream);
-/* legacy form: plain Keras Adam with a bf16 shadow, epsilon-hat form (neurst/optimizers/__init__.py:21; hparams speech_transformer.py:265-270):
- * g' = g*grad_scale; m,v update; p -= lr*sqrt(1-b2^t)/(1-b1^t) * m/(sqrt(v)+eps); optional bf16 shadow refresh + g=0.
- * numel: a multiple of 8. */
-int b200st_adam_step(float* params, float* grads, float* m, float* v, void* shadow, int64_t numel, float lr, float beta1,
-                     float beta2, float eps, int64_t step_t, float grad_scale, int32_t zero_grad, void* stream);
 
 /* layer-level forward (reference layer API).  need_bytes != NULL: only report the workspace size. */
 int b200st_encoder_forward(b200st_handle h, const b200st_buffers* buf, const float* x, const float* padding, int32_t B,

@@ -30,7 +30,7 @@ using namespace b200st;
 extern "C" {
 
 const char* b200st_last_error(void) { return g_last_error.c_str(); }
-int b200st_version(void) { return 202; }
+int b200st_version(void) { return 203; }
 int64_t b200st_launch_count(void) { return n_launches; }
 
 static GemmOperand to_operand(const b200st_operand& o) {
@@ -357,9 +357,12 @@ static void fill_tensor_table(const Model& m, TensorTable& tt) {
   for (const ParamInfo& p : m.params) tt.off8[tt.n++] = (uint32_t)(p.offset >> 3);
   tt.off8[tt.n] = (uint32_t)(m.arena_numel >> 3);
 }
+static int to_prune_step(const Model& m, const b200st_prune_args* p, PruneStep& ps);
 int b200st_optimizer_step(b200st_handle h, const b200st_optim_args* a, void* stream) {
   if (!a || !a->params || !a->grads || !a->m || !a->v) B200ST_FAIL("bad optimizer arguments");
   if (!a->loss_scale_state && a->step_t < 1) B200ST_FAIL("step_t counts from 1");
+  if (a->prune && a->frozen) B200ST_FAIL("the optimizer step takes a pruning schedule or a frozen-element bitmap, not both");
+  if ((a->prune || a->frozen) && !h) B200ST_FAIL("pruning and partial tuning need the model's handle");
   OptimArgs o{};
   o.p = a->params; o.g = a->grads; o.m = a->m; o.v = a->v;
   o.shadow = a->shadow; o.shadow_dtype = a->shadow_dtype;
@@ -381,7 +384,9 @@ int b200st_optimizer_step(b200st_handle h, const b200st_optim_args* a, void* str
     // no handle: the whole arena is one tensor
     tt.n = 1; tt.off8[0] = 0; tt.off8[1] = (uint32_t)((a->numel + 7) >> 3);
   }
-  return optimizer_step(o, tt, reinterpret_cast<cudaStream_t>(stream));
+  PruneStep ps{};
+  if (a->prune) B200ST_TRY(to_prune_step(h->m, a->prune, ps));
+  return optimizer_step(o, tt, a->prune ? &ps : nullptr, a->frozen, reinterpret_cast<cudaStream_t>(stream));
 }
 int64_t b200st_prune_scratch_bytes(int32_t n_tensors) {
   if (n_tensors < 1 || n_tensors > B200ST_PRUNE_MAX_TENSORS) return -1;
@@ -406,11 +411,8 @@ static int fill_prune_table(const int64_t* off, const int64_t* size, int n, Prun
   pt.cbase[n] = chunks;
   return 0;
 }
-int b200st_optimizer_step_pruned(b200st_handle h, const b200st_optim_args* a, const b200st_prune_args* p, void* stream) {
-  if (!h || !a || !p) B200ST_FAIL("null argument");
-  if (!a->params || !a->grads || !a->m || !a->v) B200ST_FAIL("bad optimizer arguments");
-  if (!a->loss_scale_state && a->step_t < 1) B200ST_FAIL("step_t counts from 1");
-  if (a->numel != h->m.arena_numel) B200ST_FAIL("numel does not match the handle's parameter arena");
+// the pruned tensors of model m and the schedule of p, checked as the reference checks them
+static int to_prune_step(const Model& m, const b200st_prune_args* p, PruneStep& ps) {
   if (!p->mask || !p->state || !p->scratch || !p->tensor_ids) B200ST_FAIL("pruning needs mask, tensor_ids, state and scratch");
   // the reference's constructors (pruning_schedule.py:48-57,152-157); end == begin would divide by zero in PolynomialDecay
   if (p->schedule != B200ST_PRUNE_CONSTANT && p->schedule != B200ST_PRUNE_POLYNOMIAL) B200ST_FAIL("unknown pruning schedule");
@@ -425,60 +427,30 @@ int b200st_optimizer_step_pruned(b200st_handle h, const b200st_optim_args* a, co
   const int n = p->n_tensors;
   if (n < 1 || n > kPruneMaxTensors) B200ST_FAIL("pruning takes 1.." + std::to_string(kPruneMaxTensors) + " tensors, got " + std::to_string(n));
   std::vector<int64_t> off(n), size(n);
-  std::vector<char> seen(h->m.params.size(), 0);
+  std::vector<char> seen(m.params.size(), 0);
   // the largest sparsity the schedule reaches (PolynomialDecay moves monotonically from initial to target)
   const float smax = (float)(poly ? std::max(p->initial_sparsity, p->target_sparsity) : p->target_sparsity);
   for (int i = 0; i < n; ++i) {
     const int id = p->tensor_ids[i];
-    if (id < 0 || id >= (int)h->m.params.size() || seen[id]) B200ST_FAIL("tensor_ids: bad or repeated index " + std::to_string(id));
+    if (id < 0 || id >= (int)m.params.size() || seen[id]) B200ST_FAIL("tensor_ids: bad or repeated index " + std::to_string(id));
     seen[id] = 1;
-    const ParamInfo& pi = h->m.params[id];
+    const ParamInfo& pi = m.params[id];
     off[i] = pi.offset;
     size[i] = pi.numel;
     if (std::nearbyint((float)pi.numel * (1.f - smax)) < 1.f)
       B200ST_FAIL("pruning " + pi.name + " (" + std::to_string(pi.numel) + " elements) at sparsity " + std::to_string(smax) +
                   " keeps k = 0 weights: lower the sparsity or leave the tensor out");
   }
-  PruneTable pt{};
-  B200ST_TRY(fill_prune_table(off.data(), size.data(), n, pt));
-  PruneSchedule sc{};
+  B200ST_TRY(fill_prune_table(off.data(), size.data(), n, ps.table));
+  PruneSchedule& sc = ps.schedule;
   sc.polynomial = poly ? 1 : 0;
   // pruning_schedule.py:173-174: the Python floats' difference, then float32 (a float32 subtraction can differ by an ulp)
   sc.delta = poly ? (float)(p->initial_sparsity - p->target_sparsity) : 0.f;
   sc.target = (float)p->target_sparsity;
   sc.power = p->polynomial_power;
   sc.begin = p->begin_step; sc.end = p->end_step; sc.frequency = p->frequency;
-  PruneDev pd{p->mask, p->state, p->thresholds, reinterpret_cast<uint32_t*>(p->scratch)};
-  OptimArgs o{};
-  o.p = a->params; o.g = a->grads; o.m = a->m; o.v = a->v;
-  o.shadow = a->shadow; o.shadow_dtype = a->shadow_dtype;
-  o.n = a->numel;
-  o.lr = a->lr; o.beta1 = a->beta1; o.beta2 = a->beta2; o.eps = a->eps; o.step_t = a->step_t;
-  o.grad_scale = a->grad_scale; o.zero_grad = a->zero_grad;
-  o.clip_value = a->clip_value; o.clip_norm = a->clip_norm;
-  o.tensor_sumsq = a->tensor_sumsq; o.ctl = a->loss_scale_state;
-  o.growth_steps = a->growth_steps; o.multiplier = a->multiplier;
-  TensorTable tt{};
-  fill_tensor_table(h->m, tt);
-  return optimizer_step_pruned(o, tt, pt, sc, pd, reinterpret_cast<cudaStream_t>(stream));
-}
-int b200st_optimizer_step_partial(b200st_handle h, const b200st_optim_args* a, const uint8_t* frozen, void* stream) {
-  if (!h || !a || !frozen) B200ST_FAIL("null argument");
-  if (!a->params || !a->grads || !a->m || !a->v) B200ST_FAIL("bad optimizer arguments");
-  if (!a->loss_scale_state && a->step_t < 1) B200ST_FAIL("step_t counts from 1");
-  if (a->numel != h->m.arena_numel) B200ST_FAIL("numel does not match the handle's parameter arena");
-  OptimArgs o{};
-  o.p = a->params; o.g = a->grads; o.m = a->m; o.v = a->v;
-  o.shadow = a->shadow; o.shadow_dtype = a->shadow_dtype;
-  o.n = a->numel;
-  o.lr = a->lr; o.beta1 = a->beta1; o.beta2 = a->beta2; o.eps = a->eps; o.step_t = a->step_t;
-  o.grad_scale = a->grad_scale; o.zero_grad = a->zero_grad;
-  o.clip_value = a->clip_value; o.clip_norm = a->clip_norm;
-  o.tensor_sumsq = a->tensor_sumsq; o.ctl = a->loss_scale_state;
-  o.growth_steps = a->growth_steps; o.multiplier = a->multiplier;
-  TensorTable tt{};
-  fill_tensor_table(h->m, tt);
-  return optimizer_step_partial(o, tt, frozen, reinterpret_cast<cudaStream_t>(stream));
+  ps.dev = PruneDev{p->mask, p->state, p->thresholds, reinterpret_cast<uint32_t*>(p->scratch)};
+  return 0;
 }
 int b200st_apply_mask(float* params, void* shadow, int shadow_dtype, const uint8_t* keep, int64_t n, void* stream) {
   if (!params || !keep) B200ST_FAIL("null argument");
@@ -493,13 +465,6 @@ int b200st_prune_select(float* params, void* shadow, const int64_t* offsets, con
   B200ST_TRY(fill_prune_table(offsets, sizes, n, pt));
   PruneDev pd{mask, nullptr, thresholds, reinterpret_cast<uint32_t*>(scratch)};
   return prune_select(params, shadow, pt, k, pd, reinterpret_cast<cudaStream_t>(stream));
-}
-int b200st_adam_step(float* params, float* grads, float* m, float* v, void* shadow, int64_t numel, float lr, float beta1,
-                     float beta2, float eps, int64_t step_t, float grad_scale, int32_t zero_grad, void* stream) {
-  b200st_optim_args a{};
-  a.params = params; a.grads = grads; a.m = m; a.v = v; a.shadow = shadow; a.shadow_dtype = B200ST_BF16; a.numel = numel;
-  a.lr = lr; a.beta1 = beta1; a.beta2 = beta2; a.eps = eps; a.step_t = step_t; a.grad_scale = grad_scale; a.zero_grad = zero_grad;
-  return b200st_optimizer_step(nullptr, &a, stream);
 }
 int b200st_encoder_forward(b200st_handle h, const b200st_buffers* buf, const float* x, const float* padding, int32_t B,
                            int32_t T, float* out, int32_t training, uint64_t seed, void* stream, uint64_t* need_bytes) {

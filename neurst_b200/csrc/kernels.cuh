@@ -110,7 +110,6 @@ struct OptimArgs {
   float* ctl;                         // dynamic loss scale state or null
   float growth_steps, multiplier;     // revised_dynamic_loss_scale.py:82-107 (2000, 2)
 };
-int optimizer_step(const OptimArgs& a, const TensorTable& tt, cudaStream_t s);
 
 // ---- weight pruning (prune.cu) ----------------------------------------------------------------------------------------
 // The pruned tensors travel as a kernel argument like TensorTable.  The selection works in chunks of kPruneChunk elements
@@ -151,13 +150,18 @@ int prune_control(const PruneTable& pt, const PruneSchedule& sc, const float* ct
 int prune_select_apply(float* p, void* shadow, const PruneTable& pt, const PruneDev& pd, const int32_t* turn, cudaStream_t s);
 // the selection with host-given k (tests, bench): seeds rank / prefix / the turn word, then prune_select_apply
 int prune_select(float* p, void* shadow, const PruneTable& pt, const int64_t* k, const PruneDev& pd, cudaStream_t s);
-int optimizer_step_pruned(const OptimArgs& a, const TensorTable& tt, const PruneTable& pt, const PruneSchedule& sc,
-                          const PruneDev& pd, cudaStream_t s);
-// ---- partial tuning of a pruned model (optim.cu, prune.cu) --------------------------------------------------------------
-// optimizer_step, then the elements whose bit of `frozen` is 1 keep their old weight (master and shadow); m and v move everywhere
-int optimizer_step_partial(const OptimArgs& a, const TensorTable& tt, const uint8_t* frozen, cudaStream_t s);
 // the elements whose bit of `keep` is 0 -> 0 in p[n] and in the 16-bit shadow (or null); n a multiple of 8
 int apply_mask(float* p, void* shadow, const uint8_t* keep, int64_t n, cudaStream_t s);
+// ---- optimizer step (optim.cu) ------------------------------------------------------------------------------------------
+struct PruneStep {                        // what the pruned step adds to the plain one
+  PruneTable table;
+  PruneSchedule schedule;
+  PruneDev dev;
+};
+// The plain step when `prune` and `frozen` are both null.  `prune`: the pruned step (mask off-turn, selection and new mask on
+// a turn).  `frozen`: the partial-tuning step, whose elements with bit 1 keep their old weight (master and shadow); m and v
+// move everywhere.  At most one of the two.
+int optimizer_step(const OptimArgs& a, const TensorTable& tt, const PruneStep* prune, const uint8_t* frozen, cudaStream_t s);
 int cast_f32_to_16(const float* x, void* y, int y_dtype, int64_t n, cudaStream_t s);
 // out[g] = keep-bits of elements [8g, 8g+8) of the dropout site (identical to the on-the-fly Philox decisions)
 int dropout_bits(DropoutSpec drop, int64_t n_elems, uint8_t* out, cudaStream_t s);

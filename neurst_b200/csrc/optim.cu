@@ -96,13 +96,13 @@ __global__ void step_control_kernel(float* __restrict__ sumsq, int n_tensors, fl
 enum class MaskMode { NONE, PRUNE, FREEZE };
 
 template <bool CLIP_NORM, MaskMode MODE>
-__global__ void __launch_bounds__(256) adam_kernel(const OptimArgs a, const __grid_constant__ TensorTable tt, float unscale_host,
+__global__ void __launch_bounds__(256) adam_kernel(const OptimArgs a, const __grid_constant__ TensorTable tt,
                                                    const uint8_t* __restrict__ mask, const int32_t* __restrict__ turn) {
   pdl_wait();
   pdl_trigger();
   bool apply_mask = false;
   if constexpr (MODE == MaskMode::PRUNE) apply_mask = *turn == 0;
-  float gs = a.grad_scale * unscale_host;
+  float gs = a.grad_scale;
   float t = (float)a.step_t;
   bool skip = false;
   if (a.ctl) {
@@ -212,48 +212,32 @@ static int check_arenas(const OptimArgs& a) {
   return 0;
 }
 
-int optimizer_step(const OptimArgs& a, const TensorTable& tt, cudaStream_t s) {
+template <MaskMode MODE>
+static int adam(const OptimArgs& a, const TensorTable& tt, const uint8_t* mask, const int32_t* turn, cudaStream_t s) {
+  const int grid = grid_for(a.n, 256 * 4 * 4);
+  if (a.clip_norm > 0.f) return launch(adam_kernel<true, MODE>, grid, 256, 0, s, a, tt, mask, turn);
+  return launch(adam_kernel<false, MODE>, grid, 256, 0, s, a, tt, mask, turn);
+}
+
+// Statistics and loss-scale control, then one Adam pass.  With `prune`, the reference's pruning optimizer
+// (neurst/sparsity/pruning_optimizer.py) inside the loss-scale optimizer: the pruning control (which sees whether this update
+// is applied) before the Adam pass, which applies the mask off-turn, and the selection + new mask on a turn after it.  No
+// host synchronisation: the turn is a device word every kernel reads.  With `frozen`, the reference's partial-tuning
+// optimizer (examples/prune_tune/src/partial_tuning_optimizer.py:79-88): w = w_orig * original_mask + w * tuning_mask, i.e.
+// the elements whose bit of `frozen` is 1 keep their weight; the launches are the plain step's, whose Adam pass reads
+// numel / 8 bytes more.
+int optimizer_step(const OptimArgs& a, const TensorTable& tt, const PruneStep* prune, const uint8_t* frozen, cudaStream_t s) {
+  if (prune || frozen) B200ST_CHECK(a.n > 0 && a.n % 8 == 0, "a masked step needs an arena padded to a multiple of 8 elements");
   if (a.n == 0) return 0;
   B200ST_TRY(check_arenas(a));
+  if (prune) B200ST_TRY(check_prune_table(prune->table));
   B200ST_TRY(step_stats(a, tt, s));
-  const int grid = grid_for(a.n, 256 * 4 * 4);
-  const uint8_t* no_mask = nullptr;
-  const int32_t* no_turn = nullptr;
-  if (a.clip_norm > 0.f) return launch(adam_kernel<true, MaskMode::NONE>, grid, 256, 0, s, a, tt, 1.f, no_mask, no_turn);
-  return launch(adam_kernel<false, MaskMode::NONE>, grid, 256, 0, s, a, tt, 1.f, no_mask, no_turn);
-}
-
-// The reference's pruning optimizer (neurst/sparsity/pruning_optimizer.py) inside the loss-scale optimizer: statistics and
-// loss-scale control, the pruning control (which sees whether this update is applied), Adam with the mask off-turn, and
-// the selection + new mask on a turn.  No host synchronisation: the turn is a device word every kernel reads.
-int optimizer_step_pruned(const OptimArgs& a, const TensorTable& tt, const PruneTable& pt, const PruneSchedule& sc,
-                          const PruneDev& pd, cudaStream_t s) {
-  B200ST_CHECK(a.n > 0 && a.n % 8 == 0, "the pruned step needs an arena padded to a multiple of 8 elements");
-  B200ST_CHECK(pd.mask && pd.state && pd.scratch, "the pruned step needs the mask, the state words and the scratch");
-  B200ST_TRY(check_arenas(a));
-  B200ST_TRY(check_prune_table(pt));
-  B200ST_TRY(step_stats(a, tt, s));
-  B200ST_TRY(prune_control(pt, sc, a.ctl, pd, s));
-  const int grid = grid_for(a.n, 256 * 4 * 4);
-  const uint8_t* mask = pd.mask;
-  const int32_t* turn = pd.state + 1;
-  if (a.clip_norm > 0.f) B200ST_TRY(launch(adam_kernel<true, MaskMode::PRUNE>, grid, 256, 0, s, a, tt, 1.f, mask, turn));
-  else B200ST_TRY(launch(adam_kernel<false, MaskMode::PRUNE>, grid, 256, 0, s, a, tt, 1.f, mask, turn));
-  return prune_select_apply(a.p, a.shadow, pt, pd, turn, s);
-}
-
-// The reference's partial-tuning optimizer (examples/prune_tune/src/partial_tuning_optimizer.py:79-88): the plain step, then
-// w = w_orig * original_mask + w * tuning_mask, i.e. the elements whose bit of `frozen` is 1 keep their weight.  Same
-// statistics, loss-scale control and launches as optimizer_step; the Adam pass reads numel / 8 bytes more.
-int optimizer_step_partial(const OptimArgs& a, const TensorTable& tt, const uint8_t* frozen, cudaStream_t s) {
-  B200ST_CHECK(a.n > 0 && a.n % 8 == 0, "the partial-tuning step needs an arena padded to a multiple of 8 elements");
-  B200ST_CHECK(frozen != nullptr, "the partial-tuning step needs the frozen-element bitmap");
-  B200ST_TRY(check_arenas(a));
-  B200ST_TRY(step_stats(a, tt, s));
-  const int grid = grid_for(a.n, 256 * 4 * 4);
-  const int32_t* no_turn = nullptr;
-  if (a.clip_norm > 0.f) return launch(adam_kernel<true, MaskMode::FREEZE>, grid, 256, 0, s, a, tt, 1.f, frozen, no_turn);
-  return launch(adam_kernel<false, MaskMode::FREEZE>, grid, 256, 0, s, a, tt, 1.f, frozen, no_turn);
+  if (frozen) return adam<MaskMode::FREEZE>(a, tt, frozen, nullptr, s);
+  if (!prune) return adam<MaskMode::NONE>(a, tt, nullptr, nullptr, s);
+  const int32_t* turn = prune->dev.state + 1;
+  B200ST_TRY(prune_control(prune->table, prune->schedule, a.ctl, prune->dev, s));
+  B200ST_TRY(adam<MaskMode::PRUNE>(a, tt, prune->dev.mask, turn, s));
+  return prune_select_apply(a.p, a.shadow, prune->table, prune->dev, turn, s);
 }
 
 }  // namespace b200st

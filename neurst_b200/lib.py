@@ -10,7 +10,7 @@ _LIB_PATH = os.path.join(_HERE, "libb200st.so")
 _lib = None
 
 F32, BF16, F16 = 0, 1, 2
-ABI_VERSION = 202    # must equal b200st_version(): bumped whenever a struct in include/b200st.h changes layout
+ABI_VERSION = 203    # must equal b200st_version(): bumped whenever a struct in include/b200st.h changes layout
 
 
 class B200STError(RuntimeError):
@@ -179,16 +179,6 @@ class Batch(C.Structure):
                 ("enc_out", C.c_void_p), ("wait_k", C.c_int32), ("wait_k_dev", C.c_void_p)]
 
 
-class OptimArgs(C.Structure):
-    _fields_ = [("params", C.c_void_p), ("grads", C.c_void_p), ("m", C.c_void_p), ("v", C.c_void_p),
-                ("shadow", C.c_void_p), ("shadow_dtype", C.c_int32), ("numel", C.c_int64),
-                ("lr", C.c_float), ("beta1", C.c_float), ("beta2", C.c_float), ("eps", C.c_float),
-                ("step_t", C.c_int64), ("grad_scale", C.c_float), ("zero_grad", C.c_int32),
-                ("clip_value", C.c_float), ("clip_norm", C.c_float),
-                ("tensor_sumsq", C.c_void_p), ("loss_scale_state", C.c_void_p),
-                ("growth_steps", C.c_float), ("multiplier", C.c_float)]
-
-
 PRUNE_CONSTANT, PRUNE_POLYNOMIAL = 0, 1     # B200ST_PRUNE_CONSTANT / B200ST_PRUNE_POLYNOMIAL
 PRUNE_MAX_TENSORS = 512                      # B200ST_PRUNE_MAX_TENSORS
 
@@ -198,6 +188,17 @@ class PruneArgs(C.Structure):
                 ("initial_sparsity", C.c_double), ("target_sparsity", C.c_double), ("polynomial_power", C.c_float),
                 ("begin_step", C.c_int64), ("end_step", C.c_int64), ("frequency", C.c_int64),
                 ("state", C.c_void_p), ("thresholds", C.c_void_p), ("scratch", C.c_void_p)]
+
+
+class OptimArgs(C.Structure):
+    _fields_ = [("params", C.c_void_p), ("grads", C.c_void_p), ("m", C.c_void_p), ("v", C.c_void_p),
+                ("shadow", C.c_void_p), ("shadow_dtype", C.c_int32), ("numel", C.c_int64),
+                ("lr", C.c_float), ("beta1", C.c_float), ("beta2", C.c_float), ("eps", C.c_float),
+                ("step_t", C.c_int64), ("grad_scale", C.c_float), ("zero_grad", C.c_int32),
+                ("clip_value", C.c_float), ("clip_norm", C.c_float),
+                ("tensor_sumsq", C.c_void_p), ("loss_scale_state", C.c_void_p),
+                ("growth_steps", C.c_float), ("multiplier", C.c_float),
+                ("prune", C.POINTER(PruneArgs)), ("frozen", C.c_void_p)]
 
 
 class StepOpts(C.Structure):
@@ -260,9 +261,8 @@ class EnsembleMember(C.Structure):
 EXPORTS = [
     "b200st_last_error", "b200st_version", "b200st_launch_count", "b200st_gemm", "b200st_gemm_bench", "b200st_profile_begin", "b200st_profile_end",
     "b200st_create", "b200st_destroy", "b200st_param_arena_numel", "b200st_param_count", "b200st_param_info",
-    "b200st_workspace_bytes", "b200st_forward", "b200st_forward_backward", "b200st_refresh_shadow", "b200st_adam_step", "b200st_optimizer_step",
-    "b200st_prune_scratch_bytes", "b200st_optimizer_step_pruned", "b200st_prune_select", "b200st_optimizer_step_partial",
-    "b200st_apply_mask",
+    "b200st_workspace_bytes", "b200st_forward", "b200st_forward_backward", "b200st_refresh_shadow", "b200st_optimizer_step",
+    "b200st_prune_scratch_bytes", "b200st_prune_select", "b200st_apply_mask",
     "b200st_comm_unique_id", "b200st_comm_init", "b200st_comm_broadcast", "b200st_comm_destroy", "b200st_comm_stats", "b200st_train_step",
     "b200st_encode", "b200st_encode_workspace_bytes", "b200st_decode_scratch_floats", "b200st_decode_init", "b200st_decode_step",
     "b200st_greedy_search", "b200st_greedy_used_graph", "b200st_beam_state_bytes", "b200st_beam_search",
@@ -292,10 +292,8 @@ def _declare(lib):
     lib.b200st_optimizer_step.argtypes = [C.c_void_p, C.POINTER(OptimArgs), C.c_void_p]
     lib.b200st_prune_scratch_bytes.restype = C.c_int64
     lib.b200st_prune_scratch_bytes.argtypes = [C.c_int32]
-    lib.b200st_optimizer_step_pruned.argtypes = [C.c_void_p, C.POINTER(OptimArgs), C.POINTER(PruneArgs), C.c_void_p]
     lib.b200st_prune_select.argtypes = [C.c_void_p, C.c_void_p, C.POINTER(C.c_int64), C.POINTER(C.c_int64), C.c_void_p, C.c_int32,
                                         C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]
-    lib.b200st_optimizer_step_partial.argtypes = [C.c_void_p, C.POINTER(OptimArgs), C.c_void_p, C.c_void_p]
     lib.b200st_apply_mask.argtypes = [C.c_void_p, C.c_void_p, C.c_int32, C.c_void_p, C.c_int64, C.c_void_p]
     lib.b200st_comm_unique_id.argtypes = [C.c_char_p]
     lib.b200st_comm_init.argtypes = [C.c_void_p, C.c_char_p, C.c_int32, C.c_int32]
@@ -330,8 +328,6 @@ def _declare(lib):
     lib.b200st_stream_write.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]
     lib.b200st_stream_lengths.argtypes = [C.c_void_p, C.POINTER(C.c_int32), C.POINTER(C.c_int32)]
     lib.b200st_cascade_source.argtypes = [C.POINTER(CascadeSourceArgs), C.c_void_p]
-    lib.b200st_adam_step.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64, C.c_float,
-                                     C.c_float, C.c_float, C.c_float, C.c_int64, C.c_float, C.c_int32, C.c_void_p]
     lib.b200st_encoder_forward.argtypes = [C.c_void_p, C.POINTER(Buffers), C.c_void_p, C.c_void_p, C.c_int32, C.c_int32,
                                            C.c_void_p, C.c_int32, C.c_uint64, C.c_void_p, C.POINTER(C.c_uint64)]
     lib.b200st_decoder_forward.argtypes = [C.c_void_p, C.POINTER(Buffers), C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32,

@@ -9,8 +9,8 @@ Mirror of
 
 The schedule's step is the optimizer's `iterations` after the update: the updates applied in this run, from 1, not the global
 step (examples/weight_pruning/README.md: begin / end "start from 0 not the initial_global_step").  The device evaluates the same
-rules (b200st_optimizer_step_pruned); the methods here are their float32 restatement on the host, used to check and to
-report.
+rules (b200st_optimizer_step with a prune schedule); the methods here are their float32 restatement on the host, used to
+check and to report.
 """
 import re
 

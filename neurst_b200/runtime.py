@@ -241,9 +241,9 @@ class Runtime:
         """One optimizer step over the flat arenas (b200st_optimizer_step): unscale -> clip (per gradient tensor, as
         tf.clip_by_value / tf.clip_by_norm in gradaccum_keras_model.py:228-233) -> Keras Adam -> shadow refresh -> g = 0.
         fp16 precision: the gradients carry the dynamic loss scale; a step with non-finite gradients is skipped on the
-        device (state in `self.loss_scale_state`).  `prune`: the schedule given to prune_setup(); the step is then
-        b200st_optimizer_step_pruned (mask off-turn, selection and new mask on a turn).  `frozen`: the bitmap given to
-        partial_setup(); the step is then b200st_optimizer_step_partial (the elements whose bit is 1 keep their weight)."""
+        device (state in `self.loss_scale_state`).  `prune`: the schedule given to prune_setup(); the step then prunes
+        (mask off-turn, selection and new mask on a turn).  `frozen`: the bitmap given to partial_setup(); the step then
+        tunes partially (the elements whose bit is 1 keep their weight)."""
         if prune is not None and frozen is not None:
             raise L.B200STError("adam_step takes a pruning schedule or a frozen-element bitmap, not both")
         if self.adam_m is None:
@@ -271,16 +271,15 @@ class Runtime:
             a.loss_scale_state = self.loss_scale_state.data_ptr()
             a.growth_steps, a.multiplier = float(growth_steps), float(multiplier)
         if prune is not None:
-            L.check(self.lib.b200st_optimizer_step_pruned(self.handle, C.byref(a), C.byref(self._prune_args(prune)), L._stream()))
+            a.prune = C.pointer(self._prune_args(prune))
         elif frozen is not None:
             if getattr(self, "partial_frozen", None) is not frozen:
                 raise L.B200STError("adam_step(frozen=...) needs partial_setup() with that bitmap first")
-            L.check(self.lib.b200st_optimizer_step_partial(self.handle, C.byref(a), _ptr(frozen), L._stream()))
-        else:
-            L.check(self.lib.b200st_optimizer_step(self.handle, C.byref(a), L._stream()))
+            a.frozen = frozen.data_ptr()
+        L.check(self.lib.b200st_optimizer_step(self.handle, C.byref(a), L._stream()))
         self._shadow_stale = False
 
-    # ---- weight pruning (b200st_optimizer_step_pruned) -----------------------------------------------------------------
+    # ---- weight pruning (b200st_optimizer_step with a prune schedule) -------------------------------------------------
     def prune_setup(self, schedule, names):
         """Pruning of the parameters `names` under `schedule` (neurst_b200.pruning) for the steps that follow: a fresh device
         state (the schedule's step restarts at 0, as the reference's optimizer iterations do in a new run) and the mask
@@ -369,7 +368,7 @@ class Runtime:
             total += v.numel()
         return zeros, total
 
-    # ---- partial tuning of a pruned model (b200st_optimizer_step_partial, b200st_apply_mask) ---------------------------
+    # ---- partial tuning of a pruned model (b200st_optimizer_step with a frozen bitmap, b200st_apply_mask) --------------
     def partial_setup(self, mask_bitmap):
         """Partial tuning for the steps that follow (adam_step(frozen=self.partial_frozen)): `mask_bitmap` (device uint8
         [numel / 8], derive_prune_mask's layout over every tensor) holds 1 where the weight stays frozen, 0 where it is

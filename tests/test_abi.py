@@ -92,7 +92,8 @@ def test_struct_layouts_match_the_c_header(tmp_path):
     import subprocess
     pairs = [("b200st_operand", L.Operand), ("b200st_gemm_args", L.GemmArgs), ("b200st_config", L.Config),
              ("b200st_buffers", L.Buffers), ("b200st_batch", L.Batch), ("b200st_optim_args", L.OptimArgs),
-             ("b200st_step_opts", L.StepOpts), ("b200st_decode_state", L.DecodeState), ("b200st_greedy_args", L.GreedyArgs)]
+             ("b200st_prune_args", L.PruneArgs), ("b200st_step_opts", L.StepOpts), ("b200st_decode_state", L.DecodeState),
+             ("b200st_greedy_args", L.GreedyArgs)]
     lines = ['#include <stdio.h>', '#include <stddef.h>', '#include "b200st.h"', 'int main(void) {']
     for cname, cls in pairs:
         lines.append('  printf("%s.sizeof %%zu\\n", sizeof(%s));' % (cname, cname))

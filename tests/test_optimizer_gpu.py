@@ -418,7 +418,7 @@ def test_clip_value_keeps_a_nan_gradient(precision):
         assert bool(torch.isfinite(rt.params[j + 1:]).all()), clip
 
 
-# ---- the entries without a handle -------------------------------------------------------------------------------------
+# ---- the step without a handle ----------------------------------------------------------------------------------------
 def _arena(n, seed):
     gen = torch.Generator(device="cuda").manual_seed(seed)
     p = torch.randn(n, generator=gen, device="cuda") * 0.05
@@ -432,36 +432,43 @@ def _ptr(t):
     return C.c_void_p(t.data_ptr())
 
 
-def test_handleless_entries_match_fp64_and_refuse_unpadded_arenas():
-    """b200st_adam_step and b200st_optimizer_step(NULL, ...) (the whole arena one tensor) update every element of an arena
-    padded to 8, its last one included, as the fp64 step does; an arena of another size is refused before any launch and
-    left untouched (its last numel % 4 elements would have kept their old weight, moments and gradient)."""
+def _handleless_args(p, g, m, v, n, lr, t, gs, shadow=None, **clip):
+    a = L.OptimArgs()
+    a.params, a.grads, a.m, a.v = p.data_ptr(), g.data_ptr(), m.data_ptr(), v.data_ptr()
+    if shadow is not None:
+        a.shadow, a.shadow_dtype = shadow.data_ptr(), L.BF16
+    a.numel, a.lr, a.beta1, a.beta2, a.eps = n, lr, HP["beta1"], HP["beta2"], HP["eps"]
+    a.step_t, a.grad_scale, a.zero_grad = t, gs, 1
+    a.clip_value, a.clip_norm = clip.get("clip_value", 0.0), clip.get("clip_norm", 0.0)
+    return a
+
+
+def test_handleless_step_matches_fp64_and_refuses_unpadded_arenas():
+    """b200st_optimizer_step(NULL, ...) (the whole arena one tensor), plain with a bf16 shadow and clipping, updates every
+    element of an arena padded to 8, its last one included, as the fp64 step does; an arena of another size is refused
+    before any launch and left untouched (its last numel % 4 elements would have kept their old weight, moments and
+    gradient)."""
     lib = L.load()
     n = 8 * 1253
     lr, t, gs = 2e-3, 3, 0.25
-    # legacy entry: plain Adam with a bf16 shadow
+    # plain Adam with a bf16 shadow
     p, g, m, v = _arena(n, 1)
     p0, g0, m0, v0 = (x.clone() for x in (p, g, m, v))
     shadow = torch.empty(n, dtype=torch.bfloat16, device="cuda")
-    L.check(lib.b200st_adam_step(_ptr(p), _ptr(g), _ptr(m), _ptr(v), _ptr(shadow), n, lr, HP["beta1"], HP["beta2"], HP["eps"],
-                                 t, gs, 1, L._stream()))
+    L.check(lib.b200st_optimizer_step(None, C.byref(_handleless_args(p, g, m, v, n, lr, t, gs, shadow)), L._stream()))
     pr, mr, vr, ge = R.optimizer_step(p0, g0, m0, v0, [(0, n)], f32(lr), t, grad_scale=gs, **HP)
     bp, bm, bv = _adam_bound(pr, m0, mr, vr, ge, 3 * U32, f32(lr), t, **HP)
-    _assert_within("b200st_adam_step m", m, mr, bm)
-    _assert_within("b200st_adam_step v", v, vr, bv)
-    _assert_within("b200st_adam_step p", p, pr, bp)
+    _assert_within("optimizer_step(NULL) bf16 shadow m", m, mr, bm)
+    _assert_within("optimizer_step(NULL) bf16 shadow v", v, vr, bv)
+    _assert_within("optimizer_step(NULL) bf16 shadow p", p, pr, bp)
     assert float(p[-1]) != float(p0[-1]) and torch.equal(_bits(shadow), _bits(p.to(torch.bfloat16)))
     assert int(torch.count_nonzero(g)) == 0
-    # b200st_optimizer_step without a handle, clipping by value and by the norm of the whole arena
+    # clipping by value and by the norm of the whole arena
     for clip in (dict(clip_value=0.5), dict(clip_norm=20.0)):
         p, g, m, v = _arena(n, 2)
         p0, g0, m0, v0 = (x.clone() for x in (p, g, m, v))
         sumsq = torch.zeros(2, dtype=torch.float32, device="cuda")
-        a = L.OptimArgs()
-        a.params, a.grads, a.m, a.v = p.data_ptr(), g.data_ptr(), m.data_ptr(), v.data_ptr()
-        a.numel, a.lr, a.beta1, a.beta2, a.eps = n, lr, HP["beta1"], HP["beta2"], HP["eps"]
-        a.step_t, a.grad_scale, a.zero_grad = t, gs, 1
-        a.clip_value, a.clip_norm = clip.get("clip_value", 0.0), clip.get("clip_norm", 0.0)
+        a = _handleless_args(p, g, m, v, n, lr, t, gs, **clip)
         a.tensor_sumsq = sumsq.data_ptr()
         L.check(lib.b200st_optimizer_step(None, C.byref(a), L._stream()))
         pr, mr, vr, ge = R.optimizer_step(p0, g0, m0, v0, [(0, n)], f32(lr), t, grad_scale=gs, **clip, **HP)
@@ -472,23 +479,19 @@ def test_handleless_entries_match_fp64_and_refuse_unpadded_arenas():
         _assert_within("optimizer_step(NULL) %s v" % clip, v, vr, bv)
         _assert_within("optimizer_step(NULL) %s p" % clip, p, pr, bp)
         assert float(p[-1]) != float(p0[-1]) and int(torch.count_nonzero(g)) == 0
-    # unpadded arenas: refused with the reason, nothing launched, nothing written
+    # unpadded arenas, with and without a shadow: refused with the reason, nothing launched, nothing written
     for bad in (n + 1, n + 4, 1001):
         p, g, m, v = _arena(n + 8, 3)
-        before = [x.clone() for x in (p, g, m, v)]
+        shadow = p.to(torch.bfloat16)
+        before = [x.clone() for x in (p, g, m, v, shadow)]
         torch.cuda.synchronize()
         launches = L.launch_count()
-        rc = lib.b200st_adam_step(_ptr(p), _ptr(g), _ptr(m), _ptr(v), None, bad, lr, HP["beta1"], HP["beta2"], HP["eps"],
-                                  t, gs, 1, L._stream())
-        assert rc != 0 and "multiple of 8" in lib.b200st_last_error().decode()
-        a = L.OptimArgs()
-        a.params, a.grads, a.m, a.v = p.data_ptr(), g.data_ptr(), m.data_ptr(), v.data_ptr()
-        a.numel, a.lr, a.beta1, a.beta2, a.eps, a.step_t, a.grad_scale, a.zero_grad = bad, lr, 0.9, 0.98, 1e-9, t, gs, 1
-        rc = lib.b200st_optimizer_step(None, C.byref(a), L._stream())
-        assert rc != 0 and "multiple of 8" in lib.b200st_last_error().decode()
+        for sh in (shadow, None):
+            rc = lib.b200st_optimizer_step(None, C.byref(_handleless_args(p, g, m, v, bad, lr, t, gs, sh)), L._stream())
+            assert rc != 0 and "multiple of 8" in lib.b200st_last_error().decode()
         torch.cuda.synchronize()
         assert L.launch_count() == launches, bad
-        for x, y in zip((p, g, m, v), before):
+        for x, y in zip((p, g, m, v, shadow), before):
             assert torch.equal(_bits(x), _bits(y)), bad
 
 

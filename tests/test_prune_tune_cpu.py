@@ -237,19 +237,19 @@ def test_trainer_sets_up_the_frozen_bitmap_once_and_passes_it_to_every_step():
 
 
 # ---- the C interface -----------------------------------------------------------------------------------------------------
-def test_ctypes_signatures_match_the_header(tmp_path):
+def test_step_and_mask_ctypes_signatures_match_the_header(tmp_path):
     """The header's prototypes, assigned to pointers of the types the ctypes declarations spell out (gcc -Werror refuses any
     difference), and the declarations themselves."""
     src = tmp_path / "sig.c"
     src.write_text("\n".join([
         '#include <stdint.h>', '#include "b200st.h"',
-        'int (*partial)(b200st_handle, const b200st_optim_args*, const uint8_t*, void*) = b200st_optimizer_step_partial;',
+        'int (*step)(b200st_handle, const b200st_optim_args*, void*) = b200st_optimizer_step;',
         'int (*masking)(float*, void*, int, const uint8_t*, int64_t, void*) = b200st_apply_mask;',
-        'int main(void) { return partial == 0 || masking == 0; }']))
+        'int main(void) { return step == 0 || masking == 0; }']))
     inc = os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "include")
     subprocess.run(["gcc", "-std=c99", "-Wall", "-Werror", "-c", "-I", inc, str(src), "-o", str(tmp_path / "sig.o")], check=True)
     lib = L.load()
-    assert {"b200st_optimizer_step_partial", "b200st_apply_mask"} <= set(L.EXPORTS)
-    assert lib.b200st_optimizer_step_partial.argtypes == [C.c_void_p, C.POINTER(L.OptimArgs), C.c_void_p, C.c_void_p]
+    assert {"b200st_optimizer_step", "b200st_apply_mask"} <= set(L.EXPORTS)
+    assert lib.b200st_optimizer_step.argtypes == [C.c_void_p, C.POINTER(L.OptimArgs), C.c_void_p]
     assert lib.b200st_apply_mask.argtypes == [C.c_void_p, C.c_void_p, C.c_int32, C.c_void_p, C.c_int64, C.c_void_p]
-    assert lib.b200st_optimizer_step_partial.restype is C.c_int and lib.b200st_apply_mask.restype is C.c_int
+    assert lib.b200st_optimizer_step.restype is C.c_int and lib.b200st_apply_mask.restype is C.c_int

@@ -1,6 +1,8 @@
-"""Prune-Tune on the device: b200st_optimizer_step_partial against b200st_optimizer_step on a clone of the same arena, the
-trainer with the captured step and update_cycle 2, its launches, and the whole recipe through the entries (prune and write
-mask.pkl, tune the pruned positions, resume, derive the masks without mask_pkl, mask_predict) for the text and speech models."""
+"""Prune-Tune on the device: the partial-tuning optimizer step against the plain step on a clone of the same arena, the
+refusals of the step's two masks, the trainer with the captured step and update_cycle 2, its launches, and the whole recipe
+through the entries (prune and write mask.pkl, tune the pruned positions, resume, derive the masks without mask_pkl,
+mask_predict) for the text and speech models."""
+import ctypes as C
 import os
 import shutil
 
@@ -108,6 +110,41 @@ def test_partial_step_launches_what_the_plain_step_launches():
         assert not bool(a.params[zero].any())
         if a.shadow is not None:
             assert not bool(a.shadow[zero].float().any())
+
+
+def test_optimizer_step_refuses_two_masks_and_a_mask_without_a_handle():
+    """b200st_optimizer_step with a pruning schedule and a frozen-element bitmap together, or with either and no handle, is
+    refused with the reason before any launch and writes no byte of the arenas, the masks or the pruning state; the same
+    arguments with the pruning schedule alone and the handle are accepted."""
+    rt, _ = _pair("bf16")
+    sched = PR.ConstantSparsity(target_sparsity=0.3, begin_pruning_step=0, pruning_frequency=1)
+    rt.prune_setup(sched, PR.pruned_parameters(rt.table, None, RECIPE))
+    rt.partial_setup(rt.derive_prune_mask(list(rt.table)))
+    rt.ensure_grads().normal_()
+    rt.adam_m, rt.adam_v = torch.randn_like(rt.params) * 0.1, torch.rand_like(rt.params)
+    a = L.OptimArgs()
+    a.params, a.grads, a.m, a.v = rt.params.data_ptr(), rt.grads.data_ptr(), rt.adam_m.data_ptr(), rt.adam_v.data_ptr()
+    a.shadow, a.shadow_dtype, a.numel = rt.shadow.data_ptr(), rt.prec, rt.numel
+    a.lr, a.beta1, a.beta2, a.eps, a.step_t, a.grad_scale, a.zero_grad = 1e-3, 0.9, 0.98, 1e-9, 1, 1.0, 1
+    prune = C.pointer(rt._prune_args(sched))
+    written = (rt.params, rt.grads, rt.adam_m, rt.adam_v, rt.shadow, rt.prune_mask, rt.prune_state, rt.prune_thresholds,
+               rt.prune_scratch, rt.partial_frozen)
+    before = [x.clone() for x in written]
+    torch.cuda.synchronize()
+    launches = L.launch_count()
+    for handle, p, frozen, reason in ((rt.handle, prune, rt.partial_frozen, "not both"), (None, prune, None, "handle"),
+                                      (None, None, rt.partial_frozen, "handle")):
+        a.prune, a.frozen = p, None if frozen is None else frozen.data_ptr()
+        rc = rt.lib.b200st_optimizer_step(handle, C.byref(a), L._stream())
+        assert rc != 0 and reason in rt.lib.b200st_last_error().decode(), (reason, rt.lib.b200st_last_error())
+    torch.cuda.synchronize()
+    assert L.launch_count() == launches
+    for x, y in zip(written, before):
+        assert torch.equal(x.view(torch.uint8), y.view(torch.uint8))
+    a.prune, a.frozen = prune, None
+    L.check(rt.lib.b200st_optimizer_step(rt.handle, C.byref(a), L._stream()))
+    torch.cuda.synchronize()
+    assert L.launch_count() > launches and int(rt.prune_state[0]) == 1 and not torch.equal(rt.params, before[0])
 
 
 def test_trainer_with_the_captured_step_and_update_cycle_keeps_frozen_weights():

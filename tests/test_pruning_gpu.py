@@ -1,7 +1,7 @@
-"""Weight pruning on the device (b200st_optimizer_step_pruned, b200st_prune_select) against torch restatements of the
-reference's pruning optimizer (neurst/sparsity/pruning_optimizer.py, keep_prune_property=True): the exact segmented
-selection, the step semantics over a dozen updates, the fp16 skip, the 16-bit shadow, and `train` / `predict` through the
-entry for the speech and the text model."""
+"""Weight pruning on the device (b200st_optimizer_step with a prune schedule, b200st_prune_select) against torch
+restatements of the reference's pruning optimizer (neurst/sparsity/pruning_optimizer.py, keep_prune_property=True): the
+exact segmented selection, the step semantics over a dozen updates, the fp16 skip, the 16-bit shadow, and `train` /
+`predict` through the entry for the speech and the text model."""
 import ctypes as C
 import os
 

@@ -1,5 +1,5 @@
-"""Cost of weight pruning during training (b200st_optimizer_step_pruned) on the parameter arenas of speech_transformer_s and
-transformer_big, bf16 shadow, random weights and gradients.
+"""Cost of weight pruning during training (b200st_optimizer_step with a prune schedule) on the parameter arenas of
+speech_transformer_s and transformer_big, bf16 shadow, random weights and gradients.
 
 Arms per arena, timed with CUDA events over ITERS back-to-back steps, alternated, REPEATS times after a warm-up of each:
   plain      b200st_optimizer_step (Keras Adam + shadow refresh + gradient zeroing)

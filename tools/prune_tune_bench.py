@@ -1,5 +1,5 @@
-"""Cost of the partial-tuning optimizer step (b200st_optimizer_step_partial) against the plain step (b200st_optimizer_step) on
-the parameter arenas of speech_transformer_s and transformer_big, bf16 shadow, random weights and gradients, a tenth of the
+"""Cost of the partial-tuning optimizer step (b200st_optimizer_step with a frozen bitmap) against the plain step on the
+parameter arenas of speech_transformer_s and transformer_big, bf16 shadow, random weights and gradients, a tenth of the
 weights of the recipe's pruned tensors (all but LayerNorms and modalities) zero and tuned, everything else frozen.
 
 The two arms are timed with CUDA events over ITERS back-to-back steps, alternated, REPEATS times after a warm-up of each.
